@@ -10,15 +10,19 @@ powerset classes, and file g is clustered / reconstructed on rank g mod N (`--pa
 
   value : audio-hours/sec, waveforms already resident in HBM (CUDA events, max over ranks)
   e2e   : the same through the public batch API with HOST waveforms (H2D + D2H inside the timed region)
-  roofline     : ResNet34 trunk conv kernels (~98 % of the FLOPs) measured live with CUDA events; `traffic` from the
-                 latest ncu capture of the same kernels (profiles/*_trunk_traffic.json)
+  roofline     : ResNet34 trunk conv kernels (~98 % of the FLOPs) measured live with CUDA events, against the H100 SXM
+                 data-sheet dense FP16 tensor rate
   cpu_baseline : the CPU oracle (reference-equivalent: 3 trunk passes per chunk) on a bounded sample, rank 0, N=1
   eager_cuda_baseline : the same oracle networks in PyTorch-eager CUDA fp32 with TF32 off (what the reference itself
                  would run on this GPU, utils/reproducibility.py:68-83), batch 32, CUDA events
 
 `--impl reference` times the CPU oracle arm (the reference package itself cannot be imported in this image:
-lightning / pyannote.core / asteroid_filterbanks are absent, see DESIGN.md).  Its sample is one short file per step,
+lightning / pyannote.core / asteroid_filterbanks are absent).  Its sample is one short file per step,
 end to end, normalised to the chunk density of the 10-minute workload (stated in cpu_baseline.sample).
+
+`--dump-outputs DIR` writes, after the timed steps, what the timed path returned for every file in its last step:
+DIR/<uri>_diarization.npy and DIR/<uri>_exclusive_diarization.npy (float64 rows of start s, end s, speaker index)
+and DIR/<uri>_speaker_embeddings.npy (float32 centroids).  Inputs are seeded, so two builds can be compared file by file.
 """
 import argparse
 import json
@@ -34,8 +38,9 @@ import torch
 ROOT = os.path.dirname(os.path.abspath(__file__))
 sys.path.insert(0, ROOT)
 
-METRIC = "audio-hours/sec (RTF) community-1 diarization, 16kHz mono, 1/2/4/8 B200"
-TRUNK_FLOP_PER_SEGMENT = 45.18e9   # 33 conv3x3 + 3 conv1x1 of ResNet34 at (80 x 998), SURVEY.md section 8(d)
+METRIC = "audio-hours/sec (RTF) community-1 diarization, 16kHz mono, 1/2/4/8 H100"
+PEAK_TFLOPS = 989.0                # H100 SXM data sheet, dense FP16 tensor rate at 700 W (not a measured peak)
+TRUNK_FLOP_PER_SEGMENT = 45.18e9   # 33 conv3x3 + 3 conv1x1 of ResNet34 at (80 x 998)
 
 
 def parse():
@@ -55,14 +60,11 @@ def parse():
     ap.add_argument("--no-eager-baseline", action="store_true", help="skip the PyTorch-eager CUDA fp32 leg")
     ap.add_argument("--min-warmup", type=int, default=3, help="lower only when profiling under ncu")
     ap.add_argument("--no-cpu-baseline", action="store_true", help="skip the CPU oracle leg (profiling runs)")
-    return ap.parse_args()
-
-
-def peaks():
-    try:
-        return json.load(open(os.path.join(ROOT, "MEASURED_PEAKS.json")))
-    except Exception:
-        return {}
+    ap.add_argument("--dump-outputs", metavar="DIR", help="write the last timed step's outputs as DIR/<name>.npy")
+    args = ap.parse_args()
+    if args.steps < 1:
+        ap.error("--steps must be at least 1")
+    return args
 
 
 class ClockSampler:
@@ -228,18 +230,20 @@ def eager_cuda_baseline(args, dev, chunks=64):
             f"chunk like cpu_baseline"}
 
 
-def trunk_traffic():
-    """(DRAM bytes, segments, file) of one trunk pass over an embedding sub-batch from the newest committed ncu
-    capture (profiles/*_trunk_traffic.json, produced by scripts/ncu_trunk_traffic.py from an
-    `ncu --metrics dram__bytes_*` launch list)."""
-    import glob
-
-    files = sorted(glob.glob(os.path.join(ROOT, "profiles", "r*_trunk_traffic.json")))
-    if not files:
-        return None, None, None
-    d = json.load(open(files[-1]))
-    return (d.get("dram_bytes_per_pass", d.get("dram_bytes_per_256_segments")), int(d.get("segments", 256)),
-            os.path.basename(files[-1]))
+def dump_outputs(directory, results):
+    """What the caller of the timed path receives, per file: both diarizations as (start, end, speaker index) rows
+    and the speaker embeddings."""
+    os.makedirs(directory, exist_ok=True)
+    for file, out in results:
+        uri = file["uri"]
+        for name in ("speaker_diarization", "exclusive_speaker_diarization"):
+            ann = getattr(out, name)
+            labels = {lab: i for i, lab in enumerate(sorted(ann.labels()))}
+            rows = [(seg.start, seg.end, labels[lab]) for seg, _, lab in ann.itertracks(yield_label=True)]
+            np.save(os.path.join(directory, f"{uri}_{name.replace('speaker_', '', 1)}.npy"),
+                    np.asarray(rows, dtype=np.float64).reshape(-1, 3))
+        np.save(os.path.join(directory, f"{uri}_speaker_embeddings.npy"),
+                np.asarray(out.speaker_embeddings, dtype=np.float32))
 
 
 def main():
@@ -301,12 +305,11 @@ def main():
     resident = pool.upload(files) if use_pool else pipe.upload(files)
     done = [0]
     coll_ms = []
+    last = []
 
     def step_resident():
-        n = 0
-        for _ in (pool.run_resident(resident) if use_pool else pipe.run_resident(resident)):
-            n += 1
-        done[0] = n
+        last[:] = list(pool.run_resident(resident) if use_pool else pipe.run_resident(resident))
+        done[0] = len(last)
         if use_pool:
             coll_ms.append(pool._events)
 
@@ -353,6 +356,8 @@ def main():
     if world > 1:
         dist.all_reduce(files_done)
     assert int(files_done.item()) == world * nfiles, "every file must come out of the per-file stage exactly once"
+    if args.dump_outputs:
+        dump_outputs(args.dump_outputs, last)
     ms_e2e = timed(step_e2e, max(1, args.steps))
     value = world * audio_hours / (ms_resident / 1e3)
     e2e = world * audio_hours / (ms_e2e / 1e3)
@@ -360,20 +365,15 @@ def main():
         if world > 1:
             dist.destroy_process_group()
         return
-    pk = peaks()
-    peak = pk.get("bf16_tflops_sustained", 1400.0)
+    peak = PEAK_TFLOPS
     achieved = trunk_segments * TRUNK_FLOP_PER_SEGMENT / (trunk_ms / 1e3) / 1e12 if trunk_ms > 0 else 0.0
-    traffic, traffic_segments, traffic_src = trunk_traffic()
-    sub_batch = traffic_segments or 296                    # segments of the launch unit (one embedding sub-batch)
+    sub_batch = 264                                        # segments of the launch unit (one embedding sub-batch)
     roofline = {"bound": "tensor",
-                "kernel": "ResNet34 trunk = stem + tcgen05 conv kernels, one dependent chain per embedding sub-batch "
-                          "(296 segments in the library, the launch unit below is the captured one)",
+                "kernel": "ResNet34 trunk = stem + wgmma conv kernels, one dependent chain per embedding sub-batch "
+                          f"({sub_batch} segments)",
                 "achieved": achieved, "peak": peak, "unit": "TFLOP/s", "frac": achieved / peak if peak else None,
-                "traffic": traffic, "traffic_unit": f"bytes per {sub_batch}-segment trunk pass (ncu dram read+write)",
-                "traffic_source": traffic_src,
                 "algorithmic_flop_per_launch_unit": sub_batch * TRUNK_FLOP_PER_SEGMENT,
-                "peak_source": "MEASURED_PEAKS.json bf16_tflops_sustained (fp16 = same tensor rate)"
-                if pk else "fallback 1.4 PFLOP/s sustained",
+                "peak_source": "H100 SXM data sheet, dense FP16 (a data-sheet rate, not a measured one)",
                 "trunk_ms_per_step": trunk_ms / args.steps, "seg_ms_per_step": seg_ms / args.steps}
     cpu = eager = None
     if world == 1 and not args.no_eager_baseline:
@@ -386,7 +386,8 @@ def main():
                "kind": "port", "sample": cpu_sample_text(args, t, chunks)}
     line = {"metric": METRIC, "value": value, "unit": "audio-hours/sec", "n_gpus": world, "steps": args.steps,
             "warmup": max(args.min_warmup, args.warmup), "ms_per_step": ms_resident, "higher_is_better": True, "scaling": "weak",
-            "vs_baseline": None, "dtype": "f16 tensor-core trunk (f32 accumulate) + split-f16x3 tensor-core segmentation (f32-level accuracy) + f64 clustering",
+            "vs_baseline": None, "dtype": "f16 tensor-core trunk (f32 accumulate) + split-f16x3 tensor-core segmentation (f32-level accuracy) "
+            "+ f64 clustering",
             "data": "synthetic", "config": workload_config(args, world),
             "rtf": (ms_resident / 1e3) / (audio_hours * 3600.0) / world,
             "e2e": {"value": e2e, "unit": "audio-hours/sec", "h2d_bytes_per_step": h2d, "d2h_bytes_per_step": d2h[0],

@@ -1,4 +1,4 @@
-/* b200diar.h -- C ABI of the B200-native community-1 diarization hot path.
+/* b200diar.h -- C ABI of the H100-native (sm_90a) community-1 diarization hot path.
  *
  * Drop-in boundary for pyannote.audio's sliding-window inference path.  The reference is 100 % Python and has no
  * FFI for this path, so each entry point cites the *Python* interface it replaces (paths relative to
@@ -27,7 +27,7 @@ enum b200_status {
   B200_STATUS_STATE = -4    /* weights not loaded, ctx misuse                -> RuntimeError */
 };
 
-/* fixed geometry of the path (SURVEY.md section 8) */
+/* fixed geometry of the path */
 #define B200_CHUNK_SAMPLES 160000
 #define B200_FRAMES_PER_CHUNK 589
 #define B200_LOCAL_SPEAKERS 3
@@ -43,11 +43,11 @@ int b200_version(void);
 int b200_ctx_create(b200_ctx** ctx, int device);
 int b200_ctx_destroy(b200_ctx* ctx);
 /* Tuning / A-B options (no reference counterpart; results do not depend on the sub-batch sizes):
- *   "seg_max_batch" (4736) / "emb_max_batch" (296): chunks per sub-batch = workspace size (INTEGRATION.md section 4);
- *   "conv_impl" 8 = per-layer choice of the tcgen05 conv kernels (default), 0 = CUDA-core reference conv, 1 = per-tap,
- *   2 = tcgen05 for stride-1 only, 3..6 = strip-streaming variants; "conv_fuse", "conv_fold", "conv_scfold", "conv_ghost";
- *   "seg_gemm_impl" / "seg_rec_impl" 1 = tensor cores, 0 = fp32 CUDA-core twins; "seg_conv_impl" 0 twins, 1 tensor
- *   cores, 2 sinc layer only, 3 Conv1d layers only; "fbank_share" 1 = overlapping chunks share their fbank frames;
+ *   "seg_max_batch" (2112) / "emb_max_batch" (264): chunks per sub-batch = workspace size (INTEGRATION.md section 4);
+ *   "conv_impl" 1 = wgmma tensor-core trunk convs (default), 0 = CUDA-core reference conv; "seg_gemm_impl" 1 = wgmma
+ *   split-precision GEMMs, 0 = fp32 CUDA-core twins; "seg_conv_impl" 1 = SincNet sinc / Conv1d layers as split-precision
+ *   wgmma implicit GEMMs, 0 = fp32 CUDA-core twins; "seg_rec_impl" 1 = LSTM recurrence as split-precision wgmma on
+ *   2-CTA clusters (with "seg_gemm_impl" 1), 0 = fp32 CUDA-core twin; "fbank_share" 1 = overlapping chunks share their fbank frames;
  *   "profile" 1 = CUDA-event timers around the trunk / the segmentation (b200_ctx_timer).  Unknown keys and values out
  *   of range return B200_ERR_INVALID. */
 int b200_ctx_set_option(b200_ctx* ctx, const char* key, int64_t value);
@@ -137,7 +137,7 @@ int b200_powerset_to_multilabel(b200_ctx* ctx, const uint8_t* classes, int64_t n
  * StatsPool weights; emb[num_chunks][3][256] fp32. */
 int b200_emb_forward(b200_ctx* ctx, const float* wav, const int64_t* chunk_off, const int32_t* chunk_valid,
                      int32_t num_chunks, const uint8_t* masks, float* emb, void* stream);
-/* The same with a fused all-gather for the multi-GPU chunk pool (SURVEY.md section 8e): emb_peers[n_peers] (HOST array
+/* The same with a fused all-gather for the multi-GPU chunk pool: emb_peers[n_peers] (HOST array
  * of DEVICE pointers, n_peers <= 7) are this rank's slot inside the OTHER GPUs' gather buffers (peer memory mapped
  * over NVLink, e.g. CUDA IPC / torch symmetric memory); the epilogue of the final Linear GEMM stores every output
  * tile to `emb` and to all peers (P2P stores), so the exchange overlaps the GEMM and no collective call follows.

@@ -8,7 +8,7 @@ only as the checker or as the timed CPU baseline -- never as the product.  The
 product package (``pyannote_audio_b200``) must not import anything from here
 and fails loudly when its CUDA library is missing.
 
-Parity pinning status (see DESIGN.md, "Oracle pinning"):
+Parity pinning status:
 
 * StatsPool, Powerset, VBx/PLDA, ResNet34 trunk, receptive-field arithmetic:
   PINNED -- validated in the build container against the reference's own files

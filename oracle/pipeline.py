@@ -206,7 +206,7 @@ def to_diarization(segmentations: SWF, count: SWF, stable=True) -> SWF:
     activations = activations.crop_loose(extent)
     count = count.crop_loose(extent)
     # reference: np.argsort(-activations) (default introsort, ties unstable in principle);
-    # the oracle pins ties as "descending value, then ascending cluster index" (SURVEY.md App. A).
+    # the oracle pins ties as "descending value, then ascending cluster index".
     sorted_speakers = np.argsort(-activations.data, axis=-1, kind="stable" if stable else None)
     binary = np.zeros_like(activations.data)
     for t in range(min(len(count.data), len(binary))):

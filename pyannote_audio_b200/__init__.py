@@ -1,4 +1,4 @@
-"""pyannote_audio_b200 -- B200-native (sm_100a) implementation of pyannote.audio's community-1 diarization hot path.
+"""pyannote_audio_b200 -- H100-native (sm_90a) implementation of pyannote.audio's community-1 diarization hot path.
 
 Public surface mirrors the reference for this path only:
   Inference, Model classes (PyanNet, WeSpeakerResNet34), SpeakerDiarization (+ DiarizeOutput), VBxClustering,

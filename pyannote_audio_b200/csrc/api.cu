@@ -16,20 +16,17 @@ using namespace b200;
 
 struct b200_ctx {
   int device = 0;
-  int num_sms = 148;
-  int seg_gemm_impl = 1;   // 1 = split-fp16 tcgen05 GEMMs for the LSTM input projections / linear layers, 0 = fp32 SIMT
-  int seg_conv_impl = 1;   // 1 = SincNet Conv1d(k=5) layers on tcgen05 (split fp16), 0 = fp32 CUDA-core kernel
-  int seg_rec_impl = 1;    // 1 = LSTM recurrence on the tensor cores (needs seg_gemm_impl = 1), 0 = fp32 SIMT cluster kernel
-  int conv_fuse = 1;       // 1 = layer1 BasicBlocks as one fused kernel (conv_block32_kernel) when conv_impl == 8
-  int conv_ghost = 0;      // 1 = TMEM rings with ghost blocks (no seam-split MMAs) in conv_tc4 / conv_block32
-  int conv_fold = 1;       // 1 = conv_tc3 loads one pixel box per (kh, channel block), kw taps are descriptor shifts
-  int conv_scfold = 1;     // 1 = layer2.0: the 1x1 stride-2 shortcut rides in the padded weight rows of the stride-2 conv
-  int conv_impl = 8;   // channels-as-M conv for C_out >= 128, strip-streaming conv for the narrow stride-1 3x3, per-tap conv otherwise
-  int seg_max_batch = 4736;     // chunks per segmentation sub-batch (37 LSTM tiles of 128 sequences x 2 directions = 74 clusters)
-  // chunks per embedding sub-batch.  296 = 2 x 148: the persistent conv kernels stride their items over 148 CTAs and
-  // every layer's item count is a multiple of the sub-batch (8 / 4 strips, 20 / 10 pixel tiles per segment), so all
-  // CTAs get the same number of items (256 left the last wave 30-92 % full: 516 -> 511 ms per bench step)
-  int emb_max_batch = 296;
+  int num_sms = 132;
+  int seg_gemm_impl = 1;   // 1 = split-fp16 wgmma GEMMs for the LSTM input projections / linear layers, 0 = fp32 SIMT
+  int seg_rec_impl = 1;    // 1 = LSTM recurrence as split-fp16 wgmma on 2-CTA clusters (needs seg_gemm_impl = 1), 0 = fp32 SIMT
+  int seg_conv_impl = 1;   // 1 = SincNet sinc / Conv1d layers as split-fp16 wgmma implicit GEMMs, 0 = fp32 CUDA-core twins
+  int conv_impl = 1;       // 1 = wgmma implicit-GEMM trunk convs, 0 = fp32 CUDA-core reference conv
+  // chunks per segmentation sub-batch: 2112 = 33 recurrence tiles of 64 sequences x 2 directions x 2-CTA clusters
+  // = 132 CTAs, one per SM of an H100 SXM (seg_lstm.cu launch_rec)
+  int seg_max_batch = 2112;
+  // chunks per embedding sub-batch: 264 = 2 x 132 SMs, so that the conv tiles of every layer (8 / 4 / 2 / 1 tiles
+  // of 128 pixels per image row) split evenly over the machine
+  int emb_max_batch = 264;
   int fbank_share = 1;          // 1 = overlapping hop-aligned chunks share their fbank frames (emb.cuh: FbankRun)
   int64_t launches = 0;
   SegWeights seg;
@@ -251,26 +248,6 @@ int make_conv(b200_ctx* ctx, const b200_conv_bn& src, int cin, int cout, int k, 
   int rc;
   if ((rc = upload(ctx, w, &L->w))) return rc;
   if ((rc = upload(ctx, bias, &L->bias))) return rc;
-  if (k == 3 && stride == 1 && cin == cout && (cin == 32 || cin == 64)) {   // conv_tc4_kernel: [kw][(kh, c_out)][c_in]
-    const int C = cin;
-    std::vector<__half> w4((size_t)9 * C * C);
-    for (int kh = 0; kh < 3; ++kh)
-      for (int kw = 0; kw < 3; ++kw)
-        for (int co = 0; co < C; ++co)
-          for (int ci = 0; ci < C; ++ci)
-            w4[(((size_t)kw * 3 + kh) * C + co) * C + ci] = w[((size_t)(kh * 3 + kw) * cout + co) * cin + ci];
-    if ((rc = upload(ctx, w4, &L->w4))) return rc;
-  }
-  if ((k == 3 && stride == 1 && cout >= 128) || stride == 2) {
-    // copy for the channels-as-M kernel (rows padded to 128): wide stride-1 convs, the stride-2 convs and the
-    // 1x1 stride-2 shortcuts
-    const int rows = (cout + 127) / 128 * 128;
-    std::vector<__half> w3((size_t)k * k * rows * cin, __float2half(0.f));
-    for (int t = 0; t < k * k; ++t)
-      for (int co = 0; co < cout; ++co)
-        for (int ci = 0; ci < cin; ++ci) w3[((size_t)t * rows + co) * cin + ci] = w[((size_t)t * cout + co) * cin + ci];
-    if ((rc = upload(ctx, w3, &L->w3))) return rc;
-  }
   return B200_OK;
 }
 
@@ -288,8 +265,8 @@ int b200_ctx_create(b200_ctx** out, int device) {
   B200_CHECK(device >= 0 && device < ndev, B200_ERR_INVALID, "device %d not available (%d devices)", device, ndev);
   cudaDeviceProp prop;
   B200_CUDA_OK(cudaGetDeviceProperties(&prop, device));
-  B200_CHECK(prop.major == 10, B200_ERR_STATE, "device %d is sm_%d%d; this library is built for sm_100a (B200) only",
-             device, prop.major, prop.minor);
+  B200_CHECK(prop.major == 9 && prop.minor == 0, B200_ERR_STATE,
+             "device %d is sm_%d%d; this library is built for sm_90a (H100) only", device, prop.major, prop.minor);
   b200_ctx* c = new b200_ctx();
   c->device = device;
   c->num_sms = prop.multiProcessorCount;
@@ -324,15 +301,13 @@ int b200_ctx_set_option(b200_ctx* ctx, const char* key, int64_t value) {
   else if (k == "emb_max_batch") ctx->emb_max_batch = (int)value;
   else if (k == "profile") ctx->profile = (int)value;
   else if (k == "seg_gemm_impl") ctx->seg_gemm_impl = (int)value;
-  else if (k == "seg_rec_impl") ctx->seg_rec_impl = (int)value;
   else if (k == "seg_conv_impl") ctx->seg_conv_impl = (int)value;
-  else if (k == "conv_fuse") ctx->conv_fuse = (int)value;
-  else if (k == "conv_ghost") ctx->conv_ghost = (int)value;
-  else if (k == "conv_fold") ctx->conv_fold = (int)value;
-  else if (k == "conv_scfold") ctx->conv_scfold = (int)value;
+  else if (k == "seg_rec_impl") ctx->seg_rec_impl = (int)value;
   else if (k == "fbank_share") ctx->fbank_share = (int)value;
   else B200_CHECK(false, B200_ERR_INVALID, "unknown option '%s'", key);
-  B200_CHECK(ctx->seg_max_batch >= 1 && ctx->emb_max_batch >= 1 && ctx->conv_impl >= 0 && ctx->conv_impl <= 8,
+  B200_CHECK(ctx->seg_max_batch >= 1 && ctx->emb_max_batch >= 1 && ctx->conv_impl >= 0 && ctx->conv_impl <= 1 &&
+                 ctx->seg_gemm_impl >= 0 && ctx->seg_gemm_impl <= 1 && ctx->seg_conv_impl >= 0 && ctx->seg_conv_impl <= 1 &&
+                 ctx->seg_rec_impl >= 0 && ctx->seg_rec_impl <= 1,
              B200_ERR_INVALID, "option '%s' value %lld out of range", key, (long long)value);
   return B200_OK;
 }
@@ -437,18 +412,16 @@ int b200_seg_load(b200_ctx* ctx, const b200_seg_weights* w) {
       f[125 * 80 + ch] = ch < 40 ? r[125] : 0.f;
     }
     if ((rc = upload(ctx, f, &S.sinc_f))) return rc;
-    {   // tensor-core layout of the full bank: [k-step][128 rows][16 taps] as fp16 (hi, lo), taps 251..255 zero
-      std::vector<__half> hi((size_t)16 * 128 * 16, __float2half(0.f)), lo(hi.size(), __float2half(0.f));
-      for (int ch = 0; ch < 80; ++ch)
-        for (int k = 0; k < 251; ++k) {
-          const float v = w->sinc_filters[ch * 251 + k];
-          const size_t o = ((size_t)(k / 16) * 128 + ch) * 16 + (k % 16);
-          hi[o] = __float2half(v);
-          lo[o] = __float2half(v - __half2float(hi[o]));
-        }
-      if ((rc = upload(ctx, hi, &S.sinc_tc_hi))) return rc;
-      if ((rc = upload(ctx, lo, &S.sinc_tc_lo))) return rc;
-    }
+    std::vector<__half> hi((size_t)80 * 256, __float2half(0.f)), lo(hi.size(), __float2half(0.f));
+    for (int ch = 0; ch < 80; ++ch)
+      for (int k = 0; k < 251; ++k) {
+        const float v = w->sinc_filters[ch * 251 + k];
+        const size_t o = (size_t)ch * 256 + k;
+        hi[o] = __float2half(v);
+        lo[o] = __float2half(v - __half2float(hi[o]));
+      }
+    if ((rc = upload(ctx, hi, &S.sinc_wg_hi))) return rc;
+    if ((rc = upload(ctx, lo, &S.sinc_wg_lo))) return rc;
   }
   const int nch[3] = {80, 60, 60};
   for (int i = 0; i < 3; ++i) {
@@ -466,19 +439,19 @@ int b200_seg_load(b200_ctx* ctx, const b200_seg_weights* w) {
         for (int k = 0; k < 5; ++k) wc[((size_t)ci * 5 + k) * 60 + co] = w->conv_weight[i][((size_t)co * cin[i] + ci) * 5 + k];
     if ((rc = upload(ctx, wc, &S.conv_w[i]))) return rc;
     if ((rc = upload(ctx, bc, &S.conv_b[i]))) return rc;
-    {   // tensor-core layout: [channel block of 16][tap][128 rows = c_out (60 real)][16 c_in] as fp16 (hi, lo)
-      const int ncb = (cin[i] + 15) / 16;
-      std::vector<__half> hi((size_t)ncb * 5 * 128 * 16, __float2half(0.f)), lo(hi.size(), __float2half(0.f));
+    {   // wgmma layout: [64 rows = c_out][k = tap * Cpad + c_in], Cpad = 80 | 64, padding zero
+      const int cpad = i == 0 ? 80 : 64, K = 5 * cpad;
+      std::vector<__half> hi((size_t)64 * K, __float2half(0.f)), lo(hi.size(), __float2half(0.f));
       for (int co = 0; co < 60; ++co)
         for (int ci = 0; ci < cin[i]; ++ci)
           for (int k = 0; k < 5; ++k) {
             const float v = w->conv_weight[i][((size_t)co * cin[i] + ci) * 5 + k];
-            const size_t o = ((((size_t)(ci / 16) * 5 + k) * 128) + co) * 16 + (ci % 16);
+            const size_t o = (size_t)co * K + k * cpad + ci;
             hi[o] = __float2half(v);
             lo[o] = __float2half(v - __half2float(hi[o]));
           }
-      if ((rc = upload(ctx, hi, &S.conv_tc_hi[i]))) return rc;
-      if ((rc = upload(ctx, lo, &S.conv_tc_lo[i]))) return rc;
+      if ((rc = upload(ctx, hi, &S.conv_wg_hi[i]))) return rc;
+      if ((rc = upload(ctx, lo, &S.conv_wg_lo[i]))) return rc;
     }
   }
   for (int l = 0; l < S.lstm_layers; ++l) {
@@ -516,23 +489,19 @@ int b200_seg_load(b200_ctx* ctx, const b200_seg_weights* w) {
     if ((rc = upload(ctx, wih, &S.w_ih[l]))) return rc;
     if ((rc = upload(ctx, bg, &S.b_g[l]))) return rc;
     if ((rc = upload(ctx, whh, &S.w_hh[l]))) return rc;
-    {   // tensor-core recurrence: rows (dir, rank, unit_local, gate), k contiguous (permuted, below), as fp16 (hi, lo)
-      std::vector<__half> hi((size_t)1024 * 128), lo((size_t)1024 * 128);
-      for (int d = 0; d < 2; ++d) {
-        const float* Wh = w->lstm_w_hh[l * 2 + d];
+    {   // wgmma recurrence: [dir][rank][n = 32 jj + 8 gate + u][k = unit 0..127], local unit 8 jj + u, as fp16 (hi, lo)
+      std::vector<__half> hi((size_t)4 * 256 * 128), lo(hi.size());
+      for (int d = 0; d < 2; ++d)
         for (int r = 0; r < 2; ++r)
-          for (int ul = 0; ul < 64; ++ul)
-            for (int gt = 0; gt < 4; ++gt)
-              for (int k = 0; k < 128; ++k) {
-                const float v = Wh[(size_t)(gt * 128 + 64 * r + ul) * 128 + k];
-                // K order inside a k-block of 64 units: (chunk, half, unit-in-chunk) for unit = half*32 + chunk*8 + u,
-                // so that the units the epilogue warps finish together form one 16-wide k-step (seg_lstm_tc.cu)
-                const int kl = k & 63, kp = (k & 64) | (((kl & 31) >> 3) << 4) | ((kl >> 5) << 3) | (kl & 7);
-                const size_t o = ((size_t)((d * 2 + r) * 256 + ul * 4 + gt)) * 128 + kp;
-                hi[o] = __float2half(v);
-                lo[o] = __float2half(v - __half2float(hi[o]));
-              }
-      }
+          for (int n = 0; n < 256; ++n) {
+            const int unit = 64 * r + 8 * (n / 32) + n % 8, gt = (n / 8) % 4;
+            for (int k = 0; k < 128; ++k) {
+              const float v = w->lstm_w_hh[l * 2 + d][(size_t)(gt * 128 + unit) * 128 + k];
+              const size_t o = ((size_t)(d * 2 + r) * 256 + n) * 128 + k;
+              hi[o] = __float2half(v);
+              lo[o] = __float2half(v - __half2float(hi[o]));
+            }
+          }
       if ((rc = upload(ctx, hi, &S.w_hh_hi[l]))) return rc;
       if ((rc = upload(ctx, lo, &S.w_hh_lo[l]))) return rc;
     }
@@ -591,29 +560,8 @@ int b200_emb_load(b200_ctx* ctx, const b200_emb_weights* w) {
       if ((rc = make_conv(ctx, w->block_conv1[bi], in_planes, planes[l], 3, s, &B.conv1))) return rc;
       if ((rc = make_conv(ctx, w->block_conv2[bi], planes[l], planes[l], 3, 1, &B.conv2))) return rc;
       B.has_shortcut = (s != 1 || in_planes != planes[l]);
-      if (B.has_shortcut) {
+      if (B.has_shortcut)
         if ((rc = make_conv(ctx, w->block_shortcut[bi], in_planes, planes[l], 1, s, &B.shortcut))) return rc;
-        if (planes[l] == 64 && s == 2) {
-          // the 64 zero-padded rows of conv1's 128-row channels-as-M weight tiles carry the 1x1 shortcut (centre tap)
-          const int cin = in_planes, cout = 64;
-          const b200_conv_bn &c1 = w->block_conv1[bi], &sc = w->block_shortcut[bi];
-          std::vector<__half> w3s((size_t)9 * 128 * cin, __float2half(0.f));
-          std::vector<float> bias_s(128);
-          for (int co = 0; co < cout; ++co) {
-            const float s1 = c1.bn_weight[co] / std::sqrt(c1.bn_var[co] + 1e-5f);
-            const float s2 = sc.bn_weight[co] / std::sqrt(sc.bn_var[co] + 1e-5f);
-            bias_s[co] = c1.bn_bias[co] - c1.bn_mean[co] * s1;
-            bias_s[64 + co] = sc.bn_bias[co] - sc.bn_mean[co] * s2;
-            for (int ci = 0; ci < cin; ++ci) {
-              for (int t = 0; t < 9; ++t)
-                w3s[((size_t)t * 128 + co) * cin + ci] = __float2half(c1.conv_weight[((size_t)co * cin + ci) * 9 + t] * s1);
-              w3s[((size_t)4 * 128 + 64 + co) * cin + ci] = __float2half(sc.conv_weight[(size_t)co * cin + ci] * s2);
-            }
-          }
-          if ((rc = upload(ctx, w3s, &B.conv1.w3s))) return rc;
-          if ((rc = upload(ctx, bias_s, &B.conv1.bias_s))) return rc;
-        }
-      }
       in_planes = planes[l];
       E.blocks.push_back(B);
     }
@@ -655,8 +603,7 @@ static int seg_run(b200_ctx* ctx, const float* wav, const int64_t* chunk_off, co
     ScopedTimer timer(ctx, &ctx->seg_events, st);
     if (ctx->profile) ctx->seg_chunks += nb;
     float* x0_dst = sinc_out ? sinc_out + (size_t)c0 * kFrames * 64 : x0;
-    if ((rc = sincnet_forward(ctx->seg, wav, ctx->d_off + c0, ctx->d_valid + c0, nb, region, x0_dst, ctx->seg_conv_impl,
-                              ctx->num_sms, st)))
+    if ((rc = sincnet_forward(ctx->seg, wav, ctx->d_off + c0, ctx->d_valid + c0, nb, region, x0_dst, ctx->seg_conv_impl, st)))
       return rc;
     ctx->launches += 8;
     if (sinc_out) continue;
@@ -734,33 +681,20 @@ static size_t carve_emb(int NB, void* base, EmbWs* w) {
   return align_up(off, 1024);
 }
 
-static int conv_flags(const b200_ctx* ctx) {
-  return (ctx->conv_ghost ? kConvGhost : 0) | (ctx->conv_fold ? kConvFold : 0);
-}
-
 // one BasicBlock on nb segments: A -> (Bf, Cf) -> A, in place on the residual
 static int block_run(b200_ctx* ctx, const BlockWeights& B, __half* A, __half* Bf, __half* Cf, int nb, int H, int Wd,
                      cudaStream_t st) {
   const int s = B.conv1.stride;
-  const int impl1 = (ctx->conv_impl == 2) ? (s == 1 ? 1 : 0) : ctx->conv_impl;
-  const int impl_s1 = ctx->conv_impl == 2 ? 1 : ctx->conv_impl;
   const int Ho = (H + 2 - 3) / s + 1, Wo = (Wd + 2 - 3) / s + 1;
   int rc;
-  if (ctx->conv_impl == 8 && ctx->conv_scfold && B.has_shortcut && B.conv1.w3s) {
-    // layer2.0: stride-2 conv1 and the 1x1 shortcut in one launch (the shortcut rides in the padded weight rows)
-    if ((rc = conv_s2_shortcut_forward(B.conv1, A, Bf, Cf, nb, H, Wd, ctx->num_sms, st))) return rc;
-    if ((rc = conv_forward(B.conv2, Bf, Cf, A, nb, Ho, Wo, 1, impl_s1, ctx->num_sms, st, conv_flags(ctx)))) return rc;
-    ctx->launches += 2;
-    return B200_OK;
-  }
-  if ((rc = conv_forward(B.conv1, A, nullptr, Bf, nb, H, Wd, 1, impl1, ctx->num_sms, st, conv_flags(ctx)))) return rc;
+  if ((rc = conv_forward(B.conv1, A, nullptr, Bf, nb, H, Wd, 1, ctx->conv_impl, ctx->num_sms, st))) return rc;
   const __half* res = A;
   if (B.has_shortcut) {
-    if ((rc = conv_forward(B.shortcut, A, nullptr, Cf, nb, H, Wd, 0, impl1, ctx->num_sms, st, conv_flags(ctx)))) return rc;
+    if ((rc = conv_forward(B.shortcut, A, nullptr, Cf, nb, H, Wd, 0, ctx->conv_impl, ctx->num_sms, st))) return rc;
     res = Cf;
     ctx->launches += 1;
   }
-  if ((rc = conv_forward(B.conv2, Bf, res, A, nb, Ho, Wo, 1, impl_s1, ctx->num_sms, st, conv_flags(ctx)))) return rc;
+  if ((rc = conv_forward(B.conv2, Bf, res, A, nb, Ho, Wo, 1, ctx->conv_impl, ctx->num_sms, st))) return rc;
   ctx->launches += 2;
   return B200_OK;
 }
@@ -771,8 +705,6 @@ static int trunk_run(b200_ctx* ctx, const EmbWs& w, const int* frame0, int nb, c
   const EmbWeights& E = ctx->emb;
   int rc;
   int H = kMel, Wd = kFbankFrames;
-  // (running stem + layer1 in L2-sized groups of segments was measured 12-35 % slower than whole sub-batches:
-  //  small grids lose more to tails and launch gaps than the L2 hits return)
   __half* cur = w.A;            // current activation; the other two buffers are scratch
   __half* s1 = w.Bf;
   __half* s2 = w.Cf;
@@ -780,14 +712,6 @@ static int trunk_run(b200_ctx* ctx, const EmbWs& w, const int* frame0, int nb, c
   ctx->launches += 1;
   for (const BlockWeights& B : E.blocks) {
     const int s = B.conv1.stride;
-    if (ctx->conv_impl == 8 && ctx->conv_fuse && !B.has_shortcut && s == 1 && B.conv1.C_in == 32 && B.conv1.w4 &&
-        B.conv2.w4) {
-      // layer1: the whole block in one kernel, intermediate activation kept in shared memory
-      if ((rc = conv_block32_forward(B.conv1, B.conv2, cur, s1, nb, H, Wd, ctx->num_sms, st, ctx->conv_ghost))) return rc;
-      ctx->launches += 1;
-      __half* t = cur; cur = s1; s1 = t;
-      continue;
-    }
     if ((rc = block_run(ctx, B, cur, s1, s2, nb, H, Wd, st))) return rc;
     H = (H + 2 - 3) / s + 1; Wd = (Wd + 2 - 3) / s + 1;
   }

@@ -1,4 +1,4 @@
-// Shared helpers for the B200 (sm_100a) diarization kernels.
+// Shared helpers for the diarization kernels (H100, sm_90a).
 #pragma once
 #include <cuda_runtime.h>
 #include <cuda_fp16.h>
@@ -41,7 +41,7 @@ enum {
   B200_ERR_STATE = -4,
 };
 
-// ---- fixed geometry of the community-1 hot path (SURVEY.md section 8 constants) ----
+// ---- fixed geometry of the community-1 hot path ----
 constexpr int kChunk = 160000;       // samples per 10 s chunk @16 kHz
 constexpr int kFrames = 589;         // segmentation frames per chunk
 constexpr int kSincK = 251;
@@ -61,8 +61,8 @@ constexpr int kEmbT = 125;           // ResNet time frames after 3 stride-2 stag
 constexpr int kEmbDim = 256;
 constexpr int kStatsDim = 2560;      // 256 channels x 10 freq bins
 
-// Packed fp32x2 FMA (Blackwell FFMA2): two independent IEEE fma.rn per instruction.  The FP32 kernels here are
-// limited by instruction issue / operand dispatch (ncu: FMA pipe 50 %, issue 60 %), not by the FMA lanes.
+// fp32 pairs packed in one 64-bit register: the FP32 kernels keep channel pairs together.  Hopper has no packed fp32
+// FMA, so ffma2 is two IEEE fma.rn (the same rounding as one per lane).
 typedef unsigned long long f32x2_t;
 #ifdef __CUDACC__
 __device__ __forceinline__ f32x2_t pack2(float lo, float hi) {
@@ -74,7 +74,11 @@ __device__ __forceinline__ void unpack2(f32x2_t v, float& lo, float& hi) {
   asm("mov.b64 {%0, %1}, %2;" : "=f"(lo), "=f"(hi) : "l"(v));
 }
 __device__ __forceinline__ void ffma2(f32x2_t& d, f32x2_t a, f32x2_t b) {   // d = a * b + d (lane-wise)
-  asm("fma.rn.f32x2 %0, %1, %2, %0;" : "+l"(d) : "l"(a), "l"(b));
+  float d0, d1, a0, a1, b0, b1;
+  unpack2(d, d0, d1);
+  unpack2(a, a0, a1);
+  unpack2(b, b0, b1);
+  d = pack2(__fmaf_rn(a0, b0, d0), __fmaf_rn(a1, b1, d1));
 }
 #endif
 

@@ -7,13 +7,7 @@ namespace b200 {
 struct ConvLayer {
   int C_in = 0, C_out = 0, ksize = 3, stride = 1;
   __half* w = nullptr;     // device, [tap][C_out][C_in] fp16, BN scale folded
-  __half* w4 = nullptr;    // 32->32 / 64->64 stride-1 layers: [kw][(kh, c_out) = 3C][c_in] for conv_tc4_kernel
-  __half* w3 = nullptr;    // same with C_out zero-padded to a multiple of 128 (conv_tc3_kernel's A operand)
   float* bias = nullptr;   // device, [C_out] fp32 (folded BN shift)
-  // conv_tc3_kernel only: a stride-2 3x3 conv with C_out = 64 carries the block's 1x1 stride-2 shortcut in the 64
-  // otherwise zero-padded rows of its 128-row weight tiles (shortcut weights at the centre tap): one launch, two outputs
-  __half* w3s = nullptr;   // [9][128][C_in]: rows 0..63 conv, rows 64..127 shortcut (centre tap only)
-  float* bias_s = nullptr; // [128]: conv bias | shortcut bias
 };
 
 struct ConvParams {
@@ -24,7 +18,7 @@ struct ConvParams {
   const float* bias;
   const __half* residual;
   __half* out;
-  uint32_t a_bytes, b_bytes, nstages, idesc, swizzle;
+  uint32_t a_bytes, b_bytes, nstages, swizzle;
 };
 
 struct BlockWeights {
@@ -50,19 +44,9 @@ struct EmbWeights {
   float* twiddle = nullptr;      // [256][2] cos/sin(-2 pi k / 512)
 };
 
-// flags of conv_forward / conv_block32_forward
-constexpr int kConvGhost = 1;   // TMEM rings with ghost blocks (conv_tc4 / conv_block32)
-constexpr int kConvFold = 2;    // conv_tc3: horizontal taps as descriptor shifts of one pixel box per (kh, channel block)
-// impl: 0 = SIMT reference conv, 1 = tcgen05 tensor-core conv
+// impl: 0 = SIMT reference conv, 1 = wgmma tensor-core conv
 int conv_forward(const ConvLayer& L, const __half* in, const __half* residual, __half* out, int B, int H_in, int W_in,
-                 int relu, int impl, int num_sms, cudaStream_t stream, int flags = kConvGhost | kConvFold);
-// stride-2 3x3 conv (C_out = 64) + the block's 1x1 stride-2 shortcut in ONE conv_tc3_kernel launch (L.w3s):
-// out = relu(conv(in) + b), out_sc = shortcut(in) + b_sc
-int conv_s2_shortcut_forward(const ConvLayer& L, const __half* in, __half* out, __half* out_sc, int B, int H_in,
-                             int W_in, int num_sms, cudaStream_t stream);
-// fused BasicBlock of layer1 (two 32->32 stride-1 convs + identity shortcut), out must not alias in
-int conv_block32_forward(const ConvLayer& L1, const ConvLayer& L2, const __half* in, __half* out, int B, int H, int W,
-                         int num_sms, cudaStream_t stream, int ghost = 1);
+                 int relu, int impl, int num_sms, cudaStream_t stream);
 // frame0 (device, [B], may be NULL = b * 998): first fbank row of each segment, see fbank_forward
 int conv1_forward(const float* fbank, const float* fmean, const int* frame0, const float* w, const float* bias,
                   __half* out, int B, cudaStream_t stream);

@@ -1,1532 +1,114 @@
-// WeSpeaker ResNet34 trunk convolutions for sm_100a.
+// WeSpeaker ResNet34 trunk convolutions for H100 (sm_90a).
 //
 // Reference semantics: /root/reference/src/pyannote/audio/models/embedding/wespeaker/resnet.py
 //   BasicBlock.forward :140-145 (conv3x3-BN-ReLU-conv3x3-BN + shortcut -> ReLU), ResNet.forward :413-419.
-// Eval-mode BatchNorm is folded into the conv weights / a per-channel bias on the host (emb_weights.cu).
+// Eval-mode BatchNorm is folded into the conv weights / a per-channel bias on the host (api.cu make_conv).
 //
-// conv_tc_kernel: implicit-GEMM convolution on the 5th-gen tensor cores.
+// conv_wg_kernel: implicit-GEMM convolution on the Hopper tensor cores (wgmma).
 //   GEMM view  D[M=128 output pixels of one image row][N=C_out] += A[M][K] * B[N][K]^T,
 //   K = taps * C_in walked tap by tap in chunks of Ck channels.  Activations are NHWC fp16 so that one
 //   TMA box (Ck channels x 128 consecutive pixels) lands in shared memory as a K-major, hardware-swizzled
 //   A tile; convolution padding is TMA out-of-bounds zero fill, stride-2 is the tensor map's element stride.
-//   Weights [tap][C_out][C_in] land the same way as the K-major B tile.  Accumulators live in TMEM
-//   (two stages of N columns so the epilogue of tile i overlaps the MMAs of tile i+1).
-//   Warp roles: warp0 = TMA producer, warp1 = tcgen05.mma issuer (+TMEM alloc), warps2-5 = epilogue
-//   (tcgen05.ld -> +bias (+residual) -> ReLU -> fp16 NHWC store).  Persistent over tiles.
+//   Weights [tap][C_out][C_in] land the same way as the K-major B tile.
+//   Roles: warp 8 = TMA producer over a ring of mbarrier-guarded stages; warpgroups 0 / 1 = output pixels
+//   [0, 64) / [64, 128) of the tile, fp32 accumulators in registers, epilogue (+bias (+residual) -> ReLU -> fp16
+//   NHWC store) straight from the accumulator fragments.  One CTA per tile.
 #include "common.cuh"
 #include "emb.cuh"
 #include "tc_common.cuh"
 
 namespace b200 {
 
-// ------------------------------------------------------------------------------------------------
-// tensor-core implicit GEMM conv
-// ------------------------------------------------------------------------------------------------
-constexpr int kTcThreads = 192;
+constexpr int kWgThreads = 288;
 constexpr int kTileM = 128;
 
-__global__ void __launch_bounds__(kTcThreads, 1)
-conv_tc_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB, ConvParams p) {
+template <int N, int CK>
+__global__ void __launch_bounds__(kWgThreads, N == 256 ? 1 : 2)
+conv_wg_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB, ConvParams p) {
   extern __shared__ uint8_t smem_raw[];
   const uint32_t raw = smem_u32(smem_raw);
   const uint32_t base = (raw + 1023u) & ~1023u;            // swizzle-128B operands need 1024 B alignment
-  uint8_t* gbase = smem_raw + (base - raw);
-  // [0,1024): barriers + tmem pointer, [1024,2048): bias, [2048,...): stages
-  const uint32_t bar_full = base;                            // 8 x 8 B
-  const uint32_t bar_empty = base + 64;                      // 8 x 8 B
-  const uint32_t bar_tfull = base + 128;                     // 2 x 8 B
-  const uint32_t bar_tempty = base + 144;                    // 2 x 8 B
-  uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(gbase + 192);
-  float* s_bias = reinterpret_cast<float*>(gbase + 1024);
-  const uint32_t stage0 = base + 2048;
+  const uint32_t bar_full = base, bar_empty = base + 64;    // 8 x 8 B each
+  const uint32_t stage0 = base + 1024;
   const uint32_t stage_bytes = p.a_bytes + p.b_bytes;
-
   const int warp = threadIdx.x >> 5;
-  const int lane = threadIdx.x & 31;
-  const int N = p.C_out;
+  const int wt = blockIdx.x % p.tiles_w;
+  const int bh = blockIdx.x / p.tiles_w;                    // = b * H_out + h
+  const int cchunks = p.C_in / p.Ck;
 
-  for (int i = threadIdx.x; i < N; i += blockDim.x) s_bias[i] = p.bias[i];
   if (threadIdx.x == 0) {
-    for (uint32_t s = 0; s < p.nstages; ++s) {
-      mbar_init(bar_full + 8 * s, 1);
-      mbar_init(bar_empty + 8 * s, 1);
-    }
-    for (int a = 0; a < 2; ++a) {
-      mbar_init(bar_tfull + 8 * a, 1);
-      mbar_init(bar_tempty + 8 * a, 4);
-    }
+    for (uint32_t s = 0; s < p.nstages; ++s) { mbar_init(bar_full + 8 * s, 1); mbar_init(bar_empty + 8 * s, 2); }
     asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
   }
-  if (warp == 1) {
-    asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(tmem_slot)),
-                 "r"(512u));
-    asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::);
-  }
-  tc_fence_before();
   __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem_base = *tmem_slot;
 
-  const int cchunks = p.C_in / p.Ck;
-  const int ksteps = p.Ck / 16;
-
-  if (warp == 0) {
-    const bool leader = elect_one_sync();
-    if (leader) {
-      asm volatile("prefetch.tensormap [%0];" ::"l"(reinterpret_cast<uint64_t>(&tmA)) : "memory");
-      asm volatile("prefetch.tensormap [%0];" ::"l"(reinterpret_cast<uint64_t>(&tmB)) : "memory");
-    }
-    uint32_t stage = 0, phase = 0;
-    for (int tile = blockIdx.x; tile < p.num_tiles; tile += gridDim.x) {
-      const int wt = tile % p.tiles_w;
-      const int bh = tile / p.tiles_w;
-      const int h = bh % p.H_out;
-      const int b = bh / p.H_out;
+  if (warp == 8) {
+    if ((threadIdx.x & 31) == 0) {
+      prefetch_tensormap(&tmA);
+      prefetch_tensormap(&tmB);
+      const int h = bh % p.H_out, b = bh / p.H_out;
       const int w_base = wt * kTileM * p.stride - p.pad, h_base = h * p.stride - p.pad;
+      uint32_t stage = 0, phase = 0;
       int tap = 0, cc = 0, kh = 0, kw = 0;
       for (int kb = 0; kb < p.kblocks; ++kb) {
         mbar_wait(bar_empty + 8 * stage, phase ^ 1);
-        if (leader) {
-          mbar_expect_tx(bar_full + 8 * stage, stage_bytes);
-          const uint32_t sa = stage0 + stage * stage_bytes;
-          tma_load_4d(&tmA, bar_full + 8 * stage, sa, cc * p.Ck, w_base + kw, h_base + kh, b);
-          tma_load_3d(&tmB, bar_full + 8 * stage, sa + p.a_bytes, cc * p.Ck, 0, tap);
-        }
-        __syncwarp();
+        mbar_expect_tx(bar_full + 8 * stage, stage_bytes);
+        const uint32_t sa = stage0 + stage * stage_bytes;
+        tma_load_4d(&tmA, bar_full + 8 * stage, sa, cc * p.Ck, w_base + kw, h_base + kh, b);
+        tma_load_3d(&tmB, bar_full + 8 * stage, sa + p.a_bytes, cc * p.Ck, 0, tap);
         if (++stage == p.nstages) { stage = 0; phase ^= 1; }
         if (++cc == cchunks) { cc = 0; ++tap; if (++kw == p.taps_w) { kw = 0; ++kh; } }
       }
     }
-  } else if (warp == 1) {
-    const bool leader = elect_one_sync();
-    uint32_t stage = 0, phase = 0, acc = 0, acc_phase = 0;
-    const uint32_t dhi = desc_hi((p.swizzle == 128) ? 1024u : 512u, (p.swizzle == 128) ? 2u : 4u);
-    for (int tile = blockIdx.x; tile < p.num_tiles; tile += gridDim.x) {
-      mbar_wait(bar_tempty + 8 * acc, acc_phase ^ 1);
-      tc_fence_after();
-      const uint32_t d_tmem = tmem_base + acc * (uint32_t)N;
-      for (int kb = 0; kb < p.kblocks; ++kb) {
-        mbar_wait(bar_full + 8 * stage, phase);
-        tc_fence_after();
-        if (leader) {
-          const uint32_t sa = stage0 + stage * stage_bytes;
-          const uint32_t alo = desc_lo(sa), blo = desc_lo(sa + p.a_bytes);
-          // +32 B per K=16 step inside the swizzle row: the start-address field is in 16 B units
-          tc_mma_f16(d_tmem, desc_from(dhi, alo), desc_from(dhi, blo), p.idesc, kb != 0);
-          tc_mma_f16(d_tmem, desc_from(dhi, alo + 2), desc_from(dhi, blo + 2), p.idesc, 1);
-          if (ksteps == 4) {
-            tc_mma_f16(d_tmem, desc_from(dhi, alo + 4), desc_from(dhi, blo + 4), p.idesc, 1);
-            tc_mma_f16(d_tmem, desc_from(dhi, alo + 6), desc_from(dhi, blo + 6), p.idesc, 1);
-          }
-          tc_commit(bar_empty + 8 * stage);   // frees the smem stage once these MMAs have read it
-        }
-        __syncwarp();
-        if (++stage == p.nstages) { stage = 0; phase ^= 1; }
-      }
-      if (leader) tc_commit(bar_tfull + 8 * acc);   // accumulator complete -> epilogue
-      __syncwarp();
-      acc ^= 1;
-      if (acc == 0) acc_phase ^= 1;
-    }
-  } else {
-    const int q = warp & 3;                   // TMEM lane quadrant this warp may access
-    uint32_t acc = 0, acc_phase = 0;
-    for (int tile = blockIdx.x; tile < p.num_tiles; tile += gridDim.x) {
-      const int wt = tile % p.tiles_w;
-      const int bh = tile / p.tiles_w;        // = b * H_out + h
-      mbar_wait(bar_tfull + 8 * acc, acc_phase);
-      tc_fence_after();
-      const int w = wt * kTileM + q * 32 + lane;
-      const bool valid = w < p.W_out;
-      const size_t pix = ((size_t)bh * p.W_out + (valid ? w : 0)) * (size_t)N;
-      const uint32_t taddr = tmem_base + ((uint32_t)(q * 32) << 16) + acc * (uint32_t)N;
-      for (int n0 = 0; n0 < N; n0 += 32) {
-        uint32_t r[32];
-        tc_ld32(taddr + n0, r);
-        if (valid) {
-          float v[32];
-#pragma unroll
-          for (int j = 0; j < 32; ++j) v[j] = __uint_as_float(r[j]) + s_bias[n0 + j];
-          if (p.residual) {
-            const uint4* rp = reinterpret_cast<const uint4*>(p.residual + pix + n0);
-#pragma unroll
-            for (int j4 = 0; j4 < 4; ++j4) {
-              uint4 u = __ldg(rp + j4);
-              const __half2* h2 = reinterpret_cast<const __half2*>(&u);
-#pragma unroll
-              for (int e = 0; e < 4; ++e) {
-                float2 f = __half22float2(h2[e]);
-                v[j4 * 8 + 2 * e] += f.x;
-                v[j4 * 8 + 2 * e + 1] += f.y;
-              }
-            }
-          }
-          uint4* op = reinterpret_cast<uint4*>(p.out + pix + n0);
-#pragma unroll
-          for (int j4 = 0; j4 < 4; ++j4) {
-            uint4 u;
-            __half2* h2 = reinterpret_cast<__half2*>(&u);
-#pragma unroll
-            for (int e = 0; e < 4; ++e) {
-              float a = v[j4 * 8 + 2 * e], c = v[j4 * 8 + 2 * e + 1];
-              if (p.relu) { a = fmaxf(a, 0.f); c = fmaxf(c, 0.f); }
-              h2[e] = __floats2half2_rn(a, c);
-            }
-            op[j4] = u;
-          }
-        }
-      }
-      tc_fence_before();
-      __syncwarp();
-      if (lane == 0) mbar_arrive(bar_tempty + 8 * acc);
-      acc ^= 1;
-      if (acc == 0) acc_phase ^= 1;
-    }
+    return;
   }
 
-  tc_fence_before();
-  __syncthreads();
-  if (warp == 1) {
-    tc_fence_after();
-    asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(tmem_base), "r"(512u));
+  const int wg = warp >> 2;
+  constexpr uint32_t row_bytes = CK * 2;                   // = the swizzle width (64 or 128 B)
+  float acc[N / 2];
+#pragma unroll
+  for (int i = 0; i < N / 2; ++i) acc[i] = 0.f;
+  uint32_t stage = 0, phase = 0, prev = 0;
+  for (int kb = 0; kb < p.kblocks; ++kb) {
+    mbar_wait(bar_full + 8 * stage, phase);
+    const uint32_t sa = stage0 + stage * stage_bytes;
+    const uint64_t ad = wg_desc(sa + (uint32_t)wg * 64u * row_bytes, row_bytes), bd = wg_desc(sa + p.a_bytes, row_bytes);
+    wg_fence();
+#pragma unroll
+    for (int k = 0; k < CK / 16; ++k) Wgmma<N>::mma(acc, ad + 2 * k, bd + 2 * k);   // +32 B per K=16 step
+    wg_commit();
+    wg_wait<1>();                                           // the previous stage's wgmma have read their operands
+    if (kb > 0 && (threadIdx.x & 127) == 0) mbar_arrive(bar_empty + 8 * prev);
+    prev = stage;
+    if (++stage == p.nstages) { stage = 0; phase ^= 1; }
   }
-}
+  wg_wait<0>();
 
-
-// ------------------------------------------------------------------------------------------------
-// conv_tc2_kernel: stride-1 3x3 convolution with shared-memory halo reuse ("strip streaming")
-//
-// A work item is a strip of 128 output columns x R output rows of one image.  The producer streams the R+2 input
-// rows (130 pixels wide: one halo pixel each side, zero filled by TMA at the image border) through a ring of
-// shared-memory slots ONCE; each slot feeds up to 3 output rows (kh) x 3 horizontal taps (kw).  The kw shift is a
-// descriptor trick: the A operand of tap kw starts kw pixel-rows (kw * Ck * 2 bytes) into the slot, with the UMMA
-// descriptor's base_offset field carrying the swizzle phase of the shifted start.  Up to 4 output rows accumulate
-// concurrently in TMEM (4 x N columns).  L2->smem traffic for activations drops 9x against conv_tc_kernel; weights
-// stay resident in shared memory when they fit (C_in * C_out <= 64 x 64), otherwise they stream through a B ring.
-// ------------------------------------------------------------------------------------------------
-struct ConvV2Params {
-  int B, H, W, C_in, C_out;
-  int N, n_halves, Ck, ncc, tiles_w, R, nhseg, num_items, relu;
-  int resident, n_aslots, n_bslots, base_off_mode;
-  const float* bias;
-  const __half* residual;
-  __half* out;
-  uint32_t a_bytes, a_slot_bytes, b_bytes, idesc, swizzle, w_off, a_off, b_off;
-};
-
-__device__ __forceinline__ uint64_t make_kmajor_desc_bo(uint32_t saddr, uint32_t sbo_bytes, uint32_t layout_type,
-                                                        int base_off_mode) {
-  uint64_t d = make_kmajor_desc(saddr, sbo_bytes, layout_type);
-  if (base_off_mode) d |= (uint64_t)((saddr >> 7) & 7u) << 49;
-  return d;
-}
-
-__global__ void __launch_bounds__(kTcThreads, 1)
-conv_tc2_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB, ConvV2Params p) {
-  extern __shared__ uint8_t smem_raw[];
-  const uint32_t raw = smem_u32(smem_raw);
-  const uint32_t base = (raw + 1023u) & ~1023u;
-  uint8_t* gbase = smem_raw + (base - raw);
-  // header: [0,64) a_full  [64,128) a_empty  [128,256) b_full  [256,384) b_empty  [384,416) tfull  [416,448) tempty
-  //         [448,456) wbar  [512,516) tmem slot   [1024,2048) bias
-  const uint32_t bar_afull = base, bar_aempty = base + 64, bar_bfull = base + 128, bar_bempty = base + 256;
-  const uint32_t bar_tfull = base + 384, bar_tempty = base + 416, bar_w = base + 448;
-  uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(gbase + 512);
-  float* s_bias = reinterpret_cast<float*>(gbase + 1024);
-  const uint32_t w_smem = base + p.w_off, a_smem = base + p.a_off, b_smem = base + p.b_off;
-
-  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-  const int N = p.N;
-  for (int i = threadIdx.x; i < p.C_out; i += blockDim.x) s_bias[i] = p.bias[i];
-  if (threadIdx.x == 0) {
-    for (int s = 0; s < p.n_aslots; ++s) { mbar_init(bar_afull + 8 * s, 1); mbar_init(bar_aempty + 8 * s, 1); }
-    for (int s = 0; s < p.n_bslots; ++s) { mbar_init(bar_bfull + 8 * s, 1); mbar_init(bar_bempty + 8 * s, 1); }
-    for (int a = 0; a < 4; ++a) { mbar_init(bar_tfull + 8 * a, 1); mbar_init(bar_tempty + 8 * a, 4); }
-    mbar_init(bar_w, 1);
-    asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
-  }
-  if (warp == 1) {
-    asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(tmem_slot)),
-                 "r"(512u));
-    asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::);
-  }
-  tc_fence_before();
-  __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem_base = *tmem_slot;
-  const int ksteps = p.Ck / 16;
-  const uint32_t rowbytes = p.Ck * 2;
-
-  // item -> (b, wt, hs, nh); nh fastest so that both N halves of a strip run back to back (input rows hit L2)
-  auto decode = [&](int item, int& b, int& wt, int& h0, int& h1, int& nh) {
-    nh = item % p.n_halves;
-    int t = item / p.n_halves;
-    const int hs = t % p.nhseg; t /= p.nhseg;
-    wt = t % p.tiles_w;
-    b = t / p.tiles_w;
-    h0 = hs * p.R;
-    h1 = min(p.H, h0 + p.R);
-  };
-
-  if (warp == 0) {
-    const bool leader = elect_one_sync();
-    if (leader) {
-      asm volatile("prefetch.tensormap [%0];" ::"l"(reinterpret_cast<uint64_t>(&tmA)) : "memory");
-      asm volatile("prefetch.tensormap [%0];" ::"l"(reinterpret_cast<uint64_t>(&tmB)) : "memory");
-      if (p.resident) {
-        mbar_expect_tx(bar_w, 9u * p.ncc * p.b_bytes);
-        for (int tap = 0; tap < 9; ++tap)
-          for (int cc = 0; cc < p.ncc; ++cc)
-            tma_load_3d(&tmB, bar_w, w_smem + (tap * p.ncc + cc) * p.b_bytes, cc * p.Ck, 0, tap);
+  const int lane = threadIdx.x & 31;
+  const int c0 = 2 * (lane & 3);
+#pragma unroll
+  for (int i = 0; i < 2; ++i) {
+    const int w = wt * kTileM + wg * 64 + (warp & 3) * 16 + (lane >> 2) + 8 * i;
+    if (w >= p.W_out) continue;
+    const size_t pix = ((size_t)bh * p.W_out + w) * (size_t)N;
+#pragma unroll
+    for (int j = 0; j < N / 8; ++j) {
+      const int c = 8 * j + c0;
+      const float2 bb = __ldg(reinterpret_cast<const float2*>(p.bias + c));
+      float a = acc[4 * j + 2 * i] + bb.x, d = acc[4 * j + 2 * i + 1] + bb.y;
+      if (p.residual) {
+        const float2 r = __half22float2(*reinterpret_cast<const __half2*>(p.residual + pix + c));
+        a += r.x;
+        d += r.y;
       }
+      if (p.relu) { a = fmaxf(a, 0.f); d = fmaxf(d, 0.f); }
+      *reinterpret_cast<__half2*>(p.out + pix + c) = __floats2half2_rn(a, d);
     }
-    __syncwarp();
-    uint32_t as = 0, aph = 0, bs = 0, bph = 0;
-    for (int item = blockIdx.x; item < p.num_items; item += gridDim.x) {
-      int b, wt, h0, h1, nh;
-      decode(item, b, wt, h0, h1, nh);
-      const int R = h1 - h0;
-      const int w_in = wt * kTileM - 1;
-      for (int t = 0; t < R + 2; ++t) {
-        for (int cc = 0; cc < p.ncc; ++cc) {
-          mbar_wait(bar_aempty + 8 * as, aph ^ 1);
-          if (leader) {
-            mbar_expect_tx(bar_afull + 8 * as, p.a_bytes);
-            tma_load_4d(&tmA, bar_afull + 8 * as, a_smem + as * p.a_slot_bytes, cc * p.Ck, w_in, h0 - 1 + t, b);
-          }
-          __syncwarp();
-          if (++as == (uint32_t)p.n_aslots) { as = 0; aph ^= 1; }
-          if (!p.resident) {
-            for (int kh = 0; kh < 3; ++kh) {
-              const int r = t - kh;
-              if (r < 0 || r >= R) continue;
-              for (int kw = 0; kw < 3; ++kw) {
-                mbar_wait(bar_bempty + 8 * bs, bph ^ 1);
-                if (leader) {
-                  mbar_expect_tx(bar_bfull + 8 * bs, p.b_bytes);
-                  tma_load_3d(&tmB, bar_bfull + 8 * bs, b_smem + bs * p.b_bytes, cc * p.Ck, nh * N, kh * 3 + kw);
-                }
-                __syncwarp();
-                if (++bs == (uint32_t)p.n_bslots) { bs = 0; bph ^= 1; }
-              }
-            }
-          }
-        }
-      }
-    }
-  } else if (warp == 1) {
-    const bool leader = elect_one_sync();
-    const uint32_t dhi = desc_hi((p.swizzle == 128) ? 1024u : 512u, (p.swizzle == 128) ? 2u : 4u);
-    const uint32_t row_units = rowbytes >> 4;             // one pixel row of the slot, in 16 B descriptor units
-    if (p.resident) { mbar_wait(bar_w, 0); tc_fence_after(); }
-    uint32_t as = 0, aph = 0, bs = 0, bph = 0;
-    uint32_t grow = 0;                                    // global output-row counter of this CTA
-    for (int item = blockIdx.x; item < p.num_items; item += gridDim.x) {
-      int b, wt, h0, h1, nh;
-      decode(item, b, wt, h0, h1, nh);
-      const int R = h1 - h0;
-      for (int t = 0; t < R + 2; ++t) {
-        for (int cc = 0; cc < p.ncc; ++cc) {
-          mbar_wait(bar_afull + 8 * as, aph);
-          tc_fence_after();
-          const uint32_t alo0 = desc_lo(a_smem + as * p.a_slot_bytes);
-          for (int kh = 0; kh < 3; ++kh) {
-            const int r = t - kh;
-            if (r < 0 || r >= R) continue;
-            const uint32_t g = grow + (uint32_t)r;
-            const uint32_t acc = g & 3u;
-            if (kh == 0 && cc == 0) {                     // first contribution to output row r
-              mbar_wait(bar_tempty + 8 * acc, ((g >> 2) & 1u) ^ 1u);
-              tc_fence_after();
-            }
-            const uint32_t d_tmem = tmem_base + acc * (uint32_t)N;
-            for (int kw = 0; kw < 3; ++kw) {
-              uint32_t blo;
-              if (p.resident) {
-                blo = desc_lo(w_smem + ((kh * 3 + kw) * p.ncc + cc) * p.b_bytes);
-              } else {
-                mbar_wait(bar_bfull + 8 * bs, bph);
-                tc_fence_after();
-                blo = desc_lo(b_smem + bs * p.b_bytes);
-              }
-              if (leader) {
-                // tap kw = same slot, kw pixel rows further (absolute-address swizzle: base_offset stays 0)
-                const uint32_t alo = alo0 + kw * row_units;
-                tc_mma_f16(d_tmem, desc_from(dhi, alo), desc_from(dhi, blo), p.idesc, (kh | cc | kw) != 0);
-                tc_mma_f16(d_tmem, desc_from(dhi, alo + 2), desc_from(dhi, blo + 2), p.idesc, 1);
-                if (ksteps == 4) {
-                  tc_mma_f16(d_tmem, desc_from(dhi, alo + 4), desc_from(dhi, blo + 4), p.idesc, 1);
-                  tc_mma_f16(d_tmem, desc_from(dhi, alo + 6), desc_from(dhi, blo + 6), p.idesc, 1);
-                }
-                if (!p.resident) tc_commit(bar_bempty + 8 * bs);
-              }
-              __syncwarp();
-              if (!p.resident) {
-                if (++bs == (uint32_t)p.n_bslots) { bs = 0; bph ^= 1; }
-              }
-            }
-            if (kh == 2 && cc == p.ncc - 1) {             // output row r complete
-              if (leader) tc_commit(bar_tfull + 8 * acc);
-              __syncwarp();
-            }
-          }
-          if (leader) tc_commit(bar_aempty + 8 * as);
-          __syncwarp();
-          if (++as == (uint32_t)p.n_aslots) { as = 0; aph ^= 1; }
-        }
-      }
-      grow += (uint32_t)R;
-    }
-  } else {
-    const int q = warp & 3;
-    uint32_t grow = 0;
-    for (int item = blockIdx.x; item < p.num_items; item += gridDim.x) {
-      int b, wt, h0, h1, nh;
-      decode(item, b, wt, h0, h1, nh);
-      const int R = h1 - h0;
-      const int w = wt * kTileM + q * 32 + lane;
-      const bool valid = w < p.W;
-      for (int r = 0; r < R; ++r) {
-        const uint32_t g = grow + (uint32_t)r;
-        const uint32_t acc = g & 3u;
-        const size_t pix = (((size_t)b * p.H + (h0 + r)) * p.W + (valid ? w : 0)) * (size_t)p.C_out + (size_t)nh * N;
-        uint4 rpre[4];
-        auto load_res = [&](int n0) {                    // residual does not depend on the MMAs: prefetch it
-          const uint4* rp = reinterpret_cast<const uint4*>(p.residual + pix + n0);
-#pragma unroll
-          for (int j4 = 0; j4 < 4; ++j4) rpre[j4] = valid ? __ldg(rp + j4) : make_uint4(0, 0, 0, 0);
-        };
-        if (p.residual) load_res(0);
-        mbar_wait(bar_tfull + 8 * acc, (g >> 2) & 1u);
-        tc_fence_after();
-        const uint32_t taddr = tmem_base + ((uint32_t)(q * 32) << 16) + acc * (uint32_t)N;
-        for (int n0 = 0; n0 < N; n0 += 32) {
-          uint32_t rr[32];
-          tc_ld32(taddr + n0, rr);
-          uint4 rcur[4];
-#pragma unroll
-          for (int j4 = 0; j4 < 4; ++j4) rcur[j4] = rpre[j4];
-          if (p.residual && n0 + 32 < N) load_res(n0 + 32);
-          if (valid) {
-            float v[32];
-#pragma unroll
-            for (int j = 0; j < 32; ++j) v[j] = __uint_as_float(rr[j]) + s_bias[nh * N + n0 + j];
-            if (p.residual) {
-#pragma unroll
-              for (int j4 = 0; j4 < 4; ++j4) {
-                uint4 u = rcur[j4];
-                const __half2* h2 = reinterpret_cast<const __half2*>(&u);
-#pragma unroll
-                for (int e = 0; e < 4; ++e) {
-                  float2 f = __half22float2(h2[e]);
-                  v[j4 * 8 + 2 * e] += f.x;
-                  v[j4 * 8 + 2 * e + 1] += f.y;
-                }
-              }
-            }
-            uint4* op = reinterpret_cast<uint4*>(p.out + pix + n0);
-#pragma unroll
-            for (int j4 = 0; j4 < 4; ++j4) {
-              uint4 u;
-              __half2* h2 = reinterpret_cast<__half2*>(&u);
-#pragma unroll
-              for (int e = 0; e < 4; ++e) {
-                float a = v[j4 * 8 + 2 * e], c = v[j4 * 8 + 2 * e + 1];
-                if (p.relu) { a = fmaxf(a, 0.f); c = fmaxf(c, 0.f); }
-                h2[e] = __floats2half2_rn(a, c);
-              }
-              op[j4] = u;
-            }
-          }
-        }
-        tc_fence_before();
-        __syncwarp();
-        if (lane == 0) mbar_arrive(bar_tempty + 8 * acc);
-      }
-      grow += (uint32_t)R;
-    }
-  }
-
-  tc_fence_before();
-  __syncthreads();
-  if (warp == 1) {
-    tc_fence_after();
-    asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(tmem_base), "r"(512u));
-  }
-}
-
-
-// ------------------------------------------------------------------------------------------------
-// conv_tc3_kernel: "channels-as-M" orientation for stride-1 3x3 convolutions
-//
-// Measured (profiles/r01_conv_tc_v1_summary.md, r01_launches_emb_v2): with both operands in shared memory a
-// tcgen05.mma M=128 costs >= 128 cycles per K=16 step because the A operand is read at one 32-byte row per cycle, so
-// the pixels-as-M kernels only balance when N = C_out = 256 (N=128 -> 50 %, 64 -> 25 %, 32 -> 12 % of peak).  Here the
-// roles are swapped:   D[c_out][pixel] += W_tap[c_out][c_in] * X_tap[pixel][c_in]^T
-//   A = weights tile  [128 c_out x Ck]  (rows beyond C_out are zero padding),
-//   B = activation tile [N = 256 pixels x Ck] straight from a TMA box (Ck, bw, bh) with bw*bh <= 256 pixels of one
-//       image (bh > 1 when the image is narrower than 256), zero-filled at the borders, shifted per tap,
-//   N = 256 -> 128 cycles of math per instruction = the A-read time: full tensor rate for C_out >= 128.
-// The accumulator has channels on TMEM lanes and pixels on columns, so the epilogue transposes 32x32 blocks through
-// shared memory to keep NHWC stores (and residual loads) 16-byte vectorised.
-// ------------------------------------------------------------------------------------------------
-struct ConvV3Params {
-  int B, H, W, C_in, C_out;                // H, W: OUTPUT size (the input size only lives in the tensor map)
-  int stride, pad, ksize;                  // 3x3 pad 1 (stride 1 or 2) or 1x1 pad 0 (stride 2: the block shortcuts)
-  int dbg;                                 // timing experiments only (B200_TC3_DBG): 1 = weight loads only for the
-                                           //    first stages, 2 = pixel loads only for the first stages (wrong results)
-  int fold;                                // 1: a stage holds one (kh, channel block): 3 weight taps + ONE pixel box with
-                                           //    a one-pixel halo, the kw taps are descriptor shifts (stride-1 3x3 only)
-  int pitch;                               // accumulator columns per image row of the tile: bw (+ 2 halo columns if fold)
-  int mc;                                  // fold only: CTAs per cluster that share the weight stream (TMA multicast), 1 = off
-  int Ck, ncc, kblocks, bw, bh, tiles_w, tiles_h, m_tiles, num_items, relu;
-  const float* bias;
-  const __half* residual;
-  __half* out;
-  __half* out2;                            // C_split > 0: channels >= C_split go here (no ReLU), see ConvLayer::w3s
-  int C_split;
-  uint32_t a_bytes, b_bytes, stage_bytes, nstages, idesc, swizzle;
-};
-
-constexpr int kV3Threads = 320;          // TMA warp, MMA warp, 2 x 4 epilogue warps (alternate 32-pixel chunks)
-constexpr uint32_t kV3Staging = 16384;   // 8 epilogue warps x 2 KB transpose buffer (residual in, then result out)
-
-__global__ void __launch_bounds__(kV3Threads, 1)
-conv_tc3_kernel(const __grid_constant__ CUtensorMap tmX, const __grid_constant__ CUtensorMap tmW,
-                const __grid_constant__ CUtensorMap tmWs, ConvV3Params p) {
-  extern __shared__ uint8_t smem_raw[];
-  const uint32_t raw = smem_u32(smem_raw);
-  const uint32_t base = (raw + 1023u) & ~1023u;
-  uint8_t* gbase = smem_raw + (base - raw);
-  // [0,64) full  [64,128) empty  [128,144) tfull  [144,160) tempty  [192] tmem slot  [1024,2048) bias
-  // [2048, 2048+16K) epilogue transpose staging (8 warps x 2 KB)  then the stages
-  const uint32_t bar_full = base, bar_empty = base + 64, bar_tfull = base + 128, bar_tempty = base + 144;
-  uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(gbase + 192);
-  float* s_bias = reinterpret_cast<float*>(gbase + 1024);
-  uint8_t* s_stage_ep = gbase + 2048;
-  const uint32_t stage0 = base + 2048 + kV3Staging;
-  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-
-  // Weight multicast (p.mc > 1, folded stride-1 convs): the mc CTAs of a cluster work on mc different pixel tiles of
-  // the same output-channel tile in lockstep; each loads 1/mc of every weight stage and multicasts it to all, so the
-  // L2 -> SM weight traffic (59 % of the kernel's bytes, which ran at the L2 throughput cap) drops by (mc - 1) / mc.
-  // A stage is refilled only when the MMAs of ALL CTAs have released it (multicast tcgen05.commit, count mc).
-  uint32_t crank = 0;
-  if (p.mc > 1) asm volatile("mov.u32 %0, %%cluster_ctarank;" : "=r"(crank));
-  const uint32_t mc = (uint32_t)p.mc;
-  const uint16_t cmask = (uint16_t)((1u << mc) - 1u);
-  const int cluster_id = (int)(blockIdx.x / mc), num_clusters = (int)(gridDim.x / mc);
-
-  for (int i = threadIdx.x; i < p.C_out && i < 256; i += blockDim.x) s_bias[i] = p.bias[i];
-  if (threadIdx.x == 0) {
-    for (uint32_t s = 0; s < p.nstages; ++s) { mbar_init(bar_full + 8 * s, 1); mbar_init(bar_empty + 8 * s, mc); }
-    for (int a = 0; a < 2; ++a) { mbar_init(bar_tfull + 8 * a, 1); mbar_init(bar_tempty + 8 * a, 8); }
-    asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
-  }
-  if (warp == 1) {
-    asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(tmem_slot)),
-                 "r"(512u));
-    asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::);
-  }
-  tc_fence_before();
-  __syncthreads();
-  if (mc > 1)                                              // peers' barriers exist before anything is multicast to them
-    asm volatile("barrier.cluster.arrive.release.aligned;\n\tbarrier.cluster.wait.acquire.aligned;" ::: "memory");
-  tc_fence_after();
-  const uint32_t tmem_base = *tmem_slot;
-  const int ksteps = p.Ck / 16;
-
-  // item -> (b, th, tw, mt); mt fastest; the CTAs of a cluster take consecutive pixel tiles of the same mt (tiles past
-  // the end are ghosts: zero-filled loads, no stores)
-  auto decode = [&](int item, int& b, int& h0, int& w0, int& mt) {
-    mt = item % p.m_tiles;
-    int t = (item / p.m_tiles) * (int)mc + (int)crank;
-    const int tw = t % p.tiles_w; t /= p.tiles_w;
-    const int th = t % p.tiles_h;
-    b = t / p.tiles_h;
-    h0 = th * p.bh;
-    w0 = tw * p.bw;
-  };
-
-  if (warp == 0) {
-    const bool leader = elect_one_sync();
-    if (leader) {
-      asm volatile("prefetch.tensormap [%0];" ::"l"(reinterpret_cast<uint64_t>(&tmX)) : "memory");
-      asm volatile("prefetch.tensormap [%0];" ::"l"(reinterpret_cast<uint64_t>(&tmW)) : "memory");
-    }
-    uint32_t stage = 0, phase = 0;
-    for (int item = cluster_id; item < p.num_items; item += num_clusters) {
-      int b, h0, w0, mt;
-      decode(item, b, h0, w0, mt);
-      int tap = 0, cc = 0, kh = 0, kw = 0;
-      for (int kb = 0; kb < p.kblocks; ++kb) {
-        mbar_wait(bar_empty + 8 * stage, phase ^ 1);
-        if (leader) {
-          if (!(p.fold && p.dbg)) mbar_expect_tx(bar_full + 8 * stage, p.b_bytes);   // bytes delivered by the two boxes
-          const uint32_t sa = stage0 + stage * p.stage_bytes;
-          if (p.fold && p.dbg) {
-            // experiment: after the first pass over the stages one of the two streams is no longer loaded
-            const bool warm = item != (int)blockIdx.x || kb >= (int)p.nstages;
-            const bool do_w = !(warm && p.dbg == 1), do_x = !(warm && p.dbg == 2);
-            asm volatile("mbarrier.arrive.expect_tx.shared::cta.b64 _, [%0], %1;" ::"r"(bar_full + 8 * stage),
-                         "r"((do_w ? p.a_bytes : 0u) + (do_x ? p.b_bytes - p.a_bytes : 0u)) : "memory");
-            if (do_w) tma_load_3d(&tmW, bar_full + 8 * stage, sa, cc * p.Ck, mt * 128, kh * 3);
-            if (do_x) tma_load_4d(&tmX, bar_full + 8 * stage, sa + p.a_bytes, cc * p.Ck, w0 - 1, h0 + kh - 1, b);
-          } else if (p.fold) {
-            // the three horizontal taps of row kh share one pixel box (one-pixel halo left and right, zero filled)
-            if (mc > 1) {
-              const uint32_t rows = 128u / mc, tap_bytes = 128u * (uint32_t)p.Ck * 2u;
-              const uint32_t dst = sa + crank * rows * (uint32_t)p.Ck * 2u;
-#pragma unroll
-              for (int k3 = 0; k3 < 3; ++k3)
-                tma_load_3d_mc(&tmWs, bar_full + 8 * stage, dst + k3 * tap_bytes, cc * p.Ck, mt * 128 + (int)(crank * rows),
-                               kh * 3 + k3, cmask);
-            } else {
-              tma_load_3d(&tmW, bar_full + 8 * stage, sa, cc * p.Ck, mt * 128, kh * 3);
-            }
-            tma_load_4d(&tmX, bar_full + 8 * stage, sa + p.a_bytes, cc * p.Ck, w0 - 1, h0 + kh - 1, b);
-          } else {
-            tma_load_3d(&tmW, bar_full + 8 * stage, sa, cc * p.Ck, mt * 128, tap);
-            // stride 2: the tensor map steps 2 elements along W and H, coordinates stay in input pixels
-            tma_load_4d(&tmX, bar_full + 8 * stage, sa + p.a_bytes, cc * p.Ck, w0 * p.stride + kw - p.pad,
-                        h0 * p.stride + kh - p.pad, b);
-          }
-        }
-        __syncwarp();
-        if (++stage == p.nstages) { stage = 0; phase ^= 1; }
-        if (p.fold) { if (++cc == p.ncc) { cc = 0; ++kh; } }
-        else if (++cc == p.ncc) { cc = 0; ++tap; if (++kw == p.ksize) { kw = 0; ++kh; } }
-      }
-    }
-  } else if (warp == 1) {
-    const bool leader = elect_one_sync();
-    const uint32_t dhi = desc_hi((p.swizzle == 128) ? 1024u : 512u, (p.swizzle == 128) ? 2u : 4u);
-    uint32_t stage = 0, phase = 0, acc = 0, acc_phase = 0;
-    for (int item = cluster_id; item < p.num_items; item += num_clusters) {
-      mbar_wait(bar_tempty + 8 * acc, acc_phase ^ 1);
-      tc_fence_after();
-      const uint32_t d_tmem = tmem_base + acc * 256u;
-      for (int kb = 0; kb < p.kblocks; ++kb) {
-        mbar_wait(bar_full + 8 * stage, phase);
-        tc_fence_after();
-        if (leader) {
-          const uint32_t sa = stage0 + stage * p.stage_bytes;
-          const uint32_t alo = desc_lo(sa), blo = desc_lo(sa + p.a_bytes);
-          if (p.fold) {
-            // tap kw: weight tile kw of the 3-tap box (128 rows x Ck), pixel rows shifted by kw (absolute-address
-            // swizzle: the descriptor start moves by one pixel row, base_offset stays 0)
-            const uint32_t a_tap = (128u * (uint32_t)p.Ck * 2u) >> 4, b_row = ((uint32_t)p.Ck * 2u) >> 4;
-#pragma unroll
-            for (int kw = 0; kw < 3; ++kw) {
-              tc_mma_f16(d_tmem, desc_from(dhi, alo + kw * a_tap), desc_from(dhi, blo + kw * b_row), p.idesc,
-                         (kb | kw) != 0);
-              tc_mma_f16(d_tmem, desc_from(dhi, alo + kw * a_tap + 2), desc_from(dhi, blo + kw * b_row + 2), p.idesc, 1);
-              if (ksteps == 4) {
-                tc_mma_f16(d_tmem, desc_from(dhi, alo + kw * a_tap + 4), desc_from(dhi, blo + kw * b_row + 4), p.idesc, 1);
-                tc_mma_f16(d_tmem, desc_from(dhi, alo + kw * a_tap + 6), desc_from(dhi, blo + kw * b_row + 6), p.idesc, 1);
-              }
-            }
-          } else {
-            tc_mma_f16(d_tmem, desc_from(dhi, alo), desc_from(dhi, blo), p.idesc, kb != 0);
-            tc_mma_f16(d_tmem, desc_from(dhi, alo + 2), desc_from(dhi, blo + 2), p.idesc, 1);
-            if (ksteps == 4) {
-              tc_mma_f16(d_tmem, desc_from(dhi, alo + 4), desc_from(dhi, blo + 4), p.idesc, 1);
-              tc_mma_f16(d_tmem, desc_from(dhi, alo + 6), desc_from(dhi, blo + 6), p.idesc, 1);
-            }
-          }
-          if (mc > 1) tc_commit_mc(bar_empty + 8 * stage, cmask);     // the stage is free in every CTA of the cluster
-          else tc_commit(bar_empty + 8 * stage);
-        }
-        __syncwarp();
-        if (++stage == p.nstages) { stage = 0; phase ^= 1; }
-      }
-      if (leader) tc_commit(bar_tfull + 8 * acc);
-      __syncwarp();
-      acc ^= 1;
-      if (acc == 0) acc_phase ^= 1;
-    }
-  } else {
-    // two warps per TMEM lane quadrant (= block of 32 output channels) take alternate 32-pixel chunks of the tile:
-    // with four warps the transposing epilogue of a residual conv took as long as the tile's MMAs
-    const int q = warp & 3;
-    const int half = (warp - 2) >> 2;
-    // one [32 px][32 ch] fp16 buffer per warp: the residual chunk passes through it first (coalesced 16-byte loads
-    // in, own-channel reads out), then the result goes the other way; halving the staging bought a fifth stage
-    __half* s_out = reinterpret_cast<__half*>(s_stage_ep + (half * 4 + q) * 2048);
-    const int prow = lane >> 2, ppart = lane & 3;          // cooperative 16-byte I/O: 8 pixels x 4 parts per pass
-    uint32_t acc = 0, acc_phase = 0;
-    const int npix = p.pitch * p.bh;                       // accumulator columns in use (halo columns are skipped)
-    for (int item = cluster_id; item < p.num_items; item += num_clusters) {
-      int b, h0, w0, mt;
-      decode(item, b, h0, w0, mt);
-      const int c0 = mt * 128 + q * 32;                    // first channel of this warp
-      const bool ch_ok = c0 < p.C_out;                     // C_out = 64: the upper two quadrants are zero padding
-      const float bias = ch_ok ? s_bias[c0 + lane] : 0.f;
-      // two outputs (conv | folded shortcut): channels >= C_split belong to the second tensor, which has no ReLU
-      const bool second = p.C_split > 0 && c0 >= p.C_split;
-      __half* const outp = second ? p.out2 : p.out;
-      const int cq = second ? c0 - p.C_split : c0;
-      const int cstride = p.C_split > 0 ? p.C_split : p.C_out;
-      const bool relu = p.relu && !second;
-      // global pixel index of the 4 pixels this lane moves per chunk (16-byte pieces), -1 when outside the image
-      long long gp[4], gpn[4];
-      uint4 rpre[4];
-      auto pixels = [&](int n0, long long (&dst)[4]) {
-#pragma unroll
-        for (int i = 0; i < 4; ++i) {
-          const int n = n0 + i * 8 + prow;
-          const int rr = n / p.pitch, x = n - rr * p.pitch;
-          const bool ok = ch_ok && b < p.B && n < npix && x < p.bw && (h0 + rr) < p.H && (w0 + x) < p.W;
-          dst[i] = ok ? (((long long)b * p.H + h0 + rr) * p.W + w0 + x) : -1;
-        }
-      };
-      auto load_res = [&](const long long (&g)[4]) {
-#pragma unroll
-        for (int i = 0; i < 4; ++i)
-          rpre[i] = g[i] >= 0 ? __ldg(reinterpret_cast<const uint4*>(p.residual + g[i] * cstride + cq + ppart * 8))
-                              : make_uint4(0, 0, 0, 0);
-      };
-      const int first = half * 32;
-      if (first < npix) {
-        pixels(first, gp);
-        if (p.residual) load_res(gp);                      // independent of the MMAs: issue before waiting
-      }
-      mbar_wait(bar_tfull + 8 * acc, acc_phase);
-      tc_fence_after();
-      const uint32_t taddr = tmem_base + ((uint32_t)(q * 32) << 16) + acc * 256u;
-      for (int n0 = first; n0 < npix; n0 += 64) {
-        uint32_t r[32];
-        tc_ld32(taddr + n0, r);
-        float v[32];
-#pragma unroll
-        for (int j = 0; j < 32; ++j) v[j] = __uint_as_float(r[j]) + bias;
-        const bool more = n0 + 64 < npix;
-        if (more) pixels(n0 + 64, gpn);
-        if (p.residual) {
-#pragma unroll
-          for (int i = 0; i < 4; ++i) *reinterpret_cast<uint4*>(s_out + (i * 8 + prow) * 32 + ppart * 8) = rpre[i];
-          __syncwarp();
-          if (more) load_res(gpn);                         // prefetch the next chunk's residual
-#pragma unroll
-          for (int j = 0; j < 32; ++j) v[j] += __half2float(s_out[j * 32 + lane]);
-          __syncwarp();                                    // everyone has read before the buffer is overwritten
-        }
-#pragma unroll
-        for (int j = 0; j < 32; ++j) {
-          float a = v[j];
-          if (relu) a = fmaxf(a, 0.f);
-          s_out[j * 32 + lane] = __float2half_rn(a);
-        }
-        __syncwarp();
-#pragma unroll
-        for (int i = 0; i < 4; ++i) {
-          if (gp[i] >= 0)
-            *reinterpret_cast<uint4*>(outp + gp[i] * cstride + cq + ppart * 8) =
-                *reinterpret_cast<const uint4*>(s_out + (i * 8 + prow) * 32 + ppart * 8);
-        }
-        __syncwarp();
-        if (more) {
-#pragma unroll
-          for (int i = 0; i < 4; ++i) gp[i] = gpn[i];
-        }
-      }
-      tc_fence_before();
-      __syncwarp();
-      if (lane == 0) mbar_arrive(bar_tempty + 8 * acc);
-      acc ^= 1;
-      if (acc == 0) acc_phase ^= 1;
-    }
-  }
-
-  tc_fence_before();
-  __syncthreads();
-  if (mc > 1)                                              // no CTA exits while a peer may still signal its barriers
-    asm volatile("barrier.cluster.arrive.release.aligned;\n\tbarrier.cluster.wait.acquire.aligned;" ::: "memory");
-  if (warp == 1) {
-    tc_fence_after();
-    asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(tmem_base), "r"(512u));
-  }
-}
-
-
-// ------------------------------------------------------------------------------------------------
-// conv_tc4_kernel: stride-1 3x3 convolutions with few channels (C = C_in = C_out in {32, 64}): vertical taps folded
-// into N, vertical sum done by the tensor core
-//
-// With C_out = N <= 64 the pixels-as-M kernels pay the 128-cycle A-operand read per MMA for 12-25 % of the tensor rate.
-// Here one MMA of input row t (A = 128 pixels x 16 channels, shifted by kw pixel rows inside the slot) multiplies the
-// weights of all three vertical taps at once:
-//     Q_t[m][(kh, co)] = sum_{kw, ci} X[t][m + kw - 1][ci] * W[kh][kw][co][ci]                N = 3 C
-// and   out[r] = Q_{r-1}[kh=0] + Q_r[kh=1] + Q_{r+1}[kh=2]   needs no data movement at all: the accumulators of
-// consecutive output rows are C-column blocks of a TMEM ring laid out in DESCENDING row order, so the N = 3C columns
-// of input row t land exactly on the blocks of output rows t+1, t, t-1 and the tensor core performs the vertical sum.
-// Every MMA accumulates (blocks are zeroed with tcgen05.st by the epilogue after it has drained them), the ring seam
-// and the strip borders split an MMA into two narrower ones.  3x fewer MMAs than conv_tc2_kernel, and the epilogue
-// reads C columns per row (a shuffle-based horizontal fold measured 2140 cycles per tile, 2/3 of it smem exchange).
-// ------------------------------------------------------------------------------------------------
-struct ConvV4Params {
-  int B, H, W, C, tiles_w, R, nhseg, num_items, relu, n_aslots;
-  int res_pf;                        // residual L2 prefetch distance in rows (0 = off)
-  const float* bias;
-  const __half* residual;
-  __half* out;
-  uint32_t a_bytes, a_slot_bytes, wkw_bytes, swizzle, w_off, a_off;
-  uint32_t ones_off, btile_off;      // C = 64: constant A tile (ones) and B tile (bias) of the bias MMA
-  uint32_t r_off;                    // C = 64 with a residual: n_rslots slots of 16 KB (one residual pixel row each)
-  int n_rslots;
-};
-
-// threads = TMA warp + MMA warp + G epilogue warpgroups of 4 warps (warpgroup k drains the rows r = k (mod G)) + one
-// more TMA warp that streams the residual rows into shared memory (C = 64)
-
-// Ring geometry.  The 512 TMEM columns hold P = 512 / C blocks of C columns.  GHOST = false: all P blocks form the
-// ring and a run of rows that crosses the ring seam is issued as two narrower MMAs (25 % more MMAs for C = 64, and
-// an MMA costs ~105 cycles whatever its N <= 192: scripts/micro/mma_bench.cu).  GHOST = true: the ring has P - 2
-// logical blocks; the two positions after the last real block are "ghosts" of the two blocks at the other end of the
-// ring, so a run that would wrap simply continues into them and EVERY input row is one MMA per (kw, k-step); the
-// epilogue adds the ghost block of the two affected ring slots to the real one (fp32) and zeroes both.
-template <uint32_t P, bool GHOST>
-struct TmemRing {
-  static constexpr uint32_t NBL = GHOST ? P - 2 : P;
-  __device__ static __forceinline__ uint32_t idx(uint32_t g) { return g % NBL; }
-  __device__ static __forceinline__ uint32_t phase(uint32_t g) { return (g / NBL) & 1u; }
-  __device__ static __forceinline__ uint32_t pos(uint32_t i) { return NBL - 1u - i; }          // descending rows
-  __device__ static __forceinline__ uint32_t ghost_pos(uint32_t i) { return 2u * NBL - 1u - i; }   // i >= NBL - 2
-};
-
-#ifdef B200_TC4_DEBUG
-__device__ unsigned int g_tc4_dbg = 0;
-#endif
-template <int C, bool GHOST, int G>
-__global__ void __launch_bounds__(96 + 128 * G, 1)
-conv_tc4_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB,
-                const __grid_constant__ CUtensorMap tmR, ConvV4Params p) {
-  using Ring = TmemRing<512 / C, GHOST>;
-  constexpr uint32_t NBL = Ring::NBL;
-  extern __shared__ uint8_t smem_raw[];
-  const uint32_t raw = smem_u32(smem_raw);
-  const uint32_t base = (raw + 1023u) & ~1023u;
-  uint8_t* gbase = smem_raw + (base - raw);
-  // header: [0,64) a_full  [64,128) a_empty  [128,256) tfull[16]  [256,384) tempty[16]  [384,392) wbar
-  //         [392,424) r_full[4]  [424,456) r_empty[4]  [512,516) tmem slot  [1024,1280) bias
-  const uint32_t bar_afull = base, bar_aempty = base + 64, bar_tfull = base + 128, bar_tempty = base + 256;
-  const uint32_t bar_w = base + 384, bar_rfull = base + 392, bar_rempty = base + 424;
-  uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(gbase + 512);
-  float* s_bias = reinterpret_cast<float*>(gbase + 1024);
-  const uint32_t w_smem = base + p.w_off, a_smem = base + p.a_off;
-
-  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-  // C = 64 (round 2): the bias enters through the tensor core.  The first MMA into a drained accumulator block is
-  //   D[128 px][64 co] = ONES[128][16] * BT[64][16]^T  with accumulate = 0,
-  //   ONES[.][k] = 1 for k in {0, 1, 8, 9},  BT[co][{0, 8}] = fp16(bias) / 2,  BT[co][{1, 9}] = fp16(bias - fp16(bias)) / 2
-  // (22 significant bits of the fp32 bias; both 16-byte halves of a 32-byte row hold the same values, so the tiles do
-  // not depend on the SWIZZLE_32B piece order), and the epilogue neither writes the bias back with tcgen05.st (15 %
-  // of its stall samples, and TMEM port time taken from its own tcgen05.ld) nor loads it (another 15 %: 16 LDS.128
-  // per row): one more MMA per 12.
-  constexpr bool kBiasMma = (C == 64) && !GHOST;
-  if ((int)threadIdx.x < C) s_bias[threadIdx.x] = p.bias[threadIdx.x];
-  if (kBiasMma) {
-    uint4* ones = reinterpret_cast<uint4*>(gbase + p.ones_off);      // 128 rows x 32 B
-    uint4* bt = reinterpret_cast<uint4*>(gbase + p.btile_off);       // 64 rows x 32 B
-    for (int i = threadIdx.x; i < 128 * 2; i += blockDim.x) ones[i] = make_uint4(0x3C003C00u, 0u, 0u, 0u);
-    for (int i = threadIdx.x; i < 64 * 2; i += blockDim.x) {
-      const float b = p.bias[i >> 1];
-      const __half bh = __float2half_rn(b), bl = __float2half_rn(b - __half2float(bh));
-      const __half bh2 = __float2half_rn(0.5f * __half2float(bh)), bl2 = __float2half_rn(0.5f * __half2float(bl));
-      bt[i] = make_uint4((uint32_t)__half_as_ushort(bh2) | ((uint32_t)__half_as_ushort(bl2) << 16), 0u, 0u, 0u);
-    }
-    asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
-  }
-  if (threadIdx.x == 0) {
-    for (int s = 0; s < p.n_aslots; ++s) { mbar_init(bar_afull + 8 * s, 1); mbar_init(bar_aempty + 8 * s, 1); }
-    for (uint32_t a = 0; a < NBL; ++a) { mbar_init(bar_tfull + 8 * a, 1); mbar_init(bar_tempty + 8 * a, 4); }
-    for (int r = 0; r < p.n_rslots; ++r) { mbar_init(bar_rfull + 8 * r, 1); mbar_init(bar_rempty + 8 * r, 4); }
-    mbar_init(bar_w, 1);
-    asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
-  }
-  if (warp == 1) {
-    asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(tmem_slot)),
-                 "r"(512u));
-    asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::);
-  }
-  tc_fence_before();
-  __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem_base = *tmem_slot;
-  // accumulator blocks start from the BIAS (written with tcgen05.st, re-written by the epilogue after it drained a
-  // block): the epilogue then needs no bias load / add (the smem bias loads + dependent FADDs were 45 % of its stall
-  // samples).  Ghost positions start from zero: they are added to a real block.
-  auto st_bias = [&](uint32_t ta, int hb) {                // 32 bias values of half hb from smem -> TMEM columns
-    uint32_t bb[32];
-#pragma unroll
-    for (int j4 = 0; j4 < 8; ++j4) {
-      const uint4 v = reinterpret_cast<const uint4*>(s_bias)[hb * 8 + j4];
-      bb[4 * j4] = v.x; bb[4 * j4 + 1] = v.y; bb[4 * j4 + 2] = v.z; bb[4 * j4 + 3] = v.w;
-    }
-    tc_st32_regs(ta, bb);
-  };
-  __syncthreads();                                         // s_bias visible
-  if (!kBiasMma && warp >= 2) {
-    const uint32_t grp = (uint32_t)(warp - 2) >> 2;
-    const uint32_t lanes0 = (uint32_t)((warp & 3) * 32) << 16;
-    for (uint32_t pos = grp; pos < 512u / C; pos += G) {
-#pragma unroll
-      for (int hb = 0; hb < C / 32; ++hb) {
-        const uint32_t ta = tmem_base + lanes0 + pos * (uint32_t)C + hb * 32;
-        if (pos < NBL) st_bias(ta, hb);
-        else tc_st32_zero(ta);
-      }
-    }
-    tc_wait_st();
-  }
-  tc_fence_before();
-  __syncthreads();
-  tc_fence_after();
-
-  auto decode = [&](int item, int& b, int& wt, int& h0, int& h1) {
-    const int hs = item % p.nhseg;
-    int t = item / p.nhseg;
-    wt = t % p.tiles_w;
-    b = t / p.tiles_w;
-    h0 = hs * p.R;
-    h1 = min(p.H, h0 + p.R);
-  };
-
-  if (warp == 0) {
-    const bool leader = elect_one_sync();
-    if (leader) {
-      asm volatile("prefetch.tensormap [%0];" ::"l"(reinterpret_cast<uint64_t>(&tmA)) : "memory");
-      mbar_expect_tx(bar_w, 3u * p.wkw_bytes);
-      for (int kw = 0; kw < 3; ++kw) tma_load_3d(&tmB, bar_w, w_smem + kw * p.wkw_bytes, 0, 0, kw);
-    }
-    __syncwarp();
-    uint32_t as = 0, aph = 0;
-    for (int item = blockIdx.x; item < p.num_items; item += gridDim.x) {
-      int b, wt, h0, h1;
-      decode(item, b, wt, h0, h1);
-      const int R = h1 - h0;
-      for (int t = 0; t < R + 2; ++t) {
-        mbar_wait(bar_aempty + 8 * as, aph ^ 1);
-        if (leader) {
-          mbar_expect_tx(bar_afull + 8 * as, p.a_bytes);
-          tma_load_4d(&tmA, bar_afull + 8 * as, a_smem + as * p.a_slot_bytes, 0, wt * kTileM - 1, h0 - 1 + t, b);
-        }
-        __syncwarp();
-        if (++as == (uint32_t)p.n_aslots) { as = 0; aph ^= 1; }
-      }
-    }
-  } else if (warp == 1) {
-    const bool leader = elect_one_sync();
-    constexpr uint32_t kSwz128 = (C == 64);
-    const uint32_t dhi = desc_hi(kSwz128 ? 1024u : 512u, kSwz128 ? 2u : 4u);
-    constexpr uint32_t rowbytes = (uint32_t)C * 2u, row_units = rowbytes >> 4;
-    constexpr int ksteps = C / 16;
-    const uint32_t idesc0 = (1u << 4) | ((uint32_t)(kTileM >> 4) << 24);
-    mbar_wait(bar_w, 0);
-    tc_fence_after();
-    uint32_t as = 0, aph = 0, grow = 0;
-    for (int item = blockIdx.x; item < p.num_items; item += gridDim.x) {
-      int b, wt, h0, h1;
-      decode(item, b, wt, h0, h1);
-      const int R = h1 - h0;
-      for (int t = 0; t < R + 2; ++t) {                    // input row h0 - 1 + t feeds output rows t, t-1, t-2
-        mbar_wait(bar_afull + 8 * as, aph);
-        tc_fence_after();
-        if (t < R) {                                       // output row t receives its first contribution
-          const uint32_t g = grow + (uint32_t)t;
-          mbar_wait(bar_tempty + 8 * Ring::idx(g), Ring::phase(g) ^ 1u);
-          tc_fence_after();
-          if (kBiasMma && leader) {                        // the block starts from the bias (overwrites the old row)
-            const uint32_t d32 = desc_hi(256u, 6u);        // 32-byte rows, SWIZZLE_32B, 8-row groups of 256 B
-            tc_mma_f16(tmem_base + Ring::pos(Ring::idx(g)) * (uint32_t)C, desc_from(d32, desc_lo(base + p.ones_off)),
-                       desc_from(d32, desc_lo(base + p.btile_off)), idesc0 | (((uint32_t)C >> 3) << 17), 0);
-          }
-        }
-        const uint32_t alo0 = desc_lo(a_smem + as * p.a_slot_bytes);
-        const int r_lo = max(t - 2, 0);
-        int ra = min(t, R - 1);
-        while (ra >= r_lo) {                               // runs of rows whose blocks are contiguous in TMEM
-          int rb = r_lo;
-          if (!GHOST) {                                    // the ring seam splits the run (TMEM columns do not wrap:
-                                                           // a run past column 511 faults, measured)
-            rb = ra;
-            while (rb > r_lo && Ring::idx(grow + (uint32_t)rb) != 0u) --rb;
-          }
-          const uint32_t N = (uint32_t)(ra - rb + 1) * (uint32_t)C;
-          // GHOST: a run that wraps continues into the ghost positions behind the last real block
-          const uint32_t d_tmem = tmem_base + Ring::pos(Ring::idx(grow + (uint32_t)ra)) * (uint32_t)C;
-          const uint32_t idesc = idesc0 | ((N >> 3) << 17);
-          const uint32_t bofs = (uint32_t)(t - ra) * (uint32_t)C * rowbytes;   // first vertical tap of this run
-          if (leader) {
-#pragma unroll
-            for (int kw = 0; kw < 3; ++kw) {
-              const uint32_t alo = alo0 + kw * row_units;  // absolute-address swizzle: base_offset stays 0
-              const uint32_t blo = desc_lo(w_smem + kw * p.wkw_bytes + bofs);
-#pragma unroll
-              for (int ks = 0; ks < ksteps; ++ks)
-                tc_mma_f16(d_tmem, desc_from(dhi, alo + 2 * ks), desc_from(dhi, blo + 2 * ks), idesc, 1);
-            }
-          }
-          __syncwarp();
-          ra = rb - 1;
-        }
-        if (leader) {
-          tc_commit(bar_aempty + 8 * as);
-          if (t >= 2) tc_commit(bar_tfull + 8 * Ring::idx(grow + (uint32_t)(t - 2)));   // row t-2 complete
-        }
-        __syncwarp();
-        if (++as == (uint32_t)p.n_aslots) { as = 0; aph ^= 1; }
-      }
-      grow += (uint32_t)R;
-    }
-  } else if (warp == 2 + 4 * G) {
-    // residual rows -> shared memory (C = 64): loaded from global memory in the epilogue they were its critical path
-    // (65 % of the stall samples of a residual conv sat on the first use of the residual registers, tensor pipe 36 %
-    // active); a dedicated TMA warp runs n_rslots rows ahead of the epilogue instead
-    if (kBiasMma && p.residual != nullptr && p.n_rslots > 0) {
-      const bool leader = elect_one_sync();
-      uint32_t g = 0;
-      for (int item = blockIdx.x; item < p.num_items; item += gridDim.x) {
-        int b, wt, h0, h1;
-        decode(item, b, wt, h0, h1);
-        const int R = h1 - h0;
-        for (int r = 0; r < R; ++r, ++g) {
-          const uint32_t rs = g % (uint32_t)p.n_rslots, rph = (g / (uint32_t)p.n_rslots) & 1u;
-          mbar_wait(bar_rempty + 8 * rs, rph ^ 1u);
-          if (leader) {
-            mbar_expect_tx(bar_rfull + 8 * rs, 16384u);
-            tma_load_4d(&tmR, bar_rfull + 8 * rs, base + p.r_off + rs * 16384u, 0, wt * kTileM, h0 + r, b);
-          }
-          __syncwarp();
-        }
-      }
-    }
-  } else {
-    // G epilogue warpgroups take the rows round robin: the epilogue is a chain of TMEM / memory round trips, more
-    // warps in flight hide them
-    const int q = warp & 3;
-    const uint32_t grp = (uint32_t)(warp - 2) >> 2;
-    constexpr int NJ = C / 8;                              // 16-byte pieces per pixel
-    uint32_t grow = 0;
-    for (int item = blockIdx.x; item < p.num_items; item += gridDim.x) {
-      int b, wt, h0, h1;
-      decode(item, b, wt, h0, h1);
-      const int R = h1 - h0;
-      const int w = wt * kTileM + q * 32 + lane;
-      const bool valid = w < p.W;
-      // residual rows are software-pipelined one row of this group ahead (registers): with the load issued right
-      // before the accumulator wait the epilogue stalled on it for 16 % of its samples and the MMA warp waited for
-      // TMEM blocks a third of the time (ncu, layer2 conv2)
-      uint4 rpre[NJ], rnext[NJ];
-      auto res_row = [&](int r) { return (((size_t)b * p.H + (h0 + r)) * p.W + (valid ? w : 0)) * (size_t)C; };
-      auto load_res = [&](int r, uint4 (&dst)[NJ]) {
-        const uint4* rp = reinterpret_cast<const uint4*>(p.residual + res_row(r));
-#pragma unroll
-        for (int j4 = 0; j4 < NJ; ++j4) dst[j4] = valid ? __ldg(rp + j4) : make_uint4(0, 0, 0, 0);
-      };
-      const int r_first = (int)((grp + G - (grow % G)) % G); // first row of this item handled by this warpgroup
-      constexpr bool kPipe = (G == 2);                       // register-prefetch the next row only when registers allow
-      const bool res_regs = p.residual && (!kBiasMma || p.n_rslots == 0);   // residual from global memory (registers)
-      if (res_regs && kPipe && r_first < R) load_res(r_first, rpre);
-      for (int r = r_first; r < R; r += G) {
-        const uint32_t g = grow + (uint32_t)r;
-        const uint32_t blk = Ring::idx(g);
-        const size_t pix = res_row(r);
-        if (res_regs) {
-          // rows further ahead: pull them into L2 (one 64/128-byte pixel per thread)
-          if (p.res_pf && valid && r + p.res_pf < R) {
-            const __half* nxt = p.residual + pix + (size_t)p.res_pf * p.W * C;
-            asm volatile("prefetch.global.L2 [%0];" ::"l"(nxt));
-            if (C == 64) asm volatile("prefetch.global.L2 [%0];" ::"l"(nxt + 32));
-          }
-          if (kPipe) { if (r + G < R) load_res(r + G, rnext); }
-          else load_res(r, rpre);
-        }
-        mbar_wait(bar_tfull + 8 * blk, Ring::phase(g));
-        tc_fence_after();
-        const uint32_t lanes = (uint32_t)(q * 32) << 16;
-        const uint32_t taddr = tmem_base + lanes + Ring::pos(blk) * (uint32_t)C;
-        const bool has_ghost = GHOST && blk >= NBL - 2u;   // warp-uniform
-        const uint32_t gaddr = tmem_base + lanes + Ring::ghost_pos(blk) * (uint32_t)C;
-        uint4* op = reinterpret_cast<uint4*>(p.out + pix);
-        const __half2 zero2 = __floats2half2_rn(0.f, 0.f);
-        if constexpr (kBiasMma) {
-          // the block needs nothing written back: both halves of the row are read with one wait and the block is
-          // released before the conversion / stores
-          uint32_t acc[C];
-          static_assert(C == 64 || !kBiasMma, "the bias-MMA epilogue reads 64 columns");
-          tc_ld64(taddr, acc);
-          tc_fence_before();
-          __syncwarp();
-          if (lane == 0) mbar_arrive(bar_tempty + 8 * blk);
-          if (p.residual && p.n_rslots > 0) {
-            // this thread's pixel row of the residual slot (TMA SWIZZLE_128B: 16-byte piece j sits at j ^ (row & 7))
-            const uint32_t rs = g % (uint32_t)p.n_rslots, rph = (g / (uint32_t)p.n_rslots) & 1u;
-            mbar_wait(bar_rfull + 8 * rs, rph);
-            const int m = q * 32 + lane;
-            const uint8_t* rrow = gbase + p.r_off + rs * 16384u + (uint32_t)m * 128u;
-#pragma unroll
-            for (int j4 = 0; j4 < NJ; ++j4) rpre[j4] = *reinterpret_cast<const uint4*>(rrow + ((j4 ^ (m & 7)) << 4));
-            // generic-proxy reads, then the async proxy (TMA) overwrites the slot: without this fence the arrive
-            // overtook the loads (wrong residuals now and then; found with the B200_TC4_DEBUG compare below)
-            asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
-#ifdef B200_TC4_DEBUG
-            if (valid) {                                   // compare with the residual in global memory (not yet overwritten)
-              const uint4* rp = reinterpret_cast<const uint4*>(p.residual + res_row(r));
-              for (int j4 = 0; j4 < NJ; ++j4) {
-                const uint4 gv = rp[j4];
-                if (gv.x != rpre[j4].x || gv.y != rpre[j4].y || gv.z != rpre[j4].z || gv.w != rpre[j4].w) {
-                  if (atomicAdd(&g_tc4_dbg, 1u) < 12u)
-                    printf("tc4 residual mismatch: blk %d item %d r %d g %u rs %u m %d j4 %d smem %08x global %08x\n",
-                           (int)blockIdx.x, item, r, g, rs, m, j4, rpre[j4].x, gv.x);
-                  break;
-                }
-              }
-            }
-#endif
-            __syncwarp();
-            if (lane == 0) mbar_arrive(bar_rempty + 8 * rs);
-          }
-          if (valid) {
-#pragma unroll
-            for (int j4 = 0; j4 < NJ; ++j4) {
-              float v[8];
-#pragma unroll
-              for (int e = 0; e < 8; ++e) v[e] = __uint_as_float(acc[j4 * 8 + e]);
-              if (p.residual) {
-                const __half2* h2 = reinterpret_cast<const __half2*>(&rpre[j4]);
-#pragma unroll
-                for (int e = 0; e < 4; ++e) {
-                  const float2 f = __half22float2(h2[e]);
-                  v[2 * e] += f.x;
-                  v[2 * e + 1] += f.y;
-                }
-              }
-              uint4 u;
-              __half2* o2 = reinterpret_cast<__half2*>(&u);
-#pragma unroll
-              for (int e = 0; e < 4; ++e) {
-                const __half2 hv = __floats2half2_rn(v[2 * e], v[2 * e + 1]);
-                o2[e] = p.relu ? __hmax2(hv, zero2) : hv;
-              }
-              op[j4] = u;
-            }
-          }
-        } else
-#pragma unroll
-        for (int hb = 0; hb < C / 32; ++hb) {              // 32 columns at a time (register budget)
-          uint32_t acc[32];
-          tc_ld32(taddr + hb * 32, acc);
-          if (!kBiasMma) st_bias(taddr + hb * 32, hb);     // hand the block back holding the bias
-          if (has_ghost) {
-            uint32_t gacc[32];
-            tc_ld32(gaddr + hb * 32, gacc);
-            tc_st32_zero(gaddr + hb * 32);
-#pragma unroll
-            for (int j = 0; j < 32; ++j) acc[j] = __float_as_uint(__uint_as_float(acc[j]) + __uint_as_float(gacc[j]));
-          }
-          if (hb == C / 32 - 1) {
-            if (!kBiasMma) tc_wait_st();
-            tc_fence_before();
-            __syncwarp();
-            if (lane == 0) mbar_arrive(bar_tempty + 8 * blk);
-          }
-          if (valid) {
-#pragma unroll
-            for (int jj = 0; jj < 4; ++jj) {
-              const int j4 = hb * 4 + jj;
-              float v[8] = {__uint_as_float(acc[jj * 8 + 0]), __uint_as_float(acc[jj * 8 + 1]),
-                            __uint_as_float(acc[jj * 8 + 2]), __uint_as_float(acc[jj * 8 + 3]),
-                            __uint_as_float(acc[jj * 8 + 4]), __uint_as_float(acc[jj * 8 + 5]),
-                            __uint_as_float(acc[jj * 8 + 6]), __uint_as_float(acc[jj * 8 + 7])};
-              if (p.residual) {
-                const __half2* h2 = reinterpret_cast<const __half2*>(&rpre[j4]);
-#pragma unroll
-                for (int e = 0; e < 4; ++e) {
-                  const float2 f = __half22float2(h2[e]);
-                  v[2 * e] += f.x;
-                  v[2 * e + 1] += f.y;
-                }
-              }
-              uint4 u;
-              __half2* o2 = reinterpret_cast<__half2*>(&u);
-#pragma unroll
-              for (int e = 0; e < 4; ++e) {
-                const __half2 hv = __floats2half2_rn(v[2 * e], v[2 * e + 1]);
-                o2[e] = p.relu ? __hmax2(hv, zero2) : hv;   // relu after rounding == rounding after relu
-              }
-              op[j4] = u;
-            }
-          }
-        }
-        if (kPipe && p.residual && r + G < R) {
-#pragma unroll
-          for (int j4 = 0; j4 < NJ; ++j4) rpre[j4] = rnext[j4];
-        }
-      }
-      grow += (uint32_t)R;
-    }
-  }
-
-  tc_fence_before();
-  __syncthreads();
-  if (warp == 1) {
-    tc_fence_after();
-    asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(tmem_base), "r"(512u));
   }
 }
 
 // ------------------------------------------------------------------------------------------------
-// conv_block32_kernel: a whole BasicBlock of layer1 (32 -> 32 -> 32 channels, stride 1, identity shortcut) in one pass
-//
-//     out = relu(conv2(relu(conv1(x) + b1)) + b2 + x)                    (resnet.py BasicBlock.forward, BN folded)
-//
-// conv_tc4_kernel pairs are HBM-limited on layer1 (a 256-segment sub-batch moves 5 x 1.3 GB per block).  Here the
-// intermediate activation never leaves the SM: conv1 accumulates rows in TMEM ring 1 (vertical fold as in
-// conv_tc4_kernel), epilogue warps 2-5 turn a finished row into fp16 and write it -- zero padded outside the image --
-// straight into a shared-memory slot in the swizzled K-major layout TMA would have produced, and conv2 consumes those
-// slots as its A operand into TMEM ring 2; epilogue warps 6-9 add bias + residual (re-read from L2) and store.
-// A tile yields 126 output columns: conv1 evaluates 128 (one halo column each side), the input slot holds 130.
-// ------------------------------------------------------------------------------------------------
-struct ConvBlkParams {
-  int B, H, W, tiles_w, R, nhseg, num_items, n_islots, n_mslots, lag;
-  const float* bias1;
-  const float* bias2;
-  const __half* in;
-  __half* out;
-  uint32_t slot_bytes, w1_off, w2_off, i_off, m_off;
-};
-
-constexpr int kBlkThreads = 608;   // TMA warp, conv1 MMA warp, 2 x 4 epilogue-1 warps, 2 x 4 epilogue-2 warps, conv2 MMA warp
-
-template <bool GHOST>
-__global__ void __launch_bounds__(kBlkThreads, 1)
-conv_block32_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB1,
-                    const __grid_constant__ CUtensorMap tmB2, ConvBlkParams p) {
-  // two TMEM rings of 8 positions x 32 columns: 8 logical blocks, or 6 + 2 ghost positions (see TmemRing)
-  using Ring = TmemRing<8, GHOST>;
-  constexpr uint32_t NBL = Ring::NBL;
-  extern __shared__ uint8_t smem_raw[];
-  const uint32_t raw = smem_u32(smem_raw);
-  const uint32_t base = (raw + 1023u) & ~1023u;
-  uint8_t* gbase = smem_raw + (base - raw);
-  const uint32_t bar_ifull = base, bar_iempty = base + 64, bar_mfull = base + 128, bar_mempty = base + 192;
-  const uint32_t bar_t1full = base + 256, bar_t1empty = base + 320, bar_t2full = base + 384, bar_t2empty = base + 448;
-  const uint32_t bar_w = base + 512;
-  uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(gbase + 576);
-  float* s_b1 = reinterpret_cast<float*>(gbase + 1024);
-  float* s_b2 = reinterpret_cast<float*>(gbase + 1152);
-  const uint32_t w1_smem = base + p.w1_off, w2_smem = base + p.w2_off;
-  const uint32_t i_smem = base + p.i_off, m_smem = base + p.m_off;
-  constexpr uint32_t kWkw = 3u * 32 * 32 * 2;               // one horizontal tap of a conv: [(kh, co) = 96][ci = 32] fp16
-
-  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-  if (threadIdx.x < 32) { s_b1[threadIdx.x] = p.bias1[threadIdx.x]; s_b2[threadIdx.x] = p.bias2[threadIdx.x]; }
-  if (threadIdx.x == 0) {
-    for (int s = 0; s < 8; ++s) {
-      mbar_init(bar_ifull + 8 * s, 1); mbar_init(bar_iempty + 8 * s, 1);
-      mbar_init(bar_mfull + 8 * s, 4); mbar_init(bar_mempty + 8 * s, 1);
-      mbar_init(bar_t1full + 8 * s, 1); mbar_init(bar_t1empty + 8 * s, 4);
-      mbar_init(bar_t2full + 8 * s, 1); mbar_init(bar_t2empty + 8 * s, 4);
-    }
-    mbar_init(bar_w, 1);
-    asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
-  }
-  if (warp == 1) {
-    asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(tmem_slot)),
-                 "r"(512u));
-    asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::);
-  }
-  tc_fence_before();
-  __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem_base = *tmem_slot;
-  // ring blocks start from the bias of their conv (see conv_tc4_kernel), ghost positions from zero
-  auto st_bias = [&](uint32_t ta, const float* sb) {       // the 32 bias values of a conv from smem -> TMEM columns
-    uint32_t bb[32];
-#pragma unroll
-    for (int j4 = 0; j4 < 8; ++j4) {
-      const uint4 v = reinterpret_cast<const uint4*>(sb)[j4];
-      bb[4 * j4] = v.x; bb[4 * j4 + 1] = v.y; bb[4 * j4 + 2] = v.z; bb[4 * j4 + 3] = v.w;
-    }
-    tc_st32_regs(ta, bb);
-  };
-  __syncthreads();                                          // s_b1 / s_b2 visible
-  if (warp >= 2 && warp < 18) {
-    const uint32_t grp = (uint32_t)(warp - 2) >> 2;         // 4 warpgroups x 128 columns: 0,1 -> ring 1, 2,3 -> ring 2
-    const uint32_t t0 = tmem_base + ((uint32_t)((warp & 3) * 32) << 16) + grp * 128u;
-#pragma unroll
-    for (int c = 0; c < 4; ++c) {
-      const uint32_t pos = (grp & 1u) * 4u + (uint32_t)c;  // position inside the ring
-      if (pos < NBL) st_bias(t0 + c * 32, grp < 2 ? s_b1 : s_b2);
-      else tc_st32_zero(t0 + c * 32);
-    }
-    tc_wait_st();
-  }
-  tc_fence_before();
-  __syncthreads();
-  tc_fence_after();
-
-  auto decode = [&](int item, int& b, int& wt, int& h0, int& h1) {
-    const int hs = item % p.nhseg;
-    int t = item / p.nhseg;
-    wt = t % p.tiles_w;
-    b = t / p.tiles_w;
-    h0 = hs * p.R;
-    h1 = min(p.H, h0 + p.R);
-  };
-
-  if (warp == 0) {
-    // ---- TMA producer: both weight sets once, then input rows h0-2 .. h1+1 of every item -----------------------
-    const bool leader = elect_one_sync();
-    if (leader) {
-      asm volatile("prefetch.tensormap [%0];" ::"l"(reinterpret_cast<uint64_t>(&tmA)) : "memory");
-      mbar_expect_tx(bar_w, 6u * kWkw);
-      for (int kw = 0; kw < 3; ++kw) {
-        tma_load_3d(&tmB1, bar_w, w1_smem + kw * kWkw, 0, 0, kw);
-        tma_load_3d(&tmB2, bar_w, w2_smem + kw * kWkw, 0, 0, kw);
-      }
-    }
-    __syncwarp();
-    uint32_t is = 0, iph = 0;
-    for (int item = blockIdx.x; item < p.num_items; item += gridDim.x) {
-      int b, wt, h0, h1;
-      decode(item, b, wt, h0, h1);
-      const int R = h1 - h0;
-      for (int t = 0; t < R + 4; ++t) {
-        mbar_wait(bar_iempty + 8 * is, iph ^ 1);
-        if (leader) {
-          mbar_expect_tx(bar_ifull + 8 * is, 130u * 64u);
-          tma_load_4d(&tmA, bar_ifull + 8 * is, i_smem + is * p.slot_bytes, 0, wt * 126 - 2, h0 - 2 + t, b);
-        }
-        __syncwarp();
-        if (++is == (uint32_t)p.n_islots) { is = 0; iph ^= 1; }
-      }
-    }
-  } else if (warp == 1 || warp == 18) {
-    // ---- MMA issuers: warp 1 runs conv1 over the input rows, warp 18 runs conv2 over the intermediate rows.  One warp
-    // issuing both convs spent as long on its own scalar bookkeeping as the tensor pipe needs for the MMAs (ncu: pipe
-    // 31 % active, the issuing warp back-pressured only 37 % of the time); the two instruction streams are independent
-    // (different rings, the data dependency conv1 -> epilogue 1 -> conv2 goes through the mfull barriers).
-    const bool leader = elect_one_sync();
-    const uint32_t dhi = desc_hi(512u, 4u);                 // 64-byte rows, SWIZZLE_64B
-    const uint32_t idesc0 = (1u << 4) | ((uint32_t)(kTileM >> 4) << 24);
-    mbar_wait(bar_w, 0);
-    tc_fence_after();
-    // rows [lo, hi] (descending, hi first) of a ring receive the vertical taps tap0, tap0+1, ... of source row `src`
-    auto fold = [&](uint32_t slot_addr, uint32_t w_addr, uint32_t ring_col, uint32_t grow, int src, int lo, int hi) {
-      const uint32_t alo0 = desc_lo(slot_addr);
-      int ra = hi;
-      while (ra >= lo) {
-        int rb = lo;
-        if (!GHOST) {                                       // the ring seam splits the run
-          rb = ra;
-          while (rb > lo && Ring::idx(grow + (uint32_t)rb) != 0u) --rb;
-        }
-        const uint32_t N = (uint32_t)(ra - rb + 1) * 32u;
-        const uint32_t d_tmem = tmem_base + ring_col + Ring::pos(Ring::idx(grow + (uint32_t)ra)) * 32u;
-        const uint32_t idesc = idesc0 | ((N >> 3) << 17);
-        const uint32_t bofs = (uint32_t)(src - ra) * 32u * 64u;
-        if (leader) {
-#pragma unroll
-          for (int kw = 0; kw < 3; ++kw) {
-            const uint32_t alo = alo0 + kw * 4u;            // one pixel row = 64 bytes = 4 descriptor units
-            const uint32_t blo = desc_lo(w_addr + kw * kWkw + bofs);
-            tc_mma_f16(d_tmem, desc_from(dhi, alo), desc_from(dhi, blo), idesc, 1);
-            tc_mma_f16(d_tmem, desc_from(dhi, alo + 2), desc_from(dhi, blo + 2), idesc, 1);
-          }
-        }
-        __syncwarp();
-        ra = rb - 1;
-      }
-    };
-    if (warp == 1) {
-      uint32_t is = 0, iph = 0, grow1 = 0;
-      for (int item = blockIdx.x; item < p.num_items; item += gridDim.x) {
-        int b, wt, h0, h1;
-        decode(item, b, wt, h0, h1);
-        const int R1 = h1 - h0 + 2;                           // intermediate rows
-        for (int t = 0; t < R1 + 2; ++t) {                    // input row h0 - 2 + t feeds intermediate rows t, t-1, t-2
-          mbar_wait(bar_ifull + 8 * is, iph);
-          tc_fence_after();
-          if (t < R1) {
-            const uint32_t g = grow1 + (uint32_t)t;
-            mbar_wait(bar_t1empty + 8 * Ring::idx(g), Ring::phase(g) ^ 1u);
-            tc_fence_after();
-          }
-          fold(i_smem + is * p.slot_bytes, w1_smem, 0u, grow1, t, max(t - 2, 0), min(t, R1 - 1));
-          if (leader) {
-            tc_commit(bar_iempty + 8 * is);
-            if (t >= 2) tc_commit(bar_t1full + 8 * Ring::idx(grow1 + (uint32_t)(t - 2)));
-          }
-          __syncwarp();
-          if (++is == (uint32_t)p.n_islots) { is = 0; iph ^= 1; }
-        }
-        grow1 += (uint32_t)R1;
-      }
-    } else {
-      uint32_t grow1 = 0, grow2 = 0;                          // intermediate row g lives in slot g % 8
-      for (int item = blockIdx.x; item < p.num_items; item += gridDim.x) {
-        int b, wt, h0, h1;
-        decode(item, b, wt, h0, h1);
-        const int R = h1 - h0, R1 = R + 2;                    // output rows, intermediate rows
-        for (int u = 0; u < R1; ++u) {                        // intermediate row h0 - 1 + u feeds output rows u, u-1, u-2
-          const uint32_t gm = grow1 + (uint32_t)u, ms = gm & 7u, mph = (gm >> 3) & 1u;
-          mbar_wait(bar_mfull + 8 * ms, mph);
-          tc_fence_after();
-          if (u < R) {
-            const uint32_t g = grow2 + (uint32_t)u;
-            mbar_wait(bar_t2empty + 8 * Ring::idx(g), Ring::phase(g) ^ 1u);
-            tc_fence_after();
-          }
-          fold(m_smem + ms * p.slot_bytes, w2_smem, 256u, grow2, u, max(u - 2, 0), min(u, R - 1));
-          if (leader) {
-            tc_commit(bar_mempty + 8 * ms);
-            if (u >= 2) tc_commit(bar_t2full + 8 * Ring::idx(grow2 + (uint32_t)(u - 2)));
-          }
-          __syncwarp();
-        }
-        grow1 += (uint32_t)R1;
-        grow2 += (uint32_t)R;
-      }
-    }
-  } else if (warp < 10) {
-    // ---- epilogue 1 (two warpgroups, alternate rows): ring 1 -> relu(. + b1) -> fp16 -> intermediate slot ----------
-    const int q = warp & 3;
-    const uint32_t grp = (uint32_t)(warp - 2) >> 2;
-    const int m1 = q * 32 + lane;                           // conv1 row of the tile = TMEM lane
-    uint32_t grow1 = 0;
-    for (int item = blockIdx.x; item < p.num_items; item += gridDim.x) {
-      int b, wt, h0, h1;
-      decode(item, b, wt, h0, h1);
-      const int R1 = h1 - h0 + 2;
-      const int c_img = wt * 126 - 1 + m1;
-      const bool col_ok = c_img >= 0 && c_img < p.W;
-      for (int u = 0; u < R1; ++u) {
-        const uint32_t g = grow1 + (uint32_t)u;
-        if ((g & 1u) != grp) continue;
-        const uint32_t blk = Ring::idx(g);
-        const uint32_t ms = g & 7u, mph = (g >> 3) & 1u;
-        const int row_img = h0 - 1 + u;
-        const bool keep = col_ok && row_img >= 0 && row_img < p.H;    // zero padding of conv2's input
-        mbar_wait(bar_t1full + 8 * blk, Ring::phase(g));
-        tc_fence_after();
-        const uint32_t taddr = tmem_base + ((uint32_t)(q * 32) << 16) + Ring::pos(blk) * 32u;
-        uint32_t acc[32];
-        tc_ld32(taddr, acc);
-        st_bias(taddr, s_b1);                               // hand the block back holding b1
-        if (GHOST && blk >= NBL - 2u) {                     // warp-uniform: add the ghost block of this ring slot
-          const uint32_t gaddr = tmem_base + ((uint32_t)(q * 32) << 16) + Ring::ghost_pos(blk) * 32u;
-          uint32_t gacc[32];
-          tc_ld32(gaddr, gacc);
-          tc_st32_zero(gaddr);
-#pragma unroll
-          for (int j = 0; j < 32; ++j) acc[j] = __float_as_uint(__uint_as_float(acc[j]) + __uint_as_float(gacc[j]));
-        }
-        tc_wait_st();
-        tc_fence_before();
-        __syncwarp();
-        if (lane == 0) mbar_arrive(bar_t1empty + 8 * blk);
-        mbar_wait(bar_mempty + 8 * ms, mph ^ 1);            // conv2 has finished reading this slot
-        const uint32_t row_addr = m_smem + ms * p.slot_bytes + (uint32_t)(m1 + 1) * 64u;
-        const uint32_t sw = (row_addr >> 7) & 3u;           // SWIZZLE_64B: 16-byte chunk index ^ address bits [7,9)
-        const __half2 zero2 = __floats2half2_rn(0.f, 0.f);
-#pragma unroll
-        for (int j4 = 0; j4 < 4; ++j4) {
-          uint4 v;
-          __half2* o2 = reinterpret_cast<__half2*>(&v);
-          o2[0] = __hmax2(__floats2half2_rn(__uint_as_float(acc[j4 * 8 + 0]), __uint_as_float(acc[j4 * 8 + 1])), zero2);
-          o2[1] = __hmax2(__floats2half2_rn(__uint_as_float(acc[j4 * 8 + 2]), __uint_as_float(acc[j4 * 8 + 3])), zero2);
-          o2[2] = __hmax2(__floats2half2_rn(__uint_as_float(acc[j4 * 8 + 4]), __uint_as_float(acc[j4 * 8 + 5])), zero2);
-          o2[3] = __hmax2(__floats2half2_rn(__uint_as_float(acc[j4 * 8 + 6]), __uint_as_float(acc[j4 * 8 + 7])), zero2);
-          if (!keep) v = make_uint4(0, 0, 0, 0);
-          const uint32_t a = row_addr + (((uint32_t)j4 ^ sw) << 4);
-          asm volatile("st.shared.v4.b32 [%0], {%1, %2, %3, %4};" ::"r"(a), "r"(v.x), "r"(v.y), "r"(v.z), "r"(v.w)
-                       : "memory");
-        }
-        asm volatile("fence.proxy.async.shared::cta;" ::: "memory");   // generic writes -> tcgen05.mma reads
-        __syncwarp();
-        if (lane == 0) mbar_arrive(bar_mfull + 8 * ms);
-      }
-      grow1 += (uint32_t)R1;
-    }
-  } else {
-    // ---- epilogue 2: ring 2 -> + b2 + residual -> relu -> NHWC store ---------------------------------------------
-    const int q = warp & 3;
-    const uint32_t grp = (uint32_t)(warp - 10) >> 2;
-    const int m = q * 32 + lane;
-    uint32_t grow2 = 0;
-    for (int item = blockIdx.x; item < p.num_items; item += gridDim.x) {
-      int b, wt, h0, h1;
-      decode(item, b, wt, h0, h1);
-      const int R = h1 - h0;
-      const int w = wt * 126 - 1 + m;
-      const bool valid = m >= 1 && m <= 126 && w < p.W;
-      uint4 rpre[4];                                         // residual = block input (L2: just streamed)
-      auto res_row = [&](int r) { return (((size_t)b * p.H + (h0 + r)) * p.W + (valid ? w : 0)) * 32; };
-      const int r_first = (int)((grp - (grow2 & 1u)) & 1u);
-      for (int r = r_first; r < R; r += 2) {
-        const uint32_t g = grow2 + (uint32_t)r;
-        const uint32_t blk = Ring::idx(g);
-        const size_t pix = res_row(r);
-        {
-          const uint4* rp = reinterpret_cast<const uint4*>(p.in + pix);
-#pragma unroll
-          for (int j4 = 0; j4 < 4; ++j4) rpre[j4] = valid ? __ldg(rp + j4) : make_uint4(0, 0, 0, 0);
-        }
-        mbar_wait(bar_t2full + 8 * blk, Ring::phase(g));
-        tc_fence_after();
-        const uint32_t taddr = tmem_base + ((uint32_t)(q * 32) << 16) + 256u + Ring::pos(blk) * 32u;
-        uint32_t acc[32];
-        tc_ld32(taddr, acc);
-        st_bias(taddr, s_b2);                               // hand the block back holding b2
-        if (GHOST && blk >= NBL - 2u) {
-          const uint32_t gaddr = tmem_base + ((uint32_t)(q * 32) << 16) + 256u + Ring::ghost_pos(blk) * 32u;
-          uint32_t gacc[32];
-          tc_ld32(gaddr, gacc);
-          tc_st32_zero(gaddr);
-#pragma unroll
-          for (int j = 0; j < 32; ++j) acc[j] = __float_as_uint(__uint_as_float(acc[j]) + __uint_as_float(gacc[j]));
-        }
-        tc_wait_st();
-        tc_fence_before();
-        __syncwarp();
-        if (lane == 0) mbar_arrive(bar_t2empty + 8 * blk);
-        if (valid) {
-          uint4* op = reinterpret_cast<uint4*>(p.out + pix);
-          const __half2 zero2 = __floats2half2_rn(0.f, 0.f);
-#pragma unroll
-          for (int j4 = 0; j4 < 4; ++j4) {
-            float v[8] = {__uint_as_float(acc[j4 * 8 + 0]), __uint_as_float(acc[j4 * 8 + 1]),
-                          __uint_as_float(acc[j4 * 8 + 2]), __uint_as_float(acc[j4 * 8 + 3]),
-                          __uint_as_float(acc[j4 * 8 + 4]), __uint_as_float(acc[j4 * 8 + 5]),
-                          __uint_as_float(acc[j4 * 8 + 6]), __uint_as_float(acc[j4 * 8 + 7])};
-            const __half2* h2 = reinterpret_cast<const __half2*>(&rpre[j4]);
-            uint4 u;
-            __half2* o2 = reinterpret_cast<__half2*>(&u);
-#pragma unroll
-            for (int e = 0; e < 4; ++e) {
-              const float2 f = __half22float2(h2[e]);
-              o2[e] = __hmax2(__floats2half2_rn(v[2 * e] + f.x, v[2 * e + 1] + f.y), zero2);
-            }
-            op[j4] = u;
-          }
-        }
-      }
-      grow2 += (uint32_t)R;
-    }
-  }
-
-  tc_fence_before();
-  __syncthreads();
-  if (warp == 1) {
-    tc_fence_after();
-    asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(tmem_base), "r"(512u));
-  }
-}
-
-// ------------------------------------------------------------------------------------------------
-// SIMT reference conv (same math, CUDA cores) -- debugging aid and A/B check for the tensor-core path
+// SIMT reference conv (same math, CUDA cores) -- A/B check for the tensor-core path
 // ------------------------------------------------------------------------------------------------
 __global__ void conv_simt_kernel(const __half* __restrict__ in, const __half* __restrict__ wt, ConvParams p) {
   // one thread = one output pixel x 8 output channels
@@ -1633,8 +215,8 @@ __global__ void __launch_bounds__(kC1Tile) conv1_kernel(const float* __restrict_
 #pragma unroll
       for (int kw = 0; kw < 3; ++kw) x[kh * 3 + kw] = ok ? col[kw * (kMel + 1) + hh] : 0.f;
     }
-    // channel pairs on packed FFMA2, weights as 16-byte broadcast loads (the scalar version was LDS-bound: one
-    // shared-memory load per FMA); same fma order per channel, so the result is bit-identical
+    // channel pairs, weights as 16-byte broadcast loads (a scalar version is LDS-bound: one shared-memory load per
+    // FMA); the same fma order per channel as a scalar loop, so the result is bit-identical
     f32x2_t acc2[16];
     const ulonglong2* sb2 = reinterpret_cast<const ulonglong2*>(sb);
 #pragma unroll
@@ -1679,402 +261,9 @@ PFN_encodeTiled get_encode() {
   return fn;
 }
 
-static int conv4_forward(const ConvLayer& L, const __half* in, const __half* residual, __half* out, int B, int H, int W,
-                         int relu, int ghost, int num_sms, cudaStream_t stream) {
-  const int C = L.C_in;
-  B200_CHECK(L.w4 != nullptr && L.C_in == L.C_out && (C == 32 || C == 64), B200_ERR_STATE,
-             "conv v4: folded weights missing");
-  ConvV4Params p{};
-  p.B = B; p.H = H; p.W = W; p.C = C; p.relu = relu; p.bias = L.bias; p.residual = residual; p.out = out;
-  { const char* e = getenv("B200_RES_PF"); p.res_pf = e ? atoi(e) : 4; }
-  p.swizzle = (C == 64) ? 128 : 64;
-  p.tiles_w = ceil_div(W, kTileM);
-  const int strips = B * p.tiles_w;
-  // split H so that (waves of items) x (rows streamed per item, halo included) is smallest
-  long best_cost = -1;
-  for (int nh = 1; nh <= (H > 1 ? H / 2 : 1); ++nh) {
-    const int R = ceil_div(H, nh), n = ceil_div(H, R);
-    const long cost = (long)ceil_div(strips * n, num_sms) * (R + 3);
-    if (best_cost < 0 || cost < best_cost) { best_cost = cost; p.R = R; p.nhseg = n; }
-  }
-  p.num_items = B * p.tiles_w * p.nhseg;
-  p.a_bytes = 130u * C * 2;
-  p.a_slot_bytes = (uint32_t)align_up(p.a_bytes, 1024);
-  p.wkw_bytes = 3u * C * C * 2;                              // one horizontal tap: [(kh, co) = 3C][ci = C]
-  bool res_smem = (C == 64) && residual != nullptr && !ghost;         // residual rows through shared memory
-  if (const char* e = getenv("B200_TC4_RES_SMEM")) res_smem = res_smem && atoi(e) != 0;   // A/B knob
-  int groups = (C == 64) ? 3 : 2;                          // epilogue warpgroups (A/B knob: B200_TC4_G = 2 | 3 | 4)
-  if (const char* e = getenv("B200_TC4_G")) { const int v = atoi(e); if (v >= 2 && v <= 4) groups = v; }
-  if (ghost) groups = 2;
-  // ONE residual slot per epilogue warpgroup (row g -> slot g mod G = the group that drains row g): a slot shared by
-  // several groups lets a fast group wait on a barrier two phases ahead (parity aliasing: wrong rows, corrupted
-  // arrival counts -- seen as non-deterministic results and launch failures); the load of row g starts when the
-  // group has consumed row g - G, three row times before row g's accumulator is complete
-  p.n_rslots = res_smem ? groups : 0;
-  p.n_aslots = res_smem ? (groups <= 3 ? 5 : 4) : 7;
-  if (const char* e = getenv("B200_TC4_ASLOTS")) { const int v = atoi(e); if (v >= 2 && v <= p.n_aslots) p.n_aslots = v; }
-  p.w_off = 2048;
-  p.ones_off = 2048 + (uint32_t)align_up(3u * p.wkw_bytes, 1024);
-  p.btile_off = p.ones_off + (C == 64 ? 4096u : 0u);
-  p.a_off = p.btile_off + (C == 64 ? 2048u : 0u);         // C = 64: + the constant tiles of the bias MMA (6 KB)
-  p.r_off = p.a_off + (uint32_t)p.n_aslots * (uint32_t)align_up(130u * C * 2, 1024);
-  PFN_encodeTiled enc = get_encode();
-  B200_CHECK(enc != nullptr, B200_ERR_CUDA, "cuTensorMapEncodeTiled not available from the driver");
-  const CUtensorMapSwizzle sw = (C == 64) ? CU_TENSOR_MAP_SWIZZLE_128B : CU_TENSOR_MAP_SWIZZLE_64B;
-  CUtensorMap tmA, tmB;
-  {
-    cuuint64_t dims[4] = {(cuuint64_t)C, (cuuint64_t)W, (cuuint64_t)H, (cuuint64_t)B};
-    cuuint64_t strides[3] = {(cuuint64_t)C * 2, (cuuint64_t)W * C * 2, (cuuint64_t)H * W * C * 2};
-    cuuint32_t box[4] = {(cuuint32_t)C, 130, 1, 1};
-    cuuint32_t estr[4] = {1, 1, 1, 1};
-    CUresult r = enc(&tmA, CU_TENSOR_MAP_DATA_TYPE_FLOAT16, 4, const_cast<__half*>(in), dims, strides, box, estr,
-                     CU_TENSOR_MAP_INTERLEAVE_NONE, sw, CU_TENSOR_MAP_L2_PROMOTION_L2_256B,
-                     CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
-    B200_CHECK(r == CUDA_SUCCESS, B200_ERR_CUDA, "cuTensorMapEncodeTiled(A, v4) failed: %d", (int)r);
-  }
-  {
-    cuuint64_t dims[3] = {(cuuint64_t)C, (cuuint64_t)3 * C, 3};
-    cuuint64_t strides[2] = {(cuuint64_t)C * 2, (cuuint64_t)3 * C * C * 2};
-    cuuint32_t box[3] = {(cuuint32_t)C, (cuuint32_t)3 * C, 1};
-    cuuint32_t estr[3] = {1, 1, 1};
-    CUresult r = enc(&tmB, CU_TENSOR_MAP_DATA_TYPE_FLOAT16, 3, const_cast<__half*>(L.w4), dims, strides, box, estr,
-                     CU_TENSOR_MAP_INTERLEAVE_NONE, sw, CU_TENSOR_MAP_L2_PROMOTION_L2_256B,
-                     CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
-    B200_CHECK(r == CUDA_SUCCESS, B200_ERR_CUDA, "cuTensorMapEncodeTiled(B, v4) failed: %d", (int)r);
-  }
-  CUtensorMap tmR = tmA;                                    // residual rows: [B][H][W][C], one 128-pixel row per box
-  if (res_smem) {
-    cuuint64_t dims[4] = {(cuuint64_t)C, (cuuint64_t)W, (cuuint64_t)H, (cuuint64_t)B};
-    cuuint64_t strides[3] = {(cuuint64_t)C * 2, (cuuint64_t)W * C * 2, (cuuint64_t)H * W * C * 2};
-    cuuint32_t box[4] = {(cuuint32_t)C, 128, 1, 1};
-    cuuint32_t estr[4] = {1, 1, 1, 1};
-    CUresult r = enc(&tmR, CU_TENSOR_MAP_DATA_TYPE_FLOAT16, 4, const_cast<__half*>(residual), dims, strides, box, estr,
-                     CU_TENSOR_MAP_INTERLEAVE_NONE, sw, CU_TENSOR_MAP_L2_PROMOTION_L2_256B,
-                     CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
-    B200_CHECK(r == CUDA_SUCCESS, B200_ERR_CUDA, "cuTensorMapEncodeTiled(R, v4) failed: %d", (int)r);
-  }
-  const size_t smem = 1024 + p.r_off + (size_t)p.n_rslots * 16384;
-  const int grid = p.num_items < num_sms ? p.num_items : num_sms;
-  auto launch = [&](auto kernel, int g) -> int {
-    B200_CUDA_OK(cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024));
-    kernel<<<grid, 96 + 128 * g, smem, stream>>>(tmA, tmB, tmR, p);
-    B200_CUDA_OK(cudaGetLastError());
-    return B200_OK;
-  };
-  if (ghost) return C == 32 ? launch(conv_tc4_kernel<32, true, 2>, 2) : launch(conv_tc4_kernel<64, true, 2>, 2);
-  if (C == 32) {
-    if (groups == 2) return launch(conv_tc4_kernel<32, false, 2>, 2);
-    if (groups == 3) return launch(conv_tc4_kernel<32, false, 3>, 3);
-    return launch(conv_tc4_kernel<32, false, 4>, 4);
-  }
-  if (groups == 2) return launch(conv_tc4_kernel<64, false, 2>, 2);
-  if (groups == 3) return launch(conv_tc4_kernel<64, false, 3>, 3);
-  return launch(conv_tc4_kernel<64, false, 4>, 4);
-}
-
-// fused BasicBlock (conv_block32_kernel): in -> out, out must not alias in (tiles read their neighbours' halo)
-int conv_block32_forward(const ConvLayer& L1, const ConvLayer& L2, const __half* in, __half* out, int B, int H, int W,
-                         int num_sms, cudaStream_t stream, int ghost) {
-  B200_CHECK(L1.w4 && L2.w4 && L1.C_in == 32 && L1.C_out == 32 && L2.C_in == 32 && L2.C_out == 32 && in != out,
-             B200_ERR_STATE, "conv block: needs two folded 32->32 convs and distinct buffers");
-  ConvBlkParams p{};
-  p.B = B; p.H = H; p.W = W; p.bias1 = L1.bias; p.bias2 = L2.bias; p.in = in; p.out = out;
-  p.tiles_w = ceil_div(W, 126);
-  p.lag = 4;
-  const int strips = B * p.tiles_w;
-  long best_cost = -1;
-  for (int nh = 1; nh <= (H > 1 ? H / 2 : 1); ++nh) {
-    const int R = ceil_div(H, nh), n = ceil_div(H, R);
-    const long cost = (long)ceil_div(strips * n, num_sms) * (R + 4 + p.lag + 1);
-    if (best_cost < 0 || cost < best_cost) { best_cost = cost; p.R = R; p.nhseg = n; }
-  }
-  p.num_items = B * p.tiles_w * p.nhseg;
-  p.slot_bytes = 9216;                                       // 130 pixel rows x 64 B, 1024-aligned
-  p.n_islots = 6; p.n_mslots = 8;
-  p.w1_off = 2048; p.w2_off = 2048 + 18432;
-  p.i_off = 2048 + 2 * 18432;                                // 38912 = 38 x 1024
-  p.m_off = p.i_off + p.n_islots * p.slot_bytes;
-  PFN_encodeTiled enc = get_encode();
-  B200_CHECK(enc != nullptr, B200_ERR_CUDA, "cuTensorMapEncodeTiled not available from the driver");
-  CUtensorMap tmA, tmB1, tmB2;
-  {
-    cuuint64_t dims[4] = {32, (cuuint64_t)W, (cuuint64_t)H, (cuuint64_t)B};
-    cuuint64_t strides[3] = {64, (cuuint64_t)W * 64, (cuuint64_t)H * W * 64};
-    cuuint32_t box[4] = {32, 130, 1, 1};
-    cuuint32_t estr[4] = {1, 1, 1, 1};
-    CUresult r = enc(&tmA, CU_TENSOR_MAP_DATA_TYPE_FLOAT16, 4, const_cast<__half*>(in), dims, strides, box, estr,
-                     CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_64B, CU_TENSOR_MAP_L2_PROMOTION_L2_256B,
-                     CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
-    B200_CHECK(r == CUDA_SUCCESS, B200_ERR_CUDA, "cuTensorMapEncodeTiled(A, block) failed: %d", (int)r);
-  }
-  for (int i = 0; i < 2; ++i) {
-    cuuint64_t dims[3] = {32, 96, 3};
-    cuuint64_t strides[2] = {64, 96 * 64};
-    cuuint32_t box[3] = {32, 96, 1};
-    cuuint32_t estr[3] = {1, 1, 1};
-    CUresult r = enc(i ? &tmB2 : &tmB1, CU_TENSOR_MAP_DATA_TYPE_FLOAT16, 3, const_cast<__half*>(i ? L2.w4 : L1.w4), dims,
-                     strides, box, estr, CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_64B,
-                     CU_TENSOR_MAP_L2_PROMOTION_L2_256B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
-    B200_CHECK(r == CUDA_SUCCESS, B200_ERR_CUDA, "cuTensorMapEncodeTiled(B, block) failed: %d", (int)r);
-  }
-  const size_t smem = 1024 + p.m_off + (size_t)p.n_mslots * p.slot_bytes;
-  const int grid = p.num_items < num_sms ? p.num_items : num_sms;
-  auto launch = [&](auto kernel) -> int {
-    B200_CUDA_OK(cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024));
-    kernel<<<grid, kBlkThreads, smem, stream>>>(tmA, tmB1, tmB2, p);
-    B200_CUDA_OK(cudaGetLastError());
-    return B200_OK;
-  };
-  return ghost ? launch(conv_block32_kernel<true>) : launch(conv_block32_kernel<false>);
-}
-
-static int conv3_forward(const ConvLayer& L, const __half* in, const __half* residual, __half* out, int B, int H_in,
-                         int W_in, int relu, int fold, int num_sms, cudaStream_t stream, __half* out_sc = nullptr) {
-  B200_CHECK(L.w3 != nullptr, B200_ERR_STATE, "conv v3: padded weights missing");
-  B200_CHECK(out_sc == nullptr || (L.w3s && L.bias_s && L.C_out == 64 && L.stride == 2 && L.ksize == 3),
-             B200_ERR_STATE, "conv v3: folded shortcut needs a 64-channel stride-2 3x3 conv with w3s");
-  B200_CHECK((L.ksize == 3 || L.ksize == 1) && (L.stride == 1 || L.stride == 2), B200_ERR_STATE,
-             "conv v3: %dx%d stride %d unsupported", L.ksize, L.ksize, L.stride);
-  ConvV3Params p{};
-  p.stride = L.stride; p.ksize = L.ksize; p.pad = L.ksize / 2;
-  const int H = (H_in + 2 * p.pad - L.ksize) / L.stride + 1, W = (W_in + 2 * p.pad - L.ksize) / L.stride + 1;
-  p.B = B; p.H = H; p.W = W; p.C_in = L.C_in; p.C_out = L.C_out; p.relu = relu;
-  p.bias = L.bias; p.residual = residual; p.out = out;
-  if (out_sc) { p.C_out = 128; p.C_split = 64; p.out2 = out_sc; p.bias = L.bias_s; }
-  // fold (stride-1 3x3, the 16 layer3/4 convs): the per-tap version moved every activation element L2 -> smem nine
-  // times and ran at the L2 bandwidth (10.4 TB/s, profiles/r01_conv_tc3_layer3.ncu-rep) 1.8x above its MMA floor.
-  // One stage = (kh, 32 input channels): the 3 weight taps of that row + ONE pixel box with a one-pixel halo; the kw
-  // taps are descriptor shifts of one pixel row.  Pixel traffic 9x -> 3x, 6 MMAs per stage.
-  p.fold = (L.ksize == 3 && L.stride == 1 && fold) ? 1 : 0;
-  if (const char* e = getenv("B200_TC3_DBG")) p.dbg = atoi(e);
-  int fold_ck = 32;                                        // 4 stages of 41 KB; 64 -> 2 stages of 82 KB (A/B knob)
-  if (const char* e = getenv("B200_TC3_CK")) fold_ck = atoi(e) == 64 ? 64 : 32;
-  p.Ck = p.fold ? fold_ck : ((L.C_in >= 64) ? 64 : 32);
-  p.ncc = L.C_in / p.Ck;
-  p.kblocks = p.fold ? 3 * p.ncc : L.ksize * L.ksize * p.ncc;
-  p.swizzle = (p.Ck == 64) ? 128 : 64;
-  // pixel tile: up to 256 output pixels of one image; several rows when the image is narrower.  A TMA box dimension
-  // is at most 256 elements, and a strided box spans bw * stride input pixels: stride 2 -> at most 128 per row
-  if (p.fold) {
-    // accumulator column of pixel (rr, x) = rr * (bw + 2) + x; the shifted reads need bh * (bw + 2) <= 258 rows
-    p.bw = W < 254 ? W : 254;
-    p.bh = 258 / (p.bw + 2);
-    if (p.bh > H) p.bh = H;
-    p.pitch = p.bw + 2;
-  } else {
-    const int max_bw = 256 / L.stride;
-    if (W >= max_bw) { p.bw = max_bw; p.bh = 256 / max_bw; }
-    else { p.bw = W; p.bh = 256 / W; }
-    if (p.bh > H) p.bh = H;
-    if (p.bh * L.stride > 256) p.bh = 256 / L.stride;
-    p.pitch = p.bw;
-  }
-  p.tiles_w = ceil_div(W, p.bw);
-  p.tiles_h = ceil_div(H, p.bh);
-  p.m_tiles = ceil_div(p.C_out, 128);
-  // weight multicast across a cluster (folded convs): mc CTAs share one weight stream (A/B knob: B200_TC3_MC = 1 | 2 | 4)
-  // Measured (round 2): emb_forward of 256 segments 12.90 ms (mc = 1) / 13.23 (2) / 14.22 (4) -- the bytes INTO each SM
-  // are unchanged by multicast (xbar -> L1 625 MB per launch either way), only the L2 reads drop, and the lockstep
-  // costs more than that saves: the limit is the SM ingress port, not the L2 slices.  Off by default.
-  p.mc = 1;
-  if (p.fold && !p.dbg) {
-    if (const char* e = getenv("B200_TC3_MC")) { const int v = atoi(e); if (v == 1 || v == 2 || v == 4) p.mc = v; }
-  }
-  const int pixel_tiles = B * p.tiles_h * p.tiles_w;
-  p.num_items = ceil_div(pixel_tiles, p.mc) * p.m_tiles;   // per cluster
-  const int wtaps = p.fold ? 3 : 1;                        // weight taps per stage
-  p.a_bytes = (uint32_t)wtaps * 128u * p.Ck * 2;
-  // the MMA reads N = 256 rows (from a start shifted by up to 2 rows when folding): keep the slot that large
-  const uint32_t b_full = (uint32_t)align_up((size_t)(256 + (p.fold ? 2 : 0)) * p.Ck * 2, 1024);
-  const uint32_t delivered = p.a_bytes + (uint32_t)p.pitch * p.bh * p.Ck * 2;   // bytes the two TMA boxes deliver
-  const uint32_t slot = p.a_bytes + b_full;
-  p.stage_bytes = slot;                                     // the kernel addresses stage s at stage0 + s * stage_bytes
-  p.b_bytes = delivered;                                    // bytes to expect per stage
-  p.nstages = (227u * 1024 - 1024 - 3072 - kV3Staging) / slot;   // 5 stages of 41 KB when folding
-  if (p.nstages > 8) p.nstages = 8;
-  p.idesc = (1u << 4) | ((uint32_t)(256 >> 3) << 17) | ((uint32_t)(128 >> 4) << 24);
-  PFN_encodeTiled enc = get_encode();
-  B200_CHECK(enc != nullptr, B200_ERR_CUDA, "cuTensorMapEncodeTiled not available from the driver");
-  CUtensorMap tmX, tmW;
-  {
-    cuuint64_t dims[4] = {(cuuint64_t)L.C_in, (cuuint64_t)W_in, (cuuint64_t)H_in, (cuuint64_t)B};
-    cuuint64_t strides[3] = {(cuuint64_t)L.C_in * 2, (cuuint64_t)W_in * L.C_in * 2,
-                             (cuuint64_t)H_in * W_in * L.C_in * 2};
-    cuuint32_t box[4] = {(cuuint32_t)p.Ck, (cuuint32_t)(p.pitch * L.stride), (cuuint32_t)(p.bh * L.stride), 1};
-    cuuint32_t estr[4] = {1, (cuuint32_t)L.stride, (cuuint32_t)L.stride, 1};
-    CUresult r = enc(&tmX, CU_TENSOR_MAP_DATA_TYPE_FLOAT16, 4, const_cast<__half*>(in), dims, strides, box, estr,
-                     CU_TENSOR_MAP_INTERLEAVE_NONE,
-                     p.swizzle == 128 ? CU_TENSOR_MAP_SWIZZLE_128B : CU_TENSOR_MAP_SWIZZLE_64B,
-                     CU_TENSOR_MAP_L2_PROMOTION_L2_256B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
-    B200_CHECK(r == CUDA_SUCCESS, B200_ERR_CUDA, "cuTensorMapEncodeTiled(X, v3) failed: %d", (int)r);
-  }
-  {
-    const int rows = p.m_tiles * 128;                       // padded output-channel rows
-    cuuint64_t dims[3] = {(cuuint64_t)L.C_in, (cuuint64_t)rows, (cuuint64_t)(L.ksize * L.ksize)};
-    cuuint64_t strides[2] = {(cuuint64_t)L.C_in * 2, (cuuint64_t)rows * L.C_in * 2};
-    cuuint32_t box[3] = {(cuuint32_t)p.Ck, 128, (cuuint32_t)wtaps};
-    cuuint32_t estr[3] = {1, 1, 1};
-    CUresult r = enc(&tmW, CU_TENSOR_MAP_DATA_TYPE_FLOAT16, 3, const_cast<__half*>(out_sc ? L.w3s : L.w3), dims, strides,
-                     box, estr,
-                     CU_TENSOR_MAP_INTERLEAVE_NONE,
-                     p.swizzle == 128 ? CU_TENSOR_MAP_SWIZZLE_128B : CU_TENSOR_MAP_SWIZZLE_64B,
-                     CU_TENSOR_MAP_L2_PROMOTION_L2_256B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
-    B200_CHECK(r == CUDA_SUCCESS, B200_ERR_CUDA, "cuTensorMapEncodeTiled(W, v3) failed: %d", (int)r);
-  }
-  CUtensorMap tmWs = tmW;                                   // 1/mc of one weight tap: the slice a CTA multicasts
-  if (p.mc > 1) {
-    const int rows = p.m_tiles * 128;
-    cuuint64_t dims[3] = {(cuuint64_t)L.C_in, (cuuint64_t)rows, (cuuint64_t)(L.ksize * L.ksize)};
-    cuuint64_t strides[2] = {(cuuint64_t)L.C_in * 2, (cuuint64_t)rows * L.C_in * 2};
-    cuuint32_t box[3] = {(cuuint32_t)p.Ck, (cuuint32_t)(128 / p.mc), 1};
-    cuuint32_t estr[3] = {1, 1, 1};
-    CUresult r = enc(&tmWs, CU_TENSOR_MAP_DATA_TYPE_FLOAT16, 3, const_cast<__half*>(L.w3), dims, strides, box, estr,
-                     CU_TENSOR_MAP_INTERLEAVE_NONE,
-                     p.swizzle == 128 ? CU_TENSOR_MAP_SWIZZLE_128B : CU_TENSOR_MAP_SWIZZLE_64B,
-                     CU_TENSOR_MAP_L2_PROMOTION_L2_256B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
-    B200_CHECK(r == CUDA_SUCCESS, B200_ERR_CUDA, "cuTensorMapEncodeTiled(W slice, v3) failed: %d", (int)r);
-  }
-  static bool attr_set = false;
-  if (!attr_set) {
-    B200_CUDA_OK(cudaFuncSetAttribute(conv_tc3_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024));
-    attr_set = true;
-  }
-  const size_t smem = 1024 + 2048 + kV3Staging + (size_t)p.nstages * slot;
-  int max_clusters = num_sms / p.mc;
-  cudaLaunchConfig_t cfg{};
-  cfg.blockDim = dim3(kV3Threads);
-  cfg.dynamicSmemBytes = smem;
-  cfg.stream = stream;
-  cudaLaunchAttribute attr[1];
-  attr[0].id = cudaLaunchAttributeClusterDimension;
-  attr[0].val.clusterDim.x = (unsigned)p.mc; attr[0].val.clusterDim.y = 1; attr[0].val.clusterDim.z = 1;
-  cfg.attrs = attr;
-  cfg.numAttrs = 1;
-  if (p.mc > 1) {
-    static int cached[5] = {0, 0, 0, 0, 0};                 // co-resident clusters of this size (GPC boundaries)
-    if (cached[p.mc] == 0) {
-      cfg.gridDim = dim3((unsigned)(max_clusters * p.mc));
-      int n = 0;
-      B200_CUDA_OK(cudaOccupancyMaxActiveClusters(&n, conv_tc3_kernel, &cfg));
-      cached[p.mc] = n > 0 ? n : 1;
-    }
-    if (cached[p.mc] < max_clusters) max_clusters = cached[p.mc];
-  }
-  const int nclusters = p.num_items < max_clusters ? p.num_items : max_clusters;
-  cfg.gridDim = dim3((unsigned)(nclusters * p.mc));
-  B200_CUDA_OK(cudaLaunchKernelEx(&cfg, conv_tc3_kernel, tmX, tmW, tmWs, p));
-  return B200_OK;
-}
-
-int conv_s2_shortcut_forward(const ConvLayer& L, const __half* in, __half* out, __half* out_sc, int B, int H_in,
-                             int W_in, int num_sms, cudaStream_t stream) {
-  return conv3_forward(L, in, nullptr, out, B, H_in, W_in, 1, 0, num_sms, stream, out_sc);
-}
-
-static int conv2_forward(const ConvLayer& L, const __half* in, const __half* residual, __half* out, int B, int H, int W,
-                         int relu, int base_off_mode, int num_sms, cudaStream_t stream) {
-  ConvV2Params p{};
-  p.B = B; p.H = H; p.W = W; p.C_in = L.C_in; p.C_out = L.C_out; p.relu = relu;
-  p.bias = L.bias; p.residual = residual; p.out = out; p.base_off_mode = base_off_mode;
-  p.N = L.C_out < 128 ? L.C_out : 128;
-  p.n_halves = L.C_out / p.N;
-  p.Ck = (L.C_in >= 64) ? 64 : 32;
-  p.ncc = L.C_in / p.Ck;
-  p.swizzle = (p.Ck == 64) ? 128 : 64;
-  p.tiles_w = ceil_div(W, kTileM);
-  // split H when there are too few strips to fill the machine twice
-  const int strips = B * p.tiles_w * p.n_halves;
-  int nhseg = 1;
-  if (strips < 2 * num_sms) nhseg = ceil_div(2 * num_sms, strips);
-  if (nhseg > H / 2) nhseg = H / 2 > 0 ? H / 2 : 1;
-  p.R = ceil_div(H, nhseg);
-  p.nhseg = ceil_div(H, p.R);
-  p.num_items = B * p.tiles_w * p.nhseg * p.n_halves;
-  p.a_bytes = 130u * p.Ck * 2;
-  p.a_slot_bytes = (uint32_t)align_up(p.a_bytes, 1024);
-  p.b_bytes = (uint32_t)p.N * p.Ck * 2;
-  const size_t wbytes = (size_t)9 * p.ncc * p.b_bytes;
-  p.resident = (p.n_halves == 1 && wbytes <= 80 * 1024) ? 1 : 0;
-  p.idesc = (1u << 4) | ((uint32_t)(p.N >> 3) << 17) | ((uint32_t)(kTileM >> 4) << 24);
-  uint32_t off = 2048;
-  p.w_off = off;
-  if (p.resident) off += (uint32_t)align_up(wbytes, 1024);
-  const uint32_t budget = 210 * 1024;
-  if (p.resident) {
-    p.n_bslots = 0;
-    p.n_aslots = (int)((budget - off) / p.a_slot_bytes);
-    if (p.n_aslots > 8) p.n_aslots = 8;
-    p.a_off = off;
-    p.b_off = off;
-    off += p.n_aslots * p.a_slot_bytes;
-  } else {
-    p.n_aslots = 3;
-    p.a_off = off;
-    off += p.n_aslots * p.a_slot_bytes;
-    p.n_bslots = (int)((budget - off) / p.b_bytes);
-    if (p.n_bslots > 16) p.n_bslots = 16;
-    p.b_off = off;
-    off += p.n_bslots * p.b_bytes;
-  }
-  B200_CHECK(p.n_aslots >= 2 && (p.resident || p.n_bslots >= 2), B200_ERR_STATE, "conv v2: smem budget too small");
-  PFN_encodeTiled enc = get_encode();
-  B200_CHECK(enc != nullptr, B200_ERR_CUDA, "cuTensorMapEncodeTiled not available from the driver");
-  CUtensorMap tmA, tmB;
-  {
-    cuuint64_t dims[4] = {(cuuint64_t)L.C_in, (cuuint64_t)W, (cuuint64_t)H, (cuuint64_t)B};
-    cuuint64_t strides[3] = {(cuuint64_t)L.C_in * 2, (cuuint64_t)W * L.C_in * 2, (cuuint64_t)H * W * L.C_in * 2};
-    cuuint32_t box[4] = {(cuuint32_t)p.Ck, 130, 1, 1};
-    cuuint32_t estr[4] = {1, 1, 1, 1};
-    CUresult r = enc(&tmA, CU_TENSOR_MAP_DATA_TYPE_FLOAT16, 4, const_cast<__half*>(in), dims, strides, box, estr,
-                     CU_TENSOR_MAP_INTERLEAVE_NONE,
-                     p.swizzle == 128 ? CU_TENSOR_MAP_SWIZZLE_128B : CU_TENSOR_MAP_SWIZZLE_64B,
-                     CU_TENSOR_MAP_L2_PROMOTION_L2_256B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
-    B200_CHECK(r == CUDA_SUCCESS, B200_ERR_CUDA, "cuTensorMapEncodeTiled(A, v2) failed: %d", (int)r);
-  }
-  {
-    cuuint64_t dims[3] = {(cuuint64_t)L.C_in, (cuuint64_t)L.C_out, 9};
-    cuuint64_t strides[2] = {(cuuint64_t)L.C_in * 2, (cuuint64_t)L.C_out * L.C_in * 2};
-    cuuint32_t box[3] = {(cuuint32_t)p.Ck, (cuuint32_t)p.N, 1};
-    cuuint32_t estr[3] = {1, 1, 1};
-    CUresult r = enc(&tmB, CU_TENSOR_MAP_DATA_TYPE_FLOAT16, 3, const_cast<__half*>(L.w), dims, strides, box, estr,
-                     CU_TENSOR_MAP_INTERLEAVE_NONE,
-                     p.swizzle == 128 ? CU_TENSOR_MAP_SWIZZLE_128B : CU_TENSOR_MAP_SWIZZLE_64B,
-                     CU_TENSOR_MAP_L2_PROMOTION_L2_256B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
-    B200_CHECK(r == CUDA_SUCCESS, B200_ERR_CUDA, "cuTensorMapEncodeTiled(B, v2) failed: %d", (int)r);
-  }
-  static bool attr_set = false;
-  if (!attr_set) {
-    B200_CUDA_OK(cudaFuncSetAttribute(conv_tc2_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024));
-    attr_set = true;
-  }
-  const size_t smem = 1024 + off;
-  int grid = p.num_items < num_sms ? p.num_items : num_sms;
-  conv_tc2_kernel<<<grid, kTcThreads, smem, stream>>>(tmA, tmB, p);
-  B200_CUDA_OK(cudaGetLastError());
-  return B200_OK;
-}
-
 int conv_forward(const ConvLayer& L, const __half* in, const __half* residual, __half* out, int B, int H_in, int W_in,
-                 int relu, int impl, int num_sms, cudaStream_t stream, int flags) {
-  const int ghost = flags & kConvGhost, fold = (flags & kConvFold) ? 1 : 0;
-  if (impl == 7 || impl == 8) {
-    // channels-as-M tcgen05 conv for stride-1 3x3 with C_out >= 128 (N = 256 pixels balances the A-operand read);
-    // impl 8 (default): narrower layers use the strip-streaming pixels-as-M kernel, impl 7: the per-tap kernel
-    // (impl 8 also sends the stride-2 3x3 convs and the 1x1 stride-2 shortcuts there: TMA element strides)
-    if ((L.ksize == 3 && L.stride == 1 && L.C_out >= 128) || (impl == 8 && L.stride == 2 && L.w3))
-      return conv3_forward(L, in, residual, out, B, H_in, W_in, relu, fold, num_sms, stream);
-    if (impl == 8 && L.ksize == 3 && L.stride == 1 && L.C_in == L.C_out && L.C_in <= 64 && L.w4)
-      return conv4_forward(L, in, residual, out, B, H_in, W_in, relu, ghost, num_sms, stream);   // vertical taps folded into N
-    impl = (impl == 8) ? 6 : 1;
-  }
-  if (impl >= 3) {
-    // 3: v2 for C_in >= 64 (128B swizzle), base_offset set; 4: v2 also for C_in = 32 (64B swizzle);
-    // 5 / 6: same as 3 / 4 with base_offset left at 0 (hardware-semantics A/B)
-    const bool small_ok = (impl == 4 || impl == 6);
-    if (L.ksize == 3 && L.stride == 1 && (L.C_in >= 64 || small_ok))
-      return conv2_forward(L, in, residual, out, B, H_in, W_in, relu, (impl == 3 || impl == 4) ? 1 : 0, num_sms, stream);
-    impl = 1;
-  }
+                 int relu, int impl, int num_sms, cudaStream_t stream) {
+  (void)num_sms;
   ConvParams p{};
   p.B = B; p.H_in = H_in; p.W_in = W_in; p.C_in = L.C_in; p.C_out = L.C_out;
   p.taps_h = L.ksize; p.taps_w = L.ksize; p.stride = L.stride; p.pad = L.ksize / 2;
@@ -2088,11 +277,9 @@ int conv_forward(const ConvLayer& L, const __half* in, const __half* residual, _
   p.num_tiles = B * p.H_out * p.tiles_w;
   p.a_bytes = kTileM * p.Ck * 2;
   p.b_bytes = L.C_out * p.Ck * 2;
-  const uint32_t budget = 200 * 1024;
-  p.nstages = budget / (p.a_bytes + p.b_bytes);
-  if (p.nstages > 8) p.nstages = 8;
-  // instruction descriptor (cute/arch/mma_sm100_desc.hpp InstrDescriptor): D=f32, A=B=f16, K-major both, N>>3, M>>4
-  p.idesc = (1u << 4) | ((uint32_t)(L.C_out >> 3) << 17) | ((uint32_t)(kTileM >> 4) << 24);
+  B200_CHECK(L.C_in % p.Ck == 0 && (L.C_out == 64 || L.C_out == 128 || L.C_out == 256 || (L.C_out == 32 && p.Ck == 32)),
+             B200_ERR_STATE, "conv %d -> %d channels unsupported", L.C_in, L.C_out);
+  B200_CHECK(impl == 0 || impl == 1, B200_ERR_INVALID, "conv_impl %d unknown (0 = CUDA cores, 1 = tensor cores)", impl);
 
   if (impl == 0) {
     const size_t total = (size_t)B * p.H_out * p.W_out * (L.C_out / 8);
@@ -2101,6 +288,11 @@ int conv_forward(const ConvLayer& L, const __half* in, const __half* residual, _
     return B200_OK;
   }
 
+  // C_out = 256 needs 128 accumulator registers per thread: one CTA per SM with 4 deep stages; the narrower layers
+  // run two CTAs per SM (registers allow it) on half the shared memory each
+  const uint32_t budget = L.C_out == 256 ? 200u * 1024 : 100u * 1024;
+  p.nstages = budget / (p.a_bytes + p.b_bytes);
+  if (p.nstages > 8) p.nstages = 8;
   PFN_encodeTiled enc = get_encode();
   B200_CHECK(enc != nullptr, B200_ERR_CUDA, "cuTensorMapEncodeTiled not available from the driver");
   CUtensorMap tmA, tmB;
@@ -2127,16 +319,19 @@ int conv_forward(const ConvLayer& L, const __half* in, const __half* residual, _
                      CU_TENSOR_MAP_L2_PROMOTION_L2_256B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
     B200_CHECK(r == CUDA_SUCCESS, B200_ERR_CUDA, "cuTensorMapEncodeTiled(B) failed: %d", (int)r);
   }
-  const size_t smem = 1024 + 2048 + (size_t)p.nstages * (p.a_bytes + p.b_bytes);
-  static bool attr_set = false;
-  if (!attr_set) {
-    B200_CUDA_OK(cudaFuncSetAttribute(conv_tc_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024));
-    attr_set = true;
+  const size_t smem = 1024 + 1024 + (size_t)p.nstages * (p.a_bytes + p.b_bytes);
+  auto launch = [&](auto kernel) -> int {
+    B200_CUDA_OK(cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+    kernel<<<(unsigned)p.num_tiles, kWgThreads, smem, stream>>>(tmA, tmB, p);
+    B200_CUDA_OK(cudaGetLastError());
+    return B200_OK;
+  };
+  if (p.Ck == 32) return L.C_out == 32 ? launch(conv_wg_kernel<32, 32>) : launch(conv_wg_kernel<64, 32>);
+  switch (L.C_out) {
+    case 64: return launch(conv_wg_kernel<64, 64>);
+    case 128: return launch(conv_wg_kernel<128, 64>);
+    default: return launch(conv_wg_kernel<256, 64>);
   }
-  int grid = p.num_tiles < num_sms ? p.num_tiles : num_sms;
-  conv_tc_kernel<<<grid, kTcThreads, smem, stream>>>(tmA, tmB, p);
-  B200_CUDA_OK(cudaGetLastError());
-  return B200_OK;
 }
 
 int conv1_forward(const float* fbank, const float* fmean, const int* frame0, const float* w, const float* bias,

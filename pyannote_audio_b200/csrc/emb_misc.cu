@@ -53,7 +53,7 @@ __device__ __forceinline__ void fft16_stages(float (&xr)[16], float (&xi)[16], T
 // and stages 0-7 of the register-blocked 512-point DIT schedule below already ARE two independent 256-point FFTs
 // on the two halves of the array (stage 8 was the only one that mixed them): frame A lives in elements [0, 256),
 // frame B in [256, 512), half a warp each.  Same arithmetic per butterfly, less than half of it per frame
-// (the padded imaginary half of the old complex transform was all zeros): 663 -> see profiles/ us per 256 segments.
+// (the padded imaginary half of the old complex transform was all zeros).
 __global__ void __launch_bounds__(256) fbank_kernel(const float* __restrict__ wav,
                                                     const FbankRun* __restrict__ runs, int nruns, int nrows,
                                                     const float* __restrict__ window,

@@ -1,43 +1,43 @@
-// Split-precision GEMM on the 5th-gen tensor cores with fp32-level accuracy.
+// Split-precision GEMM on the Hopper tensor cores (wgmma) with fp32-level accuracy.
 //
 //   C[M][N] = act(A[M][K] * B[N][K]^T + bias[N])          (both operands K-contiguous, like sgemm_nt)
 //
 // The reference computes PyanNet in true fp32 (TF32 disabled, utils/reproducibility.py:68-83) and a 7-way argmax
 // decides integer frame boundaries downstream, so single-pass fp16/bf16/tf32 tensor-core math is not acceptable.
 // Each fp32 operand is stored as a pair of fp16 values x = hi + lo (hi = fp16(x), lo = fp16(x - hi), 22 significant
-// bits) and the product is accumulated in fp32 TMEM as   A_hi*B_hi + A_hi*B_lo + A_lo*B_hi   (the dropped lo*lo term is
-// 2^-22 relative): three tcgen05.mma per K=16 step instead of an FFMA loop.
+// bits) and the product is accumulated in fp32 registers as   A_lo*B_hi + A_hi*B_lo + A_hi*B_hi   (the dropped lo*lo
+// term is 2^-22 relative): three wgmma per K=16 step instead of an FFMA loop.
 //
-// Used for the LSTM input projections (N = 1024, K = 64 | 256; PyanNet.py:98,226-228) and the two Linear+LeakyReLU
-// layers (N = 128, K = 256 | 128; PyanNet.py:236-238).  Same warp-specialised structure as conv_tc_kernel:
-// warp0 TMA producer, warp1 MMA issuer, warps 2-5 epilogue; persistent over (m, n) tiles, n fastest.
+// Used for the LSTM input projections (N = 1024, K = 64 | 256; PyanNet.py:98,226-228), the two Linear+LeakyReLU
+// layers (N = 128, K = 256 | 128; PyanNet.py:236-238) and the embedding Linear (N = 256, K = 5120).
+// One CTA per 128 x 128 output tile: warp 8 is the TMA producer, warpgroups 0 and 1 each own 64 rows of the tile and
+// issue their wgmma on the shared A/B stages (ring of mbarrier-guarded stages, 128-byte swizzle).
 #include "common.cuh"
 #include "seg.cuh"
 #include "tc_common.cuh"
-#include <cstdlib>
 
 namespace b200 {
 
-constexpr int kGemmThreads = 192;
+constexpr int kGemmThreads = 288;
 constexpr int kGemmM = 128;
+constexpr int kGemmN = 128;
 constexpr int kGemmK = 64;       // K per stage: one 128-byte swizzle row of fp16
+constexpr int kGemmStages = 3;
+constexpr uint32_t kGemmTile = kGemmM * kGemmK * 2;          // 16 KB: one operand half (hi or lo) of A or B
+constexpr uint32_t kGemmStageBytes = 4 * kGemmTile;
 
 struct GemmTcParams {
-  int M, N, K, kblocks, tiles_m, tiles_n, num_tiles, act, Nt;
+  int M, N, K, kblocks, tiles_n, act;
   const float* bias;
   float* C;            // fp32 output [M][ldc] or nullptr
   __half* C_hi;        // optional split output [M][ldc_h]
   __half* C_lo;
   int ldc, ldc_h;
-  uint32_t a_bytes, b_bytes, stage_bytes, nstages, idesc;
-  int gx_T;            // > 0: "gx mode" (see gemm_tc_split_gx): M tiles are (t, 128 consecutive sequences)
   // fused all-gather: the epilogue also stores every fp32 output tile to the same offsets of up to 7 PEER buffers
-  // (other GPUs' memory mapped over NVLink: P2P stores, 128 contiguous bytes per thread), so the exchange of the
-  // result overlaps the GEMM tile by tile and no separate collective runs (SURVEY.md section 8e, K11)
+  // (other GPUs' memory mapped over NVLink: P2P stores), so the exchange of the result overlaps the GEMM tile by tile
+  // and no separate collective runs
   float* C_peer[7];
   int n_peer;
-  int dbg;             // timing experiment only (B200_GEMM_DBG; wrong results): 1 = B tiles, 2 = A tiles are loaded only
-                       // for the first pass over the stages
 };
 
 __global__ void __launch_bounds__(kGemmThreads, 1)
@@ -47,173 +47,85 @@ gemm_tc_split_kernel(const __grid_constant__ CUtensorMap tmAh, const __grid_cons
   extern __shared__ uint8_t smem_raw[];
   const uint32_t raw = smem_u32(smem_raw);
   const uint32_t base = (raw + 1023u) & ~1023u;
-  uint8_t* gbase = smem_raw + (base - raw);
-  const uint32_t bar_full = base, bar_empty = base + 64, bar_tfull = base + 128, bar_tempty = base + 144;
-  uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(gbase + 192);
-  float* s_bias = reinterpret_cast<float*>(gbase + 1024);       // up to 1024 floats: [1024, 5120)
-  const uint32_t stage0 = base + 5120 + 1024;                   // keep 1024 B alignment: 6144
-  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-  const int Nt = p.Nt;
+  const uint32_t bar_full = base, bar_empty = base + 64;
+  const uint32_t stage0 = base + 1024;
+  const int warp = threadIdx.x >> 5;
+  const int tn = blockIdx.x % p.tiles_n, tm = blockIdx.x / p.tiles_n;
 
-  for (int i = threadIdx.x; i < p.N; i += blockDim.x) s_bias[i] = p.bias ? p.bias[i] : 0.f;
   if (threadIdx.x == 0) {
-    for (uint32_t s = 0; s < p.nstages; ++s) { mbar_init(bar_full + 8 * s, 1); mbar_init(bar_empty + 8 * s, 1); }
-    for (int a = 0; a < 2; ++a) { mbar_init(bar_tfull + 8 * a, 1); mbar_init(bar_tempty + 8 * a, 4); }
+    for (int s = 0; s < kGemmStages; ++s) { mbar_init(bar_full + 8 * s, 1); mbar_init(bar_empty + 8 * s, 2); }
     asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
   }
-  if (warp == 1) {
-    asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(tmem_slot)),
-                 "r"(512u));
-    asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::);
-  }
-  tc_fence_before();
   __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem_base = *tmem_slot;
 
-  if (warp == 0) {
-    const bool leader = elect_one_sync();
-    uint32_t stage = 0, phase = 0;
-    for (int tile = blockIdx.x; tile < p.num_tiles; tile += gridDim.x) {
-      const int tn = tile % p.tiles_n, tm = tile / p.tiles_n;
+  if (warp == 8) {
+    if ((threadIdx.x & 31) == 0) {
+      uint32_t stage = 0, phase = 0;
       for (int kb = 0; kb < p.kblocks; ++kb) {
         mbar_wait(bar_empty + 8 * stage, phase ^ 1);
-        if (leader) {
-          const bool warm = p.dbg && (tile != (int)blockIdx.x || kb >= (int)p.nstages);
-          const bool do_a = !(warm && p.dbg == 2), do_b = !(warm && p.dbg == 1);
-          mbar_expect_tx(bar_full + 8 * stage, (do_a ? 2 * p.a_bytes : 0u) + (do_b ? 2 * p.b_bytes : 0u));
-          const uint32_t sa = stage0 + stage * p.stage_bytes;
-          if (!do_a) {
-          } else if (p.gx_T > 0) {   // rows = 128 consecutive sequences at one time step of a [b][t][k] array
-            const int t = tm % p.gx_T, b0 = (tm / p.gx_T) * kGemmM;
-            tma_load_3d(&tmAh, bar_full + 8 * stage, sa, kb * kGemmK, t, b0);
-            tma_load_3d(&tmAl, bar_full + 8 * stage, sa + p.a_bytes, kb * kGemmK, t, b0);
-          } else {
-            tma_load_2d(&tmAh, bar_full + 8 * stage, sa, kb * kGemmK, tm * kGemmM);
-            tma_load_2d(&tmAl, bar_full + 8 * stage, sa + p.a_bytes, kb * kGemmK, tm * kGemmM);
-          }
-          if (do_b) {
-            tma_load_2d(&tmBh, bar_full + 8 * stage, sa + 2 * p.a_bytes, kb * kGemmK, tn * Nt);
-            tma_load_2d(&tmBl, bar_full + 8 * stage, sa + 2 * p.a_bytes + p.b_bytes, kb * kGemmK, tn * Nt);
-          }
-        }
-        __syncwarp();
-        if (++stage == p.nstages) { stage = 0; phase ^= 1; }
+        mbar_expect_tx(bar_full + 8 * stage, kGemmStageBytes);
+        const uint32_t sa = stage0 + stage * kGemmStageBytes;
+        tma_load_2d(&tmAh, bar_full + 8 * stage, sa, kb * kGemmK, tm * kGemmM);
+        tma_load_2d(&tmAl, bar_full + 8 * stage, sa + kGemmTile, kb * kGemmK, tm * kGemmM);
+        tma_load_2d(&tmBh, bar_full + 8 * stage, sa + 2 * kGemmTile, kb * kGemmK, tn * kGemmN);
+        tma_load_2d(&tmBl, bar_full + 8 * stage, sa + 3 * kGemmTile, kb * kGemmK, tn * kGemmN);
+        if (++stage == kGemmStages) { stage = 0; phase ^= 1; }
       }
     }
-  } else if (warp == 1) {
-    const bool leader = elect_one_sync();
-    const uint32_t dhi = desc_hi(1024u, 2u);
-    uint32_t stage = 0, phase = 0, acc = 0, acc_phase = 0;
-    for (int tile = blockIdx.x; tile < p.num_tiles; tile += gridDim.x) {
-      mbar_wait(bar_tempty + 8 * acc, acc_phase ^ 1);
-      tc_fence_after();
-      const uint32_t d_tmem = tmem_base + acc * (uint32_t)Nt;
-      for (int kb = 0; kb < p.kblocks; ++kb) {
-        mbar_wait(bar_full + 8 * stage, phase);
-        tc_fence_after();
-        if (leader) {
-          const uint32_t sa = stage0 + stage * p.stage_bytes;
-          const uint32_t ah = desc_lo(sa), al = desc_lo(sa + p.a_bytes);
-          const uint32_t bh = desc_lo(sa + 2 * p.a_bytes), bl = desc_lo(sa + 2 * p.a_bytes + p.b_bytes);
-#pragma unroll
-          for (uint32_t k = 0; k < 8; k += 2) {
-            // small cross terms first, the dominant hi*hi term last
-            tc_mma_f16(d_tmem, desc_from(dhi, al + k), desc_from(dhi, bh + k), p.idesc, (kb | (int)k) != 0);
-            tc_mma_f16(d_tmem, desc_from(dhi, ah + k), desc_from(dhi, bl + k), p.idesc, 1);
-            tc_mma_f16(d_tmem, desc_from(dhi, ah + k), desc_from(dhi, bh + k), p.idesc, 1);
-          }
-          tc_commit(bar_empty + 8 * stage);
-        }
-        __syncwarp();
-        if (++stage == p.nstages) { stage = 0; phase ^= 1; }
-      }
-      if (leader) tc_commit(bar_tfull + 8 * acc);
-      __syncwarp();
-      acc ^= 1;
-      if (acc == 0) acc_phase ^= 1;
-    }
-  } else {
-    const int q = warp & 3;
-    uint32_t acc = 0, acc_phase = 0;
-    for (int tile = blockIdx.x; tile < p.num_tiles; tile += gridDim.x) {
-      const int tn = tile % p.tiles_n, tm = tile / p.tiles_n;
-      mbar_wait(bar_tfull + 8 * acc, acc_phase);
-      tc_fence_after();
-      const int m = tm * kGemmM + q * 32 + lane;
-      const bool valid = m < p.M;
-      const uint32_t taddr = tmem_base + ((uint32_t)(q * 32) << 16) + acc * (uint32_t)Nt;
-      if (p.gx_T > 0) {
-        // gx layout [b/32][t][col/4][b%32][4]: the 32 lanes (sequences) of a warp store 512 contiguous bytes
-        const int t = tm % p.gx_T, b32 = (tm / p.gx_T) * 4 + q;
-        float4* gp = reinterpret_cast<float4*>(p.C) + ((size_t)b32 * p.gx_T + t) * (size_t)(p.N / 4) * 32 + lane;
-        for (int n0 = 0; n0 < Nt; n0 += 32) {
-          uint32_t r[32];
-          tc_ld32(taddr + n0, r);
-          const int col = tn * Nt + n0;
-#pragma unroll
-          for (int j = 0; j < 8; ++j)
-            gp[(size_t)((col >> 2) + j) * 32] =
-                make_float4(__uint_as_float(r[4 * j]) + s_bias[col + 4 * j], __uint_as_float(r[4 * j + 1]) + s_bias[col + 4 * j + 1],
-                            __uint_as_float(r[4 * j + 2]) + s_bias[col + 4 * j + 2], __uint_as_float(r[4 * j + 3]) + s_bias[col + 4 * j + 3]);
-        }
-      } else
-      for (int n0 = 0; n0 < Nt; n0 += 32) {
-        uint32_t r[32];
-        tc_ld32(taddr + n0, r);
-        if (valid) {
-          const int col = tn * Nt + n0;
-          float v[32];
-#pragma unroll
-          for (int j = 0; j < 32; ++j) {
-            float x = __uint_as_float(r[j]) + s_bias[col + j];
-            if (p.act == 1) x = x > 0.f ? x : 0.01f * x;
-            v[j] = x;
-          }
-          if (p.C) {
-            float4* op = reinterpret_cast<float4*>(p.C + (size_t)m * p.ldc + col);
-#pragma unroll
-            for (int j = 0; j < 8; ++j) op[j] = make_float4(v[4 * j], v[4 * j + 1], v[4 * j + 2], v[4 * j + 3]);
-            for (int pr = 0; pr < p.n_peer; ++pr) {        // push the same 128 bytes to every peer GPU
-              float4* pp = reinterpret_cast<float4*>(p.C_peer[pr] + (size_t)m * p.ldc + col);
-#pragma unroll
-              for (int j = 0; j < 8; ++j) pp[j] = make_float4(v[4 * j], v[4 * j + 1], v[4 * j + 2], v[4 * j + 3]);
-            }
-          }
-          if (p.C_hi) {
-            uint4* oh = reinterpret_cast<uint4*>(p.C_hi + (size_t)m * p.ldc_h + col);
-            uint4* ol = reinterpret_cast<uint4*>(p.C_lo + (size_t)m * p.ldc_h + col);
-#pragma unroll
-            for (int j4 = 0; j4 < 4; ++j4) {
-              uint4 uh, ul;
-              __half2* hh = reinterpret_cast<__half2*>(&uh);
-              __half2* hl = reinterpret_cast<__half2*>(&ul);
-#pragma unroll
-              for (int e = 0; e < 4; ++e) {
-                const float a = v[j4 * 8 + 2 * e], c = v[j4 * 8 + 2 * e + 1];
-                const __half ah = __float2half_rn(a), ch = __float2half_rn(c);
-                hh[e] = __halves2half2(ah, ch);
-                hl[e] = __floats2half2_rn(a - __half2float(ah), c - __half2float(ch));
-              }
-              oh[j4] = uh;
-              ol[j4] = ul;
-            }
-          }
-        }
-      }
-      tc_fence_before();
-      __syncwarp();
-      if (lane == 0) mbar_arrive(bar_tempty + 8 * acc);
-      acc ^= 1;
-      if (acc == 0) acc_phase ^= 1;
-    }
+    return;
   }
 
-  tc_fence_before();
-  __syncthreads();
-  if (warp == 1) {
-    tc_fence_after();
-    asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(tmem_base), "r"(512u));
+  const int wg = warp >> 2;                                 // rows [64 wg, 64 wg + 64) of the tile
+  float acc[kGemmN / 2];
+#pragma unroll
+  for (int i = 0; i < kGemmN / 2; ++i) acc[i] = 0.f;
+  uint32_t stage = 0, phase = 0, prev = 0;
+  for (int kb = 0; kb < p.kblocks; ++kb) {
+    mbar_wait(bar_full + 8 * stage, phase);
+    const uint32_t sa = stage0 + stage * kGemmStageBytes;
+    const uint64_t ah = wg_desc(sa + wg * (kGemmTile / 2), 128), al = wg_desc(sa + kGemmTile + wg * (kGemmTile / 2), 128);
+    const uint64_t bh = wg_desc(sa + 2 * kGemmTile, 128), bl = wg_desc(sa + 3 * kGemmTile, 128);
+    wg_fence();
+#pragma unroll
+    for (uint32_t k = 0; k < 8; k += 2) {
+      // small cross terms first, the dominant hi*hi term last
+      Wgmma<kGemmN>::mma(acc, al + k, bh + k);
+      Wgmma<kGemmN>::mma(acc, ah + k, bl + k);
+      Wgmma<kGemmN>::mma(acc, ah + k, bh + k);
+    }
+    wg_commit();
+    wg_wait<1>();                                           // the previous stage's wgmma have read their operands
+    if (kb > 0 && (threadIdx.x & 127) == 0) mbar_arrive(bar_empty + 8 * prev);
+    prev = stage;
+    if (++stage == kGemmStages) { stage = 0; phase ^= 1; }
+  }
+  wg_wait<0>();
+
+  const int lane = threadIdx.x & 31, w4 = warp & 3;
+  const int col0 = tn * kGemmN + 2 * (lane & 3);
+#pragma unroll
+  for (int i = 0; i < 2; ++i) {
+    const int m = tm * kGemmM + wg * 64 + w4 * 16 + (lane >> 2) + 8 * i;
+    if (m >= p.M) continue;
+#pragma unroll
+    for (int j = 0; j < kGemmN / 8; ++j) {
+      const int col = col0 + 8 * j;
+      float a = acc[4 * j + 2 * i], c = acc[4 * j + 2 * i + 1];
+      if (p.bias) { a += p.bias[col]; c += p.bias[col + 1]; }
+      if (p.act == 1) { a = a > 0.f ? a : 0.01f * a; c = c > 0.f ? c : 0.01f * c; }
+      if (p.C) {
+        const float2 v = make_float2(a, c);
+        *reinterpret_cast<float2*>(p.C + (size_t)m * p.ldc + col) = v;
+        for (int pr = 0; pr < p.n_peer; ++pr)               // push the same values to every peer GPU
+          *reinterpret_cast<float2*>(p.C_peer[pr] + (size_t)m * p.ldc + col) = v;
+      }
+      if (p.C_hi) {
+        const __half ah16 = __float2half_rn(a), ch16 = __float2half_rn(c);
+        *reinterpret_cast<__half2*>(p.C_hi + (size_t)m * p.ldc_h + col) = __halves2half2(ah16, ch16);
+        *reinterpret_cast<__half2*>(p.C_lo + (size_t)m * p.ldc_h + col) =
+            __floats2half2_rn(a - __half2float(ah16), c - __half2float(ch16));
+      }
+    }
   }
 }
 
@@ -249,85 +161,38 @@ static int make_map_2d(CUtensorMap* tm, const __half* ptr, int rows, int K, int 
   return B200_OK;
 }
 
-static int make_map_3d(CUtensorMap* tm, const __half* ptr, int NB, int T, int K, int ld) {
-  PFN_encodeTiled enc = get_encode();
-  B200_CHECK(enc != nullptr, B200_ERR_CUDA, "cuTensorMapEncodeTiled not available from the driver");
-  cuuint64_t dims[3] = {(cuuint64_t)K, (cuuint64_t)T, (cuuint64_t)NB};
-  cuuint64_t strides[2] = {(cuuint64_t)ld * 2, (cuuint64_t)T * ld * 2};
-  cuuint32_t box[3] = {(cuuint32_t)kGemmK, 1, (cuuint32_t)kGemmM};
-  cuuint32_t estr[3] = {1, 1, 1};
-  CUresult r = enc(tm, CU_TENSOR_MAP_DATA_TYPE_FLOAT16, 3, const_cast<__half*>(ptr), dims, strides, box, estr,
-                   CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_256B,
-                   CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
-  B200_CHECK(r == CUDA_SUCCESS, B200_ERR_CUDA, "cuTensorMapEncodeTiled(gemm gx) failed: %d", (int)r);
-  return B200_OK;
-}
-
-static int launch_gemm(GemmTcParams& p, const CUtensorMap& tmAh, const CUtensorMap& tmAl, const __half* B_hi,
-                       const __half* B_lo, int ldb, int num_sms, cudaStream_t stream) {
-  // N = 256 per MMA runs at the full tensor rate (N = 128 at half of it: the A operand read bounds the instruction);
-  // its 96 KB stages leave room for two instead of three
-  p.Nt = (p.N % 256 == 0) ? 256 : 128;
-  p.kblocks = p.K / kGemmK;
-  p.tiles_n = p.N / p.Nt;
-  p.num_tiles = p.tiles_m * p.tiles_n;
-  p.a_bytes = kGemmM * kGemmK * 2;
-  p.b_bytes = p.Nt * kGemmK * 2;
-  p.stage_bytes = 2 * p.a_bytes + 2 * p.b_bytes;          // 64 KB (Nt = 128) or 96 KB (Nt = 256)
-  p.nstages = p.Nt == 256 ? 2 : 3;
-  p.idesc = (1u << 4) | ((uint32_t)(p.Nt >> 3) << 17) | ((uint32_t)(kGemmM >> 4) << 24);
-  if (const char* e = getenv("B200_GEMM_DBG")) p.dbg = atoi(e);
-  CUtensorMap tmBh, tmBl;
-  int rc;
-  if ((rc = make_map_2d(&tmBh, B_hi, p.N, p.K, ldb, p.Nt))) return rc;
-  if ((rc = make_map_2d(&tmBl, B_lo, p.N, p.K, ldb, p.Nt))) return rc;
-  static bool attr_set = false;
-  if (!attr_set) {
-    B200_CUDA_OK(cudaFuncSetAttribute(gemm_tc_split_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024));
-    attr_set = true;
-  }
-  const size_t smem = 1024 + 6144 + (size_t)p.nstages * p.stage_bytes;
-  const int grid = p.num_tiles < num_sms ? p.num_tiles : num_sms;
-  gemm_tc_split_kernel<<<grid, kGemmThreads, smem, stream>>>(tmAh, tmAl, tmBh, tmBl, p);
-  B200_CUDA_OK(cudaGetLastError());
-  return B200_OK;
-}
-
 int gemm_tc_split(const __half* A_hi, const __half* A_lo, int lda, const __half* B_hi, const __half* B_lo, int ldb,
                   float* C, int ldc, __half* C_hi, __half* C_lo, int ldc_h, const float* bias, int M, int N, int K,
                   int act, int num_sms, cudaStream_t stream, float* const* C_peers, int n_peers) {
-  B200_CHECK(K % kGemmK == 0 && N % 128 == 0 && N <= 1024 && lda % 8 == 0 && ldb % 8 == 0, B200_ERR_INVALID,
+  (void)num_sms;
+  B200_CHECK(K % kGemmK == 0 && N % kGemmN == 0 && lda % 8 == 0 && ldb % 8 == 0, B200_ERR_INVALID,
              "gemm_tc_split: unsupported shape M=%d N=%d K=%d", M, N, K);
+  B200_CHECK(n_peers >= 0 && n_peers <= 7 && (n_peers == 0 || (C_peers && C)), B200_ERR_INVALID,
+             "gemm_tc_split: at most 7 peer outputs");
+  if (M == 0) return B200_OK;
   GemmTcParams p{};
   p.M = M; p.N = N; p.K = K; p.act = act; p.bias = bias; p.C = C; p.C_hi = C_hi; p.C_lo = C_lo; p.ldc = ldc;
   p.ldc_h = ldc_h;
-  B200_CHECK(n_peers >= 0 && n_peers <= 7 && (n_peers == 0 || (C_peers && C)), B200_ERR_INVALID,
-             "gemm_tc_split: at most 7 peer outputs");
   p.n_peer = n_peers;
   for (int i = 0; i < n_peers; ++i) p.C_peer[i] = C_peers[i];
-  p.tiles_m = ceil_div(M, kGemmM);
-  CUtensorMap tmAh, tmAl;
+  p.kblocks = K / kGemmK;
+  p.tiles_n = N / kGemmN;
+  CUtensorMap tmAh, tmAl, tmBh, tmBl;
   int rc;
   if ((rc = make_map_2d(&tmAh, A_hi, M, K, lda, kGemmM))) return rc;
   if ((rc = make_map_2d(&tmAl, A_lo, M, K, lda, kGemmM))) return rc;
-  return launch_gemm(p, tmAh, tmAl, B_hi, B_lo, ldb, num_sms, stream);
-}
-
-// LSTM input projection for lstm_rec_tc_kernel: A is [NB][T][K] (hi, lo), the result G = A B^T + bias is written in
-// "gx layout" [ceil(NB/128)*4][T][N/4][32][4] fp32 (sequence-major inside 32-sequence groups, padded sequences hold
-// the bias), so that a warp of 32 sequences reads/writes 512 contiguous bytes per column group.
-int gemm_tc_split_gx(const __half* A_hi, const __half* A_lo, int lda, const __half* B_hi, const __half* B_lo, int ldb,
-                     float* G, const float* bias, int NB, int T, int N, int K, int num_sms, cudaStream_t stream) {
-  B200_CHECK(K % kGemmK == 0 && N % 128 == 0 && N <= 1024 && lda % 8 == 0 && ldb % 8 == 0, B200_ERR_INVALID,
-             "gemm_tc_split_gx: unsupported shape NB=%d N=%d K=%d", NB, N, K);
-  GemmTcParams p{};
-  p.M = NB * T; p.N = N; p.K = K; p.act = 0; p.bias = bias; p.C = G; p.gx_T = T;
-  p.tiles_m = ceil_div(NB, kGemmM) * T;
-  CUtensorMap tmAh, tmAl;
-  int rc;
-  if ((rc = make_map_3d(&tmAh, A_hi, NB, T, K, lda))) return rc;
-  if ((rc = make_map_3d(&tmAl, A_lo, NB, T, K, lda))) return rc;
-  return launch_gemm(p, tmAh, tmAl, B_hi, B_lo, ldb, num_sms, stream);
+  if ((rc = make_map_2d(&tmBh, B_hi, N, K, ldb, kGemmN))) return rc;
+  if ((rc = make_map_2d(&tmBl, B_lo, N, K, ldb, kGemmN))) return rc;
+  const size_t smem = 1024 + 1024 + (size_t)kGemmStages * kGemmStageBytes;
+  static bool attr_set = false;
+  if (!attr_set) {
+    B200_CUDA_OK(cudaFuncSetAttribute(gemm_tc_split_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+    attr_set = true;
+  }
+  const unsigned grid = (unsigned)(ceil_div(M, kGemmM) * p.tiles_n);
+  gemm_tc_split_kernel<<<grid, kGemmThreads, smem, stream>>>(tmAh, tmAl, tmBh, tmBl, p);
+  B200_CUDA_OK(cudaGetLastError());
+  return B200_OK;
 }
 
 }  // namespace b200

@@ -8,21 +8,21 @@ struct SegWeights {
   bool loaded = false;
   int lstm_layers = 4;
   float wav_w = 1.f, wav_b = 0.f;   // sincnet.wav_norm1d affine
-  __half* sinc_tc_hi = nullptr;     // [16 k-steps][128 rows (80 filters)][16 taps] fp16 hi for sinc_tc_kernel
-  __half* sinc_tc_lo = nullptr;
+  __half* sinc_wg_hi = nullptr;     // [80 filters][256 taps] fp16 (hi, lo) for the wgmma sinc layer (taps >= 251 zero)
+  __half* sinc_wg_lo = nullptr;
   float* sinc_f = nullptr;          // [126][80]: half filters (k=0..124) + centre tap (k=125); cos ch 0..39, sin 40..79
   float* in_gamma[3] = {nullptr, nullptr, nullptr};   // sincnet.norm1d.{0,1,2}.weight
   float* in_beta[3] = {nullptr, nullptr, nullptr};
   float* conv_w[2] = {nullptr, nullptr};   // [CIN][5][60]
   float* conv_b[2] = {nullptr, nullptr};   // [60]
-  __half* conv_tc_hi[2] = {nullptr, nullptr};   // [ncb * 5 taps][128 rows = c_out (60 real)][16 c_in] fp16 hi
-  __half* conv_tc_lo[2] = {nullptr, nullptr};   //                                                              lo
+  __half* conv_wg_hi[2] = {nullptr, nullptr};   // [64 rows = c_out (60 real)][5 taps x Cpad channels] fp16 (hi, lo)
+  __half* conv_wg_lo[2] = {nullptr, nullptr};
   // LSTM, per layer: W_ih for both directions [1024][Kpad] with row = dir*512 + unit*4 + gate; bias = b_ih+b_hh
   float* w_ih[8] = {};
   float* b_g[8] = {};
   int k_in[8] = {};                 // padded input size (64, 256, ...)
   float* w_hh[8] = {};              // [2 dir][2 rank][128 k][256]  (smem image of the SIMT recurrent kernel)
-  __half* w_hh_hi[8] = {};          // [2 dir][2 rank][256 = (unit, gate)][128 k] fp16 (hi, lo) for lstm_rec_tc_kernel
+  __half* w_hh_hi[8] = {};          // [2 dir][2 rank][256 = 32 jj + 8 gate + u][128 k] fp16 (hi, lo), seg_lstm_wg.cu
   __half* w_hh_lo[8] = {};
   // fp16 (hi, lo) splits of the GEMM weights for the tensor-core path (gemm_tc.cu)
   __half* w_ih_hi[8] = {};
@@ -43,27 +43,21 @@ int gemm_tc_split(const __half* A_hi, const __half* A_lo, int lda, const __half*
                   float* C, int ldc, __half* C_hi, __half* C_lo, int ldc_h, const float* bias, int M, int N, int K,
                   int act, int num_sms, cudaStream_t stream, float* const* C_peers = nullptr, int n_peers = 0);
 int split_f16(const float* x, __half* hi, __half* lo, size_t n, cudaStream_t st);
-int gemm_tc_split_gx(const __half* A_hi, const __half* A_lo, int lda, const __half* B_hi, const __half* B_lo, int ldb,
-                     float* G, const float* bias, int NB, int T, int N, int K, int num_sms, cudaStream_t stream);
-// tensor-core recurrence (seg_lstm_tc.cu): G in gx layout -> layer output as fp16 (hi, lo) [NB][589][256]
-int lstm_rec_tc(const float* G, const __half* Whh_hi, const __half* Whh_lo, __half* Yh, __half* Yl, int NB,
+// tensor-core recurrence (seg_lstm_wg.cu): Gx [NB][589][1024] -> layer output as fp16 (hi, lo) [NB][589][256]
+int lstm_rec_wg(const float* Gx, const __half* Wh, const __half* Wl, __half* Yh, __half* Yl, int NB,
                 cudaStream_t stream);
 
-// tensor-core Conv1d(k=5)+MaxPool(3) (seg_conv_tc.cu)
-int in_apply_split(const float* P, const float2* affine, int NB, int C, int Cpad, int L, __half* Xh, __half* Xl,
-                   cudaStream_t stream);
-int conv5_tc_forward(const __half* Xh, const __half* Xl, const __half* Wh, const __half* Wl, const float* bias, int NB,
-                     int L_in, int L_pool, int ncb, float* Pout, double2* part, int ntiles_part, int num_sms,
-                     cudaStream_t stream);
-
-int sinc_tc_forward(const float* wav, const long long* chunk_off, const int* chunk_valid, const float2* affine,
-                    const __half* Ah, const __half* Al, int NB, float* P0, double2* part, int ntiles_part, int num_sms,
+// SincNet layers on the tensor cores (seg_conv_wg.cu); same outputs and partial sums as the fp32 twins
+int sinc_wg_forward(const float* wav, const long long* chunk_off, const int* chunk_valid, const float2* affine,
+                    const __half* Wh, const __half* Wl, int NB, float* P0, double2* part, int ntiles,
                     cudaStream_t stream);
+int conv5_wg_forward(int layer, const float* Pin, const float2* affine, const __half* Wh, const __half* Wl,
+                     const float* bias, int NB, float* Pout, double2* part, int ntiles, cudaStream_t stream);
 
 // SincNet front-end on NB chunks: wav + per-chunk (offset, valid) -> X0 [NB][589][64] fp32 (60 features + 4 zero pad)
 size_t sincnet_workspace_bytes(int NB);
 int sincnet_forward(const SegWeights& W, const float* wav, const long long* chunk_off, const int* chunk_valid, int NB,
-                    void* ws, float* x0, int conv_impl, int num_sms, cudaStream_t stream);
+                    void* ws, float* x0, int conv_impl, cudaStream_t stream);
 
 // BiLSTM stack + linear head: X0 -> class ids [NB][589] u8 (+ optional log-probs [NB][589][7])
 size_t lstm_workspace_bytes(int NB);

@@ -1,0 +1,241 @@
+// SincNet convolutions on the Hopper tensor cores (wgmma), split-precision fp16 with fp32-level accuracy.
+//
+// Reference: pyannote/audio/models/blocks/sincnet.py:70-90,163-184.  The three layers are one implicit GEMM each,
+//     D[t][n] = sum_k X[t * S + k] * W[n][k]          t = conv output position, n = output channel
+//   sinc layer:   S = 10 (stride), X = normalised samples,                      K = 256 (251 taps + zeros), N = 80
+//   Conv1d(C,60,5): S = Cpad, X = channels-last [position][Cpad] input after InstanceNorm + leaky_relu,
+//                 k = tap * Cpad + channel, K = 5 * Cpad,                                      N = 64 (60 real)
+// followed by |.| (sinc layer only), MaxPool1d(3, 3), + bias (Conv1d) and fp64 InstanceNorm partial sums per tile.
+// A CTA is one warpgroup on one tile of the fp32 twins (sinc_pool_kernel / conv5_pool_kernel): 192 positions = 64
+// pooled outputs, three m64 blocks.  The tile's input is staged once as fp16 (hi, lo) pairs; the A fragments of
+// every K = 16 step are read from it straight into registers (the im2col rows start 20 bytes apart, which no TMA
+// box or shared-memory descriptor expresses).  The weights (hi, lo) arrive by TMA as 128-byte-swizzled K-major tiles.
+// Products: A_lo*W_hi + A_hi*W_lo + A_hi*W_hi in fp32 registers, like gemm_tc.cu.
+#include "common.cuh"
+#include "seg.cuh"
+#include "tc_common.cuh"
+
+namespace b200 {
+
+constexpr int kSCThreads = 128;
+constexpr int kSCTileP = 64;                 // pooled outputs per tile (= the fp32 twins' tile)
+constexpr int kSCPos = 3 * kSCTileP;         // conv output positions per tile
+constexpr int kSCPitch = kSCPos + 1;         // epilogue staging [channel][position] pitch (floats)
+
+struct SincConvWgParams {
+  // sinc layer input
+  const float* wav;
+  const long long* chunk_off;
+  const int* chunk_valid;
+  const float2* affine;        // sinc: per-chunk waveform InstanceNorm; Conv1d: per (chunk, input channel)
+  // Conv1d input
+  const float* Pin;            // [B][CIN][Lin]
+  int Lin;
+  const float* bias;           // Conv1d: [60]
+  float* Pout;                 // [B][NREAL][Lp]
+  double2* part;               // [B][NREAL][ntiles]
+  int Lp, ntiles;
+  uint32_t xs_bytes, w_off, w_box_bytes, pool_off;
+};
+
+// CIN = 0: the sinc layer; else a Conv1d(CIN, 60, 5) with input channels padded to CPAD
+template <int CIN, int CPAD, int NW, int NREAL, int KT>
+__global__ void __launch_bounds__(kSCThreads)
+sinc_conv_wg_kernel(const __grid_constant__ CUtensorMap tmWh, const __grid_constant__ CUtensorMap tmWl,
+                    SincConvWgParams p) {
+  constexpr bool kSinc = CIN == 0;
+  constexpr int S = kSinc ? kSincStride : CPAD;
+  constexpr int kIn = kSinc ? (kSCPos - 1) * S + KT : (kSCPos + 4) * CPAD;   // staged fp16 values per (hi | lo)
+  constexpr int kBoxes = (KT + 63) / 64;
+  extern __shared__ uint8_t smem_raw[];
+  const uint32_t raw = smem_u32(smem_raw);
+  const uint32_t base = (raw + 1023u) & ~1023u;
+  uint8_t* gbase = smem_raw + (base - raw);
+  const uint32_t bar = base;
+  __half* xh = reinterpret_cast<__half*>(gbase + 1024);
+  __half* xl = xh + kIn;
+  const uint32_t w_smem = base + p.w_off;
+  const int tile = blockIdx.x, b = blockIdx.y;
+  const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
+
+  if (tid == 0) {
+    mbar_init(bar, 1);
+    asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
+  }
+  __syncthreads();
+  if (tid == 0) {
+    mbar_expect_tx(bar, 2u * kBoxes * p.w_box_bytes);
+    for (int i = 0; i < kBoxes; ++i) {
+      tma_load_2d(&tmWh, bar, w_smem + i * p.w_box_bytes, 64 * i, 0);
+      tma_load_2d(&tmWl, bar, w_smem + (kBoxes + i) * p.w_box_bytes, 64 * i, 0);
+    }
+  }
+  // ---- stage the tile's input as fp16 (hi, lo), same padding rules as the fp32 twins ------------------------------
+  if (kSinc) {
+    const float2 af = p.affine[b];
+    const float* x = p.wav + p.chunk_off[b];
+    const int valid = p.chunk_valid[b];
+    const int s0 = tile * kSCPos * kSincStride;
+    for (int i = tid; i < kIn; i += kSCThreads) {
+      const int g = s0 + i;
+      const float rv = (g < valid) ? __ldg(x + g) : 0.f;
+      const float v = (g < kChunk) ? fmaf(rv, af.x, af.y) : 0.f;
+      const __half h = __float2half_rn(v);
+      xh[i] = h;
+      xl[i] = __float2half_rn(v - __half2float(h));
+    }
+  } else {
+    constexpr int TW = kSCPos + 4;
+    const int t0 = tile * kSCPos;
+    for (int i = tid; i < CPAD * TW; i += kSCThreads) {
+      const int c = i / TW, t = i - c * TW, g = t0 + t;
+      float v = 0.f;
+      if (c < CIN && g < p.Lin) {
+        const float2 af = p.affine[b * CIN + c];
+        v = fmaf(p.Pin[((size_t)b * CIN + c) * p.Lin + g], af.x, af.y);
+        v = v > 0.f ? v : 0.01f * v;
+      }
+      const __half h = __float2half_rn(v);
+      xh[t * CPAD + c] = h;
+      xl[t * CPAD + c] = __float2half_rn(v - __half2float(h));
+    }
+  }
+  __syncthreads();
+  mbar_wait(bar, 0);
+
+  // ---- three m64 blocks x KT / 16 steps x 3 split products --------------------------------------------------------
+  float acc[3][NW / 2];
+#pragma unroll
+  for (int m = 0; m < 3; ++m)
+#pragma unroll
+    for (int i = 0; i < NW / 2; ++i) acc[m][i] = 0.f;
+  const uint32_t* xh32 = reinterpret_cast<const uint32_t*>(xh);
+  const uint32_t* xl32 = reinterpret_cast<const uint32_t*>(xl);
+  const int r0 = 16 * warp + (lane >> 2), c0 = 2 * (lane & 3);
+  for (int ks = 0; ks < KT / 16; ++ks) {
+    uint32_t ah[3][4], al[3][4];
+#pragma unroll
+    for (int m = 0; m < 3; ++m) {
+      const int t = 64 * m + r0;
+      const int i0 = (t * S + 16 * ks + c0) >> 1, i1 = ((t + 8) * S + 16 * ks + c0) >> 1;   // even offsets
+      ah[m][0] = xh32[i0]; ah[m][1] = xh32[i1]; ah[m][2] = xh32[i0 + 4]; ah[m][3] = xh32[i1 + 4];
+      al[m][0] = xl32[i0]; al[m][1] = xl32[i1]; al[m][2] = xl32[i0 + 4]; al[m][3] = xl32[i1 + 4];
+    }
+    const uint32_t wb = w_smem + (ks >> 2) * p.w_box_bytes + (ks & 3) * 32;
+    const uint64_t wh = wg_desc(wb, 128), wl = wg_desc(wb + kBoxes * p.w_box_bytes, 128);
+    wg_fence();
+#pragma unroll
+    for (int m = 0; m < 3; ++m) {
+      WgmmaRS<NW>::mma(acc[m], al[m], wh);                 // small cross terms first, hi*hi last
+      WgmmaRS<NW>::mma(acc[m], ah[m], wl);
+      WgmmaRS<NW>::mma(acc[m], ah[m], wh);
+    }
+    wg_commit();
+    wg_wait<0>();
+  }
+
+  // ---- epilogue: stage [channel][position] over the weights, pool, store, partial sums ---------------------------
+  __syncthreads();
+  float* st = reinterpret_cast<float*>(gbase + p.w_off);
+#pragma unroll
+  for (int m = 0; m < 3; ++m)
+#pragma unroll
+    for (int j = 0; j < NW / 8; ++j)
+#pragma unroll
+      for (int i = 0; i < 2; ++i)
+#pragma unroll
+        for (int e = 0; e < 2; ++e) {
+          const float v = acc[m][4 * j + 2 * i + e];
+          st[(8 * j + c0 + e) * kSCPitch + 64 * m + r0 + 8 * i] = kSinc ? fabsf(v) : v;
+        }
+  __syncthreads();
+  float* pt = reinterpret_cast<float*>(gbase + p.pool_off);   // pooled tile [NREAL][65]
+  for (int idx = tid; idx < NREAL * kSCTileP; idx += kSCThreads) {
+    const int n = idx / kSCTileP, j = idx - n * kSCTileP;
+    const float* r = st + n * kSCPitch + 3 * j;
+    float v = fmaxf(fmaxf(r[0], r[1]), r[2]);
+    if (!kSinc) v += p.bias[n];
+    const int pg = tile * kSCTileP + j;
+    const bool ok = pg < p.Lp;
+    pt[n * 65 + j] = ok ? v : 0.f;
+    if (ok) p.Pout[((size_t)b * NREAL + n) * p.Lp + pg] = v;
+  }
+  __syncthreads();
+  if (tid < NREAL) {
+    double s = 0.0, ss = 0.0;
+    for (int i = 0; i < kSCTileP; ++i) {
+      const double v = pt[tid * 65 + i];
+      s += v;
+      ss += v * v;
+    }
+    p.part[((size_t)b * NREAL + tid) * p.ntiles + tile] = make_double2(s, ss);
+  }
+}
+
+static int make_w_map(CUtensorMap* tm, const __half* ptr, int rows, int K) {
+  PFN_encodeTiled enc = get_encode();
+  B200_CHECK(enc != nullptr, B200_ERR_CUDA, "cuTensorMapEncodeTiled not available from the driver");
+  cuuint64_t dims[2] = {(cuuint64_t)K, (cuuint64_t)rows};
+  cuuint64_t strides[1] = {(cuuint64_t)K * 2};
+  cuuint32_t box[2] = {64, (cuuint32_t)rows};
+  cuuint32_t estr[2] = {1, 1};
+  CUresult r = enc(tm, CU_TENSOR_MAP_DATA_TYPE_FLOAT16, 2, const_cast<__half*>(ptr), dims, strides, box, estr,
+                   CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_256B,
+                   CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
+  B200_CHECK(r == CUDA_SUCCESS, B200_ERR_CUDA, "cuTensorMapEncodeTiled(sinc/conv weights) failed: %d", (int)r);
+  return B200_OK;
+}
+
+template <int CIN, int CPAD, int NW, int NREAL, int KT>
+static int launch_sc(const __half* Wh, const __half* Wl, SincConvWgParams p, int NB, int Lconv, cudaStream_t stream) {
+  constexpr int kIn = CIN == 0 ? (kSCPos - 1) * kSincStride + KT : (kSCPos + 4) * CPAD;
+  constexpr int kBoxes = (KT + 63) / 64;
+  p.xs_bytes = (uint32_t)align_up((size_t)kIn * 2 * sizeof(__half), 1024);
+  p.w_off = 1024 + p.xs_bytes;
+  p.w_box_bytes = NW * 128;
+  uint32_t w_bytes = 2u * kBoxes * p.w_box_bytes;
+  const uint32_t st_bytes = (uint32_t)(NW * kSCPitch * sizeof(float));
+  if (w_bytes < st_bytes) w_bytes = st_bytes;
+  p.pool_off = p.w_off + (uint32_t)align_up(w_bytes, 1024);
+  const size_t smem = 1024 + p.pool_off + (size_t)NREAL * 65 * sizeof(float);
+  B200_CHECK(smem <= 227 * 1024, B200_ERR_STATE, "sinc/conv wgmma kernel: %zu B of shared memory", smem);
+  CUtensorMap th, tl;
+  int rc;
+  if ((rc = make_w_map(&th, Wh, NW, KT))) return rc;
+  if ((rc = make_w_map(&tl, Wl, NW, KT))) return rc;
+  auto kernel = sinc_conv_wg_kernel<CIN, CPAD, NW, NREAL, KT>;
+  static bool attr_set = false;                             // one per instantiation
+  if (!attr_set) {
+    B200_CUDA_OK(cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+    attr_set = true;
+  }
+  kernel<<<dim3(ceil_div(Lconv, kSCPos), NB), kSCThreads, smem, stream>>>(th, tl, p);
+  B200_CUDA_OK(cudaGetLastError());
+  return B200_OK;
+}
+
+int sinc_wg_forward(const float* wav, const long long* chunk_off, const int* chunk_valid, const float2* affine,
+                    const __half* Wh, const __half* Wl, int NB, float* P0, double2* part, int ntiles,
+                    cudaStream_t stream) {
+  SincConvWgParams p{};
+  p.wav = wav; p.chunk_off = chunk_off; p.chunk_valid = chunk_valid; p.affine = affine;
+  p.Pout = P0; p.part = part; p.Lp = kPool0; p.ntiles = ntiles;
+  B200_CHECK(ceil_div(kSincLen, kSCPos) == ntiles, B200_ERR_STATE, "sinc tiles: %d", ntiles);
+  return launch_sc<0, 1, 80, 80, 256>(Wh, Wl, p, NB, kSincLen, stream);
+}
+
+int conv5_wg_forward(int layer, const float* Pin, const float2* affine, const __half* Wh, const __half* Wl,
+                     const float* bias, int NB, float* Pout, double2* part, int ntiles, cudaStream_t stream) {
+  SincConvWgParams p{};
+  p.affine = affine; p.bias = bias; p.Pout = Pout; p.part = part; p.ntiles = ntiles;
+  if (layer == 0) {
+    p.Pin = Pin; p.Lin = kPool0; p.Lp = kPool1;
+    B200_CHECK(ceil_div(kConv1Len, kSCPos) == ntiles, B200_ERR_STATE, "conv1 tiles: %d", ntiles);
+    return launch_sc<80, 80, 64, 60, 400>(Wh, Wl, p, NB, kConv1Len, stream);
+  }
+  p.Pin = Pin; p.Lin = kPool1; p.Lp = kPool2;
+  B200_CHECK(ceil_div(kConv2Len, kSCPos) == ntiles, B200_ERR_STATE, "conv2 tiles: %d", ntiles);
+  return launch_sc<60, 64, 64, 60, 320>(Wh, Wl, p, NB, kConv2Len, stream);
+}
+
+}  // namespace b200

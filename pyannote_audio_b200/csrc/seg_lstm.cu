@@ -198,7 +198,7 @@ static size_t carve_lstm(int NB, void* base, LstmWs* w) {
   };
   LstmWs t;
   const size_t M = (size_t)NB * kFrames;
-  t.Gx = (float*)take((size_t)align_up(NB, 128) * kFrames * 1024 * sizeof(float));   // padded for the gx layout
+  t.Gx = (float*)take(M * 1024 * sizeof(float));
   t.Ya = (float*)take(M * 256 * sizeof(float));
   t.Yb = (float*)take(M * 256 * sizeof(float));
   t.Z1 = (float*)take(M * 128 * sizeof(float));
@@ -243,20 +243,17 @@ int lstm_head_forward(const SegWeights& W, const float* x0, int NB, void* ws, un
   __half* outs_h[2] = {w.Yah, w.Ybh};
   __half* outs_l[2] = {w.Yal, w.Ybl};
   for (int l = 0; l < W.lstm_layers; ++l) {
-    if (tc && rec_impl == 1) {   // tensor-core recurrence: projections in gx layout, outputs as (hi, lo)
-      rc = gemm_tc_split_gx(in_h, in_l, W.k_in[l], W.w_ih_hi[l], W.w_ih_lo[l], W.k_in[l], w.Gx, W.b_g[l], NB, kFrames,
-                            1024, W.k_in[l], num_sms, stream);
-      if (rc) return rc;
-      if ((rc = lstm_rec_tc(w.Gx, W.w_hh_hi[l], W.w_hh_lo[l], outs_h[l & 1], outs_l[l & 1], NB, stream))) return rc;
-      in_h = outs_h[l & 1]; in_l = outs_l[l & 1];
-      continue;
-    }
     if (tc)
       rc = gemm_tc_split(in_h, in_l, W.k_in[l], W.w_ih_hi[l], W.w_ih_lo[l], W.k_in[l], w.Gx, 1024, nullptr, nullptr, 0,
                          W.b_g[l], M, 1024, W.k_in[l], 0, num_sms, stream);
     else
       rc = sgemm_nt(in, W.k_in[l], W.w_ih[l], W.k_in[l], w.Gx, 1024, W.b_g[l], M, 1024, W.k_in[l], 0, stream);
     if (rc) return rc;
+    if (tc && rec_impl == 1) {   // tensor-core recurrence (seg_lstm_wg.cu)
+      if ((rc = lstm_rec_wg(w.Gx, W.w_hh_hi[l], W.w_hh_lo[l], outs_h[l & 1], outs_l[l & 1], NB, stream))) return rc;
+      in_h = outs_h[l & 1]; in_l = outs_l[l & 1];
+      continue;
+    }
     float* y = tc ? nullptr : outs[l & 1];
     __half* yh = tc ? outs_h[l & 1] : nullptr;
     __half* yl = tc ? outs_l[l & 1] : nullptr;

@@ -1,0 +1,189 @@
+// BiLSTM recurrence on the Hopper tensor cores (wgmma), split-precision fp16 with fp32-level accuracy.
+//
+// Reference: pyannote/audio/models/segmentation/PyanNet.py:223-228 (nn.LSTM(., 128, bidirectional, batch_first)).
+// Per step t:  G[b][(unit, gate)] = Gx[b][t] + h_{t-1}[b] . W_hh^T,  c = f*c + i*g,  h = o * tanh(c).
+//
+// A 2-CTA cluster runs 64 sequences of one direction; each CTA owns 64 hidden units, i.e. the GEMM
+//     D[64 sequences][256 = (unit, gate)] += h[64][128 units] * W[256][128]^T          (m64n256, 8 K=16 steps)
+// with its W_hh slice as fp16 (hi, lo) resident in shared memory (TMA once, 128-byte swizzle) and h as the register
+// A operand.  The 256 columns are ordered  n = 32 jj + 8 gate + u  (local unit 8 jj + u), so the accumulator
+// fragment of a thread holds all four gates of local units 8 jj + 2 (lane % 4) + {0, 1} for its two rows: the gates,
+// c (registers) and the new h of those units are computed in place, and the new h pairs are exactly the thread's A
+// fragments of the K steps over its own units.  Every thread stores its 16 (hi, lo) pairs into its own CTA's and
+// (DSMEM) the peer's h buffer at the same thread index; the next step reads all eight K steps' A fragments from
+// there.  One cluster barrier per step.
+// Products: h_lo*W_hi + h_hi*W_lo + h_hi*W_hi in fp32, like gemm_tc.cu.
+#include "common.cuh"
+#include "seg.cuh"
+#include "tc_common.cuh"
+
+namespace b200 {
+
+constexpr int kRecThreads = 128;
+constexpr int kRecSeqs = 64;
+constexpr uint32_t kRecWBox = 256u * 128u;              // one [256 rows][64 k] fp16 box (32 KB)
+constexpr uint32_t kRecXOff = 1024u + 4u * kRecWBox;     // h buffers [2 parity][2 source CTA][32 regs][128 threads] u32
+
+__device__ __forceinline__ float rec_sigmoid(float x) { return 1.f / (1.f + expf(-x)); }
+
+__device__ __forceinline__ uint32_t pack_h2(float a, float b) {
+  __half2 h = __floats2half2_rn(a, b);
+  return *reinterpret_cast<uint32_t*>(&h);
+}
+
+__global__ void __cluster_dims__(2, 1, 1) __launch_bounds__(kRecThreads, 1)
+lstm_rec_wg_kernel(const __grid_constant__ CUtensorMap tmWh, const __grid_constant__ CUtensorMap tmWl,
+                   const float* __restrict__ Gx /*[NB][589][1024]*/, __half* __restrict__ Yh, __half* __restrict__ Yl,
+                   int NB, int ntiles) {
+  extern __shared__ uint8_t smem_raw[];
+  const uint32_t raw = smem_u32(smem_raw);
+  const uint32_t base = (raw + 1023u) & ~1023u;
+  const uint32_t bar = base, w_smem = base + 1024u;
+  uint32_t* xbuf = reinterpret_cast<uint32_t*>(smem_raw + (base - raw) + kRecXOff);
+  uint32_t rank;
+  asm volatile("mov.u32 %0, %%cluster_ctarank;" : "=r"(rank));
+  const int cid = blockIdx.x >> 1;
+  const int dir = cid / ntiles, tile = cid - dir * ntiles;
+  const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31, q = lane & 3;
+  uint32_t peer_x;                                       // the peer CTA's h buffers
+  asm volatile("mapa.shared::cluster.u32 %0, %1, %2;" : "=r"(peer_x) : "r"(base + kRecXOff), "r"(rank ^ 1u));
+
+  if (tid == 0) {
+    mbar_init(bar, 1);
+    asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
+    mbar_expect_tx(bar, 4u * kRecWBox);
+    const int slice = dir * 2 + (int)rank;
+    tma_load_3d(&tmWh, bar, w_smem, 0, 0, slice);
+    tma_load_3d(&tmWh, bar, w_smem + kRecWBox, 64, 0, slice);
+    tma_load_3d(&tmWl, bar, w_smem + 2 * kRecWBox, 0, 0, slice);
+    tma_load_3d(&tmWl, bar, w_smem + 3 * kRecWBox, 64, 0, slice);
+  }
+  for (int i = threadIdx.x; i < 2 * 32 * kRecThreads; i += kRecThreads) xbuf[i] = 0u;   // h_{-1} = 0 (parity 0)
+  // both CTAs of the cluster are running (and zeroed) before anything is stored into the peer
+  asm volatile("barrier.cluster.arrive.release.aligned;\n\tbarrier.cluster.wait.acquire.aligned;" ::: "memory");
+  mbar_wait(bar, 0);
+
+  int rows[2];
+  rows[0] = tile * kRecSeqs + 16 * warp + (lane >> 2);
+  rows[1] = rows[0] + 8;
+  float c[2][8][2];
+#pragma unroll
+  for (int i = 0; i < 2; ++i)
+#pragma unroll
+    for (int jj = 0; jj < 8; ++jj) c[i][jj][0] = c[i][jj][1] = 0.f;
+  const int gcol = dir * 512 + ((int)rank * 64 + 2 * q) * 4;   // + 32 jj: units 8 jj + 2q, +1, four gates each
+
+  float acc[128];
+  for (int step = 0; step < kFrames; ++step) {
+    const int t = dir ? (kFrames - 1 - step) : step;
+    // acc = Gx[b][t] (the input projection with both biases)
+#pragma unroll
+    for (int i = 0; i < 2; ++i) {
+      const bool ok = rows[i] < NB;
+      const float4* gp = reinterpret_cast<const float4*>(Gx + ((size_t)(ok ? rows[i] : 0) * kFrames + t) * 1024 + gcol);
+#pragma unroll
+      for (int jj = 0; jj < 8; ++jj) {
+        const float4 u0 = ok ? __ldg(gp + 8 * jj) : make_float4(0.f, 0.f, 0.f, 0.f);
+        const float4 u1 = ok ? __ldg(gp + 8 * jj + 1) : make_float4(0.f, 0.f, 0.f, 0.f);
+        const float v[8] = {u0.x, u0.y, u0.z, u0.w, u1.x, u1.y, u1.z, u1.w};   // (unit e, gate g) at 4 e + g
+#pragma unroll
+        for (int g = 0; g < 4; ++g)
+#pragma unroll
+          for (int e = 0; e < 2; ++e) acc[4 * (4 * jj + g) + 2 * i + e] = v[4 * e + g];
+      }
+      if (step + 1 < kFrames && ok) {                     // next step's projection into L2
+        const int tn = dir ? t - 1 : t + 1;
+        const char* np = reinterpret_cast<const char*>(Gx + ((size_t)rows[i] * kFrames + tn) * 1024 + gcol);
+#pragma unroll
+        for (int jj = 0; jj < 8; ++jj) asm volatile("prefetch.global.L2 [%0];" ::"l"(np + 128 * jj));
+      }
+    }
+    // acc += h_{t-1} W^T over the 8 K steps (K steps 4 r .. 4 r + 3 = the units of CTA r)
+    wg_fence();
+#pragma unroll
+    for (int ks = 0; ks < 8; ++ks) {
+      const int s = ks & 3;                               // K step inside one CTA's 64 units: jj = 2s, 2s + 1
+      const uint32_t* xb = xbuf + ((step & 1) * 2 + (ks >> 2)) * 32 * kRecThreads;
+      uint32_t ah[4], al[4];
+#pragma unroll
+      for (int r = 0; r < 4; ++r) {
+        const int i = r & 1, jj = 2 * s + (r >> 1);
+        ah[r] = xb[(i * 8 + jj) * kRecThreads + tid];
+        al[r] = xb[(16 + i * 8 + jj) * kRecThreads + tid];
+      }
+      const uint32_t wb = w_smem + (uint32_t)(ks >> 2) * kRecWBox + (uint32_t)(ks & 3) * 32u;
+      const uint64_t wh = wg_desc(wb, 128), wl = wg_desc(wb + 2 * kRecWBox, 128);
+      WgmmaRS<256>::mma(acc, al, wh);                      // small cross terms first, hi*hi last
+      WgmmaRS<256>::mma(acc, ah, wl);
+      WgmmaRS<256>::mma(acc, ah, wh);
+    }
+    wg_commit();
+    wg_wait<0>();
+    // gates (PyTorch order i, f, g, o), cell update, new h: both CTAs' h buffers, layer output
+    const uint32_t hoff = (uint32_t)((((step + 1) & 1) * 2 + (int)rank) * 32 * kRecThreads + tid);
+    uint32_t* own = xbuf + hoff;
+    const uint32_t px = peer_x + hoff * 4u;
+#pragma unroll
+    for (int i = 0; i < 2; ++i) {
+#pragma unroll
+      for (int jj = 0; jj < 8; ++jj) {
+        float hn[2];
+#pragma unroll
+        for (int e = 0; e < 2; ++e) {
+          const float ig = rec_sigmoid(acc[4 * (4 * jj + 0) + 2 * i + e]);
+          const float fg = rec_sigmoid(acc[4 * (4 * jj + 1) + 2 * i + e]);
+          const float gg = tanhf(acc[4 * (4 * jj + 2) + 2 * i + e]);
+          const float og = rec_sigmoid(acc[4 * (4 * jj + 3) + 2 * i + e]);
+          c[i][jj][e] = fmaf(fg, c[i][jj][e], ig * gg);
+          hn[e] = og * tanhf(c[i][jj][e]);
+        }
+        const __half h0 = __float2half_rn(hn[0]), h1 = __float2half_rn(hn[1]);
+        const __half2 hi2 = __halves2half2(h0, h1);
+        const uint32_t vh = *reinterpret_cast<const uint32_t*>(&hi2);
+        const uint32_t vl = pack_h2(hn[0] - __half2float(h0), hn[1] - __half2float(h1));
+        own[(i * 8 + jj) * kRecThreads] = vh;
+        own[(16 + i * 8 + jj) * kRecThreads] = vl;
+        asm volatile("st.shared::cluster.u32 [%0], %1;" ::"r"(px + (uint32_t)((i * 8 + jj) * kRecThreads) * 4u),
+                     "r"(vh) : "memory");
+        asm volatile("st.shared::cluster.u32 [%0], %1;" ::"r"(px + (uint32_t)((16 + i * 8 + jj) * kRecThreads) * 4u),
+                     "r"(vl) : "memory");
+        if (rows[i] < NB) {
+          const size_t o = ((size_t)rows[i] * kFrames + t) * 256 + dir * 128 + rank * 64 + 8 * jj + 2 * q;
+          *reinterpret_cast<uint32_t*>(Yh + o) = vh;
+          *reinterpret_cast<uint32_t*>(Yl + o) = vl;
+        }
+      }
+    }
+    // the peer's h of this step has landed; both CTAs are done reading the buffer the next step overwrites
+    asm volatile("barrier.cluster.arrive.release.aligned;\n\tbarrier.cluster.wait.acquire.aligned;" ::: "memory");
+  }
+}
+
+int lstm_rec_wg(const float* Gx, const __half* Wh, const __half* Wl, __half* Yh, __half* Yl, int NB,
+                cudaStream_t stream) {
+  PFN_encodeTiled enc = get_encode();
+  B200_CHECK(enc != nullptr, B200_ERR_CUDA, "cuTensorMapEncodeTiled not available from the driver");
+  CUtensorMap tm[2];
+  for (int h = 0; h < 2; ++h) {
+    cuuint64_t dims[3] = {128, 256, 4};                    // [k = unit][n = (unit, gate) column][dir * 2 + rank]
+    cuuint64_t strides[2] = {128 * 2, 256 * 128 * 2};
+    cuuint32_t box[3] = {64, 256, 1};
+    cuuint32_t estr[3] = {1, 1, 1};
+    CUresult r = enc(&tm[h], CU_TENSOR_MAP_DATA_TYPE_FLOAT16, 3, const_cast<__half*>(h ? Wl : Wh), dims, strides, box,
+                     estr, CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_128B,
+                     CU_TENSOR_MAP_L2_PROMOTION_L2_256B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
+    B200_CHECK(r == CUDA_SUCCESS, B200_ERR_CUDA, "cuTensorMapEncodeTiled(lstm W_hh) failed: %d", (int)r);
+  }
+  const size_t smem = 1024 + kRecXOff + 4u * 32u * kRecThreads * 4u;
+  static bool attr_set = false;
+  if (!attr_set) {
+    B200_CUDA_OK(cudaFuncSetAttribute(lstm_rec_wg_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+    attr_set = true;
+  }
+  const int ntiles = ceil_div(NB, kRecSeqs);
+  lstm_rec_wg_kernel<<<2 * 2 * ntiles, kRecThreads, smem, stream>>>(tm[0], tm[1], Gx, Yh, Yl, NB, ntiles);
+  B200_CUDA_OK(cudaGetLastError());
+  return B200_OK;
+}
+
+}  // namespace b200

@@ -85,7 +85,7 @@ __global__ void __launch_bounds__(128) sinc_pool_kernel(const float* __restrict_
     reinterpret_cast<float4*>(fs)[i] = reinterpret_cast<const float4*>(filt)[i];
   __syncthreads();
 
-  // accumulators as packed channel pairs (c, c+1): one FFMA2 per pair
+  // accumulators as packed channel pairs (c, c+1)
   f32x2_t ac2[3][10], as2[3][10];
 #pragma unroll
   for (int p = 0; p < 3; ++p)
@@ -215,7 +215,7 @@ __global__ void __launch_bounds__(192) conv5_pool_kernel(const float* __restrict
     }
     xin[i] = v;
   }
-  f32x2_t acc2[3][10];                 // packed channel pairs (c, c+1): one FFMA2 per pair
+  f32x2_t acc2[3][10];                 // packed channel pairs (c, c+1)
 #pragma unroll
   for (int p = 0; p < 3; ++p)
 #pragma unroll
@@ -297,7 +297,6 @@ struct SincWs {
   float2 *af_wav, *af0, *af1, *af2;
   double2 *part0, *part1, *part2;
   float *P0, *P1, *P2;
-  __half *Xh, *Xl;     // channels-last fp16 (hi, lo) input of the tensor-core conv layers
 };
 
 static size_t carve(int NB, void* base, SincWs* w) {
@@ -319,8 +318,6 @@ static size_t carve(int NB, void* base, SincWs* w) {
   t.P0 = (float*)take(sizeof(float) * (size_t)NB * 80 * kPool0);
   t.P1 = (float*)take(sizeof(float) * (size_t)NB * 60 * kPool1);
   t.P2 = (float*)take(sizeof(float) * (size_t)NB * 60 * kPool2);
-  t.Xh = (__half*)take(sizeof(__half) * (size_t)NB * kPool0 * 80);
-  t.Xl = (__half*)take(sizeof(__half) * (size_t)NB * kPool0 * 80);
   if (w) *w = t;
   return align_up(off, 256);
 }
@@ -328,7 +325,7 @@ static size_t carve(int NB, void* base, SincWs* w) {
 size_t sincnet_workspace_bytes(int NB) { return carve(NB, nullptr, nullptr); }
 
 int sincnet_forward(const SegWeights& W, const float* wav, const long long* chunk_off, const int* chunk_valid, int NB,
-                    void* ws, float* x0, int conv_impl, int num_sms, cudaStream_t stream) {
+                    void* ws, float* x0, int conv_impl, cudaStream_t stream) {
   SincWs w;
   carve(NB, ws, &w);
   static bool attr = false;
@@ -341,49 +338,39 @@ int sincnet_forward(const SegWeights& W, const float* wav, const long long* chun
     B200_CUDA_OK(cudaFuncSetAttribute(conv5_pool_kernel<60>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem_c60));
     attr = true;
   }
-  // conv_impl: 0 = fp32 CUDA-core kernels, 1 = tensor cores for all three layers (default); 2 = tensor-core sinc layer
-  // only, 3 = tensor-core Conv1d layers only (the mixed settings localise a difference between the twins)
-  const bool tc_sinc = conv_impl == 1 || conv_impl == 2, tc_conv = conv_impl == 1 || conv_impl == 3;
   wav_stats_kernel<<<NB, 512, 0, stream>>>(wav, chunk_off, chunk_valid, W.wav_w, W.wav_b, w.af_wav);
-  if (tc_sinc) {
-    const int nt0 = ceil_div(kPool0, 80);
-    const int rc0 = sinc_tc_forward(wav, chunk_off, chunk_valid, w.af_wav, W.sinc_tc_hi, W.sinc_tc_lo, NB, w.P0, w.part0,
-                                    nt0, num_sms, stream);
-    if (rc0) return rc0;
-    in_finalize_kernel<<<ceil_div(NB * 80, 128), 128, 0, stream>>>(w.part0, nt0, kPool0, 80, W.in_gamma[0],
-                                                                   W.in_beta[0], w.af0, NB * 80);
+  // conv_impl: 1 = split-fp16 wgmma kernels (default), 0 = the fp32 CUDA-core twins
+  int rc;
+  if (conv_impl) {
+    if ((rc = sinc_wg_forward(wav, chunk_off, chunk_valid, w.af_wav, W.sinc_wg_hi, W.sinc_wg_lo, NB, w.P0, w.part0,
+                              kTiles0, stream)))
+      return rc;
   } else {
     sinc_pool_kernel<<<dim3(kTiles0, NB), 128, smem_sinc, stream>>>(wav, chunk_off, chunk_valid, w.af_wav, W.sinc_f,
                                                                    w.P0, w.part0);
-    in_finalize_kernel<<<ceil_div(NB * 80, 128), 128, 0, stream>>>(w.part0, kTiles0, kPool0, 80, W.in_gamma[0],
-                                                                   W.in_beta[0], w.af0, NB * 80);
   }
-  if (tc_conv) {
-    // tensor-core path: IN + leaky-relu + split to channels-last fp16 (hi, lo), then the implicit GEMM
-    int rc;
-    const int nt1 = ceil_div(kPool1, 80), nt2 = ceil_div(kPool2, 80);
-    if ((rc = in_apply_split(w.P0, w.af0, NB, 80, 80, kPool0, w.Xh, w.Xl, stream))) return rc;
-    if ((rc = conv5_tc_forward(w.Xh, w.Xl, W.conv_tc_hi[0], W.conv_tc_lo[0], W.conv_b[0], NB, kPool0, kPool1, 5, w.P1,
-                               w.part1, nt1, num_sms, stream)))
+  in_finalize_kernel<<<ceil_div(NB * 80, 128), 128, 0, stream>>>(w.part0, kTiles0, kPool0, 80, W.in_gamma[0],
+                                                                 W.in_beta[0], w.af0, NB * 80);
+  if (conv_impl) {
+    if ((rc = conv5_wg_forward(0, w.P0, w.af0, W.conv_wg_hi[0], W.conv_wg_lo[0], W.conv_b[0], NB, w.P1, w.part1,
+                               kTiles1, stream)))
       return rc;
-    in_finalize_kernel<<<ceil_div(NB * 60, 128), 128, 0, stream>>>(w.part1, nt1, kPool1, 60, W.in_gamma[1],
-                                                                   W.in_beta[1], w.af1, NB * 60);
-    if ((rc = in_apply_split(w.P1, w.af1, NB, 60, 64, kPool1, w.Xh, w.Xl, stream))) return rc;
-    if ((rc = conv5_tc_forward(w.Xh, w.Xl, W.conv_tc_hi[1], W.conv_tc_lo[1], W.conv_b[1], NB, kPool1, kPool2, 4, w.P2,
-                               w.part2, nt2, num_sms, stream)))
-      return rc;
-    in_finalize_kernel<<<ceil_div(NB * 60, 128), 128, 0, stream>>>(w.part2, nt2, kPool2, 60, W.in_gamma[2],
-                                                                   W.in_beta[2], w.af2, NB * 60);
   } else {
     conv5_pool_kernel<80><<<dim3(kTiles1, NB), 192, smem_c80, stream>>>(w.P0, kPool0, w.af0, W.conv_w[0], W.conv_b[0],
                                                                         w.P1, kPool1, kTiles1, w.part1);
-    in_finalize_kernel<<<ceil_div(NB * 60, 128), 128, 0, stream>>>(w.part1, kTiles1, kPool1, 60, W.in_gamma[1],
-                                                                   W.in_beta[1], w.af1, NB * 60);
+  }
+  in_finalize_kernel<<<ceil_div(NB * 60, 128), 128, 0, stream>>>(w.part1, kTiles1, kPool1, 60, W.in_gamma[1],
+                                                                 W.in_beta[1], w.af1, NB * 60);
+  if (conv_impl) {
+    if ((rc = conv5_wg_forward(1, w.P1, w.af1, W.conv_wg_hi[1], W.conv_wg_lo[1], W.conv_b[1], NB, w.P2, w.part2,
+                               kTiles2, stream)))
+      return rc;
+  } else {
     conv5_pool_kernel<60><<<dim3(kTiles2, NB), 192, smem_c60, stream>>>(w.P1, kPool1, w.af1, W.conv_w[1], W.conv_b[1],
                                                                         w.P2, kPool2, kTiles2, w.part2);
-    in_finalize_kernel<<<ceil_div(NB * 60, 128), 128, 0, stream>>>(w.part2, kTiles2, kPool2, 60, W.in_gamma[2],
-                                                                   W.in_beta[2], w.af2, NB * 60);
   }
+  in_finalize_kernel<<<ceil_div(NB * 60, 128), 128, 0, stream>>>(w.part2, kTiles2, kPool2, 60, W.in_gamma[2],
+                                                                 W.in_beta[2], w.af2, NB * 60);
   const size_t total = (size_t)NB * kFrames * 64;
   in_apply_transpose_kernel<<<(unsigned)((total + 255) / 256), 256, 0, stream>>>(w.P2, w.af2, x0, NB);
   B200_CUDA_OK(cudaGetLastError());

@@ -105,7 +105,7 @@ class Inference(BaseInference):
         window_size = self.model.audio.get_num_samples(self.duration)
         step_size = round(self.step * sample_rate)
         if window_size != ops.CHUNK:
-            raise ValueError("the sm_100a segmentation kernels are specialised for 10 s chunks at 16 kHz")
+            raise ValueError("the segmentation kernels are specialised for 10 s chunks at 16 kHz")
         _, num_samples = waveform.shape
         off, valid, num_chunks, has_last = chunk_layout(num_samples, window_size, step_size)
         ctx = self.model._ctx()

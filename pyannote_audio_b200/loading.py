@@ -96,7 +96,7 @@ def _pipeline_class(name: str):
         from .vad import VoiceActivityDetection
 
         return VoiceActivityDetection
-    raise NotImplementedError(f"pipeline '{name}' has no sm_100a implementation (SpeakerDiarization and "
+    raise NotImplementedError(f"pipeline '{name}' has no CUDA implementation here (SpeakerDiarization and "
                               f"VoiceActivityDetection are available)")
 
 

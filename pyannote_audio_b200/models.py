@@ -29,7 +29,7 @@ def get_context(device) -> "ops.Context":
     device = torch.device(device)
     if device.type != "cuda":
         raise RuntimeError(
-            f"pyannote_audio_b200 models only run on CUDA (B200 / sm_100a) devices, not on '{device}': move the "
+            f"pyannote_audio_b200 models only run on CUDA (H100 / sm_90a) devices, not on '{device}': move the "
             f"model with .to(torch.device('cuda'))")
     index = device.index if device.index is not None else torch.cuda.current_device()
     if index not in _CONTEXTS:
@@ -118,7 +118,7 @@ class Model(nn.Module):
         class_name = meta["architecture"]["class"]
         klass = {"PyanNet": PyanNet, "WeSpeakerResNet34": WeSpeakerResNet34}.get(class_name)
         if klass is None:
-            raise NotImplementedError(f"architecture {meta['architecture']['module']}.{class_name} has no sm_100a "
+            raise NotImplementedError(f"architecture {meta['architecture']['module']}.{class_name} has no CUDA "
                                       f"implementation (community-1 uses PyanNet and WeSpeakerResNet34)")
         if cls not in (Model, klass) and not issubclass(klass, cls):
             raise ValueError(f"checkpoint holds a {class_name}, not a {cls.__name__}")
@@ -250,7 +250,7 @@ class PyanNet(Model):
         if (lstm_hp["hidden_size"], lstm_hp["bidirectional"], lstm_hp["monolithic"]) != (128, True, True) or \
                 not (1 <= lstm_hp["num_layers"] <= 4) or (linear_hp["hidden_size"], linear_hp["num_layers"]) != (128, 2) \
                 or sinc_hp["stride"] != 10:
-            raise NotImplementedError("the sm_100a kernels implement the community-1 PyanNet shape only: "
+            raise NotImplementedError("the CUDA kernels implement the community-1 PyanNet shape only: "
                                       "SincNet stride 10, 1-4 bidirectional LSTM layers of 128, 2 linear layers of 128")
         self.hparams.sincnet, self.hparams.lstm, self.hparams.linear = sinc_hp, lstm_hp, linear_hp
         self.sincnet = _SincNetParams()
@@ -348,7 +348,7 @@ class WeSpeakerResNet34(Model):
         super().__init__(sample_rate=sample_rate, num_channels=num_channels)
         if (sample_rate, num_mel_bins, frame_length, frame_shift, dither, window_type, use_energy) != \
                 (16000, 80, 25, 10, 0.0, "hamming", False):
-            raise NotImplementedError("the sm_100a fbank kernel implements the community-1 configuration only "
+            raise NotImplementedError("the fbank kernel implements the community-1 configuration only "
                                       "(16 kHz, 80 mel bins, 25/10 ms hamming frames, no dither, no energy)")
         self.resnet = _ResNet34Params()
         self.specifications = Specifications(problem=Problem.REPRESENTATION, resolution=Resolution.CHUNK, duration=10.0)

@@ -66,7 +66,7 @@ class Context:
         self.lib = _lib.load()
         device = torch.device(device)
         if device.type != "cuda":
-            raise _lib.B200Error(f"pyannote_audio_b200 runs on CUDA (sm_100a) devices only, got '{device}'")
+            raise _lib.B200Error(f"pyannote_audio_b200 runs on CUDA (sm_90a) devices only, got '{device}'")
         if not torch.cuda.is_available():
             raise _lib.B200Error("no CUDA device is visible: pyannote_audio_b200 has no CPU fallback")
         self.device = torch.device("cuda", device.index if device.index is not None else torch.cuda.current_device())
@@ -77,7 +77,8 @@ class Context:
         self.seg_loaded = False
         self.emb_loaded = False
         self.owners = {}          # slot ("seg" | "emb") -> stamp of the model whose weights are resident (models.py)
-        # A/B knob for scripts (same role as the B200_* variables the library reads): B200_OPTIONS="key=value,..."
+        # A/B knob for scripts (like B200_CONV_IMPL / B200_EMB_MAX_BATCH / B200_SEG_MAX_BATCH, which the library
+        # reads itself): B200_OPTIONS="key=value,..."
         # is applied through b200_ctx_set_option, so unknown keys / bad values fail loudly
         import os
 

@@ -1,10 +1,10 @@
 """Multi-GPU sharding of the hot path (one process per GPU, torch.distributed; NCCL on GPUs, gloo in CPU tests).
 
-The reference has no inference-time parallelism at all (SURVEY.md section 2.2); the path shards naturally:
+The reference has no inference-time parallelism at all; the path shards naturally:
   * many files  -> ``ChunkPool``: the chunks of all files form one global pool, every rank runs PyanNet + WeSpeaker on
     its share and writes the results straight into its slice of ONE packed buffer, a single in-place NCCL all-gather
     replicates (embeddings (C,3,256) f32 | powerset classes (C,589) u8) on every GPU, then file g is clustered /
-    reconstructed on rank g mod N (SURVEY.md section 8e; hook point core/pipeline.py:497-508).  File-level sharding
+    reconstructed on rank g mod N (hook point core/pipeline.py:497-508).  File-level sharding
     without any collective stays available (bench.py --parallelism files);
   * one long file -> ``apply_sharded``: contiguous chunk ranges per rank (chunk c only needs samples
     [c*step, c*step+160000)), the same all-gather, clustering replicated.

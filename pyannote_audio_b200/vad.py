@@ -1,7 +1,7 @@
 """Voice activity detection pipeline (mirror of /root/reference/src/pyannote/audio/pipelines/
 voice_activity_detection.py:66-204) reusing the diarization kernels: PyanNet sliding window -> speech indicator per
 frame (max over the speakers of the powerset multilabel) -> Hamming-windowed overlap-add on the device
-(b200_aggregate) -> Binarize.  SURVEY.md section 8(f) row 3."""
+(b200_aggregate) -> Binarize."""
 from __future__ import annotations
 
 from typing import Callable, Mapping, Optional, Union

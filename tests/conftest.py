@@ -9,7 +9,7 @@ if ROOT not in sys.path:
 
 
 def pytest_configure(config):
-    config.addinivalue_line("markers", "gpu: needs a B200 (runs under `pytest -m gpu` on the GPU box)")
+    config.addinivalue_line("markers", "gpu: needs an H100 (runs under `pytest -m gpu`)")
 
 
 @pytest.fixture(scope="session")
@@ -20,8 +20,8 @@ def golden():
 
 
 def pytest_report_header(config):
-    """Which GPU ran the `-m gpu` tests (serial number, clocks, ECC state): boxes of the pool differ, and a mismatch
-    that never reproduces (profiles/r02_profile_summary.md, third session) can only be followed up with this."""
+    """Which GPU ran the `-m gpu` tests (serial number, clocks, ECC state): GPUs of a pool differ, and a mismatch
+    that never reproduces can only be followed up with this."""
     import shutil
     import subprocess
 

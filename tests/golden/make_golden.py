@@ -4,7 +4,7 @@
     PYTHONPATH=. python tests/golden/make_golden.py
 
 Nothing here is needed at test time; the committed .npz is.  (The reference package as a whole cannot be imported
-in this environment, see SURVEY.md section 8c; these five leaf modules can.)
+in this environment; these five leaf modules can.)
 """
 import numpy as np
 import torch

@@ -345,7 +345,7 @@ def test_apply_sharded_single_rank(pipeline):
 
 
 def test_audio_ingest_on_device(dev, pipeline, tmp_path):
-    """SURVEY section 8(f) row 1: PCM -> float, downmix, resample to 16 kHz on the device (b200_audio_ingest) against
+    """PCM -> float, downmix, resample to 16 kHz on the device (b200_audio_ingest) against
     the reference's host path (core/io.py:223-265: mean over channels, then torchaudio.functional.resample)."""
     import torchaudio.functional as AF
     from scipy.io import wavfile
@@ -407,7 +407,7 @@ def test_audio_ingest_on_device(dev, pipeline, tmp_path):
 
 
 def test_aggregate_and_vad_on_device(dev, models, oracle_models):
-    """SURVEY section 8(f) row 3: Inference.aggregate on the device (bit-identical to numpy's arithmetic, NaN-aware,
+    """Inference.aggregate on the device (bit-identical to numpy's arithmetic, NaN-aware,
     hamming / warm-up windows, skip_average) and the VoiceActivityDetection pipeline built on it."""
     from pyannote_audio_b200.inference import Inference
     from pyannote_audio_b200.core import SlidingWindow, SlidingWindowFeature

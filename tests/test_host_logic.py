@@ -25,7 +25,7 @@ def test_chunk_layout_matches_oracle_chunking(T):
             got[: valid[c]] = wav[0, off[c]: off[c] + valid[c]].numpy()
             assert np.array_equal(ref, got)
     assert len(off) == num_chunks + int(has_last)
-    # SURVEY.md section 8: 30 s -> 21 chunks, 10 min -> 591
+    # 30 s -> 21 chunks, 10 min -> 591
     if T == 480000:
         assert len(off) == 21
     if T == 9600000:

@@ -109,7 +109,7 @@ def test_slide_plumbing_config0():
 
 
 def test_to_diarization_tie_rule_only_differs_from_numpy_default_on_ties():
-    """np.argsort's default kind is not stable on every host (SURVEY.md Appendix A): the reference's top-`count`
+    """np.argsort's default kind is not stable on every host: the reference's top-`count`
     selection is ambiguous exactly where cluster activations tie at the selection boundary.  The oracle pins
     "descending activation, then ascending cluster index"; check that numpy's default order on THIS host agrees with
     it everywhere except at such ties (a reference ambiguity, not a parity failure)."""

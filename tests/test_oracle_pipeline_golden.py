@@ -61,7 +61,7 @@ def test_speaker_count_reconstruct_and_annotation_match_reference(ref):
         np.testing.assert_allclose([disc.sw.start, disc.sw.duration, disc.sw.step], ref[f"rec_{name}_sw"], atol=1e-15)
         # The reference picks the `count` most active clusters with numpy's DEFAULT argsort, whose order of equal
         # activations depends on the numpy build (x86-simd-sort on AVX-512 / AVX2 is not stable); the oracle fixes it
-        # as "descending activation, then ascending cluster index" (SURVEY.md appendix A).  So: identical wherever the
+        # as "descending activation, then ascending cluster index".  So: identical wherever the
         # choice is unique, and on every other frame both picked the same NUMBER of clusters with the same activations.
         act = P.aggregate(P.clustered_segmentations(P.SWF(binar.copy(), CHUNKS), hard), c.sw, hamming=False,
                           missing=0.0, skip_average=True).data[: len(want)]
