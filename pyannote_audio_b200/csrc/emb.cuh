@@ -14,11 +14,13 @@ struct ConvParams {
   int B, H_in, W_in, C_in;
   int H_out, W_out, C_out;
   int taps_h, taps_w, stride, pad;
-  int Ck, kblocks, tiles_w, num_tiles, relu;
+  int Ck, tiles_w, num_tiles, relu;
   const float* bias;
   const __half* residual;
   __half* out;
-  uint32_t a_bytes, b_bytes, nstages, swizzle;
+  // tensor-core plan: a stage = a box of a_rows pixels x Ck channels (a_tx bytes, padded to a_bytes) + the weights of
+  // one or three taps x C_out x Ck (b_bytes)
+  uint32_t a_rows, a_tx, a_bytes, b_bytes, nstages, swizzle;
 };
 
 struct BlockWeights {

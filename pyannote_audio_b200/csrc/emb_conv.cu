@@ -4,15 +4,23 @@
 //   BasicBlock.forward :140-145 (conv3x3-BN-ReLU-conv3x3-BN + shortcut -> ReLU), ResNet.forward :413-419.
 // Eval-mode BatchNorm is folded into the conv weights / a per-channel bias on the host (api.cu make_conv).
 //
-// conv_wg_kernel: implicit-GEMM convolution on the Hopper tensor cores (wgmma).
-//   GEMM view  D[M=128 output pixels of one image row][N=C_out] += A[M][K] * B[N][K]^T,
-//   K = taps * C_in walked tap by tap in chunks of Ck channels.  Activations are NHWC fp16 so that one
-//   TMA box (Ck channels x 128 consecutive pixels) lands in shared memory as a K-major, hardware-swizzled
-//   A tile; convolution padding is TMA out-of-bounds zero fill, stride-2 is the tensor map's element stride.
-//   Weights [tap][C_out][C_in] land the same way as the K-major B tile.
-//   Roles: warp 8 = TMA producer over a ring of mbarrier-guarded stages; warpgroups 0 / 1 = output pixels
-//   [0, 64) / [64, 128) of the tile, fp32 accumulators in registers, epilogue (+bias (+residual) -> ReLU -> fp16
-//   NHWC store) straight from the accumulator fragments.  One CTA per tile.
+// conv_tc_kernel: implicit-GEMM convolution on the Hopper tensor cores (wgmma).
+//   GEMM view  D[M=128 output pixels of one image row][N=C_out] += A[M][K] * B[N][K]^T,  K = taps * C_in walked tap by
+//   tap in chunks of Ck channels.  Activations are NHWC fp16 so that one TMA box (Ck channels x consecutive pixels)
+//   lands in shared memory as a K-major, hardware-swizzled A tile; convolution padding is TMA out-of-bounds zero fill,
+//   stride 2 is the tensor map's element stride.  Weights [tap][C_out][C_in] land the same way as K-major B tiles.
+//   A stage of the mbarrier ring, filled by a TMA producer warp (warp 8), holds the operands of AW taps:
+//   AW = 3 (stride-1 3x3 convs, one channel chunk, C_out <= 64: layers 1 and 2, 13 of the 35): one box of 128 + 8 pixels
+//     and the kh row's three weight taps.  Tap kw reads the box from pixel row kw on, so neighbouring taps do not fetch
+//     the same pixels again, and a stage covers three taps.
+//   AW = 1 (everything else): one 128-pixel box and one weight tap.
+//   Either way the K walk is (tap, chunk), so every output sums its products in the same order.  With several chunks
+//   (layers 3 and 4) a three-tap stage would change that order to (kh, chunk, kw) and with it the last bits.
+//   The A operand comes straight from shared memory, the descriptor start moved by kw rows of 128 B, except for
+//   Ck = 32 with AW = 3 (64-B rows: layer 1): those fragments are read with ldmatrix, the 64-B swizzle applied in
+//   software, and issued as register-A wgmma.
+//   Warpgroups 0 / 1 = output pixels [0, 64) / [64, 128) of the tile, fp32 accumulators in registers, epilogue
+//   (+bias (+residual) -> ReLU -> fp16 NHWC store) straight from the accumulator fragments.  One CTA per tile.
 #include "common.cuh"
 #include "emb.cuh"
 #include "tc_common.cuh"
@@ -21,10 +29,12 @@ namespace b200 {
 
 constexpr int kWgThreads = 288;
 constexpr int kTileM = 128;
+constexpr int kRowHalo = 8;                                 // 128 + 2 pixels needed for three taps, 8 keeps 8-row groups
 
-template <int N, int CK>
+template <int N, int CK, int AW>
 __global__ void __launch_bounds__(kWgThreads, N == 256 ? 1 : 2)
-conv_wg_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB, ConvParams p) {
+conv_tc_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB, ConvParams p) {
+  constexpr bool kRegA = AW == 3 && CK == 32;
   extern __shared__ uint8_t smem_raw[];
   const uint32_t raw = smem_u32(smem_raw);
   const uint32_t base = (raw + 1023u) & ~1023u;            // swizzle-128B operands need 1024 B alignment
@@ -34,7 +44,8 @@ conv_wg_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ 
   const int warp = threadIdx.x >> 5;
   const int wt = blockIdx.x % p.tiles_w;
   const int bh = blockIdx.x / p.tiles_w;                    // = b * H_out + h
-  const int cchunks = p.C_in / p.Ck;
+  const int cchunks = p.C_in / CK;
+  const int kw_steps = p.taps_w / AW;
 
   if (threadIdx.x == 0) {
     for (uint32_t s = 0; s < p.nstages; ++s) { mbar_init(bar_full + 8 * s, 1); mbar_init(bar_empty + 8 * s, 2); }
@@ -49,42 +60,68 @@ conv_wg_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ 
       const int h = bh % p.H_out, b = bh / p.H_out;
       const int w_base = wt * kTileM * p.stride - p.pad, h_base = h * p.stride - p.pad;
       uint32_t stage = 0, phase = 0;
-      int tap = 0, cc = 0, kh = 0, kw = 0;
-      for (int kb = 0; kb < p.kblocks; ++kb) {
-        mbar_wait(bar_empty + 8 * stage, phase ^ 1);
-        mbar_expect_tx(bar_full + 8 * stage, stage_bytes);
-        const uint32_t sa = stage0 + stage * stage_bytes;
-        tma_load_4d(&tmA, bar_full + 8 * stage, sa, cc * p.Ck, w_base + kw, h_base + kh, b);
-        tma_load_3d(&tmB, bar_full + 8 * stage, sa + p.a_bytes, cc * p.Ck, 0, tap);
-        if (++stage == p.nstages) { stage = 0; phase ^= 1; }
-        if (++cc == cchunks) { cc = 0; ++tap; if (++kw == p.taps_w) { kw = 0; ++kh; } }
-      }
+      for (int kh = 0; kh < p.taps_h; ++kh)
+        for (int kw = 0; kw < p.taps_w; kw += AW)
+          for (int cc = 0; cc < cchunks; ++cc) {
+            mbar_wait(bar_empty + 8 * stage, phase ^ 1);
+            mbar_expect_tx(bar_full + 8 * stage, p.a_tx + p.b_bytes);
+            const uint32_t sa = stage0 + stage * stage_bytes;
+            tma_load_4d(&tmA, bar_full + 8 * stage, sa, cc * CK, w_base + kw, h_base + kh, b);
+            tma_load_3d(&tmB, bar_full + 8 * stage, sa + p.a_bytes, cc * CK, 0, kh * p.taps_w + kw);
+            if (++stage == p.nstages) { stage = 0; phase ^= 1; }
+          }
     }
     return;
   }
 
   const int wg = warp >> 2;
+  const int lane = threadIdx.x & 31;
   constexpr uint32_t row_bytes = CK * 2;                   // = the swizzle width (64 or 128 B)
+  constexpr uint32_t b_tap_bytes = N * row_bytes;
   float acc[N / 2];
 #pragma unroll
   for (int i = 0; i < N / 2; ++i) acc[i] = 0.f;
+  const int kblocks = p.taps_h * kw_steps * cchunks;
   uint32_t stage = 0, phase = 0, prev = 0;
-  for (int kb = 0; kb < p.kblocks; ++kb) {
+  for (int kb = 0; kb < kblocks; ++kb) {
     mbar_wait(bar_full + 8 * stage, phase);
-    const uint32_t sa = stage0 + stage * stage_bytes;
-    const uint64_t ad = wg_desc(sa + (uint32_t)wg * 64u * row_bytes, row_bytes), bd = wg_desc(sa + p.a_bytes, row_bytes);
+    const uint32_t st = stage0 + stage * stage_bytes;
+    const uint32_t sa = st + (uint32_t)wg * 64u * row_bytes, sb = st + p.a_bytes;
+    uint32_t af[AW][CK / 16][4];
+    if constexpr (kRegA) {
+      // pixel row r of this warp's 16 (lanes 0-15 / 16-31: K columns 0-7 / 8-15 of each step) at 64-B rows, 16-B
+      // chunk c stored at chunk c ^ ((row >> 1) & 3) (64-B swizzle; a_bytes keeps stages 1024-B aligned)
+#pragma unroll
+      for (int t = 0; t < AW; ++t)
+#pragma unroll
+        for (int k = 0; k < CK / 16; ++k) {
+          const uint32_t row = (uint32_t)(wg * 64 + (warp & 3) * 16 + (lane & 15) + t);
+          const uint32_t chunk = (uint32_t)(2 * k + (lane >> 4)) ^ ((row >> 1) & 3u);
+          ldsm_x4(af[t][k], st + row * row_bytes + chunk * 16u);
+        }
+    }
     wg_fence();
 #pragma unroll
-    for (int k = 0; k < CK / 16; ++k) Wgmma<N>::mma(acc, ad + 2 * k, bd + 2 * k);   // +32 B per K=16 step
+    for (int t = 0; t < AW; ++t) {
+      const uint64_t bd = wg_desc(sb + t * b_tap_bytes, row_bytes);
+      if constexpr (kRegA) {
+#pragma unroll
+        for (int k = 0; k < CK / 16; ++k) WgmmaRS<N>::mma(acc, af[t][k], bd + 2 * k);
+      } else {
+        const uint64_t ad = wg_desc(sa + t * row_bytes, row_bytes);
+#pragma unroll
+        for (int k = 0; k < CK / 16; ++k) Wgmma<N>::mma(acc, ad + 2 * k, bd + 2 * k);   // +32 B per K=16 step
+      }
+    }
     wg_commit();
-    wg_wait<1>();                                           // the previous stage's wgmma have read their operands
+    if constexpr (kRegA) wg_wait<0>();                     // the fragments are rewritten by the next ldmatrix
+    else wg_wait<1>();                                      // the previous stage's wgmma have read their operands
     if (kb > 0 && (threadIdx.x & 127) == 0) mbar_arrive(bar_empty + 8 * prev);
     prev = stage;
     if (++stage == p.nstages) { stage = 0; phase ^= 1; }
   }
   wg_wait<0>();
 
-  const int lane = threadIdx.x & 31;
   const int c0 = 2 * (lane & 3);
 #pragma unroll
   for (int i = 0; i < 2; ++i) {
@@ -272,12 +309,10 @@ int conv_forward(const ConvLayer& L, const __half* in, const __half* residual, _
   p.relu = relu; p.bias = L.bias; p.residual = residual; p.out = out;
   p.Ck = (L.C_in >= 64) ? 64 : 32;
   p.swizzle = (p.Ck == 64) ? 128 : 64;
-  p.kblocks = L.ksize * L.ksize * (L.C_in / p.Ck);
   p.tiles_w = ceil_div(p.W_out, kTileM);
   p.num_tiles = B * p.H_out * p.tiles_w;
-  p.a_bytes = kTileM * p.Ck * 2;
-  p.b_bytes = L.C_out * p.Ck * 2;
-  B200_CHECK(L.C_in % p.Ck == 0 && (L.C_out == 64 || L.C_out == 128 || L.C_out == 256 || (L.C_out == 32 && p.Ck == 32)),
+  B200_CHECK(L.C_in % p.Ck == 0 && (L.C_out == 64 || (L.C_out >= 128 && L.C_out <= 256 && L.C_out % 128 == 0 && p.Ck == 64) ||
+                                    (L.C_out == 32 && p.Ck == 32)),
              B200_ERR_STATE, "conv %d -> %d channels unsupported", L.C_in, L.C_out);
   B200_CHECK(impl == 0 || impl == 1, B200_ERR_INVALID, "conv_impl %d unknown (0 = CUDA cores, 1 = tensor cores)", impl);
 
@@ -288,11 +323,21 @@ int conv_forward(const ConvLayer& L, const __half* in, const __half* residual, _
     return B200_OK;
   }
 
+  // stride-1 3x3 convs with one channel chunk stage three taps at a time on one box of 128 + 8 pixels (AW = 3); from
+  // C_out = 128 on three weight taps would leave room for a single stage
+  const int AW = (L.ksize == 3 && L.stride == 1 && L.C_in == p.Ck && L.C_out <= 64) ? 3 : 1;
+  p.a_rows = AW == 3 ? kTileM + kRowHalo : kTileM;
+  p.a_tx = p.a_rows * p.Ck * 2;
+  p.a_bytes = (p.a_tx + 1023u) & ~1023u;
+  p.b_bytes = (uint32_t)(AW * L.C_out * p.Ck * 2);
   // C_out = 256 needs 128 accumulator registers per thread: one CTA per SM with 4 deep stages; the narrower layers
   // run two CTAs per SM (registers allow it) on half the shared memory each
   const uint32_t budget = L.C_out == 256 ? 200u * 1024 : 100u * 1024;
   p.nstages = budget / (p.a_bytes + p.b_bytes);
   if (p.nstages > 8) p.nstages = 8;
+  // a C_out = 32 tile has only three stages of work; a deeper ring would only keep other CTAs off the SM
+  if (AW == 3 && p.nstages > 3) p.nstages = 3;
+  B200_CHECK(p.nstages >= 2, B200_ERR_STATE, "conv %d -> %d: shared memory plan too shallow", L.C_in, L.C_out);
   PFN_encodeTiled enc = get_encode();
   B200_CHECK(enc != nullptr, B200_ERR_CUDA, "cuTensorMapEncodeTiled not available from the driver");
   CUtensorMap tmA, tmB;
@@ -300,7 +345,7 @@ int conv_forward(const ConvLayer& L, const __half* in, const __half* residual, _
     cuuint64_t dims[4] = {(cuuint64_t)L.C_in, (cuuint64_t)W_in, (cuuint64_t)H_in, (cuuint64_t)B};
     cuuint64_t strides[3] = {(cuuint64_t)L.C_in * 2, (cuuint64_t)W_in * L.C_in * 2,
                              (cuuint64_t)H_in * W_in * L.C_in * 2};
-    cuuint32_t box[4] = {(cuuint32_t)p.Ck, (cuuint32_t)(kTileM * L.stride), 1, 1};
+    cuuint32_t box[4] = {(cuuint32_t)p.Ck, (cuuint32_t)(p.a_rows * L.stride), 1, 1};
     cuuint32_t estr[4] = {1, (cuuint32_t)L.stride, 1, 1};
     CUresult r = enc(&tmA, CU_TENSOR_MAP_DATA_TYPE_FLOAT16, 4, const_cast<__half*>(in), dims, strides, box, estr,
                      CU_TENSOR_MAP_INTERLEAVE_NONE,
@@ -311,7 +356,7 @@ int conv_forward(const ConvLayer& L, const __half* in, const __half* residual, _
   {
     cuuint64_t dims[3] = {(cuuint64_t)L.C_in, (cuuint64_t)L.C_out, (cuuint64_t)(L.ksize * L.ksize)};
     cuuint64_t strides[2] = {(cuuint64_t)L.C_in * 2, (cuuint64_t)L.C_out * L.C_in * 2};
-    cuuint32_t box[3] = {(cuuint32_t)p.Ck, (cuuint32_t)L.C_out, 1};
+    cuuint32_t box[3] = {(cuuint32_t)p.Ck, (cuuint32_t)L.C_out, (cuuint32_t)AW};
     cuuint32_t estr[3] = {1, 1, 1};
     CUresult r = enc(&tmB, CU_TENSOR_MAP_DATA_TYPE_FLOAT16, 3, const_cast<__half*>(L.w), dims, strides, box, estr,
                      CU_TENSOR_MAP_INTERLEAVE_NONE,
@@ -326,11 +371,15 @@ int conv_forward(const ConvLayer& L, const __half* in, const __half* residual, _
     B200_CUDA_OK(cudaGetLastError());
     return B200_OK;
   };
-  if (p.Ck == 32) return L.C_out == 32 ? launch(conv_wg_kernel<32, 32>) : launch(conv_wg_kernel<64, 32>);
+  if (AW == 3) {
+    if (p.Ck == 32) return L.C_out == 32 ? launch(conv_tc_kernel<32, 32, 3>) : launch(conv_tc_kernel<64, 32, 3>);
+    return launch(conv_tc_kernel<64, 64, 3>);
+  }
+  if (p.Ck == 32) return L.C_out == 32 ? launch(conv_tc_kernel<32, 32, 1>) : launch(conv_tc_kernel<64, 32, 1>);
   switch (L.C_out) {
-    case 64: return launch(conv_wg_kernel<64, 64>);
-    case 128: return launch(conv_wg_kernel<128, 64>);
-    default: return launch(conv_wg_kernel<256, 64>);
+    case 64: return launch(conv_tc_kernel<64, 64, 1>);
+    case 128: return launch(conv_tc_kernel<128, 64, 1>);
+    default: return launch(conv_tc_kernel<256, 64, 1>);
   }
 }
 

@@ -56,10 +56,19 @@ __device__ __forceinline__ void prefetch_tensormap(const CUtensorMap* tm) {
 // wgmma shared-memory descriptor of a K-major operand tile written by TMA with hardware swizzle (8-row core groups
 // `sbo_bytes` apart):  [0,14) start >> 4 | [16,30) LBO >> 4 (unused for swizzled K-major, 1) | [32,46) SBO >> 4 |
 // [62,64) layout (1 = 128B, 2 = 64B swizzle).  A K step of 16 fp16 inside the swizzle row adds 32 B to the start.
+// The swizzle follows the shared-memory address bits, so a tile may also start whole rows into a staged box (the trunk
+// convs' kw shift) with the base offset [49,52) left at 0; setting it to (start >> 7) & 7 gives wrong products.
 __device__ __forceinline__ uint64_t wg_desc(uint32_t saddr, uint32_t swizzle_bytes) {
   const uint64_t layout = swizzle_bytes == 128 ? 1u : 2u;
   return (uint64_t)((saddr & 0x3FFFFu) >> 4) | ((uint64_t)1 << 16) | ((uint64_t)((8u * swizzle_bytes) >> 4) << 32) |
          (layout << 62);
+}
+// ldmatrix x4: lanes 8i .. 8i + 7 address the rows of 8 x 8 fp16 matrix i, which lands in r[i]
+__device__ __forceinline__ void ldsm_x4(uint32_t* r, uint32_t saddr) {
+  asm volatile("ldmatrix.sync.aligned.m8n8.x4.shared.b16 {%0, %1, %2, %3}, [%4];"
+               : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3])
+               : "r"(saddr)
+               : "memory");
 }
 __device__ __forceinline__ void wg_fence() { asm volatile("wgmma.fence.sync.aligned;" ::: "memory"); }
 __device__ __forceinline__ void wg_commit() { asm volatile("wgmma.commit_group.sync.aligned;" ::: "memory"); }
@@ -117,6 +126,16 @@ struct Wgmma<256> {
 template <int N>
 struct WgmmaRS;
 template <>
+struct WgmmaRS<32> {
+  __device__ __forceinline__ static void mma(float* d, const uint32_t* a, uint64_t b) {
+    asm volatile(
+        "wgmma.mma_async.sync.aligned.m64n32k16.f32.f16.f16 "
+        "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15}, {%16, %17, %18, %19}, %20, 1, 1, 1, 0;"
+        : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15])
+        : "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "l"(b));
+  }
+};
+template <>
 struct WgmmaRS<64> {
   __device__ __forceinline__ static void mma(float* d, const uint32_t* a, uint64_t b) {
     asm volatile(
@@ -136,7 +155,6 @@ struct WgmmaRS<80> {
         : "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "l"(b));
   }
 };
-
 template <>
 struct WgmmaRS<256> {
   __device__ __forceinline__ static void mma(float* d, const uint32_t* a, uint64_t b) {

@@ -1,0 +1,165 @@
+"""Per-conv profile of the ResNet34 trunk: time, TFLOP/s, operand fill and unique HBM traffic of each trunk conv.
+
+    python scripts/trunk_profile.py                  # the library in this tree (needs a GPU)
+    python scripts/trunk_profile.py --root OTHER --plan per-tap   # another tree's build, with its launch plan
+    python scripts/trunk_profile.py --model-only     # the byte model alone (no GPU)
+
+`ctx.emb_trunk` runs on --batch segments (the library's embedding sub-batch) under torch.profiler with CUDA
+activities, after warm-up.  The trunk convs are the kernel launches between the stem (`conv1_kernel`) and
+`frames_to_nchw`, in the order of trunk_convs() below.
+
+Byte model, per segment (computed from the shapes, not measured):
+  fill  = bytes TMA moves from L2 into shared memory for the operands, for the launch plan of conv_forward:
+          per-tap : every (tap, channel chunk) stages a 128-pixel activation box and one weight tile
+          reuse   : stride-1 3x3 convs with one channel chunk and C_out <= 64 (layers 1 and 2) stage one 136-pixel
+                    activation box per kh for the three kw taps, and every weight tile; the other convs stay per-tap
+  HBM   = input + output (+ residual) activations once, and the weights once per launch shared by --batch segments
+"""
+import argparse
+import os
+import subprocess
+import sys
+
+TILE_M = 128
+HALO = 8
+
+
+def trunk_convs():
+    """(layer, name, C_in, C_out, ksize, stride, H_in, W_in, has_residual) of the 35 trunk convs in launch order."""
+    convs = []
+    H, W, C = 80, 998, 32
+    for li, (cout, blocks, stride) in enumerate(((32, 3, 1), (64, 4, 2), (128, 6, 2), (256, 3, 2)), start=1):
+        for bi in range(blocks):
+            s = stride if bi == 0 else 1
+            Ho, Wo = (H + 2 - 3) // s + 1, (W + 2 - 3) // s + 1
+            convs.append((li, f"layer{li}.{bi}.conv1", C, cout, 3, s, H, W, False))
+            if s != 1 or C != cout:
+                convs.append((li, f"layer{li}.{bi}.shortcut", C, cout, 1, s, H, W, False))
+            convs.append((li, f"layer{li}.{bi}.conv2", cout, cout, 3, 1, Ho, Wo, True))
+            H, W, C = Ho, Wo, cout
+    return convs
+
+
+def conv_model(c, plan, batch):
+    """(GFLOP, fill MB, unique HBM MB) per segment of one conv."""
+    _, _, cin, cout, k, s, H, W, res = c
+    pad = k // 2
+    Ho, Wo = (H + 2 * pad - k) // s + 1, (W + 2 * pad - k) // s + 1
+    ck = 64 if cin >= 64 else 32
+    chunks = cin // ck
+    tiles = Ho * -(-Wo // TILE_M)
+    b_tile = cout * ck * 2
+    reuse = plan == "reuse" and k == 3 and s == 1 and cin == ck and cout <= 64
+    if reuse:
+        fill = tiles * (k * chunks * (TILE_M + HALO) * ck * 2 + k * k * chunks * b_tile)
+    else:
+        fill = tiles * k * k * chunks * (TILE_M * ck * 2 + b_tile)
+    act_out = Ho * Wo * cout * 2
+    hbm = H * W * cin * 2 + act_out * (2 if res else 1) + k * k * cin * cout * 2 / batch
+    return 2.0 * Ho * Wo * cout * cin * k * k / 1e9, fill / 1e6, hbm / 1e6
+
+
+def print_model(plan, batch):
+    rows = [(c, *conv_model(c, plan, batch)) for c in trunk_convs()]
+    print(f"byte model ({plan} plan), per segment:")
+    print(f"{'layer':>6} {'convs':>5} {'GFLOP':>7} {'fill MB':>8} {'HBM MB':>7} {'FLOP/fill B':>11} {'FLOP/HBM B':>10}")
+    tot = [0, 0.0, 0.0, 0.0]
+    for li in (1, 2, 3, 4):
+        sel = [r for r in rows if r[0][0] == li]
+        g, f, h = (sum(r[i] for r in sel) for i in (1, 2, 3))
+        tot = [tot[0] + len(sel), tot[1] + g, tot[2] + f, tot[3] + h]
+        print(f"{li:>6} {len(sel):>5} {g:7.2f} {f:8.1f} {h:7.1f} {g * 1e3 / f:11.0f} {g * 1e3 / h:10.0f}")
+    print(f"{'total':>6} {tot[0]:>5} {tot[1]:7.2f} {tot[2]:8.1f} {tot[3]:7.1f} {tot[1] * 1e3 / tot[2]:11.0f} "
+          f"{tot[1] * 1e3 / tot[3]:10.0f}")
+    return rows
+
+
+def gpu_info():
+    try:
+        out = subprocess.run(["nvidia-smi", "--query-gpu=name,power.limit,clocks.sm,clocks.max.sm",
+                              "--format=csv,noheader", "-i", "0"], capture_output=True, text=True, timeout=30).stdout
+        return out.strip()
+    except (OSError, subprocess.SubprocessError) as e:
+        return f"nvidia-smi unavailable ({e})"
+
+
+def main():
+    ap = argparse.ArgumentParser(description=__doc__, formatter_class=argparse.RawDescriptionHelpFormatter)
+    ap.add_argument("--root", default=os.path.dirname(os.path.dirname(os.path.abspath(__file__))),
+                    help="tree whose built library is timed (default: this one)")
+    ap.add_argument("--plan", choices=["reuse", "per-tap"], default="reuse",
+                    help="launch plan of the timed library for the byte model (per-tap: a library whose trunk convs "
+                         "stage one activation box per tap)")
+    ap.add_argument("--batch", type=int, default=264, help="segments per emb_trunk call (library sub-batch: 264)")
+    ap.add_argument("--iters", type=int, default=5, help="profiled emb_trunk calls")
+    ap.add_argument("--model-only", action="store_true", help="print the byte model and exit (no GPU needed)")
+    args = ap.parse_args()
+
+    rows = print_model(args.plan, args.batch)
+    if args.model_only:
+        return
+
+    sys.path.insert(0, os.path.abspath(args.root))
+    import torch
+    from torch.profiler import ProfilerActivity, profile
+
+    from pyannote_audio_b200 import ops, synthetic as syn
+
+    if not torch.cuda.is_available():
+        raise SystemExit("no CUDA device: only --model-only runs without a GPU")
+    dev = torch.device("cuda:0")
+    ctx = ops.Context(dev)
+    ctx.load_embedding(syn.make_embedding_state_dict(1))
+    g = torch.Generator().manual_seed(0)
+    fb = (torch.randn((args.batch, 998, 80), generator=g) * 2.0).to(dev)
+    for _ in range(3):
+        ctx.emb_trunk(fb)
+    torch.cuda.synchronize()
+    with profile(activities=[ProfilerActivity.CUDA]) as prof:
+        for _ in range(args.iters):
+            ctx.emb_trunk(fb)
+        torch.cuda.synchronize()
+    info = gpu_info()
+
+    evs = sorted((e for e in prof.events() if e.device_type == torch.autograd.DeviceType.CUDA),
+                 key=lambda e: e.time_range.start)
+    runs, cur = [], None
+    for e in evs:
+        if "conv1_kernel" in e.name:
+            cur = []
+        elif "frames_to_nchw" in e.name:
+            if cur is not None:
+                runs.append(cur)
+            cur = None
+        elif cur is not None and "conv" in e.name:
+            cur.append(e.time_range.end - e.time_range.start)        # us
+    n = len(rows)
+    runs = [r for r in runs if len(r) == n]
+    if not runs:
+        raise SystemExit(f"found no emb_trunk call with {n} conv launches between conv1_kernel and frames_to_nchw")
+    us = [sum(r[i] for r in runs) / len(runs) for i in range(n)]
+
+    print(f"\nGPU: {info}   (name, power limit, SM clock now, max SM clock)")
+    print(f"root {os.path.abspath(args.root)}, {args.batch} segments per call, mean of {len(runs)} calls\n")
+    print(f"{'conv':<20} {'Cin>Cout':>9} {'k/s':>4} {'HxW in':>8} {'us':>8} {'TFLOP/s':>8} {'fill GB/s':>9} {'HBM GB/s':>9}")
+    tot_us = 0.0
+    per_layer = {}
+    for (c, gf, fmb, hmb), t in zip(rows, us):
+        _, name, cin, cout, k, s, H, W, _ = c
+        sec = t * 1e-6
+        tot_us += t
+        L = per_layer.setdefault(c[0], [0.0, 0.0, 0.0, 0.0])
+        L[0] += t; L[1] += gf; L[2] += fmb; L[3] += hmb
+        print(f"{name:<20} {f'{cin}>{cout}':>9} {f'{k}/{s}':>4} {f'{H}x{W}':>8} {t:8.1f} "
+              f"{gf * args.batch / sec / 1e3:8.1f} {fmb * args.batch / sec / 1e3:9.0f} {hmb * args.batch / sec / 1e3:9.0f}")
+    print()
+    for li, (t, gf, fmb, hmb) in sorted(per_layer.items()):
+        sec = t * 1e-6
+        print(f"layer{li}: {t / 1e3:7.3f} ms  {gf * args.batch / sec / 1e3:6.1f} TFLOP/s  "
+              f"fill {fmb * args.batch / sec / 1e3:6.0f} GB/s  HBM {hmb * args.batch / sec / 1e3:6.0f} GB/s")
+    print(f"trunk convs: {tot_us / 1e3:.3f} ms per call of {args.batch} segments "
+          f"({tot_us / args.batch:.1f} us per segment)")
+
+
+if __name__ == "__main__":
+    main()
