@@ -161,6 +161,21 @@ int64_t b200_emb_fbank_plan(const int64_t* chunk_off, const int32_t* chunk_valid
                             int32_t share, int32_t* frame0, int32_t* rows_per_sub_batch);
 /* ResNet.forward_frames on a given fbank (resnet.py:399-419): frames[num_chunks][256][10][125] fp32 (NCHW). */
 int b200_emb_trunk(b200_ctx* ctx, const float* fbank, int32_t num_chunks, float* frames, void* stream);
+/* WeSpeakerResNet34.forward (models/embedding/wespeaker/__init__.py:324-343) on utterances of one length
+ * num_samples >= 400 (a (num_utts, 1, num_samples) tensor): utterance i = wav[off[i] .. off[i] + num_samples), off a
+ * HOST array.  compute_fbank (:113-139) gives T0 = 1 + (num_samples - 400) / 160 frames, the trunk
+ * (resnet.py:347-368) T = T0 after layer 1 and (T + 2 - 3) / 2 + 1 after each of layers 2-4; StatsPool
+ * (models/blocks/pooling.py:30-61, 76-130) weights are interpolated onto the T frames with torch's CUDA nearest index.
+ * weights: NULL (mean and std(correction=1) over the T frames; T = 1 gives NaN) or fp32 DEVICE
+ * [num_utts][num_speakers][num_weights], any real values.  emb: fp32 DEVICE [num_utts][max(num_speakers, 1)][256].
+ * Utterances run in sub-batches of max(1, emb_max_batch * 998 / T0); one utterance longer than emb_max_batch * 998
+ * fbank frames (263 472 = 43.9 min with the default) returns B200_STATUS_INVALID. */
+int b200_emb_forward_utt(b200_ctx* ctx, const float* wav, const int64_t* off, int64_t num_samples, int32_t num_utts,
+                         const float* weights, int32_t num_speakers, int32_t num_weights, float* emb, void* stream);
+/* ResNet.forward_embedding on caller frames (resnet.py:370-397, wespeaker/__init__.py:304-322): frames fp32 DEVICE
+ * NCHW [B][256][10][T] (what forward_frames returns), weights and emb as in b200_emb_forward_utt. */
+int b200_emb_forward_embedding(b200_ctx* ctx, const float* frames, int32_t B, int32_t T, const float* weights,
+                               int32_t num_speakers, int32_t num_weights, float* emb, void* stream);
 /* StatsPool.forward (models/blocks/pooling.py:76-130): seq[B][F][T], weights[B][S][Tw] or NULL -> out[B][S][2F]. */
 int b200_stats_pool(b200_ctx* ctx, const float* seq, const float* weights, float* out, int32_t B, int32_t F, int32_t T,
                     int32_t S, int32_t Tw, void* stream);

@@ -1,7 +1,8 @@
 """pyannote_audio_b200 -- H100-native (sm_90a) implementation of pyannote.audio's community-1 diarization hot path.
 
 Public surface mirrors the reference for this path only:
-  Inference, Model classes (PyanNet, WeSpeakerResNet34), SpeakerDiarization (+ DiarizeOutput), VBxClustering,
+  Inference, Model classes (PyanNet, WeSpeakerResNet34), SpeakerDiarization (+ DiarizeOutput), SpeakerEmbedding,
+  VoiceActivityDetection, VBxClustering,
   AgglomerativeClustering, PLDA, Audio, and the pyannote.core value types they exchange.
 All compute goes through libb200diar.so (C ABI in include/b200diar.h); there is no CPU fallback.
 """
@@ -15,7 +16,7 @@ _LAZY = {
     "WeSpeakerResNet34": "models", "SpeakerDiarization": "pipeline", "DiarizeOutput": "pipeline",
     "PretrainedSpeakerEmbedding": "pipeline", "VBxClustering": "clustering",
     "AgglomerativeClustering": "clustering", "PLDA": "clustering", "VoiceActivityDetection": "vad",
-    "Binarize": "signal", "Pipeline": "loading",
+    "Binarize": "signal", "Pipeline": "loading", "SpeakerEmbedding": "speaker_verification",
 }
 
 

@@ -699,24 +699,27 @@ static int block_run(b200_ctx* ctx, const BlockWeights& B, __half* A, __half* Bf
   return B200_OK;
 }
 
-// conv1 + 16 BasicBlocks; returns the buffer holding the result (NHWC fp16 [nb][10][125][256])
-static int trunk_run(b200_ctx* ctx, const EmbWs& w, const int* frame0, int nb, cudaStream_t st,
-                     const __half** result) {
+// conv1 + 16 BasicBlocks on nb segments of T0 fbank frames; returns the buffer holding the result (NHWC fp16
+// [nb][10][T][256]) and its width T: T0 after layer 1, then (T + 2 - 3) / 2 + 1 after each of layers 2, 3 and 4
+// (125 for the 998 frames of 10 s)
+static int trunk_run(b200_ctx* ctx, const EmbWs& w, const int* frame0, int nb, int T0, cudaStream_t st,
+                     const __half** result, int* T_out) {
   const EmbWeights& E = ctx->emb;
   int rc;
-  int H = kMel, Wd = kFbankFrames;
+  int H = kMel, Wd = T0;
   __half* cur = w.A;            // current activation; the other two buffers are scratch
   __half* s1 = w.Bf;
   __half* s2 = w.Cf;
-  if ((rc = conv1_forward(w.fbank, w.fmean, frame0, E.conv1_w, E.conv1_b, cur, nb, st))) return rc;
+  if ((rc = conv1_forward(w.fbank, w.fmean, frame0, E.conv1_w, E.conv1_b, cur, nb, T0, st))) return rc;
   ctx->launches += 1;
   for (const BlockWeights& B : E.blocks) {
     const int s = B.conv1.stride;
     if ((rc = block_run(ctx, B, cur, s1, s2, nb, H, Wd, st))) return rc;
     H = (H + 2 - 3) / s + 1; Wd = (Wd + 2 - 3) / s + 1;
   }
-  B200_CHECK(H == 10 && Wd == kEmbT, B200_ERR_STATE, "unexpected trunk output %dx%d", H, Wd);
+  B200_CHECK(H == 10 && (T0 != kFbankFrames || Wd == kEmbT), B200_ERR_STATE, "unexpected trunk output %dx%d", H, Wd);
   *result = cur;
+  *T_out = Wd;
   return B200_OK;
 }
 
@@ -771,12 +774,13 @@ static int emb_forward_impl(b200_ctx* ctx, const float* wav, const int64_t* chun
     const int nb = (num_chunks - c0) < nbmax ? (num_chunks - c0) : nbmax;
     const int sb = c0 / nbmax;
     if ((rc = fbank_forward(ctx->emb, wav, ctx->d_runs + plan.run_base[sb], plan.run_base[sb + 1] - plan.run_base[sb],
-                            plan.nrows[sb], ctx->d_frame0 + c0, nb, w.fbank, w.fmean, st)))
+                            plan.nrows[sb], ctx->d_frame0 + c0, nb, kFbankFrames, w.fbank, w.fmean, st)))
       return rc;
     ctx->launches += 2;
     {
       ScopedTimer timer(ctx, &ctx->trunk_events, st);
-      if ((rc = trunk_run(ctx, w, ctx->d_frame0 + c0, nb, st, &feat))) return rc;
+      int T = 0;
+      if ((rc = trunk_run(ctx, w, ctx->d_frame0 + c0, nb, kFbankFrames, st, &feat, &T))) return rc;
     }
     if (ctx->profile) ctx->trunk_segments += nb;
     const size_t o = (size_t)c0 * kSpeakers * 2 * kStatsDim;
@@ -806,8 +810,8 @@ int b200_emb_fbank(b200_ctx* ctx, const float* wav, const int64_t* chunk_off, co
   FbankPlan plan;                                            // output layout [B][998][80]: one private run per chunk
   if ((rc = push_fbank_plan(ctx, chunk_off, chunk_valid, num_chunks, num_chunks, false, &plan, st))) return rc;
   float* fmean = reinterpret_cast<float*>(ctx->ws);
-  if ((rc = fbank_forward(ctx->emb, wav, ctx->d_runs, num_chunks, plan.nrows[0], ctx->d_frame0, num_chunks, fbank, fmean,
-                          st)))
+  if ((rc = fbank_forward(ctx->emb, wav, ctx->d_runs, num_chunks, plan.nrows[0], ctx->d_frame0, num_chunks, kFbankFrames,
+                          fbank, fmean, st)))
     return rc;
   ctx->launches += 3;
   return fbank_center(fbank, fmean, num_chunks, st);
@@ -844,11 +848,111 @@ int b200_emb_trunk(b200_ctx* ctx, const float* fbank, int32_t num_chunks, float*
                                  (size_t)nb * kFbankFrames * kMel * sizeof(float), cudaMemcpyDeviceToDevice, st));
     B200_CUDA_OK(cudaMemsetAsync(w.fmean, 0, (size_t)nb * kMel * sizeof(float), st));
     const __half* feat = nullptr;
-    if ((rc = trunk_run(ctx, w, nullptr, nb, st, &feat))) return rc;
-    if ((rc = frames_to_nchw(feat, frames + (size_t)c0 * 256 * 10 * kEmbT, nb, st))) return rc;
+    int T = 0;
+    if ((rc = trunk_run(ctx, w, nullptr, nb, kFbankFrames, st, &feat, &T))) return rc;
+    if ((rc = frames_to_nchw(feat, frames + (size_t)c0 * 256 * 10 * kEmbT, nb, T, st))) return rc;
     ctx->launches += 1;
   }
   return B200_OK;
+}
+
+// ---- embeddings of utterances of any length ------------------------------------------------------------
+static int emb_linear(b200_ctx* ctx, const __half* st_hi, const __half* st_lo, int64_t rows, float* emb, cudaStream_t st) {
+  const int rc = gemm_tc_split(st_hi, st_lo, 2 * kStatsDim, ctx->emb.seg1_w_hi, ctx->emb.seg1_w_lo, 2 * kStatsDim, emb,
+                               kEmbDim, nullptr, nullptr, 0, ctx->emb.seg1_b, (int)rows, kEmbDim, 2 * kStatsDim, 0,
+                               ctx->num_sms, st);
+  ctx->launches += 1;
+  return rc;
+}
+
+int b200_emb_forward_utt(b200_ctx* ctx, const float* wav, const int64_t* off, int64_t num_samples, int32_t num_utts,
+                         const float* weights, int32_t num_speakers, int32_t num_weights, float* emb, void* stream) {
+  B200_CHECK(ctx && ctx->emb.loaded, B200_ERR_STATE, "embedding weights not loaded");
+  B200_CHECK(wav && off && emb && num_utts >= 0, B200_ERR_INVALID, "bad arguments");
+  B200_CHECK(num_samples >= 400, B200_ERR_INVALID,
+             "utterances of %lld samples are shorter than one 400-sample fbank frame", (long long)num_samples);
+  B200_CHECK(!weights || (num_speakers >= 1 && num_weights >= 1), B200_ERR_INVALID,
+             "weights need num_speakers >= 1 and num_weights >= 1 (got %d, %d)", (int)num_speakers, (int)num_weights);
+  if (num_utts == 0) return B200_OK;
+  for (int i = 0; i < num_utts; ++i)
+    B200_CHECK(off[i] >= 0, B200_ERR_INVALID, "utterance %d: negative offset %lld", i, (long long)off[i]);
+  // a sub-batch holds at most emb_max_batch x 998 fbank frames: the workspace of emb_max_batch 10 s chunks
+  const int64_t T0l = 1 + (num_samples - 400) / 160;
+  const int64_t budget = (int64_t)ctx->emb_max_batch * kFbankFrames;
+  B200_CHECK(T0l <= budget, B200_ERR_INVALID,
+             "an utterance of %lld samples has %lld fbank frames, more than the %lld frames of one embedding sub-batch "
+             "(emb_max_batch %d x 998): set the option emb_max_batch to at least %lld, or embed shorter excerpts",
+             (long long)num_samples, (long long)T0l, (long long)budget, ctx->emb_max_batch,
+             (long long)((T0l + kFbankFrames - 1) / kFbankFrames));
+  DeviceGuard g(ctx->device);
+  cudaStream_t st = (cudaStream_t)stream;
+  const int T0 = (int)T0l;
+  const int S = weights ? num_speakers : 1;
+  const int nbu = (int)std::min<int64_t>(num_utts, std::max<int64_t>(1, budget / T0));   // utterances per sub-batch
+  const int nbc = (int)(((int64_t)nbu * T0 + kFbankFrames - 1) / kFbankFrames);          // the same bytes in chunks
+  int T = T0;                                                                            // trunk output width
+  for (int l = 0; l < 3; ++l) T = (T + 2 - 3) / 2 + 1;
+  const size_t rows = (size_t)num_utts * S;
+  const size_t split_bytes = align_up(rows * 2 * kStatsDim * sizeof(__half), 1024);
+  const size_t sub_bytes = carve_emb(nbc, nullptr, nullptr);
+  // fmean ([nbu][80] fp32) lives in the Bf scratch until the first block, the pooling partials in Cf after the
+  // trunk: both fit since nbu * T0 <= nbc * 998 frames and Bf / Cf hold nbc * 998 * 80 * 32 fp16
+  const size_t act_bytes = (size_t)nbc * kMel * kFbankFrames * 32 * sizeof(__half);
+  const size_t part_bytes = pool_scratch_bytes(nbu, S, T);
+  B200_CHECK(part_bytes <= act_bytes, B200_ERR_INVALID,
+             "%d speakers x %d frames: pooling scratch exceeds the sub-batch workspace", S, T);
+  int rc = ensure_ws(ctx, sub_bytes + 2 * split_bytes + 4096);
+  if (rc) return rc;
+  if ((rc = ensure_meta(ctx, num_utts))) return rc;
+  std::vector<b200::FbankRun> runs((size_t)num_utts);                                    // one private run each
+  for (int i = 0; i < num_utts; ++i) runs[i] = b200::FbankRun{(long long)off[i], (i % nbu) * T0, (int)num_samples};
+  B200_CUDA_OK(cudaMemcpyAsync(ctx->d_runs, runs.data(), sizeof(b200::FbankRun) * runs.size(), cudaMemcpyHostToDevice, st));
+  EmbWs w;
+  carve_emb(nbc, ctx->ws, &w);
+  w.fmean = reinterpret_cast<float*>(w.Bf);
+  double* part = reinterpret_cast<double*>(w.Cf);
+  __half* st_hi = reinterpret_cast<__half*>(reinterpret_cast<char*>(ctx->ws) + sub_bytes);
+  __half* st_lo = reinterpret_cast<__half*>(reinterpret_cast<char*>(ctx->ws) + sub_bytes + split_bytes);
+  for (int u0 = 0; u0 < num_utts; u0 += nbu) {
+    const int nb = std::min(nbu, num_utts - u0);
+    if ((rc = fbank_forward(ctx->emb, wav, ctx->d_runs + u0, nb, nb * T0, nullptr, nb, T0, w.fbank, w.fmean, st)))
+      return rc;
+    ctx->launches += 2;
+    const __half* feat = nullptr;
+    int Tt = 0;
+    if ((rc = trunk_run(ctx, w, nullptr, nb, T0, st, &feat, &Tt))) return rc;
+    B200_CHECK(Tt == T, B200_ERR_STATE, "trunk output width %d, expected %d", Tt, T);
+    const size_t o = (size_t)u0 * S * 2 * kStatsDim;
+    if ((rc = weighted_pool_forward(feat, nullptr, weights ? weights + (size_t)u0 * S * num_weights : nullptr, nb, T, S,
+                                    num_weights, part, st_hi + o, st_lo + o, st)))
+      return rc;
+    ctx->launches += T <= kPoolSlice ? 1 : 3;
+  }
+  return emb_linear(ctx, st_hi, st_lo, (int64_t)rows, emb, st);
+}
+
+int b200_emb_forward_embedding(b200_ctx* ctx, const float* frames, int32_t B, int32_t T, const float* weights,
+                               int32_t num_speakers, int32_t num_weights, float* emb, void* stream) {
+  B200_CHECK(ctx && ctx->emb.loaded, B200_ERR_STATE, "embedding weights not loaded");
+  B200_CHECK(frames && emb && B >= 0 && T >= 1, B200_ERR_INVALID, "bad arguments");
+  B200_CHECK(!weights || (num_speakers >= 1 && num_weights >= 1), B200_ERR_INVALID,
+             "weights need num_speakers >= 1 and num_weights >= 1 (got %d, %d)", (int)num_speakers, (int)num_weights);
+  if (B == 0) return B200_OK;
+  DeviceGuard g(ctx->device);
+  cudaStream_t st = (cudaStream_t)stream;
+  const int S = weights ? num_speakers : 1;
+  const size_t rows = (size_t)B * S;
+  const size_t split_bytes = align_up(rows * 2 * kStatsDim * sizeof(__half), 1024);
+  const size_t part_bytes = align_up(pool_scratch_bytes(B, S, T), 1024);
+  int rc = ensure_ws(ctx, 2 * split_bytes + part_bytes + 4096);
+  if (rc) return rc;
+  char* base = reinterpret_cast<char*>(ctx->ws);
+  __half* st_hi = reinterpret_cast<__half*>(base);
+  __half* st_lo = reinterpret_cast<__half*>(base + split_bytes);
+  double* part = part_bytes ? reinterpret_cast<double*>(base + 2 * split_bytes) : nullptr;
+  if ((rc = weighted_pool_forward(nullptr, frames, weights, B, T, S, num_weights, part, st_hi, st_lo, st))) return rc;
+  ctx->launches += T <= kPoolSlice ? 1 : 3;
+  return emb_linear(ctx, st_hi, st_lo, (int64_t)rows, emb, st);
 }
 
 int b200_stats_pool(b200_ctx* ctx, const float* seq, const float* weights, float* out, int32_t B, int32_t F, int32_t T,

@@ -49,9 +49,10 @@ struct EmbWeights {
 // impl: 0 = SIMT reference conv, 1 = wgmma tensor-core conv
 int conv_forward(const ConvLayer& L, const __half* in, const __half* residual, __half* out, int B, int H_in, int W_in,
                  int relu, int impl, int num_sms, cudaStream_t stream);
-// frame0 (device, [B], may be NULL = b * 998): first fbank row of each segment, see fbank_forward
+// T0 fbank frames per segment (998 for 10 s); frame0 (device, [B], may be NULL = b * T0): first fbank row of each
+// segment, see fbank_forward.  out: NHWC fp16 [B][80][T0][32]
 int conv1_forward(const float* fbank, const float* fmean, const int* frame0, const float* w, const float* bias,
-                  __half* out, int B, cudaStream_t stream);
+                  __half* out, int B, int T0, cudaStream_t stream);
 
 // fbank with SHARED FRAMES.  The sliding chunks of a file overlap by 90 % and a chunk step of 16000 samples is exactly
 // 100 frame hops, so frame k of chunk c IS frame k - 100 of chunk c + 1: the same 400 samples through the same
@@ -65,15 +66,27 @@ struct FbankRun {
   int row0;        // first row of the run in `fbank`
   int limit;       // valid samples counted from src (INT_MAX for runs of full chunks)
 };
+// fmean[b] = mean of the T0 rows of segment b (frame0 as in conv1_forward)
 int fbank_forward(const EmbWeights& W, const float* wav, const FbankRun* runs, int nruns, int nrows,
-                  const int* frame0, int B, float* fbank, float* fmean, cudaStream_t stream);
+                  const int* frame0, int B, int T0, float* fbank, float* fmean, cudaStream_t stream);
 int fbank_center(float* fbank, const float* fmean, int B, cudaStream_t stream);
-// NHWC fp16 [B][10][125][256] -> NCHW fp32 [B][256][10][125]
-int frames_to_nchw(const __half* feat, float* out, int B, cudaStream_t stream);
+// NHWC fp16 [B][10][T][256] -> NCHW fp32 [B][256][10][T]
+int frames_to_nchw(const __half* feat, float* out, int B, int T, cudaStream_t stream);
 
 // masked statistics pooling: feat [B][10][125][256] fp16 NHWC, masks [B][3][589] u8 -> stats [B*3][5120] fp32
 int stats_pool_forward(const __half* feat, const unsigned char* masks, float* stats, __half* stats_hi,
                        __half* stats_lo, int B, cudaStream_t stream);
+// weighted statistics pooling for any T, S and Tw (pooling.py:30-61, 76-130) -> the fp16 (hi, lo) rows of the Linear:
+// feat NHWC fp16 [B][10][T][256] (trunk output) or frames NCHW fp32 [B][256][10][T] (caller frames, exactly one of
+// the two), w fp32 [B][S][Tw] any real values or NULL (mean and std(correction=1) over the T frames, S = 1).  The
+// weights reach the T frames by torch's CUDA nearest index (upsample_nearest1d).  T is split into slices of
+// kPoolSlice frames; with one slice the sums are the stats_pool_forward ones in the same order, with several the
+// per-slice fp32 sums are combined in fp64 in slice order (deterministic, no atomics).  part: fp64 scratch of
+// pool_scratch_bytes(B, S, T) bytes (none with one slice).  Rows of stats_hi / stats_lo: (b * S + s) * 5120.
+constexpr int kPoolSlice = 512;
+size_t pool_scratch_bytes(int B, int S, int T);
+int weighted_pool_forward(const __half* feat, const float* frames, const float* w, int B, int T, int S, int Tw,
+                          double* part, __half* stats_hi, __half* stats_lo, cudaStream_t stream);
 // generic weighted pooling used by the known-answer tests: seq [B][F][T] fp32, w [B][S][Tw] fp32 -> [B][S][2F]
 int stats_pool_generic(const float* seq, const float* w, float* out, int B, int F, int T, int S, int Tw,
                        cudaStream_t stream);

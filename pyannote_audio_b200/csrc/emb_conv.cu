@@ -219,31 +219,34 @@ __global__ void conv_simt_kernel(const __half* __restrict__ in, const __half* __
 // first conv: 1 -> 32 channels on the (mean-centred) fbank, fp32 in, fp16 NHWC out
 //   x[b][h=f][w=t] = fbank[b][t][f] - mean[b][f]   (resnet.py:411-413 permute + wespeaker/__init__.py:138)
 // ------------------------------------------------------------------------------------------------
-// block = (b, tile of 128 time frames): the (130 x 80) fbank tile is staged in shared memory with coalesced reads,
+// block = (b, tile of 128 of the T0 time frames): the (130 x 80) fbank tile is staged in shared memory with coalesced reads,
 // then thread = time frame walks the 80 frequency rows so that every warp store is 32 x 64 B contiguous.
 constexpr int kC1Tile = 128;
 __global__ void __launch_bounds__(kC1Tile) conv1_kernel(const float* __restrict__ fbank, const float* __restrict__ fmean,
                              const int* __restrict__ frame0, const float* __restrict__ w /*[32][9] folded*/, const float* __restrict__ bias /*[32]*/,
-                             __half* __restrict__ out, int B) {
+                             __half* __restrict__ out, int T0) {
   __shared__ __align__(16) float sw[9 * 32];               // [tap][channel]: one LDS.128 = 4 channels of a tap
   __shared__ __align__(16) float sb[32];
   __shared__ float sx[(kC1Tile + 2) * (kMel + 1)];        // [t][f], +1 padding against bank conflicts
-  const int b = blockIdx.y, t0 = blockIdx.x * kC1Tile;
-  const size_t r0 = frame0 ? (size_t)frame0[b] : (size_t)b * kFbankFrames;     // first fbank row of this segment
+  const int b = blockIdx.x, t0 = blockIdx.y * kC1Tile;    // segments on x: a sub-batch of 1-frame ones holds 263 472
+  const size_t r0 = frame0 ? (size_t)frame0[b] : (size_t)b * T0;             // first fbank row of this segment
   for (int i = threadIdx.x; i < 288; i += blockDim.x) sw[(i % 9) * 32 + i / 9] = w[i];
   if (threadIdx.x < 32) sb[threadIdx.x] = bias[threadIdx.x];
   for (int i = threadIdx.x; i < (kC1Tile + 2) * kMel; i += blockDim.x) {
     const int tt = i / kMel, f = i - tt * kMel;
     const int t = t0 - 1 + tt;
     float v = 0.f;
-    if (t >= 0 && t < kFbankFrames) v = fbank[(r0 + t) * kMel + f] - fmean[b * kMel + f];
+    if (t >= 0 && t < T0) v = fbank[(r0 + t) * kMel + f] - fmean[(size_t)b * kMel + f];
     sx[tt * (kMel + 1) + f] = v;
   }
   __syncthreads();
   const int t = t0 + threadIdx.x;
-  if (t >= kFbankFrames) return;
+  if (t >= T0) return;
   const float* col = sx + threadIdx.x * (kMel + 1);        // rows tt = threadIdx.x + {0,1,2} <-> t-1, t, t+1
   for (int h = 0; h < kMel; ++h) {
+    // re-read the weights from shared memory in every row: hoisted out of the loop, 288 weights + 32 biases do not
+    // fit in the register file and spill to local memory
+    asm volatile("" ::: "memory");
     float x[9];
 #pragma unroll
     for (int kh = 0; kh < 3; ++kh) {
@@ -276,7 +279,7 @@ __global__ void __launch_bounds__(kC1Tile) conv1_kernel(const float* __restrict_
       unpack2(acc2[c], a0, a1);
       o[c] = __floats2half2_rn(fmaxf(a0, 0.f), fmaxf(a1, 0.f));
     }
-    uint4* op = reinterpret_cast<uint4*>(out + (((size_t)b * kMel + h) * kFbankFrames + t) * 32);
+    uint4* op = reinterpret_cast<uint4*>(out + (((size_t)b * kMel + h) * T0 + t) * 32);
     const uint4* src = reinterpret_cast<const uint4*>(o);
 #pragma unroll
     for (int i = 0; i < 4; ++i) op[i] = src[i];
@@ -384,9 +387,9 @@ int conv_forward(const ConvLayer& L, const __half* in, const __half* residual, _
 }
 
 int conv1_forward(const float* fbank, const float* fmean, const int* frame0, const float* w, const float* bias,
-                  __half* out, int B, cudaStream_t stream) {
-  dim3 grid(ceil_div(kFbankFrames, kC1Tile), B);
-  conv1_kernel<<<grid, kC1Tile, 0, stream>>>(fbank, fmean, frame0, w, bias, out, B);
+                  __half* out, int B, int T0, cudaStream_t stream) {
+  dim3 grid(B, ceil_div(T0, kC1Tile));
+  conv1_kernel<<<grid, kC1Tile, 0, stream>>>(fbank, fmean, frame0, w, bias, out, T0);
   B200_CUDA_OK(cudaGetLastError());
   return B200_OK;
 }

@@ -180,20 +180,21 @@ __global__ void __launch_bounds__(256) fbank_kernel(const float* __restrict__ wa
 }
 
 __global__ void __launch_bounds__(640) fbank_mean_kernel(const float* __restrict__ fb, const int* __restrict__ frame0,
-                                                         float* __restrict__ fmean) {
-  // 8 groups of 80 threads each sum an eighth of the frames in fp64, combined in group order
+                                                         int T0, float* __restrict__ fmean) {
+  // 8 groups of 80 threads each sum an eighth of the T0 frames in fp64, combined in group order
   __shared__ double part[8][kMel];
   const int b = blockIdx.x, m = threadIdx.x % kMel, g = threadIdx.x / kMel;
-  const size_t r0 = frame0 ? (size_t)frame0[b] : (size_t)b * kFbankFrames;
+  const size_t r0 = frame0 ? (size_t)frame0[b] : (size_t)b * T0;
   double s = 0.0;
-  for (int t = g; t < kFbankFrames; t += 8) s += (double)fb[(r0 + t) * kMel + m];
+#pragma unroll 8
+  for (int t = g; t < T0; t += 8) s += (double)fb[(r0 + t) * kMel + m];
   part[g][m] = s;
   __syncthreads();
   if (g == 0) {
     double tot = 0.0;
 #pragma unroll
     for (int k = 0; k < 8; ++k) tot += part[k][m];
-    fmean[b * kMel + m] = (float)(tot / kFbankFrames);
+    fmean[(size_t)b * kMel + m] = (float)(tot / T0);
   }
 }
 
@@ -212,30 +213,30 @@ int fbank_center(float* fbank, const float* fmean, int B, cudaStream_t stream) {
   return B200_OK;
 }
 
-__global__ void frames_to_nchw_kernel(const __half* __restrict__ feat, float* __restrict__ out, size_t total) {
+__global__ void frames_to_nchw_kernel(const __half* __restrict__ feat, float* __restrict__ out, int T, size_t total) {
   const size_t idx = (size_t)blockIdx.x * blockDim.x + threadIdx.x;   // over NCHW output
   if (idx >= total) return;
-  const int t = idx % kEmbT;
-  const int h = (idx / kEmbT) % 10;
-  const int c = (idx / (kEmbT * 10)) % 256;
-  const size_t b = idx / ((size_t)kEmbT * 10 * 256);
-  out[idx] = __half2float(feat[((b * 10 + h) * kEmbT + t) * 256 + c]);
+  const size_t t = idx % T;
+  const size_t h = (idx / T) % 10;
+  const size_t c = (idx / ((size_t)T * 10)) % 256;
+  const size_t b = idx / ((size_t)T * 10 * 256);
+  out[idx] = __half2float(feat[((b * 10 + h) * T + t) * 256 + c]);
 }
 
-int frames_to_nchw(const __half* feat, float* out, int B, cudaStream_t stream) {
-  const size_t total = (size_t)B * 256 * 10 * kEmbT;
-  frames_to_nchw_kernel<<<(unsigned)((total + 255) / 256), 256, 0, stream>>>(feat, out, total);
+int frames_to_nchw(const __half* feat, float* out, int B, int T, cudaStream_t stream) {
+  const size_t total = (size_t)B * 256 * 10 * T;
+  frames_to_nchw_kernel<<<(unsigned)((total + 255) / 256), 256, 0, stream>>>(feat, out, T, total);
   B200_CUDA_OK(cudaGetLastError());
   return B200_OK;
 }
 
 int fbank_forward(const EmbWeights& W, const float* wav, const FbankRun* runs, int nruns, int nrows,
-                  const int* frame0, int B, float* fbank, float* fmean, cudaStream_t stream) {
+                  const int* frame0, int B, int T0, float* fbank, float* fmean, cudaStream_t stream) {
   const unsigned grid = (unsigned)ceil_div(nrows, 16);      // 8 warps x 2 frame rows per block
   fbank_kernel<<<grid, 256, 0, stream>>>(wav, runs, nruns, nrows, W.window, W.twiddle, W.mel_w, W.mel_start,
                                          W.mel_len, W.mel_off, fbank);
   B200_CUDA_OK(cudaGetLastError());
-  fbank_mean_kernel<<<B, 640, 0, stream>>>(fbank, frame0, fmean);
+  fbank_mean_kernel<<<B, 640, 0, stream>>>(fbank, frame0, T0, fmean);
   B200_CUDA_OK(cudaGetLastError());
   return B200_OK;
 }
@@ -313,7 +314,178 @@ int stats_pool_forward(const __half* feat, const unsigned char* masks, float* st
   return B200_OK;
 }
 
-// generic fp32 version (any F, T, S, Tw) used by the known-answer tests of the reference
+// ------------------------------------------------------------------------------------------------
+// weighted statistics pooling for any T, S and Tw (utterances of any length, caller frames, soft weights)
+// ------------------------------------------------------------------------------------------------
+// torch's CUDA nearest index (upsample_nearest1d, the device F.interpolate(mode="nearest") runs on): scale is
+// (float)Tw / T, src = min(floor(dst * scale), Tw - 1), with the exact special cases T == Tw and T == 2 Tw.  Not the
+// integer t * Tw / T of stats_pool_kernel: the two differ on a few frames of long sequences.
+__device__ __forceinline__ int nearest_src(int dst, int T, int Tw, float scale) {
+  if (T == Tw) return dst;
+  if (T == 2 * Tw) return dst >> 1;
+  return min((int)floorf((float)dst * scale), Tw - 1);
+}
+
+__device__ __forceinline__ float to_f(__half v) { return __half2float(v); }
+__device__ __forceinline__ float to_f(float v) { return v; }
+
+__device__ __forceinline__ void store_split(__half* hi, __half* lo, size_t row, int c, int h, float mean, float sdv) {
+  const __half mh = __float2half_rn(mean), sh = __float2half_rn(sdv);
+  hi[row + c * 10 + h] = mh;
+  lo[row + c * 10 + h] = __float2half_rn(mean - __half2float(mh));
+  hi[row + kStatsDim + c * 10 + h] = sh;
+  lo[row + kStatsDim + c * 10 + h] = __float2half_rn(sdv - __half2float(sh));
+}
+
+struct PoolArgs {
+  const void* x;          // NHWC fp16 feat or NCHW fp32 frames
+  const float* w;         // [B][S][Tw] or NULL
+  int S, T, Tw, nslices;
+  float scale;            // (float)Tw / T
+  double* part;           // [B * S][10][nslices][4][256]: sum w (sum x), sum w^2, sum w x, sum w (x - mean)^2
+  __half *hi, *lo;
+};
+
+// x of (b, h, channel c): NHWC [B][10][T][256] (stride 256 between frames) or NCHW [B][256][10][T] (stride 1)
+template <typename X>
+__device__ __forceinline__ const X* pool_row(const PoolArgs& a, int b, int h, int c, size_t* stride) {
+  const X* x = static_cast<const X*>(a.x);
+  if constexpr (sizeof(X) == 2) { *stride = 256; return x + ((size_t)b * 10 + h) * a.T * 256 + c; }
+  else { *stride = 1; return x + (((size_t)b * 256 + c) * 10 + h) * a.T; }
+}
+
+// PHASE 0: the whole sequence in one slice, finished here (the stats_pool_kernel sums, in its order);
+// PHASE 1: per-slice fp32 sums; PHASE 2: per-slice sum of w (x - mean)^2 around the mean of all slices' sums.
+// grid (B * S * 10, nslices), thread = channel
+template <int PHASE, typename X>
+__global__ void __launch_bounds__(256) wpool_kernel(PoolArgs a) {
+  __shared__ float s_w[kPoolSlice];
+  const int row = blockIdx.x / 10, h = blockIdx.x % 10, c = threadIdx.x;   // row = b * S + s
+  const int b = row / a.S, sl = blockIdx.y;
+  const int t0 = sl * kPoolSlice, t1 = min(a.T, t0 + kPoolSlice);
+  size_t xs;
+  const X* xp = pool_row<X>(a, b, h, c, &xs);
+  const bool weighted = a.w != nullptr;
+  if (weighted) {
+    const float* wr = a.w + (size_t)row * a.Tw;
+    for (int i = threadIdx.x; i < t1 - t0; i += blockDim.x) s_w[i] = wr[nearest_src(t0 + i, a.T, a.Tw, a.scale)];
+  }
+  __syncthreads();
+  double* part = a.part + (((size_t)row * 10 + h) * a.nslices) * 4 * 256 + c;   // slot k of slice j: [(j*4+k)*256]
+  if (PHASE == 0 || PHASE == 1) {
+    float v1 = 0.f, v2 = 0.f, sx = 0.f;
+    if (weighted) {
+      for (int t = t0; t < t1; ++t) {
+        const float x = to_f(xp[(size_t)t * xs]);
+        const float w = s_w[t - t0];
+        v1 += w;
+        v2 += w * w;
+        sx += x * w;
+      }
+    } else {
+      for (int t = t0; t < t1; ++t) sx += to_f(xp[(size_t)t * xs]);
+    }
+    if (PHASE == 1) {
+      part[(sl * 4 + 0) * 256] = weighted ? (double)v1 : (double)sx;
+      part[(sl * 4 + 1) * 256] = (double)v2;
+      part[(sl * 4 + 2) * 256] = (double)sx;
+      return;
+    }
+    const size_t orow = (size_t)row * (2 * kStatsDim);
+    if (weighted) {
+      v1 += 1e-8f;
+      const float mean = sx / v1;
+      float sd = 0.f;
+      for (int t = t0; t < t1; ++t) {
+        const float d = to_f(xp[(size_t)t * xs]) - mean;
+        sd += d * d * s_w[t - t0];
+      }
+      const float var = sd / (v1 - v2 / v1 + 1e-8f);
+      store_split(a.hi, a.lo, orow, c, h, mean, sqrtf(var));
+    } else {                                               // torch mean / std(correction=1): T = 1 gives NaN
+      const float mean = sx / a.T;
+      float acc = 0.f;
+      for (int t = t0; t < t1; ++t) {
+        const float d = to_f(xp[(size_t)t * xs]) - mean;
+        acc += d * d;
+      }
+      store_split(a.hi, a.lo, orow, c, h, mean, sqrtf(acc / (a.T - 1)));
+    }
+  } else {
+    double s0 = 0.0, s2 = 0.0;                             // every slice's sums, in slice order
+    for (int j = 0; j < a.nslices; ++j) { s0 += part[(j * 4 + 0) * 256]; s2 += part[(j * 4 + 2) * 256]; }
+    const float mean = weighted ? (float)(s2 / (s0 + 1e-8)) : (float)(s0 / a.T);
+    float sd = 0.f;
+    for (int t = t0; t < t1; ++t) {
+      const float d = to_f(xp[(size_t)t * xs]) - mean;
+      sd += weighted ? d * d * s_w[t - t0] : d * d;
+    }
+    part[(sl * 4 + 3) * 256] = (double)sd;
+  }
+}
+
+// combine the slices in fp64, in slice order; grid B * S * 10, thread = channel
+__global__ void __launch_bounds__(256) wpool_final_kernel(PoolArgs a) {
+  const int row = blockIdx.x / 10, h = blockIdx.x % 10, c = threadIdx.x;
+  const double* part = a.part + (((size_t)row * 10 + h) * a.nslices) * 4 * 256 + c;
+  double s[4] = {0.0, 0.0, 0.0, 0.0};
+  for (int j = 0; j < a.nslices; ++j)
+#pragma unroll
+    for (int k = 0; k < 4; ++k) s[k] += part[(j * 4 + k) * 256];
+  float mean;
+  double var;
+  if (a.w) {
+    const double v1 = s[0] + 1e-8;
+    mean = (float)(s[2] / v1);
+    var = s[3] / (v1 - s[1] / v1 + 1e-8);
+  } else {
+    mean = (float)(s[0] / a.T);
+    var = s[3] / (double)(a.T - 1);
+  }
+  store_split(a.hi, a.lo, (size_t)row * (2 * kStatsDim), c, h, mean, (float)sqrt(var));
+}
+
+size_t pool_scratch_bytes(int B, int S, int T) {
+  const int nslices = ceil_div(T, kPoolSlice);
+  return nslices > 1 ? (size_t)B * S * 10 * nslices * 4 * 256 * sizeof(double) : 0;
+}
+
+int weighted_pool_forward(const __half* feat, const float* frames, const float* w, int B, int T, int S, int Tw,
+                          double* part, __half* stats_hi, __half* stats_lo, cudaStream_t stream) {
+  B200_CHECK((feat == nullptr) != (frames == nullptr) && T >= 1 && S >= 1 && (w == nullptr ? S == 1 : Tw >= 1),
+             B200_ERR_INVALID, "weighted pooling: bad arguments");
+  PoolArgs a;
+  a.x = feat ? (const void*)feat : (const void*)frames;
+  a.w = w;
+  a.S = S; a.T = T; a.Tw = w ? Tw : T;
+  a.nslices = ceil_div(T, kPoolSlice);
+  a.scale = (float)a.Tw / (float)T;
+  a.part = part;
+  a.hi = stats_hi; a.lo = stats_lo;
+  B200_CHECK(a.nslices <= 65535 && (size_t)B * S * 10 <= 0x7fffffffu, B200_ERR_INVALID,
+             "weighted pooling: %d frames x %lld rows is too large", T, (long long)B * S);
+  B200_CHECK(a.nslices == 1 || part != nullptr, B200_ERR_INVALID, "weighted pooling: scratch missing");
+  const dim3 grid((unsigned)((size_t)B * S * 10), (unsigned)a.nslices);
+  if (a.nslices == 1) {
+    if (feat) wpool_kernel<0, __half><<<grid, 256, 0, stream>>>(a);
+    else wpool_kernel<0, float><<<grid, 256, 0, stream>>>(a);
+  } else {
+    if (feat) {
+      wpool_kernel<1, __half><<<grid, 256, 0, stream>>>(a);
+      wpool_kernel<2, __half><<<grid, 256, 0, stream>>>(a);
+    } else {
+      wpool_kernel<1, float><<<grid, 256, 0, stream>>>(a);
+      wpool_kernel<2, float><<<grid, 256, 0, stream>>>(a);
+    }
+    wpool_final_kernel<<<grid.x, 256, 0, stream>>>(a);
+  }
+  B200_CUDA_OK(cudaGetLastError());
+  return B200_OK;
+}
+
+// generic fp32 version (any F, T, S, Tw) used by the known-answer tests of the reference.  It keeps the integer index
+// t * Tw / T, which differs from torch's CUDA nearest index (nearest_src above) on a few frames of long sequences;
+// moving it to nearest_src is left for later.
 __global__ void stats_pool_generic_kernel(const float* __restrict__ seq, const float* __restrict__ w,
                                           float* __restrict__ out, int B, int F, int T, int S, int Tw) {
   const int idx = blockIdx.x * blockDim.x + threadIdx.x;

@@ -16,7 +16,7 @@ import torch
 from . import ops
 from .audio import AudioFile
 from .core import Resolution, Segment, SlidingWindow, SlidingWindowFeature, Specifications
-from .models import Model
+from .models import Model, WeSpeakerResNet34
 
 
 class BaseInference:
@@ -124,6 +124,8 @@ class Inference(BaseInference):
         return cls, wav_dev, off, valid
 
     def slide(self, waveform: torch.Tensor, sample_rate: int, hook: Optional[Callable] = None):
+        if isinstance(self.model, WeSpeakerResNet34):
+            return self._slide_embedding(waveform, sample_rate, hook=hook)
         cls, _, off, _ = self.slide_device(waveform, sample_rate, return_logp=self.conversion != "powerset")
         total = len(off)
         if hook is not None:
@@ -150,6 +152,30 @@ class Inference(BaseInference):
         if has_last:
             aggregated.data = aggregated.crop(Segment(0.0, num_samples / sample_rate), mode="loose")
         return aggregated
+
+    def _slide_embedding(self, waveform: torch.Tensor, sample_rate: int, hook: Optional[Callable] = None):
+        """One embedding per window (inference.py:261-313 for a Resolution.CHUNK model): the chunks are cut as the
+        reference cuts them, the last one zero-padded to the full window, and all of them (they have one length) go
+        through one library call over a resident copy of the file -> SlidingWindowFeature (chunks, 256)."""
+        window_size = self.model.audio.get_num_samples(self.duration)
+        step_size = round(self.step * sample_rate)
+        _, num_samples = waveform.shape
+        off, _, _, _ = chunk_layout(num_samples, window_size, step_size)
+        total = len(off)
+        if hook is not None:
+            hook(completed=0, total=total)
+        ctx = self.model._ctx()
+        wav_dev = torch.zeros(int(off[-1]) + window_size, dtype=torch.float32, device=ctx.device)
+        wav_dev[:num_samples].copy_(waveform[0])
+        try:
+            emb = ctx.emb_forward_utt(wav_dev, off, window_size)
+        except MemoryError:
+            raise MemoryError(f"batch_size ({self.batch_size: d}) is probably too large. "
+                              f"Try with a smaller value until memory error disappears.")
+        outputs = emb[:, 0].cpu().numpy()
+        if hook is not None:
+            hook(completed=total, total=total)
+        return SlidingWindowFeature(outputs, SlidingWindow(start=0.0, duration=self.duration, step=self.step))
 
     def __call__(self, file: AudioFile, hook: Optional[Callable] = None):
         waveform, sample_rate = self.model.audio(file)

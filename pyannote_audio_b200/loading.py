@@ -96,8 +96,12 @@ def _pipeline_class(name: str):
         from .vad import VoiceActivityDetection
 
         return VoiceActivityDetection
-    raise NotImplementedError(f"pipeline '{name}' has no CUDA implementation here (SpeakerDiarization and "
-                              f"VoiceActivityDetection are available)")
+    if short == "SpeakerEmbedding":
+        from .speaker_verification import SpeakerEmbedding
+
+        return SpeakerEmbedding
+    raise NotImplementedError(f"pipeline '{name}' has no CUDA implementation here (SpeakerDiarization, "
+                              f"VoiceActivityDetection and SpeakerEmbedding are available)")
 
 
 def resolve_pipeline(checkpoint, revision: Optional[str] = None, subfolder: Optional[str] = None, token=None,

@@ -390,7 +390,16 @@ class WeSpeakerResNet34(Model):
         return self._ctx().emb_trunk(self.compute_fbank(waveforms))
 
     def forward(self, waveforms: torch.Tensor, weights: Optional[torch.Tensor] = None) -> torch.Tensor:
-        """waveforms (batch, 1, 160000), weights (batch, 589) or (batch, speakers<=3, 589) in {0,1}."""
+        """waveforms (batch, 1, samples) with samples >= 400, weights (batch, frames) or (batch, speakers<=3, frames) in
+        {0,1}.  10 s chunks take the diarization path (weights over the 589 segmentation frames); other lengths
+        interpolate any number of weight frames onto the trunk frames."""
+        b, c, s = waveforms.shape
+        if c != 1:
+            raise ValueError(f"WeSpeaker kernels expect mono waveforms, got {c} channels")
+        if s < 400:
+            raise ValueError(f"WeSpeaker needs at least 400 samples (one 25 ms fbank frame), got {s}")
+        if s != ops.CHUNK:
+            return self._forward_utt(waveforms, weights)
         ctx, flat, off, valid = self._flat(waveforms)
         b = len(off)
         if weights is None:
@@ -407,3 +416,24 @@ class WeSpeakerResNet34(Model):
         masks[:, : w.shape[1]] = w.to(ctx.device).to(torch.uint8)
         emb = ctx.emb_forward(flat, off, valid, masks)[:, : w.shape[1]]
         return emb[:, 0] if squeeze else emb
+
+    def _forward_utt(self, waveforms: torch.Tensor, weights: Optional[torch.Tensor]) -> torch.Tensor:
+        b, _, s = waveforms.shape
+        squeeze = weights is None or weights.dim() == 2
+        if weights is not None:
+            w = weights.unsqueeze(1) if weights.dim() == 2 else weights
+            if w.dim() != 3 or w.shape[0] != b or w.shape[1] > 3 or w.shape[2] < 1:
+                raise ValueError("weights must be (batch, frames) or (batch, speakers<=3, frames)")
+            if not bool(((w == 0) | (w == 1)).all()):
+                raise ValueError("the masked statistics pooling kernel takes binary (0/1) weights")
+            weights = w
+        ctx = self._ctx()
+        flat = waveforms.to(device=ctx.device, dtype=torch.float32).reshape(-1).contiguous()
+        emb = ctx.emb_forward_utt(flat, np.arange(b, dtype=np.int64) * s, s, weights=weights)
+        return emb[:, 0] if squeeze else emb
+
+    def forward_embedding(self, frames: torch.Tensor, weights: Optional[torch.Tensor] = None) -> torch.Tensor:
+        """Frame-wise features (batch, 256, 10, frames) -> (batch, 256), or (batch, speakers, 256) for
+        (batch, speakers, frames) weights.  Any number of frames, any real weights, any number of speakers."""
+        emb = self._ctx().emb_forward_embedding(frames, weights=weights)
+        return emb if weights is not None and weights.dim() == 3 else emb[:, 0]

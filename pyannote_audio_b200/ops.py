@@ -254,6 +254,53 @@ class Context:
                                                      _ptr(masks), _ptr(emb), _stream(self.device)))
         return emb
 
+    def _pool_weights(self, weights: Optional[torch.Tensor], n: int):
+        """(n, Tw) or (n, S, Tw) fp32 pooling weights on this device -> (tensor or None, S, Tw)."""
+        if weights is None:
+            return None, 1, 0
+        if weights.dim() == 2:
+            weights = weights.unsqueeze(1)
+        if weights.dim() != 3 or weights.shape[0] != n or weights.shape[1] < 1 or weights.shape[2] < 1:
+            raise ValueError(f"weights must have shape ({n}, frames) or ({n}, speakers, frames), got "
+                             f"{tuple(weights.shape)}")
+        weights = weights.to(device=self.device, dtype=torch.float32).contiguous()
+        return weights, int(weights.shape[1]), int(weights.shape[2])
+
+    def emb_forward_utt(self, wav, off, num_samples: int, weights: Optional[torch.Tensor] = None,
+                        out: Optional[torch.Tensor] = None):
+        """Embeddings of utterances of one length: utterance i = wav[off[i] : off[i] + num_samples] (any length >= 400
+        samples).  ``weights``: None or (n, Tw) / (n, S, Tw) soft pooling weights (any Tw, interpolated onto the
+        trunk frames) -> (n, max(S, 1), 256) float32."""
+        if wav.device != self.device or wav.dtype != torch.float32 or not wav.is_contiguous():
+            raise ValueError(f"waveform must be a contiguous float32 tensor on {self.device}")
+        off = np.ascontiguousarray(off, dtype=np.int64).reshape(-1)
+        n, num_samples = len(off), int(num_samples)
+        if num_samples < 400:
+            raise ValueError(f"utterances of {num_samples} samples are shorter than one 400-sample fbank frame")
+        if n and (int(off.min()) < 0 or int(off.max()) + num_samples > wav.numel()):
+            raise ValueError("an utterance reads outside the waveform buffer")
+        w, S, Tw = self._pool_weights(weights, n)
+        emb = self._out(out, (n, S, EMB_DIM), torch.float32)
+        with torch.cuda.device(self.device):
+            _lib.check(self.lib.b200_emb_forward_utt(self._h, _ptr(wav), off.ctypes.data, num_samples, n, _ptr(w),
+                                                     S if w is not None else 0, Tw, _ptr(emb), _stream(self.device)))
+        return emb
+
+    def emb_forward_embedding(self, frames: torch.Tensor, weights: Optional[torch.Tensor] = None):
+        """ResNet.forward_embedding on frames (B, 256, 10, T) -> (B, max(S, 1), 256) float32; weights as in
+        emb_forward_utt."""
+        if frames.dim() != 4 or tuple(frames.shape[1:3]) != (256, 10) or frames.shape[3] < 1:
+            raise ValueError(f"frames must have shape (batch, 256, 10, frames), got {tuple(frames.shape)}")
+        frames = frames.to(device=self.device, dtype=torch.float32).contiguous()
+        B, T = int(frames.shape[0]), int(frames.shape[3])
+        w, S, Tw = self._pool_weights(weights, B)
+        emb = torch.empty((B, S, EMB_DIM), dtype=torch.float32, device=self.device)
+        with torch.cuda.device(self.device):
+            _lib.check(self.lib.b200_emb_forward_embedding(self._h, _ptr(frames), B, T, _ptr(w),
+                                                           S if w is not None else 0, Tw, _ptr(emb),
+                                                           _stream(self.device)))
+        return emb
+
     def push(self, src: torch.Tensor, peers: Sequence[int]):
         """P2P copy of a contiguous device tensor to raw peer addresses (same layout), on the current stream."""
         if not peers or src.numel() == 0:
