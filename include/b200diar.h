@@ -124,6 +124,15 @@ int b200_audio_ingest(b200_ctx* ctx, const void* pcm, int32_t format, int32_t ch
  * (argmax of the LogSoftmax output, utils/powerset.py:135-140); optional log-probabilities [num_chunks][589][7]. */
 int b200_seg_forward(b200_ctx* ctx, const float* wav, const int64_t* chunk_off, const int32_t* chunk_valid,
                      int32_t num_chunks, uint8_t* classes, float* logp, void* stream);
+/* PyanNet.forward on windows of any length (models/segmentation/PyanNet.py:223-240): window i covers
+ * wav[chunk_off[i] .. chunk_off[i] + window), of which the first chunk_valid[i] <= window samples are real (zero padding
+ * after them, inference.py:270-278).  Every InstanceNorm normalises over the whole padded window.  F = 1 + (window - 251)
+ * / 10 frames, then MaxPool 3, Conv1d 5, MaxPool 3, Conv1d 5, MaxPool 3 (589 for 160000); window >= 1261 (F >= 2).
+ * Output classes[num_chunks][F], optional logp[num_chunks][F][7].  Windows run in sub-batches of at most
+ * seg_max_batch x 160000 samples; one window longer than that (5.87 h with the default) returns B200_STATUS_INVALID.
+ * b200_seg_forward is this function with window = 160000. */
+int b200_seg_forward_window(b200_ctx* ctx, const float* wav, const int64_t* chunk_off, const int32_t* chunk_valid,
+                            int32_t num_chunks, int32_t window, uint8_t* classes, float* logp, void* stream);
 /* SincNet.forward alone (models/blocks/sincnet.py:163-184): out[num_chunks][589][60] fp32 (frame-major). */
 int b200_sincnet_forward(b200_ctx* ctx, const float* wav, const int64_t* chunk_off, const int32_t* chunk_valid,
                          int32_t num_chunks, float* out, void* stream);
@@ -203,6 +212,12 @@ int b200_reconstruct(b200_ctx* ctx, const uint8_t* seg, const int8_t* hard_clust
 int b200_aggregate(b200_ctx* ctx, const float* scores, const int32_t* start_frame, int32_t num_chunks,
                    int32_t num_frames, int32_t num_classes, const double* hamming, const double* warm_up,
                    int32_t skip_average, float missing, float epsilon, float* out, void* stream);
+/* The same for chunks of any frames_per_chunk frames: scores[num_chunks][frames_per_chunk][K], hamming / warm_up
+ * fp64[frames_per_chunk] or NULL.  b200_aggregate is this function with frames_per_chunk = 589. */
+int b200_aggregate_window(b200_ctx* ctx, const float* scores, const int32_t* start_frame, int32_t num_chunks,
+                          int32_t num_frames, int32_t frames_per_chunk, int32_t num_classes, const double* hamming,
+                          const double* warm_up, int32_t skip_average, float missing, float epsilon, float* out,
+                          void* stream);
 /* VoiceActivityDetection's pre-aggregation step (pipelines/voice_activity_detection.py:111-114: max over the
  * speakers of the multilabel output) straight from the powerset classes: speech[n] fp32 in {0,1}. */
 int b200_powerset_speech(b200_ctx* ctx, const uint8_t* classes, int64_t n, float* speech, void* stream);

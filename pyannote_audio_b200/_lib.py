@@ -55,6 +55,8 @@ _PROTOS = {
     "b200_emb_load": (C.c_int, [C.c_void_p, C.POINTER(EmbWeights)]),
     "b200_seg_forward": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_int32, C.c_void_p, C.c_void_p,
                                    C.c_void_p]),
+    "b200_seg_forward_window": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_int32, C.c_int32,
+                                          C.c_void_p, C.c_void_p, C.c_void_p]),
     "b200_sincnet_forward": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_int32, C.c_void_p,
                                        C.c_void_p]),
     "b200_powerset_to_multilabel": (C.c_int, [C.c_void_p, C.c_void_p, C.c_int64, C.c_void_p, C.c_void_p]),
@@ -95,6 +97,9 @@ _PROTOS = {
                                     C.c_int32, C.c_void_p, C.c_int64, C.c_void_p]),
     "b200_aggregate": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_int32, C.c_int32, C.c_int32, C.c_void_p,
                                  C.c_void_p, C.c_int32, C.c_float, C.c_float, C.c_void_p, C.c_void_p]),
+    "b200_aggregate_window": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_int32, C.c_int32, C.c_int32, C.c_int32,
+                                        C.c_void_p, C.c_void_p, C.c_int32, C.c_float, C.c_float, C.c_void_p,
+                                        C.c_void_p]),
     "b200_powerset_speech": (C.c_int, [C.c_void_p, C.c_void_p, C.c_int64, C.c_void_p, C.c_void_p]),
     "b200_plda_transform": (C.c_int, [C.c_void_p, C.c_void_p, C.c_int32, C.c_int32, C.c_int32, C.c_int32, C.c_void_p,
                                       C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p]),

@@ -124,11 +124,12 @@ int ensure_meta(b200_ctx* ctx, int n) {
   return B200_OK;
 }
 
-int push_meta(b200_ctx* ctx, const int64_t* off, const int32_t* valid, int n, cudaStream_t st) {
+int push_meta(b200_ctx* ctx, const int64_t* off, const int32_t* valid, int n, cudaStream_t st,
+              int max_valid = kChunk) {
   int rc = ensure_meta(ctx, n);
   if (rc) return rc;
   for (int i = 0; i < n; ++i)
-    B200_CHECK(valid[i] >= 0 && valid[i] <= kChunk && off[i] >= 0, B200_ERR_INVALID,
+    B200_CHECK(valid[i] >= 0 && valid[i] <= max_valid && off[i] >= 0, B200_ERR_INVALID,
                "chunk %d: offset %lld / valid %d out of range", i, (long long)off[i], (int)valid[i]);
   B200_CUDA_OK(cudaMemcpyAsync(ctx->d_off, off, sizeof(long long) * n, cudaMemcpyHostToDevice, st));
   B200_CUDA_OK(cudaMemcpyAsync(ctx->d_valid, valid, sizeof(int) * n, cudaMemcpyHostToDevice, st));
@@ -583,32 +584,45 @@ int b200_emb_load(b200_ctx* ctx, const b200_emb_weights* w) {
 }
 
 // ------------------------------------------------------------------------------------------------------
+// PyanNet on n windows of `window` samples.  A sub-batch holds at most seg_max_batch x 160000 window samples (the
+// workspace of seg_max_batch 10 s chunks) and at most 65535 windows (the y extent of the SincNet grids).
 static int seg_run(b200_ctx* ctx, const float* wav, const int64_t* chunk_off, const int32_t* chunk_valid, int n,
-                   uint8_t* classes, float* logp, float* sinc_out, cudaStream_t st) {
+                   int window, uint8_t* classes, float* logp, float* sinc_out, cudaStream_t st) {
   B200_CHECK(ctx && ctx->seg.loaded, B200_ERR_STATE, "segmentation weights not loaded");
   B200_CHECK(wav && chunk_off && chunk_valid && n >= 0, B200_ERR_INVALID, "bad arguments");
+  B200_CHECK(window >= kSegMinWindow, B200_ERR_INVALID,
+             "windows of %d samples are too short: PyanNet needs at least %d samples (2 output frames)", window,
+             kSegMinWindow);
+  const int64_t budget = (int64_t)ctx->seg_max_batch * kChunk;
+  B200_CHECK(window <= budget, B200_ERR_INVALID,
+             "a window of %d samples is longer than the %lld samples of one segmentation sub-batch (seg_max_batch %d x "
+             "160000): set the option seg_max_batch to at least %lld, or segment shorter excerpts",
+             window, (long long)budget, ctx->seg_max_batch, (long long)((window + kChunk - 1) / kChunk));
   if (n == 0) return B200_OK;
   DeviceGuard g(ctx->device);
-  const int nbmax = n < ctx->seg_max_batch ? n : ctx->seg_max_batch;
-  const size_t x0_bytes = align_up((size_t)nbmax * kFrames * 64 * sizeof(float), 1024);
-  const size_t sinc_b = sincnet_workspace_bytes(nbmax), lstm_b = lstm_workspace_bytes(nbmax);
+  const SegGeom geom = seg_geom(window);
+  const int T = geom.pool2;
+  const int nbmax = (int)std::min<int64_t>(std::min<int64_t>(n, budget / window), 65535);
+  const size_t x0_bytes = align_up((size_t)nbmax * T * 64 * sizeof(float), 1024);
+  const size_t sinc_b = sincnet_workspace_bytes(geom, nbmax), lstm_b = lstm_workspace_bytes(nbmax, T);
   const size_t big = sinc_b > lstm_b ? sinc_b : lstm_b;    // the two phases reuse the same region
   int rc = ensure_ws(ctx, x0_bytes + big + 4096);
   if (rc) return rc;
-  if ((rc = push_meta(ctx, chunk_off, chunk_valid, n, st))) return rc;
+  if ((rc = push_meta(ctx, chunk_off, chunk_valid, n, st, window))) return rc;
   float* x0 = reinterpret_cast<float*>(ctx->ws);
   void* region = reinterpret_cast<char*>(ctx->ws) + x0_bytes;
   for (int c0 = 0; c0 < n; c0 += nbmax) {
     const int nb = (n - c0) < nbmax ? (n - c0) : nbmax;
     ScopedTimer timer(ctx, &ctx->seg_events, st);
     if (ctx->profile) ctx->seg_chunks += nb;
-    float* x0_dst = sinc_out ? sinc_out + (size_t)c0 * kFrames * 64 : x0;
-    if ((rc = sincnet_forward(ctx->seg, wav, ctx->d_off + c0, ctx->d_valid + c0, nb, region, x0_dst, ctx->seg_conv_impl, st)))
+    float* x0_dst = sinc_out ? sinc_out + (size_t)c0 * T * 64 : x0;
+    if ((rc = sincnet_forward(ctx->seg, geom, wav, ctx->d_off + c0, ctx->d_valid + c0, nb, region, x0_dst,
+                              ctx->seg_conv_impl, st)))
       return rc;
-    ctx->launches += 8;
+    ctx->launches += sincnet_launches(geom);
     if (sinc_out) continue;
-    if ((rc = lstm_head_forward(ctx->seg, x0, nb, region, classes + (size_t)c0 * kFrames,
-                                logp ? logp + (size_t)c0 * kFrames * kClasses : nullptr, ctx->num_sms,
+    if ((rc = lstm_head_forward(ctx->seg, x0, nb, T, region, classes + (size_t)c0 * T,
+                                logp ? logp + (size_t)c0 * T * kClasses : nullptr, ctx->num_sms,
                                 ctx->seg_gemm_impl, ctx->seg_rec_impl, st)))
       return rc;
     ctx->launches += 2 * ctx->seg.lstm_layers + 3;
@@ -616,11 +630,16 @@ static int seg_run(b200_ctx* ctx, const float* wav, const int64_t* chunk_off, co
   return B200_OK;
 }
 
-int b200_seg_forward(b200_ctx* ctx, const float* wav, const int64_t* chunk_off, const int32_t* chunk_valid,
-                     int32_t num_chunks, uint8_t* classes, float* logp, void* stream) {
+int b200_seg_forward_window(b200_ctx* ctx, const float* wav, const int64_t* chunk_off, const int32_t* chunk_valid,
+                            int32_t num_chunks, int32_t window, uint8_t* classes, float* logp, void* stream) {
   if (num_chunks == 0) return B200_OK;
   B200_CHECK(classes != nullptr, B200_ERR_INVALID, "classes is NULL");
-  return seg_run(ctx, wav, chunk_off, chunk_valid, num_chunks, classes, logp, nullptr, (cudaStream_t)stream);
+  return seg_run(ctx, wav, chunk_off, chunk_valid, num_chunks, window, classes, logp, nullptr, (cudaStream_t)stream);
+}
+
+int b200_seg_forward(b200_ctx* ctx, const float* wav, const int64_t* chunk_off, const int32_t* chunk_valid,
+                     int32_t num_chunks, uint8_t* classes, float* logp, void* stream) {
+  return b200_seg_forward_window(ctx, wav, chunk_off, chunk_valid, num_chunks, kChunk, classes, logp, stream);
 }
 
 __global__ void strip_pad_kernel(const float* __restrict__ x64, float* __restrict__ out, size_t rows) {
@@ -638,7 +657,7 @@ int b200_sincnet_forward(b200_ctx* ctx, const float* wav, const int64_t* chunk_o
   float* tmp = nullptr;
   const size_t rows = (size_t)num_chunks * kFrames;
   B200_CUDA_OK(cudaMalloc((void**)&tmp, rows * 64 * sizeof(float)));
-  int rc = seg_run(ctx, wav, chunk_off, chunk_valid, num_chunks, nullptr, nullptr, tmp, st);
+  int rc = seg_run(ctx, wav, chunk_off, chunk_valid, num_chunks, kChunk, nullptr, nullptr, tmp, st);
   if (rc == B200_OK) {
     strip_pad_kernel<<<(unsigned)((rows * 60 + 255) / 256), 256, 0, st>>>(tmp, out, rows);
     ctx->launches += 1;
@@ -984,15 +1003,24 @@ int b200_reconstruct(b200_ctx* ctx, const uint8_t* seg, const int8_t* hard_clust
                      count, discrete, (cudaStream_t)stream);
 }
 
-int b200_aggregate(b200_ctx* ctx, const float* scores, const int32_t* start_frame, int32_t num_chunks,
-                   int32_t num_frames, int32_t num_classes, const double* hamming, const double* warm_up,
-                   int32_t skip_average, float missing, float epsilon, float* out, void* stream) {
-  B200_CHECK(ctx && scores && start_frame && out && num_chunks > 0 && num_frames > 0 && num_classes > 0,
+int b200_aggregate_window(b200_ctx* ctx, const float* scores, const int32_t* start_frame, int32_t num_chunks,
+                          int32_t num_frames, int32_t frames_per_chunk, int32_t num_classes, const double* hamming,
+                          const double* warm_up, int32_t skip_average, float missing, float epsilon, float* out,
+                          void* stream) {
+  B200_CHECK(ctx && scores && start_frame && out && num_chunks > 0 && num_frames > 0 && frames_per_chunk > 0 &&
+                 num_classes > 0,
              B200_ERR_INVALID, "bad arguments");
   DeviceGuard g(ctx->device);
   ctx->launches += 1;
-  return aggregate_scores(scores, start_frame, num_chunks, num_frames, num_classes, hamming, warm_up, skip_average,
-                          missing, epsilon, out, (cudaStream_t)stream);
+  return aggregate_scores(scores, start_frame, num_chunks, num_frames, frames_per_chunk, num_classes, hamming, warm_up,
+                          skip_average, missing, epsilon, out, (cudaStream_t)stream);
+}
+
+int b200_aggregate(b200_ctx* ctx, const float* scores, const int32_t* start_frame, int32_t num_chunks,
+                   int32_t num_frames, int32_t num_classes, const double* hamming, const double* warm_up,
+                   int32_t skip_average, float missing, float epsilon, float* out, void* stream) {
+  return b200_aggregate_window(ctx, scores, start_frame, num_chunks, num_frames, kFrames, num_classes, hamming,
+                               warm_up, skip_average, missing, epsilon, out, stream);
 }
 
 int b200_powerset_speech(b200_ctx* ctx, const uint8_t* classes, int64_t n, float* speech, void* stream) {

@@ -32,12 +32,12 @@ int powerset_to_multilabel(const unsigned char* cls, long long n, unsigned char*
   return B200_OK;
 }
 
-// first chunk whose window [start, start+589) may contain frame f  (start_frame is non-decreasing)
-__device__ __forceinline__ int first_chunk(const int* __restrict__ sf, int C, int f) {
+// first chunk whose window [start, start+nf) may contain frame f  (start_frame is non-decreasing)
+__device__ __forceinline__ int first_chunk(const int* __restrict__ sf, int C, int f, int nf = kFrames) {
   int lo = 0, hi = C;
   while (lo < hi) {
     const int mid = (lo + hi) >> 1;
-    if (sf[mid] + kFrames <= f) lo = mid + 1; else hi = mid;
+    if (sf[mid] + nf <= f) lo = mid + 1; else hi = mid;
   }
   return lo;
 }
@@ -64,12 +64,12 @@ int speaker_count(const unsigned char* seg, const int* sf, int C, int F, unsigne
 }
 
 // ---- generic float overlap-add: Inference.aggregate (core/inference.py:498-620) ------------------------------------
-// One thread per (frame, class) gathers the (<= 11) chunks covering the frame in ascending chunk order, i.e. in the
-// order numpy's per-chunk `+=` scatter visits them, and reproduces numpy's mixed-precision arithmetic exactly: the
-// float32 accumulators are updated as float32(float64(acc) + ((float64(score) * mask) * hamming) * warm_up), the
+// Chunks of any nf frames.  One thread per (frame, class) gathers the chunks covering the frame in ascending chunk
+// order, i.e. in the order numpy's per-chunk `+=` scatter visits them, and reproduces numpy's mixed-precision
+// arithmetic exactly: the float32 accumulators are updated as float32(float64(acc) + ((float64(score) * mask) * hamming) * warm_up), the
 // average is a float32 division by max(count, float32(epsilon)), frames no chunk contributed to get `missing`.
 __global__ void __launch_bounds__(256)
-aggregate_kernel(const float* __restrict__ scores, const int* __restrict__ sf, int C, int F, int K,
+aggregate_kernel(const float* __restrict__ scores, const int* __restrict__ sf, int C, int F, int nf, int K,
                  const double* __restrict__ hamming, const double* __restrict__ warm, int skip_average, float missing,
                  float epsilon, float* __restrict__ out) {
   const long long idx = (long long)blockIdx.x * blockDim.x + threadIdx.x;
@@ -77,9 +77,9 @@ aggregate_kernel(const float* __restrict__ scores, const int* __restrict__ sf, i
   const int f = (int)(idx / K), k = (int)(idx - (long long)f * K);
   float agg = 0.f, cnt = 0.f;
   bool any = false;
-  for (int c = first_chunk(sf, C, f); c < C && sf[c] <= f; ++c) {
+  for (int c = first_chunk(sf, C, f, nf); c < C && sf[c] <= f; ++c) {
     const int t = f - sf[c];
-    const float s = scores[((size_t)c * kFrames + t) * K + k];
+    const float s = scores[((size_t)c * nf + t) * K + k];
     const bool valid = !isnan(s);
     const double h = hamming ? hamming[t] : 1.0, w = warm ? warm[t] : 1.0;
     const double m = valid ? 1.0 : 0.0;
@@ -93,11 +93,12 @@ aggregate_kernel(const float* __restrict__ scores, const int* __restrict__ sf, i
   out[idx] = r;
 }
 
-int aggregate_scores(const float* scores, const int* sf, int C, int F, int K, const double* hamming, const double* warm,
-                     int skip_average, float missing, float epsilon, float* out, cudaStream_t stream) {
+int aggregate_scores(const float* scores, const int* sf, int C, int F, int nf, int K, const double* hamming,
+                     const double* warm, int skip_average, float missing, float epsilon, float* out,
+                     cudaStream_t stream) {
   const long long n = (long long)F * K;
-  aggregate_kernel<<<(unsigned)((n + 255) / 256), 256, 0, stream>>>(scores, sf, C, F, K, hamming, warm, skip_average,
-                                                                     missing, epsilon, out);
+  aggregate_kernel<<<(unsigned)((n + 255) / 256), 256, 0, stream>>>(scores, sf, C, F, nf, K, hamming, warm,
+                                                                     skip_average, missing, epsilon, out);
   B200_CUDA_OK(cudaGetLastError());
   return B200_OK;
 }

@@ -6,8 +6,9 @@ int speaker_count(const unsigned char* seg, const int* sf, int C, int F, unsigne
 int reconstruct(const unsigned char* seg, const signed char* hard, const int* sf, int C, int F, int Kout,
                 const unsigned char* count, unsigned char* out, cudaStream_t stream);
 int frame_transitions(const unsigned char* discrete, int F, int K, int cap, int* buf, cudaStream_t stream);
-int aggregate_scores(const float* scores, const int* sf, int C, int F, int K, const double* hamming, const double* warm,
-                     int skip_average, float missing, float epsilon, float* out, cudaStream_t stream);
+int aggregate_scores(const float* scores, const int* sf, int C, int F, int nf, int K, const double* hamming,
+                     const double* warm, int skip_average, float missing, float epsilon, float* out,
+                     cudaStream_t stream);
 int powerset_speech(const unsigned char* cls, long long n, float* out, cudaStream_t stream);
 int push_bytes(const void* src, long long bytes, void* const* dsts, int n, cudaStream_t stream);
 int clean_frames(const unsigned char* seg, int C, int* clean, unsigned char* active, cudaStream_t stream);

@@ -4,6 +4,29 @@
 
 namespace b200 {
 
+// Per-stage lengths of PyanNet on a window of W samples (models/blocks/sincnet.py:163-184): sinc conv (K 251,
+// stride 10), MaxPool 3, Conv1d 5, MaxPool 3, Conv1d 5, MaxPool 3.  W = 160000 gives the kSincLen .. kPool2 constants.
+constexpr int kSegMinWindow = 1261;  // shortest window with 2 frames (one frame cannot be instance-normalised)
+constexpr int kSegTileP = 64;        // pooled outputs per SincNet tile
+struct SegGeom {
+  int W, sinc_len, pool0, conv1_len, pool1, conv2_len, pool2;
+  int tiles0, tiles1, tiles2;        // ceil(pool / 64): tiles (and InstanceNorm partial sums) per stage
+};
+inline SegGeom seg_geom(int W) {
+  SegGeom g;
+  g.W = W;
+  g.sinc_len = 1 + (W - kSincK) / kSincStride;
+  g.pool0 = g.sinc_len / 3;
+  g.conv1_len = g.pool0 - 4;
+  g.pool1 = g.conv1_len / 3;
+  g.conv2_len = g.pool1 - 4;
+  g.pool2 = g.conv2_len / 3;
+  g.tiles0 = (g.pool0 + kSegTileP - 1) / kSegTileP;
+  g.tiles1 = (g.pool1 + kSegTileP - 1) / kSegTileP;
+  g.tiles2 = (g.pool2 + kSegTileP - 1) / kSegTileP;
+  return g;
+}
+
 struct SegWeights {
   bool loaded = false;
   int lstm_layers = 4;
@@ -43,25 +66,27 @@ int gemm_tc_split(const __half* A_hi, const __half* A_lo, int lda, const __half*
                   float* C, int ldc, __half* C_hi, __half* C_lo, int ldc_h, const float* bias, int M, int N, int K,
                   int act, int num_sms, cudaStream_t stream, float* const* C_peers = nullptr, int n_peers = 0);
 int split_f16(const float* x, __half* hi, __half* lo, size_t n, cudaStream_t st);
-// tensor-core recurrence (seg_lstm_wg.cu): Gx [NB][589][1024] -> layer output as fp16 (hi, lo) [NB][589][256]
-int lstm_rec_wg(const float* Gx, const __half* Wh, const __half* Wl, __half* Yh, __half* Yl, int NB,
+// tensor-core recurrence (seg_lstm_wg.cu): Gx [NB][T][1024] -> layer output as fp16 (hi, lo) [NB][T][256]
+int lstm_rec_wg(const float* Gx, const __half* Wh, const __half* Wl, __half* Yh, __half* Yl, int NB, int T,
                 cudaStream_t stream);
 
 // SincNet layers on the tensor cores (seg_conv_wg.cu); same outputs and partial sums as the fp32 twins
-int sinc_wg_forward(const float* wav, const long long* chunk_off, const int* chunk_valid, const float2* affine,
-                    const __half* Wh, const __half* Wl, int NB, float* P0, double2* part, int ntiles,
+int sinc_wg_forward(const SegGeom& g, const float* wav, const long long* chunk_off, const int* chunk_valid,
+                    const float2* affine, const __half* Wh, const __half* Wl, int NB, float* P0, double2* part,
                     cudaStream_t stream);
-int conv5_wg_forward(int layer, const float* Pin, const float2* affine, const __half* Wh, const __half* Wl,
-                     const float* bias, int NB, float* Pout, double2* part, int ntiles, cudaStream_t stream);
+int conv5_wg_forward(const SegGeom& g, int layer, const float* Pin, const float2* affine, const __half* Wh,
+                     const __half* Wl, const float* bias, int NB, float* Pout, double2* part, cudaStream_t stream);
 
-// SincNet front-end on NB chunks: wav + per-chunk (offset, valid) -> X0 [NB][589][64] fp32 (60 features + 4 zero pad)
-size_t sincnet_workspace_bytes(int NB);
-int sincnet_forward(const SegWeights& W, const float* wav, const long long* chunk_off, const int* chunk_valid, int NB,
-                    void* ws, float* x0, int conv_impl, cudaStream_t stream);
+// SincNet front-end on NB windows of g.W samples: wav + per-window (offset, valid) -> X0 [NB][g.pool2][64] fp32
+// (60 features + 4 zero pad)
+size_t sincnet_workspace_bytes(const SegGeom& g, int NB);
+int sincnet_launches(const SegGeom& g);   // kernels sincnet_forward launches per sub-batch
+int sincnet_forward(const SegWeights& W, const SegGeom& g, const float* wav, const long long* chunk_off,
+                    const int* chunk_valid, int NB, void* ws, float* x0, int conv_impl, cudaStream_t stream);
 
-// BiLSTM stack + linear head: X0 -> class ids [NB][589] u8 (+ optional log-probs [NB][589][7])
-size_t lstm_workspace_bytes(int NB);
-int lstm_head_forward(const SegWeights& W, const float* x0, int NB, void* ws, unsigned char* cls, float* logp,
+// BiLSTM stack + linear head on sequences of T frames: X0 -> class ids [NB][T] u8 (+ optional log-probs [NB][T][7])
+size_t lstm_workspace_bytes(int NB, int T);
+int lstm_head_forward(const SegWeights& W, const float* x0, int NB, int T, void* ws, unsigned char* cls, float* logp,
                       int num_sms, int gemm_impl, int rec_impl, cudaStream_t stream);
 
 }  // namespace b200

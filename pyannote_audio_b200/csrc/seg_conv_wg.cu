@@ -27,6 +27,7 @@ struct SincConvWgParams {
   const float* wav;
   const long long* chunk_off;
   const int* chunk_valid;
+  int W;                       // window samples: staged positions at or past W are zero
   const float2* affine;        // sinc: per-chunk waveform InstanceNorm; Conv1d: per (chunk, input channel)
   // Conv1d input
   const float* Pin;            // [B][CIN][Lin]
@@ -79,7 +80,7 @@ sinc_conv_wg_kernel(const __grid_constant__ CUtensorMap tmWh, const __grid_const
     for (int i = tid; i < kIn; i += kSCThreads) {
       const int g = s0 + i;
       const float rv = (g < valid) ? __ldg(x + g) : 0.f;
-      const float v = (g < kChunk) ? fmaf(rv, af.x, af.y) : 0.f;
+      const float v = (g < p.W) ? fmaf(rv, af.x, af.y) : 0.f;
       const __half h = __float2half_rn(v);
       xh[i] = h;
       xl[i] = __float2half_rn(v - __half2float(h));
@@ -187,7 +188,7 @@ static int make_w_map(CUtensorMap* tm, const __half* ptr, int rows, int K) {
 }
 
 template <int CIN, int CPAD, int NW, int NREAL, int KT>
-static int launch_sc(const __half* Wh, const __half* Wl, SincConvWgParams p, int NB, int Lconv, cudaStream_t stream) {
+static int launch_sc(const __half* Wh, const __half* Wl, SincConvWgParams p, int NB, cudaStream_t stream) {
   constexpr int kIn = CIN == 0 ? (kSCPos - 1) * kSincStride + KT : (kSCPos + 4) * CPAD;
   constexpr int kBoxes = (KT + 63) / 64;
   p.xs_bytes = (uint32_t)align_up((size_t)kIn * 2 * sizeof(__half), 1024);
@@ -209,33 +210,30 @@ static int launch_sc(const __half* Wh, const __half* Wl, SincConvWgParams p, int
     B200_CUDA_OK(cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
     attr_set = true;
   }
-  kernel<<<dim3(ceil_div(Lconv, kSCPos), NB), kSCThreads, smem, stream>>>(th, tl, p);
+  kernel<<<dim3(p.ntiles, NB), kSCThreads, smem, stream>>>(th, tl, p);   // one tile per 64 pooled outputs
   B200_CUDA_OK(cudaGetLastError());
   return B200_OK;
 }
 
-int sinc_wg_forward(const float* wav, const long long* chunk_off, const int* chunk_valid, const float2* affine,
-                    const __half* Wh, const __half* Wl, int NB, float* P0, double2* part, int ntiles,
+int sinc_wg_forward(const SegGeom& g, const float* wav, const long long* chunk_off, const int* chunk_valid,
+                    const float2* affine, const __half* Wh, const __half* Wl, int NB, float* P0, double2* part,
                     cudaStream_t stream) {
   SincConvWgParams p{};
-  p.wav = wav; p.chunk_off = chunk_off; p.chunk_valid = chunk_valid; p.affine = affine;
-  p.Pout = P0; p.part = part; p.Lp = kPool0; p.ntiles = ntiles;
-  B200_CHECK(ceil_div(kSincLen, kSCPos) == ntiles, B200_ERR_STATE, "sinc tiles: %d", ntiles);
-  return launch_sc<0, 1, 80, 80, 256>(Wh, Wl, p, NB, kSincLen, stream);
+  p.wav = wav; p.chunk_off = chunk_off; p.chunk_valid = chunk_valid; p.W = g.W; p.affine = affine;
+  p.Pout = P0; p.part = part; p.Lp = g.pool0; p.ntiles = g.tiles0;
+  return launch_sc<0, 1, 80, 80, 256>(Wh, Wl, p, NB, stream);
 }
 
-int conv5_wg_forward(int layer, const float* Pin, const float2* affine, const __half* Wh, const __half* Wl,
-                     const float* bias, int NB, float* Pout, double2* part, int ntiles, cudaStream_t stream) {
+int conv5_wg_forward(const SegGeom& g, int layer, const float* Pin, const float2* affine, const __half* Wh,
+                     const __half* Wl, const float* bias, int NB, float* Pout, double2* part, cudaStream_t stream) {
   SincConvWgParams p{};
-  p.affine = affine; p.bias = bias; p.Pout = Pout; p.part = part; p.ntiles = ntiles;
+  p.affine = affine; p.bias = bias; p.Pout = Pout; p.part = part; p.Pin = Pin;
   if (layer == 0) {
-    p.Pin = Pin; p.Lin = kPool0; p.Lp = kPool1;
-    B200_CHECK(ceil_div(kConv1Len, kSCPos) == ntiles, B200_ERR_STATE, "conv1 tiles: %d", ntiles);
-    return launch_sc<80, 80, 64, 60, 400>(Wh, Wl, p, NB, kConv1Len, stream);
+    p.Lin = g.pool0; p.Lp = g.pool1; p.ntiles = g.tiles1;
+    return launch_sc<80, 80, 64, 60, 400>(Wh, Wl, p, NB, stream);
   }
-  p.Pin = Pin; p.Lin = kPool1; p.Lp = kPool2;
-  B200_CHECK(ceil_div(kConv2Len, kSCPos) == ntiles, B200_ERR_STATE, "conv2 tiles: %d", ntiles);
-  return launch_sc<60, 64, 64, 60, 320>(Wh, Wl, p, NB, kConv2Len, stream);
+  p.Lin = g.pool1; p.Lp = g.pool2; p.ntiles = g.tiles2;
+  return launch_sc<60, 64, 64, 60, 320>(Wh, Wl, p, NB, stream);
 }
 
 }  // namespace b200

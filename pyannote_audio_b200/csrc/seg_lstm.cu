@@ -7,7 +7,7 @@
 // Per layer: (1) input projection for both directions as one fp32 GEMM (sgemm.cu) into Gx[b][t][1024] with column
 // order (dir, unit, gate) and both biases folded; (2) the recurrence as a persistent kernel on a 2-CTA cluster:
 // each CTA keeps the W_hh slice of 64 hidden units (all 4 gates, 128 KB fp32) resident in shared memory for the
-// whole 589-step chunk, computes its gates for a tile of NBT sequences, updates c/h in registers and publishes
+// whole T-step window, computes its gates for a tile of NBT sequences, updates c/h in registers and publishes
 // its h slice into BOTH CTAs' shared memory (DSMEM), one cluster barrier per step.
 #include "common.cuh"
 #include "seg.cuh"
@@ -24,9 +24,9 @@ __device__ __forceinline__ float sigmoidf_(float x) { return 1.f / (1.f + expf(-
 // unit 64*rank + 2*tx + p, gates i,f,g,o at smem columns p*128 + tx*4 + gate.
 template <int RB>
 __global__ void __cluster_dims__(2, 1, 1) __launch_bounds__(256, 1)
-lstm_rec_kernel(const float* __restrict__ Gx /*[NB][589][1024]*/, const float* __restrict__ Whh /*[2][2][128][256]*/,
-                float* __restrict__ Y /*[NB][589][256] or null*/, __half* __restrict__ Yh, __half* __restrict__ Yl,
-                int NB, int ntiles) {
+lstm_rec_kernel(const float* __restrict__ Gx /*[NB][T][1024]*/, const float* __restrict__ Whh /*[2][2][128][256]*/,
+                float* __restrict__ Y /*[NB][T][256] or null*/, __half* __restrict__ Yh, __half* __restrict__ Yl,
+                int NB, int T, int ntiles) {
   constexpr int NBT = 8 * RB;
   extern __shared__ float sm[];
   float* Ws = sm;                         // [128][256]
@@ -57,7 +57,7 @@ lstm_rec_kernel(const float* __restrict__ Gx /*[NB][589][1024]*/, const float* _
     for (int r = 0; r < RB; ++r) {
       const int b = b0 + r;
       if (b < NB) {
-        const float4* p = reinterpret_cast<const float4*>(Gx + ((size_t)b * kFrames + t) * 1024 + gcol);
+        const float4* p = reinterpret_cast<const float4*>(Gx + ((size_t)b * T + t) * 1024 + gcol);
         const float4 u = __ldg(p), v = __ldg(p + 1);
         dst[r][0] = u.x; dst[r][1] = u.y; dst[r][2] = u.z; dst[r][3] = u.w;
         dst[r][4] = v.x; dst[r][5] = v.y; dst[r][6] = v.z; dst[r][7] = v.w;
@@ -67,11 +67,11 @@ lstm_rec_kernel(const float* __restrict__ Gx /*[NB][589][1024]*/, const float* _
       }
     }
   };
-  load_gx(dir ? kFrames - 1 : 0, gx);
+  load_gx(dir ? T - 1 : 0, gx);
   cluster.sync();
 
-  for (int step = 0; step < kFrames; ++step) {
-    const int t = dir ? (kFrames - 1 - step) : step;
+  for (int step = 0; step < T; ++step) {
+    const int t = dir ? (T - 1 - step) : step;
     const float* hcur = hb + (step & 1) * 128 * NBT;
     float* hnext = hb + ((step + 1) & 1) * 128 * NBT;
     float* hnext_peer = hb_peer + ((step + 1) & 1) * 128 * NBT;
@@ -80,7 +80,7 @@ lstm_rec_kernel(const float* __restrict__ Gx /*[NB][589][1024]*/, const float* _
     for (int r = 0; r < RB; ++r)
 #pragma unroll
       for (int j = 0; j < 8; ++j) acc[r][j] = gx[r][j];
-    if (step + 1 < kFrames) load_gx(dir ? t - 1 : t + 1, gx);      // prefetch next step's input projection
+    if (step + 1 < T) load_gx(dir ? t - 1 : t + 1, gx);      // prefetch next step's input projection
 
 #pragma unroll 4
     for (int k = 0; k < 128; ++k) {
@@ -124,7 +124,7 @@ lstm_rec_kernel(const float* __restrict__ Gx /*[NB][589][1024]*/, const float* _
       }
       const int b = b0 + r;
       if (b < NB) {
-        const size_t o = ((size_t)b * kFrames + t) * 256 + dir * 128 + rank * 64 + 2 * tx;
+        const size_t o = ((size_t)b * T + t) * 256 + dir * 128 + rank * 64 + 2 * tx;
         if (Y) *reinterpret_cast<float2*>(Y + o) = make_float2(hn[0], hn[1]);
         if (Yh) {   // fp16 (hi, lo) split consumed by the tensor-core GEMM of the next layer
           const __half h0 = __float2half_rn(hn[0]), h1 = __float2half_rn(hn[1]);
@@ -188,7 +188,7 @@ struct LstmWs {
   float *Gx, *Ya, *Yb, *Z1, *Z2;
   __half *Xh, *Xl, *Yah, *Yal, *Ybh, *Ybl, *Z1h, *Z1l;
 };
-static size_t carve_lstm(int NB, void* base, LstmWs* w) {
+static size_t carve_lstm(int NB, int T, void* base, LstmWs* w) {
   size_t off = 0;
   auto take = [&](size_t bytes) {
     off = align_up(off, 256);
@@ -197,7 +197,7 @@ static size_t carve_lstm(int NB, void* base, LstmWs* w) {
     return p;
   };
   LstmWs t;
-  const size_t M = (size_t)NB * kFrames;
+  const size_t M = (size_t)NB * T;
   t.Gx = (float*)take(M * 1024 * sizeof(float));
   t.Ya = (float*)take(M * 256 * sizeof(float));
   t.Yb = (float*)take(M * 256 * sizeof(float));
@@ -214,25 +214,25 @@ static size_t carve_lstm(int NB, void* base, LstmWs* w) {
   if (w) *w = t;
   return align_up(off, 256);
 }
-size_t lstm_workspace_bytes(int NB) { return carve_lstm(NB, nullptr, nullptr); }
+size_t lstm_workspace_bytes(int NB, int T) { return carve_lstm(NB, T, nullptr, nullptr); }
 
 template <int RB>
-static int launch_rec(const float* Gx, const float* Whh, float* Y, __half* Yh, __half* Yl, int NB,
+static int launch_rec(const float* Gx, const float* Whh, float* Y, __half* Yh, __half* Yl, int NB, int T,
                       cudaStream_t stream) {
   constexpr int NBT = 8 * RB;
   const int ntiles = ceil_div(NB, NBT);
   const size_t smem = (128 * 256 + 2 * 128 * NBT) * sizeof(float);
   B200_CUDA_OK(cudaFuncSetAttribute(lstm_rec_kernel<RB>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-  lstm_rec_kernel<RB><<<2 * 2 * ntiles, 256, smem, stream>>>(Gx, Whh, Y, Yh, Yl, NB, ntiles);
+  lstm_rec_kernel<RB><<<2 * 2 * ntiles, 256, smem, stream>>>(Gx, Whh, Y, Yh, Yl, NB, T, ntiles);
   B200_CUDA_OK(cudaGetLastError());
   return B200_OK;
 }
 
-int lstm_head_forward(const SegWeights& W, const float* x0, int NB, void* ws, unsigned char* cls, float* logp,
+int lstm_head_forward(const SegWeights& W, const float* x0, int NB, int T, void* ws, unsigned char* cls, float* logp,
                       int num_sms, int gemm_impl, int rec_impl, cudaStream_t stream) {
   LstmWs w;
-  carve_lstm(NB, ws, &w);
-  const int M = NB * kFrames;
+  carve_lstm(NB, T, ws, &w);
+  const int M = NB * T;          // rows of every GEMM (< 2^31); element offsets M * 1024 are formed in size_t
   const int clusters = num_sms / 2;
   const bool tc = gemm_impl != 0;
   int rc;
@@ -250,7 +250,7 @@ int lstm_head_forward(const SegWeights& W, const float* x0, int NB, void* ws, un
       rc = sgemm_nt(in, W.k_in[l], W.w_ih[l], W.k_in[l], w.Gx, 1024, W.b_g[l], M, 1024, W.k_in[l], 0, stream);
     if (rc) return rc;
     if (tc && rec_impl == 1) {   // tensor-core recurrence (seg_lstm_wg.cu)
-      if ((rc = lstm_rec_wg(w.Gx, W.w_hh_hi[l], W.w_hh_lo[l], outs_h[l & 1], outs_l[l & 1], NB, stream))) return rc;
+      if ((rc = lstm_rec_wg(w.Gx, W.w_hh_hi[l], W.w_hh_lo[l], outs_h[l & 1], outs_l[l & 1], NB, T, stream))) return rc;
       in_h = outs_h[l & 1]; in_l = outs_l[l & 1];
       continue;
     }
@@ -258,9 +258,9 @@ int lstm_head_forward(const SegWeights& W, const float* x0, int NB, void* ws, un
     __half* yh = tc ? outs_h[l & 1] : nullptr;
     __half* yl = tc ? outs_l[l & 1] : nullptr;
     // largest batch tile that still fills the machine with 2-CTA clusters
-    if (2 * ceil_div(NB, 64) >= clusters) rc = launch_rec<8>(w.Gx, W.w_hh[l], y, yh, yl, NB, stream);
-    else if (2 * ceil_div(NB, 32) >= clusters) rc = launch_rec<4>(w.Gx, W.w_hh[l], y, yh, yl, NB, stream);
-    else rc = launch_rec<2>(w.Gx, W.w_hh[l], y, yh, yl, NB, stream);
+    if (2 * ceil_div(NB, 64) >= clusters) rc = launch_rec<8>(w.Gx, W.w_hh[l], y, yh, yl, NB, T, stream);
+    else if (2 * ceil_div(NB, 32) >= clusters) rc = launch_rec<4>(w.Gx, W.w_hh[l], y, yh, yl, NB, T, stream);
+    else rc = launch_rec<2>(w.Gx, W.w_hh[l], y, yh, yl, NB, T, stream);
     if (rc) return rc;
     in = y; in_h = yh; in_l = yl;
   }

@@ -33,8 +33,8 @@ __device__ __forceinline__ uint32_t pack_h2(float a, float b) {
 
 __global__ void __cluster_dims__(2, 1, 1) __launch_bounds__(kRecThreads, 1)
 lstm_rec_wg_kernel(const __grid_constant__ CUtensorMap tmWh, const __grid_constant__ CUtensorMap tmWl,
-                   const float* __restrict__ Gx /*[NB][589][1024]*/, __half* __restrict__ Yh, __half* __restrict__ Yl,
-                   int NB, int ntiles) {
+                   const float* __restrict__ Gx /*[NB][T][1024]*/, __half* __restrict__ Yh, __half* __restrict__ Yl,
+                   int NB, int T, int ntiles) {
   extern __shared__ uint8_t smem_raw[];
   const uint32_t raw = smem_u32(smem_raw);
   const uint32_t base = (raw + 1023u) & ~1023u;
@@ -74,13 +74,13 @@ lstm_rec_wg_kernel(const __grid_constant__ CUtensorMap tmWh, const __grid_consta
   const int gcol = dir * 512 + ((int)rank * 64 + 2 * q) * 4;   // + 32 jj: units 8 jj + 2q, +1, four gates each
 
   float acc[128];
-  for (int step = 0; step < kFrames; ++step) {
-    const int t = dir ? (kFrames - 1 - step) : step;
+  for (int step = 0; step < T; ++step) {
+    const int t = dir ? (T - 1 - step) : step;
     // acc = Gx[b][t] (the input projection with both biases)
 #pragma unroll
     for (int i = 0; i < 2; ++i) {
       const bool ok = rows[i] < NB;
-      const float4* gp = reinterpret_cast<const float4*>(Gx + ((size_t)(ok ? rows[i] : 0) * kFrames + t) * 1024 + gcol);
+      const float4* gp = reinterpret_cast<const float4*>(Gx + ((size_t)(ok ? rows[i] : 0) * T + t) * 1024 + gcol);
 #pragma unroll
       for (int jj = 0; jj < 8; ++jj) {
         const float4 u0 = ok ? __ldg(gp + 8 * jj) : make_float4(0.f, 0.f, 0.f, 0.f);
@@ -91,9 +91,9 @@ lstm_rec_wg_kernel(const __grid_constant__ CUtensorMap tmWh, const __grid_consta
 #pragma unroll
           for (int e = 0; e < 2; ++e) acc[4 * (4 * jj + g) + 2 * i + e] = v[4 * e + g];
       }
-      if (step + 1 < kFrames && ok) {                     // next step's projection into L2
+      if (step + 1 < T && ok) {                     // next step's projection into L2
         const int tn = dir ? t - 1 : t + 1;
-        const char* np = reinterpret_cast<const char*>(Gx + ((size_t)rows[i] * kFrames + tn) * 1024 + gcol);
+        const char* np = reinterpret_cast<const char*>(Gx + ((size_t)rows[i] * T + tn) * 1024 + gcol);
 #pragma unroll
         for (int jj = 0; jj < 8; ++jj) asm volatile("prefetch.global.L2 [%0];" ::"l"(np + 128 * jj));
       }
@@ -148,7 +148,7 @@ lstm_rec_wg_kernel(const __grid_constant__ CUtensorMap tmWh, const __grid_consta
         asm volatile("st.shared::cluster.u32 [%0], %1;" ::"r"(px + (uint32_t)((16 + i * 8 + jj) * kRecThreads) * 4u),
                      "r"(vl) : "memory");
         if (rows[i] < NB) {
-          const size_t o = ((size_t)rows[i] * kFrames + t) * 256 + dir * 128 + rank * 64 + 8 * jj + 2 * q;
+          const size_t o = ((size_t)rows[i] * T + t) * 256 + dir * 128 + rank * 64 + 8 * jj + 2 * q;
           *reinterpret_cast<uint32_t*>(Yh + o) = vh;
           *reinterpret_cast<uint32_t*>(Yl + o) = vl;
         }
@@ -159,7 +159,7 @@ lstm_rec_wg_kernel(const __grid_constant__ CUtensorMap tmWh, const __grid_consta
   }
 }
 
-int lstm_rec_wg(const float* Gx, const __half* Wh, const __half* Wl, __half* Yh, __half* Yl, int NB,
+int lstm_rec_wg(const float* Gx, const __half* Wh, const __half* Wl, __half* Yh, __half* Yl, int NB, int T,
                 cudaStream_t stream) {
   PFN_encodeTiled enc = get_encode();
   B200_CHECK(enc != nullptr, B200_ERR_CUDA, "cuTensorMapEncodeTiled not available from the driver");
@@ -181,7 +181,7 @@ int lstm_rec_wg(const float* Gx, const __half* Wh, const __half* Wl, __half* Yh,
     attr_set = true;
   }
   const int ntiles = ceil_div(NB, kRecSeqs);
-  lstm_rec_wg_kernel<<<2 * 2 * ntiles, kRecThreads, smem, stream>>>(tm[0], tm[1], Gx, Yh, Yl, NB, ntiles);
+  lstm_rec_wg_kernel<<<2 * 2 * ntiles, kRecThreads, smem, stream>>>(tm[0], tm[1], Gx, Yh, Yl, NB, T, ntiles);
   B200_CUDA_OK(cudaGetLastError());
   return B200_OK;
 }

@@ -4,12 +4,13 @@
 //   wav_norm1d (InstanceNorm1d(1, affine), instance stats, biased var, eps 1e-5)
 //   -> 80 sinc band-pass FIRs (K=251, stride 10) -> |.| -> MaxPool1d(3,3) -> InstanceNorm1d(80) -> leaky_relu
 //   -> Conv1d(80,60,5) -> MaxPool -> InstanceNorm1d(60) -> leaky_relu
-//   -> Conv1d(60,60,5) -> MaxPool -> InstanceNorm1d(60) -> leaky_relu            => (B,60,589)
+//   -> Conv1d(60,60,5) -> MaxPool -> InstanceNorm1d(60) -> leaky_relu            => (B,60,F), F = 589 for 10 s
 //
-// Kernel plan (each InstanceNorm needs whole-chunk statistics, so every stage ends in per-tile partial sums and
-// the normalisation + leaky_relu is applied by the *consumer* when it loads its input tile):
+// Kernel plan for windows of any length W (SegGeom).  Each InstanceNorm needs whole-window statistics, so every stage
+// ends in per-tile partial sums and the normalisation + leaky_relu is applied by the *consumer* when it loads its
+// input tile:
 //   wav_stats -> sinc_pool -> in_finalize -> conv5_pool<80> -> in_finalize -> conv5_pool<60> -> in_finalize
-//   -> in_apply_transpose (writes the LSTM input [B][589][64], zero-padded 60->64).
+//   -> in_apply_transpose (writes the LSTM input [B][F][64], zero-padded 60->64).
 // The sinc filters are (anti)symmetric (cos bank even, sin bank odd), which halves the multiplies:
 //   cos: sum_k<125 f[k]*(x[a+k]+x[a+250-k]) + f[125]*x[a+125];  sin: sum_k<125 f[k]*(x[a+k]-x[a+250-k]).
 #include "common.cuh"
@@ -17,21 +18,35 @@
 
 namespace b200 {
 
-constexpr int kTileP = 64;                          // pooled outputs per tile
-constexpr int kTiles0 = (kPool0 + kTileP - 1) / kTileP;   // 84
-constexpr int kTiles1 = (kPool1 + kTileP - 1) / kTileP;   // 28
-constexpr int kTiles2 = (kPool2 + kTileP - 1) / kTileP;   // 10
+constexpr int kTileP = kSegTileP;                   // pooled outputs per tile
+constexpr int kWavSlice = kChunk;                   // samples per wav_stats block (a 10 s window is one block)
+constexpr int kFinGroup = 128;                      // partial sums one thread combines per InstanceNorm level
 
-// ---- per-chunk waveform statistics -> affine (scale, shift) --------------------------------------
+// ---- per-window waveform statistics -> affine (scale, shift) -------------------------------------
+// Every InstanceNorm normalises over the whole padded window: the zero padding counts, so the denominators are W.
+__device__ __forceinline__ float2 wav_affine(double S, double SS, int W, float gamma, float beta) {
+  const double mean = S / W;                           // zero padding counts (the reference pads, then normalises)
+  double var = SS / W - mean * mean;
+  if (var < 0) var = 0;
+  const float rstd = (float)(1.0 / sqrt(var + 1e-5));
+  const float sc = gamma * rstd;
+  return make_float2(sc, beta - (float)mean * sc);
+}
+
+// grid (ceil(W / kWavSlice), NB): block (slice, b) sums the real samples of one slice.  With one slice the block
+// writes the affine itself; otherwise it writes (sum, sum of squares) and wav_finalize_kernel combines the slices
+// in slice order, so a window's result does not depend on the other windows of its sub-batch.
 __global__ void __launch_bounds__(512) wav_stats_kernel(const float* __restrict__ wav,
                                                         const long long* __restrict__ chunk_off,
-                                                        const int* __restrict__ chunk_valid, float gamma, float beta,
-                                                        float2* __restrict__ affine) {
-  const int b = blockIdx.x;
+                                                        const int* __restrict__ chunk_valid, int W, float gamma,
+                                                        float beta, float2* __restrict__ affine,
+                                                        double2* __restrict__ part) {
+  const int slice = blockIdx.x, b = blockIdx.y, nslices = gridDim.x;
   const float* x = wav + chunk_off[b];
-  const int valid = chunk_valid[b];
+  const int lo = slice * kWavSlice;
+  const int hi = (int)min((long long)chunk_valid[b], (long long)lo + kWavSlice);
   double s = 0.0, ss = 0.0;
-  for (int i = threadIdx.x; i < valid; i += blockDim.x) {
+  for (int i = lo + threadIdx.x; i < hi; i += blockDim.x) {
     const double v = x[i];
     s += v;
     ss += v * v;
@@ -46,13 +61,22 @@ __global__ void __launch_bounds__(512) wav_stats_kernel(const float* __restrict_
   if (threadIdx.x == 0) {
     double S = 0, SS = 0;
     for (int i = 0; i < 16; ++i) { S += sh[0][i]; SS += sh[1][i]; }
-    const double mean = S / kChunk;                      // zero padding counts (the reference pads, then normalises)
-    double var = SS / kChunk - mean * mean;
-    if (var < 0) var = 0;
-    const float rstd = (float)(1.0 / sqrt(var + 1e-5));
-    const float sc = gamma * rstd;
-    affine[b] = make_float2(sc, beta - (float)mean * sc);
+    if (nslices == 1) affine[b] = wav_affine(S, SS, W, gamma, beta);
+    else part[(size_t)b * nslices + slice] = make_double2(S, SS);
   }
+}
+
+__global__ void wav_finalize_kernel(const double2* __restrict__ part, int nslices, int W, float gamma, float beta,
+                                    float2* __restrict__ affine, int NB) {
+  const int b = blockIdx.x * blockDim.x + threadIdx.x;
+  if (b >= NB) return;
+  double S = 0, SS = 0;
+  for (int t = 0; t < nslices; ++t) {
+    const double2 p = part[(size_t)b * nslices + t];
+    S += p.x;
+    SS += p.y;
+  }
+  affine[b] = wav_affine(S, SS, W, gamma, beta);
 }
 
 // ---- sinc conv + abs + maxpool3 ------------------------------------------------------------------
@@ -63,8 +87,8 @@ __global__ void __launch_bounds__(128) sinc_pool_kernel(const float* __restrict_
                                                         const int* __restrict__ chunk_valid,
                                                         const float2* __restrict__ affine,
                                                         const float* __restrict__ filt /*[126][80]*/,
-                                                        float* __restrict__ P0 /*[B][80][5325]*/,
-                                                        double2* __restrict__ part /*[B][80][kTiles0]*/) {
+                                                        int W, float* __restrict__ P0 /*[B][80][Lp]*/, int Lp,
+                                                        int ntiles, double2* __restrict__ part /*[B][80][ntiles]*/) {
   extern __shared__ float sm[];
   float* xs = sm;                    // 2176
   float* fs = sm + 2176;             // 126*80
@@ -79,7 +103,7 @@ __global__ void __launch_bounds__(128) sinc_pool_kernel(const float* __restrict_
   for (int i = tid; i < 2176; i += 128) {
     const int g = s0 + i;
     const float raw = (g < valid) ? x[g] : 0.f;
-    xs[i] = (g < kChunk) ? fmaf(raw, af.x, af.y) : 0.f;
+    xs[i] = (g < W) ? fmaf(raw, af.x, af.y) : 0.f;
   }
   for (int i = tid; i < 126 * 80 / 4; i += 128)
     reinterpret_cast<float4*>(fs)[i] = reinterpret_cast<const float4*>(filt)[i];
@@ -140,7 +164,7 @@ __global__ void __launch_bounds__(128) sinc_pool_kernel(const float* __restrict_
   __syncthreads();                   // everyone done with fs -> reuse as pooled tile [80][65]
   float* pt = fs;
   const int pglob = tile * kTileP + j;
-  const bool ok = pglob < kPool0;
+  const bool ok = pglob < Lp;
 #pragma unroll
   for (int c = 0; c < 20; ++c) {
     const float vc = fmaxf(fmaxf(fabsf(ac[0][c]), fabsf(ac[1][c])), fabsf(ac[2][c]));
@@ -149,8 +173,8 @@ __global__ void __launch_bounds__(128) sinc_pool_kernel(const float* __restrict_
     pt[chc * 65 + j] = ok ? vc : 0.f;
     pt[chs * 65 + j] = ok ? vs : 0.f;
     if (ok) {
-      P0[((size_t)b * 80 + chc) * kPool0 + pglob] = vc;
-      P0[((size_t)b * 80 + chs) * kPool0 + pglob] = vs;
+      P0[((size_t)b * 80 + chc) * Lp + pglob] = vc;
+      P0[((size_t)b * 80 + chs) * Lp + pglob] = vs;
     }
   }
   __syncthreads();
@@ -161,7 +185,7 @@ __global__ void __launch_bounds__(128) sinc_pool_kernel(const float* __restrict_
       s += v;
       ss += v * v;
     }
-    part[((size_t)b * 80 + tid) * kTiles0 + tile] = make_double2(s, ss);
+    part[((size_t)b * 80 + tid) * ntiles + tile] = make_double2(s, ss);
   }
 }
 
@@ -184,6 +208,40 @@ __global__ void in_finalize_kernel(const double2* __restrict__ part, int ntiles,
   const float rstd = (float)(1.0 / sqrt(var + 1e-5));
   const float sc = gamma[c] * rstd;
   affine[idx] = make_float2(sc, beta[c] - (float)mean * sc);
+}
+
+// Long windows have thousands of tiles per (window, channel): one level of the reduction combines the partial sums
+// of kFinGroup consecutive tiles, in tile order, per thread.
+__global__ void part_reduce_kernel(const double2* __restrict__ in, int n_in, double2* __restrict__ out, int n_out,
+                                   int rows) {
+  const int idx = blockIdx.x * blockDim.x + threadIdx.x;
+  if (idx >= rows * n_out) return;
+  const int row = idx / n_out, g = idx - row * n_out;
+  const double2* p = in + (size_t)row * n_in + (size_t)g * kFinGroup;
+  const int n = min(kFinGroup, n_in - g * kFinGroup);
+  double s = 0, ss = 0;
+  for (int t = 0; t < n; ++t) {
+    s += p[t].x;
+    ss += p[t].y;
+  }
+  out[idx] = make_double2(s, ss);
+}
+
+// partial sums [rows][ntiles] -> affine [rows]; up to kFinGroup tiles (every stage of a 10 s window) take the single
+// in_finalize_kernel pass, more are first combined in groups into red0 / red1 (ping-pong)
+static void in_stats(const double2* part, int ntiles, double2* red0, double2* red1, int n, int C, const float* gamma,
+                     const float* beta, float2* affine, int rows, cudaStream_t stream) {
+  const double2* cur = part;
+  double2* bufs[2] = {red0, red1};
+  int k = 0;
+  while (ntiles > kFinGroup) {
+    const int n_out = ceil_div(ntiles, kFinGroup);
+    part_reduce_kernel<<<ceil_div(rows * n_out, 256), 256, 0, stream>>>(cur, ntiles, bufs[k], n_out, rows);
+    cur = bufs[k];
+    ntiles = n_out;
+    k ^= 1;
+  }
+  in_finalize_kernel<<<ceil_div(rows, 128), 128, 0, stream>>>(cur, ntiles, n, C, gamma, beta, affine, rows);
 }
 
 // ---- Conv1d(CIN,60,5) + maxpool3 on the normalised, leaky-relu'd input --------------------------------
@@ -274,19 +332,19 @@ __global__ void __launch_bounds__(192) conv5_pool_kernel(const float* __restrict
   }
 }
 
-// ---- final InstanceNorm + leaky_relu + transpose to the LSTM input layout [B][589][64] ----------------
+// ---- final InstanceNorm + leaky_relu + transpose to the LSTM input layout [B][T][64] -----------------
 __global__ void in_apply_transpose_kernel(const float* __restrict__ P2, const float2* __restrict__ affine,
-                                          float* __restrict__ x0, int NB) {
+                                          float* __restrict__ x0, int NB, int T) {
   const size_t idx = (size_t)blockIdx.x * blockDim.x + threadIdx.x;
-  const size_t total = (size_t)NB * kFrames * 64;
+  const size_t total = (size_t)NB * T * 64;
   if (idx >= total) return;
   const int c = idx & 63;
-  const int t = (idx >> 6) % kFrames;
-  const int b = idx / ((size_t)kFrames * 64);
+  const int row = (int)(idx >> 6);
+  const int b = row / T, t = row - b * T;
   float v = 0.f;
   if (c < 60) {
     const float2 af = affine[b * 60 + c];
-    v = fmaf(P2[((size_t)b * 60 + c) * kPool2 + t], af.x, af.y);
+    v = fmaf(P2[((size_t)b * 60 + c) * T + t], af.x, af.y);
     v = v > 0.f ? v : 0.01f * v;
   }
   x0[idx] = v;
@@ -295,11 +353,13 @@ __global__ void in_apply_transpose_kernel(const float* __restrict__ P2, const fl
 // ---- host ------------------------------------------------------------------------------------------
 struct SincWs {
   float2 *af_wav, *af0, *af1, *af2;
-  double2 *part0, *part1, *part2;
+  double2 *wav_part, *part0, *part1, *part2, *red0, *red1;
   float *P0, *P1, *P2;
 };
 
-static size_t carve(int NB, void* base, SincWs* w) {
+static int wav_slices(const SegGeom& g) { return ceil_div(g.W, kWavSlice); }
+
+static size_t carve(const SegGeom& g, int NB, void* base, SincWs* w) {
   size_t off = 0;
   auto take = [&](size_t bytes) {
     off = align_up(off, 256);
@@ -312,22 +372,37 @@ static size_t carve(int NB, void* base, SincWs* w) {
   t.af0 = (float2*)take(sizeof(float2) * NB * 80);
   t.af1 = (float2*)take(sizeof(float2) * NB * 60);
   t.af2 = (float2*)take(sizeof(float2) * NB * 60);
-  t.part0 = (double2*)take(sizeof(double2) * (size_t)NB * 80 * kTiles0);
-  t.part1 = (double2*)take(sizeof(double2) * (size_t)NB * 60 * kTiles1);
-  t.part2 = (double2*)take(sizeof(double2) * (size_t)NB * 60 * kTiles2);
-  t.P0 = (float*)take(sizeof(float) * (size_t)NB * 80 * kPool0);
-  t.P1 = (float*)take(sizeof(float) * (size_t)NB * 60 * kPool1);
-  t.P2 = (float*)take(sizeof(float) * (size_t)NB * 60 * kPool2);
+  t.part0 = (double2*)take(sizeof(double2) * (size_t)NB * 80 * g.tiles0);
+  t.part1 = (double2*)take(sizeof(double2) * (size_t)NB * 60 * g.tiles1);
+  t.part2 = (double2*)take(sizeof(double2) * (size_t)NB * 60 * g.tiles2);
+  t.P0 = (float*)take(sizeof(float) * (size_t)NB * 80 * g.pool0);
+  t.P1 = (float*)take(sizeof(float) * (size_t)NB * 60 * g.pool1);
+  t.P2 = (float*)take(sizeof(float) * (size_t)NB * 60 * g.pool2);
+  t.wav_part = nullptr;
+  t.red0 = t.red1 = nullptr;
+  if (wav_slices(g) > 1) t.wav_part = (double2*)take(sizeof(double2) * (size_t)NB * wav_slices(g));
+  if (g.tiles0 > kFinGroup) {   // the largest stage's first reduction level; later levels are smaller
+    const size_t n = (size_t)NB * 80 * ceil_div(g.tiles0, kFinGroup);
+    t.red0 = (double2*)take(sizeof(double2) * n);
+    t.red1 = (double2*)take(sizeof(double2) * n);
+  }
   if (w) *w = t;
   return align_up(off, 256);
 }
 
-size_t sincnet_workspace_bytes(int NB) { return carve(NB, nullptr, nullptr); }
+size_t sincnet_workspace_bytes(const SegGeom& g, int NB) { return carve(g, NB, nullptr, nullptr); }
 
-int sincnet_forward(const SegWeights& W, const float* wav, const long long* chunk_off, const int* chunk_valid, int NB,
-                    void* ws, float* x0, int conv_impl, cudaStream_t stream) {
+int sincnet_launches(const SegGeom& g) {
+  int n = 8 + (wav_slices(g) > 1);
+  for (int t : {g.tiles0, g.tiles1, g.tiles2})
+    for (; t > kFinGroup; t = ceil_div(t, kFinGroup)) ++n;
+  return n;
+}
+
+int sincnet_forward(const SegWeights& W, const SegGeom& g, const float* wav, const long long* chunk_off,
+                    const int* chunk_valid, int NB, void* ws, float* x0, int conv_impl, cudaStream_t stream) {
   SincWs w;
-  carve(NB, ws, &w);
+  carve(g, NB, ws, &w);
   static bool attr = false;
   const size_t smem_sinc = (2176 + 126 * 80) * sizeof(float);
   const size_t smem_c80 = (80 * 196 + 20 * 300) * sizeof(float);
@@ -338,41 +413,43 @@ int sincnet_forward(const SegWeights& W, const float* wav, const long long* chun
     B200_CUDA_OK(cudaFuncSetAttribute(conv5_pool_kernel<60>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem_c60));
     attr = true;
   }
-  wav_stats_kernel<<<NB, 512, 0, stream>>>(wav, chunk_off, chunk_valid, W.wav_w, W.wav_b, w.af_wav);
+  const int nslices = wav_slices(g);
+  wav_stats_kernel<<<dim3(nslices, NB), 512, 0, stream>>>(wav, chunk_off, chunk_valid, g.W, W.wav_w, W.wav_b,
+                                                          w.af_wav, w.wav_part);
+  if (nslices > 1)
+    wav_finalize_kernel<<<ceil_div(NB, 128), 128, 0, stream>>>(w.wav_part, nslices, g.W, W.wav_w, W.wav_b, w.af_wav,
+                                                               NB);
   // conv_impl: 1 = split-fp16 wgmma kernels (default), 0 = the fp32 CUDA-core twins
   int rc;
   if (conv_impl) {
-    if ((rc = sinc_wg_forward(wav, chunk_off, chunk_valid, w.af_wav, W.sinc_wg_hi, W.sinc_wg_lo, NB, w.P0, w.part0,
-                              kTiles0, stream)))
+    if ((rc = sinc_wg_forward(g, wav, chunk_off, chunk_valid, w.af_wav, W.sinc_wg_hi, W.sinc_wg_lo, NB, w.P0, w.part0,
+                              stream)))
       return rc;
   } else {
-    sinc_pool_kernel<<<dim3(kTiles0, NB), 128, smem_sinc, stream>>>(wav, chunk_off, chunk_valid, w.af_wav, W.sinc_f,
-                                                                   w.P0, w.part0);
+    sinc_pool_kernel<<<dim3(g.tiles0, NB), 128, smem_sinc, stream>>>(wav, chunk_off, chunk_valid, w.af_wav, W.sinc_f,
+                                                                    g.W, w.P0, g.pool0, g.tiles0, w.part0);
   }
-  in_finalize_kernel<<<ceil_div(NB * 80, 128), 128, 0, stream>>>(w.part0, kTiles0, kPool0, 80, W.in_gamma[0],
-                                                                 W.in_beta[0], w.af0, NB * 80);
+  in_stats(w.part0, g.tiles0, w.red0, w.red1, g.pool0, 80, W.in_gamma[0], W.in_beta[0], w.af0, NB * 80, stream);
   if (conv_impl) {
-    if ((rc = conv5_wg_forward(0, w.P0, w.af0, W.conv_wg_hi[0], W.conv_wg_lo[0], W.conv_b[0], NB, w.P1, w.part1,
-                               kTiles1, stream)))
+    if ((rc = conv5_wg_forward(g, 0, w.P0, w.af0, W.conv_wg_hi[0], W.conv_wg_lo[0], W.conv_b[0], NB, w.P1, w.part1,
+                               stream)))
       return rc;
   } else {
-    conv5_pool_kernel<80><<<dim3(kTiles1, NB), 192, smem_c80, stream>>>(w.P0, kPool0, w.af0, W.conv_w[0], W.conv_b[0],
-                                                                        w.P1, kPool1, kTiles1, w.part1);
+    conv5_pool_kernel<80><<<dim3(g.tiles1, NB), 192, smem_c80, stream>>>(w.P0, g.pool0, w.af0, W.conv_w[0],
+                                                                         W.conv_b[0], w.P1, g.pool1, g.tiles1, w.part1);
   }
-  in_finalize_kernel<<<ceil_div(NB * 60, 128), 128, 0, stream>>>(w.part1, kTiles1, kPool1, 60, W.in_gamma[1],
-                                                                 W.in_beta[1], w.af1, NB * 60);
+  in_stats(w.part1, g.tiles1, w.red0, w.red1, g.pool1, 60, W.in_gamma[1], W.in_beta[1], w.af1, NB * 60, stream);
   if (conv_impl) {
-    if ((rc = conv5_wg_forward(1, w.P1, w.af1, W.conv_wg_hi[1], W.conv_wg_lo[1], W.conv_b[1], NB, w.P2, w.part2,
-                               kTiles2, stream)))
+    if ((rc = conv5_wg_forward(g, 1, w.P1, w.af1, W.conv_wg_hi[1], W.conv_wg_lo[1], W.conv_b[1], NB, w.P2, w.part2,
+                               stream)))
       return rc;
   } else {
-    conv5_pool_kernel<60><<<dim3(kTiles2, NB), 192, smem_c60, stream>>>(w.P1, kPool1, w.af1, W.conv_w[1], W.conv_b[1],
-                                                                        w.P2, kPool2, kTiles2, w.part2);
+    conv5_pool_kernel<60><<<dim3(g.tiles2, NB), 192, smem_c60, stream>>>(w.P1, g.pool1, w.af1, W.conv_w[1],
+                                                                         W.conv_b[1], w.P2, g.pool2, g.tiles2, w.part2);
   }
-  in_finalize_kernel<<<ceil_div(NB * 60, 128), 128, 0, stream>>>(w.part2, kTiles2, kPool2, 60, W.in_gamma[2],
-                                                                 W.in_beta[2], w.af2, NB * 60);
-  const size_t total = (size_t)NB * kFrames * 64;
-  in_apply_transpose_kernel<<<(unsigned)((total + 255) / 256), 256, 0, stream>>>(w.P2, w.af2, x0, NB);
+  in_stats(w.part2, g.tiles2, w.red0, w.red1, g.pool2, 60, W.in_gamma[2], W.in_beta[2], w.af2, NB * 60, stream);
+  const size_t total = (size_t)NB * g.pool2 * 64;
+  in_apply_transpose_kernel<<<(unsigned)((total + 255) / 256), 256, 0, stream>>>(w.P2, w.af2, x0, NB, g.pool2);
   B200_CUDA_OK(cudaGetLastError());
   return B200_OK;
 }

@@ -87,7 +87,7 @@ class Inference(BaseInference):
 
     # ---- forward ------------------------------------------------------------------------------------
     def infer(self, chunks: torch.Tensor) -> np.ndarray:
-        """(batch, channel, sample) chunks -> (batch, 589, 3) multilabel {0,1} (or (batch,589,7) log-probs)."""
+        """(batch, channel, sample) chunks -> (batch, frames, 3) multilabel {0,1} (or (batch, frames, 7) log-probs)."""
         try:
             logp = self.model(chunks)
         except MemoryError:
@@ -100,12 +100,12 @@ class Inference(BaseInference):
         return ctx.powerset_to_multilabel(cls).cpu().numpy().astype(np.float32)
 
     def slide_device(self, waveform: torch.Tensor, sample_rate: int, return_logp: bool = False):
-        """Device-resident result of the sliding window: (classes (C,589) u8 tensor, wav_dev, off, valid);
-        with ``return_logp`` the first entry is the pair (classes, log-probabilities (C,589,7) f32)."""
+        """Device-resident result of the sliding window: (classes (C,F) u8 tensor, wav_dev, off, valid), F frames
+        per window of ``duration``; with ``return_logp`` the first entry is the pair (classes, log-probabilities
+        (C,F,7) f32)."""
         window_size = self.model.audio.get_num_samples(self.duration)
         step_size = round(self.step * sample_rate)
-        if window_size != ops.CHUNK:
-            raise ValueError("the segmentation kernels are specialised for 10 s chunks at 16 kHz")
+        ops.check_seg_window(window_size)
         _, num_samples = waveform.shape
         off, valid, num_chunks, has_last = chunk_layout(num_samples, window_size, step_size)
         ctx = self.model._ctx()
@@ -117,7 +117,7 @@ class Inference(BaseInference):
             src = src.contiguous()
         wav_dev[:num_samples].copy_(src, non_blocking=True)
         try:
-            cls = self.model.forward_chunks(wav_dev, off, valid, return_logp=return_logp)
+            cls = self.model.forward_chunks(wav_dev, off, valid, return_logp=return_logp, window=window_size)
         except MemoryError:
             raise MemoryError(f"batch_size ({self.batch_size: d}) is probably too large. "
                               f"Try with a smaller value until memory error disappears.")
@@ -148,7 +148,8 @@ class Inference(BaseInference):
         aggregated = self.aggregate_device(SlidingWindowFeature(np.asarray(outputs), chunks_sw), frames,
                                            warm_up=self.warm_up, hamming=True, missing=0.0)
         _, num_samples = waveform.shape
-        has_last = (num_samples < ops.CHUNK) or (num_samples - ops.CHUNK) % round(self.step * sample_rate) > 0
+        _, _, _, has_last = chunk_layout(num_samples, self.model.audio.get_num_samples(self.duration),
+                                         round(self.step * sample_rate))
         if has_last:
             aggregated.data = aggregated.crop(Segment(0.0, num_samples / sample_rate), mode="loose")
         return aggregated
@@ -205,7 +206,7 @@ class Inference(BaseInference):
                          warm_up: Tuple[float, float] = (0.0, 0.0), epsilon: float = 1e-12, hamming: bool = False,
                          missing: float = np.nan, skip_average: bool = False) -> SlidingWindowFeature:
         """Inference.aggregate on the device (b200_aggregate): same arguments, bit-identical result.  ``scores.data``
-        may be a host array or a device tensor of shape (chunks, 589, classes)."""
+        may be a host array or a device tensor of shape (chunks, frames, classes)."""
         ctx = self.model._ctx()
         data = scores.data
         if not isinstance(data, torch.Tensor):

@@ -290,20 +290,24 @@ class PyanNet(Model):
     def _upload(self, ctx):
         ctx.load_segmentation(self.state_dict())
 
-    def forward_chunks(self, wav: torch.Tensor, chunk_off, chunk_valid, return_logp: bool = False, out=None):
-        """Hot-path entry: chunks addressed inside one resident device waveform (no unfold copy)."""
-        return self._ctx().seg_forward(wav, chunk_off, chunk_valid, return_logp=return_logp, out=out)
+    def forward_chunks(self, wav: torch.Tensor, chunk_off, chunk_valid, return_logp: bool = False, out=None,
+                       window: int = ops.CHUNK):
+        """Hot-path entry: windows of ``window`` samples addressed inside one resident device waveform (no unfold
+        copy) -> classes (chunks, num_frames(window)) uint8."""
+        ops.check_seg_window(window)
+        return self._ctx().seg_forward(wav, chunk_off, chunk_valid, return_logp=return_logp, out=out, window=window)
 
     def forward(self, waveforms: torch.Tensor) -> torch.Tensor:
-        """waveforms (batch, channel, sample) -> log-probabilities (batch, 589, 7)."""
+        """waveforms (batch, channel, samples), samples >= 1261 -> log-probabilities (batch, num_frames(samples), 7)."""
         b, c, s = waveforms.shape
-        if c != 1 or s != ops.CHUNK:
-            raise ValueError(f"PyanNet kernels expect mono {ops.CHUNK}-sample (10 s @ 16 kHz) chunks, got {c}x{s}")
+        if c != 1:
+            raise ValueError(f"PyanNet kernels expect mono waveforms, got {c} channels")
+        ops.check_seg_window(s)
         ctx = self._ctx()
         flat = waveforms.to(device=ctx.device, dtype=torch.float32).reshape(-1).contiguous()
         off = np.arange(b, dtype=np.int64) * s
         valid = np.full(b, s, dtype=np.int32)
-        _, logp = ctx.seg_forward(flat, off, valid, return_logp=True)
+        _, logp = ctx.seg_forward(flat, off, valid, return_logp=True, window=s)
         return logp
 
 

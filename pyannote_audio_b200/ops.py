@@ -17,6 +17,20 @@ FRAMES = 589
 SPEAKERS = 3
 CLASSES = 7
 EMB_DIM = 256
+SEG_MIN_SAMPLES = 1261     # shortest PyanNet window: 2 output frames (one frame cannot be instance-normalised)
+
+
+def seg_num_frames(num_samples: int) -> int:
+    """PyanNet output frames of a window (models/segmentation/PyanNet.py num_frames): sinc conv (251, stride 10),
+    MaxPool 3, Conv1d 5, MaxPool 3, Conv1d 5, MaxPool 3.  589 for 160000 samples."""
+    n = 1 + (int(num_samples) - 251) // 10
+    return ((n // 3 - 4) // 3 - 4) // 3
+
+
+def check_seg_window(num_samples: int):
+    if int(num_samples) < SEG_MIN_SAMPLES:
+        raise ValueError(f"PyanNet needs windows of at least {SEG_MIN_SAMPLES} samples (2 output frames), got "
+                         f"{int(num_samples)}")
 
 
 def _ptr(t: Optional[torch.Tensor]):
@@ -207,14 +221,21 @@ class Context:
             raise ValueError(f"`out` must be a contiguous {dtype} tensor of shape {tuple(shape)} on {self.device}")
         return out
 
-    def seg_forward(self, wav, chunk_off, chunk_valid, return_logp=False, out: Optional[torch.Tensor] = None):
+    def seg_forward(self, wav, chunk_off, chunk_valid, return_logp=False, out: Optional[torch.Tensor] = None,
+                    window: int = CHUNK):
+        """PyanNet on windows of ``window`` samples (>= 1261): window i = wav[off[i] : off[i] + window], of which the
+        first valid[i] samples are real (zeros after) -> classes (n, F) uint8 (+ log-probabilities (n, F, 7)),
+        F = seg_num_frames(window)."""
+        check_seg_window(window)
+        window = int(window)
         off, valid = self._chunks(wav, chunk_off, chunk_valid)
         n = len(off)
-        cls = self._out(out, (n, FRAMES), torch.uint8)
-        logp = torch.empty((n, FRAMES, CLASSES), dtype=torch.float32, device=self.device) if return_logp else None
+        F = seg_num_frames(window)
+        cls = self._out(out, (n, F), torch.uint8)
+        logp = torch.empty((n, F, CLASSES), dtype=torch.float32, device=self.device) if return_logp else None
         with torch.cuda.device(self.device):
-            _lib.check(self.lib.b200_seg_forward(self._h, _ptr(wav), off.ctypes.data, valid.ctypes.data, n, _ptr(cls),
-                                                 _ptr(logp), _stream(self.device)))
+            _lib.check(self.lib.b200_seg_forward_window(self._h, _ptr(wav), off.ctypes.data, valid.ctypes.data, n,
+                                                        window, _ptr(cls), _ptr(logp), _stream(self.device)))
         return (cls, logp) if return_logp else cls
 
     def sincnet_forward(self, wav, chunk_off, chunk_valid):
@@ -463,30 +484,31 @@ class Context:
     def aggregate(self, scores: torch.Tensor, start_frame, num_frames: int, hamming: bool = False,
                   warm_up=(0.0, 0.0), chunk_duration: float = 10.0, epsilon: float = 1e-12,
                   missing: float = float("nan"), skip_average: bool = False) -> torch.Tensor:
-        """scores (C,589,K) float32 device (NaN = missing) -> (num_frames, K) float32 device, bit-identical to
-        Inference.aggregate's numpy arithmetic (core/inference.py:498-620)."""
+        """scores (C, F, K) float32 device (NaN = missing; any F frames per chunk) -> (num_frames, K) float32 device,
+        bit-identical to Inference.aggregate's numpy arithmetic (core/inference.py:498-620)."""
         if scores.dtype != torch.float32 or scores.device != self.device or scores.dim() != 3 or \
-                scores.shape[1] != FRAMES:
-            raise ValueError(f"scores must be a float32 (chunks, {FRAMES}, classes) tensor on {self.device}")
+                scores.shape[1] < 1:
+            raise ValueError(f"scores must be a float32 (chunks, frames, classes) tensor on {self.device}")
         scores = scores.contiguous()
+        F = int(scores.shape[1])
         sf = self.start_frames(start_frame)
-        ham = self._window("hamming", lambda: np.hamming(FRAMES)) if hamming else None
-        wl = round(warm_up[0] / chunk_duration * FRAMES)
-        wr = round(warm_up[1] / chunk_duration * FRAMES)
+        ham = self._window(("hamming", F), lambda: np.hamming(F)) if hamming else None
+        wl = round(warm_up[0] / chunk_duration * F)
+        wr = round(warm_up[1] / chunk_duration * F)
         warm = None
         if wl or wr:
             def build():
-                w = np.ones(FRAMES)
+                w = np.ones(F)
                 w[:wl] = epsilon
-                w[FRAMES - wr:] = epsilon
+                w[F - wr:] = epsilon
                 return w
-            warm = self._window(("warm", wl, wr, epsilon), build)
+            warm = self._window(("warm", F, wl, wr, epsilon), build)
         out = torch.empty((num_frames, scores.shape[2]), dtype=torch.float32, device=self.device)
         with torch.cuda.device(self.device):
-            _lib.check(self.lib.b200_aggregate(self._h, _ptr(scores), _ptr(sf), sf.numel(), int(num_frames),
-                                               int(scores.shape[2]), _ptr(ham), _ptr(warm), int(skip_average),
-                                               float(missing), float(np.float32(epsilon)), _ptr(out),
-                                               _stream(self.device)))
+            _lib.check(self.lib.b200_aggregate_window(self._h, _ptr(scores), _ptr(sf), sf.numel(), int(num_frames), F,
+                                                      int(scores.shape[2]), _ptr(ham), _ptr(warm), int(skip_average),
+                                                      float(missing), float(np.float32(epsilon)), _ptr(out),
+                                                      _stream(self.device)))
         return out
 
     def powerset_speech(self, cls: torch.Tensor) -> torch.Tensor:

@@ -239,6 +239,7 @@ def apply_sharded(pipeline, file, group=None, **kwargs):
     from .inference import chunk_layout
     from .models import get_context
 
+    pipeline._require_10s_window()
     ctx = get_context(pipeline.device)
     file = pipeline._audio.validate_file(file)
     wav, sr = pipeline._audio(file)

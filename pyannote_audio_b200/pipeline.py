@@ -156,6 +156,14 @@ def binarize_frames(discrete: Optional[np.ndarray], frames: SlidingWindow, min_d
     return ann, rows
 
 
+def require_10s_window(window_size: int):
+    """Speaker diarization runs on 10 s segmentation windows only: the embedding masks and the speaker counting /
+    reconstruction kernels are laid out for 589 frames per chunk."""
+    if int(window_size) != ops.CHUNK:
+        raise ValueError(f"speaker diarization needs 10 s ({ops.CHUNK}-sample) segmentation windows, got "
+                         f"{int(window_size)} samples: use Inference or VoiceActivityDetection for other durations")
+
+
 class SpeakerDiarization:
     def __init__(self, legacy: bool = False, segmentation: Union[PyanNet, Mapping, None] = None,
                  segmentation_step: float = 0.1, embedding: Union[WeSpeakerResNet34, Mapping, None] = None,
@@ -195,9 +203,10 @@ class SpeakerDiarization:
         self.klustering = clustering
         self.der_variant = der_variant or {"collar": 0.0, "skip_overlap": False}
         self._plda = PLDA(plda) if isinstance(plda, Mapping) else plda
+        duration = segmentation.specifications.duration
+        require_10s_window(segmentation.audio.get_num_samples(duration))
         segmentation.to(device)
         embedding.to(device)
-        duration = segmentation.specifications.duration
         self._segmentation = Inference(segmentation, duration=duration, step=self.segmentation_step * duration,
                                        skip_aggregation=True, batch_size=segmentation_batch_size)
         self._embedding = PretrainedSpeakerEmbedding(embedding, device=device)
@@ -305,6 +314,7 @@ class SpeakerDiarization:
     def get_embeddings(self, file, binary_segmentations: SlidingWindowFeature, exclude_overlap: bool = False,
                        hook: Optional[Callable] = None) -> np.ndarray:
         """(C,3,256) float32 embeddings; reference loop speaker_diarization.py:332-478."""
+        self._require_10s_window()
         ctx = get_context(self.device)
         waveform, sr = self._audio(file)
         seg = torch.from_numpy(np.nan_to_num(binary_segmentations.data).astype(np.uint8)).to(ctx.device)
@@ -362,8 +372,13 @@ class SpeakerDiarization:
         yield from self.run_resident(resident, num_speakers=num_speakers, min_speakers=min_speakers,
                                      max_speakers=max_speakers, hook=hook, return_artifacts=return_artifacts)
 
+    def _require_10s_window(self):
+        inf = self._segmentation
+        require_10s_window(inf.model.audio.get_num_samples(inf.duration))
+
     def upload(self, files: Sequence[AudioFile]) -> dict:
         """H2D: one device buffer for all files, every chunk window addressable (zero padded tails)."""
+        self._require_10s_window()
         ctx = get_context(self.device)
         files = [self._audio.validate_file(f) for f in files]
         step_size = round(self._segmentation.step * self._embedding.sample_rate)

@@ -9,10 +9,9 @@ from typing import Callable, Mapping, Optional, Union
 import numpy as np
 import torch
 
-from . import ops
 from .audio import AudioFile
 from .core import Annotation, Segment, SlidingWindow, SlidingWindowFeature
-from .inference import Inference
+from .inference import Inference, chunk_layout
 from .models import PyanNet
 from .signal import Binarize
 
@@ -63,16 +62,18 @@ class VoiceActivityDetection:
         between the network and the overlap-add."""
         inf = self._segmentation
         waveform, sample_rate = inf.model.audio(file)
-        cls, _, off, _ = inf.slide_device(waveform, sample_rate)
+        cls, _, off, _ = inf.slide_device(waveform, sample_rate)                  # (C,F) u8, F frames per window
         if hook is not None:
             hook(completed=len(off), total=len(off))
         ctx = inf.model._ctx()
-        speech = ctx.powerset_speech(cls)                                           # (C,589,1) f32 on the device
+        speech = ctx.powerset_speech(cls)                                           # (C,F,1) f32 on the device
         chunks_sw = SlidingWindow(start=0.0, duration=inf.duration, step=inf.step)
         agg = inf.aggregate_device(SlidingWindowFeature(speech, chunks_sw), inf.model.receptive_field,
                                    warm_up=inf.warm_up, hamming=True, missing=0.0)
         num_samples = waveform.shape[1]
-        if (num_samples < ops.CHUNK) or (num_samples - ops.CHUNK) % round(inf.step * sample_rate) > 0:
+        _, _, _, has_last = chunk_layout(num_samples, inf.model.audio.get_num_samples(inf.duration),
+                                         round(inf.step * sample_rate))
+        if has_last:
             agg.data = agg.crop(Segment(0.0, num_samples / sample_rate), mode="loose")
         return agg
 
