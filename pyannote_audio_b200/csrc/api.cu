@@ -20,7 +20,8 @@ struct b200_ctx {
   int seg_gemm_impl = 1;   // 1 = split-fp16 wgmma GEMMs for the LSTM input projections / linear layers, 0 = fp32 SIMT
   int seg_rec_impl = 1;    // 1 = LSTM recurrence as split-fp16 wgmma on 2-CTA clusters (needs seg_gemm_impl = 1), 0 = fp32 SIMT
   int seg_conv_impl = 1;   // 1 = SincNet sinc / Conv1d layers as split-fp16 wgmma implicit GEMMs, 0 = fp32 CUDA-core twins
-  int conv_impl = 1;       // 1 = wgmma implicit-GEMM trunk convs, 0 = fp32 CUDA-core reference conv
+  int conv_impl = 1;       // 1 = wgmma implicit-GEMM trunk convs, 0 = fp32 CUDA-core reference conv, 2 = wgmma with
+                           // one weight tap per stage for every conv (bit-exact reference of 1)
   // chunks per segmentation sub-batch: 2112 = 33 recurrence tiles of 64 sequences x 2 directions x 2-CTA clusters
   // = 132 CTAs, one per SM of an H100 SXM (seg_lstm.cu launch_rec)
   int seg_max_batch = 2112;
@@ -306,7 +307,7 @@ int b200_ctx_set_option(b200_ctx* ctx, const char* key, int64_t value) {
   else if (k == "seg_rec_impl") ctx->seg_rec_impl = (int)value;
   else if (k == "fbank_share") ctx->fbank_share = (int)value;
   else B200_CHECK(false, B200_ERR_INVALID, "unknown option '%s'", key);
-  B200_CHECK(ctx->seg_max_batch >= 1 && ctx->emb_max_batch >= 1 && ctx->conv_impl >= 0 && ctx->conv_impl <= 1 &&
+  B200_CHECK(ctx->seg_max_batch >= 1 && ctx->emb_max_batch >= 1 && ctx->conv_impl >= 0 && ctx->conv_impl <= 2 &&
                  ctx->seg_gemm_impl >= 0 && ctx->seg_gemm_impl <= 1 && ctx->seg_conv_impl >= 0 && ctx->seg_conv_impl <= 1 &&
                  ctx->seg_rec_impl >= 0 && ctx->seg_rec_impl <= 1,
              B200_ERR_INVALID, "option '%s' value %lld out of range", key, (long long)value);

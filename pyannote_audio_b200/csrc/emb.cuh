@@ -15,11 +15,12 @@ struct ConvParams {
   int H_out, W_out, C_out;
   int taps_h, taps_w, stride, pad;
   int Ck, tiles_w, num_tiles, relu;
+  int band, bands;         // conv_row_kernel: output rows per unit, units per column strip (num_tiles = units)
   const float* bias;
   const __half* residual;
   __half* out;
-  // tensor-core plan: a stage = a box of a_rows pixels x Ck channels (a_tx bytes, padded to a_bytes) + the weights of
-  // one or three taps x C_out x Ck (b_bytes)
+  // tensor-core plan: a box of a_rows pixels x Ck channels (a_tx bytes, padded to a_bytes); conv_tc_kernel: a stage =
+  // a box + the weights of one tap x C_out x Ck (b_bytes); conv_row_kernel: a stage = a row slot
   uint32_t a_rows, a_tx, a_bytes, b_bytes, nstages, swizzle;
 };
 
@@ -46,7 +47,8 @@ struct EmbWeights {
   float* twiddle = nullptr;      // [256][2] cos/sin(-2 pi k / 512)
 };
 
-// impl: 0 = SIMT reference conv, 1 = wgmma tensor-core conv
+// impl: 0 = SIMT reference conv, 1 = wgmma tensor-core convs (conv_row_kernel where it applies), 2 = conv_tc_kernel for
+// every conv (the bit-exact reference of conv_row_kernel)
 int conv_forward(const ConvLayer& L, const __half* in, const __half* residual, __half* out, int B, int H_in, int W_in,
                  int relu, int impl, int num_sms, cudaStream_t stream);
 // T0 fbank frames per segment (998 for 10 s); frame0 (device, [B], may be NULL = b * T0): first fbank row of each

@@ -4,23 +4,29 @@
 //   BasicBlock.forward :140-145 (conv3x3-BN-ReLU-conv3x3-BN + shortcut -> ReLU), ResNet.forward :413-419.
 // Eval-mode BatchNorm is folded into the conv weights / a per-channel bias on the host (api.cu make_conv).
 //
-// conv_tc_kernel: implicit-GEMM convolution on the Hopper tensor cores (wgmma).
+// conv_tc_kernel: implicit-GEMM convolution on the Hopper tensor cores (wgmma), one CTA per output tile.
 //   GEMM view  D[M=128 output pixels of one image row][N=C_out] += A[M][K] * B[N][K]^T,  K = taps * C_in walked tap by
 //   tap in chunks of Ck channels.  Activations are NHWC fp16 so that one TMA box (Ck channels x consecutive pixels)
 //   lands in shared memory as a K-major, hardware-swizzled A tile; convolution padding is TMA out-of-bounds zero fill,
 //   stride 2 is the tensor map's element stride.  Weights [tap][C_out][C_in] land the same way as K-major B tiles.
-//   A stage of the mbarrier ring, filled by a TMA producer warp (warp 8), holds the operands of AW taps:
-//   AW = 3 (stride-1 3x3 convs, one channel chunk, C_out <= 64: layers 1 and 2, 13 of the 35): one box of 128 + 8 pixels
-//     and the kh row's three weight taps.  Tap kw reads the box from pixel row kw on, so neighbouring taps do not fetch
-//     the same pixels again, and a stage covers three taps.
-//   AW = 1 (everything else): one 128-pixel box and one weight tap.
-//   Either way the K walk is (tap, chunk), so every output sums its products in the same order.  With several chunks
-//   (layers 3 and 4) a three-tap stage would change that order to (kh, chunk, kw) and with it the last bits.
-//   The A operand comes straight from shared memory, the descriptor start moved by kw rows of 128 B, except for
-//   Ck = 32 with AW = 3 (64-B rows: layer 1): those fragments are read with ldmatrix, the 64-B swizzle applied in
-//   software, and issued as register-A wgmma.
+//   A stage of the mbarrier ring, filled by a TMA producer warp (warp 8), holds one 128-pixel box and one weight tap.
 //   Warpgroups 0 / 1 = output pixels [0, 64) / [64, 128) of the tile, fp32 accumulators in registers, epilogue
-//   (+bias (+residual) -> ReLU -> fp16 NHWC store) straight from the accumulator fragments.  One CTA per tile.
+//   (+bias (+residual) -> ReLU -> fp16 NHWC store) straight from the accumulator fragments.
+// conv_row_kernel: the stride-1 3x3 convs with one channel chunk and C_in = C_out (32 or 64: layers 1 and 2, 13 of the
+//   35), which are bound by HBM rather than by the tensor cores.  Persistent: about num_sms CTAs (two per SM for
+//   C_out = 32) walk units of one segment x one 128-pixel column tile x a band of consecutive output rows.
+//   - The nine weight taps are loaded once per CTA and stay in shared memory.
+//   - Input rows h0 - 1 .. h1 of a band are staged once each, as one box of 128 + 8 pixels, in a ring of row slots;
+//     output row h reads slots h - 1, h, h + 1, and tap (kh, kw) reads slot kh from pixel row kw on.  A slot is freed
+//     after its three consumer rows are done (rows at the band edges arrive for the missing ones).
+//   - Warpgroups 0 / 1 take alternate output rows, each a whole 128-pixel row as two m64 wgmma per K step, so one
+//     warpgroup's epilogue runs while the other's MMAs do.
+//   The A operand comes straight from shared memory, the descriptor start moved by kw rows of 128 B, except for
+//   Ck = 32 (64-B rows: layer 1): those fragments are read with ldmatrix, the 64-B swizzle applied in software, and
+//   issued as register-A wgmma.
+//   Each output sums its products in the (tap, 16-channel step) order of conv_tc_kernel, and the epilogue is the same,
+//   so the two kernels give bit-identical results.  With several channel chunks (layers 3 and 4) staging a row once
+//   for three taps would change that order to (kh, chunk, kw) and with it the last bits.
 #include "common.cuh"
 #include "emb.cuh"
 #include "tc_common.cuh"
@@ -30,11 +36,46 @@ namespace b200 {
 constexpr int kWgThreads = 288;
 constexpr int kTileM = 128;
 constexpr int kRowHalo = 8;                                 // 128 + 2 pixels needed for three taps, 8 keeps 8-row groups
+constexpr int kMaxSlots = 16;                               // row slots of conv_row_kernel (barrier area: 1024 B)
 
-template <int N, int CK, int AW>
+// +bias (+residual) -> ReLU -> fp16 of the 64 x N accumulator fragment of output pixels [w0, w0 + 64) of image row
+// `row` (= b * H_out + h).  A residual aliasing `out` is read before it is overwritten, by the same thread.
+template <int N>
+__device__ __forceinline__ void conv_epilogue(const float* acc, const ConvParams& p, size_t row, int w0) {
+  const int lane = threadIdx.x & 31;
+  const int c0 = 2 * (lane & 3);
+#pragma unroll
+  for (int i = 0; i < 2; ++i) {
+    const int w = w0 + ((threadIdx.x >> 5) & 3) * 16 + (lane >> 2) + 8 * i;
+    if (w >= p.W_out) continue;
+    const size_t pix = (row * p.W_out + w) * (size_t)N;
+    // up to C_out = 64 all of the pixel's residual loads are issued before its first store: `out` may alias
+    // `residual`, so a load after a store cannot be hoisted and each would wait a full memory round trip (from 128 on
+    // the registers are not there: conv_tc_kernel<256> would spill)
+    __half2 res[N / 8];
+    if (N <= 64 && p.residual) {
+#pragma unroll
+      for (int j = 0; j < N / 8; ++j) res[j] = *reinterpret_cast<const __half2*>(p.residual + pix + 8 * j + c0);
+    }
+#pragma unroll
+    for (int j = 0; j < N / 8; ++j) {
+      const int c = 8 * j + c0;
+      const float2 bb = __ldg(reinterpret_cast<const float2*>(p.bias + c));
+      float a = acc[4 * j + 2 * i] + bb.x, d = acc[4 * j + 2 * i + 1] + bb.y;
+      if (p.residual) {
+        const float2 r = __half22float2(N <= 64 ? res[j] : *reinterpret_cast<const __half2*>(p.residual + pix + c));
+        a += r.x;
+        d += r.y;
+      }
+      if (p.relu) { a = fmaxf(a, 0.f); d = fmaxf(d, 0.f); }
+      *reinterpret_cast<__half2*>(p.out + pix + c) = __floats2half2_rn(a, d);
+    }
+  }
+}
+
+template <int N, int CK>
 __global__ void __launch_bounds__(kWgThreads, N == 256 ? 1 : 2)
 conv_tc_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB, ConvParams p) {
-  constexpr bool kRegA = AW == 3 && CK == 32;
   extern __shared__ uint8_t smem_raw[];
   const uint32_t raw = smem_u32(smem_raw);
   const uint32_t base = (raw + 1023u) & ~1023u;            // swizzle-128B operands need 1024 B alignment
@@ -45,7 +86,6 @@ conv_tc_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ 
   const int wt = blockIdx.x % p.tiles_w;
   const int bh = blockIdx.x / p.tiles_w;                    // = b * H_out + h
   const int cchunks = p.C_in / CK;
-  const int kw_steps = p.taps_w / AW;
 
   if (threadIdx.x == 0) {
     for (uint32_t s = 0; s < p.nstages; ++s) { mbar_init(bar_full + 8 * s, 1); mbar_init(bar_empty + 8 * s, 2); }
@@ -61,7 +101,7 @@ conv_tc_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ 
       const int w_base = wt * kTileM * p.stride - p.pad, h_base = h * p.stride - p.pad;
       uint32_t stage = 0, phase = 0;
       for (int kh = 0; kh < p.taps_h; ++kh)
-        for (int kw = 0; kw < p.taps_w; kw += AW)
+        for (int kw = 0; kw < p.taps_w; ++kw)
           for (int cc = 0; cc < cchunks; ++cc) {
             mbar_wait(bar_empty + 8 * stage, phase ^ 1);
             mbar_expect_tx(bar_full + 8 * stage, p.a_tx + p.b_bytes);
@@ -75,72 +115,146 @@ conv_tc_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ 
   }
 
   const int wg = warp >> 2;
-  const int lane = threadIdx.x & 31;
   constexpr uint32_t row_bytes = CK * 2;                   // = the swizzle width (64 or 128 B)
-  constexpr uint32_t b_tap_bytes = N * row_bytes;
   float acc[N / 2];
 #pragma unroll
   for (int i = 0; i < N / 2; ++i) acc[i] = 0.f;
-  const int kblocks = p.taps_h * kw_steps * cchunks;
+  const int kblocks = p.taps_h * p.taps_w * cchunks;
   uint32_t stage = 0, phase = 0, prev = 0;
   for (int kb = 0; kb < kblocks; ++kb) {
     mbar_wait(bar_full + 8 * stage, phase);
     const uint32_t st = stage0 + stage * stage_bytes;
     const uint32_t sa = st + (uint32_t)wg * 64u * row_bytes, sb = st + p.a_bytes;
-    uint32_t af[AW][CK / 16][4];
-    if constexpr (kRegA) {
-      // pixel row r of this warp's 16 (lanes 0-15 / 16-31: K columns 0-7 / 8-15 of each step) at 64-B rows, 16-B
-      // chunk c stored at chunk c ^ ((row >> 1) & 3) (64-B swizzle; a_bytes keeps stages 1024-B aligned)
-#pragma unroll
-      for (int t = 0; t < AW; ++t)
-#pragma unroll
-        for (int k = 0; k < CK / 16; ++k) {
-          const uint32_t row = (uint32_t)(wg * 64 + (warp & 3) * 16 + (lane & 15) + t);
-          const uint32_t chunk = (uint32_t)(2 * k + (lane >> 4)) ^ ((row >> 1) & 3u);
-          ldsm_x4(af[t][k], st + row * row_bytes + chunk * 16u);
-        }
-    }
     wg_fence();
+    const uint64_t ad = wg_desc(sa, row_bytes), bd = wg_desc(sb, row_bytes);
 #pragma unroll
-    for (int t = 0; t < AW; ++t) {
-      const uint64_t bd = wg_desc(sb + t * b_tap_bytes, row_bytes);
-      if constexpr (kRegA) {
-#pragma unroll
-        for (int k = 0; k < CK / 16; ++k) WgmmaRS<N>::mma(acc, af[t][k], bd + 2 * k);
-      } else {
-        const uint64_t ad = wg_desc(sa + t * row_bytes, row_bytes);
-#pragma unroll
-        for (int k = 0; k < CK / 16; ++k) Wgmma<N>::mma(acc, ad + 2 * k, bd + 2 * k);   // +32 B per K=16 step
-      }
-    }
+    for (int k = 0; k < CK / 16; ++k) Wgmma<N>::mma(acc, ad + 2 * k, bd + 2 * k);   // +32 B per K=16 step
     wg_commit();
-    if constexpr (kRegA) wg_wait<0>();                     // the fragments are rewritten by the next ldmatrix
-    else wg_wait<1>();                                      // the previous stage's wgmma have read their operands
+    wg_wait<1>();                                           // the previous stage's wgmma have read their operands
     if (kb > 0 && (threadIdx.x & 127) == 0) mbar_arrive(bar_empty + 8 * prev);
     prev = stage;
     if (++stage == p.nstages) { stage = 0; phase ^= 1; }
   }
   wg_wait<0>();
+  conv_epilogue<N>(acc, p, (size_t)bh, wt * kTileM + wg * 64);
+}
 
-  const int c0 = 2 * (lane & 3);
-#pragma unroll
-  for (int i = 0; i < 2; ++i) {
-    const int w = wt * kTileM + wg * 64 + (warp & 3) * 16 + (lane >> 2) + 8 * i;
-    if (w >= p.W_out) continue;
-    const size_t pix = ((size_t)bh * p.W_out + w) * (size_t)N;
-#pragma unroll
-    for (int j = 0; j < N / 8; ++j) {
-      const int c = 8 * j + c0;
-      const float2 bb = __ldg(reinterpret_cast<const float2*>(p.bias + c));
-      float a = acc[4 * j + 2 * i] + bb.x, d = acc[4 * j + 2 * i + 1] + bb.y;
-      if (p.residual) {
-        const float2 r = __half22float2(*reinterpret_cast<const __half2*>(p.residual + pix + c));
-        a += r.x;
-        d += r.y;
+template <int N, int CK>
+__global__ void __launch_bounds__(kWgThreads, N == 32 ? 2 : 1)
+conv_row_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB, ConvParams p) {
+  constexpr uint32_t row_bytes = CK * 2;                   // = the swizzle width (64 or 128 B)
+  constexpr uint32_t b_tap_bytes = N * row_bytes;
+  extern __shared__ uint8_t smem_raw[];
+  const uint32_t base = (smem_u32(smem_raw) + 1023u) & ~1023u;
+  const uint32_t bar_w = base, bar_full = base + 8, bar_empty = base + 8 + 8 * kMaxSlots;
+  const uint32_t wts = base + 1024;                         // 9 taps x [N][CK]
+  const uint32_t slot0 = wts + 9 * b_tap_bytes;             // 18 / 72 KB: slots stay 1024-B aligned
+  const uint32_t nslots = p.nstages;
+  const int warp = threadIdx.x >> 5;
+
+  if (threadIdx.x == 0) {
+    mbar_init(bar_w, 1);
+    for (uint32_t s = 0; s < nslots; ++s) { mbar_init(bar_full + 8 * s, 1); mbar_init(bar_empty + 8 * s, 3); }
+    asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
+  }
+  __syncthreads();
+
+  // unit u: column tile u % tiles_w (neighbouring CTAs share the halo pixels in L2), then band, then segment
+  if (warp == 8) {
+    if ((threadIdx.x & 31) == 0) {
+      prefetch_tensormap(&tmA);
+      prefetch_tensormap(&tmB);
+      mbar_expect_tx(bar_w, 9 * b_tap_bytes);
+      for (int kh = 0; kh < 3; ++kh) tma_load_3d(&tmB, bar_w, wts + 3 * kh * b_tap_bytes, 0, 0, 3 * kh);
+      uint32_t s = 0;                                       // input rows staged so far
+      for (int u = blockIdx.x; u < p.num_tiles; u += gridDim.x) {
+        const int wt = u % p.tiles_w, t = u / p.tiles_w;
+        const int h0 = (t % p.bands) * p.band, b = t / p.bands;
+        const int n = min(p.band, p.H_out - h0);
+        for (int r = 0; r < n + 2; ++r, ++s) {
+          const uint32_t slot = s % nslots;
+          mbar_wait(bar_empty + 8 * slot, ((s / nslots) & 1) ^ 1);
+          mbar_expect_tx(bar_full + 8 * slot, p.a_tx);
+          tma_load_4d(&tmA, bar_full + 8 * slot, slot0 + slot * p.a_bytes, 0, wt * kTileM - 1, h0 - 1 + r, b);
+        }
       }
-      if (p.relu) { a = fmaxf(a, 0.f); d = fmaxf(d, 0.f); }
-      *reinterpret_cast<__half2*>(p.out + pix + c) = __floats2half2_rn(a, d);
     }
+    return;
+  }
+
+  const int wg = __shfl_sync(0xffffffffu, warp >> 2, 0);  // warp-uniform to the compiler: no wgmma serialisation
+  const int lane = threadIdx.x & 31;
+  mbar_wait(bar_w, 0);
+  uint32_t s = 0;                                           // first input row of the current unit
+  int item = 0;                                             // output rows walked so far; row `item` is warpgroup item & 1's
+  for (int u = blockIdx.x; u < p.num_tiles; u += gridDim.x) {
+    const int wt = u % p.tiles_w, t = u / p.tiles_w;
+    const int h0 = (t % p.bands) * p.band, b = t / p.bands;
+    const int n = min(p.band, p.H_out - h0);
+    for (int j = 0; j < n; ++j, ++item) {
+      if ((item & 1) != wg) continue;
+      float acc[2][N / 2];                                  // output pixels [0, 64) / [64, 128) of the row
+#pragma unroll
+      for (int m = 0; m < 2; ++m)
+#pragma unroll
+        for (int i = 0; i < N / 2; ++i) {
+          acc[m][i] = 0.f;
+          asm volatile("" : "+f"(acc[m][i]));               // zeroed before the first wg_fence, not sunk past it
+        }
+#pragma unroll
+      for (int kh = 0; kh < 3; ++kh) {
+        const uint32_t q = s + j + kh, slot = q % nslots;
+        mbar_wait(bar_full + 8 * slot, (q / nslots) & 1);
+        const uint32_t sa = slot0 + slot * p.a_bytes;
+        if constexpr (CK == 32) {
+          // pixel row r of this warp's 16 (lanes 0-15 / 16-31: K columns 0-7 / 8-15 of each step) at 64-B rows, 16-B
+          // chunk c stored at chunk c ^ ((row >> 1) & 3) (64-B swizzle; slots are 1024-B aligned)
+#pragma unroll
+          for (int kw = 0; kw < 3; ++kw) {
+            uint32_t af[2][CK / 16][4];
+#pragma unroll
+            for (int m = 0; m < 2; ++m)
+#pragma unroll
+              for (int k = 0; k < CK / 16; ++k) {
+                const uint32_t row = (uint32_t)(m * 64 + (warp & 3) * 16 + (lane & 15) + kw);
+                const uint32_t chunk = (uint32_t)(2 * k + (lane >> 4)) ^ ((row >> 1) & 3u);
+                ldsm_x4(af[m][k], sa + row * row_bytes + chunk * 16u);
+              }
+            wg_fence();
+            const uint64_t bd = wg_desc(wts + (3 * kh + kw) * b_tap_bytes, row_bytes);
+#pragma unroll
+            for (int k = 0; k < CK / 16; ++k)
+#pragma unroll
+              for (int m = 0; m < 2; ++m) WgmmaRS<N>::mma(acc[m], af[m][k], bd + 2 * k);
+            wg_commit();
+            wg_wait<0>();                                   // the fragments are rewritten by the next ldmatrix
+          }
+        } else {
+          wg_fence();
+#pragma unroll
+          for (int kw = 0; kw < 3; ++kw) {
+            const uint64_t bd = wg_desc(wts + (3 * kh + kw) * b_tap_bytes, row_bytes);
+#pragma unroll
+            for (int m = 0; m < 2; ++m) {
+              const uint64_t ad = wg_desc(sa + (uint32_t)(m * 64 + kw) * row_bytes, row_bytes);
+#pragma unroll
+              for (int k = 0; k < CK / 16; ++k) Wgmma<N>::mma(acc[m], ad + 2 * k, bd + 2 * k);
+            }
+          }
+          wg_commit();
+        }
+      }
+      wg_wait<0>();
+      // slot of input row j + kh: one arrival per consumer row, the band's first / last row also for the missing ones
+      if ((threadIdx.x & 127) == 0)
+#pragma unroll
+        for (int kh = 0; kh < 3; ++kh)
+          mbar_arrive_n(bar_empty + 8 * ((s + j + kh) % nslots), 1 + (j == 0 ? 2 - kh : 0) + (j == n - 1 ? kh : 0));
+      const size_t row = (size_t)b * p.H_out + h0 + j;
+#pragma unroll
+      for (int m = 0; m < 2; ++m) conv_epilogue<N>(acc[m], p, row, wt * kTileM + m * 64);
+    }
+    s += n + 2;
   }
 }
 
@@ -303,7 +417,6 @@ PFN_encodeTiled get_encode() {
 
 int conv_forward(const ConvLayer& L, const __half* in, const __half* residual, __half* out, int B, int H_in, int W_in,
                  int relu, int impl, int num_sms, cudaStream_t stream) {
-  (void)num_sms;
   ConvParams p{};
   p.B = B; p.H_in = H_in; p.W_in = W_in; p.C_in = L.C_in; p.C_out = L.C_out;
   p.taps_h = L.ksize; p.taps_w = L.ksize; p.stride = L.stride; p.pad = L.ksize / 2;
@@ -317,7 +430,8 @@ int conv_forward(const ConvLayer& L, const __half* in, const __half* residual, _
   B200_CHECK(L.C_in % p.Ck == 0 && (L.C_out == 64 || (L.C_out >= 128 && L.C_out <= 256 && L.C_out % 128 == 0 && p.Ck == 64) ||
                                     (L.C_out == 32 && p.Ck == 32)),
              B200_ERR_STATE, "conv %d -> %d channels unsupported", L.C_in, L.C_out);
-  B200_CHECK(impl == 0 || impl == 1, B200_ERR_INVALID, "conv_impl %d unknown (0 = CUDA cores, 1 = tensor cores)", impl);
+  B200_CHECK(impl >= 0 && impl <= 2, B200_ERR_INVALID,
+             "conv_impl %d unknown (0 = CUDA cores, 1 = tensor cores, 2 = tensor cores, one weight tap per stage)", impl);
 
   if (impl == 0) {
     const size_t total = (size_t)B * p.H_out * p.W_out * (L.C_out / 8);
@@ -326,21 +440,41 @@ int conv_forward(const ConvLayer& L, const __half* in, const __half* residual, _
     return B200_OK;
   }
 
-  // stride-1 3x3 convs with one channel chunk stage three taps at a time on one box of 128 + 8 pixels (AW = 3); from
-  // C_out = 128 on three weight taps would leave room for a single stage
-  const int AW = (L.ksize == 3 && L.stride == 1 && L.C_in == p.Ck && L.C_out <= 64) ? 3 : 1;
-  p.a_rows = AW == 3 ? kTileM + kRowHalo : kTileM;
+  // conv_row_kernel for the stride-1 3x3 convs with one channel chunk and C_in = C_out; impl 2 keeps every conv on
+  // conv_tc_kernel, the bit-exact reference of the row kernel
+  const bool rows = impl == 1 && L.ksize == 3 && L.stride == 1 && L.C_in == p.Ck && L.C_out == L.C_in;
+  p.a_rows = rows ? kTileM + kRowHalo : kTileM;
   p.a_tx = p.a_rows * p.Ck * 2;
   p.a_bytes = (p.a_tx + 1023u) & ~1023u;
-  p.b_bytes = (uint32_t)(AW * L.C_out * p.Ck * 2);
-  // C_out = 256 needs 128 accumulator registers per thread: one CTA per SM with 4 deep stages; the narrower layers
-  // run two CTAs per SM (registers allow it) on half the shared memory each
-  const uint32_t budget = L.C_out == 256 ? 200u * 1024 : 100u * 1024;
-  p.nstages = budget / (p.a_bytes + p.b_bytes);
-  if (p.nstages > 8) p.nstages = 8;
-  // a C_out = 32 tile has only three stages of work; a deeper ring would only keep other CTAs off the SM
-  if (AW == 3 && p.nstages > 3) p.nstages = 3;
-  B200_CHECK(p.nstages >= 2, B200_ERR_STATE, "conv %d -> %d: shared memory plan too shallow", L.C_in, L.C_out);
+  size_t smem;
+  int ctas = 0;
+  if (rows) {
+    // resident weights + as many row slots as fit: two CTAs per SM for C_out = 32 (113 KB each), one for C_out = 64
+    // (227 KB: 72 KB weights + 9 slots of 17 KB)
+    const int per_sm = L.C_out == 32 ? 2 : 1;
+    const size_t budget = per_sm == 2 ? 113u * 1024 : 227u * 1024;
+    const size_t fixed = 2048 + (size_t)9 * L.C_out * p.Ck * 2;
+    p.nstages = (uint32_t)std::min<size_t>(kMaxSlots, (budget - fixed) / p.a_bytes);
+    // two warpgroups on consecutive rows hold four slots; the rest lets the producer run ahead
+    B200_CHECK(p.nstages >= 6, B200_ERR_STATE, "conv %d -> %d: row ring too shallow", L.C_in, L.C_out);
+    smem = fixed + (size_t)p.nstages * p.a_bytes;
+    // full-height bands while the column strips fill every CTA (a 264-segment sub-batch: 2112 / 1056 strips for
+    // layers 1 / 2), else shorter bands so that small batches still reach every SM; each band re-stages two halo rows
+    ctas = per_sm * num_sms;
+    const int strips = B * p.tiles_w;
+    const int nbands = std::min(p.H_out, ceil_div(ctas, strips));
+    p.band = ceil_div(p.H_out, nbands);
+    p.bands = ceil_div(p.H_out, p.band);
+    p.num_tiles = strips * p.bands;
+  } else {
+    p.b_bytes = (uint32_t)(L.C_out * p.Ck * 2);
+    // C_out = 256 needs 128 accumulator registers per thread: one CTA per SM with 4 deep stages; the narrower layers
+    // run two CTAs per SM (registers allow it) on half the shared memory each
+    const uint32_t budget = L.C_out == 256 ? 200u * 1024 : 100u * 1024;
+    p.nstages = std::min(budget / (p.a_bytes + p.b_bytes), 8u);
+    B200_CHECK(p.nstages >= 2, B200_ERR_STATE, "conv %d -> %d: shared memory plan too shallow", L.C_in, L.C_out);
+    smem = 1024 + 1024 + (size_t)p.nstages * (p.a_bytes + p.b_bytes);
+  }
   PFN_encodeTiled enc = get_encode();
   B200_CHECK(enc != nullptr, B200_ERR_CUDA, "cuTensorMapEncodeTiled not available from the driver");
   CUtensorMap tmA, tmB;
@@ -357,9 +491,10 @@ int conv_forward(const ConvLayer& L, const __half* in, const __half* residual, _
     B200_CHECK(r == CUDA_SUCCESS, B200_ERR_CUDA, "cuTensorMapEncodeTiled(A) failed: %d", (int)r);
   }
   {
+    // conv_row_kernel loads the nine taps as three boxes of three
     cuuint64_t dims[3] = {(cuuint64_t)L.C_in, (cuuint64_t)L.C_out, (cuuint64_t)(L.ksize * L.ksize)};
     cuuint64_t strides[2] = {(cuuint64_t)L.C_in * 2, (cuuint64_t)L.C_out * L.C_in * 2};
-    cuuint32_t box[3] = {(cuuint32_t)p.Ck, (cuuint32_t)L.C_out, (cuuint32_t)AW};
+    cuuint32_t box[3] = {(cuuint32_t)p.Ck, (cuuint32_t)L.C_out, rows ? 3u : 1u};
     cuuint32_t estr[3] = {1, 1, 1};
     CUresult r = enc(&tmB, CU_TENSOR_MAP_DATA_TYPE_FLOAT16, 3, const_cast<__half*>(L.w), dims, strides, box, estr,
                      CU_TENSOR_MAP_INTERLEAVE_NONE,
@@ -367,22 +502,19 @@ int conv_forward(const ConvLayer& L, const __half* in, const __half* residual, _
                      CU_TENSOR_MAP_L2_PROMOTION_L2_256B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
     B200_CHECK(r == CUDA_SUCCESS, B200_ERR_CUDA, "cuTensorMapEncodeTiled(B) failed: %d", (int)r);
   }
-  const size_t smem = 1024 + 1024 + (size_t)p.nstages * (p.a_bytes + p.b_bytes);
   auto launch = [&](auto kernel) -> int {
     B200_CUDA_OK(cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-    kernel<<<(unsigned)p.num_tiles, kWgThreads, smem, stream>>>(tmA, tmB, p);
+    const int grid = rows ? std::min(p.num_tiles, ctas) : p.num_tiles;
+    kernel<<<(unsigned)grid, kWgThreads, smem, stream>>>(tmA, tmB, p);
     B200_CUDA_OK(cudaGetLastError());
     return B200_OK;
   };
-  if (AW == 3) {
-    if (p.Ck == 32) return L.C_out == 32 ? launch(conv_tc_kernel<32, 32, 3>) : launch(conv_tc_kernel<64, 32, 3>);
-    return launch(conv_tc_kernel<64, 64, 3>);
-  }
-  if (p.Ck == 32) return L.C_out == 32 ? launch(conv_tc_kernel<32, 32, 1>) : launch(conv_tc_kernel<64, 32, 1>);
+  if (rows) return p.Ck == 32 ? launch(conv_row_kernel<32, 32>) : launch(conv_row_kernel<64, 64>);
+  if (p.Ck == 32) return L.C_out == 32 ? launch(conv_tc_kernel<32, 32>) : launch(conv_tc_kernel<64, 32>);
   switch (L.C_out) {
-    case 64: return launch(conv_tc_kernel<64, 64, 1>);
-    case 128: return launch(conv_tc_kernel<128, 64, 1>);
-    default: return launch(conv_tc_kernel<256, 64, 1>);
+    case 64: return launch(conv_tc_kernel<64, 64>);
+    case 128: return launch(conv_tc_kernel<128, 64>);
+    default: return launch(conv_tc_kernel<256, 64>);
   }
 }
 

@@ -1,7 +1,7 @@
 """Per-conv profile of the ResNet34 trunk: time, TFLOP/s, operand fill and unique HBM traffic of each trunk conv.
 
     python scripts/trunk_profile.py                  # the library in this tree (needs a GPU)
-    python scripts/trunk_profile.py --root OTHER --plan per-tap   # another tree's build, with its launch plan
+    python scripts/trunk_profile.py --root OTHER --plan reuse     # another tree's build, with its launch plan
     python scripts/trunk_profile.py --model-only     # the byte model alone (no GPU)
 
 `ctx.emb_trunk` runs on --batch segments (the library's embedding sub-batch) under torch.profiler with CUDA
@@ -13,6 +13,9 @@ Byte model, per segment (computed from the shapes, not measured):
           per-tap : every (tap, channel chunk) stages a 128-pixel activation box and one weight tile
           reuse   : stride-1 3x3 convs with one channel chunk and C_out <= 64 (layers 1 and 2) stage one 136-pixel
                     activation box per kh for the three kw taps, and every weight tile; the other convs stay per-tap
+          resident: the stride-1 3x3 convs with one channel chunk and C_in = C_out (layers 1 and 2) stage each input
+                    row of a band of output rows once as a 136-pixel box (plus two halo rows per band) and their nine
+                    weight taps once per CTA (--sms CTAs per SM count as in conv_forward); the other convs stay per-tap
   HBM   = input + output (+ residual) activations once, and the weights once per launch shared by --batch segments
 """
 import argparse
@@ -40,7 +43,15 @@ def trunk_convs():
     return convs
 
 
-def conv_model(c, plan, batch):
+def resident_plan(cout, ho, tiles_w, batch, sms):
+    """(CTAs, output rows per band, bands) of conv_row_kernel, as conv_forward chooses them."""
+    ctas = (2 if cout == 32 else 1) * sms
+    strips = batch * tiles_w
+    band = -(-ho // min(ho, -(-ctas // strips)))
+    return min(ctas, strips * -(-ho // band)), band, -(-ho // band)
+
+
+def conv_model(c, plan, batch, sms=132):
     """(GFLOP, fill MB, unique HBM MB) per segment of one conv."""
     _, _, cin, cout, k, s, H, W, res = c
     pad = k // 2
@@ -50,7 +61,11 @@ def conv_model(c, plan, batch):
     tiles = Ho * -(-Wo // TILE_M)
     b_tile = cout * ck * 2
     reuse = plan == "reuse" and k == 3 and s == 1 and cin == ck and cout <= 64
-    if reuse:
+    if plan == "resident" and k == 3 and s == 1 and cin == ck and cout == cin:
+        tiles_w = -(-Wo // TILE_M)
+        ctas, _, bands = resident_plan(cout, Ho, tiles_w, batch, sms)
+        fill = tiles_w * (Ho + 2 * bands) * (TILE_M + HALO) * ck * 2 + ctas * k * k * b_tile / batch
+    elif reuse:
         fill = tiles * (k * chunks * (TILE_M + HALO) * ck * 2 + k * k * chunks * b_tile)
     else:
         fill = tiles * k * k * chunks * (TILE_M * ck * 2 + b_tile)
@@ -59,8 +74,8 @@ def conv_model(c, plan, batch):
     return 2.0 * Ho * Wo * cout * cin * k * k / 1e9, fill / 1e6, hbm / 1e6
 
 
-def print_model(plan, batch):
-    rows = [(c, *conv_model(c, plan, batch)) for c in trunk_convs()]
+def print_model(plan, batch, sms):
+    rows = [(c, *conv_model(c, plan, batch, sms)) for c in trunk_convs()]
     print(f"byte model ({plan} plan), per segment:")
     print(f"{'layer':>6} {'convs':>5} {'GFLOP':>7} {'fill MB':>8} {'HBM MB':>7} {'FLOP/fill B':>11} {'FLOP/HBM B':>10}")
     tot = [0, 0.0, 0.0, 0.0]
@@ -87,15 +102,16 @@ def main():
     ap = argparse.ArgumentParser(description=__doc__, formatter_class=argparse.RawDescriptionHelpFormatter)
     ap.add_argument("--root", default=os.path.dirname(os.path.dirname(os.path.abspath(__file__))),
                     help="tree whose built library is timed (default: this one)")
-    ap.add_argument("--plan", choices=["reuse", "per-tap"], default="reuse",
-                    help="launch plan of the timed library for the byte model (per-tap: a library whose trunk convs "
-                         "stage one activation box per tap)")
+    ap.add_argument("--plan", choices=["resident", "reuse", "per-tap"], default="resident",
+                    help="launch plan of the timed library for the byte model (reuse: a library whose layer 1 and 2 "
+                         "convs stage one box per kh; per-tap: one box per tap)")
+    ap.add_argument("--sms", type=int, default=132, help="SMs of the GPU for the resident plan (H100 SXM: 132)")
     ap.add_argument("--batch", type=int, default=264, help="segments per emb_trunk call (library sub-batch: 264)")
     ap.add_argument("--iters", type=int, default=5, help="profiled emb_trunk calls")
     ap.add_argument("--model-only", action="store_true", help="print the byte model and exit (no GPU needed)")
     args = ap.parse_args()
 
-    rows = print_model(args.plan, args.batch)
+    rows = print_model(args.plan, args.batch, args.sms)
     if args.model_only:
         return
 
