@@ -103,6 +103,25 @@ typedef struct b200_emb_weights {
 /* the same for WeSpeakerResNet34 (models/embedding/wespeaker/__init__.py:324-372): eval-mode BatchNorm is folded into
  * the conv weights / biases, conv weights go to fp16 [tap][c_out][c_in] plus the per-kernel re-layouts. */
 int b200_emb_load(b200_ctx* ctx, const b200_emb_weights* w);
+/* WeSpeakerResNet152 / 221 / 293 (models/embedding/wespeaker/resnet.py:148-212, 477-508; __init__.py:375-466): the same
+ * stem, strides and TSTP pooling with Bottleneck blocks, num_blocks {3, 8, 36, 3}, {6, 16, 48, 3} or {10, 20, 64, 3}
+ * (any counts >= 1 are accepted).  The block arrays have sum(num_blocks) entries in block order; block_shortcut[i]
+ * has conv_weight == NULL exactly where the block has no shortcut (stride 1 and in_planes == 4 * planes).
+ * The trunk outputs C = 1024 channels (256 for ResNet34), the statistics are 20 * C = 20480 wide. */
+typedef struct b200_emb_bottleneck_weights {
+  int32_t num_blocks[4];
+  b200_conv_bn stem;                          /* resnet.conv1 / resnet.bn1                               */
+  const b200_conv_bn* block_conv1;            /* resnet.layerL.i.conv1 / bn1 (1x1, in -> p)              */
+  const b200_conv_bn* block_conv2;            /* resnet.layerL.i.conv2 / bn2 (3x3, stride, p -> p)       */
+  const b200_conv_bn* block_conv3;            /* resnet.layerL.i.conv3 / bn3 (1x1, p -> 4p)              */
+  const b200_conv_bn* block_shortcut;         /* resnet.layerL.i.shortcut.{0,1} (1x1, stride, in -> 4p)  */
+  const float* seg1_weight;                   /* resnet.seg_1.weight [256][20480]                        */
+  const float* seg1_bias;                     /* [256]                                                   */
+} b200_emb_bottleneck_weights;
+/* Loads a bottleneck trunk into the ctx's one embedding slot (replacing a ResNet34 loaded by b200_emb_load, and the
+ * other way round).  BN folding and the fp16 layouts as b200_emb_load.  The embedding entry points below then run
+ * this trunk.  Bad arguments or inconsistent shortcuts return B200_STATUS_INVALID. */
+int b200_emb_load_bottleneck(b200_ctx* ctx, const b200_emb_bottleneck_weights* w);
 
 /* ---- audio ingest: Audio.__call__ / Audio.downmix_and_resample (core/io.py:223-265, 306-351) -----------------
  * pcm is a DEVICE buffer holding the raw decoded audio: B200_PCM_S16_INTERLEAVED = int16 [frame][channel] (what a
@@ -141,7 +160,8 @@ int b200_powerset_to_multilabel(b200_ctx* ctx, const uint8_t* classes, int64_t n
 
 /* ---- embeddings: SpeakerDiarization.get_embeddings hot loop (pipelines/speaker_diarization.py:399-459) over
  * PyannoteAudioPretrainedSpeakerEmbedding.__call__ (pipelines/speaker_verification.py:704-716) and
- * WeSpeakerResNet34.forward (models/embedding/wespeaker/__init__.py:324-343).  One trunk pass per chunk, the three
+ * WeSpeakerResNet34.forward (models/embedding/wespeaker/__init__.py:324-343), or the loaded bottleneck trunk's.  One
+ * trunk pass per chunk, the three
  * local speakers share it (forward_frames + forward_embedding, :288-322); masks[num_chunks][3][589] u8 are the
  * StatsPool weights; emb[num_chunks][3][256] fp32. */
 int b200_emb_forward(b200_ctx* ctx, const float* wav, const int64_t* chunk_off, const int32_t* chunk_valid,
@@ -168,7 +188,8 @@ int b200_emb_fbank(b200_ctx* ctx, const float* wav, const int64_t* chunk_off, co
  * fbank rows computed per sub-batch (998 * chunks without sharing).  Returns the number of runs, < 0 on bad arguments. */
 int64_t b200_emb_fbank_plan(const int64_t* chunk_off, const int32_t* chunk_valid, int32_t num_chunks, int32_t sub_batch,
                             int32_t share, int32_t* frame0, int32_t* rows_per_sub_batch);
-/* ResNet.forward_frames on a given fbank (resnet.py:399-419): frames[num_chunks][256][10][125] fp32 (NCHW). */
+/* ResNet.forward_frames on a given fbank (resnet.py:399-419): frames[num_chunks][C][10][125] fp32 (NCHW), C = 256 for
+ * ResNet34 and 1024 for a bottleneck trunk. */
 int b200_emb_trunk(b200_ctx* ctx, const float* fbank, int32_t num_chunks, float* frames, void* stream);
 /* WeSpeakerResNet34.forward (models/embedding/wespeaker/__init__.py:324-343) on utterances of one length
  * num_samples >= 400 (a (num_utts, 1, num_samples) tensor): utterance i = wav[off[i] .. off[i] + num_samples), off a
@@ -182,7 +203,8 @@ int b200_emb_trunk(b200_ctx* ctx, const float* fbank, int32_t num_chunks, float*
 int b200_emb_forward_utt(b200_ctx* ctx, const float* wav, const int64_t* off, int64_t num_samples, int32_t num_utts,
                          const float* weights, int32_t num_speakers, int32_t num_weights, float* emb, void* stream);
 /* ResNet.forward_embedding on caller frames (resnet.py:370-397, wespeaker/__init__.py:304-322): frames fp32 DEVICE
- * NCHW [B][256][10][T] (what forward_frames returns), weights and emb as in b200_emb_forward_utt. */
+ * NCHW [B][C][10][T] (what forward_frames returns; C = 256 for ResNet34, 1024 for a bottleneck trunk), weights and
+ * emb as in b200_emb_forward_utt. */
 int b200_emb_forward_embedding(b200_ctx* ctx, const float* frames, int32_t B, int32_t T, const float* weights,
                                int32_t num_speakers, int32_t num_weights, float* emb, void* stream);
 /* StatsPool.forward (models/blocks/pooling.py:76-130): seq[B][F][T], weights[B][S][Tw] or NULL -> out[B][S][2F]. */

@@ -37,6 +37,12 @@ class EmbWeights(C.Structure):
                 ("block_shortcut", ConvBN * 16), ("seg1_weight", c_float_p), ("seg1_bias", c_float_p)]
 
 
+class EmbBottleneckWeights(C.Structure):
+    _fields_ = [("num_blocks", C.c_int32 * 4), ("stem", ConvBN), ("block_conv1", C.POINTER(ConvBN)),
+                ("block_conv2", C.POINTER(ConvBN)), ("block_conv3", C.POINTER(ConvBN)),
+                ("block_shortcut", C.POINTER(ConvBN)), ("seg1_weight", c_float_p), ("seg1_bias", c_float_p)]
+
+
 class B200Error(RuntimeError):
     pass
 
@@ -53,6 +59,7 @@ _PROTOS = {
     "b200_ctx_timer": (C.c_int, [C.c_void_p, C.c_char_p, C.POINTER(C.c_double), C.POINTER(C.c_int64)]),
     "b200_seg_load": (C.c_int, [C.c_void_p, C.POINTER(SegWeights)]),
     "b200_emb_load": (C.c_int, [C.c_void_p, C.POINTER(EmbWeights)]),
+    "b200_emb_load_bottleneck": (C.c_int, [C.c_void_p, C.POINTER(EmbBottleneckWeights)]),
     "b200_seg_forward": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_int32, C.c_void_p, C.c_void_p,
                                    C.c_void_p]),
     "b200_seg_forward_window": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_int32, C.c_int32,

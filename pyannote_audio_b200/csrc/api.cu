@@ -553,6 +553,8 @@ int b200_emb_load(b200_ctx* ctx, const b200_emb_weights* w) {
     if ((rc = upload(ctx, cb, &E.conv1_b))) return rc;
   }
   E.blocks.clear();
+  E.bottlenecks.clear();
+  E.C = 256;
   const int planes[4] = {32, 64, 128, 256}, nblk[4] = {3, 4, 6, 3}, strides[4] = {1, 2, 2, 2};
   int in_planes = 32, bi = 0;
   for (int l = 0; l < 4; ++l)
@@ -569,6 +571,79 @@ int b200_emb_load(b200_ctx* ctx, const b200_emb_weights* w) {
     }
   B200_CHECK(w->seg1_weight && w->seg1_bias, B200_ERR_INVALID, "seg_1 missing");
   std::vector<float> sw(w->seg1_weight, w->seg1_weight + (size_t)256 * 5120), sb(w->seg1_bias, w->seg1_bias + 256);
+  {
+    std::vector<__half> hi(sw.size()), lo(sw.size());
+    for (size_t i = 0; i < sw.size(); ++i) {
+      hi[i] = __float2half(sw[i]);
+      lo[i] = __float2half(sw[i] - __half2float(hi[i]));
+    }
+    if ((rc = upload(ctx, hi, &E.seg1_w_hi))) return rc;
+    if ((rc = upload(ctx, lo, &E.seg1_w_lo))) return rc;
+  }
+  if ((rc = upload(ctx, sw, &E.seg1_w))) return rc;
+  if ((rc = upload(ctx, sb, &E.seg1_b))) return rc;
+  E.loaded = true;
+  return B200_OK;
+}
+
+int b200_emb_load_bottleneck(b200_ctx* ctx, const b200_emb_bottleneck_weights* w) {
+  B200_CHECK(ctx && w, B200_ERR_INVALID, "NULL ctx/weights");
+  for (int l = 0; l < 4; ++l)
+    B200_CHECK(w->num_blocks[l] >= 1 && w->num_blocks[l] <= 1024, B200_ERR_INVALID,
+               "layer %d: %d blocks (expected 1 .. 1024)", l + 1, (int)w->num_blocks[l]);
+  B200_CHECK(w->block_conv1 && w->block_conv2 && w->block_conv3 && w->block_shortcut, B200_ERR_INVALID,
+             "block arrays missing");
+  // the shortcut of block i exists exactly where Bottleneck has one (resnet.py:165-176)
+  {
+    int in_planes = 32, bi = 0;
+    for (int l = 0; l < 4; ++l)
+      for (int i = 0; i < w->num_blocks[l]; ++i, ++bi) {
+        const int p = 32 << l, s = (i == 0 && l > 0) ? 2 : 1;
+        const bool need = s != 1 || in_planes != 4 * p;
+        B200_CHECK(need == (w->block_shortcut[bi].conv_weight != nullptr), B200_ERR_INVALID,
+                   "layer%d.%d: shortcut %s (stride %d, %d -> %d channels)", l + 1, i, need ? "missing" : "unexpected",
+                   s, in_planes, 4 * p);
+        in_planes = 4 * p;
+      }
+  }
+  B200_CHECK(w->seg1_weight && w->seg1_bias, B200_ERR_INVALID, "seg_1 missing");
+  DeviceGuard g(ctx->device);
+  EmbWeights& E = ctx->emb;
+  int rc;
+  E.loaded = false;
+  release_weights(ctx, &ctx->owned_emb);
+  E.blocks.clear();
+  E.bottlenecks.clear();
+  E.C = 1024;
+  if ((rc = build_fbank_constants(ctx))) return rc;
+  {
+    const b200_conv_bn& s = w->stem;
+    B200_CHECK(s.conv_weight && s.bn_weight && s.bn_bias && s.bn_mean && s.bn_var, B200_ERR_INVALID, "stem missing");
+    std::vector<float> cw(32 * 9), cb(32);
+    for (int c = 0; c < 32; ++c) {
+      const float sc = s.bn_weight[c] / std::sqrt(s.bn_var[c] + 1e-5f);
+      cb[c] = s.bn_bias[c] - s.bn_mean[c] * sc;
+      for (int k = 0; k < 9; ++k) cw[c * 9 + k] = s.conv_weight[c * 9 + k] * sc;
+    }
+    if ((rc = upload(ctx, cw, &E.conv1_w))) return rc;
+    if ((rc = upload(ctx, cb, &E.conv1_b))) return rc;
+  }
+  int in_planes = 32, bi = 0;
+  for (int l = 0; l < 4; ++l)
+    for (int i = 0; i < w->num_blocks[l]; ++i, ++bi) {
+      BottleneckWeights B;
+      const int p = 32 << l, s = (i == 0 && l > 0) ? 2 : 1;
+      if ((rc = make_conv(ctx, w->block_conv1[bi], in_planes, p, 1, 1, &B.conv1))) return rc;
+      if ((rc = make_conv(ctx, w->block_conv2[bi], p, p, 3, s, &B.conv2))) return rc;
+      if ((rc = make_conv(ctx, w->block_conv3[bi], p, 4 * p, 1, 1, &B.conv3))) return rc;
+      B.has_shortcut = w->block_shortcut[bi].conv_weight != nullptr;
+      if (B.has_shortcut)
+        if ((rc = make_conv(ctx, w->block_shortcut[bi], in_planes, 4 * p, 1, s, &B.shortcut))) return rc;
+      in_planes = 4 * p;
+      E.bottlenecks.push_back(B);
+    }
+  const size_t K = (size_t)2 * 10 * E.C;
+  std::vector<float> sw(w->seg1_weight, w->seg1_weight + (size_t)kEmbDim * K), sb(w->seg1_bias, w->seg1_bias + kEmbDim);
   {
     std::vector<__half> hi(sw.size()), lo(sw.size());
     for (size_t i = 0; i < sw.size(); ++i) {
@@ -679,9 +754,13 @@ int b200_powerset_to_multilabel(b200_ctx* ctx, const uint8_t* classes, int64_t n
 // ------------------------------------------------------------------------------------------------------
 struct EmbWs {
   float *fbank, *fmean, *stats;
-  __half *A, *Bf, *Cf;
+  __half *A, *Bf, *Cf, *D;
+  size_t cf_bytes;
 };
-static size_t carve_emb(int NB, void* base, EmbWs* w) {
+// ResNet34: A, Bf and Cf hold the largest activation, layer 1's 32 channels at 80 x 998 per chunk.  Bottleneck trunk
+// (every later layer is half the size of layer 1 at the same width): A and D the 4p = 128 channels of layer 1, Bf
+// layer 2 block 0's conv1 output (64 channels at layer 1's resolution), Cf layer 1's conv2 output (32 channels).
+static size_t carve_emb(const EmbWeights& E, int NB, void* base, EmbWs* w) {
   size_t off = 0;
   auto take = [&](size_t bytes) {
     off = align_up(off, 1024);
@@ -693,10 +772,13 @@ static size_t carve_emb(int NB, void* base, EmbWs* w) {
   const size_t act = (size_t)NB * kMel * kFbankFrames * 32 * sizeof(__half);   // largest activation (layer1)
   t.fbank = (float*)take((size_t)NB * kFbankFrames * kMel * sizeof(float));
   t.fmean = (float*)take((size_t)NB * kMel * sizeof(float));
-  t.stats = (float*)take((size_t)NB * kSpeakers * 2 * kStatsDim * sizeof(float));
-  t.A = (__half*)take(act);
-  t.Bf = (__half*)take(act);
+  t.stats = (float*)take((size_t)NB * kSpeakers * 2 * 10 * E.C * sizeof(float));
+  const bool bn = !E.bottlenecks.empty();
+  t.A = (__half*)take(bn ? 4 * act : act);
+  t.Bf = (__half*)take(bn ? 2 * act : act);
   t.Cf = (__half*)take(act);
+  t.D = bn ? (__half*)take(4 * act) : nullptr;
+  t.cf_bytes = act;
   if (w) *w = t;
   return align_up(off, 1024);
 }
@@ -719,9 +801,30 @@ static int block_run(b200_ctx* ctx, const BlockWeights& B, __half* A, __half* Bf
   return B200_OK;
 }
 
-// conv1 + 16 BasicBlocks on nb segments of T0 fbank frames; returns the buffer holding the result (NHWC fp16
-// [nb][10][T][256]) and its width T: T0 after layer 1, then (T + 2 - 3) / 2 + 1 after each of layers 2, 3 and 4
-// (125 for the 998 frames of 10 s)
+// one Bottleneck on nb segments: conv1 A -> Bf, conv2 Bf -> Cf, shortcut A -> D, conv3 Cf (+ A or D) -> A, in place
+// on the residual as block_run
+static int bottleneck_run(b200_ctx* ctx, const BottleneckWeights& B, __half* A, __half* Bf, __half* Cf, __half* D,
+                          int nb, int H, int Wd, cudaStream_t st) {
+  const int s = B.conv2.stride;
+  const int Ho = (H + 2 - 3) / s + 1, Wo = (Wd + 2 - 3) / s + 1;
+  const int impl = ctx->conv_impl, sms = ctx->num_sms;
+  int rc;
+  if ((rc = conv_forward(B.conv1, A, nullptr, Bf, nb, H, Wd, 1, impl, sms, st))) return rc;
+  if ((rc = conv_forward(B.conv2, Bf, nullptr, Cf, nb, H, Wd, 1, impl, sms, st))) return rc;
+  const __half* res = A;
+  if (B.has_shortcut) {
+    if ((rc = conv_forward(B.shortcut, A, nullptr, D, nb, H, Wd, 0, impl, sms, st))) return rc;
+    res = D;
+    ctx->launches += 1;
+  }
+  if ((rc = conv_forward(B.conv3, Cf, res, A, nb, Ho, Wo, 1, impl, sms, st))) return rc;
+  ctx->launches += 3;
+  return B200_OK;
+}
+
+// conv1 + the 16 BasicBlocks (or the Bottlenecks) on nb segments of T0 fbank frames; returns the buffer holding the
+// result (NHWC fp16 [nb][10][T][C]) and its width T: T0 after layer 1, then (T + 2 - 3) / 2 + 1 after each of layers
+// 2, 3 and 4 (125 for the 998 frames of 10 s)
 static int trunk_run(b200_ctx* ctx, const EmbWs& w, const int* frame0, int nb, int T0, cudaStream_t st,
                      const __half** result, int* T_out) {
   const EmbWeights& E = ctx->emb;
@@ -735,6 +838,11 @@ static int trunk_run(b200_ctx* ctx, const EmbWs& w, const int* frame0, int nb, i
   for (const BlockWeights& B : E.blocks) {
     const int s = B.conv1.stride;
     if ((rc = block_run(ctx, B, cur, s1, s2, nb, H, Wd, st))) return rc;
+    H = (H + 2 - 3) / s + 1; Wd = (Wd + 2 - 3) / s + 1;
+  }
+  for (const BottleneckWeights& B : E.bottlenecks) {
+    const int s = B.conv2.stride;
+    if ((rc = bottleneck_run(ctx, B, cur, s1, s2, w.D, nb, H, Wd, st))) return rc;
     H = (H + 2 - 3) / s + 1; Wd = (Wd + 2 - 3) / s + 1;
   }
   B200_CHECK(H == 10 && (T0 != kFbankFrames || Wd == kEmbT), B200_ERR_STATE, "unexpected trunk output %dx%d", H, Wd);
@@ -776,17 +884,19 @@ static int emb_forward_impl(b200_ctx* ctx, const float* wav, const int64_t* chun
   DeviceGuard g(ctx->device);
   cudaStream_t st = (cudaStream_t)stream;
   const int nbmax = num_chunks < ctx->emb_max_batch ? num_chunks : ctx->emb_max_batch;
-  // pooled statistics of ALL chunks as fp16 (hi, lo) pairs -> one tensor-core GEMM for the Linear 5120 -> 256
+  // pooled statistics of ALL chunks as fp16 (hi, lo) pairs -> one tensor-core GEMM for the Linear 20 C -> 256
+  // (5120 -> 256 for ResNet34; 20480 -> 256 for a bottleneck trunk, 80 KB of pairs per row)
+  const int C = ctx->emb.C;
   const size_t rows = (size_t)num_chunks * kSpeakers;
-  const size_t split_bytes = align_up(rows * 2 * kStatsDim * sizeof(__half), 1024);
-  const size_t sub_bytes = carve_emb(nbmax, nullptr, nullptr);
+  const size_t split_bytes = align_up(rows * 2 * 10 * C * sizeof(__half), 1024);
+  const size_t sub_bytes = carve_emb(ctx->emb, nbmax, nullptr, nullptr);
   int rc = ensure_ws(ctx, sub_bytes + 2 * split_bytes + 4096);
   if (rc) return rc;
   if ((rc = push_meta(ctx, chunk_off, chunk_valid, num_chunks, st))) return rc;
   FbankPlan plan;
   if ((rc = push_fbank_plan(ctx, chunk_off, chunk_valid, num_chunks, nbmax, ctx->fbank_share != 0, &plan, st))) return rc;
   EmbWs w;
-  carve_emb(nbmax, ctx->ws, &w);
+  carve_emb(ctx->emb, nbmax, ctx->ws, &w);
   __half* st_hi = reinterpret_cast<__half*>(reinterpret_cast<char*>(ctx->ws) + sub_bytes);
   __half* st_lo = reinterpret_cast<__half*>(reinterpret_cast<char*>(ctx->ws) + sub_bytes + split_bytes);
   const __half* feat = nullptr;
@@ -803,15 +913,16 @@ static int emb_forward_impl(b200_ctx* ctx, const float* wav, const int64_t* chun
       if ((rc = trunk_run(ctx, w, ctx->d_frame0 + c0, nb, kFbankFrames, st, &feat, &T))) return rc;
     }
     if (ctx->profile) ctx->trunk_segments += nb;
-    const size_t o = (size_t)c0 * kSpeakers * 2 * kStatsDim;
-    if ((rc = stats_pool_forward(feat, masks + (size_t)c0 * kSpeakers * kFrames, nullptr, st_hi + o, st_lo + o, nb, st)))
+    const size_t o = (size_t)c0 * kSpeakers * 2 * 10 * C;
+    if ((rc = stats_pool_forward(feat, masks + (size_t)c0 * kSpeakers * kFrames, nullptr, st_hi + o, st_lo + o, nb, C,
+                                 st)))
       return rc;
     ctx->launches += 1;
   }
-  // the Linear 5120 -> 256 of ALL chunks; with peers its epilogue also pushes every tile to the other GPUs (fused
+  // the Linear 20 C -> 256 of ALL chunks; with peers its epilogue also pushes every tile to the other GPUs (fused
   // all-gather of the embeddings over NVLink)
-  rc = gemm_tc_split(st_hi, st_lo, 2 * kStatsDim, ctx->emb.seg1_w_hi, ctx->emb.seg1_w_lo, 2 * kStatsDim, emb, kEmbDim,
-                     nullptr, nullptr, 0, ctx->emb.seg1_b, (int)rows, kEmbDim, 2 * kStatsDim, 0, ctx->num_sms, st,
+  rc = gemm_tc_split(st_hi, st_lo, 20 * C, ctx->emb.seg1_w_hi, ctx->emb.seg1_w_lo, 20 * C, emb, kEmbDim,
+                     nullptr, nullptr, 0, ctx->emb.seg1_b, (int)rows, kEmbDim, 20 * C, 0, ctx->num_sms, st,
                      emb_peers, n_peers);
   ctx->launches += 1;
   return rc;
@@ -858,10 +969,11 @@ int b200_emb_trunk(b200_ctx* ctx, const float* fbank, int32_t num_chunks, float*
   DeviceGuard g(ctx->device);
   cudaStream_t st = (cudaStream_t)stream;
   const int nbmax = num_chunks < ctx->emb_max_batch ? num_chunks : ctx->emb_max_batch;
-  int rc = ensure_ws(ctx, carve_emb(nbmax, nullptr, nullptr) + 4096);
+  int rc = ensure_ws(ctx, carve_emb(ctx->emb, nbmax, nullptr, nullptr) + 4096);
   if (rc) return rc;
   EmbWs w;
-  carve_emb(nbmax, ctx->ws, &w);
+  carve_emb(ctx->emb, nbmax, ctx->ws, &w);
+  const int C = ctx->emb.C;
   for (int c0 = 0; c0 < num_chunks; c0 += nbmax) {
     const int nb = (num_chunks - c0) < nbmax ? (num_chunks - c0) : nbmax;
     B200_CUDA_OK(cudaMemcpyAsync(w.fbank, fbank + (size_t)c0 * kFbankFrames * kMel,
@@ -870,7 +982,7 @@ int b200_emb_trunk(b200_ctx* ctx, const float* fbank, int32_t num_chunks, float*
     const __half* feat = nullptr;
     int T = 0;
     if ((rc = trunk_run(ctx, w, nullptr, nb, kFbankFrames, st, &feat, &T))) return rc;
-    if ((rc = frames_to_nchw(feat, frames + (size_t)c0 * 256 * 10 * kEmbT, nb, T, st))) return rc;
+    if ((rc = frames_to_nchw(feat, frames + (size_t)c0 * C * 10 * kEmbT, nb, T, C, st))) return rc;
     ctx->launches += 1;
   }
   return B200_OK;
@@ -878,9 +990,9 @@ int b200_emb_trunk(b200_ctx* ctx, const float* fbank, int32_t num_chunks, float*
 
 // ---- embeddings of utterances of any length ------------------------------------------------------------
 static int emb_linear(b200_ctx* ctx, const __half* st_hi, const __half* st_lo, int64_t rows, float* emb, cudaStream_t st) {
-  const int rc = gemm_tc_split(st_hi, st_lo, 2 * kStatsDim, ctx->emb.seg1_w_hi, ctx->emb.seg1_w_lo, 2 * kStatsDim, emb,
-                               kEmbDim, nullptr, nullptr, 0, ctx->emb.seg1_b, (int)rows, kEmbDim, 2 * kStatsDim, 0,
-                               ctx->num_sms, st);
+  const int K = 20 * ctx->emb.C;
+  const int rc = gemm_tc_split(st_hi, st_lo, K, ctx->emb.seg1_w_hi, ctx->emb.seg1_w_lo, K, emb, kEmbDim, nullptr,
+                               nullptr, 0, ctx->emb.seg1_b, (int)rows, kEmbDim, K, 0, ctx->num_sms, st);
   ctx->launches += 1;
   return rc;
 }
@@ -912,14 +1024,15 @@ int b200_emb_forward_utt(b200_ctx* ctx, const float* wav, const int64_t* off, in
   const int nbc = (int)(((int64_t)nbu * T0 + kFbankFrames - 1) / kFbankFrames);          // the same bytes in chunks
   int T = T0;                                                                            // trunk output width
   for (int l = 0; l < 3; ++l) T = (T + 2 - 3) / 2 + 1;
+  const int C = ctx->emb.C;
   const size_t rows = (size_t)num_utts * S;
-  const size_t split_bytes = align_up(rows * 2 * kStatsDim * sizeof(__half), 1024);
-  const size_t sub_bytes = carve_emb(nbc, nullptr, nullptr);
+  const size_t split_bytes = align_up(rows * 2 * 10 * C * sizeof(__half), 1024);
+  EmbWs w;
+  const size_t sub_bytes = carve_emb(ctx->emb, nbc, nullptr, &w);
   // fmean ([nbu][80] fp32) lives in the Bf scratch until the first block, the pooling partials in Cf after the
-  // trunk: both fit since nbu * T0 <= nbc * 998 frames and Bf / Cf hold nbc * 998 * 80 * 32 fp16
-  const size_t act_bytes = (size_t)nbc * kMel * kFbankFrames * 32 * sizeof(__half);
-  const size_t part_bytes = pool_scratch_bytes(nbu, S, T);
-  B200_CHECK(part_bytes <= act_bytes, B200_ERR_INVALID,
+  // trunk: fmean fits since nbu * T0 <= nbc * 998 frames and Bf / Cf hold at least nbc * 998 * 80 * 32 fp16
+  const size_t part_bytes = pool_scratch_bytes(nbu, S, T, C);
+  B200_CHECK(part_bytes <= w.cf_bytes, B200_ERR_INVALID,
              "%d speakers x %d frames: pooling scratch exceeds the sub-batch workspace", S, T);
   int rc = ensure_ws(ctx, sub_bytes + 2 * split_bytes + 4096);
   if (rc) return rc;
@@ -927,8 +1040,7 @@ int b200_emb_forward_utt(b200_ctx* ctx, const float* wav, const int64_t* off, in
   std::vector<b200::FbankRun> runs((size_t)num_utts);                                    // one private run each
   for (int i = 0; i < num_utts; ++i) runs[i] = b200::FbankRun{(long long)off[i], (i % nbu) * T0, (int)num_samples};
   B200_CUDA_OK(cudaMemcpyAsync(ctx->d_runs, runs.data(), sizeof(b200::FbankRun) * runs.size(), cudaMemcpyHostToDevice, st));
-  EmbWs w;
-  carve_emb(nbc, ctx->ws, &w);
+  carve_emb(ctx->emb, nbc, ctx->ws, &w);
   w.fmean = reinterpret_cast<float*>(w.Bf);
   double* part = reinterpret_cast<double*>(w.Cf);
   __half* st_hi = reinterpret_cast<__half*>(reinterpret_cast<char*>(ctx->ws) + sub_bytes);
@@ -942,9 +1054,9 @@ int b200_emb_forward_utt(b200_ctx* ctx, const float* wav, const int64_t* off, in
     int Tt = 0;
     if ((rc = trunk_run(ctx, w, nullptr, nb, T0, st, &feat, &Tt))) return rc;
     B200_CHECK(Tt == T, B200_ERR_STATE, "trunk output width %d, expected %d", Tt, T);
-    const size_t o = (size_t)u0 * S * 2 * kStatsDim;
+    const size_t o = (size_t)u0 * S * 2 * 10 * C;
     if ((rc = weighted_pool_forward(feat, nullptr, weights ? weights + (size_t)u0 * S * num_weights : nullptr, nb, T, S,
-                                    num_weights, part, st_hi + o, st_lo + o, st)))
+                                    num_weights, C, part, st_hi + o, st_lo + o, st)))
       return rc;
     ctx->launches += T <= kPoolSlice ? 1 : 3;
   }
@@ -961,16 +1073,17 @@ int b200_emb_forward_embedding(b200_ctx* ctx, const float* frames, int32_t B, in
   DeviceGuard g(ctx->device);
   cudaStream_t st = (cudaStream_t)stream;
   const int S = weights ? num_speakers : 1;
+  const int C = ctx->emb.C;
   const size_t rows = (size_t)B * S;
-  const size_t split_bytes = align_up(rows * 2 * kStatsDim * sizeof(__half), 1024);
-  const size_t part_bytes = align_up(pool_scratch_bytes(B, S, T), 1024);
+  const size_t split_bytes = align_up(rows * 2 * 10 * C * sizeof(__half), 1024);
+  const size_t part_bytes = align_up(pool_scratch_bytes(B, S, T, C), 1024);
   int rc = ensure_ws(ctx, 2 * split_bytes + part_bytes + 4096);
   if (rc) return rc;
   char* base = reinterpret_cast<char*>(ctx->ws);
   __half* st_hi = reinterpret_cast<__half*>(base);
   __half* st_lo = reinterpret_cast<__half*>(base + split_bytes);
   double* part = part_bytes ? reinterpret_cast<double*>(base + 2 * split_bytes) : nullptr;
-  if ((rc = weighted_pool_forward(nullptr, frames, weights, B, T, S, num_weights, part, st_hi, st_lo, st))) return rc;
+  if ((rc = weighted_pool_forward(nullptr, frames, weights, B, T, S, num_weights, C, part, st_hi, st_lo, st))) return rc;
   ctx->launches += T <= kPoolSlice ? 1 : 3;
   return emb_linear(ctx, st_hi, st_lo, (int64_t)rows, emb, st);
 }

@@ -1,4 +1,4 @@
-// Embedding path (kaldi fbank -> ResNet34 trunk -> masked stats pooling -> Linear) declarations.
+// Embedding path (kaldi fbank -> ResNet34 or bottleneck ResNet trunk -> masked stats pooling -> Linear) declarations.
 #pragma once
 #include "common.cuh"
 
@@ -29,12 +29,20 @@ struct BlockWeights {
   bool has_shortcut = false;
 };
 
+// Bottleneck (resnet.py:148-212): 1x1 conv1 (in -> p), 3x3 conv2 (p -> p, stride), 1x1 conv3 (p -> 4p)
+struct BottleneckWeights {
+  ConvLayer conv1, conv2, conv3, shortcut;
+  bool has_shortcut = false;
+};
+
 struct EmbWeights {
   bool loaded = false;
+  int C = 256;                   // trunk output channels: 256 (ResNet34) or 1024 (bottleneck trunks)
   float* conv1_w = nullptr;      // [32][9] folded
   float* conv1_b = nullptr;      // [32]
-  std::vector<BlockWeights> blocks;   // 16 BasicBlocks
-  float* seg1_w = nullptr;       // [256][5120] fp32 (PyTorch layout)
+  std::vector<BlockWeights> blocks;             // ResNet34: 16 BasicBlocks
+  std::vector<BottleneckWeights> bottlenecks;   // ResNet152 / 221 / 293: the Bottleneck blocks (blocks is empty)
+  float* seg1_w = nullptr;       // [256][20 C] fp32 (PyTorch layout)
   float* seg1_b = nullptr;       // [256]
   __half* seg1_w_hi = nullptr;   // fp16 (hi, lo) split of seg1_w for the tensor-core GEMM
   __half* seg1_w_lo = nullptr;
@@ -72,22 +80,24 @@ struct FbankRun {
 int fbank_forward(const EmbWeights& W, const float* wav, const FbankRun* runs, int nruns, int nrows,
                   const int* frame0, int B, int T0, float* fbank, float* fmean, cudaStream_t stream);
 int fbank_center(float* fbank, const float* fmean, int B, cudaStream_t stream);
-// NHWC fp16 [B][10][T][256] -> NCHW fp32 [B][256][10][T]
-int frames_to_nchw(const __half* feat, float* out, int B, int T, cudaStream_t stream);
+// NHWC fp16 [B][10][T][C] -> NCHW fp32 [B][C][10][T]
+int frames_to_nchw(const __half* feat, float* out, int B, int T, int C, cudaStream_t stream);
 
-// masked statistics pooling: feat [B][10][125][256] fp16 NHWC, masks [B][3][589] u8 -> stats [B*3][5120] fp32
+// masked statistics pooling: feat [B][10][125][C] fp16 NHWC (C = 256 or 1024), masks [B][3][589] u8 -> stats
+// [B*3][20 C] fp32
 int stats_pool_forward(const __half* feat, const unsigned char* masks, float* stats, __half* stats_hi,
-                       __half* stats_lo, int B, cudaStream_t stream);
+                       __half* stats_lo, int B, int C, cudaStream_t stream);
 // weighted statistics pooling for any T, S and Tw (pooling.py:30-61, 76-130) -> the fp16 (hi, lo) rows of the Linear:
-// feat NHWC fp16 [B][10][T][256] (trunk output) or frames NCHW fp32 [B][256][10][T] (caller frames, exactly one of
+// feat NHWC fp16 [B][10][T][C] (trunk output) or frames NCHW fp32 [B][C][10][T] (caller frames, exactly one of
 // the two), w fp32 [B][S][Tw] any real values or NULL (mean and std(correction=1) over the T frames, S = 1).  The
 // weights reach the T frames by torch's CUDA nearest index (upsample_nearest1d).  T is split into slices of
 // kPoolSlice frames; with one slice the sums are the stats_pool_forward ones in the same order, with several the
 // per-slice fp32 sums are combined in fp64 in slice order (deterministic, no atomics).  part: fp64 scratch of
-// pool_scratch_bytes(B, S, T) bytes (none with one slice).  Rows of stats_hi / stats_lo: (b * S + s) * 5120.
+// pool_scratch_bytes(B, S, T, C) bytes (none with one slice).  Rows of stats_hi / stats_lo: (b * S + s) * 20 C.
+// C = 256 or 1024.
 constexpr int kPoolSlice = 512;
-size_t pool_scratch_bytes(int B, int S, int T);
-int weighted_pool_forward(const __half* feat, const float* frames, const float* w, int B, int T, int S, int Tw,
+size_t pool_scratch_bytes(int B, int S, int T, int C);
+int weighted_pool_forward(const __half* feat, const float* frames, const float* w, int B, int T, int S, int Tw, int C,
                           double* part, __half* stats_hi, __half* stats_lo, cudaStream_t stream);
 // generic weighted pooling used by the known-answer tests: seq [B][F][T] fp32, w [B][S][Tw] fp32 -> [B][S][2F]
 int stats_pool_generic(const float* seq, const float* w, float* out, int B, int F, int T, int S, int Tw,

@@ -40,15 +40,16 @@ constexpr int kMaxSlots = 16;                               // row slots of conv
 
 // +bias (+residual) -> ReLU -> fp16 of the 64 x N accumulator fragment of output pixels [w0, w0 + 64) of image row
 // `row` (= b * H_out + h).  A residual aliasing `out` is read before it is overwritten, by the same thread.
-template <int N>
+// WIDE: the fragment is output channels [n0, n0 + N) of C_out (n0 = blockIdx.y * N), pixels C_out channels apart.
+template <int N, bool WIDE = false>
 __device__ __forceinline__ void conv_epilogue(const float* acc, const ConvParams& p, size_t row, int w0) {
   const int lane = threadIdx.x & 31;
-  const int c0 = 2 * (lane & 3);
+  const int c0 = 2 * (lane & 3) + (WIDE ? (int)blockIdx.y * N : 0);
 #pragma unroll
   for (int i = 0; i < 2; ++i) {
     const int w = w0 + ((threadIdx.x >> 5) & 3) * 16 + (lane >> 2) + 8 * i;
     if (w >= p.W_out) continue;
-    const size_t pix = (row * p.W_out + w) * (size_t)N;
+    const size_t pix = (row * p.W_out + w) * (size_t)(WIDE ? p.C_out : N);
     // up to C_out = 64 all of the pixel's residual loads are issued before its first store: `out` may alias
     // `residual`, so a load after a store cannot be hoisted and each would wait a full memory round trip (from 128 on
     // the registers are not there: conv_tc_kernel<256> would spill)
@@ -73,7 +74,8 @@ __device__ __forceinline__ void conv_epilogue(const float* acc, const ConvParams
   }
 }
 
-template <int N, int CK>
+// WIDE: C_out > 256 (the bottleneck trunk's 512 / 1024-channel 1x1 convs), grid.y = the 256-channel column tile
+template <int N, int CK, bool WIDE = false>
 __global__ void __launch_bounds__(kWgThreads, N == 256 ? 1 : 2)
 conv_tc_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB, ConvParams p) {
   extern __shared__ uint8_t smem_raw[];
@@ -107,7 +109,8 @@ conv_tc_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ 
             mbar_expect_tx(bar_full + 8 * stage, p.a_tx + p.b_bytes);
             const uint32_t sa = stage0 + stage * stage_bytes;
             tma_load_4d(&tmA, bar_full + 8 * stage, sa, cc * CK, w_base + kw, h_base + kh, b);
-            tma_load_3d(&tmB, bar_full + 8 * stage, sa + p.a_bytes, cc * CK, 0, kh * p.taps_w + kw);
+            tma_load_3d(&tmB, bar_full + 8 * stage, sa + p.a_bytes, cc * CK, WIDE ? (int)blockIdx.y * N : 0,
+                        kh * p.taps_w + kw);
             if (++stage == p.nstages) { stage = 0; phase ^= 1; }
           }
     }
@@ -136,7 +139,7 @@ conv_tc_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ 
     if (++stage == p.nstages) { stage = 0; phase ^= 1; }
   }
   wg_wait<0>();
-  conv_epilogue<N>(acc, p, (size_t)bh, wt * kTileM + wg * 64);
+  conv_epilogue<N, WIDE>(acc, p, (size_t)bh, wt * kTileM + wg * 64);
 }
 
 template <int N, int CK>
@@ -427,9 +430,12 @@ int conv_forward(const ConvLayer& L, const __half* in, const __half* residual, _
   p.swizzle = (p.Ck == 64) ? 128 : 64;
   p.tiles_w = ceil_div(p.W_out, kTileM);
   p.num_tiles = B * p.H_out * p.tiles_w;
-  B200_CHECK(L.C_in % p.Ck == 0 && (L.C_out == 64 || (L.C_out >= 128 && L.C_out <= 256 && L.C_out % 128 == 0 && p.Ck == 64) ||
-                                    (L.C_out == 32 && p.Ck == 32)),
+  // C_out 32 / 64 / 128 with either channel chunk; 256 and, as 256-wide column tiles (grid.y), 512 / 768 / 1024
+  // with Ck = 64
+  B200_CHECK(L.C_in % p.Ck == 0 && (L.C_out == 32 || L.C_out == 64 || L.C_out == 128 ||
+                                    (L.C_out % 256 == 0 && L.C_out <= 1024 && p.Ck == 64)),
              B200_ERR_STATE, "conv %d -> %d channels unsupported", L.C_in, L.C_out);
+  const int n_tile = std::min(L.C_out, 256);               // output channels per CTA of conv_tc_kernel
   B200_CHECK(impl >= 0 && impl <= 2, B200_ERR_INVALID,
              "conv_impl %d unknown (0 = CUDA cores, 1 = tensor cores, 2 = tensor cores, one weight tap per stage)", impl);
 
@@ -467,10 +473,10 @@ int conv_forward(const ConvLayer& L, const __half* in, const __half* residual, _
     p.bands = ceil_div(p.H_out, p.band);
     p.num_tiles = strips * p.bands;
   } else {
-    p.b_bytes = (uint32_t)(L.C_out * p.Ck * 2);
+    p.b_bytes = (uint32_t)(n_tile * p.Ck * 2);
     // C_out = 256 needs 128 accumulator registers per thread: one CTA per SM with 4 deep stages; the narrower layers
     // run two CTAs per SM (registers allow it) on half the shared memory each
-    const uint32_t budget = L.C_out == 256 ? 200u * 1024 : 100u * 1024;
+    const uint32_t budget = n_tile == 256 ? 200u * 1024 : 100u * 1024;
     p.nstages = std::min(budget / (p.a_bytes + p.b_bytes), 8u);
     B200_CHECK(p.nstages >= 2, B200_ERR_STATE, "conv %d -> %d: shared memory plan too shallow", L.C_in, L.C_out);
     smem = 1024 + 1024 + (size_t)p.nstages * (p.a_bytes + p.b_bytes);
@@ -494,7 +500,7 @@ int conv_forward(const ConvLayer& L, const __half* in, const __half* residual, _
     // conv_row_kernel loads the nine taps as three boxes of three
     cuuint64_t dims[3] = {(cuuint64_t)L.C_in, (cuuint64_t)L.C_out, (cuuint64_t)(L.ksize * L.ksize)};
     cuuint64_t strides[2] = {(cuuint64_t)L.C_in * 2, (cuuint64_t)L.C_out * L.C_in * 2};
-    cuuint32_t box[3] = {(cuuint32_t)p.Ck, (cuuint32_t)L.C_out, rows ? 3u : 1u};
+    cuuint32_t box[3] = {(cuuint32_t)p.Ck, (cuuint32_t)n_tile, rows ? 3u : 1u};
     cuuint32_t estr[3] = {1, 1, 1};
     CUresult r = enc(&tmB, CU_TENSOR_MAP_DATA_TYPE_FLOAT16, 3, const_cast<__half*>(L.w), dims, strides, box, estr,
                      CU_TENSOR_MAP_INTERLEAVE_NONE,
@@ -504,17 +510,25 @@ int conv_forward(const ConvLayer& L, const __half* in, const __half* residual, _
   }
   auto launch = [&](auto kernel) -> int {
     B200_CUDA_OK(cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-    const int grid = rows ? std::min(p.num_tiles, ctas) : p.num_tiles;
-    kernel<<<(unsigned)grid, kWgThreads, smem, stream>>>(tmA, tmB, p);
+    const dim3 grid((unsigned)(rows ? std::min(p.num_tiles, ctas) : p.num_tiles), (unsigned)(L.C_out / n_tile));
+    kernel<<<grid, kWgThreads, smem, stream>>>(tmA, tmB, p);
     B200_CUDA_OK(cudaGetLastError());
     return B200_OK;
   };
   if (rows) return p.Ck == 32 ? launch(conv_row_kernel<32, 32>) : launch(conv_row_kernel<64, 64>);
-  if (p.Ck == 32) return L.C_out == 32 ? launch(conv_tc_kernel<32, 32>) : launch(conv_tc_kernel<64, 32>);
+  if (p.Ck == 32) {
+    switch (L.C_out) {
+      case 32: return launch(conv_tc_kernel<32, 32>);
+      case 64: return launch(conv_tc_kernel<64, 32>);
+      default: return launch(conv_tc_kernel<128, 32>);   // bottleneck layer 1: conv3 / shortcut 32 -> 128
+    }
+  }
   switch (L.C_out) {
+    case 32: return launch(conv_tc_kernel<32, 64>);       // bottleneck layer 1: conv1 128 -> 32
     case 64: return launch(conv_tc_kernel<64, 64>);
     case 128: return launch(conv_tc_kernel<128, 64>);
-    default: return launch(conv_tc_kernel<256, 64>);
+    case 256: return launch(conv_tc_kernel<256, 64>);
+    default: return launch(conv_tc_kernel<256, 64, true>);
   }
 }
 

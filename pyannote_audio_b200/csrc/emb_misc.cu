@@ -213,19 +213,20 @@ int fbank_center(float* fbank, const float* fmean, int B, cudaStream_t stream) {
   return B200_OK;
 }
 
-__global__ void frames_to_nchw_kernel(const __half* __restrict__ feat, float* __restrict__ out, int T, size_t total) {
+__global__ void frames_to_nchw_kernel(const __half* __restrict__ feat, float* __restrict__ out, int T, int C,
+                                      size_t total) {
   const size_t idx = (size_t)blockIdx.x * blockDim.x + threadIdx.x;   // over NCHW output
   if (idx >= total) return;
   const size_t t = idx % T;
   const size_t h = (idx / T) % 10;
-  const size_t c = (idx / ((size_t)T * 10)) % 256;
-  const size_t b = idx / ((size_t)T * 10 * 256);
-  out[idx] = __half2float(feat[((b * 10 + h) * T + t) * 256 + c]);
+  const size_t c = (idx / ((size_t)T * 10)) % C;
+  const size_t b = idx / ((size_t)T * 10 * C);
+  out[idx] = __half2float(feat[((b * 10 + h) * T + t) * C + c]);
 }
 
-int frames_to_nchw(const __half* feat, float* out, int B, int T, cudaStream_t stream) {
-  const size_t total = (size_t)B * 256 * 10 * T;
-  frames_to_nchw_kernel<<<(unsigned)((total + 255) / 256), 256, 0, stream>>>(feat, out, T, total);
+int frames_to_nchw(const __half* feat, float* out, int B, int T, int C, cudaStream_t stream) {
+  const size_t total = (size_t)B * C * 10 * T;
+  frames_to_nchw_kernel<<<(unsigned)((total + 255) / 256), 256, 0, stream>>>(feat, out, T, C, total);
   B200_CUDA_OK(cudaGetLastError());
   return B200_OK;
 }
@@ -242,15 +243,16 @@ int fbank_forward(const EmbWeights& W, const float* wav, const FbankRun* runs, i
 }
 
 // ------------------------------------------------------------------------------------------------
-// masked stats pooling on the trunk output, all 3 local speakers from one pass
+// masked stats pooling on the trunk output, all 3 local speakers from one pass; C = trunk channels (256 or 1024)
 // ------------------------------------------------------------------------------------------------
+template <int C>
 __global__ void __launch_bounds__(256) stats_pool_kernel(const __half* __restrict__ feat,
                                                          const unsigned char* __restrict__ masks,
                                                          float* __restrict__ stats, __half* __restrict__ stats_hi,
                                                          __half* __restrict__ stats_lo) {
-  // grid (10 freq rows, B); thread = channel c; feat[b][h][t][c]
+  // grid (10 freq rows, B, C / 256); thread = channel c; feat[b][h][t][c]
   __shared__ float s_w[kSpeakers][kEmbT];
-  const int h = blockIdx.x, b = blockIdx.y, c = threadIdx.x;
+  const int h = blockIdx.x, b = blockIdx.y, c = (C == 256 ? 0 : (int)blockIdx.z * 256) + threadIdx.x;
   for (int i = threadIdx.x; i < kSpeakers * kEmbT; i += blockDim.x) {
     const int s = i / kEmbT, t = i % kEmbT;
     // F.interpolate(mode="nearest"): src = floor(dst * in / out)   (pooling.py:116-117)
@@ -258,12 +260,12 @@ __global__ void __launch_bounds__(256) stats_pool_kernel(const __half* __restric
     s_w[s][t] = (float)masks[((size_t)b * kSpeakers + s) * kFrames + src];
   }
   __syncthreads();
-  const __half* fp = feat + (((size_t)b * 10 + h) * kEmbT) * 256 + c;
+  const __half* fp = feat + (((size_t)b * 10 + h) * kEmbT) * C + c;
   float v1[kSpeakers], v2[kSpeakers], sx[kSpeakers];
 #pragma unroll
   for (int s = 0; s < kSpeakers; ++s) { v1[s] = 0.f; v2[s] = 0.f; sx[s] = 0.f; }
   for (int t = 0; t < kEmbT; ++t) {
-    const float x = __half2float(fp[(size_t)t * 256]);
+    const float x = __half2float(fp[(size_t)t * C]);
 #pragma unroll
     for (int s = 0; s < kSpeakers; ++s) {
       const float w = s_w[s][t];
@@ -280,7 +282,7 @@ __global__ void __launch_bounds__(256) stats_pool_kernel(const __half* __restric
     sd[s] = 0.f;
   }
   for (int t = 0; t < kEmbT; ++t) {
-    const float x = __half2float(fp[(size_t)t * 256]);
+    const float x = __half2float(fp[(size_t)t * C]);
 #pragma unroll
     for (int s = 0; s < kSpeakers; ++s) {
       const float d = x - mean[s];
@@ -290,26 +292,28 @@ __global__ void __launch_bounds__(256) stats_pool_kernel(const __half* __restric
 #pragma unroll
   for (int s = 0; s < kSpeakers; ++s) {
     const float var = sd[s] / (v1[s] - v2[s] / v1[s] + 1e-8f);
-    const size_t row = ((size_t)b * kSpeakers + s) * (2 * kStatsDim);
+    const size_t row = ((size_t)b * kSpeakers + s) * (2 * 10 * C);
     const float sdv = sqrtf(var);
     if (stats) {
       stats[row + c * 10 + h] = mean[s];
-      stats[row + kStatsDim + c * 10 + h] = sdv;
+      stats[row + 10 * C + c * 10 + h] = sdv;
     }
-    if (stats_hi) {   // (hi, lo) fp16 split consumed by gemm_tc_split (Linear 5120 -> 256)
+    if (stats_hi) {   // (hi, lo) fp16 split consumed by gemm_tc_split (Linear 20 C -> 256)
       const __half mh = __float2half_rn(mean[s]), sh = __float2half_rn(sdv);
       stats_hi[row + c * 10 + h] = mh;
       stats_lo[row + c * 10 + h] = __float2half_rn(mean[s] - __half2float(mh));
-      stats_hi[row + kStatsDim + c * 10 + h] = sh;
-      stats_lo[row + kStatsDim + c * 10 + h] = __float2half_rn(sdv - __half2float(sh));
+      stats_hi[row + 10 * C + c * 10 + h] = sh;
+      stats_lo[row + 10 * C + c * 10 + h] = __float2half_rn(sdv - __half2float(sh));
     }
   }
 }
 
 int stats_pool_forward(const __half* feat, const unsigned char* masks, float* stats, __half* stats_hi,
-                       __half* stats_lo, int B, cudaStream_t stream) {
-  dim3 grid(10, B);
-  stats_pool_kernel<<<grid, 256, 0, stream>>>(feat, masks, stats, stats_hi, stats_lo);
+                       __half* stats_lo, int B, int C, cudaStream_t stream) {
+  B200_CHECK(C == 256 || C == 1024, B200_ERR_STATE, "stats pooling: %d channels unsupported", C);
+  dim3 grid(10, B, C / 256);
+  if (C == 256) stats_pool_kernel<256><<<grid, 256, 0, stream>>>(feat, masks, stats, stats_hi, stats_lo);
+  else stats_pool_kernel<1024><<<grid, 256, 0, stream>>>(feat, masks, stats, stats_hi, stats_lo);
   B200_CUDA_OK(cudaGetLastError());
   return B200_OK;
 }
@@ -329,12 +333,14 @@ __device__ __forceinline__ int nearest_src(int dst, int T, int Tw, float scale) 
 __device__ __forceinline__ float to_f(__half v) { return __half2float(v); }
 __device__ __forceinline__ float to_f(float v) { return v; }
 
+// stats row of C channels: mean at c * 10 + h, std 10 * C further
+template <int C>
 __device__ __forceinline__ void store_split(__half* hi, __half* lo, size_t row, int c, int h, float mean, float sdv) {
   const __half mh = __float2half_rn(mean), sh = __float2half_rn(sdv);
   hi[row + c * 10 + h] = mh;
   lo[row + c * 10 + h] = __float2half_rn(mean - __half2float(mh));
-  hi[row + kStatsDim + c * 10 + h] = sh;
-  lo[row + kStatsDim + c * 10 + h] = __float2half_rn(sdv - __half2float(sh));
+  hi[row + 10 * C + c * 10 + h] = sh;
+  lo[row + 10 * C + c * 10 + h] = __float2half_rn(sdv - __half2float(sh));
 }
 
 struct PoolArgs {
@@ -342,36 +348,37 @@ struct PoolArgs {
   const float* w;         // [B][S][Tw] or NULL
   int S, T, Tw, nslices;
   float scale;            // (float)Tw / T
-  double* part;           // [B * S][10][nslices][4][256]: sum w (sum x), sum w^2, sum w x, sum w (x - mean)^2
+  double* part;           // [B * S][10][nslices][4][C]: sum w (sum x), sum w^2, sum w x, sum w (x - mean)^2
   __half *hi, *lo;
 };
 
-// x of (b, h, channel c): NHWC [B][10][T][256] (stride 256 between frames) or NCHW [B][256][10][T] (stride 1)
-template <typename X>
+// x of (b, h, channel c): NHWC [B][10][T][C] (stride C between frames) or NCHW [B][C][10][T] (stride 1)
+template <typename X, int C>
 __device__ __forceinline__ const X* pool_row(const PoolArgs& a, int b, int h, int c, size_t* stride) {
   const X* x = static_cast<const X*>(a.x);
-  if constexpr (sizeof(X) == 2) { *stride = 256; return x + ((size_t)b * 10 + h) * a.T * 256 + c; }
-  else { *stride = 1; return x + (((size_t)b * 256 + c) * 10 + h) * a.T; }
+  if constexpr (sizeof(X) == 2) { *stride = C; return x + ((size_t)b * 10 + h) * a.T * C + c; }
+  else { *stride = 1; return x + (((size_t)b * C + c) * 10 + h) * a.T; }
 }
 
 // PHASE 0: the whole sequence in one slice, finished here (the stats_pool_kernel sums, in its order);
 // PHASE 1: per-slice fp32 sums; PHASE 2: per-slice sum of w (x - mean)^2 around the mean of all slices' sums.
-// grid (B * S * 10, nslices), thread = channel
-template <int PHASE, typename X>
+// grid (B * S * 10, nslices, C / 256), thread = channel
+template <int PHASE, typename X, int C>
 __global__ void __launch_bounds__(256) wpool_kernel(PoolArgs a) {
   __shared__ float s_w[kPoolSlice];
-  const int row = blockIdx.x / 10, h = blockIdx.x % 10, c = threadIdx.x;   // row = b * S + s
+  const int row = blockIdx.x / 10, h = blockIdx.x % 10;                      // row = b * S + s
+  const int c = (C == 256 ? 0 : (int)blockIdx.z * 256) + threadIdx.x;
   const int b = row / a.S, sl = blockIdx.y;
   const int t0 = sl * kPoolSlice, t1 = min(a.T, t0 + kPoolSlice);
   size_t xs;
-  const X* xp = pool_row<X>(a, b, h, c, &xs);
+  const X* xp = pool_row<X, C>(a, b, h, c, &xs);
   const bool weighted = a.w != nullptr;
   if (weighted) {
     const float* wr = a.w + (size_t)row * a.Tw;
     for (int i = threadIdx.x; i < t1 - t0; i += blockDim.x) s_w[i] = wr[nearest_src(t0 + i, a.T, a.Tw, a.scale)];
   }
   __syncthreads();
-  double* part = a.part + (((size_t)row * 10 + h) * a.nslices) * 4 * 256 + c;   // slot k of slice j: [(j*4+k)*256]
+  double* part = a.part + (((size_t)row * 10 + h) * a.nslices) * 4 * C + c;     // slot k of slice j: [(j*4+k)*C]
   if (PHASE == 0 || PHASE == 1) {
     float v1 = 0.f, v2 = 0.f, sx = 0.f;
     if (weighted) {
@@ -386,12 +393,12 @@ __global__ void __launch_bounds__(256) wpool_kernel(PoolArgs a) {
       for (int t = t0; t < t1; ++t) sx += to_f(xp[(size_t)t * xs]);
     }
     if (PHASE == 1) {
-      part[(sl * 4 + 0) * 256] = weighted ? (double)v1 : (double)sx;
-      part[(sl * 4 + 1) * 256] = (double)v2;
-      part[(sl * 4 + 2) * 256] = (double)sx;
+      part[(sl * 4 + 0) * C] = weighted ? (double)v1 : (double)sx;
+      part[(sl * 4 + 1) * C] = (double)v2;
+      part[(sl * 4 + 2) * C] = (double)sx;
       return;
     }
-    const size_t orow = (size_t)row * (2 * kStatsDim);
+    const size_t orow = (size_t)row * (2 * 10 * C);
     if (weighted) {
       v1 += 1e-8f;
       const float mean = sx / v1;
@@ -401,7 +408,7 @@ __global__ void __launch_bounds__(256) wpool_kernel(PoolArgs a) {
         sd += d * d * s_w[t - t0];
       }
       const float var = sd / (v1 - v2 / v1 + 1e-8f);
-      store_split(a.hi, a.lo, orow, c, h, mean, sqrtf(var));
+      store_split<C>(a.hi, a.lo, orow, c, h, mean, sqrtf(var));
     } else {                                               // torch mean / std(correction=1): T = 1 gives NaN
       const float mean = sx / a.T;
       float acc = 0.f;
@@ -409,29 +416,31 @@ __global__ void __launch_bounds__(256) wpool_kernel(PoolArgs a) {
         const float d = to_f(xp[(size_t)t * xs]) - mean;
         acc += d * d;
       }
-      store_split(a.hi, a.lo, orow, c, h, mean, sqrtf(acc / (a.T - 1)));
+      store_split<C>(a.hi, a.lo, orow, c, h, mean, sqrtf(acc / (a.T - 1)));
     }
   } else {
     double s0 = 0.0, s2 = 0.0;                             // every slice's sums, in slice order
-    for (int j = 0; j < a.nslices; ++j) { s0 += part[(j * 4 + 0) * 256]; s2 += part[(j * 4 + 2) * 256]; }
+    for (int j = 0; j < a.nslices; ++j) { s0 += part[(j * 4 + 0) * C]; s2 += part[(j * 4 + 2) * C]; }
     const float mean = weighted ? (float)(s2 / (s0 + 1e-8)) : (float)(s0 / a.T);
     float sd = 0.f;
     for (int t = t0; t < t1; ++t) {
       const float d = to_f(xp[(size_t)t * xs]) - mean;
       sd += weighted ? d * d * s_w[t - t0] : d * d;
     }
-    part[(sl * 4 + 3) * 256] = (double)sd;
+    part[(sl * 4 + 3) * C] = (double)sd;
   }
 }
 
-// combine the slices in fp64, in slice order; grid B * S * 10, thread = channel
+// combine the slices in fp64, in slice order; grid (B * S * 10, 1, C / 256), thread = channel
+template <int C>
 __global__ void __launch_bounds__(256) wpool_final_kernel(PoolArgs a) {
-  const int row = blockIdx.x / 10, h = blockIdx.x % 10, c = threadIdx.x;
-  const double* part = a.part + (((size_t)row * 10 + h) * a.nslices) * 4 * 256 + c;
+  const int row = blockIdx.x / 10, h = blockIdx.x % 10;
+  const int c = (C == 256 ? 0 : (int)blockIdx.z * 256) + threadIdx.x;
+  const double* part = a.part + (((size_t)row * 10 + h) * a.nslices) * 4 * C + c;
   double s[4] = {0.0, 0.0, 0.0, 0.0};
   for (int j = 0; j < a.nslices; ++j)
 #pragma unroll
-    for (int k = 0; k < 4; ++k) s[k] += part[(j * 4 + k) * 256];
+    for (int k = 0; k < 4; ++k) s[k] += part[(j * 4 + k) * C];
   float mean;
   double var;
   if (a.w) {
@@ -442,15 +451,33 @@ __global__ void __launch_bounds__(256) wpool_final_kernel(PoolArgs a) {
     mean = (float)(s[0] / a.T);
     var = s[3] / (double)(a.T - 1);
   }
-  store_split(a.hi, a.lo, (size_t)row * (2 * kStatsDim), c, h, mean, (float)sqrt(var));
+  store_split<C>(a.hi, a.lo, (size_t)row * (2 * 10 * C), c, h, mean, (float)sqrt(var));
 }
 
-size_t pool_scratch_bytes(int B, int S, int T) {
+size_t pool_scratch_bytes(int B, int S, int T, int C) {
   const int nslices = ceil_div(T, kPoolSlice);
-  return nslices > 1 ? (size_t)B * S * 10 * nslices * 4 * 256 * sizeof(double) : 0;
+  return nslices > 1 ? (size_t)B * S * 10 * nslices * 4 * C * sizeof(double) : 0;
 }
 
-int weighted_pool_forward(const __half* feat, const float* frames, const float* w, int B, int T, int S, int Tw,
+template <int C>
+static void wpool_launch(const PoolArgs& a, bool nhwc, size_t rows, cudaStream_t stream) {
+  const dim3 grid((unsigned)(rows * 10), (unsigned)a.nslices, C / 256);
+  if (a.nslices == 1) {
+    if (nhwc) wpool_kernel<0, __half, C><<<grid, 256, 0, stream>>>(a);
+    else wpool_kernel<0, float, C><<<grid, 256, 0, stream>>>(a);
+  } else {
+    if (nhwc) {
+      wpool_kernel<1, __half, C><<<grid, 256, 0, stream>>>(a);
+      wpool_kernel<2, __half, C><<<grid, 256, 0, stream>>>(a);
+    } else {
+      wpool_kernel<1, float, C><<<grid, 256, 0, stream>>>(a);
+      wpool_kernel<2, float, C><<<grid, 256, 0, stream>>>(a);
+    }
+    wpool_final_kernel<C><<<dim3(grid.x, 1, C / 256), 256, 0, stream>>>(a);
+  }
+}
+
+int weighted_pool_forward(const __half* feat, const float* frames, const float* w, int B, int T, int S, int Tw, int C,
                           double* part, __half* stats_hi, __half* stats_lo, cudaStream_t stream) {
   B200_CHECK((feat == nullptr) != (frames == nullptr) && T >= 1 && S >= 1 && (w == nullptr ? S == 1 : Tw >= 1),
              B200_ERR_INVALID, "weighted pooling: bad arguments");
@@ -465,20 +492,9 @@ int weighted_pool_forward(const __half* feat, const float* frames, const float* 
   B200_CHECK(a.nslices <= 65535 && (size_t)B * S * 10 <= 0x7fffffffu, B200_ERR_INVALID,
              "weighted pooling: %d frames x %lld rows is too large", T, (long long)B * S);
   B200_CHECK(a.nslices == 1 || part != nullptr, B200_ERR_INVALID, "weighted pooling: scratch missing");
-  const dim3 grid((unsigned)((size_t)B * S * 10), (unsigned)a.nslices);
-  if (a.nslices == 1) {
-    if (feat) wpool_kernel<0, __half><<<grid, 256, 0, stream>>>(a);
-    else wpool_kernel<0, float><<<grid, 256, 0, stream>>>(a);
-  } else {
-    if (feat) {
-      wpool_kernel<1, __half><<<grid, 256, 0, stream>>>(a);
-      wpool_kernel<2, __half><<<grid, 256, 0, stream>>>(a);
-    } else {
-      wpool_kernel<1, float><<<grid, 256, 0, stream>>>(a);
-      wpool_kernel<2, float><<<grid, 256, 0, stream>>>(a);
-    }
-    wpool_final_kernel<<<grid.x, 256, 0, stream>>>(a);
-  }
+  B200_CHECK(C == 256 || C == 1024, B200_ERR_STATE, "weighted pooling: %d channels unsupported", C);
+  if (C == 256) wpool_launch<256>(a, feat != nullptr, (size_t)B * S, stream);
+  else wpool_launch<1024>(a, feat != nullptr, (size_t)B * S, stream);
   B200_CUDA_OK(cudaGetLastError());
   return B200_OK;
 }

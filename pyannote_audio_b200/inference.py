@@ -16,7 +16,7 @@ import torch
 from . import ops
 from .audio import AudioFile
 from .core import Resolution, Segment, SlidingWindow, SlidingWindowFeature, Specifications
-from .models import Model, WeSpeakerResNet34
+from .models import BaseWeSpeakerResNet, Model
 
 
 class BaseInference:
@@ -124,7 +124,7 @@ class Inference(BaseInference):
         return cls, wav_dev, off, valid
 
     def slide(self, waveform: torch.Tensor, sample_rate: int, hook: Optional[Callable] = None):
-        if isinstance(self.model, WeSpeakerResNet34):
+        if isinstance(self.model, BaseWeSpeakerResNet):
             return self._slide_embedding(waveform, sample_rate, hook=hook)
         cls, _, off, _ = self.slide_device(waveform, sample_rate, return_logp=self.conversion != "powerset")
         total = len(off)

@@ -1,10 +1,11 @@
-"""Model-level seam: ``PyanNet`` and ``WeSpeakerResNet34`` with the reference's state-dict keys and ``forward``
+"""Model-level seam: ``PyanNet`` and the WeSpeaker ResNets (``WeSpeakerResNet34`` and the bottleneck
+``WeSpeakerResNet152`` / ``221`` / ``293``) with the reference's state-dict keys and ``forward``
 contract, computing through libb200diar.so (no torch ops on the forward path, no CPU fallback).
 
 Reference interfaces mirrored (paths relative to /root/reference/src/pyannote/audio):
   core/model.py:69-183 (Model: specifications, audio, receptive_field, device)
   models/segmentation/PyanNet.py:92-240 (ctor hyper-parameters, num_frames, receptive field, forward)
-  models/embedding/wespeaker/__init__.py:41-372 (forward / forward_frames / forward_embedding / dimension)
+  models/embedding/wespeaker/__init__.py:41-466 (forward / forward_frames / forward_embedding / dimension)
 """
 from __future__ import annotations
 
@@ -116,10 +117,11 @@ class Model(nn.Module):
         loaded = torch.load(path, map_location=map_location, weights_only=False, pickle_module=_checkpoint_pickle)
         meta = loaded["pyannote.audio"]
         class_name = meta["architecture"]["class"]
-        klass = {"PyanNet": PyanNet, "WeSpeakerResNet34": WeSpeakerResNet34}.get(class_name)
+        klass = {"PyanNet": PyanNet, "WeSpeakerResNet34": WeSpeakerResNet34, "WeSpeakerResNet152": WeSpeakerResNet152,
+                 "WeSpeakerResNet221": WeSpeakerResNet221, "WeSpeakerResNet293": WeSpeakerResNet293}.get(class_name)
         if klass is None:
             raise NotImplementedError(f"architecture {meta['architecture']['module']}.{class_name} has no CUDA "
-                                      f"implementation (community-1 uses PyanNet and WeSpeakerResNet34)")
+                                      f"implementation (PyanNet and WeSpeakerResNet34 / 152 / 221 / 293 have one)")
         if cls not in (Model, klass) and not issubclass(klass, cls):
             raise ValueError(f"checkpoint holds a {class_name}, not a {cls.__name__}")
         hparams = dict(loaded.get("hyper_parameters", {}))
@@ -341,7 +343,46 @@ class _ResNet34Params(nn.Module):
         self.seg_1 = nn.Linear(5120, 256)
 
 
-class WeSpeakerResNet34(Model):
+class _BottleneckParams(nn.Module):
+    """A Bottleneck block (resnet.py:148-176): 1x1 in -> p, 3x3 p -> p with the stride, 1x1 p -> 4p."""
+
+    def __init__(self, in_planes, planes, stride):
+        super().__init__()
+        self.conv1 = nn.Conv2d(in_planes, planes, 1, bias=False)
+        self.bn1 = nn.BatchNorm2d(planes)
+        self.conv2 = nn.Conv2d(planes, planes, 3, stride=stride, padding=1, bias=False)
+        self.bn2 = nn.BatchNorm2d(planes)
+        self.conv3 = nn.Conv2d(planes, 4 * planes, 1, bias=False)
+        self.bn3 = nn.BatchNorm2d(4 * planes)
+        self.shortcut = nn.Sequential()
+        if stride != 1 or in_planes != 4 * planes:
+            self.shortcut = nn.Sequential(nn.Conv2d(in_planes, 4 * planes, 1, stride=stride, bias=False),
+                                          nn.BatchNorm2d(4 * planes))
+
+
+class _BottleneckResNetParams(nn.Module):
+    """Parameter container with the key names of the bottleneck ResNet (resnet.py:214-252, 477-508), two_emb_layer
+    False: 1024 trunk channels, seg_1 20480 -> 256."""
+
+    def __init__(self, num_blocks):
+        super().__init__()
+        self.conv1 = nn.Conv2d(1, 32, 3, stride=1, padding=1, bias=False)
+        self.bn1 = nn.BatchNorm2d(32)
+        in_planes = 32
+        for li, (planes, n, stride) in enumerate(zip((32, 64, 128, 256), num_blocks, (1, 2, 2, 2)), start=1):
+            blocks = []
+            for s in [stride] + [1] * (n - 1):
+                blocks.append(_BottleneckParams(in_planes, planes, s))
+                in_planes = 4 * planes
+            setattr(self, f"layer{li}", nn.Sequential(*blocks))
+        self.seg_1 = nn.Linear(20480, 256)
+
+
+class BaseWeSpeakerResNet(Model):
+    """What the WeSpeaker ResNets share (wespeaker/__init__.py:41-322): the fbank, the frame arithmetic, TSTP pooling
+    and the 256-dimensional embedding.  Subclasses build ``resnet``, the parameter container of their trunk, in
+    ``_make_resnet``."""
+
     _SLOT = "emb"
     _HPARAMS = ("sample_rate", "num_channels", "num_mel_bins", "frame_length", "frame_shift", "dither",
                 "window_type", "use_energy")
@@ -354,11 +395,14 @@ class WeSpeakerResNet34(Model):
                 (16000, 80, 25, 10, 0.0, "hamming", False):
             raise NotImplementedError("the fbank kernel implements the community-1 configuration only "
                                       "(16 kHz, 80 mel bins, 25/10 ms hamming frames, no dither, no energy)")
-        self.resnet = _ResNet34Params()
+        self.resnet = self._make_resnet()
         self.specifications = Specifications(problem=Problem.REPRESENTATION, resolution=Resolution.CHUNK, duration=10.0)
         self.eval()
         for p in self.parameters():
             p.requires_grad_(False)
+
+    def _make_resnet(self) -> nn.Module:
+        raise NotImplementedError
 
     @property
     def dimension(self) -> int:
@@ -437,7 +481,32 @@ class WeSpeakerResNet34(Model):
         return emb[:, 0] if squeeze else emb
 
     def forward_embedding(self, frames: torch.Tensor, weights: Optional[torch.Tensor] = None) -> torch.Tensor:
-        """Frame-wise features (batch, 256, 10, frames) -> (batch, 256), or (batch, speakers, 256) for
-        (batch, speakers, frames) weights.  Any number of frames, any real weights, any number of speakers."""
+        """Frame-wise features (batch, C, 10, frames) -> (batch, 256), or (batch, speakers, 256) for
+        (batch, speakers, frames) weights; C = 256 for ResNet34 and 1024 for the bottleneck ResNets.  Any number of
+        frames, any real weights, any number of speakers."""
         emb = self._ctx().emb_forward_embedding(frames, weights=weights)
         return emb if weights is not None and weights.dim() == 3 else emb[:, 0]
+
+
+class WeSpeakerResNet34(BaseWeSpeakerResNet):
+    def _make_resnet(self):
+        return _ResNet34Params()
+
+
+class _BottleneckWeSpeakerResNet(BaseWeSpeakerResNet):
+    NUM_BLOCKS = ()             # Bottleneck blocks per layer
+
+    def _make_resnet(self):
+        return _BottleneckResNetParams(self.NUM_BLOCKS)
+
+
+class WeSpeakerResNet152(_BottleneckWeSpeakerResNet):
+    NUM_BLOCKS = (3, 8, 36, 3)
+
+
+class WeSpeakerResNet221(_BottleneckWeSpeakerResNet):
+    NUM_BLOCKS = (6, 16, 48, 3)
+
+
+class WeSpeakerResNet293(_BottleneckWeSpeakerResNet):
+    NUM_BLOCKS = (10, 20, 64, 3)

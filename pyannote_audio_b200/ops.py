@@ -90,6 +90,7 @@ class Context:
         self._h = h
         self.seg_loaded = False
         self.emb_loaded = False
+        self.emb_channels = 256   # trunk output channels of the loaded embedding model: 256 (ResNet34) or 1024
         self.owners = {}          # slot ("seg" | "emb") -> stamp of the model whose weights are resident (models.py)
         # A/B knob for scripts (like B200_CONV_IMPL / B200_EMB_MAX_BATCH / B200_SEG_MAX_BATCH, which the library
         # reads itself): B200_OPTIONS="key=value,..."
@@ -182,6 +183,8 @@ class Context:
             dst.bn_mean = f(bn + ".running_mean")
             dst.bn_var = f(bn + ".running_var")
 
+        if "resnet.layer1.0.conv3.weight" in sd:
+            return self._load_bottleneck(sd, f, conv_bn)
         w = _lib.EmbWeights()
         conv_bn(w.stem, "resnet.conv1", "resnet.bn1")
         bi = 0
@@ -196,8 +199,42 @@ class Context:
         w.seg1_weight = f("resnet.seg_1.weight")
         w.seg1_bias = f("resnet.seg_1.bias")
         self.owners.pop("emb", None)
+        self.emb_loaded = False
         _lib.check(self.lib.b200_emb_load(self._h, C.byref(w)))
-        self.emb_loaded = True
+        self.emb_loaded, self.emb_channels = True, 256
+
+    def _load_bottleneck(self, sd, f, conv_bn):
+        """WeSpeakerResNet152 / 221 / 293 (Bottleneck blocks, resnet.py:148-212): the block counts come from the keys."""
+        counts = []
+        for li in range(1, 5):
+            n = 0
+            while f"resnet.layer{li}.{n}.conv1.weight" in sd:
+                n += 1
+            counts.append(n)
+        total = sum(counts)
+        arrays = [(_lib.ConvBN * total)() for _ in range(4)]
+        conv1, conv2, conv3, shortcut = arrays
+        bi = 0
+        for li, n in enumerate(counts, start=1):
+            for i in range(n):
+                p = f"resnet.layer{li}.{i}"
+                conv_bn(conv1[bi], p + ".conv1", p + ".bn1")
+                conv_bn(conv2[bi], p + ".conv2", p + ".bn2")
+                conv_bn(conv3[bi], p + ".conv3", p + ".bn3")
+                if p + ".shortcut.0.weight" in sd:
+                    conv_bn(shortcut[bi], p + ".shortcut.0", p + ".shortcut.1")
+                bi += 1
+        w = _lib.EmbBottleneckWeights()
+        for li, n in enumerate(counts):
+            w.num_blocks[li] = n
+        conv_bn(w.stem, "resnet.conv1", "resnet.bn1")
+        w.block_conv1, w.block_conv2, w.block_conv3, w.block_shortcut = arrays
+        w.seg1_weight = f("resnet.seg_1.weight")
+        w.seg1_bias = f("resnet.seg_1.bias")
+        self.owners.pop("emb", None)
+        self.emb_loaded = False
+        _lib.check(self.lib.b200_emb_load_bottleneck(self._h, C.byref(w)))
+        self.emb_loaded, self.emb_channels = True, 1024
 
     # ---- helpers ---------------------------------------------------------------------------------
     def _chunks(self, wav: torch.Tensor, chunk_off, chunk_valid):
@@ -308,10 +345,11 @@ class Context:
         return emb
 
     def emb_forward_embedding(self, frames: torch.Tensor, weights: Optional[torch.Tensor] = None):
-        """ResNet.forward_embedding on frames (B, 256, 10, T) -> (B, max(S, 1), 256) float32; weights as in
-        emb_forward_utt."""
-        if frames.dim() != 4 or tuple(frames.shape[1:3]) != (256, 10) or frames.shape[3] < 1:
-            raise ValueError(f"frames must have shape (batch, 256, 10, frames), got {tuple(frames.shape)}")
+        """ResNet.forward_embedding on frames (B, C, 10, T) -> (B, max(S, 1), 256) float32, C the trunk channels of
+        the loaded model (256 for ResNet34, 1024 for the bottleneck ResNets); weights as in emb_forward_utt."""
+        c = self.emb_channels
+        if frames.dim() != 4 or tuple(frames.shape[1:3]) != (c, 10) or frames.shape[3] < 1:
+            raise ValueError(f"frames must have shape (batch, {c}, 10, frames), got {tuple(frames.shape)}")
         frames = frames.to(device=self.device, dtype=torch.float32).contiguous()
         B, T = int(frames.shape[0]), int(frames.shape[3])
         w, S, Tw = self._pool_weights(weights, B)
@@ -343,7 +381,7 @@ class Context:
     def emb_trunk(self, fbank: torch.Tensor):
         n = fbank.shape[0]
         fbank = fbank.contiguous()
-        out = torch.empty((n, 256, 10, 125), dtype=torch.float32, device=self.device)
+        out = torch.empty((n, self.emb_channels, 10, 125), dtype=torch.float32, device=self.device)
         with torch.cuda.device(self.device):
             _lib.check(self.lib.b200_emb_trunk(self._h, _ptr(fbank), n, _ptr(out), _stream(self.device)))
         return out

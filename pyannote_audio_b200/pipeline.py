@@ -30,7 +30,7 @@ from .audio import Audio, AudioFile
 from .clustering import PLDA, AgglomerativeClustering, VBxClustering
 from .core import Annotation, SlidingWindow, SlidingWindowFeature
 from .inference import Inference, chunk_layout
-from .models import PyanNet, WeSpeakerResNet34, get_context
+from .models import BaseWeSpeakerResNet, PyanNet, WeSpeakerResNet34, get_context
 
 
 def set_num_speakers(num_speakers=None, min_speakers=None, max_speakers=None):
@@ -63,7 +63,7 @@ class DiarizeOutput:
 class PretrainedSpeakerEmbedding:
     """pipelines/speaker_verification.py:622-716 (PyannoteAudioPretrainedSpeakerEmbedding) over the CUDA model."""
 
-    def __init__(self, embedding: WeSpeakerResNet34, device: Optional[torch.device] = None):
+    def __init__(self, embedding: BaseWeSpeakerResNet, device: Optional[torch.device] = None):
         self.embedding = embedding
         self.model_ = embedding
         self.model_.eval()
@@ -166,7 +166,7 @@ def require_10s_window(window_size: int):
 
 class SpeakerDiarization:
     def __init__(self, legacy: bool = False, segmentation: Union[PyanNet, Mapping, None] = None,
-                 segmentation_step: float = 0.1, embedding: Union[WeSpeakerResNet34, Mapping, None] = None,
+                 segmentation_step: float = 0.1, embedding: Union[BaseWeSpeakerResNet, Mapping, None] = None,
                  embedding_exclude_overlap: bool = False, plda: Union[PLDA, Mapping, None] = None,
                  clustering: str = "VBxClustering", embedding_batch_size: int = 1, segmentation_batch_size: int = 1,
                  der_variant: Optional[dict] = None, token=None, cache_dir=None,
@@ -192,8 +192,8 @@ class SpeakerDiarization:
             model = WeSpeakerResNet34()
             model.load_state_dict(embedding)
             embedding = model
-        if not isinstance(segmentation, PyanNet) or not isinstance(embedding, WeSpeakerResNet34):
-            raise ValueError("`segmentation` / `embedding` must be PyanNet / WeSpeakerResNet34 instances or their "
+        if not isinstance(segmentation, PyanNet) or not isinstance(embedding, BaseWeSpeakerResNet):
+            raise ValueError("`segmentation` / `embedding` must be PyanNet / WeSpeaker ResNet instances or their "
                              "state dicts (no network access here: pretrained hub checkpoints cannot be fetched)")
         self.segmentation_model = segmentation
         self.segmentation_step = segmentation_step

@@ -6,7 +6,7 @@ from . import synthetic as syn
 
 
 def reference_style_checkpoint(kind):
-    """A Lightning-format pytorch_model.bin as the reference writes it (model.py:244-256): state_dict +
+    """``kind``: "seg" (PyanNet), "emb" (WeSpeakerResNet34) or "emb293" (WeSpeakerResNet293).  A Lightning-format pytorch_model.bin as the reference writes it (model.py:244-256): state_dict +
     hyper_parameters + checkpoint["pyannote.audio"] whose `specifications` is pickled under the REFERENCE's module
     path pyannote.audio.core.task (registered here only while pickling, then removed again)."""
     import dataclasses
@@ -58,6 +58,15 @@ def reference_style_checkpoint(kind):
                                          Problem.MONO_LABEL_CLASSIFICATION, Resolution.FRAME, 10.0,
                                          classes=["speaker#1", "speaker#2", "speaker#3"], powerset_max_classes=2,
                                          permutation_invariant=True)}}
+        elif kind == "emb293":
+            ck = {"state_dict": syn.make_bottleneck_state_dict(293, 1),
+                  "hyper_parameters": {"sample_rate": 16000, "num_channels": 1, "num_mel_bins": 80,
+                                       "frame_length": 25, "frame_shift": 10, "dither": 0.0,
+                                       "window_type": "hamming", "use_energy": False},
+                  "pyannote.audio": {"versions": {"pyannote.audio": "4.0.0"},
+                                     "architecture": {"module": "pyannote.audio.models.embedding.wespeaker",
+                                                      "class": "WeSpeakerResNet293"},
+                                     "specifications": Specifications(Problem.REPRESENTATION, Resolution.CHUNK, 10.0)}}
         else:
             ck = {"state_dict": syn.make_embedding_state_dict(1),
                   "hyper_parameters": {"sample_rate": 16000, "num_channels": 1, "num_mel_bins": 80,

@@ -6,7 +6,8 @@ with the *reference's state-dict key names and shapes* (real checkpoints drop in
 * segmentation: ``PyanNet`` (SincNet + 4-layer BiLSTM(128) + 2xLinear(128) + Linear(7));
   keys as in /root/reference/src/pyannote/audio/models/segmentation/PyanNet.py:92-161 and
   models/blocks/sincnet.py:41-79 (module tree: tutorials/training_a_model.ipynb:1001-1016)
-* embedding: ``WeSpeakerResNet34``; keys as in models/embedding/wespeaker/resnet.py:233-252
+* embedding: ``WeSpeakerResNet34``; keys as in models/embedding/wespeaker/resnet.py:233-252; the bottleneck
+  ``WeSpeakerResNet152`` / ``221`` / ``293`` (resnet.py:148-212) with ``make_bottleneck_state_dict``
 * PLDA: ``xvec_transform.npz{mean1,mean2,lda}`` + ``plda.npz{mu,tr,psi}`` (utils/vbx.py:195-199)
 
 Audio: a synthetic multi-speaker "conversation" (harmonic sources, 3-6 Hz amplitude modulation,
@@ -131,6 +132,40 @@ def make_embedding_state_dict(seed: int = 1, centered: bool = True) -> "OrderedD
         path = os.path.join(os.path.dirname(__file__), "data", "synthetic_embedding_bias_seed1.npz")
         if os.path.exists(path):
             sd["resnet.seg_1.bias"] = torch.from_numpy(np.load(path)["bias"]).clone()
+    return sd
+
+
+BOTTLENECK_BLOCKS = {152: (3, 8, 36, 3), 221: (6, 16, 48, 3), 293: (10, 20, 64, 3)}
+
+
+def make_bottleneck_state_dict(depth: int = 293, seed: int = 1) -> "OrderedDict[str, torch.Tensor]":
+    """WeSpeakerResNet152 / 221 / 293 weights with the keys of the reference's bottleneck ResNet (resnet.py:148-212,
+    214-252, two_emb_layer=False).  Trained bottleneck ResNets end each residual branch on a small BatchNorm scale;
+    drawing bn3.weight around 0.1 (not the 0.8-1.2 of the other BatchNorms) keeps the residual stream in a realistic
+    range through the 100 blocks of ResNet293 instead of growing with depth, which the fp16 trunk could not hold."""
+    g = torch.Generator().manual_seed(seed)
+    sd = OrderedDict()
+    _conv(sd, "resnet.conv1.weight", 32, 1, 3, g)
+    _bn(sd, "resnet.bn1", 32, g)
+    in_planes = 32
+    for li, (planes, n, stride) in enumerate(zip((32, 64, 128, 256), BOTTLENECK_BLOCKS[depth], (1, 2, 2, 2)),
+                                             start=1):
+        for bi in range(n):
+            s = stride if bi == 0 else 1
+            p = f"resnet.layer{li}.{bi}"
+            _conv(sd, p + ".conv1.weight", planes, in_planes, 1, g)
+            _bn(sd, p + ".bn1", planes, g)
+            _conv(sd, p + ".conv2.weight", planes, planes, 3, g)
+            _bn(sd, p + ".bn2", planes, g)
+            _conv(sd, p + ".conv3.weight", 4 * planes, planes, 1, g)
+            _bn(sd, p + ".bn3", 4 * planes, g)
+            sd[p + ".bn3.weight"] = 0.05 + 0.1 * torch.rand(4 * planes, generator=g)
+            if s != 1 or in_planes != 4 * planes:
+                _conv(sd, p + ".shortcut.0.weight", 4 * planes, in_planes, 1, g, gain=0.8)
+                _bn(sd, p + ".shortcut.1", 4 * planes, g)
+            in_planes = 4 * planes
+    sd["resnet.seg_1.weight"] = torch.randn(256, 20480, generator=g) / math.sqrt(20480)
+    sd["resnet.seg_1.bias"] = 0.01 * torch.randn(256, generator=g)
     return sd
 
 

@@ -1,6 +1,7 @@
-"""Per-conv profile of the ResNet34 trunk: time, TFLOP/s, operand fill and unique HBM traffic of each trunk conv.
+"""Per-conv profile of a WeSpeaker trunk: time, TFLOP/s, operand fill and unique HBM traffic of each trunk conv.
 
-    python scripts/trunk_profile.py                  # the library in this tree (needs a GPU)
+    python scripts/trunk_profile.py                  # the library in this tree (needs a GPU), ResNet34
+    python scripts/trunk_profile.py --model resnet293   # a bottleneck trunk (resnet152 | resnet221 | resnet293)
     python scripts/trunk_profile.py --root OTHER --plan reuse     # another tree's build, with its launch plan
     python scripts/trunk_profile.py --model-only     # the byte model alone (no GPU)
 
@@ -10,7 +11,8 @@ activities, after warm-up.  The trunk convs are the kernel launches between the 
 
 Byte model, per segment (computed from the shapes, not measured):
   fill  = bytes TMA moves from L2 into shared memory for the operands, for the launch plan of conv_forward:
-          per-tap : every (tap, channel chunk) stages a 128-pixel activation box and one weight tile
+          per-tap : every (tap, channel chunk) stages a 128-pixel activation box and one weight tile (per 256-channel
+                    column tile for C_out > 256)
           reuse   : stride-1 3x3 convs with one channel chunk and C_out <= 64 (layers 1 and 2) stage one 136-pixel
                     activation box per kh for the three kw taps, and every weight tile; the other convs stay per-tap
           resident: the stride-1 3x3 convs with one channel chunk and C_in = C_out (layers 1 and 2) stage each input
@@ -27,10 +29,27 @@ TILE_M = 128
 HALO = 8
 
 
-def trunk_convs():
-    """(layer, name, C_in, C_out, ksize, stride, H_in, W_in, has_residual) of the 35 trunk convs in launch order."""
+BOTTLENECK_BLOCKS = {"resnet152": (3, 8, 36, 3), "resnet221": (6, 16, 48, 3), "resnet293": (10, 20, 64, 3)}
+
+
+def trunk_convs(model="resnet34"):
+    """(layer, name, C_in, C_out, ksize, stride, H_in, W_in, has_residual) of the trunk convs in launch order (35 for
+    ResNet34; conv1, conv2, shortcut, conv3 per Bottleneck, api.cu bottleneck_run)."""
     convs = []
     H, W, C = 80, 998, 32
+    if model != "resnet34":
+        for li, (p, blocks, stride) in enumerate(zip((32, 64, 128, 256), BOTTLENECK_BLOCKS[model], (1, 2, 2, 2)),
+                                                 start=1):
+            for bi in range(blocks):
+                s = stride if bi == 0 else 1
+                Ho, Wo = (H + 2 - 3) // s + 1, (W + 2 - 3) // s + 1
+                convs.append((li, f"layer{li}.{bi}.conv1", C, p, 1, 1, H, W, False))
+                convs.append((li, f"layer{li}.{bi}.conv2", p, p, 3, s, H, W, False))
+                if s != 1 or C != 4 * p:
+                    convs.append((li, f"layer{li}.{bi}.shortcut", C, 4 * p, 1, s, H, W, False))
+                convs.append((li, f"layer{li}.{bi}.conv3", p, 4 * p, 1, 1, Ho, Wo, True))
+                H, W, C = Ho, Wo, 4 * p
+        return convs
     for li, (cout, blocks, stride) in enumerate(((32, 3, 1), (64, 4, 2), (128, 6, 2), (256, 3, 2)), start=1):
         for bi in range(blocks):
             s = stride if bi == 0 else 1
@@ -58,8 +77,9 @@ def conv_model(c, plan, batch, sms=132):
     Ho, Wo = (H + 2 * pad - k) // s + 1, (W + 2 * pad - k) // s + 1
     ck = 64 if cin >= 64 else 32
     chunks = cin // ck
-    tiles = Ho * -(-Wo // TILE_M)
-    b_tile = cout * ck * 2
+    n_tile = min(cout, 256)
+    tiles = Ho * -(-Wo // TILE_M) * (cout // n_tile)
+    b_tile = n_tile * ck * 2
     reuse = plan == "reuse" and k == 3 and s == 1 and cin == ck and cout <= 64
     if plan == "resident" and k == 3 and s == 1 and cin == ck and cout == cin:
         tiles_w = -(-Wo // TILE_M)
@@ -74,9 +94,9 @@ def conv_model(c, plan, batch, sms=132):
     return 2.0 * Ho * Wo * cout * cin * k * k / 1e9, fill / 1e6, hbm / 1e6
 
 
-def print_model(plan, batch, sms):
-    rows = [(c, *conv_model(c, plan, batch, sms)) for c in trunk_convs()]
-    print(f"byte model ({plan} plan), per segment:")
+def print_model(plan, batch, sms, model="resnet34"):
+    rows = [(c, *conv_model(c, plan, batch, sms)) for c in trunk_convs(model)]
+    print(f"byte model of {model} ({plan} plan), per segment:")
     print(f"{'layer':>6} {'convs':>5} {'GFLOP':>7} {'fill MB':>8} {'HBM MB':>7} {'FLOP/fill B':>11} {'FLOP/HBM B':>10}")
     tot = [0, 0.0, 0.0, 0.0]
     for li in (1, 2, 3, 4):
@@ -109,9 +129,11 @@ def main():
     ap.add_argument("--batch", type=int, default=264, help="segments per emb_trunk call (library sub-batch: 264)")
     ap.add_argument("--iters", type=int, default=5, help="profiled emb_trunk calls")
     ap.add_argument("--model-only", action="store_true", help="print the byte model and exit (no GPU needed)")
+    ap.add_argument("--model", choices=["resnet34", *BOTTLENECK_BLOCKS], default="resnet34",
+                    help="trunk to profile (synthetic weights)")
     args = ap.parse_args()
 
-    rows = print_model(args.plan, args.batch, args.sms)
+    rows = print_model(args.plan, args.batch, args.sms, args.model)
     if args.model_only:
         return
 
@@ -125,7 +147,8 @@ def main():
         raise SystemExit("no CUDA device: only --model-only runs without a GPU")
     dev = torch.device("cuda:0")
     ctx = ops.Context(dev)
-    ctx.load_embedding(syn.make_embedding_state_dict(1))
+    ctx.load_embedding(syn.make_embedding_state_dict(1) if args.model == "resnet34" else
+                       syn.make_bottleneck_state_dict(int(args.model[len("resnet"):]), 1))
     g = torch.Generator().manual_seed(0)
     fb = (torch.randn((args.batch, 998, 80), generator=g) * 2.0).to(dev)
     for _ in range(3):
