@@ -123,6 +123,31 @@ typedef struct b200_emb_bottleneck_weights {
  * this trunk.  Bad arguments or inconsistent shortcuts return B200_STATUS_INVALID. */
 int b200_emb_load_bottleneck(b200_ctx* ctx, const b200_emb_bottleneck_weights* w);
 
+/* XVectorSincNet (models/embedding/xvector.py:205-349), the architecture of pyannote/embedding: the SincNet front end
+ * of PyanNet (same fields and meaning as in b200_seg_weights), five TDNN layers Conv1d -> LeakyReLU -> BatchNorm1d
+ * (eval, eps 1e-5) with (C_out, kernel, dilation) = (512, 5, 1), (512, 3, 2), (512, 3, 3), (512, 1, 1), (1500, 1, 1),
+ * StatsPool (mean and std of the 1500 channels) and the Linear 3000 -> dimension. */
+typedef struct b200_xvec_weights {
+  float wav_norm_weight, wav_norm_bias;       /* sincnet.wav_norm1d.{weight,bias}                       */
+  const float* sinc_filters;                  /* [80][251] realised ParamSincFB bank (cos 0..39, sin 40..79) */
+  const float* norm_weight[3];                /* sincnet.norm1d.{0,1,2}.weight  (80, 60, 60)            */
+  const float* norm_bias[3];
+  const float* conv_weight[2];                /* sincnet.conv1d.{1,2}.weight  [60][80][5], [60][60][5]  */
+  const float* conv_bias[2];
+  const float* tdnn_weight[5];                /* tdnns.{0,3,6,9,12}.weight [C_out][C_in][kernel]        */
+  const float* tdnn_bias[5];                  /* tdnns.{0,3,6,9,12}.bias [C_out]                        */
+  const float* bn_weight[5];                  /* tdnns.{2,5,8,11,14}.weight [C_out]                     */
+  const float* bn_bias[5];
+  const float* bn_mean[5];                    /* tdnns.{2,5,8,11,14}.running_mean                       */
+  const float* bn_var[5];                     /* tdnns.{2,5,8,11,14}.running_var                        */
+  int32_t dimension;                          /* embedding size (512 for pyannote/embedding)            */
+  const float* embedding_weight;              /* embedding.weight [dimension][3000]                     */
+  const float* embedding_bias;                /* [dimension]                                            */
+} b200_xvec_weights;
+/* Loads XVectorSincNet into the ctx's own slot: a PyanNet, a WeSpeaker ResNet and an XVectorSincNet stay resident
+ * side by side.  fp16 (hi, lo) splits and the BatchNorm scale / shift are made here, once. */
+int b200_xvec_load(b200_ctx* ctx, const b200_xvec_weights* w);
+
 /* ---- audio ingest: Audio.__call__ / Audio.downmix_and_resample (core/io.py:223-265, 306-351) -----------------
  * pcm is a DEVICE buffer holding the raw decoded audio: B200_PCM_S16_INTERLEAVED = int16 [frame][channel] (what a
  * PCM WAV holds; half the PCIe bytes of float32) or B200_PCM_F32_PLANAR = float32 [channel][frame] (the reference's
@@ -207,6 +232,14 @@ int b200_emb_forward_utt(b200_ctx* ctx, const float* wav, const int64_t* off, in
  * emb as in b200_emb_forward_utt. */
 int b200_emb_forward_embedding(b200_ctx* ctx, const float* frames, int32_t B, int32_t T, const float* weights,
                                int32_t num_speakers, int32_t num_weights, float* emb, void* stream);
+/* XVectorSincNet.forward (models/embedding/xvector.py:329-349) on utterances of one length num_samples >= 4771,
+ * arguments as in b200_emb_forward_utt.  SincNet gives F frames (b200_seg_forward_window's arithmetic), the TDNN
+ * stack T = F - 14; StatsPool weights [num_utts][num_speakers][num_weights] (any real values, NULL = mean and
+ * std(correction=1)) reach the T frames by torch's CUDA nearest index.  emb: fp32 DEVICE
+ * [num_utts][max(num_speakers, 1)][dimension].  Utterances run in sub-batches of at most emb_max_batch x 160000
+ * samples; one utterance longer than that (43.9 min with the default) returns B200_STATUS_INVALID. */
+int b200_xvec_forward(b200_ctx* ctx, const float* wav, const int64_t* off, int64_t num_samples, int32_t num_utts,
+                      const float* weights, int32_t num_speakers, int32_t num_weights, float* emb, void* stream);
 /* StatsPool.forward (models/blocks/pooling.py:76-130): seq[B][F][T], weights[B][S][Tw] or NULL -> out[B][S][2F]. */
 int b200_stats_pool(b200_ctx* ctx, const float* seq, const float* weights, float* out, int32_t B, int32_t F, int32_t T,
                     int32_t S, int32_t Tw, void* stream);

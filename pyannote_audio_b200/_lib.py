@@ -43,6 +43,18 @@ class EmbBottleneckWeights(C.Structure):
                 ("block_shortcut", C.POINTER(ConvBN)), ("seg1_weight", c_float_p), ("seg1_bias", c_float_p)]
 
 
+class XvecWeights(C.Structure):
+    _fields_ = [
+        ("wav_norm_weight", C.c_float), ("wav_norm_bias", C.c_float),
+        ("sinc_filters", c_float_p),
+        ("norm_weight", c_float_p * 3), ("norm_bias", c_float_p * 3),
+        ("conv_weight", c_float_p * 2), ("conv_bias", c_float_p * 2),
+        ("tdnn_weight", c_float_p * 5), ("tdnn_bias", c_float_p * 5),
+        ("bn_weight", c_float_p * 5), ("bn_bias", c_float_p * 5), ("bn_mean", c_float_p * 5), ("bn_var", c_float_p * 5),
+        ("dimension", C.c_int32), ("embedding_weight", c_float_p), ("embedding_bias", c_float_p),
+    ]
+
+
 class B200Error(RuntimeError):
     pass
 
@@ -60,6 +72,9 @@ _PROTOS = {
     "b200_seg_load": (C.c_int, [C.c_void_p, C.POINTER(SegWeights)]),
     "b200_emb_load": (C.c_int, [C.c_void_p, C.POINTER(EmbWeights)]),
     "b200_emb_load_bottleneck": (C.c_int, [C.c_void_p, C.POINTER(EmbBottleneckWeights)]),
+    "b200_xvec_load": (C.c_int, [C.c_void_p, C.POINTER(XvecWeights)]),
+    "b200_xvec_forward": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_int64, C.c_int32, C.c_void_p, C.c_int32,
+                                    C.c_int32, C.c_void_p, C.c_void_p]),
     "b200_seg_forward": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_int32, C.c_void_p, C.c_void_p,
                                    C.c_void_p]),
     "b200_seg_forward_window": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_int32, C.c_int32,

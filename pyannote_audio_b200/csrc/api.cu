@@ -14,6 +14,27 @@
 
 using namespace b200;
 
+// XVectorSincNet (models/embedding/xvector.py:205-349): the SincNet front end, five TDNN layers (Conv1d -> LeakyReLU
+// -> eval BatchNorm1d) as implicit GEMMs on gemm_tc_split, statistics pooling and the embedding Linear
+constexpr int kXvecLayers = 5;
+constexpr int kXvecMinSamples = 4771;   // 15 SincNet frames: the TDNN stack (receptive field 15) gives one frame
+constexpr int kXvecStatsLd = 3008;      // 2 x 1500 statistics, padded to whole 64-wide k-blocks
+struct XvecWeights {
+  bool loaded = false;
+  SincNetWeights sinc;
+  int taps[kXvecLayers] = {5, 3, 3, 1, 1}, dil[kXvecLayers] = {1, 2, 3, 1, 1};
+  int cin_pad[kXvecLayers] = {64, 512, 512, 512, 512}, cout_pad[kXvecLayers] = {512, 512, 512, 512, 1536};
+  __half* w_hi[kXvecLayers] = {};   // [cout_pad][taps x cin_pad] fp16 (hi, lo), k = tap * cin_pad + c_in, zero padded
+  __half* w_lo[kXvecLayers] = {};
+  float* bias[kXvecLayers] = {};    // [cout_pad] conv bias
+  float* scale[kXvecLayers] = {};   // [cout_pad] BN gamma / sqrt(var + eps) (0 on padded channels)
+  float* shift[kXvecLayers] = {};   // [cout_pad] BN beta - mean * scale
+  int dim = 512, dim_pad = 512;     // embedding dimension, rounded up to 128
+  __half* emb_hi = nullptr;         // [dim_pad][3008] fp16 (hi, lo) of embedding.weight, zero padded
+  __half* emb_lo = nullptr;
+  float* emb_b = nullptr;           // [dim_pad]
+};
+
 struct b200_ctx {
   int device = 0;
   int num_sms = 132;
@@ -32,7 +53,8 @@ struct b200_ctx {
   int64_t launches = 0;
   SegWeights seg;
   EmbWeights emb;
-  std::vector<void*> owned_seg, owned_emb;   // device allocations holding the weights of each network
+  XvecWeights xvec;
+  std::vector<void*> owned_seg, owned_emb, owned_xvec;   // device allocations holding the weights of each network
   std::vector<void*>* owned = &owned_seg;    // where upload() records allocations (set by the load entry points)
   void* ws = nullptr;
   size_t ws_cap = 0;
@@ -253,6 +275,78 @@ int make_conv(b200_ctx* ctx, const b200_conv_bn& src, int cin, int cout, int k, 
   return B200_OK;
 }
 
+// the SincNet half of a loader (sincnet.wav_norm1d, the ParamSincFB bank, sincnet.norm1d.*, sincnet.conv1d.{1,2}) in
+// the layouts of both implementations; PyanNet and XVectorSincNet share it
+int load_sincnet(b200_ctx* ctx, float wav_w, float wav_b, const float* sinc_filters, const float* const norm_weight[3],
+                 const float* const norm_bias[3], const float* const conv_weight[2], const float* const conv_bias[2],
+                 SincNetWeights* out) {
+  SincNetWeights& S = *out;
+  S.wav_w = wav_w;
+  S.wav_b = wav_b;
+  int rc;
+  {  // half filter bank [126][80]; the kernel relies on the (anti)symmetry of ParamSincFB filters
+    B200_CHECK(sinc_filters, B200_ERR_INVALID, "sinc_filters is NULL");
+    std::vector<float> f(126 * 80);
+    for (int ch = 0; ch < 80; ++ch) {
+      const float* r = sinc_filters + ch * 251;
+      const float sign = ch < 40 ? 1.f : -1.f;
+      float mx = 0.f, err = 0.f;
+      for (int k = 0; k < 125; ++k) {
+        mx = std::fmax(mx, std::fabs(r[k]));
+        err = std::fmax(err, std::fabs(r[k] - sign * r[250 - k]));
+        f[k * 80 + ch] = r[k];
+      }
+      if (ch >= 40) err = std::fmax(err, std::fabs(r[125]));
+      B200_CHECK(err <= 1e-6f * (mx + 1e-30f) + 1e-12f, B200_ERR_INVALID,
+                 "sinc filter %d is not (anti)symmetric (err %g): not a ParamSincFB bank", ch, (double)err);
+      f[125 * 80 + ch] = ch < 40 ? r[125] : 0.f;
+    }
+    if ((rc = upload(ctx, f, &S.sinc_f))) return rc;
+    std::vector<__half> hi((size_t)80 * 256, __float2half(0.f)), lo(hi.size(), __float2half(0.f));
+    for (int ch = 0; ch < 80; ++ch)
+      for (int k = 0; k < 251; ++k) {
+        const float v = sinc_filters[ch * 251 + k];
+        const size_t o = (size_t)ch * 256 + k;
+        hi[o] = __float2half(v);
+        lo[o] = __float2half(v - __half2float(hi[o]));
+      }
+    if ((rc = upload(ctx, hi, &S.sinc_wg_hi))) return rc;
+    if ((rc = upload(ctx, lo, &S.sinc_wg_lo))) return rc;
+  }
+  const int nch[3] = {80, 60, 60};
+  for (int i = 0; i < 3; ++i) {
+    B200_CHECK(norm_weight[i] && norm_bias[i], B200_ERR_INVALID, "norm1d.%d missing", i);
+    std::vector<float> gmm(norm_weight[i], norm_weight[i] + nch[i]), bt(norm_bias[i], norm_bias[i] + nch[i]);
+    if ((rc = upload(ctx, gmm, &S.in_gamma[i]))) return rc;
+    if ((rc = upload(ctx, bt, &S.in_beta[i]))) return rc;
+  }
+  const int cin[2] = {80, 60};
+  for (int i = 0; i < 2; ++i) {
+    B200_CHECK(conv_weight[i] && conv_bias[i], B200_ERR_INVALID, "conv1d.%d missing", i + 1);
+    std::vector<float> wc((size_t)cin[i] * 5 * 60), bc(conv_bias[i], conv_bias[i] + 60);
+    for (int co = 0; co < 60; ++co)
+      for (int ci = 0; ci < cin[i]; ++ci)
+        for (int k = 0; k < 5; ++k) wc[((size_t)ci * 5 + k) * 60 + co] = conv_weight[i][((size_t)co * cin[i] + ci) * 5 + k];
+    if ((rc = upload(ctx, wc, &S.conv_w[i]))) return rc;
+    if ((rc = upload(ctx, bc, &S.conv_b[i]))) return rc;
+    {   // wgmma layout: [64 rows = c_out][k = tap * Cpad + c_in], Cpad = 80 | 64, padding zero
+      const int cpad = i == 0 ? 80 : 64, K = 5 * cpad;
+      std::vector<__half> hi((size_t)64 * K, __float2half(0.f)), lo(hi.size(), __float2half(0.f));
+      for (int co = 0; co < 60; ++co)
+        for (int ci = 0; ci < cin[i]; ++ci)
+          for (int k = 0; k < 5; ++k) {
+            const float v = conv_weight[i][((size_t)co * cin[i] + ci) * 5 + k];
+            const size_t o = (size_t)co * K + k * cpad + ci;
+            hi[o] = __float2half(v);
+            lo[o] = __float2half(v - __half2float(hi[o]));
+          }
+      if ((rc = upload(ctx, hi, &S.conv_wg_hi[i]))) return rc;
+      if ((rc = upload(ctx, lo, &S.conv_wg_lo[i]))) return rc;
+    }
+  }
+  return B200_OK;
+}
+
 }  // namespace
 
 extern "C" {
@@ -285,6 +379,7 @@ int b200_ctx_destroy(b200_ctx* ctx) {
   cudaDeviceSynchronize();
   for (void* p : ctx->owned_seg) cudaFree(p);
   for (void* p : ctx->owned_emb) cudaFree(p);
+  for (void* p : ctx->owned_xvec) cudaFree(p);
   for (auto& t : ctx->resample_tables) cudaFree(t.dev);
   if (ctx->ws) cudaFree(ctx->ws);
   if (ctx->d_off) cudaFree(ctx->d_off);
@@ -393,69 +488,10 @@ int b200_seg_load(b200_ctx* ctx, const b200_seg_weights* w) {
   S.loaded = false;
   release_weights(ctx, &ctx->owned_seg);
   S.lstm_layers = w->lstm_layers;
-  S.wav_w = w->wav_norm_weight;
-  S.wav_b = w->wav_norm_bias;
   int rc;
-  {  // half filter bank [126][80]; the kernel relies on the (anti)symmetry of ParamSincFB filters
-    B200_CHECK(w->sinc_filters, B200_ERR_INVALID, "sinc_filters is NULL");
-    std::vector<float> f(126 * 80);
-    for (int ch = 0; ch < 80; ++ch) {
-      const float* r = w->sinc_filters + ch * 251;
-      const float sign = ch < 40 ? 1.f : -1.f;
-      float mx = 0.f, err = 0.f;
-      for (int k = 0; k < 125; ++k) {
-        mx = std::fmax(mx, std::fabs(r[k]));
-        err = std::fmax(err, std::fabs(r[k] - sign * r[250 - k]));
-        f[k * 80 + ch] = r[k];
-      }
-      if (ch >= 40) err = std::fmax(err, std::fabs(r[125]));
-      B200_CHECK(err <= 1e-6f * (mx + 1e-30f) + 1e-12f, B200_ERR_INVALID,
-                 "sinc filter %d is not (anti)symmetric (err %g): not a ParamSincFB bank", ch, (double)err);
-      f[125 * 80 + ch] = ch < 40 ? r[125] : 0.f;
-    }
-    if ((rc = upload(ctx, f, &S.sinc_f))) return rc;
-    std::vector<__half> hi((size_t)80 * 256, __float2half(0.f)), lo(hi.size(), __float2half(0.f));
-    for (int ch = 0; ch < 80; ++ch)
-      for (int k = 0; k < 251; ++k) {
-        const float v = w->sinc_filters[ch * 251 + k];
-        const size_t o = (size_t)ch * 256 + k;
-        hi[o] = __float2half(v);
-        lo[o] = __float2half(v - __half2float(hi[o]));
-      }
-    if ((rc = upload(ctx, hi, &S.sinc_wg_hi))) return rc;
-    if ((rc = upload(ctx, lo, &S.sinc_wg_lo))) return rc;
-  }
-  const int nch[3] = {80, 60, 60};
-  for (int i = 0; i < 3; ++i) {
-    B200_CHECK(w->norm_weight[i] && w->norm_bias[i], B200_ERR_INVALID, "norm1d.%d missing", i);
-    std::vector<float> gmm(w->norm_weight[i], w->norm_weight[i] + nch[i]), bt(w->norm_bias[i], w->norm_bias[i] + nch[i]);
-    if ((rc = upload(ctx, gmm, &S.in_gamma[i]))) return rc;
-    if ((rc = upload(ctx, bt, &S.in_beta[i]))) return rc;
-  }
-  const int cin[2] = {80, 60};
-  for (int i = 0; i < 2; ++i) {
-    B200_CHECK(w->conv_weight[i] && w->conv_bias[i], B200_ERR_INVALID, "conv1d.%d missing", i + 1);
-    std::vector<float> wc((size_t)cin[i] * 5 * 60), bc(w->conv_bias[i], w->conv_bias[i] + 60);
-    for (int co = 0; co < 60; ++co)
-      for (int ci = 0; ci < cin[i]; ++ci)
-        for (int k = 0; k < 5; ++k) wc[((size_t)ci * 5 + k) * 60 + co] = w->conv_weight[i][((size_t)co * cin[i] + ci) * 5 + k];
-    if ((rc = upload(ctx, wc, &S.conv_w[i]))) return rc;
-    if ((rc = upload(ctx, bc, &S.conv_b[i]))) return rc;
-    {   // wgmma layout: [64 rows = c_out][k = tap * Cpad + c_in], Cpad = 80 | 64, padding zero
-      const int cpad = i == 0 ? 80 : 64, K = 5 * cpad;
-      std::vector<__half> hi((size_t)64 * K, __float2half(0.f)), lo(hi.size(), __float2half(0.f));
-      for (int co = 0; co < 60; ++co)
-        for (int ci = 0; ci < cin[i]; ++ci)
-          for (int k = 0; k < 5; ++k) {
-            const float v = w->conv_weight[i][((size_t)co * cin[i] + ci) * 5 + k];
-            const size_t o = (size_t)co * K + k * cpad + ci;
-            hi[o] = __float2half(v);
-            lo[o] = __float2half(v - __half2float(hi[o]));
-          }
-      if ((rc = upload(ctx, hi, &S.conv_wg_hi[i]))) return rc;
-      if ((rc = upload(ctx, lo, &S.conv_wg_lo[i]))) return rc;
-    }
-  }
+  if ((rc = load_sincnet(ctx, w->wav_norm_weight, w->wav_norm_bias, w->sinc_filters, w->norm_weight, w->norm_bias,
+                         w->conv_weight, w->conv_bias, &S.sinc)))
+    return rc;
   for (int l = 0; l < S.lstm_layers; ++l) {
     const int I = l == 0 ? 60 : 256, Kp = l == 0 ? 64 : 256;
     S.k_in[l] = Kp;
@@ -692,7 +728,7 @@ static int seg_run(b200_ctx* ctx, const float* wav, const int64_t* chunk_off, co
     ScopedTimer timer(ctx, &ctx->seg_events, st);
     if (ctx->profile) ctx->seg_chunks += nb;
     float* x0_dst = sinc_out ? sinc_out + (size_t)c0 * T * 64 : x0;
-    if ((rc = sincnet_forward(ctx->seg, geom, wav, ctx->d_off + c0, ctx->d_valid + c0, nb, region, x0_dst,
+    if ((rc = sincnet_forward(ctx->seg.sinc, geom, wav, ctx->d_off + c0, ctx->d_valid + c0, nb, region, x0_dst,
                               ctx->seg_conv_impl, st)))
       return rc;
     ctx->launches += sincnet_launches(geom);
@@ -1095,6 +1131,192 @@ int b200_stats_pool(b200_ctx* ctx, const float* seq, const float* weights, float
   DeviceGuard g(ctx->device);
   ctx->launches += 1;
   return stats_pool_generic(seq, weights, out, B, F, T, S, weights ? Tw : T, (cudaStream_t)stream);
+}
+
+// ---- XVectorSincNet ----------------------------------------------------------------------------------------
+int b200_xvec_load(b200_ctx* ctx, const b200_xvec_weights* w) {
+  B200_CHECK(ctx && w, B200_ERR_INVALID, "NULL ctx/weights");
+  B200_CHECK(w->dimension >= 1 && w->dimension <= 65536, B200_ERR_INVALID, "embedding dimension %d unsupported",
+             (int)w->dimension);
+  for (int l = 0; l < kXvecLayers; ++l)
+    B200_CHECK(w->tdnn_weight[l] && w->tdnn_bias[l] && w->bn_weight[l] && w->bn_bias[l] && w->bn_mean[l] && w->bn_var[l],
+               B200_ERR_INVALID, "tdnns.%d / tdnns.%d missing", 3 * l, 3 * l + 2);
+  B200_CHECK(w->embedding_weight && w->embedding_bias, B200_ERR_INVALID, "embedding missing");
+  DeviceGuard g(ctx->device);
+  XvecWeights& X = ctx->xvec;
+  X.loaded = false;
+  release_weights(ctx, &ctx->owned_xvec);
+  int rc;
+  if ((rc = load_sincnet(ctx, w->wav_norm_weight, w->wav_norm_bias, w->sinc_filters, w->norm_weight, w->norm_bias,
+                         w->conv_weight, w->conv_bias, &X.sinc)))
+    return rc;
+  const int cin[kXvecLayers] = {60, 512, 512, 512, 512}, cout[kXvecLayers] = {512, 512, 512, 512, 1500};
+  for (int l = 0; l < kXvecLayers; ++l) {
+    const int k = X.taps[l], cp = X.cin_pad[l], np = X.cout_pad[l], K = k * cp;
+    std::vector<__half> hi((size_t)np * K, __float2half(0.f)), lo(hi.size(), __float2half(0.f));
+    std::vector<float> bias(np, 0.f), scale(np, 0.f), shift(np, 0.f);
+    for (int co = 0; co < cout[l]; ++co) {
+      for (int ci = 0; ci < cin[l]; ++ci)
+        for (int j = 0; j < k; ++j) {
+          const float v = w->tdnn_weight[l][((size_t)co * cin[l] + ci) * k + j];
+          const size_t o = (size_t)co * K + j * cp + ci;
+          hi[o] = __float2half(v);
+          lo[o] = __float2half(v - __half2float(hi[o]));
+        }
+      bias[co] = w->tdnn_bias[l][co];
+      scale[co] = w->bn_weight[l][co] / std::sqrt(w->bn_var[l][co] + 1e-5f);
+      shift[co] = w->bn_bias[l][co] - w->bn_mean[l][co] * scale[co];
+    }
+    if ((rc = upload(ctx, hi, &X.w_hi[l]))) return rc;
+    if ((rc = upload(ctx, lo, &X.w_lo[l]))) return rc;
+    if ((rc = upload(ctx, bias, &X.bias[l]))) return rc;
+    if ((rc = upload(ctx, scale, &X.scale[l]))) return rc;
+    if ((rc = upload(ctx, shift, &X.shift[l]))) return rc;
+  }
+  X.dim = w->dimension;
+  X.dim_pad = (int)ceil_div(X.dim, 128) * 128;
+  {
+    std::vector<__half> hi((size_t)X.dim_pad * kXvecStatsLd, __float2half(0.f)), lo(hi.size(), __float2half(0.f));
+    std::vector<float> b(X.dim_pad, 0.f);
+    for (int n = 0; n < X.dim; ++n) {
+      for (int kk = 0; kk < 3000; ++kk) {
+        const float v = w->embedding_weight[(size_t)n * 3000 + kk];
+        const size_t o = (size_t)n * kXvecStatsLd + kk;
+        hi[o] = __float2half(v);
+        lo[o] = __float2half(v - __half2float(hi[o]));
+      }
+      b[n] = w->embedding_bias[n];
+    }
+    if ((rc = upload(ctx, hi, &X.emb_hi))) return rc;
+    if ((rc = upload(ctx, lo, &X.emb_lo))) return rc;
+    if ((rc = upload(ctx, b, &X.emb_b))) return rc;
+  }
+  X.loaded = true;
+  return B200_OK;
+}
+
+// Workspace of an XVectorSincNet sub-batch of nb windows of g.W samples (M = nb x F rows, F = g.pool2 SincNet frames):
+// X0 fp32 [M][64] and its (hi, lo) split, two ping-pong activations P / Q [M][512] fp16 (hi, lo), the last layer's fp32
+// rows Y [M][1536] (sharing its region with the SincNet scratch, which is dead by then) and the pooling partials.
+struct XvecWs {
+  float* x0;
+  __half *xh, *xl, *ph, *pl, *qh, *ql;
+  float* y;
+  void* sinc;
+  double* part;
+};
+static size_t carve_xvec(const SegGeom& g, int nb, int S, void* base, XvecWs* w) {
+  size_t off = 0;
+  auto take = [&](size_t bytes) {
+    off = align_up(off, 1024);
+    void* p = base ? (char*)base + off : nullptr;
+    off += bytes;
+    return p;
+  };
+  const size_t M = (size_t)nb * g.pool2;
+  XvecWs t;
+  t.x0 = (float*)take(M * 64 * sizeof(float));
+  t.xh = (__half*)take(M * 64 * sizeof(__half));
+  t.xl = (__half*)take(M * 64 * sizeof(__half));
+  t.ph = (__half*)take(M * 512 * sizeof(__half));
+  t.pl = (__half*)take(M * 512 * sizeof(__half));
+  t.qh = (__half*)take(M * 512 * sizeof(__half));
+  t.ql = (__half*)take(M * 512 * sizeof(__half));
+  t.y = (float*)take(std::max(M * kPoolRowsLd * sizeof(float), sincnet_workspace_bytes(g, nb)));
+  t.sinc = t.y;
+  t.part = (double*)take(pool_scratch_bytes(nb, S, g.pool2 - 14, kPoolRowsLd, 1));
+  if (w) *w = t;
+  return align_up(off, 1024);
+}
+
+int b200_xvec_forward(b200_ctx* ctx, const float* wav, const int64_t* off, int64_t num_samples, int32_t num_utts,
+                      const float* weights, int32_t num_speakers, int32_t num_weights, float* emb, void* stream) {
+  B200_CHECK(ctx && ctx->xvec.loaded, B200_ERR_STATE, "XVectorSincNet weights not loaded");
+  B200_CHECK(wav && off && emb && num_utts >= 0, B200_ERR_INVALID, "bad arguments");
+  B200_CHECK(num_samples >= kXvecMinSamples, B200_ERR_INVALID,
+             "utterances of %lld samples are too short: XVectorSincNet needs at least %d samples (15 SincNet frames "
+             "for one TDNN output frame)", (long long)num_samples, kXvecMinSamples);
+  B200_CHECK(!weights || (num_speakers >= 1 && num_weights >= 1), B200_ERR_INVALID,
+             "weights need num_speakers >= 1 and num_weights >= 1 (got %d, %d)", (int)num_speakers, (int)num_weights);
+  // a sub-batch holds at most emb_max_batch x 160000 samples (the same budget as the WeSpeaker sub-batches)
+  const int64_t budget = (int64_t)ctx->emb_max_batch * kChunk;
+  B200_CHECK(num_samples <= budget, B200_ERR_INVALID,
+             "an utterance of %lld samples is longer than the %lld samples of one embedding sub-batch (emb_max_batch %d "
+             "x 160000): set the option emb_max_batch to at least %lld, or embed shorter excerpts",
+             (long long)num_samples, (long long)budget, ctx->emb_max_batch,
+             (long long)((num_samples + kChunk - 1) / kChunk));
+  if (num_utts == 0) return B200_OK;
+  for (int i = 0; i < num_utts; ++i)
+    B200_CHECK(off[i] >= 0, B200_ERR_INVALID, "utterance %d: negative offset %lld", i, (long long)off[i]);
+  DeviceGuard g(ctx->device);
+  cudaStream_t st = (cudaStream_t)stream;
+  const XvecWeights& X = ctx->xvec;
+  const SegGeom geom = seg_geom((int)num_samples);
+  const int F = geom.pool2, T = F - 14;                     // TDNN output frames (xvector.py:255-275)
+  const int S = weights ? num_speakers : 1;
+  const int nbmax = (int)std::min<int64_t>(std::min<int64_t>(num_utts, budget / num_samples), 65535);
+  const size_t rows = (size_t)num_utts * S;
+  const size_t split_bytes = align_up(rows * kXvecStatsLd * sizeof(__half), 1024);
+  const size_t out_bytes = X.dim_pad != X.dim ? align_up(rows * X.dim_pad * sizeof(float), 1024) : 0;
+  const size_t sub_bytes = carve_xvec(geom, nbmax, S, nullptr, nullptr);
+  int rc = ensure_ws(ctx, sub_bytes + 2 * split_bytes + out_bytes + 4096);
+  if (rc) return rc;
+  {
+    std::vector<int32_t> valid((size_t)num_utts, (int32_t)num_samples);
+    if ((rc = push_meta(ctx, off, valid.data(), num_utts, st, (int)num_samples))) return rc;
+  }
+  XvecWs w;
+  carve_xvec(geom, nbmax, S, ctx->ws, &w);
+  char* tail = reinterpret_cast<char*>(ctx->ws) + sub_bytes;
+  __half* st_hi = reinterpret_cast<__half*>(tail);
+  __half* st_lo = reinterpret_cast<__half*>(tail + split_bytes);
+  float* out = out_bytes ? reinterpret_cast<float*>(tail + 2 * split_bytes) : emb;
+  B200_CUDA_OK(cudaMemsetAsync(st_hi, 0, 2 * split_bytes, st));   // the 8 padding columns of every statistics row
+  ctx->launches += 1;
+  for (int u0 = 0; u0 < num_utts; u0 += nbmax) {
+    const int nb = std::min(nbmax, num_utts - u0);
+    const int M = nb * F;
+    if ((rc = sincnet_forward(X.sinc, geom, wav, ctx->d_off + u0, ctx->d_valid + u0, nb, w.sinc, w.x0, 1, st)))
+      return rc;
+    ctx->launches += sincnet_launches(geom);
+    if ((rc = split_f16(w.x0, w.xh, w.xl, (size_t)M * 64, st))) return rc;
+    ctx->launches += 1;
+    // Every window keeps the row stride F through the stack: output row b * F + t of layer l reads input rows
+    // b * F + t + j * dil.  Rows t >= F - 4, F - 8, F - 14 (layers 1, 2, 3-5) compute values nothing uses, since a
+    // valid row of layer l + 1 reads only valid rows of layer l and the pooling reads the first T = F - 14 rows of
+    // every window; taps past the last row of the buffer read zeros (TMA out-of-bounds fill).
+    const __half* in_h[kXvecLayers] = {w.xh, w.ph, w.qh, w.ph, w.qh};
+    const __half* in_l[kXvecLayers] = {w.xl, w.pl, w.ql, w.pl, w.ql};
+    __half* out_h[kXvecLayers - 1] = {w.ph, w.qh, w.ph, w.qh};
+    __half* out_l[kXvecLayers - 1] = {w.pl, w.ql, w.pl, w.ql};
+    for (int l = 0; l < kXvecLayers; ++l) {
+      GemmTaps tp;
+      tp.taps = X.taps[l];
+      tp.dil = X.dil[l];
+      tp.scale = X.scale[l];
+      tp.shift = X.shift[l];
+      const int K = X.taps[l] * X.cin_pad[l], N = X.cout_pad[l];
+      const bool last = l == kXvecLayers - 1;
+      rc = gemm_tc_split(in_h[l], in_l[l], X.cin_pad[l], X.w_hi[l], X.w_lo[l], K, last ? w.y : nullptr, N,
+                         last ? nullptr : out_h[l], last ? nullptr : out_l[l], N, X.bias[l], M, N, K, 1,
+                         ctx->num_sms, st, nullptr, 0, tp);
+      if (rc) return rc;
+      ctx->launches += 1;
+    }
+    const size_t o = (size_t)u0 * S * kXvecStatsLd;
+    if ((rc = weighted_pool_rows(w.y, F, T, 1500, weights ? weights + (size_t)u0 * S * num_weights : nullptr, nb, S,
+                                 num_weights, w.part, st_hi + o, st_lo + o, kXvecStatsLd, st)))
+      return rc;
+    ctx->launches += T <= kPoolSlice ? 1 : 3;
+  }
+  rc = gemm_tc_split(st_hi, st_lo, kXvecStatsLd, X.emb_hi, X.emb_lo, kXvecStatsLd, out, X.dim_pad, nullptr, nullptr, 0,
+                     X.emb_b, (int)rows, X.dim_pad, kXvecStatsLd, 0, ctx->num_sms, st);
+  ctx->launches += 1;
+  if (rc) return rc;
+  if (out != emb)
+    B200_CUDA_OK(cudaMemcpy2DAsync(emb, (size_t)X.dim * sizeof(float), out, (size_t)X.dim_pad * sizeof(float),
+                                   (size_t)X.dim * sizeof(float), rows, cudaMemcpyDeviceToDevice, st));
+  return B200_OK;
 }
 
 // ------------------------------------------------------------------------------------------------------

@@ -96,9 +96,15 @@ int stats_pool_forward(const __half* feat, const unsigned char* masks, float* st
 // pool_scratch_bytes(B, S, T, C) bytes (none with one slice).  Rows of stats_hi / stats_lo: (b * S + s) * 20 C.
 // C = 256 or 1024.
 constexpr int kPoolSlice = 512;
-size_t pool_scratch_bytes(int B, int S, int T, int C);
+size_t pool_scratch_bytes(int B, int S, int T, int C, int H = 10);
 int weighted_pool_forward(const __half* feat, const float* frames, const float* w, int B, int T, int S, int Tw, int C,
                           double* part, __half* stats_hi, __half* stats_lo, cudaStream_t stream);
+// the same pooling on frame-major fp32 rows x [B][F][kPoolRowsLd] (XVectorSincNet's last TDNN layer): the first T
+// frames and the first C channels of every sequence -> stats rows of ld_out fp16 (hi, lo), mean at c and std at C + c
+// (StatsPool's [mean, std] concatenation).  part: pool_scratch_bytes(B, S, T, kPoolRowsLd, 1) bytes.
+constexpr int kPoolRowsLd = 1536;
+int weighted_pool_rows(const float* x, int F, int T, int C, const float* w, int B, int S, int Tw, double* part,
+                       __half* stats_hi, __half* stats_lo, int ld_out, cudaStream_t stream);
 // generic weighted pooling used by the known-answer tests: seq [B][F][T] fp32, w [B][S][Tw] fp32 -> [B][S][2F]
 int stats_pool_generic(const float* seq, const float* w, float* out, int B, int F, int T, int S, int Tw,
                        cudaStream_t stream);

@@ -11,6 +11,7 @@
 // interpolation of the 589-frame mask onto the 125 trunk frames, weighted mean and weighted unbiased std.
 #include "common.cuh"
 #include "emb.cuh"
+#include <type_traits>
 
 namespace b200 {
 
@@ -333,52 +334,64 @@ __device__ __forceinline__ int nearest_src(int dst, int T, int Tw, float scale) 
 __device__ __forceinline__ float to_f(__half v) { return __half2float(v); }
 __device__ __forceinline__ float to_f(float v) { return v; }
 
-// stats row of C channels: mean at c * 10 + h, std 10 * C further
-template <int C>
-__device__ __forceinline__ void store_split(__half* hi, __half* lo, size_t row, int c, int h, float mean, float sdv) {
+// feature layouts of the pooled sequence: NHWC fp16 [B][10][T][C] (trunk output), NCHW fp32 [B][C][10][T] (caller
+// frames), frame-major fp32 rows [B][F][C] of which the first T frames are pooled (TDNN output, one "height")
+enum { kPoolNHWC = 0, kPoolNCHW = 1, kPoolRows = 2 };
+template <int L> using PoolX = typename std::conditional<L == kPoolNHWC, __half, float>::type;
+template <int L> __host__ __device__ constexpr int pool_h() { return L == kPoolRows ? 1 : 10; }
+
+// stats row of Cv channels at H heights: mean at c * H + h, std H * Cv further (the ResNet rows: H = 10, Cv = C)
+__device__ __forceinline__ void store_split(__half* hi, __half* lo, size_t row, int c, int h, int H, int Cv, float mean,
+                                            float sdv) {
   const __half mh = __float2half_rn(mean), sh = __float2half_rn(sdv);
-  hi[row + c * 10 + h] = mh;
-  lo[row + c * 10 + h] = __float2half_rn(mean - __half2float(mh));
-  hi[row + 10 * C + c * 10 + h] = sh;
-  lo[row + 10 * C + c * 10 + h] = __float2half_rn(sdv - __half2float(sh));
+  hi[row + c * H + h] = mh;
+  lo[row + c * H + h] = __float2half_rn(mean - __half2float(mh));
+  hi[row + H * Cv + c * H + h] = sh;
+  lo[row + H * Cv + c * H + h] = __float2half_rn(sdv - __half2float(sh));
 }
 
 struct PoolArgs {
-  const void* x;          // NHWC fp16 feat or NCHW fp32 frames
+  const void* x;          // NHWC fp16 feat, NCHW fp32 frames or fp32 rows
   const float* w;         // [B][S][Tw] or NULL
   int S, T, Tw, nslices;
   float scale;            // (float)Tw / T
-  double* part;           // [B * S][10][nslices][4][C]: sum w (sum x), sum w^2, sum w x, sum w (x - mean)^2
+  int Cv;                 // channels pooled (C, or fewer than the row width C of kPoolRows)
+  int F;                  // kPoolRows: frames per sequence (row stride of a sequence, >= T)
+  int ld_out;             // width of an output stats row
+  double* part;           // [B * S][H][nslices][4][C]: sum w (sum x), sum w^2, sum w x, sum w (x - mean)^2
   __half *hi, *lo;
 };
 
-// x of (b, h, channel c): NHWC [B][10][T][C] (stride C between frames) or NCHW [B][C][10][T] (stride 1)
-template <typename X, int C>
-__device__ __forceinline__ const X* pool_row(const PoolArgs& a, int b, int h, int c, size_t* stride) {
-  const X* x = static_cast<const X*>(a.x);
-  if constexpr (sizeof(X) == 2) { *stride = C; return x + ((size_t)b * 10 + h) * a.T * C + c; }
-  else { *stride = 1; return x + (((size_t)b * C + c) * 10 + h) * a.T; }
+// x of (b, h, channel c) and the stride between its frames
+template <int L, int C>
+__device__ __forceinline__ const PoolX<L>* pool_row(const PoolArgs& a, int b, int h, int c, size_t* stride) {
+  const PoolX<L>* x = static_cast<const PoolX<L>*>(a.x);
+  if constexpr (L == kPoolNHWC) { *stride = C; return x + ((size_t)b * 10 + h) * a.T * C + c; }
+  else if constexpr (L == kPoolNCHW) { *stride = 1; return x + (((size_t)b * C + c) * 10 + h) * a.T; }
+  else { *stride = C; return x + (size_t)b * a.F * C + c; }
 }
 
 // PHASE 0: the whole sequence in one slice, finished here (the stats_pool_kernel sums, in its order);
 // PHASE 1: per-slice fp32 sums; PHASE 2: per-slice sum of w (x - mean)^2 around the mean of all slices' sums.
-// grid (B * S * 10, nslices, C / 256), thread = channel
-template <int PHASE, typename X, int C>
+// grid (B * S * H, nslices, C / 256), thread = channel
+template <int PHASE, int L, int C>
 __global__ void __launch_bounds__(256) wpool_kernel(PoolArgs a) {
+  constexpr int H = pool_h<L>();
   __shared__ float s_w[kPoolSlice];
-  const int row = blockIdx.x / 10, h = blockIdx.x % 10;                      // row = b * S + s
+  const int row = blockIdx.x / H, h = blockIdx.x % H;                        // row = b * S + s
   const int c = (C == 256 ? 0 : (int)blockIdx.z * 256) + threadIdx.x;
   const int b = row / a.S, sl = blockIdx.y;
   const int t0 = sl * kPoolSlice, t1 = min(a.T, t0 + kPoolSlice);
   size_t xs;
-  const X* xp = pool_row<X, C>(a, b, h, c, &xs);
+  const PoolX<L>* xp = pool_row<L, C>(a, b, h, c, &xs);
   const bool weighted = a.w != nullptr;
   if (weighted) {
     const float* wr = a.w + (size_t)row * a.Tw;
     for (int i = threadIdx.x; i < t1 - t0; i += blockDim.x) s_w[i] = wr[nearest_src(t0 + i, a.T, a.Tw, a.scale)];
   }
   __syncthreads();
-  double* part = a.part + (((size_t)row * 10 + h) * a.nslices) * 4 * C + c;     // slot k of slice j: [(j*4+k)*C]
+  if (L == kPoolRows && c >= a.Cv) return;                   // padding channels of the rows
+  double* part = a.part + (((size_t)row * H + h) * a.nslices) * 4 * C + c;      // slot k of slice j: [(j*4+k)*C]
   if (PHASE == 0 || PHASE == 1) {
     float v1 = 0.f, v2 = 0.f, sx = 0.f;
     if (weighted) {
@@ -398,7 +411,7 @@ __global__ void __launch_bounds__(256) wpool_kernel(PoolArgs a) {
       part[(sl * 4 + 2) * C] = (double)sx;
       return;
     }
-    const size_t orow = (size_t)row * (2 * 10 * C);
+    const size_t orow = (size_t)row * a.ld_out;
     if (weighted) {
       v1 += 1e-8f;
       const float mean = sx / v1;
@@ -408,7 +421,7 @@ __global__ void __launch_bounds__(256) wpool_kernel(PoolArgs a) {
         sd += d * d * s_w[t - t0];
       }
       const float var = sd / (v1 - v2 / v1 + 1e-8f);
-      store_split<C>(a.hi, a.lo, orow, c, h, mean, sqrtf(var));
+      store_split(a.hi, a.lo, orow, c, h, H, a.Cv, mean, sqrtf(var));
     } else {                                               // torch mean / std(correction=1): T = 1 gives NaN
       const float mean = sx / a.T;
       float acc = 0.f;
@@ -416,7 +429,7 @@ __global__ void __launch_bounds__(256) wpool_kernel(PoolArgs a) {
         const float d = to_f(xp[(size_t)t * xs]) - mean;
         acc += d * d;
       }
-      store_split<C>(a.hi, a.lo, orow, c, h, mean, sqrtf(acc / (a.T - 1)));
+      store_split(a.hi, a.lo, orow, c, h, H, a.Cv, mean, sqrtf(acc / (a.T - 1)));
     }
   } else {
     double s0 = 0.0, s2 = 0.0;                             // every slice's sums, in slice order
@@ -431,12 +444,14 @@ __global__ void __launch_bounds__(256) wpool_kernel(PoolArgs a) {
   }
 }
 
-// combine the slices in fp64, in slice order; grid (B * S * 10, 1, C / 256), thread = channel
-template <int C>
+// combine the slices in fp64, in slice order; grid (B * S * H, 1, C / 256), thread = channel
+template <int L, int C>
 __global__ void __launch_bounds__(256) wpool_final_kernel(PoolArgs a) {
-  const int row = blockIdx.x / 10, h = blockIdx.x % 10;
+  constexpr int H = pool_h<L>();
+  const int row = blockIdx.x / H, h = blockIdx.x % H;
   const int c = (C == 256 ? 0 : (int)blockIdx.z * 256) + threadIdx.x;
-  const double* part = a.part + (((size_t)row * 10 + h) * a.nslices) * 4 * C + c;
+  if (L == kPoolRows && c >= a.Cv) return;
+  const double* part = a.part + (((size_t)row * H + h) * a.nslices) * 4 * C + c;
   double s[4] = {0.0, 0.0, 0.0, 0.0};
   for (int j = 0; j < a.nslices; ++j)
 #pragma unroll
@@ -451,50 +466,73 @@ __global__ void __launch_bounds__(256) wpool_final_kernel(PoolArgs a) {
     mean = (float)(s[0] / a.T);
     var = s[3] / (double)(a.T - 1);
   }
-  store_split<C>(a.hi, a.lo, (size_t)row * (2 * 10 * C), c, h, mean, (float)sqrt(var));
+  store_split(a.hi, a.lo, (size_t)row * a.ld_out, c, h, H, a.Cv, mean, (float)sqrt(var));
 }
 
-size_t pool_scratch_bytes(int B, int S, int T, int C) {
+size_t pool_scratch_bytes(int B, int S, int T, int C, int H) {
   const int nslices = ceil_div(T, kPoolSlice);
-  return nslices > 1 ? (size_t)B * S * 10 * nslices * 4 * C * sizeof(double) : 0;
+  return nslices > 1 ? (size_t)B * S * H * nslices * 4 * C * sizeof(double) : 0;
 }
 
-template <int C>
-static void wpool_launch(const PoolArgs& a, bool nhwc, size_t rows, cudaStream_t stream) {
-  const dim3 grid((unsigned)(rows * 10), (unsigned)a.nslices, C / 256);
+template <int L, int C>
+static void wpool_launch(const PoolArgs& a, size_t rows, cudaStream_t stream) {
+  const dim3 grid((unsigned)(rows * pool_h<L>()), (unsigned)a.nslices, C / 256);
   if (a.nslices == 1) {
-    if (nhwc) wpool_kernel<0, __half, C><<<grid, 256, 0, stream>>>(a);
-    else wpool_kernel<0, float, C><<<grid, 256, 0, stream>>>(a);
+    wpool_kernel<0, L, C><<<grid, 256, 0, stream>>>(a);
   } else {
-    if (nhwc) {
-      wpool_kernel<1, __half, C><<<grid, 256, 0, stream>>>(a);
-      wpool_kernel<2, __half, C><<<grid, 256, 0, stream>>>(a);
-    } else {
-      wpool_kernel<1, float, C><<<grid, 256, 0, stream>>>(a);
-      wpool_kernel<2, float, C><<<grid, 256, 0, stream>>>(a);
-    }
-    wpool_final_kernel<C><<<dim3(grid.x, 1, C / 256), 256, 0, stream>>>(a);
+    wpool_kernel<1, L, C><<<grid, 256, 0, stream>>>(a);
+    wpool_kernel<2, L, C><<<grid, 256, 0, stream>>>(a);
+    wpool_final_kernel<L, C><<<dim3(grid.x, 1, C / 256), 256, 0, stream>>>(a);
   }
+}
+
+static int pool_args(const void* x, const float* w, int B, int T, int S, int Tw, double* part, __half* stats_hi,
+                     __half* stats_lo, PoolArgs* a) {
+  B200_CHECK(x != nullptr && T >= 1 && S >= 1 && (w == nullptr ? S == 1 : Tw >= 1), B200_ERR_INVALID,
+             "weighted pooling: bad arguments");
+  a->x = x;
+  a->w = w;
+  a->S = S; a->T = T; a->Tw = w ? Tw : T;
+  a->nslices = ceil_div(T, kPoolSlice);
+  a->scale = (float)a->Tw / (float)T;
+  a->part = part;
+  a->hi = stats_hi; a->lo = stats_lo;
+  B200_CHECK(a->nslices <= 65535 && (size_t)B * S * 10 <= 0x7fffffffu, B200_ERR_INVALID,
+             "weighted pooling: %d frames x %lld rows is too large", T, (long long)B * S);
+  B200_CHECK(a->nslices == 1 || part != nullptr, B200_ERR_INVALID, "weighted pooling: scratch missing");
+  return B200_OK;
 }
 
 int weighted_pool_forward(const __half* feat, const float* frames, const float* w, int B, int T, int S, int Tw, int C,
                           double* part, __half* stats_hi, __half* stats_lo, cudaStream_t stream) {
-  B200_CHECK((feat == nullptr) != (frames == nullptr) && T >= 1 && S >= 1 && (w == nullptr ? S == 1 : Tw >= 1),
-             B200_ERR_INVALID, "weighted pooling: bad arguments");
+  B200_CHECK((feat == nullptr) != (frames == nullptr), B200_ERR_INVALID, "weighted pooling: bad arguments");
   PoolArgs a;
-  a.x = feat ? (const void*)feat : (const void*)frames;
-  a.w = w;
-  a.S = S; a.T = T; a.Tw = w ? Tw : T;
-  a.nslices = ceil_div(T, kPoolSlice);
-  a.scale = (float)a.Tw / (float)T;
-  a.part = part;
-  a.hi = stats_hi; a.lo = stats_lo;
-  B200_CHECK(a.nslices <= 65535 && (size_t)B * S * 10 <= 0x7fffffffu, B200_ERR_INVALID,
-             "weighted pooling: %d frames x %lld rows is too large", T, (long long)B * S);
-  B200_CHECK(a.nslices == 1 || part != nullptr, B200_ERR_INVALID, "weighted pooling: scratch missing");
+  int rc;
+  if ((rc = pool_args(feat ? (const void*)feat : (const void*)frames, w, B, T, S, Tw, part, stats_hi, stats_lo, &a)))
+    return rc;
+  a.Cv = C; a.F = T; a.ld_out = 2 * 10 * C;
   B200_CHECK(C == 256 || C == 1024, B200_ERR_STATE, "weighted pooling: %d channels unsupported", C);
-  if (C == 256) wpool_launch<256>(a, feat != nullptr, (size_t)B * S, stream);
-  else wpool_launch<1024>(a, feat != nullptr, (size_t)B * S, stream);
+  const size_t rows = (size_t)B * S;
+  if (C == 256) {
+    if (feat) wpool_launch<kPoolNHWC, 256>(a, rows, stream);
+    else wpool_launch<kPoolNCHW, 256>(a, rows, stream);
+  } else {
+    if (feat) wpool_launch<kPoolNHWC, 1024>(a, rows, stream);
+    else wpool_launch<kPoolNCHW, 1024>(a, rows, stream);
+  }
+  B200_CUDA_OK(cudaGetLastError());
+  return B200_OK;
+}
+
+int weighted_pool_rows(const float* x, int F, int T, int C, const float* w, int B, int S, int Tw, double* part,
+                       __half* stats_hi, __half* stats_lo, int ld_out, cudaStream_t stream) {
+  PoolArgs a;
+  int rc;
+  if ((rc = pool_args(x, w, B, T, S, Tw, part, stats_hi, stats_lo, &a))) return rc;
+  B200_CHECK(C >= 1 && C <= kPoolRowsLd && T <= F && ld_out >= 2 * C, B200_ERR_INVALID,
+             "weighted pooling: %d channels of %d-wide rows, %d of %d frames", C, kPoolRowsLd, T, F);
+  a.Cv = C; a.F = F; a.ld_out = ld_out;
+  wpool_launch<kPoolRows, kPoolRowsLd>(a, (size_t)B * S, stream);
   B200_CUDA_OK(cudaGetLastError());
   return B200_OK;
 }

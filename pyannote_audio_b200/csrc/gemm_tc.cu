@@ -9,7 +9,8 @@
 // term is 2^-22 relative): three wgmma per K=16 step instead of an FFMA loop.
 //
 // Used for the LSTM input projections (N = 1024, K = 64 | 256; PyanNet.py:98,226-228), the two Linear+LeakyReLU
-// layers (N = 128, K = 256 | 128; PyanNet.py:236-238) and the embedding Linear (N = 256, K = 5120).
+// layers (N = 128, K = 256 | 128; PyanNet.py:236-238), the embedding Linears (N = 256, K = 5120; N = 512, K = 3008)
+// and, as implicit GEMMs, the dilated TDNN layers of XVectorSincNet (xvector.py:205-252, see GemmTaps in seg.cuh).
 // One CTA per 128 x 128 output tile: warp 8 is the TMA producer, warpgroups 0 and 1 each own 64 rows of the tile and
 // issue their wgmma on the shared A/B stages (ring of mbarrier-guarded stages, 128-byte swizzle).
 #include "common.cuh"
@@ -38,6 +39,10 @@ struct GemmTcParams {
   // and no separate collective runs
   float* C_peer[7];
   int n_peer;
+  // implicit GEMM over taps: k-block kb belongs to tap kb / tap_kb and reads A rows shifted by tap * dil
+  int tap_kb, dil;
+  const float* scale;  // post-activation affine (or nullptr)
+  const float* shift;
 };
 
 __global__ void __launch_bounds__(kGemmThreads, 1)
@@ -65,8 +70,10 @@ gemm_tc_split_kernel(const __grid_constant__ CUtensorMap tmAh, const __grid_cons
         mbar_wait(bar_empty + 8 * stage, phase ^ 1);
         mbar_expect_tx(bar_full + 8 * stage, kGemmStageBytes);
         const uint32_t sa = stage0 + stage * kGemmStageBytes;
-        tma_load_2d(&tmAh, bar_full + 8 * stage, sa, kb * kGemmK, tm * kGemmM);
-        tma_load_2d(&tmAl, bar_full + 8 * stage, sa + kGemmTile, kb * kGemmK, tm * kGemmM);
+        // one tap: tap = 0 and the A box is (kb * 64, tm * 128) as for a plain GEMM
+        const int tap = kb / p.tap_kb, ka = (kb - tap * p.tap_kb) * kGemmK, ra = tm * kGemmM + tap * p.dil;
+        tma_load_2d(&tmAh, bar_full + 8 * stage, sa, ka, ra);
+        tma_load_2d(&tmAl, bar_full + 8 * stage, sa + kGemmTile, ka, ra);
         tma_load_2d(&tmBh, bar_full + 8 * stage, sa + 2 * kGemmTile, kb * kGemmK, tn * kGemmN);
         tma_load_2d(&tmBl, bar_full + 8 * stage, sa + 3 * kGemmTile, kb * kGemmK, tn * kGemmN);
         if (++stage == kGemmStages) { stage = 0; phase ^= 1; }
@@ -113,6 +120,7 @@ gemm_tc_split_kernel(const __grid_constant__ CUtensorMap tmAh, const __grid_cons
       float a = acc[4 * j + 2 * i], c = acc[4 * j + 2 * i + 1];
       if (p.bias) { a += p.bias[col]; c += p.bias[col + 1]; }
       if (p.act == 1) { a = a > 0.f ? a : 0.01f * a; c = c > 0.f ? c : 0.01f * c; }
+      if (p.scale) { a = a * p.scale[col] + p.shift[col]; c = c * p.scale[col + 1] + p.shift[col + 1]; }
       if (p.C) {
         const float2 v = make_float2(a, c);
         *reinterpret_cast<float2*>(p.C + (size_t)m * p.ldc + col) = v;
@@ -163,10 +171,14 @@ static int make_map_2d(CUtensorMap* tm, const __half* ptr, int rows, int K, int 
 
 int gemm_tc_split(const __half* A_hi, const __half* A_lo, int lda, const __half* B_hi, const __half* B_lo, int ldb,
                   float* C, int ldc, __half* C_hi, __half* C_lo, int ldc_h, const float* bias, int M, int N, int K,
-                  int act, int num_sms, cudaStream_t stream, float* const* C_peers, int n_peers) {
+                  int act, int num_sms, cudaStream_t stream, float* const* C_peers, int n_peers,
+                  const GemmTaps& taps) {
   (void)num_sms;
   B200_CHECK(K % kGemmK == 0 && N % kGemmN == 0 && lda % 8 == 0 && ldb % 8 == 0, B200_ERR_INVALID,
              "gemm_tc_split: unsupported shape M=%d N=%d K=%d", M, N, K);
+  B200_CHECK(taps.taps >= 1 && K % (taps.taps * kGemmK) == 0 && taps.dil >= 0 &&
+                 (taps.scale == nullptr) == (taps.shift == nullptr),
+             B200_ERR_INVALID, "gemm_tc_split: %d taps do not split K=%d into 64-wide k-blocks", taps.taps, K);
   B200_CHECK(n_peers >= 0 && n_peers <= 7 && (n_peers == 0 || (C_peers && C)), B200_ERR_INVALID,
              "gemm_tc_split: at most 7 peer outputs");
   if (M == 0) return B200_OK;
@@ -177,10 +189,16 @@ int gemm_tc_split(const __half* A_hi, const __half* A_lo, int lda, const __half*
   for (int i = 0; i < n_peers; ++i) p.C_peer[i] = C_peers[i];
   p.kblocks = K / kGemmK;
   p.tiles_n = N / kGemmN;
+  const int Ka = K / taps.taps;                             // A width: one tap's channels
+  p.tap_kb = Ka / kGemmK;
+  p.dil = taps.dil;
+  p.scale = taps.scale;
+  p.shift = taps.shift;
   CUtensorMap tmAh, tmAl, tmBh, tmBl;
   int rc;
-  if ((rc = make_map_2d(&tmAh, A_hi, M, K, lda, kGemmM))) return rc;
-  if ((rc = make_map_2d(&tmAl, A_lo, M, K, lda, kGemmM))) return rc;
+  // rows of the shifted taps past M read as zero (TMA out-of-bounds fill)
+  if ((rc = make_map_2d(&tmAh, A_hi, M, Ka, lda, kGemmM))) return rc;
+  if ((rc = make_map_2d(&tmAl, A_lo, M, Ka, lda, kGemmM))) return rc;
   if ((rc = make_map_2d(&tmBh, B_hi, N, K, ldb, kGemmN))) return rc;
   if ((rc = make_map_2d(&tmBl, B_lo, N, K, ldb, kGemmN))) return rc;
   const size_t smem = 1024 + 1024 + (size_t)kGemmStages * kGemmStageBytes;

@@ -27,9 +27,8 @@ inline SegGeom seg_geom(int W) {
   return g;
 }
 
-struct SegWeights {
-  bool loaded = false;
-  int lstm_layers = 4;
+// SincNet front end (models/blocks/sincnet.py:41-79), shared by PyanNet and XVectorSincNet
+struct SincNetWeights {
   float wav_w = 1.f, wav_b = 0.f;   // sincnet.wav_norm1d affine
   __half* sinc_wg_hi = nullptr;     // [80 filters][256 taps] fp16 (hi, lo) for the wgmma sinc layer (taps >= 251 zero)
   __half* sinc_wg_lo = nullptr;
@@ -40,6 +39,12 @@ struct SegWeights {
   float* conv_b[2] = {nullptr, nullptr};   // [60]
   __half* conv_wg_hi[2] = {nullptr, nullptr};   // [64 rows = c_out (60 real)][5 taps x Cpad channels] fp16 (hi, lo)
   __half* conv_wg_lo[2] = {nullptr, nullptr};
+};
+
+struct SegWeights {
+  bool loaded = false;
+  int lstm_layers = 4;
+  SincNetWeights sinc;
   // LSTM, per layer: W_ih for both directions [1024][Kpad] with row = dir*512 + unit*4 + gate; bias = b_ih+b_hh
   float* w_ih[8] = {};
   float* b_g[8] = {};
@@ -61,10 +66,19 @@ struct SegWeights {
 int sgemm_nt(const float* A, int lda, const float* Bw, int ldb, float* C, int ldc, const float* bias, int M, int N,
              int K, int act, cudaStream_t stream);
 
+// Implicit-GEMM extension of gemm_tc_split (TDNN layers of XVectorSincNet): A is [M][Cpad] with Cpad = K / taps,
+// output row r reads A rows r + j * dil for the taps j = 0 .. taps - 1 (K ordered tap-major), and the epilogue
+// applies y = act(acc + bias) * scale + shift per column (eval-mode BatchNorm after the activation) when scale != NULL.
+struct GemmTaps {
+  int taps = 1, dil = 0;
+  const float* scale = nullptr;
+  const float* shift = nullptr;
+};
 // split-precision tensor-core GEMM (gemm_tc.cu): C = act(A B^T + bias), A/B as fp16 (hi, lo) pairs
 int gemm_tc_split(const __half* A_hi, const __half* A_lo, int lda, const __half* B_hi, const __half* B_lo, int ldb,
                   float* C, int ldc, __half* C_hi, __half* C_lo, int ldc_h, const float* bias, int M, int N, int K,
-                  int act, int num_sms, cudaStream_t stream, float* const* C_peers = nullptr, int n_peers = 0);
+                  int act, int num_sms, cudaStream_t stream, float* const* C_peers = nullptr, int n_peers = 0,
+                  const GemmTaps& taps = GemmTaps());
 int split_f16(const float* x, __half* hi, __half* lo, size_t n, cudaStream_t st);
 // tensor-core recurrence (seg_lstm_wg.cu): Gx [NB][T][1024] -> layer output as fp16 (hi, lo) [NB][T][256]
 int lstm_rec_wg(const float* Gx, const __half* Wh, const __half* Wl, __half* Yh, __half* Yl, int NB, int T,
@@ -81,7 +95,7 @@ int conv5_wg_forward(const SegGeom& g, int layer, const float* Pin, const float2
 // (60 features + 4 zero pad)
 size_t sincnet_workspace_bytes(const SegGeom& g, int NB);
 int sincnet_launches(const SegGeom& g);   // kernels sincnet_forward launches per sub-batch
-int sincnet_forward(const SegWeights& W, const SegGeom& g, const float* wav, const long long* chunk_off,
+int sincnet_forward(const SincNetWeights& W, const SegGeom& g, const float* wav, const long long* chunk_off,
                     const int* chunk_valid, int NB, void* ws, float* x0, int conv_impl, cudaStream_t stream);
 
 // BiLSTM stack + linear head on sequences of T frames: X0 -> class ids [NB][T] u8 (+ optional log-probs [NB][T][7])

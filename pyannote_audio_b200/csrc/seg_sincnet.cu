@@ -399,7 +399,7 @@ int sincnet_launches(const SegGeom& g) {
   return n;
 }
 
-int sincnet_forward(const SegWeights& W, const SegGeom& g, const float* wav, const long long* chunk_off,
+int sincnet_forward(const SincNetWeights& W, const SegGeom& g, const float* wav, const long long* chunk_off,
                     const int* chunk_valid, int NB, void* ws, float* x0, int conv_impl, cudaStream_t stream) {
   SincWs w;
   carve(g, NB, ws, &w);

@@ -16,7 +16,7 @@ import torch
 from . import ops
 from .audio import AudioFile
 from .core import Resolution, Segment, SlidingWindow, SlidingWindowFeature, Specifications
-from .models import BaseWeSpeakerResNet, Model
+from .models import Model
 
 
 class BaseInference:
@@ -124,7 +124,7 @@ class Inference(BaseInference):
         return cls, wav_dev, off, valid
 
     def slide(self, waveform: torch.Tensor, sample_rate: int, hook: Optional[Callable] = None):
-        if isinstance(self.model, BaseWeSpeakerResNet):
+        if self.model.specifications.resolution == Resolution.CHUNK:      # embedding models
             return self._slide_embedding(waveform, sample_rate, hook=hook)
         cls, _, off, _ = self.slide_device(waveform, sample_rate, return_logp=self.conversion != "powerset")
         total = len(off)
@@ -157,7 +157,7 @@ class Inference(BaseInference):
     def _slide_embedding(self, waveform: torch.Tensor, sample_rate: int, hook: Optional[Callable] = None):
         """One embedding per window (inference.py:261-313 for a Resolution.CHUNK model): the chunks are cut as the
         reference cuts them, the last one zero-padded to the full window, and all of them (they have one length) go
-        through one library call over a resident copy of the file -> SlidingWindowFeature (chunks, 256)."""
+        through one library call over a resident copy of the file -> SlidingWindowFeature (chunks, dimension)."""
         window_size = self.model.audio.get_num_samples(self.duration)
         step_size = round(self.step * sample_rate)
         _, num_samples = waveform.shape
@@ -169,7 +169,7 @@ class Inference(BaseInference):
         wav_dev = torch.zeros(int(off[-1]) + window_size, dtype=torch.float32, device=ctx.device)
         wav_dev[:num_samples].copy_(waveform[0])
         try:
-            emb = ctx.emb_forward_utt(wav_dev, off, window_size)
+            emb = self.model.forward_utterances(wav_dev, off, window_size)
         except MemoryError:
             raise MemoryError(f"batch_size ({self.batch_size: d}) is probably too large. "
                               f"Try with a smaller value until memory error disappears.")

@@ -1,11 +1,12 @@
-"""Model-level seam: ``PyanNet`` and the WeSpeaker ResNets (``WeSpeakerResNet34`` and the bottleneck
-``WeSpeakerResNet152`` / ``221`` / ``293``) with the reference's state-dict keys and ``forward``
-contract, computing through libb200diar.so (no torch ops on the forward path, no CPU fallback).
+"""Model-level seam: ``PyanNet``, the WeSpeaker ResNets (``WeSpeakerResNet34`` and the bottleneck
+``WeSpeakerResNet152`` / ``221`` / ``293``) and ``XVectorSincNet`` with the reference's state-dict keys and
+``forward`` contract, computing through libb200diar.so (no torch ops on the forward path, no CPU fallback).
 
 Reference interfaces mirrored (paths relative to /root/reference/src/pyannote/audio):
   core/model.py:69-183 (Model: specifications, audio, receptive_field, device)
   models/segmentation/PyanNet.py:92-240 (ctor hyper-parameters, num_frames, receptive field, forward)
   models/embedding/wespeaker/__init__.py:41-466 (forward / forward_frames / forward_embedding / dimension)
+  models/embedding/xvector.py:205-349 (XVectorSincNet)
 """
 from __future__ import annotations
 
@@ -59,7 +60,7 @@ class Model(nn.Module):
         self._weights_version = 0
         self.register_load_state_dict_post_hook(lambda module, incompatible: module._bump_weights())
 
-    _SLOT = ""          # "seg" | "emb": the context slot this model family uploads into
+    _SLOT = ""          # "seg" | "emb" | "xvec": the context slot this model family uploads into
 
     def _bump_weights(self):
         self._weights_version += 1
@@ -118,10 +119,12 @@ class Model(nn.Module):
         meta = loaded["pyannote.audio"]
         class_name = meta["architecture"]["class"]
         klass = {"PyanNet": PyanNet, "WeSpeakerResNet34": WeSpeakerResNet34, "WeSpeakerResNet152": WeSpeakerResNet152,
-                 "WeSpeakerResNet221": WeSpeakerResNet221, "WeSpeakerResNet293": WeSpeakerResNet293}.get(class_name)
+                 "WeSpeakerResNet221": WeSpeakerResNet221, "WeSpeakerResNet293": WeSpeakerResNet293,
+                 "XVectorSincNet": XVectorSincNet}.get(class_name)
         if klass is None:
             raise NotImplementedError(f"architecture {meta['architecture']['module']}.{class_name} has no CUDA "
-                                      f"implementation (PyanNet and WeSpeakerResNet34 / 152 / 221 / 293 have one)")
+                                      f"implementation (PyanNet, WeSpeakerResNet34 / 152 / 221 / 293 and "
+                                      f"XVectorSincNet have one)")
         if cls not in (Model, klass) and not issubclass(klass, cls):
             raise ValueError(f"checkpoint holds a {class_name}, not a {cls.__name__}")
         hparams = dict(loaded.get("hyper_parameters", {}))
@@ -408,8 +411,17 @@ class BaseWeSpeakerResNet(Model):
     def dimension(self) -> int:
         return 256
 
+    # smallest input for which kaldi.fbank yields a frame (speaker_verification.py:688-702 finds it by bisection on
+    # exceptions; with a 400-sample analysis window the bisection converges to 400)
+    min_num_samples = 400
+
     def _upload(self, ctx):
         ctx.load_embedding(self.state_dict())
+
+    def forward_utterances(self, wav: torch.Tensor, off, num_samples: int, weights: Optional[torch.Tensor] = None):
+        """Embeddings of utterances of one length inside one device waveform (ops.Context.emb_forward_utt):
+        soft (n, Tw) / (n, S, Tw) weights or None -> (n, max(S, 1), 256)."""
+        return self._ctx().emb_forward_utt(wav, off, num_samples, weights=weights)
 
     def num_frames(self, num_samples: int) -> int:
         n = _conv1d_num_frames(num_samples, 400, 160)
@@ -510,3 +522,87 @@ class WeSpeakerResNet221(_BottleneckWeSpeakerResNet):
 
 class WeSpeakerResNet293(_BottleneckWeSpeakerResNet):
     NUM_BLOCKS = (10, 20, 64, 3)
+
+
+class XVectorSincNet(Model):
+    """x-vector on the SincNet front end (xvector.py:205-349; the architecture of pyannote/embedding): SincNet, five
+    dilated TDNN layers (Conv1d -> LeakyReLU -> BatchNorm1d), StatsPool and a Linear to ``dimension``."""
+
+    _SLOT = "xvec"
+    _HPARAMS = ("sincnet", "dimension", "sample_rate", "num_channels")
+    KERNEL = [5, 3, 3, 1, 1]
+    DILATION = [1, 2, 3, 1, 1]
+    min_num_samples = ops.XVEC_MIN_SAMPLES
+
+    def __init__(self, sample_rate: int = 16000, num_channels: int = 1, sincnet: Optional[dict] = None,
+                 dimension: int = 512):
+        super().__init__(sample_rate=sample_rate, num_channels=num_channels)
+        sinc_hp = {"stride": 10}
+        sinc_hp.update(sincnet or {})
+        sinc_hp["sample_rate"] = sample_rate
+        if sample_rate != 16000 or sinc_hp["stride"] != 10 or num_channels != 1 or int(dimension) < 1:
+            raise NotImplementedError("the CUDA kernels implement XVectorSincNet on mono 16 kHz audio with SincNet "
+                                      "stride 10 and a positive embedding dimension only")
+        self.hparams.sincnet, self.hparams.dimension = sinc_hp, int(dimension)
+        self.sincnet = _SincNetParams()
+        layers, in_channel = [], 60
+        for (_, out_channel, k, d) in ops.XVEC_TDNN:
+            layers += [nn.Conv1d(in_channel, out_channel, k, dilation=d), nn.LeakyReLU(), nn.BatchNorm1d(out_channel)]
+            in_channel = out_channel
+        self.tdnns = nn.ModuleList(layers)
+        self.embedding = nn.Linear(2 * in_channel, int(dimension))
+        self.specifications = Specifications(problem=Problem.REPRESENTATION, resolution=Resolution.CHUNK, duration=10.0)
+        self.eval()
+        for p in self.parameters():
+            p.requires_grad_(False)
+
+    @property
+    def dimension(self) -> int:
+        return self.hparams.dimension
+
+    def num_frames(self, num_samples: int) -> int:
+        n = num_samples
+        for k, s in zip(PyanNet.KERNEL, PyanNet.STRIDE):
+            n = _conv1d_num_frames(n, k, s)
+        for k, d in zip(self.KERNEL, self.DILATION):
+            n = _conv1d_num_frames(n, k, 1, d=d)
+        return n
+
+    def receptive_field_size(self, num_frames: int = 1) -> int:
+        rf = num_frames
+        for k, d in reversed(list(zip(self.KERNEL, self.DILATION))):
+            rf = 1 + (k - 1) * d + (rf - 1)
+        for k, s in reversed(list(zip(PyanNet.KERNEL, PyanNet.STRIDE))):
+            rf = 1 + (k - 1) + (rf - 1) * s
+        return rf
+
+    def receptive_field_center(self, frame: int = 0) -> int:
+        c = frame
+        for k, d in reversed(list(zip(self.KERNEL, self.DILATION))):
+            c = c + (1 + (k - 1) * d - 1) // 2
+        for k, s in reversed(list(zip(PyanNet.KERNEL, PyanNet.STRIDE))):
+            c = c * s + (k - 1) // 2
+        return c
+
+    def _upload(self, ctx):
+        ctx.load_xvector(self.state_dict())
+
+    def forward_utterances(self, wav: torch.Tensor, off, num_samples: int, weights: Optional[torch.Tensor] = None):
+        """Embeddings of utterances of one length inside one device waveform (ops.Context.xvec_forward): soft
+        (n, Tw) / (n, S, Tw) weights or None -> (n, max(S, 1), dimension)."""
+        return self._ctx().xvec_forward(wav, off, num_samples, weights=weights)
+
+    def forward(self, waveforms: torch.Tensor, weights: Optional[torch.Tensor] = None) -> torch.Tensor:
+        """waveforms (batch, 1, samples) with samples >= 4771, weights None, (batch, frames) or
+        (batch, speakers, frames) of any real values -> (batch, dimension) or (batch, speakers, dimension)."""
+        b, c, s = waveforms.shape
+        if c != 1:
+            raise ValueError(f"XVectorSincNet kernels expect mono waveforms, got {c} channels")
+        if s < ops.XVEC_MIN_SAMPLES:
+            raise ValueError(f"XVectorSincNet needs at least {ops.XVEC_MIN_SAMPLES} samples, got {s}")
+        if weights is not None and (weights.dim() not in (2, 3) or weights.shape[0] != b or weights.shape[-1] < 1):
+            raise ValueError("weights must be (batch, frames) or (batch, speakers, frames)")
+        ctx = self._ctx()
+        flat = waveforms.to(device=ctx.device, dtype=torch.float32).reshape(-1).contiguous()
+        emb = self.forward_utterances(flat, np.arange(b, dtype=np.int64) * s, s, weights=weights)
+        return emb if weights is not None and weights.dim() == 3 else emb[:, 0]

@@ -18,6 +18,8 @@ SPEAKERS = 3
 CLASSES = 7
 EMB_DIM = 256
 SEG_MIN_SAMPLES = 1261     # shortest PyanNet window: 2 output frames (one frame cannot be instance-normalised)
+XVEC_MIN_SAMPLES = 4771    # shortest XVectorSincNet input: 15 SincNet frames, one frame after the TDNN layers
+XVEC_TDNN = ((60, 512, 5, 1), (512, 512, 3, 2), (512, 512, 3, 3), (512, 512, 1, 1), (512, 1500, 1, 1))
 
 
 def seg_num_frames(num_samples: int) -> int:
@@ -91,7 +93,9 @@ class Context:
         self.seg_loaded = False
         self.emb_loaded = False
         self.emb_channels = 256   # trunk output channels of the loaded embedding model: 256 (ResNet34) or 1024
-        self.owners = {}          # slot ("seg" | "emb") -> stamp of the model whose weights are resident (models.py)
+        self.xvec_loaded = False
+        self.xvec_dimension = 512
+        self.owners = {}          # slot ("seg" | "emb" | "xvec") -> stamp of the model whose weights are resident
         # A/B knob for scripts (like B200_CONV_IMPL / B200_EMB_MAX_BATCH / B200_SEG_MAX_BATCH, which the library
         # reads itself): B200_OPTIONS="key=value,..."
         # is applied through b200_ctx_set_option, so unknown keys / bad values fail loudly
@@ -202,6 +206,50 @@ class Context:
         self.emb_loaded = False
         _lib.check(self.lib.b200_emb_load(self._h, C.byref(w)))
         self.emb_loaded, self.emb_channels = True, 256
+
+    def load_xvector(self, sd: Mapping[str, torch.Tensor]):
+        """XVectorSincNet weights (models/embedding/xvector.py:205-252) into the ctx's own slot."""
+        keep = []
+
+        def f(name):
+            t = sd[name].detach().to(torch.float32).cpu().contiguous()
+            keep.append(t)
+            return _fp(t)
+
+        w = _lib.XvecWeights()
+        w.wav_norm_weight = float(sd["sincnet.wav_norm1d.weight"].reshape(-1)[0])
+        w.wav_norm_bias = float(sd["sincnet.wav_norm1d.bias"].reshape(-1)[0])
+        p = "sincnet.conv1d.0.filterbank."
+        bank = sinc_filter_bank(sd[p + "low_hz_"], sd[p + "band_hz_"], sd.get(p + "window_"), sd.get(p + "n_"))
+        keep.append(bank)
+        w.sinc_filters = _fp(bank)
+        for i in range(3):
+            w.norm_weight[i] = f(f"sincnet.norm1d.{i}.weight")
+            w.norm_bias[i] = f(f"sincnet.norm1d.{i}.bias")
+        for i in range(2):
+            w.conv_weight[i] = f(f"sincnet.conv1d.{i + 1}.weight")
+            w.conv_bias[i] = f(f"sincnet.conv1d.{i + 1}.bias")
+        for layer, (cin, cout, k, _) in enumerate(XVEC_TDNN):
+            conv, bn = f"tdnns.{3 * layer}", f"tdnns.{3 * layer + 2}"
+            if tuple(sd[conv + ".weight"].shape) != (cout, cin, k):
+                raise ValueError(f"{conv}.weight has shape {tuple(sd[conv + '.weight'].shape)}, expected "
+                                 f"{(cout, cin, k)}")
+            w.tdnn_weight[layer] = f(conv + ".weight")
+            w.tdnn_bias[layer] = f(conv + ".bias")
+            w.bn_weight[layer] = f(bn + ".weight")
+            w.bn_bias[layer] = f(bn + ".bias")
+            w.bn_mean[layer] = f(bn + ".running_mean")
+            w.bn_var[layer] = f(bn + ".running_var")
+        dim, k_in = sd["embedding.weight"].shape
+        if k_in != 3000:
+            raise ValueError(f"embedding.weight has {k_in} inputs, expected 3000")
+        w.dimension = int(dim)
+        w.embedding_weight = f("embedding.weight")
+        w.embedding_bias = f("embedding.bias")
+        self.owners.pop("xvec", None)
+        self.xvec_loaded = False
+        _lib.check(self.lib.b200_xvec_load(self._h, C.byref(w)))
+        self.xvec_loaded, self.xvec_dimension = True, int(dim)
 
     def _load_bottleneck(self, sd, f, conv_bn):
         """WeSpeakerResNet152 / 221 / 293 (Bottleneck blocks, resnet.py:148-212): the block counts come from the keys."""
@@ -342,6 +390,26 @@ class Context:
         with torch.cuda.device(self.device):
             _lib.check(self.lib.b200_emb_forward_utt(self._h, _ptr(wav), off.ctypes.data, num_samples, n, _ptr(w),
                                                      S if w is not None else 0, Tw, _ptr(emb), _stream(self.device)))
+        return emb
+
+    def xvec_forward(self, wav, off, num_samples: int, weights: Optional[torch.Tensor] = None,
+                     out: Optional[torch.Tensor] = None):
+        """XVectorSincNet embeddings of utterances of one length: utterance i = wav[off[i] : off[i] + num_samples]
+        (>= 4771 samples).  ``weights``: None or (n, Tw) / (n, S, Tw) pooling weights of any real values (any Tw,
+        nearest-interpolated onto the TDNN frames) -> (n, max(S, 1), dimension) float32."""
+        if wav.device != self.device or wav.dtype != torch.float32 or not wav.is_contiguous():
+            raise ValueError(f"waveform must be a contiguous float32 tensor on {self.device}")
+        off = np.ascontiguousarray(off, dtype=np.int64).reshape(-1)
+        n, num_samples = len(off), int(num_samples)
+        if num_samples < XVEC_MIN_SAMPLES:
+            raise ValueError(f"XVectorSincNet needs at least {XVEC_MIN_SAMPLES} samples, got {num_samples}")
+        if n and (int(off.min()) < 0 or int(off.max()) + num_samples > wav.numel()):
+            raise ValueError("an utterance reads outside the waveform buffer")
+        w, S, Tw = self._pool_weights(weights, n)
+        emb = self._out(out, (n, S, self.xvec_dimension), torch.float32)
+        with torch.cuda.device(self.device):
+            _lib.check(self.lib.b200_xvec_forward(self._h, _ptr(wav), off.ctypes.data, num_samples, n, _ptr(w),
+                                                  S if w is not None else 0, Tw, _ptr(emb), _stream(self.device)))
         return emb
 
     def emb_forward_embedding(self, frames: torch.Tensor, weights: Optional[torch.Tensor] = None):

@@ -8,15 +8,15 @@ import numpy as np
 import torch
 
 from .audio import AudioFile
-from .models import BaseWeSpeakerResNet, PyanNet, WeSpeakerResNet34
+from .models import BaseWeSpeakerResNet, PyanNet, WeSpeakerResNet34, XVectorSincNet
 
 
 class SpeakerEmbedding:
-    """``apply(file)`` -> (1, 256) ndarray.  Without ``segmentation`` the statistics pooling runs over the whole file;
-    with it, frames are weighted by the cubed aggregated speech score of the voice activity detection
-    (max over the speakers of the segmentation model), interpolated onto the trunk frames."""
+    """``apply(file)`` -> (1, dimension) ndarray.  Without ``segmentation`` the statistics pooling runs over the whole
+    file; with it, frames are weighted by the cubed aggregated speech score of the voice activity detection
+    (max over the speakers of the segmentation model), interpolated onto the model's frames."""
 
-    def __init__(self, embedding: Union[BaseWeSpeakerResNet, Mapping, str, None] = None,
+    def __init__(self, embedding: Union[BaseWeSpeakerResNet, XVectorSincNet, Mapping, str, None] = None,
                  segmentation: Union[PyanNet, Mapping, str, None] = None, token=None, cache_dir=None,
                  device: Optional[torch.device] = None):
         from .loading import get_model, is_checkpoint_spec
@@ -27,9 +27,9 @@ class SpeakerEmbedding:
             model = WeSpeakerResNet34()
             model.load_state_dict(embedding)
             embedding = model
-        if not isinstance(embedding, BaseWeSpeakerResNet):
-            raise ValueError("`embedding` must be a WeSpeaker ResNet instance, a ResNet34 state dict or a local checkpoint "
-                             "(no hub access here)")
+        if not isinstance(embedding, (BaseWeSpeakerResNet, XVectorSincNet)):
+            raise ValueError("`embedding` must be a WeSpeaker ResNet or XVectorSincNet instance, a ResNet34 state dict "
+                             "or a local checkpoint (no hub access here)")
         device = device or torch.device("cuda", torch.cuda.current_device() if torch.cuda.is_available() else 0)
         self.embedding = embedding
         self.segmentation = segmentation
@@ -58,11 +58,12 @@ class SpeakerEmbedding:
             with torch.inference_mode():
                 return model(waveform[None]).cpu().numpy()
         weights = torch.from_numpy(self.speech_weights(file))[None].to(model.device)
-        ctx = model._ctx()
-        wav = waveform[0].to(device=ctx.device, dtype=torch.float32).contiguous()
-        if wav.numel() < 400:
-            raise ValueError(f"WeSpeaker needs at least 400 samples (one 25 ms fbank frame), got {wav.numel()}")
-        # soft weights: straight to the library (forward itself keeps the binary-mask contract)
-        return ctx.emb_forward_utt(wav, np.zeros(1, dtype=np.int64), wav.numel(), weights=weights)[:, 0].cpu().numpy()
+        wav = waveform[0].to(device=model.device, dtype=torch.float32).contiguous()
+        if wav.numel() < model.min_num_samples:
+            raise ValueError(f"{type(model).__name__} needs at least {model.min_num_samples} samples, got "
+                             f"{wav.numel()}")
+        # soft weights: the model's utterance entry (WeSpeaker's forward keeps the binary-mask contract)
+        return model.forward_utterances(wav, np.zeros(1, dtype=np.int64), wav.numel(),
+                                        weights=weights)[:, 0].cpu().numpy()
 
     __call__ = apply

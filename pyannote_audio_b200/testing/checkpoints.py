@@ -6,7 +6,8 @@ from . import synthetic as syn
 
 
 def reference_style_checkpoint(kind):
-    """``kind``: "seg" (PyanNet), "emb" (WeSpeakerResNet34) or "emb293" (WeSpeakerResNet293).  A Lightning-format pytorch_model.bin as the reference writes it (model.py:244-256): state_dict +
+    """``kind``: "seg" (PyanNet), "emb" (WeSpeakerResNet34), "emb293" (WeSpeakerResNet293) or "xvec"
+    (XVectorSincNet).  A Lightning-format pytorch_model.bin as the reference writes it (model.py:244-256): state_dict +
     hyper_parameters + checkpoint["pyannote.audio"] whose `specifications` is pickled under the REFERENCE's module
     path pyannote.audio.core.task (registered here only while pickling, then removed again)."""
     import dataclasses
@@ -67,6 +68,14 @@ def reference_style_checkpoint(kind):
                                      "architecture": {"module": "pyannote.audio.models.embedding.wespeaker",
                                                       "class": "WeSpeakerResNet293"},
                                      "specifications": Specifications(Problem.REPRESENTATION, Resolution.CHUNK, 10.0)}}
+        elif kind == "xvec":
+            ck = {"state_dict": syn.make_xvector_state_dict(3),
+                  "hyper_parameters": {"sincnet": {"stride": 10, "sample_rate": 16000}, "dimension": 512,
+                                       "sample_rate": 16000, "num_channels": 1},
+                  "pyannote.audio": {"versions": {"pyannote.audio": "4.0.0"},
+                                     "architecture": {"module": "pyannote.audio.models.embedding.xvector",
+                                                      "class": "XVectorSincNet"},
+                                     "specifications": Specifications(Problem.REPRESENTATION, Resolution.CHUNK, 3.0)}}
         else:
             ck = {"state_dict": syn.make_embedding_state_dict(1),
                   "hyper_parameters": {"sample_rate": 16000, "num_channels": 1, "num_mel_bins": 80,

@@ -8,6 +8,7 @@ with the *reference's state-dict key names and shapes* (real checkpoints drop in
   models/blocks/sincnet.py:41-79 (module tree: tutorials/training_a_model.ipynb:1001-1016)
 * embedding: ``WeSpeakerResNet34``; keys as in models/embedding/wespeaker/resnet.py:233-252; the bottleneck
   ``WeSpeakerResNet152`` / ``221`` / ``293`` (resnet.py:148-212) with ``make_bottleneck_state_dict``
+* x-vector: ``XVectorSincNet`` with ``make_xvector_state_dict``; keys as in models/embedding/xvector.py:205-252
 * PLDA: ``xvec_transform.npz{mean1,mean2,lda}`` + ``plda.npz{mu,tr,psi}`` (utils/vbx.py:195-199)
 
 Audio: a synthetic multi-speaker "conversation" (harmonic sources, 3-6 Hz amplitude modulation,
@@ -166,6 +167,31 @@ def make_bottleneck_state_dict(depth: int = 293, seed: int = 1) -> "OrderedDict[
             in_planes = 4 * planes
     sd["resnet.seg_1.weight"] = torch.randn(256, 20480, generator=g) / math.sqrt(20480)
     sd["resnet.seg_1.bias"] = 0.01 * torch.randn(256, generator=g)
+    return sd
+
+
+XVECTOR_TDNN = ((60, 512, 5), (512, 512, 3), (512, 512, 3), (512, 512, 1), (512, 1500, 1))
+
+
+def make_xvector_state_dict(seed: int = 3, dimension: int = 512) -> "OrderedDict[str, torch.Tensor]":
+    """XVectorSincNet weights with the reference's keys (xvector.py:205-252): the SincNet front end drawn like
+    make_segmentation_state_dict's, then per TDNN layer a Conv1d of gain 1.5 / sqrt(fan_in) and a BatchNorm1d whose
+    running statistics are those of a LeakyReLU of a zero-mean input of standard deviation ~1.5 (mean ~0.6, variance
+    ~0.8), so that every layer's output stays O(1) on synthetic speech; the Linear 3000 -> dimension has unit gain."""
+    g = torch.Generator().manual_seed(seed)
+    sd = OrderedDict((k, v) for k, v in make_segmentation_state_dict(seed, fitted_classifier=False).items()
+                     if k.startswith("sincnet."))
+    for layer, (cin, cout, k) in enumerate(XVECTOR_TDNN):
+        conv, bn = f"tdnns.{3 * layer}", f"tdnns.{3 * layer + 2}"
+        sd[conv + ".weight"] = torch.randn(cout, cin, k, generator=g) * (1.5 / math.sqrt(cin * k))
+        sd[conv + ".bias"] = 0.05 * torch.randn(cout, generator=g)
+        sd[bn + ".weight"] = 0.8 + 0.4 * torch.rand(cout, generator=g)
+        sd[bn + ".bias"] = 0.1 * torch.randn(cout, generator=g)
+        sd[bn + ".running_mean"] = 0.6 * (1.0 + 0.2 * torch.randn(cout, generator=g))
+        sd[bn + ".running_var"] = 0.8 * (0.75 + 0.5 * torch.rand(cout, generator=g))
+        sd[bn + ".num_batches_tracked"] = torch.tensor(1000, dtype=torch.long)
+    sd["embedding.weight"] = torch.randn(dimension, 3000, generator=g) / math.sqrt(3000)
+    sd["embedding.bias"] = 0.01 * torch.randn(dimension, generator=g)
     return sd
 
 
