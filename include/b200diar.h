@@ -80,8 +80,18 @@ typedef struct b200_seg_weights {
   const float* classifier_bias;               /* [7]      */
 } b200_seg_weights;
 /* Model.load_state_dict / Model.from_pretrained (core/model.py:497-655) for PyanNet: host fp32 arrays in PyTorch layouts;
- * fp16 (hi, lo) splits, LSTM shared-memory images and the sinc bank's tensor-core layout are made here, once. */
+ * fp16 (hi, lo) splits, LSTM shared-memory images and the sinc bank's tensor-core layout are made here, once.
+ * b200_seg_load is b200_seg_load_head(ctx, w, 7, B200_SEG_LOGSOFTMAX): the community-1 powerset head. */
 int b200_seg_load(b200_ctx* ctx, const b200_seg_weights* w);
+/* PyanNet with any classifier head (models/segmentation/PyanNet.py:141-161, core/model.py:271-300):
+ * classifier_weight is [num_classes][128], classifier_bias [num_classes], 1 <= num_classes <= 32.
+ * B200_SEG_LOGSOFTMAX: mono-label / powerset problems, run with b200_seg_forward_window;
+ * B200_SEG_SIGMOID: binary / multi-label problems, run with b200_seg_forward_scores.
+ * Other class counts or activations return B200_STATUS_INVALID. */
+#define B200_SEG_LOGSOFTMAX 0
+#define B200_SEG_SIGMOID 1
+#define B200_SEG_MAX_CLASSES 32
+int b200_seg_load_head(b200_ctx* ctx, const b200_seg_weights* w, int32_t num_classes, int32_t activation);
 
 /* WeSpeakerResNet34 (models/embedding/wespeaker/resnet.py:84-145, 214-252).  conv weight [Cout][Cin][k][k] fp32,
  * eval-mode BatchNorm2d given by (weight, bias, running_mean, running_var), eps 1e-5; folded by the library. */
@@ -168,20 +178,34 @@ int b200_audio_ingest(b200_ctx* ctx, const void* pcm, int32_t format, int32_t ch
  * (argmax of the LogSoftmax output, utils/powerset.py:135-140); optional log-probabilities [num_chunks][589][7]. */
 int b200_seg_forward(b200_ctx* ctx, const float* wav, const int64_t* chunk_off, const int32_t* chunk_valid,
                      int32_t num_chunks, uint8_t* classes, float* logp, void* stream);
-/* PyanNet.forward on windows of any length (models/segmentation/PyanNet.py:223-240): window i covers
+/* PyanNet.forward of a log-softmax head on windows of any length (models/segmentation/PyanNet.py:223-240): window i covers
  * wav[chunk_off[i] .. chunk_off[i] + window), of which the first chunk_valid[i] <= window samples are real (zero padding
  * after them, inference.py:270-278).  Every InstanceNorm normalises over the whole padded window.  F = 1 + (window - 251)
  * / 10 frames, then MaxPool 3, Conv1d 5, MaxPool 3, Conv1d 5, MaxPool 3 (589 for 160000); window >= 1261 (F >= 2).
- * Output classes[num_chunks][F], optional logp[num_chunks][F][7].  Windows run in sub-batches of at most
- * seg_max_batch x 160000 samples; one window longer than that (5.87 h with the default) returns B200_STATUS_INVALID.
+ * Output classes[num_chunks][F] (argmax, ties to the first class), optional logp[num_chunks][F][K], K the loaded head's
+ * class count.  Windows run in sub-batches of at most seg_max_batch x 160000 samples; one window longer than that
+ * (5.87 h with the default) returns B200_STATUS_INVALID, and so does a loaded sigmoid head.
  * b200_seg_forward is this function with window = 160000. */
 int b200_seg_forward_window(b200_ctx* ctx, const float* wav, const int64_t* chunk_off, const int32_t* chunk_valid,
                             int32_t num_chunks, int32_t window, uint8_t* classes, float* logp, void* stream);
+/* The same for a sigmoid head (binary / multi-label problems): scores[num_chunks][F][K] fp32 in [0, 1] and / or
+ * max_scores[num_chunks][F], the maximum over the K scores of each frame (VoiceActivityDetection's
+ * pre_aggregation_hook, pipelines/voice_activity_detection.py:111-114, fused into the classifier); either may be NULL,
+ * not both.  A loaded log-softmax head returns B200_STATUS_INVALID. */
+int b200_seg_forward_scores(b200_ctx* ctx, const float* wav, const int64_t* chunk_off, const int32_t* chunk_valid,
+                            int32_t num_chunks, int32_t window, float* scores, float* max_scores, void* stream);
 /* SincNet.forward alone (models/blocks/sincnet.py:163-184): out[num_chunks][589][60] fp32 (frame-major). */
 int b200_sincnet_forward(b200_ctx* ctx, const float* wav, const int64_t* chunk_off, const int32_t* chunk_valid,
                          int32_t num_chunks, float* out, void* stream);
 /* Powerset.to_multilabel, hard (utils/powerset.py:115-140): classes[n] -> multilabel[n][3] in {0,1} (u8). */
 int b200_powerset_to_multilabel(b200_ctx* ctx, const uint8_t* classes, int64_t n, uint8_t* multilabel, void* stream);
+/* The same for any powerset: num_speakers <= 32 speakers with at most max_per_frame per frame, classes in the
+ * reference's order (set size 0 .. max_per_frame, itertools.combinations within each size); num_classes must be the
+ * powerset's class count (at most 32), else B200_STATUS_INVALID.  multilabel[n][num_speakers]; class ids
+ * >= num_classes give an all-zero row.  b200_powerset_to_multilabel is this function with (7, 3, 2). */
+int b200_powerset_to_multilabel_generic(b200_ctx* ctx, const uint8_t* classes, int64_t n, int32_t num_classes,
+                                        int32_t num_speakers, int32_t max_per_frame, uint8_t* multilabel,
+                                        void* stream);
 
 /* ---- embeddings: SpeakerDiarization.get_embeddings hot loop (pipelines/speaker_diarization.py:399-459) over
  * PyannoteAudioPretrainedSpeakerEmbedding.__call__ (pipelines/speaker_verification.py:704-716) and
@@ -276,6 +300,10 @@ int b200_aggregate_window(b200_ctx* ctx, const float* scores, const int32_t* sta
 /* VoiceActivityDetection's pre-aggregation step (pipelines/voice_activity_detection.py:111-114: max over the
  * speakers of the multilabel output) straight from the powerset classes: speech[n] fp32 in {0,1}. */
 int b200_powerset_speech(b200_ctx* ctx, const uint8_t* classes, int64_t n, float* speech, void* stream);
+/* The same for any powerset (arguments and checks as b200_powerset_to_multilabel_generic): speech[n] = 1 where the
+ * class is a non-empty speaker set.  b200_powerset_speech is this function with (7, 3, 2). */
+int b200_powerset_speech_generic(b200_ctx* ctx, const uint8_t* classes, int64_t n, int32_t num_classes,
+                                 int32_t num_speakers, int32_t max_per_frame, float* speech, void* stream);
 
 /* Onsets / offsets of a discrete diarization discrete[num_frames][num_clusters] u8 (to_annotation ->
  * Binarize(onset=offset=0.5), pipelines/utils/diarization.py:188-218, utils/signal.py:254-318) as unordered events

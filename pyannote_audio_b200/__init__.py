@@ -2,7 +2,7 @@
 
 Public surface mirrors the reference for this path only:
   Inference, Model classes (PyanNet, WeSpeakerResNet34 / 152 / 221 / 293, XVectorSincNet), SpeakerDiarization (+ DiarizeOutput), SpeakerEmbedding,
-  VoiceActivityDetection, VBxClustering,
+  VoiceActivityDetection, MultiLabelSegmentation, VBxClustering,
   AgglomerativeClustering, PLDA, Audio, and the pyannote.core value types they exchange.
 All compute goes through libb200diar.so (C ABI in include/b200diar.h); there is no CPU fallback.
 """
@@ -17,6 +17,7 @@ _LAZY = {
     "WeSpeakerResNet293": "models", "BaseWeSpeakerResNet": "models", "XVectorSincNet": "models", "SpeakerDiarization": "pipeline", "DiarizeOutput": "pipeline",
     "PretrainedSpeakerEmbedding": "pipeline", "VBxClustering": "clustering",
     "AgglomerativeClustering": "clustering", "PLDA": "clustering", "VoiceActivityDetection": "vad",
+    "MultiLabelSegmentation": "multilabel",
     "Binarize": "signal", "Pipeline": "loading", "SpeakerEmbedding": "speaker_verification",
 }
 

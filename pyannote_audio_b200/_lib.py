@@ -70,6 +70,7 @@ _PROTOS = {
     "b200_ctx_launch_count": (C.c_int64, [C.c_void_p]),
     "b200_ctx_timer": (C.c_int, [C.c_void_p, C.c_char_p, C.POINTER(C.c_double), C.POINTER(C.c_int64)]),
     "b200_seg_load": (C.c_int, [C.c_void_p, C.POINTER(SegWeights)]),
+    "b200_seg_load_head": (C.c_int, [C.c_void_p, C.POINTER(SegWeights), C.c_int32, C.c_int32]),
     "b200_emb_load": (C.c_int, [C.c_void_p, C.POINTER(EmbWeights)]),
     "b200_emb_load_bottleneck": (C.c_int, [C.c_void_p, C.POINTER(EmbBottleneckWeights)]),
     "b200_xvec_load": (C.c_int, [C.c_void_p, C.POINTER(XvecWeights)]),
@@ -79,9 +80,13 @@ _PROTOS = {
                                    C.c_void_p]),
     "b200_seg_forward_window": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_int32, C.c_int32,
                                           C.c_void_p, C.c_void_p, C.c_void_p]),
+    "b200_seg_forward_scores": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_int32, C.c_int32,
+                                          C.c_void_p, C.c_void_p, C.c_void_p]),
     "b200_sincnet_forward": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_int32, C.c_void_p,
                                        C.c_void_p]),
     "b200_powerset_to_multilabel": (C.c_int, [C.c_void_p, C.c_void_p, C.c_int64, C.c_void_p, C.c_void_p]),
+    "b200_powerset_to_multilabel_generic": (C.c_int, [C.c_void_p, C.c_void_p, C.c_int64, C.c_int32, C.c_int32,
+                                                      C.c_int32, C.c_void_p, C.c_void_p]),
     "b200_emb_forward": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_int32, C.c_void_p, C.c_void_p,
                                    C.c_void_p]),
     "b200_emb_forward_push": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_int32, C.c_void_p, C.c_void_p,
@@ -123,6 +128,8 @@ _PROTOS = {
                                         C.c_void_p, C.c_void_p, C.c_int32, C.c_float, C.c_float, C.c_void_p,
                                         C.c_void_p]),
     "b200_powerset_speech": (C.c_int, [C.c_void_p, C.c_void_p, C.c_int64, C.c_void_p, C.c_void_p]),
+    "b200_powerset_speech_generic": (C.c_int, [C.c_void_p, C.c_void_p, C.c_int64, C.c_int32, C.c_int32, C.c_int32,
+                                               C.c_void_p, C.c_void_p]),
     "b200_plda_transform": (C.c_int, [C.c_void_p, C.c_void_p, C.c_int32, C.c_int32, C.c_int32, C.c_int32, C.c_void_p,
                                       C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p]),
     "b200_weighted_centroids": (C.c_int, [C.c_void_p, C.c_void_p, C.c_int32, C.c_int32, C.c_void_p, C.c_int32,

@@ -479,8 +479,12 @@ int b200_audio_ingest(b200_ctx* ctx, const void* pcm, int32_t format, int32_t ch
 }
 
 // ------------------------------------------------------------------------------------------------------
-int b200_seg_load(b200_ctx* ctx, const b200_seg_weights* w) {
+int b200_seg_load_head(b200_ctx* ctx, const b200_seg_weights* w, int32_t num_classes, int32_t activation) {
   B200_CHECK(ctx && w, B200_ERR_INVALID, "NULL ctx/weights");
+  B200_CHECK(num_classes >= 1 && num_classes <= kSegMaxClasses, B200_ERR_INVALID,
+             "a classifier of %d classes is unsupported (1 .. %d)", (int)num_classes, kSegMaxClasses);
+  B200_CHECK(activation == B200_SEG_LOGSOFTMAX || activation == B200_SEG_SIGMOID, B200_ERR_INVALID,
+             "unknown classifier activation %d (B200_SEG_LOGSOFTMAX = 0, B200_SEG_SIGMOID = 1)", (int)activation);
   DeviceGuard g(ctx->device);
   SegWeights& S = ctx->seg;
   B200_CHECK(w->lstm_layers >= 1 && w->lstm_layers <= 4, B200_ERR_INVALID, "lstm_layers=%d unsupported",
@@ -488,6 +492,8 @@ int b200_seg_load(b200_ctx* ctx, const b200_seg_weights* w) {
   S.loaded = false;
   release_weights(ctx, &ctx->owned_seg);
   S.lstm_layers = w->lstm_layers;
+  S.num_classes = num_classes;
+  S.activation = activation == B200_SEG_SIGMOID ? kSegSigmoid : kSegLogSoftmax;
   int rc;
   if ((rc = load_sincnet(ctx, w->wav_norm_weight, w->wav_norm_bias, w->sinc_filters, w->norm_weight, w->norm_bias,
                          w->conv_weight, w->conv_bias, &S.sinc)))
@@ -561,11 +567,16 @@ int b200_seg_load(b200_ctx* ctx, const b200_seg_weights* w) {
     if ((rc = upload(ctx, lb, &S.lin_b[i]))) return rc;
   }
   B200_CHECK(w->classifier_weight && w->classifier_bias, B200_ERR_INVALID, "classifier missing");
-  std::vector<float> cw(w->classifier_weight, w->classifier_weight + 7 * 128), cb(w->classifier_bias, w->classifier_bias + 7);
+  std::vector<float> cw(w->classifier_weight, w->classifier_weight + (size_t)num_classes * 128),
+      cb(w->classifier_bias, w->classifier_bias + num_classes);
   if ((rc = upload(ctx, cw, &S.cls_w))) return rc;
   if ((rc = upload(ctx, cb, &S.cls_b))) return rc;
   S.loaded = true;
   return B200_OK;
+}
+
+int b200_seg_load(b200_ctx* ctx, const b200_seg_weights* w) {
+  return b200_seg_load_head(ctx, w, kClasses, B200_SEG_LOGSOFTMAX);
 }
 
 int b200_emb_load(b200_ctx* ctx, const b200_emb_weights* w) {
@@ -699,7 +710,7 @@ int b200_emb_load_bottleneck(b200_ctx* ctx, const b200_emb_bottleneck_weights* w
 // PyanNet on n windows of `window` samples.  A sub-batch holds at most seg_max_batch x 160000 window samples (the
 // workspace of seg_max_batch 10 s chunks) and at most 65535 windows (the y extent of the SincNet grids).
 static int seg_run(b200_ctx* ctx, const float* wav, const int64_t* chunk_off, const int32_t* chunk_valid, int n,
-                   int window, uint8_t* classes, float* logp, float* sinc_out, cudaStream_t st) {
+                   int window, const SegHeadOut& out, float* sinc_out, cudaStream_t st) {
   B200_CHECK(ctx && ctx->seg.loaded, B200_ERR_STATE, "segmentation weights not loaded");
   B200_CHECK(wav && chunk_off && chunk_valid && n >= 0, B200_ERR_INVALID, "bad arguments");
   B200_CHECK(window >= kSegMinWindow, B200_ERR_INVALID,
@@ -733,9 +744,14 @@ static int seg_run(b200_ctx* ctx, const float* wav, const int64_t* chunk_off, co
       return rc;
     ctx->launches += sincnet_launches(geom);
     if (sinc_out) continue;
-    if ((rc = lstm_head_forward(ctx->seg, x0, nb, T, region, classes + (size_t)c0 * T,
-                                logp ? logp + (size_t)c0 * T * kClasses : nullptr, ctx->num_sms,
-                                ctx->seg_gemm_impl, ctx->seg_rec_impl, st)))
+    const size_t row0 = (size_t)c0 * T, K = ctx->seg.num_classes;
+    SegHeadOut sub;
+    sub.cls = out.cls ? out.cls + row0 : nullptr;
+    sub.logp = out.logp ? out.logp + row0 * K : nullptr;
+    sub.scores = out.scores ? out.scores + row0 * K : nullptr;
+    sub.max_scores = out.max_scores ? out.max_scores + row0 : nullptr;
+    if ((rc = lstm_head_forward(ctx->seg, x0, nb, T, region, sub, ctx->num_sms, ctx->seg_gemm_impl, ctx->seg_rec_impl,
+                                st)))
       return rc;
     ctx->launches += 2 * ctx->seg.lstm_layers + 3;
   }
@@ -744,9 +760,26 @@ static int seg_run(b200_ctx* ctx, const float* wav, const int64_t* chunk_off, co
 
 int b200_seg_forward_window(b200_ctx* ctx, const float* wav, const int64_t* chunk_off, const int32_t* chunk_valid,
                             int32_t num_chunks, int32_t window, uint8_t* classes, float* logp, void* stream) {
+  B200_CHECK(!(ctx && ctx->seg.loaded && ctx->seg.activation != kSegLogSoftmax), B200_ERR_INVALID,
+             "the loaded segmentation head is a sigmoid (multi-label / binary) head: call b200_seg_forward_scores");
   if (num_chunks == 0) return B200_OK;
   B200_CHECK(classes != nullptr, B200_ERR_INVALID, "classes is NULL");
-  return seg_run(ctx, wav, chunk_off, chunk_valid, num_chunks, window, classes, logp, nullptr, (cudaStream_t)stream);
+  SegHeadOut out;
+  out.cls = classes;
+  out.logp = logp;
+  return seg_run(ctx, wav, chunk_off, chunk_valid, num_chunks, window, out, nullptr, (cudaStream_t)stream);
+}
+
+int b200_seg_forward_scores(b200_ctx* ctx, const float* wav, const int64_t* chunk_off, const int32_t* chunk_valid,
+                            int32_t num_chunks, int32_t window, float* scores, float* max_scores, void* stream) {
+  B200_CHECK(!(ctx && ctx->seg.loaded && ctx->seg.activation != kSegSigmoid), B200_ERR_INVALID,
+             "the loaded segmentation head is a log-softmax (powerset / mono-label) head: call b200_seg_forward_window");
+  if (num_chunks == 0) return B200_OK;
+  B200_CHECK(scores || max_scores, B200_ERR_INVALID, "scores and max_scores are both NULL");
+  SegHeadOut out;
+  out.scores = scores;
+  out.max_scores = max_scores;
+  return seg_run(ctx, wav, chunk_off, chunk_valid, num_chunks, window, out, nullptr, (cudaStream_t)stream);
 }
 
 int b200_seg_forward(b200_ctx* ctx, const float* wav, const int64_t* chunk_off, const int32_t* chunk_valid,
@@ -769,7 +802,7 @@ int b200_sincnet_forward(b200_ctx* ctx, const float* wav, const int64_t* chunk_o
   float* tmp = nullptr;
   const size_t rows = (size_t)num_chunks * kFrames;
   B200_CUDA_OK(cudaMalloc((void**)&tmp, rows * 64 * sizeof(float)));
-  int rc = seg_run(ctx, wav, chunk_off, chunk_valid, num_chunks, kChunk, nullptr, nullptr, tmp, st);
+  int rc = seg_run(ctx, wav, chunk_off, chunk_valid, num_chunks, kChunk, SegHeadOut(), tmp, st);
   if (rc == B200_OK) {
     strip_pad_kernel<<<(unsigned)((rows * 60 + 255) / 256), 256, 0, st>>>(tmp, out, rows);
     ctx->launches += 1;
@@ -779,12 +812,30 @@ int b200_sincnet_forward(b200_ctx* ctx, const float* wav, const int64_t* chunk_o
   return rc;
 }
 
-int b200_powerset_to_multilabel(b200_ctx* ctx, const uint8_t* classes, int64_t n, uint8_t* multilabel, void* stream) {
+// the map of num_speakers / max_per_frame, checked against the caller's class count
+static int powerset_map_for(int32_t num_classes, int32_t num_speakers, int32_t max_per_frame, PowersetMap* map) {
+  if (!powerset_map(num_speakers, max_per_frame, map)) return B200_ERR_INVALID;
+  B200_CHECK(map->K == num_classes, B200_ERR_INVALID,
+             "a powerset of %d speakers with at most %d per frame has %d classes, not %d", (int)num_speakers,
+             (int)max_per_frame, map->K, (int)num_classes);
+  return B200_OK;
+}
+
+int b200_powerset_to_multilabel_generic(b200_ctx* ctx, const uint8_t* classes, int64_t n, int32_t num_classes,
+                                        int32_t num_speakers, int32_t max_per_frame, uint8_t* multilabel,
+                                        void* stream) {
   B200_CHECK(ctx && classes && multilabel && n >= 0, B200_ERR_INVALID, "bad arguments");
+  PowersetMap map;
+  int rc;
+  if ((rc = powerset_map_for(num_classes, num_speakers, max_per_frame, &map))) return rc;
   if (n == 0) return B200_OK;
   DeviceGuard g(ctx->device);
   ctx->launches += 1;
-  return powerset_to_multilabel(classes, n, multilabel, (cudaStream_t)stream);
+  return powerset_to_multilabel(classes, n, map, multilabel, (cudaStream_t)stream);
+}
+
+int b200_powerset_to_multilabel(b200_ctx* ctx, const uint8_t* classes, int64_t n, uint8_t* multilabel, void* stream) {
+  return b200_powerset_to_multilabel_generic(ctx, classes, n, kClasses, kSpeakers, 2, multilabel, stream);
 }
 
 // ------------------------------------------------------------------------------------------------------
@@ -1359,12 +1410,20 @@ int b200_aggregate(b200_ctx* ctx, const float* scores, const int32_t* start_fram
                                warm_up, skip_average, missing, epsilon, out, stream);
 }
 
-int b200_powerset_speech(b200_ctx* ctx, const uint8_t* classes, int64_t n, float* speech, void* stream) {
+int b200_powerset_speech_generic(b200_ctx* ctx, const uint8_t* classes, int64_t n, int32_t num_classes,
+                                 int32_t num_speakers, int32_t max_per_frame, float* speech, void* stream) {
   B200_CHECK(ctx && classes && speech && n >= 0, B200_ERR_INVALID, "bad arguments");
+  PowersetMap map;
+  int rc;
+  if ((rc = powerset_map_for(num_classes, num_speakers, max_per_frame, &map))) return rc;
   if (n == 0) return B200_OK;
   DeviceGuard g(ctx->device);
   ctx->launches += 1;
-  return powerset_speech(classes, n, speech, (cudaStream_t)stream);
+  return powerset_speech(classes, n, map, speech, (cudaStream_t)stream);
+}
+
+int b200_powerset_speech(b200_ctx* ctx, const uint8_t* classes, int64_t n, float* speech, void* stream) {
+  return b200_powerset_speech_generic(ctx, classes, n, kClasses, kSpeakers, 2, speech, stream);
 }
 
 int b200_frame_transitions(b200_ctx* ctx, const uint8_t* discrete, int32_t num_frames, int32_t num_clusters,

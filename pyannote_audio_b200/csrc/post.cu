@@ -14,20 +14,45 @@
 
 namespace b200 {
 
-__constant__ unsigned char kPowersetMap[7][3] = {{0, 0, 0}, {1, 0, 0}, {0, 1, 0}, {0, 0, 1},
-                                                 {1, 1, 0}, {1, 0, 1}, {0, 1, 1}};
-
-__global__ void powerset_kernel(const unsigned char* __restrict__ cls, long long n, unsigned char* __restrict__ ml) {
-  const long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x;
-  if (i >= n) return;
-  const int c = cls[i] < 7 ? cls[i] : 0;
-  ml[i * 3 + 0] = kPowersetMap[c][0];
-  ml[i * 3 + 1] = kPowersetMap[c][1];
-  ml[i * 3 + 2] = kPowersetMap[c][2];
+static void powerset_sets(int N, int size, int first, unsigned set, PowersetMap* map) {
+  if (size == 0) { map->mask[map->K++] = set; return; }
+  for (int j = first; j <= N - size; ++j) powerset_sets(N, size - 1, j + 1, set | (1u << j), map);
 }
 
-int powerset_to_multilabel(const unsigned char* cls, long long n, unsigned char* ml, cudaStream_t stream) {
-  powerset_kernel<<<(unsigned)((n + 255) / 256), 256, 0, stream>>>(cls, n, ml);
+bool powerset_map(int N, int M, PowersetMap* map) {
+  if (N < 1 || N > 32 || M < 1 || M > N) {
+    set_error("powerset of %d speakers with at most %d per frame: need 1 <= max_per_frame <= speakers <= 32", N, M);
+    return false;
+  }
+  unsigned long long classes = 0, binom = 1;                 // sum of C(N, k) for k = 0 .. M
+  for (int k = 0; k <= M; ++k) {
+    classes += binom;
+    binom = binom * (N - k) / (k + 1);
+  }
+  if (classes > (unsigned long long)kPowersetMaxClasses) {
+    set_error("powerset of %d speakers with at most %d per frame has %llu classes; at most %d are supported", N, M,
+              classes, kPowersetMaxClasses);
+    return false;
+  }
+  *map = PowersetMap();
+  map->N = N;
+  for (int size = 0; size <= M; ++size) powerset_sets(N, size, 0, 0u, map);
+  return true;
+}
+
+// Powerset.to_multilabel, hard (utils/powerset.py:115-140), for N speakers and at most M per frame: class c is the
+// speaker set mask[c] (bit j = speaker j).  Class ids >= K map to the empty set, as the 7-class kernel always did.
+__global__ void powerset_kernel(const unsigned char* __restrict__ cls, long long n, PowersetMap map,
+                                unsigned char* __restrict__ ml) {
+  const long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x;
+  if (i >= n) return;
+  const unsigned m = cls[i] < map.K ? map.mask[cls[i]] : 0u;
+  for (int j = 0; j < map.N; ++j) ml[i * map.N + j] = (m >> j) & 1u;
+}
+
+int powerset_to_multilabel(const unsigned char* cls, long long n, const PowersetMap& map, unsigned char* ml,
+                           cudaStream_t stream) {
+  powerset_kernel<<<(unsigned)((n + 255) / 256), 256, 0, stream>>>(cls, n, map, ml);
   B200_CUDA_OK(cudaGetLastError());
   return B200_OK;
 }
@@ -103,16 +128,17 @@ int aggregate_scores(const float* scores, const int* sf, int C, int F, int nf, i
   return B200_OK;
 }
 
-// speech score of a powerset frame = max over the speakers of its multilabel row = (class != 0); this is what
-// VoiceActivityDetection's pre_aggregation_hook (np.max(scores, axis=-1, keepdims=True),
-// pipelines/voice_activity_detection.py:111-114) makes of the (C,589,3) multilabel output
-__global__ void powerset_speech_kernel(const unsigned char* __restrict__ cls, long long n, float* __restrict__ out) {
+// speech score of a powerset frame = max over the speakers of its multilabel row = (its speaker set is not empty);
+// this is what VoiceActivityDetection's pre_aggregation_hook (np.max(scores, axis=-1, keepdims=True),
+// pipelines/voice_activity_detection.py:111-114) makes of the multilabel output
+__global__ void powerset_speech_kernel(const unsigned char* __restrict__ cls, long long n, PowersetMap map,
+                                       float* __restrict__ out) {
   const long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x;
-  if (i < n) out[i] = (cls[i] != 0 && cls[i] < 7) ? 1.f : 0.f;
+  if (i < n) out[i] = (cls[i] < map.K && map.mask[cls[i]] != 0u) ? 1.f : 0.f;
 }
 
-int powerset_speech(const unsigned char* cls, long long n, float* out, cudaStream_t stream) {
-  powerset_speech_kernel<<<(unsigned)((n + 255) / 256), 256, 0, stream>>>(cls, n, out);
+int powerset_speech(const unsigned char* cls, long long n, const PowersetMap& map, float* out, cudaStream_t stream) {
+  powerset_speech_kernel<<<(unsigned)((n + 255) / 256), 256, 0, stream>>>(cls, n, map, out);
   B200_CUDA_OK(cudaGetLastError());
   return B200_OK;
 }

@@ -1,4 +1,4 @@
-// Segmentation path (PyanNet: SincNet front-end -> 4x BiLSTM -> Linear x2 -> classifier -> powerset argmax).
+// Segmentation path (PyanNet: SincNet front-end -> 4x BiLSTM -> Linear x2 -> classifier -> powerset argmax or sigmoid).
 #pragma once
 #include "common.cuh"
 
@@ -41,9 +41,17 @@ struct SincNetWeights {
   __half* conv_wg_lo[2] = {nullptr, nullptr};
 };
 
+// classifier heads (models/segmentation/PyanNet.py:152-161, core/model.py:271-300): Linear(128, K) then log-softmax
+// (mono-label / powerset problems) or sigmoid (binary / multi-label problems)
+constexpr int kSegLogSoftmax = 0;
+constexpr int kSegSigmoid = 1;
+constexpr int kSegMaxClasses = 32;
+
 struct SegWeights {
   bool loaded = false;
   int lstm_layers = 4;
+  int num_classes = kClasses;       // K, 1 .. kSegMaxClasses
+  int activation = kSegLogSoftmax;
   SincNetWeights sinc;
   // LSTM, per layer: W_ih for both directions [1024][Kpad] with row = dir*512 + unit*4 + gate; bias = b_ih+b_hh
   float* w_ih[8] = {};
@@ -59,8 +67,8 @@ struct SegWeights {
   __half* lin_w_lo[2] = {nullptr, nullptr};
   float* lin_w[2] = {nullptr, nullptr};   // [128][256], [128][128]
   float* lin_b[2] = {nullptr, nullptr};
-  float* cls_w = nullptr;           // [7][128]
-  float* cls_b = nullptr;           // [7]
+  float* cls_w = nullptr;           // [K][128]
+  float* cls_b = nullptr;           // [K]
 };
 
 int sgemm_nt(const float* A, int lda, const float* Bw, int ldb, float* C, int ldc, const float* bias, int M, int N,
@@ -98,9 +106,17 @@ int sincnet_launches(const SegGeom& g);   // kernels sincnet_forward launches pe
 int sincnet_forward(const SincNetWeights& W, const SegGeom& g, const float* wav, const long long* chunk_off,
                     const int* chunk_valid, int NB, void* ws, float* x0, int conv_impl, cudaStream_t stream);
 
-// BiLSTM stack + linear head on sequences of T frames: X0 -> class ids [NB][T] u8 (+ optional log-probs [NB][T][7])
+// Outputs of the classifier, written straight to the caller's buffers.  Log-softmax heads: cls [NB][T] u8 (+ optional
+// logp [NB][T][K]); sigmoid heads: scores [NB][T][K] and / or max_scores [NB][T] (either may be null).
+struct SegHeadOut {
+  unsigned char* cls = nullptr;
+  float* logp = nullptr;
+  float* scores = nullptr;
+  float* max_scores = nullptr;
+};
+// BiLSTM stack + linear layers + classifier on sequences of T frames
 size_t lstm_workspace_bytes(int NB, int T);
-int lstm_head_forward(const SegWeights& W, const float* x0, int NB, int T, void* ws, unsigned char* cls, float* logp,
+int lstm_head_forward(const SegWeights& W, const float* x0, int NB, int T, void* ws, const SegHeadOut& out,
                       int num_sms, int gemm_impl, int rec_impl, cudaStream_t stream);
 
 }  // namespace b200

@@ -1,4 +1,4 @@
-// BiLSTM stack + linear head + powerset argmax for PyanNet (fp32 SIMT).
+// BiLSTM stack + linear head + classifier (powerset log-softmax / argmax, or sigmoid) for PyanNet (fp32 SIMT).
 //
 // Reference: /root/reference/src/pyannote/audio/models/segmentation/PyanNet.py:223-240
 //   nn.LSTM(60, 128, num_layers=4, bidirectional, batch_first) -> 2x leaky_relu(Linear) -> Linear(128,7)
@@ -12,6 +12,8 @@
 #include "common.cuh"
 #include "seg.cuh"
 #include <cooperative_groups.h>
+#include <array>
+#include <utility>
 
 namespace cg = cooperative_groups;
 
@@ -137,23 +139,28 @@ lstm_rec_kernel(const float* __restrict__ Gx /*[NB][T][1024]*/, const float* __r
   }
 }
 
-// ---- classifier 128 -> 7, log-softmax, argmax (one warp per frame) ---------------------------------------
+// ---- classifier 128 -> K (one warp per frame) -------------------------------------------------------------
+// kSegLogSoftmax: log-softmax + argmax -> cls [M] u8 (+ logp [M][K]); kSegSigmoid: sigmoid -> scores [M][K] and/or
+// the per-frame maximum over the K scores [M] (VoiceActivityDetection's pre_aggregation_hook, np.max(axis=-1)).
+// K is a template parameter so that the logits stay in registers; K = 7 with log-softmax is the community-1 head.
+template <int K, int ACT>
 __global__ void __launch_bounds__(256) classifier_kernel(const float* __restrict__ Z /*[M][128]*/,
-                                                         const float* __restrict__ Wc /*[7][128]*/,
+                                                         const float* __restrict__ Wc /*[K][128]*/,
                                                          const float* __restrict__ bc, unsigned char* __restrict__ cls,
-                                                         float* __restrict__ logp, int M) {
-  __shared__ float sw[kClasses * 128];
-  __shared__ float sb[8];
-  for (int i = threadIdx.x; i < kClasses * 128; i += blockDim.x) sw[i] = Wc[i];
-  if (threadIdx.x < kClasses) sb[threadIdx.x] = bc[threadIdx.x];
+                                                         float* __restrict__ logp, float* __restrict__ scores,
+                                                         float* __restrict__ max_scores, int M) {
+  __shared__ float sw[K * 128];
+  __shared__ float sb[K < 8 ? 8 : K];
+  for (int i = threadIdx.x; i < K * 128; i += blockDim.x) sw[i] = Wc[i];
+  if (threadIdx.x < K) sb[threadIdx.x] = bc[threadIdx.x];
   __syncthreads();
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
   const int row = blockIdx.x * 8 + warp;
   if (row >= M) return;
   const float4 z = *reinterpret_cast<const float4*>(Z + (size_t)row * 128 + lane * 4);
-  float v[kClasses];
+  float v[K];
 #pragma unroll
-  for (int k = 0; k < kClasses; ++k) {
+  for (int k = 0; k < K; ++k) {
     const float4 w = *reinterpret_cast<const float4*>(sw + k * 128 + lane * 4);
     float s = z.x * w.x;
     s = fmaf(z.y, w.y, s);
@@ -163,25 +170,43 @@ __global__ void __launch_bounds__(256) classifier_kernel(const float* __restrict
     for (int o = 16; o > 0; o >>= 1) s += __shfl_xor_sync(0xffffffffu, s, o);
     v[k] = s + sb[k];
   }
-  if (lane == 0) {
-    float mx = v[0];
+  if (lane != 0) return;
+  if (ACT == kSegSigmoid) {
+    float mx = 0.f;
 #pragma unroll
-    for (int k = 1; k < kClasses; ++k) mx = fmaxf(mx, v[k]);
-    float se = 0.f;
-#pragma unroll
-    for (int k = 0; k < kClasses; ++k) se += expf(v[k] - mx);
-    const float lse = logf(se);
-    int best = 0;
-    float bv = 0.f;
-#pragma unroll
-    for (int k = 0; k < kClasses; ++k) {
-      const float lp = (v[k] - mx) - lse;
-      if (logp) logp[(size_t)row * kClasses + k] = lp;
-      if (k == 0 || lp > bv) { bv = lp; best = k; }     // first maximum wins, like torch.argmax
+    for (int k = 0; k < K; ++k) {
+      const float p = sigmoidf_(v[k]);
+      if (scores) scores[(size_t)row * K + k] = p;
+      mx = k == 0 ? p : fmaxf(mx, p);
     }
-    cls[row] = (unsigned char)best;
+    if (max_scores) max_scores[row] = mx;
+    return;
   }
+  float mx = v[0];
+#pragma unroll
+  for (int k = 1; k < K; ++k) mx = fmaxf(mx, v[k]);
+  float se = 0.f;
+#pragma unroll
+  for (int k = 0; k < K; ++k) se += expf(v[k] - mx);
+  const float lse = logf(se);
+  int best = 0;
+  float bv = 0.f;
+#pragma unroll
+  for (int k = 0; k < K; ++k) {
+    const float lp = (v[k] - mx) - lse;
+    if (logp) logp[(size_t)row * K + k] = lp;
+    if (k == 0 || lp > bv) { bv = lp; best = k; }     // first maximum wins, like torch.argmax
+  }
+  cls[row] = (unsigned char)best;
 }
+
+typedef void (*ClassifierFn)(const float*, const float*, const float*, unsigned char*, float*, float*, float*, int);
+template <int ACT, int... I>
+static std::array<ClassifierFn, sizeof...(I)> classifier_table(std::integer_sequence<int, I...>) {
+  return {{&classifier_kernel<I + 1, ACT>...}};
+}
+static const auto kLogSoftmaxHeads = classifier_table<kSegLogSoftmax>(std::make_integer_sequence<int, kSegMaxClasses>());
+static const auto kSigmoidHeads = classifier_table<kSegSigmoid>(std::make_integer_sequence<int, kSegMaxClasses>());
 
 // ---- host ------------------------------------------------------------------------------------------
 struct LstmWs {
@@ -228,7 +253,7 @@ static int launch_rec(const float* Gx, const float* Whh, float* Y, __half* Yh, _
   return B200_OK;
 }
 
-int lstm_head_forward(const SegWeights& W, const float* x0, int NB, int T, void* ws, unsigned char* cls, float* logp,
+int lstm_head_forward(const SegWeights& W, const float* x0, int NB, int T, void* ws, const SegHeadOut& out,
                       int num_sms, int gemm_impl, int rec_impl, cudaStream_t stream) {
   LstmWs w;
   carve_lstm(NB, T, ws, &w);
@@ -277,7 +302,8 @@ int lstm_head_forward(const SegWeights& W, const float* x0, int NB, int T, void*
     rc = sgemm_nt(w.Z1, 128, W.lin_w[1], 128, w.Z2, 128, W.lin_b[1], M, 128, 128, 1, stream);
     if (rc) return rc;
   }
-  classifier_kernel<<<ceil_div(M, 8), 256, 0, stream>>>(w.Z2, W.cls_w, W.cls_b, cls, logp, M);
+  const ClassifierFn head = (W.activation == kSegSigmoid ? kSigmoidHeads : kLogSoftmaxHeads)[W.num_classes - 1];
+  head<<<ceil_div(M, 8), 256, 0, stream>>>(w.Z2, W.cls_w, W.cls_b, out.cls, out.logp, out.scores, out.max_scores, M);
   B200_CUDA_OK(cudaGetLastError());
   return B200_OK;
 }

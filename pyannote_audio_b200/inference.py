@@ -2,8 +2,8 @@
 
 Same constructor, attributes, exceptions and static helpers (``aggregate`` / ``trim``) as the reference's
 ``Inference``; what changes is underneath ``slide``: the waveform is copied to the device ONCE, all chunks are
-addressed in place (no unfold copy, no per-batch H2D/D2H), PyanNet + powerset argmax run in libb200diar.so, and the
-result comes back in one D2H copy per file.
+addressed in place (no unfold copy, no per-batch H2D/D2H), PyanNet + its head (powerset argmax, or sigmoid scores)
+run in libb200diar.so, and the result comes back in one D2H copy per file.
 """
 from __future__ import annotations
 
@@ -34,6 +34,10 @@ def chunk_layout(num_samples: int, window_size: int, step_size: int):
     off = np.arange(total, dtype=np.int64) * step_size
     valid = np.minimum(window_size, num_samples - off).astype(np.int32)
     return off, valid, num_chunks, has_last_chunk
+
+
+def _host(x):
+    return x.cpu().numpy() if isinstance(x, torch.Tensor) else x
 
 
 class Inference(BaseInference):
@@ -87,7 +91,8 @@ class Inference(BaseInference):
 
     # ---- forward ------------------------------------------------------------------------------------
     def infer(self, chunks: torch.Tensor) -> np.ndarray:
-        """(batch, channel, sample) chunks -> (batch, frames, 3) multilabel {0,1} (or (batch, frames, 7) log-probs)."""
+        """(batch, channel, sample) chunks -> (batch, frames, speakers) multilabel {0,1} of a powerset model, else the
+        model's output: (batch, frames, K) log-probabilities or sigmoid scores."""
         try:
             logp = self.model(chunks)
         except MemoryError:
@@ -95,14 +100,19 @@ class Inference(BaseInference):
                               f"Try with a smaller value until memory error disappears.")
         if self.conversion == "identity":
             return logp.cpu().numpy()
-        ctx = self.model._ctx()
         cls = torch.argmax(logp, dim=-1).to(torch.uint8).contiguous()
-        return ctx.powerset_to_multilabel(cls).cpu().numpy().astype(np.float32)
+        return self._to_multilabel(cls).cpu().numpy().astype(np.float32)
 
-    def slide_device(self, waveform: torch.Tensor, sample_rate: int, return_logp: bool = False):
-        """Device-resident result of the sliding window: (classes (C,F) u8 tensor, wav_dev, off, valid), F frames
-        per window of ``duration``; with ``return_logp`` the first entry is the pair (classes, log-probabilities
-        (C,F,7) f32)."""
+    def _to_multilabel(self, cls: torch.Tensor) -> torch.Tensor:
+        specs = self.model.specifications
+        return self.model._ctx().powerset_to_multilabel(cls, len(specs.classes), specs.powerset_max_classes)
+
+    def slide_device(self, waveform: torch.Tensor, sample_rate: int, return_logp: bool = False,
+                     reduce_max: bool = False):
+        """Device-resident result of the sliding window: (output, wav_dev, off, valid), F frames per window of
+        ``duration``.  The output of a log-softmax head is classes (C,F) u8, or with ``return_logp`` the pair
+        (classes, log-probabilities (C,F,K) f32); that of a sigmoid head is its scores (C,F,K) f32, or with
+        ``reduce_max`` their per-frame maximum (C,F,1)."""
         window_size = self.model.audio.get_num_samples(self.duration)
         step_size = round(self.step * sample_rate)
         ops.check_seg_window(window_size)
@@ -117,7 +127,8 @@ class Inference(BaseInference):
             src = src.contiguous()
         wav_dev[:num_samples].copy_(src, non_blocking=True)
         try:
-            cls = self.model.forward_chunks(wav_dev, off, valid, return_logp=return_logp, window=window_size)
+            cls = self.model.forward_chunks(wav_dev, off, valid, return_logp=return_logp, window=window_size,
+                                            reduce_max=reduce_max)
         except MemoryError:
             raise MemoryError(f"batch_size ({self.batch_size: d}) is probably too large. "
                               f"Try with a smaller value until memory error disappears.")
@@ -126,26 +137,29 @@ class Inference(BaseInference):
     def slide(self, waveform: torch.Tensor, sample_rate: int, hook: Optional[Callable] = None):
         if self.model.specifications.resolution == Resolution.CHUNK:      # embedding models
             return self._slide_embedding(waveform, sample_rate, hook=hook)
-        cls, _, off, _ = self.slide_device(waveform, sample_rate, return_logp=self.conversion != "powerset")
+        specs = self.model.specifications
+        sigmoid = ops.seg_activation(specs) == ops.SEG_SIGMOID
+        out, _, off, _ = self.slide_device(waveform, sample_rate,
+                                           return_logp=not sigmoid and self.conversion != "powerset")
         total = len(off)
         if hook is not None:
             hook(completed=0, total=total)
-        ctx = self.model._ctx()
         if self.conversion == "powerset":
-            outputs = ctx.powerset_to_multilabel(cls).cpu().numpy().astype(np.float32)
-        else:                                   # skip_conversion=True: raw powerset log-probabilities (:130-141)
-            outputs = cls[1].cpu().numpy()
+            outputs = self._to_multilabel(out).cpu().numpy().astype(np.float32)
+        elif sigmoid:                           # multi-label / binary scores: aggregated on the device as they are
+            outputs = out
+        else:                                   # skip_conversion=True: raw log-probabilities (:130-141)
+            outputs = out[1].cpu().numpy()
         if hook is not None:
             hook(completed=total, total=total)
         frames = self.model.receptive_field
         chunks_sw = SlidingWindow(start=0.0, duration=self.duration, step=self.step)
-        specs = self.model.specifications
         if self.skip_aggregation or specs.resolution == Resolution.CHUNK or \
                 (specs.permutation_invariant and self.pre_aggregation_hook is None):
-            return SlidingWindowFeature(outputs, chunks_sw)
+            return SlidingWindowFeature(_host(outputs), chunks_sw)
         if self.pre_aggregation_hook is not None:
-            outputs = self.pre_aggregation_hook(outputs)
-        aggregated = self.aggregate_device(SlidingWindowFeature(np.asarray(outputs), chunks_sw), frames,
+            outputs = np.asarray(self.pre_aggregation_hook(_host(outputs)))
+        aggregated = self.aggregate_device(SlidingWindowFeature(outputs, chunks_sw), frames,
                                            warm_up=self.warm_up, hamming=True, missing=0.0)
         _, num_samples = waveform.shape
         _, _, _, has_last = chunk_layout(num_samples, self.model.audio.get_num_samples(self.duration),

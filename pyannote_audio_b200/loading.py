@@ -100,8 +100,12 @@ def _pipeline_class(name: str):
         from .speaker_verification import SpeakerEmbedding
 
         return SpeakerEmbedding
+    if short == "MultiLabelSegmentation":
+        from .multilabel import MultiLabelSegmentation
+
+        return MultiLabelSegmentation
     raise NotImplementedError(f"pipeline '{name}' has no CUDA implementation here (SpeakerDiarization, "
-                              f"VoiceActivityDetection and SpeakerEmbedding are available)")
+                              f"VoiceActivityDetection, SpeakerEmbedding and MultiLabelSegmentation are available)")
 
 
 def resolve_pipeline(checkpoint, revision: Optional[str] = None, subfolder: Optional[str] = None, token=None,

@@ -234,7 +234,9 @@ class _SincNetParams(nn.Module):
 
 
 class PyanNet(Model):
-    """SincNet > LSTM > Feed forward > Classifier, community-1 shape (4 BiLSTM layers of 128, 2x128 linear)."""
+    """SincNet > LSTM > Feed forward > Classifier, community-1 trunk (1-4 BiLSTM layers of 128, 2x128 linear) with
+    any head of 1 to 32 classes: log-softmax for powerset / mono-label problems, sigmoid for binary and multi-label
+    problems (core/model.py:271-300)."""
 
     _SLOT = "seg"
     _HPARAMS = ("sincnet", "lstm", "linear", "sample_rate", "num_channels")
@@ -262,17 +264,37 @@ class PyanNet(Model):
         self.lstm = nn.LSTM(60, hidden_size=128, num_layers=lstm_hp["num_layers"], bidirectional=True,
                             batch_first=True)
         self.linear = nn.ModuleList([nn.Linear(256, 128), nn.Linear(128, 128)])
-        self.classifier = nn.Linear(128, 7)
         self.specifications = Specifications(problem=Problem.MONO_LABEL_CLASSIFICATION, resolution=Resolution.FRAME,
                                              duration=duration, warm_up=(0.0, 0.0),
                                              classes=["speaker#1", "speaker#2", "speaker#3"], powerset_max_classes=2,
                                              permutation_invariant=True)
+
+    @property
+    def specifications(self) -> Specifications:
+        return self._specifications
+
+    @specifications.setter
+    def specifications(self, specifications: Specifications):
+        """As the reference's Model.specifications setter followed by PyanNet.build (core/model.py:131-146,
+        PyanNet.py:152-161): the classifier becomes a fresh Linear(128, dimension).  Heads without a kernel (more than
+        32 classes, or a problem that is not a classification) are refused here, before any device work."""
+        if isinstance(specifications, (tuple, list)):
+            raise ValueError("PyanNet does not support multi-tasking.")
+        if not isinstance(specifications, Specifications):
+            raise ValueError("Only regular specifications or tuple of specifications are supported.")
+        ops.seg_activation(specifications)
+        dimension = specifications.num_powerset_classes if specifications.powerset else len(specifications.classes)
+        ops.check_seg_classes(dimension)
+        self._specifications = specifications
+        self.classifier = nn.Linear(128, dimension).to(self._dummy.device)
         for p in self.parameters():
             p.requires_grad_(False)
+        self._bump_weights()
 
     @property
     def dimension(self) -> int:
-        return self.specifications.num_powerset_classes
+        specs = self.specifications
+        return specs.num_powerset_classes if specs.powerset else len(specs.classes)
 
     def num_frames(self, num_samples: int) -> int:
         n = num_samples
@@ -293,17 +315,21 @@ class PyanNet(Model):
         return c
 
     def _upload(self, ctx):
-        ctx.load_segmentation(self.state_dict())
+        ctx.load_segmentation(self.state_dict(), self.specifications)
 
     def forward_chunks(self, wav: torch.Tensor, chunk_off, chunk_valid, return_logp: bool = False, out=None,
-                       window: int = ops.CHUNK):
+                       window: int = ops.CHUNK, reduce_max: bool = False):
         """Hot-path entry: windows of ``window`` samples addressed inside one resident device waveform (no unfold
-        copy) -> classes (chunks, num_frames(window)) uint8."""
+        copy) -> classes (chunks, num_frames(window)) uint8 for a log-softmax head, sigmoid scores
+        (chunks, num_frames(window), dimension) float32 (or their per-frame maximum with ``reduce_max``) for a
+        sigmoid head (ops.Context.seg_forward)."""
         ops.check_seg_window(window)
-        return self._ctx().seg_forward(wav, chunk_off, chunk_valid, return_logp=return_logp, out=out, window=window)
+        return self._ctx().seg_forward(wav, chunk_off, chunk_valid, return_logp=return_logp, out=out, window=window,
+                                       reduce_max=reduce_max)
 
     def forward(self, waveforms: torch.Tensor) -> torch.Tensor:
-        """waveforms (batch, channel, samples), samples >= 1261 -> log-probabilities (batch, num_frames(samples), 7)."""
+        """waveforms (batch, channel, samples), samples >= 1261 -> (batch, num_frames(samples), dimension):
+        log-probabilities of a log-softmax head, sigmoid scores of a sigmoid head."""
         b, c, s = waveforms.shape
         if c != 1:
             raise ValueError(f"PyanNet kernels expect mono waveforms, got {c} channels")
@@ -312,6 +338,8 @@ class PyanNet(Model):
         flat = waveforms.to(device=ctx.device, dtype=torch.float32).reshape(-1).contiguous()
         off = np.arange(b, dtype=np.int64) * s
         valid = np.full(b, s, dtype=np.int32)
+        if ops.seg_activation(self.specifications) == ops.SEG_SIGMOID:
+            return ctx.seg_forward(flat, off, valid, window=s)
         _, logp = ctx.seg_forward(flat, off, valid, return_logp=True, window=s)
         return logp
 

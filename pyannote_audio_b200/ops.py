@@ -16,6 +16,8 @@ CHUNK = 160000
 FRAMES = 589
 SPEAKERS = 3
 CLASSES = 7
+SEG_MAX_CLASSES = 32       # largest classifier head of the segmentation kernels (and largest powerset)
+SEG_LOGSOFTMAX, SEG_SIGMOID = 0, 1
 EMB_DIM = 256
 SEG_MIN_SAMPLES = 1261     # shortest PyanNet window: 2 output frames (one frame cannot be instance-normalised)
 XVEC_MIN_SAMPLES = 4771    # shortest XVectorSincNet input: 15 SincNet frames, one frame after the TDNN layers
@@ -33,6 +35,42 @@ def check_seg_window(num_samples: int):
     if int(num_samples) < SEG_MIN_SAMPLES:
         raise ValueError(f"PyanNet needs windows of at least {SEG_MIN_SAMPLES} samples (2 output frames), got "
                          f"{int(num_samples)}")
+
+
+def check_seg_classes(num_classes: int):
+    if not 1 <= int(num_classes) <= SEG_MAX_CLASSES:
+        raise NotImplementedError(f"a PyanNet classifier of {int(num_classes)} classes has no CUDA kernel: the "
+                                  f"segmentation heads have 1 to {SEG_MAX_CLASSES} classes")
+
+
+def powerset_mapping(num_speakers: int, max_per_frame: int) -> np.ndarray:
+    """(K, num_speakers) uint8 mapping of utils/powerset.py (build_mapping): set size 0 .. max_per_frame,
+    itertools.combinations within each size.  Raises ValueError outside the kernels' range (K <= 32)."""
+    from itertools import combinations
+    from math import comb
+
+    n, m = int(num_speakers), int(max_per_frame)
+    if not 1 <= m <= n <= 32:
+        raise ValueError(f"powerset of {n} speakers with at most {m} per frame: need 1 <= max_per_frame <= "
+                         f"speakers <= 32")
+    k = sum(comb(n, i) for i in range(m + 1))
+    if k > SEG_MAX_CLASSES:
+        raise ValueError(f"powerset of {n} speakers with at most {m} per frame has {k} classes; at most "
+                         f"{SEG_MAX_CLASSES} are supported")
+    rows = [[1 if j in s else 0 for j in range(n)] for size in range(m + 1) for s in combinations(range(n), size)]
+    return np.array(rows, dtype=np.uint8)
+
+
+def seg_activation(specifications) -> int:
+    """Activation of a PyanNet head (core/model.py:271-300): sigmoid for binary and multi-label problems, log-softmax
+    for mono-label (powerset) problems."""
+    from .core import Problem
+
+    if specifications.problem in (Problem.BINARY_CLASSIFICATION, Problem.MULTI_LABEL_CLASSIFICATION):
+        return SEG_SIGMOID
+    if specifications.problem == Problem.MONO_LABEL_CLASSIFICATION:
+        return SEG_LOGSOFTMAX
+    raise NotImplementedError(f"PyanNet heads for {specifications.problem} have no CUDA kernel")
 
 
 def _ptr(t: Optional[torch.Tensor]):
@@ -91,6 +129,8 @@ class Context:
         _lib.check(self.lib.b200_ctx_create(C.byref(h), self.device.index))
         self._h = h
         self.seg_loaded = False
+        self.seg_classes = CLASSES           # classifier head of the loaded PyanNet: K classes, log-softmax or sigmoid
+        self.seg_activation = SEG_LOGSOFTMAX
         self.emb_loaded = False
         self.emb_channels = 256   # trunk output channels of the loaded embedding model: 256 (ResNet34) or 1024
         self.xvec_loaded = False
@@ -130,7 +170,12 @@ class Context:
         return float(ms.value), int(units.value)
 
     # ---- weights ---------------------------------------------------------------------------------
-    def load_segmentation(self, sd: Mapping[str, torch.Tensor]):
+    def load_segmentation(self, sd: Mapping[str, torch.Tensor], specifications=None):
+        """PyanNet weights.  The head has ``classifier.weight``'s K rows (1 .. 32); its activation comes from
+        ``specifications`` (sigmoid for binary / multi-label problems), log-softmax without them."""
+        num_classes = int(sd["classifier.weight"].shape[0])
+        check_seg_classes(num_classes)
+        activation = SEG_LOGSOFTMAX if specifications is None else seg_activation(specifications)
         keep = []
 
         def f(name):
@@ -166,11 +211,10 @@ class Context:
             w.linear_bias[i] = f(f"linear.{i}.bias")
         w.classifier_weight = f("classifier.weight")
         w.classifier_bias = f("classifier.bias")
-        if sd["classifier.weight"].shape[0] != CLASSES:
-            raise ValueError("only the 7-class powerset (3 speakers, max 2 simultaneous) head is supported")
         self.owners.pop("seg", None)          # whoever uploaded before no longer owns the slot
-        _lib.check(self.lib.b200_seg_load(self._h, C.byref(w)))
-        self.seg_loaded = True
+        self.seg_loaded = False
+        _lib.check(self.lib.b200_seg_load_head(self._h, C.byref(w), num_classes, activation))
+        self.seg_loaded, self.seg_classes, self.seg_activation = True, num_classes, activation
 
     def load_embedding(self, sd: Mapping[str, torch.Tensor]):
         keep = []
@@ -307,17 +351,30 @@ class Context:
         return out
 
     def seg_forward(self, wav, chunk_off, chunk_valid, return_logp=False, out: Optional[torch.Tensor] = None,
-                    window: int = CHUNK):
+                    window: int = CHUNK, reduce_max: bool = False):
         """PyanNet on windows of ``window`` samples (>= 1261): window i = wav[off[i] : off[i] + window], of which the
-        first valid[i] samples are real (zeros after) -> classes (n, F) uint8 (+ log-probabilities (n, F, 7)),
-        F = seg_num_frames(window)."""
+        first valid[i] samples are real (zeros after); F = seg_num_frames(window), K the loaded head's classes.
+        Log-softmax head -> classes (n, F) uint8 (+ log-probabilities (n, F, K)).  Sigmoid head -> scores (n, F, K)
+        float32, or with ``reduce_max`` their per-frame maximum (n, F, 1) computed in the same kernel."""
         check_seg_window(window)
         window = int(window)
         off, valid = self._chunks(wav, chunk_off, chunk_valid)
         n = len(off)
         F = seg_num_frames(window)
+        K = self.seg_classes
+        if self.seg_activation == SEG_SIGMOID:
+            if return_logp:
+                raise ValueError("the loaded segmentation head is a sigmoid head: it has scores, not log-probabilities")
+            scores = self._out(out, (n, F, 1 if reduce_max else K), torch.float32)
+            with torch.cuda.device(self.device):
+                _lib.check(self.lib.b200_seg_forward_scores(
+                    self._h, _ptr(wav), off.ctypes.data, valid.ctypes.data, n, window,
+                    None if reduce_max else _ptr(scores), _ptr(scores) if reduce_max else None, _stream(self.device)))
+            return scores
+        if reduce_max:
+            raise ValueError("reduce_max needs a sigmoid segmentation head (use powerset_speech for a powerset head)")
         cls = self._out(out, (n, F), torch.uint8)
-        logp = torch.empty((n, F, CLASSES), dtype=torch.float32, device=self.device) if return_logp else None
+        logp = torch.empty((n, F, K), dtype=torch.float32, device=self.device) if return_logp else None
         with torch.cuda.device(self.device):
             _lib.check(self.lib.b200_seg_forward_window(self._h, _ptr(wav), off.ctypes.data, valid.ctypes.data, n,
                                                         window, _ptr(cls), _ptr(logp), _stream(self.device)))
@@ -332,11 +389,15 @@ class Context:
                                                      _ptr(out), _stream(self.device)))
         return out
 
-    def powerset_to_multilabel(self, cls: torch.Tensor):
-        out = torch.empty(tuple(cls.shape) + (SPEAKERS,), dtype=torch.uint8, device=self.device)
+    def powerset_to_multilabel(self, cls: torch.Tensor, num_speakers: int = SPEAKERS, max_per_frame: int = 2):
+        """(…) uint8 powerset classes of ``num_speakers`` speakers with at most ``max_per_frame`` per frame ->
+        (…, num_speakers) uint8 multilabel (Powerset.to_multilabel, hard)."""
+        k = len(powerset_mapping(num_speakers, max_per_frame))
+        out = torch.empty(tuple(cls.shape) + (int(num_speakers),), dtype=torch.uint8, device=self.device)
         with torch.cuda.device(self.device):
-            _lib.check(self.lib.b200_powerset_to_multilabel(self._h, _ptr(cls), cls.numel(), _ptr(out),
-                                                            _stream(self.device)))
+            _lib.check(self.lib.b200_powerset_to_multilabel_generic(self._h, _ptr(cls.contiguous()), cls.numel(), k,
+                                                                    int(num_speakers), int(max_per_frame), _ptr(out),
+                                                                    _stream(self.device)))
         return out
 
     # ---- embeddings ------------------------------------------------------------------------------
@@ -617,12 +678,14 @@ class Context:
                                                       _stream(self.device)))
         return out
 
-    def powerset_speech(self, cls: torch.Tensor) -> torch.Tensor:
+    def powerset_speech(self, cls: torch.Tensor, num_speakers: int = SPEAKERS, max_per_frame: int = 2) -> torch.Tensor:
         """(…) uint8 powerset classes -> (…, 1) float32 speech indicator (max over the speakers of the multilabel)."""
+        k = len(powerset_mapping(num_speakers, max_per_frame))
         out = torch.empty(tuple(cls.shape) + (1,), dtype=torch.float32, device=self.device)
         with torch.cuda.device(self.device):
-            _lib.check(self.lib.b200_powerset_speech(self._h, _ptr(cls.contiguous()), cls.numel(), _ptr(out),
-                                                     _stream(self.device)))
+            _lib.check(self.lib.b200_powerset_speech_generic(self._h, _ptr(cls.contiguous()), cls.numel(), k,
+                                                             int(num_speakers), int(max_per_frame), _ptr(out),
+                                                             _stream(self.device)))
         return out
 
     def clean_frames(self, seg: torch.Tensor):

@@ -164,6 +164,15 @@ def require_10s_window(window_size: int):
                          f"{int(window_size)} samples: use Inference or VoiceActivityDetection for other durations")
 
 
+def require_community_head(specifications):
+    """Speaker diarization runs on the community-1 head only: a powerset of 3 speakers with at most 2 per frame (the
+    embedding masks, speaker counting and reconstruction kernels take 3 binary local speakers)."""
+    if not specifications.powerset or (len(specifications.classes), specifications.powerset_max_classes) != (3, 2):
+        raise ValueError("speaker diarization needs the community-1 segmentation head (a powerset of 3 speakers with "
+                         "at most 2 per frame): use Inference, VoiceActivityDetection or MultiLabelSegmentation for "
+                         "other heads")
+
+
 class SpeakerDiarization:
     def __init__(self, legacy: bool = False, segmentation: Union[PyanNet, Mapping, None] = None,
                  segmentation_step: float = 0.1, embedding: Union[BaseWeSpeakerResNet, Mapping, None] = None,
@@ -204,6 +213,7 @@ class SpeakerDiarization:
         self.der_variant = der_variant or {"collar": 0.0, "skip_overlap": False}
         self._plda = PLDA(plda) if isinstance(plda, Mapping) else plda
         duration = segmentation.specifications.duration
+        require_community_head(segmentation.specifications)
         require_10s_window(segmentation.audio.get_num_samples(duration))
         segmentation.to(device)
         embedding.to(device)
@@ -374,6 +384,7 @@ class SpeakerDiarization:
 
     def _require_10s_window(self):
         inf = self._segmentation
+        require_community_head(inf.model.specifications)
         require_10s_window(inf.model.audio.get_num_samples(inf.duration))
 
     def upload(self, files: Sequence[AudioFile]) -> dict:

@@ -6,8 +6,10 @@ from . import synthetic as syn
 
 
 def reference_style_checkpoint(kind):
-    """``kind``: "seg" (PyanNet), "emb" (WeSpeakerResNet34), "emb293" (WeSpeakerResNet293) or "xvec"
-    (XVectorSincNet).  A Lightning-format pytorch_model.bin as the reference writes it (model.py:244-256): state_dict +
+    """``kind``: "seg" (PyanNet, community-1 head), "seg_multilabel" (PyanNet with a 4-label sigmoid head,
+    permutation_invariant=False), "seg_binary" (a 1-class sigmoid ["speech"] head), "seg_powerset42" (a powerset
+    head of 4 speakers with at most 2 per frame, 11 classes), "emb" (WeSpeakerResNet34), "emb293"
+    (WeSpeakerResNet293) or "xvec" (XVectorSincNet).  A Lightning-format pytorch_model.bin as the reference writes it (model.py:244-256): state_dict +
     hyper_parameters + checkpoint["pyannote.audio"] whose `specifications` is pickled under the REFERENCE's module
     path pyannote.audio.core.task (registered here only while pickling, then removed again)."""
     import dataclasses
@@ -46,8 +48,19 @@ def reference_style_checkpoint(kind):
         for c in (Problem, Resolution, Specifications):
             c.__module__, c.__qualname__ = "pyannote.audio.core.task", c.__name__
             setattr(mods["pyannote.audio.core.task"], c.__name__, c)
-        if kind == "seg":
-            ck = {"state_dict": syn.make_segmentation_state_dict(0),
+        heads = {"seg": (7, Specifications(Problem.MONO_LABEL_CLASSIFICATION, Resolution.FRAME, 10.0,
+                                           classes=["speaker#1", "speaker#2", "speaker#3"], powerset_max_classes=2,
+                                           permutation_invariant=True)),
+                 "seg_multilabel": (4, Specifications(Problem.MULTI_LABEL_CLASSIFICATION, Resolution.FRAME, 5.0,
+                                                      classes=["speech", "music", "noise", "laughter"])),
+                 "seg_binary": (1, Specifications(Problem.BINARY_CLASSIFICATION, Resolution.FRAME, 5.0,
+                                                  classes=["speech"])),
+                 "seg_powerset42": (11, Specifications(Problem.MONO_LABEL_CLASSIFICATION, Resolution.FRAME, 10.0,
+                                                       classes=[f"speaker#{i}" for i in range(1, 5)],
+                                                       powerset_max_classes=2, permutation_invariant=True))}
+        if kind in heads:
+            num_classes, specs = heads[kind]
+            ck = {"state_dict": syn.make_segmentation_state_dict(0, num_classes=num_classes),
                   "hyper_parameters": {"sincnet": {"stride": 10}, "linear": {"hidden_size": 128, "num_layers": 2},
                                        "lstm": {"hidden_size": 128, "num_layers": 4, "bidirectional": True,
                                                 "monolithic": True, "dropout": 0.0},
@@ -55,10 +68,7 @@ def reference_style_checkpoint(kind):
                   "pyannote.audio": {"versions": {"pyannote.audio": "4.0.0"},
                                      "architecture": {"module": "pyannote.audio.models.segmentation.PyanNet",
                                                       "class": "PyanNet"},
-                                     "specifications": Specifications(
-                                         Problem.MONO_LABEL_CLASSIFICATION, Resolution.FRAME, 10.0,
-                                         classes=["speaker#1", "speaker#2", "speaker#3"], powerset_max_classes=2,
-                                         permutation_invariant=True)}}
+                                     "specifications": specs}}
         elif kind == "emb293":
             ck = {"state_dict": syn.make_bottleneck_state_dict(293, 1),
                   "hyper_parameters": {"sample_rate": 16000, "num_channels": 1, "num_mel_bins": 80,
