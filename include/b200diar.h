@@ -355,7 +355,9 @@ int b200_vbx_batched(b200_ctx* ctx, const double* fea, const double* phi, const 
                      int32_t num_problems, int32_t D, double Fa, double Fb, int32_t max_iters, double epsilon,
                      double* gamma, double* pi, int32_t* iters, void* stream);
 /* constrained_argmax / argmax (clustering.py:127-140, 658-665): soft[num_chunks][3][K] fp64 device ->
- * hard[num_chunks][3] int8 device (-2 = unassigned). */
+ * hard[num_chunks][3] int8 device (-2 = unassigned), K at most 127.  Constrained: the optimum that
+ * scipy's linear_sum_assignment(maximize=True) returns, ties included (soft must be NaN-free).  Unconstrained:
+ * np.argmax per speaker (first maximum; a NaN counts as the maximum). */
 int b200_assign(b200_ctx* ctx, const double* soft, int32_t num_chunks, int32_t num_clusters, int32_t constrained,
                 int8_t* hard, void* stream);
 

@@ -132,14 +132,22 @@ class BaseClustering:
         return ctx.assign(soft, constrained=True).cpu().numpy()
 
     def _assign(self, ctx, emb64, centroids, active, constrained):
+        """``active`` (C,3) bool: VBx gives inactive speakers the score ``soft.min() - 1`` before the constrained
+        assignment (clustering.py:655-663); None: scores as computed (assign_embeddings, :142-212)."""
         C = emb64.shape[0]
         K = centroids.shape[0]
         e2k = ctx.cdist_cosine(emb64.reshape(-1, emb64.shape[-1]), centroids).reshape(C, ops.SPEAKERS, K)
         soft = 2 - e2k
-        if constrained:
+        if not constrained:
+            return ctx.assign(soft, constrained=False), soft
+        # with a NaN embedding row (filter_embeddings drops it from training, but it is still assigned) `const` is NaN
+        # too and so are the inactive rows; constrained_argmax (:127-132) gives the solver NaN replaced by the
+        # nan-minimum, and the caller gets `soft` with its NaN
+        if active is not None:
             const = soft.min() - 1.0
             soft = torch.where(active[:, :, None], soft, const)
-        hard = ctx.assign(soft, constrained=constrained)
+        nanmin = torch.nan_to_num(soft, nan=float("inf")).min()
+        hard = ctx.assign(torch.where(torch.isnan(soft), nanmin, soft), constrained=True)
         return hard, soft
 
 
@@ -419,5 +427,5 @@ class AgglomerativeClustering(BaseClustering):
         # centroids = float32 means of the float32 rows, like assign_embeddings (clustering.py:182-188)
         centroids = torch.from_numpy(np.vstack([np.mean(train32[train_clusters == k], axis=0)
                                                 for k in range(K)]).astype(np.float64)).to(ctx.device)
-        hard, soft = self._assign(ctx, emb64, centroids.contiguous(), active, self.constrained_assignment)
+        hard, soft = self._assign(ctx, emb64, centroids.contiguous(), None, self.constrained_assignment)
         return hard.cpu().numpy(), soft.cpu().numpy(), centroids.cpu().numpy()

@@ -1485,9 +1485,9 @@ int b200_plda_transform(b200_ctx* ctx, const double* x, int32_t n, int32_t Din, 
 
 int b200_weighted_centroids(b200_ctx* ctx, const double* q, int32_t n, int32_t S, const int32_t* kept, int32_t K,
                             const double* train, int32_t dim, double* centroids, void* stream) {
-  B200_CHECK(ctx && q && kept && train && centroids && n >= 1 && S >= 1 && K >= 0 && dim >= 1, B200_ERR_INVALID,
-             "bad arguments");
-  if (K == 0) return B200_OK;
+  B200_CHECK(ctx && q && train && n >= 1 && S >= 1 && K >= 0 && dim >= 1, B200_ERR_INVALID, "bad arguments");
+  if (K == 0) return B200_OK;        // no speaker kept: empty `kept` and `centroids` (null data pointers)
+  B200_CHECK(kept && centroids, B200_ERR_INVALID, "bad arguments");
   DeviceGuard g(ctx->device);
   ctx->launches += 1;
   return weighted_centroids(q, n, S, kept, K, train, dim, centroids, (cudaStream_t)stream);
@@ -1525,6 +1525,8 @@ int b200_vbx(b200_ctx* ctx, const double* fea, const double* phi, int32_t n, int
 int b200_assign(b200_ctx* ctx, const double* soft, int32_t num_chunks, int32_t num_clusters, int32_t constrained,
                 int8_t* hard, void* stream) {
   B200_CHECK(ctx && soft && hard && num_chunks >= 0 && num_clusters >= 1, B200_ERR_INVALID, "bad arguments");
+  B200_CHECK(num_clusters <= 127, B200_ERR_INVALID, "assign: %d clusters, at most 127 fit the int8 cluster ids",
+             (int)num_clusters);
   if (num_chunks == 0) return B200_OK;
   DeviceGuard g(ctx->device);
   ctx->launches += 1;

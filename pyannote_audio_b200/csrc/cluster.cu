@@ -521,6 +521,67 @@ vbx_kernel(const VbxJob* __restrict__ jobs, const double* __restrict__ fea_all, 
 // ------------------------------------------------------------------------------------------------------
 // constrained assignment: maximise sum of soft[c][s][k] over injective maps of (up to 3) speakers to clusters
 // ------------------------------------------------------------------------------------------------------
+// The reference solves it with scipy.optimize.linear_sum_assignment(maximize=True) (clustering.py:127-140).  Chunks
+// with inactive speakers have rows that are all one constant, so optima are tied exactly and the answer is whichever
+// optimum the solver reaches.  The kernel therefore runs the same solver: the shortest augmenting path method of
+// Crouse (2016) on the negated costs, transposed when there are fewer clusters than speakers, columns scanned from the
+// last to the first, and ties of the path minimum resolved towards a free column.  It also makes the same choice on
+// near-ties, because it does the same additions and subtractions in the same order.
+constexpr int kAssignMaxK = 127;     // cluster ids are int8
+
+__device__ void assign_lsap(const double* __restrict__ p, int K, signed char* __restrict__ h) {
+  const bool tr = K < 3;             // tall 3 x K cost matrix: solve its transpose (clusters pick speakers)
+  const int nr = tr ? K : 3, nc = tr ? 3 : K;
+  double u[3], v[kAssignMaxK], spc[kAssignMaxK];
+  int col4row[3], row4col[kAssignMaxK], path[kAssignMaxK], rem[kAssignMaxK];
+  bool SR[3], SC[kAssignMaxK];
+  for (int i = 0; i < nr; ++i) { u[i] = 0.0; col4row[i] = -1; }
+  for (int j = 0; j < nc; ++j) { v[j] = 0.0; row4col[j] = -1; path[j] = -1; }
+  for (int cur = 0; cur < nr; ++cur) {
+    for (int i = 0; i < nr; ++i) SR[i] = false;
+    for (int j = 0; j < nc; ++j) { SC[j] = false; spc[j] = INFINITY; rem[j] = nc - j - 1; }
+    int nrem = nc, i = cur, sink = -1;
+    double minv = 0.0;
+    while (sink == -1) {
+      int index = -1;
+      double lowest = INFINITY;
+      SR[i] = true;
+      for (int it = 0; it < nrem; ++it) {
+        const int j = rem[it];
+        const double cost = -(tr ? p[j * K + i] : p[i * K + j]);
+        const double r = __dsub_rn(__dsub_rn(__dadd_rn(minv, cost), u[i]), v[j]);
+        if (r < spc[j]) { path[j] = i; spc[j] = r; }
+        if (spc[j] < lowest || (spc[j] == lowest && row4col[j] == -1)) { lowest = spc[j]; index = it; }
+      }
+      minv = lowest;
+      const int j = rem[index];
+      if (row4col[j] == -1) sink = j;
+      else i = row4col[j];
+      SC[j] = true;
+      rem[index] = rem[--nrem];
+    }
+    u[cur] = __dadd_rn(u[cur], minv);
+    for (int a = 0; a < nr; ++a)
+      if (SR[a] && a != cur) u[a] = __dadd_rn(u[a], __dsub_rn(minv, spc[col4row[a]]));
+    for (int b = 0; b < nc; ++b)
+      if (SC[b]) v[b] = __dsub_rn(v[b], __dsub_rn(minv, spc[b]));
+    for (int j = sink;;) {           // augment along the path back to the current row
+      const int a = path[j];
+      row4col[j] = a;
+      const int t = col4row[a];
+      col4row[a] = j;
+      j = t;
+      if (a == cur) break;
+    }
+  }
+  h[0] = h[1] = h[2] = -2;
+  if (tr) {
+    for (int k = 0; k < K; ++k) h[col4row[k]] = (signed char)k;
+  } else {
+    for (int s = 0; s < 3; ++s) h[s] = (signed char)col4row[s];
+  }
+}
+
 __global__ void assign_kernel(const double* __restrict__ soft, int C, int K, int constrained,
                               signed char* __restrict__ hard) {
   const int c = blockIdx.x * blockDim.x + threadIdx.x;
@@ -528,40 +589,16 @@ __global__ void assign_kernel(const double* __restrict__ soft, int C, int K, int
   const double* p = soft + (size_t)c * 3 * K;
   signed char* h = hard + c * 3;
   if (!constrained) {
+    // np.argmax: the first maximum, and a NaN counts as the maximum (the first NaN wins)
     for (int s = 0; s < 3; ++s) {
       int best = 0;
-      for (int k = 1; k < K; ++k)
-        if (p[s * K + k] > p[s * K + best]) best = k;
+      for (int k = 1; k < K && !isnan(p[s * K + best]); ++k)
+        if (isnan(p[s * K + k]) || p[s * K + k] > p[s * K + best]) best = k;
       h[s] = (signed char)best;
     }
     return;
   }
-  h[0] = h[1] = h[2] = -2;
-  double bestv = -DBL_MAX;
-  if (K >= 3) {
-    for (int k0 = 0; k0 < K; ++k0)
-      for (int k1 = 0; k1 < K; ++k1) {
-        if (k1 == k0) continue;
-        for (int k2 = 0; k2 < K; ++k2) {
-          if (k2 == k0 || k2 == k1) continue;
-          const double v = p[k0] + p[K + k1] + p[2 * K + k2];
-          if (v > bestv) { bestv = v; h[0] = k0; h[1] = k1; h[2] = k2; }
-        }
-      }
-  } else if (K == 2) {
-    // two of the three speakers get the two clusters
-    for (int s0 = 0; s0 < 3; ++s0)
-      for (int s1 = 0; s1 < 3; ++s1) {
-        if (s1 == s0) continue;
-        const double v = p[s0 * K + 0] + p[s1 * K + 1];
-        if (v > bestv) { bestv = v; h[0] = h[1] = h[2] = -2; h[s0] = 0; h[s1] = 1; }
-      }
-  } else if (K == 1) {
-    int best = 0;
-    for (int s = 1; s < 3; ++s)
-      if (p[s] > p[best]) best = s;
-    h[best] = 0;
-  }
+  assign_lsap(p, K, h);
 }
 
 // ------------------------------------------------------------------------------------------------------
