@@ -48,8 +48,9 @@ int b200_ctx_destroy(b200_ctx* ctx);
  *   split-precision GEMMs, 0 = fp32 CUDA-core twins; "seg_conv_impl" 1 = SincNet sinc / Conv1d layers as split-precision
  *   wgmma implicit GEMMs, 0 = fp32 CUDA-core twins; "seg_rec_impl" 1 = LSTM recurrence as split-precision wgmma on
  *   2-CTA clusters (with "seg_gemm_impl" 1), 0 = fp32 CUDA-core twin; "fbank_share" 1 = overlapping chunks share their fbank frames;
- *   "profile" 1 = CUDA-event timers around the trunk / the segmentation (b200_ctx_timer).  Unknown keys and values out
- *   of range return B200_ERR_INVALID. */
+ *   "profile" 1 = CUDA-event timers around the trunk / the segmentation (b200_ctx_timer); "linkage_grid_min" (32769,
+ *   from 2 up to that default): the smallest linkage problem that runs on the whole-GPU path (b200_linkage_centroid).
+ *   Unknown keys and values out of range return B200_ERR_INVALID. */
 int b200_ctx_set_option(b200_ctx* ctx, const char* key, int64_t value);
 /* number of kernels this ctx has launched so far (bench.py's gpu_launches claim) */
 int64_t b200_ctx_launch_count(const b200_ctx* ctx);
@@ -321,15 +322,24 @@ int b200_clean_frames(b200_ctx* ctx, const uint8_t* seg, int32_t num_chunks, int
  * normalize: 0 = rows as given, 1 = L2-normalised in fp64, 2 = rows hold float32 values and are normalised exactly as
  * numpy does on float32 embeddings (x / np.linalg.norm(x, axis=1, keepdims=True): float32 pairwise sum, float32
  * sqrt and division; clustering.py:597-599) before widening; Z[n-1][4] fp64 device in scipy's format.
- * Limits: n <= 32768 observations per problem (a dense n x n fp64 distance matrix lives in the ctx workspace: 8 n^2
- * bytes, 8.6 GB at the limit); longer recordings must be clustered in windows by the caller. */
+ * Problems of n <= 32768 observations run one CTA each over a dense n x n fp64 distance matrix in the ctx workspace
+ * (8 n^2 bytes).  Larger ones (n >= option "linkage_grid_min") run one after another, each on the whole GPU (a
+ * cooperative grid) over scipy's condensed distances, 4 n (n - 1) bytes allocated stream-ordered for the call and freed
+ * before it returns (4.3 GB at n = 32 768, 17 GB at 65 536, 40 GB at 100 000); the limit is device memory
+ * (B200_STATUS_OOM, with n and the bytes in the message, when the allocation fails).  Both paths emit the same Z bit
+ * for bit.  At most 1 048 560 observations per problem. */
 int b200_linkage_centroid(b200_ctx* ctx, const double* x, int32_t n, int32_t dim, int32_t normalize, double* Z,
                           void* stream);
-/* the same (clustering.py:594-603) for num_problems independent problems in ONE launch (one CTA each): rows of problem f are
+/* the same (clustering.py:594-603) for num_problems independent problems in ONE launch (one CTA each; problems above
+ * the threshold then take the whole-GPU path in turn): rows of problem f are
  * x[row_offsets[f] .. row_offsets[f+1]) (row_offsets: HOST int32[num_problems+1]); Z rows are concatenated, problem
  * f contributing max(n_f - 1, 0) rows. */
 int b200_linkage_centroid_batched(b200_ctx* ctx, const double* x, const int32_t* row_offsets, int32_t num_problems,
                                   int32_t dim, int32_t normalize, double* Z, void* stream);
+/* host only: device bytes a b200_linkage_centroid_batched call with these HOST row_offsets needs at the default
+ * "linkage_grid_min" = the ctx workspace it grows to plus the per-call packed distances of its largest problem above
+ * the threshold.  Negative status for bad arguments (num_problems < 1, dim < 1, decreasing offsets). */
+int64_t b200_linkage_bytes(const int32_t* row_offsets, int32_t num_problems, int32_t dim);
 /* fcluster(Z, t, criterion="distance") (clustering.py:604, 385): HOST arrays, labels[n] 1-based like scipy. */
 int b200_fcluster_distance(const double* Z, int32_t n, double t, int32_t* labels);
 /* PLDA.__call__ (core/plda.py:50-63; xvec_tf / plda_tf of utils/vbx.py:211-217): x[n][Din] fp64 device ->

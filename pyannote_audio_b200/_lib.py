@@ -110,6 +110,7 @@ _PROTOS = {
                                         C.c_void_p]),
     "b200_linkage_centroid_batched": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_int32, C.c_int32, C.c_int32,
                                                 C.c_void_p, C.c_void_p]),
+    "b200_linkage_bytes": (C.c_int64, [C.c_void_p, C.c_int32, C.c_int32]),
     "b200_vbx_batched": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_int32, C.c_int32,
                                    C.c_double, C.c_double, C.c_int32, C.c_double, C.c_void_p, C.c_void_p, C.c_void_p,
                                    C.c_void_p]),

@@ -50,6 +50,9 @@ struct b200_ctx {
   // of 128 pixels per image row) split evenly over the machine
   int emb_max_batch = 264;
   int fbank_share = 1;          // 1 = overlapping hop-aligned chunks share their fbank frames (emb.cuh: FbankRun)
+  // smallest linkage problem that runs on the whole GPU over packed distances (cluster.cuh); at most the default, so
+  // that every problem the dense one-CTA kernel cannot hold goes there
+  int linkage_grid_min = kLinkGridMinDefault;
   int64_t launches = 0;
   SegWeights seg;
   EmbWeights emb;
@@ -401,6 +404,11 @@ int b200_ctx_set_option(b200_ctx* ctx, const char* key, int64_t value) {
   else if (k == "seg_conv_impl") ctx->seg_conv_impl = (int)value;
   else if (k == "seg_rec_impl") ctx->seg_rec_impl = (int)value;
   else if (k == "fbank_share") ctx->fbank_share = (int)value;
+  else if (k == "linkage_grid_min") {
+    B200_CHECK(value >= 2 && value <= kLinkGridMinDefault, B200_ERR_INVALID, "option '%s' value %lld out of range",
+               key, (long long)value);
+    ctx->linkage_grid_min = (int)value;
+  }
   else B200_CHECK(false, B200_ERR_INVALID, "unknown option '%s'", key);
   B200_CHECK(ctx->seg_max_batch >= 1 && ctx->emb_max_batch >= 1 && ctx->conv_impl >= 0 && ctx->conv_impl <= 2 &&
                  ctx->seg_gemm_impl >= 0 && ctx->seg_gemm_impl <= 1 && ctx->seg_conv_impl >= 0 && ctx->seg_conv_impl <= 1 &&
@@ -1445,19 +1453,35 @@ int b200_clean_frames(b200_ctx* ctx, const uint8_t* seg, int32_t num_chunks, int
 }
 
 // ------------------------------------------------------------------------------------------------------
+static int check_linkage_offsets(const int32_t* row_offsets, int32_t num_problems) {
+  for (int f = 0; f < num_problems; ++f)
+    B200_CHECK(row_offsets[f + 1] >= row_offsets[f] && row_offsets[f + 1] - row_offsets[f] <= kLinkMaxRows,
+               B200_ERR_INVALID, "linkage: problem %d has %d observations (row offsets must be non-decreasing, at most "
+               "%d per problem)", f, (int)(row_offsets[f + 1] - row_offsets[f]), kLinkMaxRows);
+  return B200_OK;
+}
+
+int64_t b200_linkage_bytes(const int32_t* row_offsets, int32_t num_problems, int32_t dim) {
+  B200_CHECK(row_offsets && num_problems >= 1 && dim >= 1 && row_offsets[0] >= 0, B200_ERR_INVALID, "bad arguments");
+  const int rc = check_linkage_offsets(row_offsets, num_problems);
+  if (rc) return rc;
+  return (int64_t)(linkage_workspace_bytes_batched(row_offsets, num_problems, dim, kLinkGridMinDefault) +
+                   linkage_grid_bytes(row_offsets, num_problems, kLinkGridMinDefault));
+}
+
 int b200_linkage_centroid_batched(b200_ctx* ctx, const double* x, const int32_t* row_offsets, int32_t num_problems,
                                   int32_t dim, int32_t normalize, double* Z, void* stream) {
   B200_CHECK(ctx && x && row_offsets && Z && num_problems >= 1 && dim >= 1, B200_ERR_INVALID, "bad arguments");
-  for (int f = 0; f < num_problems; ++f)
-    B200_CHECK(row_offsets[f + 1] >= row_offsets[f] && row_offsets[f + 1] - row_offsets[f] <= 32768, B200_ERR_INVALID,
-               "linkage: problem %d has %d observations (row offsets must be non-decreasing, at most 32768 per problem "
-               "= about 3 h of audio at a 1 s step: cluster longer recordings in windows)", f,
-               (int)(row_offsets[f + 1] - row_offsets[f]));
-  DeviceGuard g(ctx->device);
-  int rc = ensure_ws(ctx, linkage_workspace_bytes_batched(row_offsets, num_problems, dim));
+  int rc = check_linkage_offsets(row_offsets, num_problems);
   if (rc) return rc;
-  ctx->launches += 2 + num_problems;
-  return linkage_centroid_batched(x, row_offsets, num_problems, dim, normalize, Z, ctx->ws, (cudaStream_t)stream);
+  DeviceGuard g(ctx->device);
+  rc = ensure_ws(ctx, linkage_workspace_bytes_batched(row_offsets, num_problems, dim, ctx->linkage_grid_min));
+  if (rc) return rc;
+  int big = 0;
+  for (int f = 0; f < num_problems; ++f) big += row_offsets[f + 1] - row_offsets[f] >= ctx->linkage_grid_min;
+  ctx->launches += 2 + num_problems + big;
+  return linkage_centroid_batched(x, row_offsets, num_problems, dim, normalize, Z, ctx->ws, (cudaStream_t)stream,
+                                  ctx->linkage_grid_min);
 }
 
 int b200_linkage_centroid(b200_ctx* ctx, const double* x, int32_t n, int32_t dim, int32_t normalize, double* Z,

@@ -11,12 +11,16 @@
 #include "common.cuh"
 #include "cluster.cuh"
 #include <cfloat>
+#include <algorithm>
 #include <cmath>
+#include <cooperative_groups.h>
+
+namespace cg = cooperative_groups;
 
 namespace b200 {
 
 // ------------------------------------------------------------------------------------------------------
-// pairwise Euclidean distances (full symmetric matrix, diagonal unused)
+// pairwise Euclidean distances (full symmetric matrix with unused diagonal, or scipy's condensed triangle)
 // ------------------------------------------------------------------------------------------------------
 __global__ void normalize_rows_kernel(const double* __restrict__ x, double* __restrict__ y, int n, int dim) {
   const int i = blockIdx.x;
@@ -75,7 +79,17 @@ __global__ void normalize_rows_np_f32_kernel(const double* __restrict__ x, doubl
   for (int d = 0; d < dim; ++d) y[(size_t)i * dim + d] = (double)__fdiv_rn((float)r[d], nrm);
 }
 
+// packed row k of scipy's condensed distance vector (upper triangle, row-major): element j > k is row[j], with
+// 64-bit offsets (the condensed index passes 2^31 at n ~ 65k)
+__host__ __device__ __forceinline__ long long packed_row(int k, int n) {
+  return (long long)k * n - (long long)k * (k + 1) / 2 - k - 1;
+}
+
+// kPacked = false: full symmetric n x n matrix, diagonal DBL_MAX; true: condensed upper triangle (scipy's pdist
+// layout, n (n - 1) / 2 values).  The per-pair arithmetic is the same code for both layouts.
+template <bool kPacked>
 __global__ void pdist_kernel(const double* __restrict__ x, double* __restrict__ D, int n, int dim) {
+  if (kPacked && blockIdx.x < blockIdx.y) return;          // tile entirely below the diagonal
   // 16x16 tile of pairs per block, operands staged through shared memory in chunks of 32 dims
   __shared__ double xi[16][33], xj[16][33];
   const int i = blockIdx.y * 16 + threadIdx.y, j = blockIdx.x * 16 + threadIdx.x;
@@ -96,7 +110,11 @@ __global__ void pdist_kernel(const double* __restrict__ x, double* __restrict__ 
     }
     __syncthreads();
   }
-  if (i < n && j < n) D[(size_t)i * n + j] = (i == j) ? DBL_MAX : sqrt(s);
+  if (kPacked) {
+    if (i < j && j < n) D[packed_row(i, n) + j] = sqrt(s);
+  } else {
+    if (i < n && j < n) D[(size_t)i * n + j] = (i == j) ? DBL_MAX : sqrt(s);
+  }
 }
 
 // ------------------------------------------------------------------------------------------------------
@@ -130,28 +148,30 @@ __device__ __forceinline__ MinPair warp_min(MinPair m) {
 }
 
 // nearest alive j > k of row k among the columns j = k + 1 + first, + stride, ...  (four independent loads in flight
-// per thread); min_pair is an order-independent (value, index) minimum, so any split of a row gives the same answer
-__device__ __forceinline__ MinPair row_nn_part(const double* __restrict__ D, const unsigned char* alive, int n, int k,
+// per thread); min_pair is an order-independent (value, index) minimum, so any split of a row gives the same answer.
+// row[j] is d(k, j).  kL2: load through L2 only (the grid-wide kernel reads values other CTAs have just written).
+template <bool kL2 = false>
+__device__ __forceinline__ MinPair row_nn_part(const double* __restrict__ row, const unsigned char* alive, int n, int k,
                                                int first, int stride) {
+  auto ld = [&](int j) { return kL2 ? __ldcg(row + j) : row[j]; };
   MinPair m{DBL_MAX, n};
-  const double* row = D + (size_t)k * n;
   int j = k + 1 + first;
   for (; j + 3 * stride < n; j += 4 * stride) {
-    const double v0 = row[j], v1 = row[j + stride], v2 = row[j + 2 * stride], v3 = row[j + 3 * stride];
+    const double v0 = ld(j), v1 = ld(j + stride), v2 = ld(j + 2 * stride), v3 = ld(j + 3 * stride);
     if (alive[j]) m = min_pair(m, MinPair{v0, j});
     if (alive[j + stride]) m = min_pair(m, MinPair{v1, j + stride});
     if (alive[j + 2 * stride]) m = min_pair(m, MinPair{v2, j + 2 * stride});
     if (alive[j + 3 * stride]) m = min_pair(m, MinPair{v3, j + 3 * stride});
   }
   for (; j < n; j += stride)
-    if (alive[j]) m = min_pair(m, MinPair{row[j], j});
+    if (alive[j]) m = min_pair(m, MinPair{ld(j), j});
   return m;
 }
 
 // nearest alive j > k of row k, computed by one warp
 __device__ __forceinline__ void row_nn(const double* __restrict__ D, const unsigned char* alive, int n, int k, int lane,
                                        double* nn_d, int* nn_i) {
-  const MinPair m = warp_min(row_nn_part(D, alive, n, k, lane, 32));
+  const MinPair m = warp_min(row_nn_part(D + (size_t)k * n, alive, n, k, lane, 32));
   if (lane == 0) { nn_d[k] = m.v; nn_i[k] = m.i; }
 }
 
@@ -286,7 +306,7 @@ __global__ void __launch_bounds__(1024) linkage_centroid_kernel(const LinkJob* _
         const int t = t0 + g;
         const int k = t < nt ? todo[t] : -1;
         MinPair part{DBL_MAX, n};
-        if (k >= 0) part = warp_min(row_nn_part(D, alive, n, k, wl * 32 + lane, W * 32));
+        if (k >= 0) part = warp_min(row_nn_part(D + (size_t)k * n, alive, n, k, wl * 32 + lane, W * 32));
         if (W == 1) {
           if (k >= 0 && lane == 0) { nn_d[k] = part.v; nn_i[k] = part.i; }
         } else {
@@ -302,6 +322,117 @@ __global__ void __launch_bounds__(1024) linkage_centroid_kernel(const LinkJob* _
       }
       __syncthreads();
     }
+  }
+}
+
+// ------------------------------------------------------------------------------------------------------
+// centroid linkage of one large problem on the whole GPU: a cooperative grid over the packed distances
+// ------------------------------------------------------------------------------------------------------
+constexpr int kLinkGridThreads = 512;        // one CTA per SM; 128 registers a thread keep the merge loop unspilled
+constexpr int kLinkGridMaxCtas = 1024;
+// scratch after the job table: per-CTA partial minima of phases A and B (2 x kLinkGridMaxCtas) and the re-scan count
+constexpr size_t kLinkGridScratch = 2 * kLinkGridMaxCtas * sizeof(MinPair) + 256;
+
+// (value, index) minimum over the CTA, returned to every thread (every warp reduces the warp minima itself)
+__device__ __forceinline__ MinPair block_min(MinPair m, MinPair* s_red, int n) {
+  constexpr int kWarps = kLinkGridThreads / 32;
+  m = warp_min(m);
+  __syncthreads();                                         // s_red free again
+  if ((threadIdx.x & 31) == 0) s_red[threadIdx.x >> 5] = m;
+  __syncthreads();
+  const int lane = threadIdx.x & 31;
+  return warp_min(lane < kWarps ? s_red[lane] : MinPair{DBL_MAX, n});
+}
+
+// The merges of linkage_centroid_kernel, each split over every CTA with three grid-wide barriers:
+//   (A) per-CTA minima of the nearest-neighbour candidates; after the barrier every CTA reduces the partials to the
+//       same closest pair (x, y);
+//   (B) the Lance-Williams update of every alive k and the maintenance of the candidates of rows k < y, spread over
+//       the grid; per-CTA minima of y's new neighbour among k > y; rows whose candidate was x or y are queued;
+//   (C) each queued row is re-scanned by one CTA; CTA 0 installs y's candidate, size and id.
+// Every reduction is the order-independent min_pair over the same values, and the arithmetic is lw_centroid, so Z is
+// bit-identical to the one-CTA kernel's.  Per-row state lives in global memory; P is the condensed upper triangle.
+__global__ void __launch_bounds__(kLinkGridThreads, 1)
+linkage_centroid_grid_kernel(double* P, int n, double* Z, double* nn_d, int* nn_i, int* size, int* id,
+                             unsigned char* alive, int* todo, int* ntodo, MinPair* part) {
+  cg::grid_group grid = cg::this_grid();
+  __shared__ MinPair s_red[kLinkGridThreads / 32];
+  const int tid = threadIdx.x, lane = tid & 31, nb = gridDim.x;
+  const int gtid = blockIdx.x * kLinkGridThreads + tid, gthreads = nb * kLinkGridThreads;
+  const int gwarp = gtid >> 5, gwarps = gthreads >> 5;
+  for (int i = gtid; i < n; i += gthreads) { size[i] = 1; id[i] = i; alive[i] = 1; }
+  grid.sync();
+  for (int k = gwarp; k < n; k += gwarps) {
+    const MinPair m = warp_min(row_nn_part<true>(P + packed_row(k, n), alive, n, k, lane, 32));
+    if (lane == 0) { nn_d[k] = m.v; nn_i[k] = m.i; }
+  }
+  grid.sync();
+
+  for (int m = 0; m < n - 1; ++m) {
+    // A. global closest pair
+    MinPair best{DBL_MAX, n};
+    for (int i = gtid; i < n; i += gthreads)
+      if (alive[i] && nn_i[i] < n) best = min_pair(best, MinPair{nn_d[i], i});
+    best = block_min(best, s_red, n);
+    if (tid == 0) part[blockIdx.x] = best;
+    if (gtid == 0) *ntodo = 0;                             // every read of the previous merge's count is done
+    grid.sync();
+    MinPair b{DBL_MAX, n};
+    for (int c = lane; c < nb; c += 32) b = min_pair(b, part[c]);
+    b = warp_min(b);
+    const int x = b.i, y = nn_i[x];                        // x < y: candidates only look right
+    const double dxy = b.v;
+    const double nx = size[x], ny = size[y];
+    if (gtid == 0) {
+      const int ia = id[x], ib = id[y];
+      Z[(size_t)m * 4 + 0] = ia < ib ? ia : ib;
+      Z[(size_t)m * 4 + 1] = ia < ib ? ib : ia;
+      Z[(size_t)m * 4 + 2] = dxy;
+      Z[(size_t)m * 4 + 3] = nx + ny;
+      alive[x] = 0;                                        // row x is skipped below by its own thread either way
+    }
+    // B. Lance-Williams update (merged cluster lives in slot y, slot x dies) + candidate maintenance
+    MinPair ybest{DBL_MAX, n};
+    for (int k = gtid; k < n; k += gthreads) {
+      if (!alive[k] || k == x || k == y) continue;
+      const double dxk = P[k < x ? packed_row(k, n) + x : packed_row(x, n) + k];
+      double* pyk = P + (k < y ? packed_row(k, n) + y : packed_row(y, n) + k);
+      const double dn = lw_centroid(dxk, *pyk, dxy, nx, ny);
+      *pyk = dn;
+      if (k > y) {
+        ybest = min_pair(ybest, MinPair{dn, k});           // new nearest neighbour of y among j > y
+      } else {
+        const int cur = nn_i[k];
+        if (cur == x || cur == y) {
+          todo[atomicAdd(ntodo, 1)] = k;                   // its candidate vanished or changed: re-scan
+        } else if (dn < nn_d[k] || (dn == nn_d[k] && y < cur)) {
+          nn_d[k] = dn;
+          nn_i[k] = y;
+        }
+      }
+    }
+    ybest = block_min(ybest, s_red, n);
+    if (tid == 0) part[nb + blockIdx.x] = ybest;
+    grid.sync();
+    // C. y's candidate from the partials of B; queued rows re-scanned, one CTA per row
+    if (blockIdx.x == 0 && tid < 32) {
+      MinPair yb{DBL_MAX, n};
+      for (int c = lane; c < nb; c += 32) yb = min_pair(yb, part[nb + c]);
+      yb = warp_min(yb);
+      if (lane == 0) {
+        nn_d[y] = yb.v;
+        nn_i[y] = yb.i;
+        size[y] = (int)(nx + ny);
+        id[y] = n + m;
+      }
+    }
+    const int nt = *ntodo;
+    for (int t = blockIdx.x; t < nt; t += nb) {            // uniform over the CTA
+      const int k = todo[t];
+      const MinPair r = block_min(row_nn_part<true>(P + packed_row(k, n), alive, n, k, tid, kLinkGridThreads), s_red, n);
+      if (tid == 0) { nn_d[k] = r.v; nn_i[k] = r.i; }
+    }
+    grid.sync();
   }
 }
 
@@ -604,33 +735,71 @@ __global__ void assign_kernel(const double* __restrict__ soft, int C, int K, int
 // ------------------------------------------------------------------------------------------------------
 // host wrappers
 // ------------------------------------------------------------------------------------------------------
-size_t linkage_workspace_bytes_batched(const int* row_offsets, int nfiles, int dim) {
+size_t linkage_workspace_bytes_batched(const int* row_offsets, int nfiles, int dim, int grid_min) {
   size_t d = 0;
+  bool grid = false;
   const int ntot = row_offsets[nfiles];
   for (int f = 0; f < nfiles; ++f) {
     const size_t n = row_offsets[f + 1] - row_offsets[f];
-    d += n * n;
+    if ((long long)n >= grid_min) grid = true;
+    else d += n * n;
   }
   return align_up(d * 8, 256) + align_up((size_t)ntot * dim * 8, 256) + (size_t)(ntot + nfiles + 64) * 40 +
-         (size_t)nfiles * sizeof(LinkJob) + 8192;
+         (size_t)nfiles * sizeof(LinkJob) + 8192 + (grid ? kLinkGridScratch : 0);
 }
 
+// the packed distances of the largest whole-GPU problem: allocated for the call, shared by its large problems
+size_t linkage_grid_bytes(const int* row_offsets, int nfiles, int grid_min) {
+  size_t big = 0;
+  for (int f = 0; f < nfiles; ++f) {
+    const size_t n = row_offsets[f + 1] - row_offsets[f];
+    if ((long long)n >= grid_min && 4 * n * (n - 1) > big) big = 4 * n * (n - 1);
+  }
+  return big;
+}
+
+// a stream-ordered device allocation freed when the scope ends (after the work queued on `st` before the free)
+struct StreamFree {
+  void* p;
+  cudaStream_t st;
+  ~StreamFree() {
+    if (p) cudaFreeAsync(p, st);
+  }
+};
+
 int linkage_centroid_batched(const double* x, const int* row_offsets, int nfiles, int dim, int normalize, double* Z,
-                             void* ws, cudaStream_t st) {
+                             void* ws, cudaStream_t st, int grid_min) {
   const int ntot = row_offsets[nfiles];
   std::vector<LinkJob> jobs(nfiles);
+  std::vector<int> big;                  // problems for the whole-GPU path: no CTA of the batched kernel (n = 0)
   size_t d = 0;
   int z = 0;
   for (int f = 0; f < nfiles; ++f) {
     const int n = row_offsets[f + 1] - row_offsets[f];
-    jobs[f].n = n;
+    const bool grid = n >= grid_min;
+    if (grid) big.push_back(f);
+    jobs[f].n = grid ? 0 : n;
     jobs[f].row_off = row_offsets[f];
     jobs[f].z_off = z;
     jobs[f].pad = 0;
     jobs[f].d_off = (long long)d;
-    d += (size_t)n * n;
+    if (!grid) d += (size_t)n * n;
     z += n > 1 ? n - 1 : 0;
   }
+  double* P = nullptr;
+  const size_t p_bytes = linkage_grid_bytes(row_offsets, nfiles, grid_min);
+  if (p_bytes) {
+    const cudaError_t e = cudaMallocAsync((void**)&P, p_bytes, st);
+    if (e != cudaSuccess) {
+      cudaGetLastError();
+      int nmax = 0;
+      for (int f : big) nmax = std::max(nmax, row_offsets[f + 1] - row_offsets[f]);
+      set_error("linkage: %d observations need %llu bytes of device memory for their packed distances "
+                "(4 n (n - 1)): %s", nmax, (unsigned long long)p_bytes, cudaGetErrorString(e));
+      return e == cudaErrorMemoryAllocation ? B200_ERR_OOM : B200_ERR_CUDA;
+    }
+  }
+  StreamFree free_p{P, st};              // every return below releases the packed distances
   char* p = (char*)ws;
   double* D = (double*)p; p += align_up(d * 8, 256);
   double* xn = (double*)p; p += align_up((size_t)ntot * dim * 8, 256);
@@ -652,7 +821,7 @@ int linkage_centroid_batched(const double* x, const int* row_offsets, int nfiles
     const int n = jobs[f].n;
     if (n < 2) continue;
     dim3 grid(ceil_div(n, 16), ceil_div(n, 16));
-    pdist_kernel<<<grid, dim3(16, 16), 0, st>>>(src + (size_t)jobs[f].row_off * dim, D + jobs[f].d_off, n, dim);
+    pdist_kernel<false><<<grid, dim3(16, 16), 0, st>>>(src + (size_t)jobs[f].row_off * dim, D + jobs[f].d_off, n, dim);
   }
   static bool link_attr = false;
   const size_t link_smem_bytes = (size_t)kLinkSmemRows * 17;
@@ -663,6 +832,33 @@ int linkage_centroid_batched(const double* x, const int* row_offsets, int nfiles
   }
   linkage_centroid_kernel<<<nfiles, 1024, link_smem_bytes, st>>>(djobs, D, Z, nn_d, nn_i, size, id, alive, todo);
   B200_CUDA_OK(cudaGetLastError());
+  if (big.empty()) return B200_OK;
+
+  // large problems, one after another: packed distances, then a cooperative grid of one CTA per SM
+  MinPair* part = (MinPair*)(p + align_up((size_t)nfiles * sizeof(LinkJob), 256));
+  int* ntodo = (int*)(part + 2 * kLinkGridMaxCtas);
+  int dev = 0, sms = 0, per_sm = 0;
+  B200_CUDA_OK(cudaGetDevice(&dev));
+  B200_CUDA_OK(cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev));
+  B200_CUDA_OK(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, linkage_centroid_grid_kernel, kLinkGridThreads, 0));
+  B200_CHECK(per_sm >= 1, B200_ERR_CUDA, "linkage: the whole-GPU kernel does not fit on an SM");
+  const int nb = std::min(sms, kLinkGridMaxCtas);
+  for (int f : big) {
+    int n = row_offsets[f + 1] - row_offsets[f];
+    dim3 grid(ceil_div(n, 16), ceil_div(n, 16));
+    pdist_kernel<true><<<grid, dim3(16, 16), 0, st>>>(src + (size_t)row_offsets[f] * dim, P, n, dim);
+    B200_CUDA_OK(cudaGetLastError());
+    double* Zf = Z + (size_t)jobs[f].z_off * 4;
+    const int ro = row_offsets[f];
+    double* nn_d_f = nn_d + ro;
+    int *nn_i_f = nn_i + ro, *size_f = size + ro, *id_f = id + ro, *todo_f = todo + ro + f;
+    unsigned char* alive_f = alive + ro;
+    void* args[] = {&P, &n, &Zf, &nn_d_f, &nn_i_f, &size_f, &id_f, &alive_f, &todo_f, &ntodo, &part};
+    B200_CUDA_OK(cudaLaunchCooperativeKernel((const void*)linkage_centroid_grid_kernel, dim3(nb),
+                                             dim3(kLinkGridThreads), args, 0, st));
+  }
+  free_p.p = nullptr;
+  B200_CUDA_OK(cudaFreeAsync(P, st));
   return B200_OK;
 }
 

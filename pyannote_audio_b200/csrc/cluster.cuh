@@ -1,9 +1,14 @@
 #pragma once
 #include "common.cuh"
 namespace b200 {
-size_t linkage_workspace_bytes_batched(const int* row_offsets, int nfiles, int dim);
+// problems of at least this many observations take the whole-GPU linkage path (packed distances allocated per call);
+// smaller ones the batched one-CTA-per-problem kernel with a dense matrix in the workspace
+constexpr int kLinkGridMinDefault = 32769;
+constexpr int kLinkMaxRows = 1048560;          // 65535 tiles of 16 rows in the distance kernel's grid
+size_t linkage_workspace_bytes_batched(const int* row_offsets, int nfiles, int dim, int grid_min);
+size_t linkage_grid_bytes(const int* row_offsets, int nfiles, int grid_min);
 int linkage_centroid_batched(const double* x, const int* row_offsets, int nfiles, int dim, int normalize, double* Z,
-                             void* ws, cudaStream_t st);
+                             void* ws, cudaStream_t st, int grid_min);
 int plda_transform(const double* x, int n, int Din, int Dout, int L, const double* mean1, const double* mean2,
                    const double* lda, const double* mu, const double* trT, double* fea, cudaStream_t st);
 int weighted_centroids(const double* q, int n, int S, const int* kept, int K, const double* train, int dim,

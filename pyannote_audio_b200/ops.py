@@ -738,6 +738,17 @@ def weighted_centroids(self, q: torch.Tensor, kept: torch.Tensor, train: torch.T
     return out
 
 
+def _linkage_check(call):
+    """Runs a linkage ABI call.  A file above 32 768 observations allocates its packed distances outside torch's
+    caching allocator, so memory torch holds cached (e.g. from the segmentation and embedding of that same file) cannot
+    serve it: on an allocation failure the cache is returned to the device and the call made once more."""
+    try:
+        _lib.check(call())
+    except MemoryError:
+        torch.cuda.empty_cache()
+        _lib.check(call())
+
+
 @_ctx_method
 def linkage_centroid(self, x: torch.Tensor, normalize=True) -> torch.Tensor:
     """x (n, dim) float64 on device -> Z (n-1, 4) float64 on device (scipy linkage format)."""
@@ -745,8 +756,8 @@ def linkage_centroid(self, x: torch.Tensor, normalize=True) -> torch.Tensor:
     x = x.contiguous()
     Z = torch.empty((n - 1, 4), dtype=torch.float64, device=self.device)
     with torch.cuda.device(self.device):
-        _lib.check(self.lib.b200_linkage_centroid(self._h, _ptr(x), n, dim, _norm_mode(normalize), _ptr(Z),
-                                                  _stream(self.device)))
+        _linkage_check(lambda: self.lib.b200_linkage_centroid(self._h, _ptr(x), n, dim, _norm_mode(normalize),
+                                                              _ptr(Z), _stream(self.device)))
     return Z
 
 
@@ -805,9 +816,20 @@ def linkage_centroid_batched(self, x: torch.Tensor, row_offsets, normalize=True)
     nz = int(np.maximum(np.diff(ro) - 1, 0).sum())
     Z = torch.empty((nz, 4), dtype=torch.float64, device=self.device)
     with torch.cuda.device(self.device):
-        _lib.check(self.lib.b200_linkage_centroid_batched(self._h, _ptr(x), ro.ctypes.data, len(ro) - 1, x.shape[1],
-                                                          _norm_mode(normalize), _ptr(Z), _stream(self.device)))
+        _linkage_check(lambda: self.lib.b200_linkage_centroid_batched(self._h, _ptr(x), ro.ctypes.data, len(ro) - 1,
+                                                                      x.shape[1], _norm_mode(normalize), _ptr(Z),
+                                                                      _stream(self.device)))
     return Z
+
+
+def linkage_bytes(row_offsets, dim: int) -> int:
+    """Device bytes ``linkage_centroid_batched`` needs for these problems (host only, no device): the workspace it grows
+    to plus the per-call packed distances of its largest problem above 32 768 observations."""
+    ro = np.ascontiguousarray(row_offsets, dtype=np.int32)
+    nbytes = int(_lib.load().b200_linkage_bytes(ro.ctypes.data, len(ro) - 1, int(dim)))
+    if nbytes <= 0:
+        _lib.check(nbytes)
+    return nbytes
 
 
 @_ctx_method
