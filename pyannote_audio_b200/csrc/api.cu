@@ -94,6 +94,19 @@ int upload(b200_ctx* ctx, const std::vector<T>& h, T** out) {
   return B200_OK;
 }
 
+// operand of gemm_tc_split and the wgmma kernels: an fp32 array, already in its device layout with zeros in the
+// padding, uploaded as fp16 (hi, lo) with hi = fp16(v), lo = fp16(v - hi)
+int upload_split(b200_ctx* ctx, const std::vector<float>& h, __half** hi, __half** lo) {
+  std::vector<__half> vh(h.size()), vl(h.size());
+  for (size_t i = 0; i < h.size(); ++i) {
+    vh[i] = __float2half(h[i]);
+    vl[i] = __float2half(h[i] - __half2float(vh[i]));
+  }
+  int rc;
+  if ((rc = upload(ctx, vh, hi))) return rc;
+  return upload(ctx, vl, lo);
+}
+
 cudaEvent_t take_event(b200_ctx* ctx) {
   if (!ctx->event_pool.empty()) {
     cudaEvent_t e = ctx->event_pool.back();
@@ -278,6 +291,29 @@ int make_conv(b200_ctx* ctx, const b200_conv_bn& src, int cin, int cout, int k, 
   return B200_OK;
 }
 
+// the WeSpeaker stem (resnet.conv1 1 -> 32 channels, 3 x 3) with resnet.bn1 folded in, fp32 for conv1_forward
+int load_stem(b200_ctx* ctx, const b200_conv_bn& s, EmbWeights* E) {
+  B200_CHECK(s.conv_weight && s.bn_weight && s.bn_bias && s.bn_mean && s.bn_var, B200_ERR_INVALID, "stem missing");
+  std::vector<float> cw(32 * 9), cb(32);
+  for (int c = 0; c < 32; ++c) {
+    const float sc = s.bn_weight[c] / std::sqrt(s.bn_var[c] + 1e-5f);
+    cb[c] = s.bn_bias[c] - s.bn_mean[c] * sc;
+    for (int k = 0; k < 9; ++k) cw[c * 9 + k] = s.conv_weight[c * 9 + k] * sc;
+  }
+  int rc;
+  if ((rc = upload(ctx, cw, &E->conv1_w))) return rc;
+  return upload(ctx, cb, &E->conv1_b);
+}
+
+// the WeSpeaker resnet.seg_1 Linear (K = 20 C inputs -> 256), fp32 and split for gemm_tc_split
+int load_seg1(b200_ctx* ctx, const float* weight, const float* bias, size_t K, EmbWeights* E) {
+  std::vector<float> sw(weight, weight + (size_t)kEmbDim * K), sb(bias, bias + kEmbDim);
+  int rc;
+  if ((rc = upload_split(ctx, sw, &E->seg1_w_hi, &E->seg1_w_lo))) return rc;
+  if ((rc = upload(ctx, sw, &E->seg1_w))) return rc;
+  return upload(ctx, sb, &E->seg1_b);
+}
+
 // the SincNet half of a loader (sincnet.wav_norm1d, the ParamSincFB bank, sincnet.norm1d.*, sincnet.conv1d.{1,2}) in
 // the layouts of both implementations; PyanNet and XVectorSincNet share it
 int load_sincnet(b200_ctx* ctx, float wav_w, float wav_b, const float* sinc_filters, const float* const norm_weight[3],
@@ -305,16 +341,10 @@ int load_sincnet(b200_ctx* ctx, float wav_w, float wav_b, const float* sinc_filt
       f[125 * 80 + ch] = ch < 40 ? r[125] : 0.f;
     }
     if ((rc = upload(ctx, f, &S.sinc_f))) return rc;
-    std::vector<__half> hi((size_t)80 * 256, __float2half(0.f)), lo(hi.size(), __float2half(0.f));
+    std::vector<float> wg((size_t)80 * 256, 0.f);          // wgmma layout: [80][256], taps zero padded
     for (int ch = 0; ch < 80; ++ch)
-      for (int k = 0; k < 251; ++k) {
-        const float v = sinc_filters[ch * 251 + k];
-        const size_t o = (size_t)ch * 256 + k;
-        hi[o] = __float2half(v);
-        lo[o] = __float2half(v - __half2float(hi[o]));
-      }
-    if ((rc = upload(ctx, hi, &S.sinc_wg_hi))) return rc;
-    if ((rc = upload(ctx, lo, &S.sinc_wg_lo))) return rc;
+      for (int k = 0; k < 251; ++k) wg[(size_t)ch * 256 + k] = sinc_filters[ch * 251 + k];
+    if ((rc = upload_split(ctx, wg, &S.sinc_wg_hi, &S.sinc_wg_lo))) return rc;
   }
   const int nch[3] = {80, 60, 60};
   for (int i = 0; i < 3; ++i) {
@@ -326,26 +356,19 @@ int load_sincnet(b200_ctx* ctx, float wav_w, float wav_b, const float* sinc_filt
   const int cin[2] = {80, 60};
   for (int i = 0; i < 2; ++i) {
     B200_CHECK(conv_weight[i] && conv_bias[i], B200_ERR_INVALID, "conv1d.%d missing", i + 1);
-    std::vector<float> wc((size_t)cin[i] * 5 * 60), bc(conv_bias[i], conv_bias[i] + 60);
+    // wgmma layout: [64 rows = c_out][k = tap * Cpad + c_in], Cpad = 80 | 64, padding zero
+    const int cpad = i == 0 ? 80 : 64, K = 5 * cpad;
+    std::vector<float> wc((size_t)cin[i] * 5 * 60), wg((size_t)64 * K, 0.f), bc(conv_bias[i], conv_bias[i] + 60);
     for (int co = 0; co < 60; ++co)
       for (int ci = 0; ci < cin[i]; ++ci)
-        for (int k = 0; k < 5; ++k) wc[((size_t)ci * 5 + k) * 60 + co] = conv_weight[i][((size_t)co * cin[i] + ci) * 5 + k];
+        for (int k = 0; k < 5; ++k) {
+          const float v = conv_weight[i][((size_t)co * cin[i] + ci) * 5 + k];
+          wc[((size_t)ci * 5 + k) * 60 + co] = v;
+          wg[(size_t)co * K + k * cpad + ci] = v;
+        }
     if ((rc = upload(ctx, wc, &S.conv_w[i]))) return rc;
     if ((rc = upload(ctx, bc, &S.conv_b[i]))) return rc;
-    {   // wgmma layout: [64 rows = c_out][k = tap * Cpad + c_in], Cpad = 80 | 64, padding zero
-      const int cpad = i == 0 ? 80 : 64, K = 5 * cpad;
-      std::vector<__half> hi((size_t)64 * K, __float2half(0.f)), lo(hi.size(), __float2half(0.f));
-      for (int co = 0; co < 60; ++co)
-        for (int ci = 0; ci < cin[i]; ++ci)
-          for (int k = 0; k < 5; ++k) {
-            const float v = conv_weight[i][((size_t)co * cin[i] + ci) * 5 + k];
-            const size_t o = (size_t)co * K + k * cpad + ci;
-            hi[o] = __float2half(v);
-            lo[o] = __float2half(v - __half2float(hi[o]));
-          }
-      if ((rc = upload(ctx, hi, &S.conv_wg_hi[i]))) return rc;
-      if ((rc = upload(ctx, lo, &S.conv_wg_lo[i]))) return rc;
-    }
+    if ((rc = upload_split(ctx, wg, &S.conv_wg_hi[i], &S.conv_wg_lo[i]))) return rc;
   }
   return B200_OK;
 }
@@ -529,48 +552,27 @@ int b200_seg_load_head(b200_ctx* ctx, const b200_seg_weights* w, int32_t num_cla
                 whh[(((size_t)(d * 2 + r) * 128 + k) * 256) + p * 128 + tx * 4 + gt] = Wh[(size_t)(gt * 128 + unit) * 128 + k];
               }
     }
-    {
-      std::vector<__half> hi(wih.size()), lo(wih.size());
-      for (size_t i = 0; i < wih.size(); ++i) {
-        hi[i] = __float2half(wih[i]);
-        lo[i] = __float2half(wih[i] - __half2float(hi[i]));
-      }
-      if ((rc = upload(ctx, hi, &S.w_ih_hi[l]))) return rc;
-      if ((rc = upload(ctx, lo, &S.w_ih_lo[l]))) return rc;
-    }
+    if ((rc = upload_split(ctx, wih, &S.w_ih_hi[l], &S.w_ih_lo[l]))) return rc;
     if ((rc = upload(ctx, wih, &S.w_ih[l]))) return rc;
     if ((rc = upload(ctx, bg, &S.b_g[l]))) return rc;
     if ((rc = upload(ctx, whh, &S.w_hh[l]))) return rc;
-    {   // wgmma recurrence: [dir][rank][n = 32 jj + 8 gate + u][k = unit 0..127], local unit 8 jj + u, as fp16 (hi, lo)
-      std::vector<__half> hi((size_t)4 * 256 * 128), lo(hi.size());
-      for (int d = 0; d < 2; ++d)
-        for (int r = 0; r < 2; ++r)
-          for (int n = 0; n < 256; ++n) {
-            const int unit = 64 * r + 8 * (n / 32) + n % 8, gt = (n / 8) % 4;
-            for (int k = 0; k < 128; ++k) {
-              const float v = w->lstm_w_hh[l * 2 + d][(size_t)(gt * 128 + unit) * 128 + k];
-              const size_t o = ((size_t)(d * 2 + r) * 256 + n) * 128 + k;
-              hi[o] = __float2half(v);
-              lo[o] = __float2half(v - __half2float(hi[o]));
-            }
-          }
-      if ((rc = upload(ctx, hi, &S.w_hh_hi[l]))) return rc;
-      if ((rc = upload(ctx, lo, &S.w_hh_lo[l]))) return rc;
-    }
+    // wgmma recurrence: [dir][rank][n = 32 jj + 8 gate + u][k = unit 0..127], local unit 8 jj + u
+    std::vector<float> whh_wg((size_t)4 * 256 * 128);
+    for (int d = 0; d < 2; ++d)
+      for (int r = 0; r < 2; ++r)
+        for (int n = 0; n < 256; ++n) {
+          const int unit = 64 * r + 8 * (n / 32) + n % 8, gt = (n / 8) % 4;
+          for (int k = 0; k < 128; ++k)
+            whh_wg[((size_t)(d * 2 + r) * 256 + n) * 128 + k] =
+                w->lstm_w_hh[l * 2 + d][(size_t)(gt * 128 + unit) * 128 + k];
+        }
+    if ((rc = upload_split(ctx, whh_wg, &S.w_hh_hi[l], &S.w_hh_lo[l]))) return rc;
   }
   const int lin_in[2] = {256, 128};
   for (int i = 0; i < 2; ++i) {
     B200_CHECK(w->linear_weight[i] && w->linear_bias[i], B200_ERR_INVALID, "linear.%d missing", i);
     std::vector<float> lw(w->linear_weight[i], w->linear_weight[i] + 128 * lin_in[i]), lb(w->linear_bias[i], w->linear_bias[i] + 128);
-    {
-      std::vector<__half> hi(lw.size()), lo(lw.size());
-      for (size_t j = 0; j < lw.size(); ++j) {
-        hi[j] = __float2half(lw[j]);
-        lo[j] = __float2half(lw[j] - __half2float(hi[j]));
-      }
-      if ((rc = upload(ctx, hi, &S.lin_w_hi[i]))) return rc;
-      if ((rc = upload(ctx, lo, &S.lin_w_lo[i]))) return rc;
-    }
+    if ((rc = upload_split(ctx, lw, &S.lin_w_hi[i], &S.lin_w_lo[i]))) return rc;
     if ((rc = upload(ctx, lw, &S.lin_w[i]))) return rc;
     if ((rc = upload(ctx, lb, &S.lin_b[i]))) return rc;
   }
@@ -595,18 +597,7 @@ int b200_emb_load(b200_ctx* ctx, const b200_emb_weights* w) {
   E.loaded = false;
   release_weights(ctx, &ctx->owned_emb);
   if ((rc = build_fbank_constants(ctx))) return rc;
-  {
-    const b200_conv_bn& s = w->stem;
-    B200_CHECK(s.conv_weight && s.bn_weight && s.bn_bias && s.bn_mean && s.bn_var, B200_ERR_INVALID, "stem missing");
-    std::vector<float> cw(32 * 9), cb(32);
-    for (int c = 0; c < 32; ++c) {
-      const float sc = s.bn_weight[c] / std::sqrt(s.bn_var[c] + 1e-5f);
-      cb[c] = s.bn_bias[c] - s.bn_mean[c] * sc;
-      for (int k = 0; k < 9; ++k) cw[c * 9 + k] = s.conv_weight[c * 9 + k] * sc;
-    }
-    if ((rc = upload(ctx, cw, &E.conv1_w))) return rc;
-    if ((rc = upload(ctx, cb, &E.conv1_b))) return rc;
-  }
+  if ((rc = load_stem(ctx, w->stem, &E))) return rc;
   E.blocks.clear();
   E.bottlenecks.clear();
   E.C = 256;
@@ -625,18 +616,7 @@ int b200_emb_load(b200_ctx* ctx, const b200_emb_weights* w) {
       E.blocks.push_back(B);
     }
   B200_CHECK(w->seg1_weight && w->seg1_bias, B200_ERR_INVALID, "seg_1 missing");
-  std::vector<float> sw(w->seg1_weight, w->seg1_weight + (size_t)256 * 5120), sb(w->seg1_bias, w->seg1_bias + 256);
-  {
-    std::vector<__half> hi(sw.size()), lo(sw.size());
-    for (size_t i = 0; i < sw.size(); ++i) {
-      hi[i] = __float2half(sw[i]);
-      lo[i] = __float2half(sw[i] - __half2float(hi[i]));
-    }
-    if ((rc = upload(ctx, hi, &E.seg1_w_hi))) return rc;
-    if ((rc = upload(ctx, lo, &E.seg1_w_lo))) return rc;
-  }
-  if ((rc = upload(ctx, sw, &E.seg1_w))) return rc;
-  if ((rc = upload(ctx, sb, &E.seg1_b))) return rc;
+  if ((rc = load_seg1(ctx, w->seg1_weight, w->seg1_bias, 5120, &E))) return rc;
   E.loaded = true;
   return B200_OK;
 }
@@ -671,18 +651,7 @@ int b200_emb_load_bottleneck(b200_ctx* ctx, const b200_emb_bottleneck_weights* w
   E.bottlenecks.clear();
   E.C = 1024;
   if ((rc = build_fbank_constants(ctx))) return rc;
-  {
-    const b200_conv_bn& s = w->stem;
-    B200_CHECK(s.conv_weight && s.bn_weight && s.bn_bias && s.bn_mean && s.bn_var, B200_ERR_INVALID, "stem missing");
-    std::vector<float> cw(32 * 9), cb(32);
-    for (int c = 0; c < 32; ++c) {
-      const float sc = s.bn_weight[c] / std::sqrt(s.bn_var[c] + 1e-5f);
-      cb[c] = s.bn_bias[c] - s.bn_mean[c] * sc;
-      for (int k = 0; k < 9; ++k) cw[c * 9 + k] = s.conv_weight[c * 9 + k] * sc;
-    }
-    if ((rc = upload(ctx, cw, &E.conv1_w))) return rc;
-    if ((rc = upload(ctx, cb, &E.conv1_b))) return rc;
-  }
+  if ((rc = load_stem(ctx, w->stem, &E))) return rc;
   int in_planes = 32, bi = 0;
   for (int l = 0; l < 4; ++l)
     for (int i = 0; i < w->num_blocks[l]; ++i, ++bi) {
@@ -697,19 +666,7 @@ int b200_emb_load_bottleneck(b200_ctx* ctx, const b200_emb_bottleneck_weights* w
       in_planes = 4 * p;
       E.bottlenecks.push_back(B);
     }
-  const size_t K = (size_t)2 * 10 * E.C;
-  std::vector<float> sw(w->seg1_weight, w->seg1_weight + (size_t)kEmbDim * K), sb(w->seg1_bias, w->seg1_bias + kEmbDim);
-  {
-    std::vector<__half> hi(sw.size()), lo(sw.size());
-    for (size_t i = 0; i < sw.size(); ++i) {
-      hi[i] = __float2half(sw[i]);
-      lo[i] = __float2half(sw[i] - __half2float(hi[i]));
-    }
-    if ((rc = upload(ctx, hi, &E.seg1_w_hi))) return rc;
-    if ((rc = upload(ctx, lo, &E.seg1_w_lo))) return rc;
-  }
-  if ((rc = upload(ctx, sw, &E.seg1_w))) return rc;
-  if ((rc = upload(ctx, sb, &E.seg1_b))) return rc;
+  if ((rc = load_seg1(ctx, w->seg1_weight, w->seg1_bias, (size_t)2 * 10 * E.C, &E))) return rc;
   E.loaded = true;
   return B200_OK;
 }
@@ -856,26 +813,20 @@ struct EmbWs {
 // (every later layer is half the size of layer 1 at the same width): A and D the 4p = 128 channels of layer 1, Bf
 // layer 2 block 0's conv1 output (64 channels at layer 1's resolution), Cf layer 1's conv2 output (32 channels).
 static size_t carve_emb(const EmbWeights& E, int NB, void* base, EmbWs* w) {
-  size_t off = 0;
-  auto take = [&](size_t bytes) {
-    off = align_up(off, 1024);
-    void* p = base ? (char*)base + off : nullptr;
-    off += bytes;
-    return p;
-  };
+  Workspace ws(base, 1024);
   EmbWs t;
   const size_t act = (size_t)NB * kMel * kFbankFrames * 32 * sizeof(__half);   // largest activation (layer1)
-  t.fbank = (float*)take((size_t)NB * kFbankFrames * kMel * sizeof(float));
-  t.fmean = (float*)take((size_t)NB * kMel * sizeof(float));
-  t.stats = (float*)take((size_t)NB * kSpeakers * 2 * 10 * E.C * sizeof(float));
+  t.fbank = (float*)ws.take((size_t)NB * kFbankFrames * kMel * sizeof(float));
+  t.fmean = (float*)ws.take((size_t)NB * kMel * sizeof(float));
+  t.stats = (float*)ws.take((size_t)NB * kSpeakers * 2 * 10 * E.C * sizeof(float));
   const bool bn = !E.bottlenecks.empty();
-  t.A = (__half*)take(bn ? 4 * act : act);
-  t.Bf = (__half*)take(bn ? 2 * act : act);
-  t.Cf = (__half*)take(act);
-  t.D = bn ? (__half*)take(4 * act) : nullptr;
+  t.A = (__half*)ws.take(bn ? 4 * act : act);
+  t.Bf = (__half*)ws.take(bn ? 2 * act : act);
+  t.Cf = (__half*)ws.take(act);
+  t.D = bn ? (__half*)ws.take(4 * act) : nullptr;
   t.cf_bytes = act;
   if (w) *w = t;
-  return align_up(off, 1024);
+  return ws.bytes();
 }
 
 // one BasicBlock on nb segments: A -> (Bf, Cf) -> A, in place on the residual
@@ -1212,22 +1163,16 @@ int b200_xvec_load(b200_ctx* ctx, const b200_xvec_weights* w) {
   const int cin[kXvecLayers] = {60, 512, 512, 512, 512}, cout[kXvecLayers] = {512, 512, 512, 512, 1500};
   for (int l = 0; l < kXvecLayers; ++l) {
     const int k = X.taps[l], cp = X.cin_pad[l], np = X.cout_pad[l], K = k * cp;
-    std::vector<__half> hi((size_t)np * K, __float2half(0.f)), lo(hi.size(), __float2half(0.f));
-    std::vector<float> bias(np, 0.f), scale(np, 0.f), shift(np, 0.f);
+    std::vector<float> wt((size_t)np * K, 0.f), bias(np, 0.f), scale(np, 0.f), shift(np, 0.f);
     for (int co = 0; co < cout[l]; ++co) {
       for (int ci = 0; ci < cin[l]; ++ci)
-        for (int j = 0; j < k; ++j) {
-          const float v = w->tdnn_weight[l][((size_t)co * cin[l] + ci) * k + j];
-          const size_t o = (size_t)co * K + j * cp + ci;
-          hi[o] = __float2half(v);
-          lo[o] = __float2half(v - __half2float(hi[o]));
-        }
+        for (int j = 0; j < k; ++j)
+          wt[(size_t)co * K + j * cp + ci] = w->tdnn_weight[l][((size_t)co * cin[l] + ci) * k + j];
       bias[co] = w->tdnn_bias[l][co];
       scale[co] = w->bn_weight[l][co] / std::sqrt(w->bn_var[l][co] + 1e-5f);
       shift[co] = w->bn_bias[l][co] - w->bn_mean[l][co] * scale[co];
     }
-    if ((rc = upload(ctx, hi, &X.w_hi[l]))) return rc;
-    if ((rc = upload(ctx, lo, &X.w_lo[l]))) return rc;
+    if ((rc = upload_split(ctx, wt, &X.w_hi[l], &X.w_lo[l]))) return rc;
     if ((rc = upload(ctx, bias, &X.bias[l]))) return rc;
     if ((rc = upload(ctx, scale, &X.scale[l]))) return rc;
     if ((rc = upload(ctx, shift, &X.shift[l]))) return rc;
@@ -1235,19 +1180,12 @@ int b200_xvec_load(b200_ctx* ctx, const b200_xvec_weights* w) {
   X.dim = w->dimension;
   X.dim_pad = (int)ceil_div(X.dim, 128) * 128;
   {
-    std::vector<__half> hi((size_t)X.dim_pad * kXvecStatsLd, __float2half(0.f)), lo(hi.size(), __float2half(0.f));
-    std::vector<float> b(X.dim_pad, 0.f);
+    std::vector<float> ew((size_t)X.dim_pad * kXvecStatsLd, 0.f), b(X.dim_pad, 0.f);
     for (int n = 0; n < X.dim; ++n) {
-      for (int kk = 0; kk < 3000; ++kk) {
-        const float v = w->embedding_weight[(size_t)n * 3000 + kk];
-        const size_t o = (size_t)n * kXvecStatsLd + kk;
-        hi[o] = __float2half(v);
-        lo[o] = __float2half(v - __half2float(hi[o]));
-      }
+      for (int kk = 0; kk < 3000; ++kk) ew[(size_t)n * kXvecStatsLd + kk] = w->embedding_weight[(size_t)n * 3000 + kk];
       b[n] = w->embedding_bias[n];
     }
-    if ((rc = upload(ctx, hi, &X.emb_hi))) return rc;
-    if ((rc = upload(ctx, lo, &X.emb_lo))) return rc;
+    if ((rc = upload_split(ctx, ew, &X.emb_hi, &X.emb_lo))) return rc;
     if ((rc = upload(ctx, b, &X.emb_b))) return rc;
   }
   X.loaded = true;
@@ -1265,27 +1203,21 @@ struct XvecWs {
   double* part;
 };
 static size_t carve_xvec(const SegGeom& g, int nb, int S, void* base, XvecWs* w) {
-  size_t off = 0;
-  auto take = [&](size_t bytes) {
-    off = align_up(off, 1024);
-    void* p = base ? (char*)base + off : nullptr;
-    off += bytes;
-    return p;
-  };
+  Workspace ws(base, 1024);
   const size_t M = (size_t)nb * g.pool2;
   XvecWs t;
-  t.x0 = (float*)take(M * 64 * sizeof(float));
-  t.xh = (__half*)take(M * 64 * sizeof(__half));
-  t.xl = (__half*)take(M * 64 * sizeof(__half));
-  t.ph = (__half*)take(M * 512 * sizeof(__half));
-  t.pl = (__half*)take(M * 512 * sizeof(__half));
-  t.qh = (__half*)take(M * 512 * sizeof(__half));
-  t.ql = (__half*)take(M * 512 * sizeof(__half));
-  t.y = (float*)take(std::max(M * kPoolRowsLd * sizeof(float), sincnet_workspace_bytes(g, nb)));
+  t.x0 = (float*)ws.take(M * 64 * sizeof(float));
+  t.xh = (__half*)ws.take(M * 64 * sizeof(__half));
+  t.xl = (__half*)ws.take(M * 64 * sizeof(__half));
+  t.ph = (__half*)ws.take(M * 512 * sizeof(__half));
+  t.pl = (__half*)ws.take(M * 512 * sizeof(__half));
+  t.qh = (__half*)ws.take(M * 512 * sizeof(__half));
+  t.ql = (__half*)ws.take(M * 512 * sizeof(__half));
+  t.y = (float*)ws.take(std::max(M * kPoolRowsLd * sizeof(float), sincnet_workspace_bytes(g, nb)));
   t.sinc = t.y;
-  t.part = (double*)take(pool_scratch_bytes(nb, S, g.pool2 - 14, kPoolRowsLd, 1));
+  t.part = (double*)ws.take(pool_scratch_bytes(nb, S, g.pool2 - 14, kPoolRowsLd, 1));
   if (w) *w = t;
-  return align_up(off, 1024);
+  return ws.bytes();
 }
 
 int b200_xvec_forward(b200_ctx* ctx, const float* wav, const int64_t* off, int64_t num_samples, int32_t num_utts,

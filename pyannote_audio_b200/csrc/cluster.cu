@@ -823,13 +823,9 @@ int linkage_centroid_batched(const double* x, const int* row_offsets, int nfiles
     dim3 grid(ceil_div(n, 16), ceil_div(n, 16));
     pdist_kernel<false><<<grid, dim3(16, 16), 0, st>>>(src + (size_t)jobs[f].row_off * dim, D + jobs[f].d_off, n, dim);
   }
-  static bool link_attr = false;
   const size_t link_smem_bytes = (size_t)kLinkSmemRows * 17;
-  if (!link_attr) {
-    B200_CUDA_OK(cudaFuncSetAttribute(linkage_centroid_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize,
-                                      (int)link_smem_bytes));
-    link_attr = true;
-  }
+  B200_CUDA_OK(cudaFuncSetAttribute(linkage_centroid_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize,
+                                    (int)link_smem_bytes));
   linkage_centroid_kernel<<<nfiles, 1024, link_smem_bytes, st>>>(djobs, D, Z, nn_d, nn_i, size, id, alive, todo);
   B200_CUDA_OK(cudaGetLastError());
   if (big.empty()) return B200_OK;

@@ -85,18 +85,21 @@ __device__ __forceinline__ void ffma2(f32x2_t& d, f32x2_t a, f32x2_t b) {   // d
 inline int ceil_div(int a, int b) { return (a + b - 1) / b; }
 inline size_t align_up(size_t x, size_t a) { return (x + a - 1) / a * a; }
 
-// Bump allocator over one cudaMalloc'd workspace (owned by the ctx; kernels never allocate).
+// Bump allocator that carves the buffers of one launch sequence out of the ctx's workspace (kernels never
+// allocate), each buffer starting on an `align`-byte boundary.  With a null base it only measures: take() returns
+// nullptr and bytes() is what the layout needs.
 struct Workspace {
-  char* base = nullptr;
-  size_t cap = 0;
+  char* base;
+  size_t align;
   size_t off = 0;
-  void reset() { off = 0; }
-  void* take(size_t bytes) {
-    size_t o = align_up(off, 1024);
-    if (o + bytes > cap) return nullptr;
-    off = o + bytes;
-    return base + o;
+  Workspace(void* b, size_t a) : base(static_cast<char*>(b)), align(a) {}
+  void* take(size_t n) {
+    off = align_up(off, align);
+    void* p = base ? base + off : nullptr;
+    off += n;
+    return p;
   }
+  size_t bytes() const { return align_up(off, align); }
 };
 
 }  // namespace b200

@@ -406,7 +406,11 @@ __global__ void __launch_bounds__(kC1Tile) conv1_kernel(const float* __restrict_
 // ------------------------------------------------------------------------------------------------
 // host side
 // ------------------------------------------------------------------------------------------------
-PFN_encodeTiled get_encode() {
+typedef CUresult (*PFN_encodeTiled)(CUtensorMap*, CUtensorMapDataType, cuuint32_t, void*, const cuuint64_t*,
+                                    const cuuint64_t*, const cuuint32_t*, const cuuint32_t*, CUtensorMapInterleave,
+                                    CUtensorMapSwizzle, CUtensorMapL2promotion, CUtensorMapFloatOOBfill);
+
+static PFN_encodeTiled get_encode() {
   static PFN_encodeTiled fn = nullptr;
   if (!fn) {
     void* ptr = nullptr;
@@ -416,6 +420,18 @@ PFN_encodeTiled get_encode() {
       fn = reinterpret_cast<PFN_encodeTiled>(ptr);
   }
   return fn;
+}
+
+int encode_f16_map(CUtensorMap* tm, int rank, const void* ptr, const cuuint64_t* dims, const cuuint64_t* strides,
+                   const cuuint32_t* box, const cuuint32_t* estr, CUtensorMapSwizzle swizzle, const char* what) {
+  PFN_encodeTiled enc = get_encode();
+  B200_CHECK(enc != nullptr, B200_ERR_CUDA, "cuTensorMapEncodeTiled not available from the driver");
+  const cuuint32_t ones[5] = {1, 1, 1, 1, 1};
+  CUresult r = enc(tm, CU_TENSOR_MAP_DATA_TYPE_FLOAT16, (cuuint32_t)rank, const_cast<void*>(ptr), dims, strides, box,
+                   estr ? estr : ones, CU_TENSOR_MAP_INTERLEAVE_NONE, swizzle, CU_TENSOR_MAP_L2_PROMOTION_L2_256B,
+                   CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
+  B200_CHECK(r == CUDA_SUCCESS, B200_ERR_CUDA, "cuTensorMapEncodeTiled(%s) failed: %d", what, (int)r);
+  return B200_OK;
 }
 
 int conv_forward(const ConvLayer& L, const __half* in, const __half* residual, __half* out, int B, int H_in, int W_in,
@@ -481,32 +497,23 @@ int conv_forward(const ConvLayer& L, const __half* in, const __half* residual, _
     B200_CHECK(p.nstages >= 2, B200_ERR_STATE, "conv %d -> %d: shared memory plan too shallow", L.C_in, L.C_out);
     smem = 1024 + 1024 + (size_t)p.nstages * (p.a_bytes + p.b_bytes);
   }
-  PFN_encodeTiled enc = get_encode();
-  B200_CHECK(enc != nullptr, B200_ERR_CUDA, "cuTensorMapEncodeTiled not available from the driver");
+  const CUtensorMapSwizzle swz = p.swizzle == 128 ? CU_TENSOR_MAP_SWIZZLE_128B : CU_TENSOR_MAP_SWIZZLE_64B;
   CUtensorMap tmA, tmB;
+  int rc;
   {
-    cuuint64_t dims[4] = {(cuuint64_t)L.C_in, (cuuint64_t)W_in, (cuuint64_t)H_in, (cuuint64_t)B};
-    cuuint64_t strides[3] = {(cuuint64_t)L.C_in * 2, (cuuint64_t)W_in * L.C_in * 2,
-                             (cuuint64_t)H_in * W_in * L.C_in * 2};
-    cuuint32_t box[4] = {(cuuint32_t)p.Ck, (cuuint32_t)(p.a_rows * L.stride), 1, 1};
-    cuuint32_t estr[4] = {1, (cuuint32_t)L.stride, 1, 1};
-    CUresult r = enc(&tmA, CU_TENSOR_MAP_DATA_TYPE_FLOAT16, 4, const_cast<__half*>(in), dims, strides, box, estr,
-                     CU_TENSOR_MAP_INTERLEAVE_NONE,
-                     p.swizzle == 128 ? CU_TENSOR_MAP_SWIZZLE_128B : CU_TENSOR_MAP_SWIZZLE_64B,
-                     CU_TENSOR_MAP_L2_PROMOTION_L2_256B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
-    B200_CHECK(r == CUDA_SUCCESS, B200_ERR_CUDA, "cuTensorMapEncodeTiled(A) failed: %d", (int)r);
+    const cuuint64_t dims[4] = {(cuuint64_t)L.C_in, (cuuint64_t)W_in, (cuuint64_t)H_in, (cuuint64_t)B};
+    const cuuint64_t strides[3] = {(cuuint64_t)L.C_in * 2, (cuuint64_t)W_in * L.C_in * 2,
+                                   (cuuint64_t)H_in * W_in * L.C_in * 2};
+    const cuuint32_t box[4] = {(cuuint32_t)p.Ck, (cuuint32_t)(p.a_rows * L.stride), 1, 1};
+    const cuuint32_t estr[4] = {1, (cuuint32_t)L.stride, 1, 1};
+    if ((rc = encode_f16_map(&tmA, 4, in, dims, strides, box, estr, swz, "A"))) return rc;
   }
   {
     // conv_row_kernel loads the nine taps as three boxes of three
-    cuuint64_t dims[3] = {(cuuint64_t)L.C_in, (cuuint64_t)L.C_out, (cuuint64_t)(L.ksize * L.ksize)};
-    cuuint64_t strides[2] = {(cuuint64_t)L.C_in * 2, (cuuint64_t)L.C_out * L.C_in * 2};
-    cuuint32_t box[3] = {(cuuint32_t)p.Ck, (cuuint32_t)n_tile, rows ? 3u : 1u};
-    cuuint32_t estr[3] = {1, 1, 1};
-    CUresult r = enc(&tmB, CU_TENSOR_MAP_DATA_TYPE_FLOAT16, 3, const_cast<__half*>(L.w), dims, strides, box, estr,
-                     CU_TENSOR_MAP_INTERLEAVE_NONE,
-                     p.swizzle == 128 ? CU_TENSOR_MAP_SWIZZLE_128B : CU_TENSOR_MAP_SWIZZLE_64B,
-                     CU_TENSOR_MAP_L2_PROMOTION_L2_256B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
-    B200_CHECK(r == CUDA_SUCCESS, B200_ERR_CUDA, "cuTensorMapEncodeTiled(B) failed: %d", (int)r);
+    const cuuint64_t dims[3] = {(cuuint64_t)L.C_in, (cuuint64_t)L.C_out, (cuuint64_t)(L.ksize * L.ksize)};
+    const cuuint64_t strides[2] = {(cuuint64_t)L.C_in * 2, (cuuint64_t)L.C_out * L.C_in * 2};
+    const cuuint32_t box[3] = {(cuuint32_t)p.Ck, (cuuint32_t)n_tile, rows ? 3u : 1u};
+    if ((rc = encode_f16_map(&tmB, 3, L.w, dims, strides, box, nullptr, swz, "B"))) return rc;
   }
   auto launch = [&](auto kernel) -> int {
     B200_CUDA_OK(cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));

@@ -155,20 +155,6 @@ int split_f16(const float* x, __half* hi, __half* lo, size_t n, cudaStream_t st)
   return B200_OK;
 }
 
-static int make_map_2d(CUtensorMap* tm, const __half* ptr, int rows, int K, int ld, int box_rows) {
-  PFN_encodeTiled enc = get_encode();
-  B200_CHECK(enc != nullptr, B200_ERR_CUDA, "cuTensorMapEncodeTiled not available from the driver");
-  cuuint64_t dims[2] = {(cuuint64_t)K, (cuuint64_t)rows};
-  cuuint64_t strides[1] = {(cuuint64_t)ld * 2};
-  cuuint32_t box[2] = {(cuuint32_t)kGemmK, (cuuint32_t)box_rows};
-  cuuint32_t estr[2] = {1, 1};
-  CUresult r = enc(tm, CU_TENSOR_MAP_DATA_TYPE_FLOAT16, 2, const_cast<__half*>(ptr), dims, strides, box, estr,
-                   CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_256B,
-                   CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
-  B200_CHECK(r == CUDA_SUCCESS, B200_ERR_CUDA, "cuTensorMapEncodeTiled(gemm) failed: %d", (int)r);
-  return B200_OK;
-}
-
 int gemm_tc_split(const __half* A_hi, const __half* A_lo, int lda, const __half* B_hi, const __half* B_lo, int ldb,
                   float* C, int ldc, __half* C_hi, __half* C_lo, int ldc_h, const float* bias, int M, int N, int K,
                   int act, int num_sms, cudaStream_t stream, float* const* C_peers, int n_peers,
@@ -195,18 +181,18 @@ int gemm_tc_split(const __half* A_hi, const __half* A_lo, int lda, const __half*
   p.scale = taps.scale;
   p.shift = taps.shift;
   CUtensorMap tmAh, tmAl, tmBh, tmBl;
+  const cuuint64_t a_dims[2] = {(cuuint64_t)Ka, (cuuint64_t)M}, a_str[1] = {(cuuint64_t)lda * 2};
+  const cuuint64_t b_dims[2] = {(cuuint64_t)K, (cuuint64_t)N}, b_str[1] = {(cuuint64_t)ldb * 2};
+  const cuuint32_t a_box[2] = {kGemmK, kGemmM}, b_box[2] = {kGemmK, kGemmN};
+  const CUtensorMapSwizzle swz = CU_TENSOR_MAP_SWIZZLE_128B;
   int rc;
   // rows of the shifted taps past M read as zero (TMA out-of-bounds fill)
-  if ((rc = make_map_2d(&tmAh, A_hi, M, Ka, lda, kGemmM))) return rc;
-  if ((rc = make_map_2d(&tmAl, A_lo, M, Ka, lda, kGemmM))) return rc;
-  if ((rc = make_map_2d(&tmBh, B_hi, N, K, ldb, kGemmN))) return rc;
-  if ((rc = make_map_2d(&tmBl, B_lo, N, K, ldb, kGemmN))) return rc;
+  if ((rc = encode_f16_map(&tmAh, 2, A_hi, a_dims, a_str, a_box, nullptr, swz, "gemm"))) return rc;
+  if ((rc = encode_f16_map(&tmAl, 2, A_lo, a_dims, a_str, a_box, nullptr, swz, "gemm"))) return rc;
+  if ((rc = encode_f16_map(&tmBh, 2, B_hi, b_dims, b_str, b_box, nullptr, swz, "gemm"))) return rc;
+  if ((rc = encode_f16_map(&tmBl, 2, B_lo, b_dims, b_str, b_box, nullptr, swz, "gemm"))) return rc;
   const size_t smem = 1024 + 1024 + (size_t)kGemmStages * kGemmStageBytes;
-  static bool attr_set = false;
-  if (!attr_set) {
-    B200_CUDA_OK(cudaFuncSetAttribute(gemm_tc_split_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-    attr_set = true;
-  }
+  B200_CUDA_OK(cudaFuncSetAttribute(gemm_tc_split_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
   const unsigned grid = (unsigned)(ceil_div(M, kGemmM) * p.tiles_n);
   gemm_tc_split_kernel<<<grid, kGemmThreads, smem, stream>>>(tmAh, tmAl, tmBh, tmBl, p);
   B200_CUDA_OK(cudaGetLastError());

@@ -173,20 +173,6 @@ sinc_conv_wg_kernel(const __grid_constant__ CUtensorMap tmWh, const __grid_const
   }
 }
 
-static int make_w_map(CUtensorMap* tm, const __half* ptr, int rows, int K) {
-  PFN_encodeTiled enc = get_encode();
-  B200_CHECK(enc != nullptr, B200_ERR_CUDA, "cuTensorMapEncodeTiled not available from the driver");
-  cuuint64_t dims[2] = {(cuuint64_t)K, (cuuint64_t)rows};
-  cuuint64_t strides[1] = {(cuuint64_t)K * 2};
-  cuuint32_t box[2] = {64, (cuuint32_t)rows};
-  cuuint32_t estr[2] = {1, 1};
-  CUresult r = enc(tm, CU_TENSOR_MAP_DATA_TYPE_FLOAT16, 2, const_cast<__half*>(ptr), dims, strides, box, estr,
-                   CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_256B,
-                   CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
-  B200_CHECK(r == CUDA_SUCCESS, B200_ERR_CUDA, "cuTensorMapEncodeTiled(sinc/conv weights) failed: %d", (int)r);
-  return B200_OK;
-}
-
 template <int CIN, int CPAD, int NW, int NREAL, int KT>
 static int launch_sc(const __half* Wh, const __half* Wl, SincConvWgParams p, int NB, cudaStream_t stream) {
   constexpr int kIn = CIN == 0 ? (kSCPos - 1) * kSincStride + KT : (kSCPos + 4) * CPAD;
@@ -201,15 +187,15 @@ static int launch_sc(const __half* Wh, const __half* Wl, SincConvWgParams p, int
   const size_t smem = 1024 + p.pool_off + (size_t)NREAL * 65 * sizeof(float);
   B200_CHECK(smem <= 227 * 1024, B200_ERR_STATE, "sinc/conv wgmma kernel: %zu B of shared memory", smem);
   CUtensorMap th, tl;
+  const cuuint64_t dims[2] = {(cuuint64_t)KT, (cuuint64_t)NW}, strides[1] = {(cuuint64_t)KT * 2};
+  const cuuint32_t box[2] = {64, (cuuint32_t)NW};
   int rc;
-  if ((rc = make_w_map(&th, Wh, NW, KT))) return rc;
-  if ((rc = make_w_map(&tl, Wl, NW, KT))) return rc;
+  if ((rc = encode_f16_map(&th, 2, Wh, dims, strides, box, nullptr, CU_TENSOR_MAP_SWIZZLE_128B, "sinc/conv weights")))
+    return rc;
+  if ((rc = encode_f16_map(&tl, 2, Wl, dims, strides, box, nullptr, CU_TENSOR_MAP_SWIZZLE_128B, "sinc/conv weights")))
+    return rc;
   auto kernel = sinc_conv_wg_kernel<CIN, CPAD, NW, NREAL, KT>;
-  static bool attr_set = false;                             // one per instantiation
-  if (!attr_set) {
-    B200_CUDA_OK(cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-    attr_set = true;
-  }
+  B200_CUDA_OK(cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
   kernel<<<dim3(p.ntiles, NB), kSCThreads, smem, stream>>>(th, tl, p);   // one tile per 64 pooled outputs
   B200_CUDA_OK(cudaGetLastError());
   return B200_OK;

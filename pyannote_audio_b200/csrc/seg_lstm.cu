@@ -214,30 +214,24 @@ struct LstmWs {
   __half *Xh, *Xl, *Yah, *Yal, *Ybh, *Ybl, *Z1h, *Z1l;
 };
 static size_t carve_lstm(int NB, int T, void* base, LstmWs* w) {
-  size_t off = 0;
-  auto take = [&](size_t bytes) {
-    off = align_up(off, 256);
-    void* p = base ? (char*)base + off : nullptr;
-    off += bytes;
-    return p;
-  };
+  Workspace ws(base, 256);
   LstmWs t;
   const size_t M = (size_t)NB * T;
-  t.Gx = (float*)take(M * 1024 * sizeof(float));
-  t.Ya = (float*)take(M * 256 * sizeof(float));
-  t.Yb = (float*)take(M * 256 * sizeof(float));
-  t.Z1 = (float*)take(M * 128 * sizeof(float));
-  t.Z2 = (float*)take(M * 128 * sizeof(float));
-  t.Xh = (__half*)take(M * 64 * sizeof(__half));
-  t.Xl = (__half*)take(M * 64 * sizeof(__half));
-  t.Yah = (__half*)take(M * 256 * sizeof(__half));
-  t.Yal = (__half*)take(M * 256 * sizeof(__half));
-  t.Ybh = (__half*)take(M * 256 * sizeof(__half));
-  t.Ybl = (__half*)take(M * 256 * sizeof(__half));
-  t.Z1h = (__half*)take(M * 128 * sizeof(__half));
-  t.Z1l = (__half*)take(M * 128 * sizeof(__half));
+  t.Gx = (float*)ws.take(M * 1024 * sizeof(float));
+  t.Ya = (float*)ws.take(M * 256 * sizeof(float));
+  t.Yb = (float*)ws.take(M * 256 * sizeof(float));
+  t.Z1 = (float*)ws.take(M * 128 * sizeof(float));
+  t.Z2 = (float*)ws.take(M * 128 * sizeof(float));
+  t.Xh = (__half*)ws.take(M * 64 * sizeof(__half));
+  t.Xl = (__half*)ws.take(M * 64 * sizeof(__half));
+  t.Yah = (__half*)ws.take(M * 256 * sizeof(__half));
+  t.Yal = (__half*)ws.take(M * 256 * sizeof(__half));
+  t.Ybh = (__half*)ws.take(M * 256 * sizeof(__half));
+  t.Ybl = (__half*)ws.take(M * 256 * sizeof(__half));
+  t.Z1h = (__half*)ws.take(M * 128 * sizeof(__half));
+  t.Z1l = (__half*)ws.take(M * 128 * sizeof(__half));
   if (w) *w = t;
-  return align_up(off, 256);
+  return ws.bytes();
 }
 size_t lstm_workspace_bytes(int NB, int T) { return carve_lstm(NB, T, nullptr, nullptr); }
 

@@ -161,25 +161,17 @@ lstm_rec_wg_kernel(const __grid_constant__ CUtensorMap tmWh, const __grid_consta
 
 int lstm_rec_wg(const float* Gx, const __half* Wh, const __half* Wl, __half* Yh, __half* Yl, int NB, int T,
                 cudaStream_t stream) {
-  PFN_encodeTiled enc = get_encode();
-  B200_CHECK(enc != nullptr, B200_ERR_CUDA, "cuTensorMapEncodeTiled not available from the driver");
   CUtensorMap tm[2];
-  for (int h = 0; h < 2; ++h) {
-    cuuint64_t dims[3] = {128, 256, 4};                    // [k = unit][n = (unit, gate) column][dir * 2 + rank]
-    cuuint64_t strides[2] = {128 * 2, 256 * 128 * 2};
-    cuuint32_t box[3] = {64, 256, 1};
-    cuuint32_t estr[3] = {1, 1, 1};
-    CUresult r = enc(&tm[h], CU_TENSOR_MAP_DATA_TYPE_FLOAT16, 3, const_cast<__half*>(h ? Wl : Wh), dims, strides, box,
-                     estr, CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_128B,
-                     CU_TENSOR_MAP_L2_PROMOTION_L2_256B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
-    B200_CHECK(r == CUDA_SUCCESS, B200_ERR_CUDA, "cuTensorMapEncodeTiled(lstm W_hh) failed: %d", (int)r);
-  }
+  const cuuint64_t dims[3] = {128, 256, 4};                 // [k = unit][n = (unit, gate) column][dir * 2 + rank]
+  const cuuint64_t strides[2] = {128 * 2, 256 * 128 * 2};
+  const cuuint32_t box[3] = {64, 256, 1};
+  int rc;
+  for (int h = 0; h < 2; ++h)
+    if ((rc = encode_f16_map(&tm[h], 3, h ? Wl : Wh, dims, strides, box, nullptr, CU_TENSOR_MAP_SWIZZLE_128B,
+                             "lstm W_hh")))
+      return rc;
   const size_t smem = 1024 + kRecXOff + 4u * 32u * kRecThreads * 4u;
-  static bool attr_set = false;
-  if (!attr_set) {
-    B200_CUDA_OK(cudaFuncSetAttribute(lstm_rec_wg_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-    attr_set = true;
-  }
+  B200_CUDA_OK(cudaFuncSetAttribute(lstm_rec_wg_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
   const int ntiles = ceil_div(NB, kRecSeqs);
   lstm_rec_wg_kernel<<<2 * 2 * ntiles, kRecThreads, smem, stream>>>(tm[0], tm[1], Gx, Yh, Yl, NB, T, ntiles);
   B200_CUDA_OK(cudaGetLastError());

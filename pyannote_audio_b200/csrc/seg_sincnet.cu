@@ -360,34 +360,28 @@ struct SincWs {
 static int wav_slices(const SegGeom& g) { return ceil_div(g.W, kWavSlice); }
 
 static size_t carve(const SegGeom& g, int NB, void* base, SincWs* w) {
-  size_t off = 0;
-  auto take = [&](size_t bytes) {
-    off = align_up(off, 256);
-    void* p = base ? (char*)base + off : nullptr;
-    off += bytes;
-    return p;
-  };
+  Workspace ws(base, 256);
   SincWs t;
-  t.af_wav = (float2*)take(sizeof(float2) * NB);
-  t.af0 = (float2*)take(sizeof(float2) * NB * 80);
-  t.af1 = (float2*)take(sizeof(float2) * NB * 60);
-  t.af2 = (float2*)take(sizeof(float2) * NB * 60);
-  t.part0 = (double2*)take(sizeof(double2) * (size_t)NB * 80 * g.tiles0);
-  t.part1 = (double2*)take(sizeof(double2) * (size_t)NB * 60 * g.tiles1);
-  t.part2 = (double2*)take(sizeof(double2) * (size_t)NB * 60 * g.tiles2);
-  t.P0 = (float*)take(sizeof(float) * (size_t)NB * 80 * g.pool0);
-  t.P1 = (float*)take(sizeof(float) * (size_t)NB * 60 * g.pool1);
-  t.P2 = (float*)take(sizeof(float) * (size_t)NB * 60 * g.pool2);
+  t.af_wav = (float2*)ws.take(sizeof(float2) * NB);
+  t.af0 = (float2*)ws.take(sizeof(float2) * NB * 80);
+  t.af1 = (float2*)ws.take(sizeof(float2) * NB * 60);
+  t.af2 = (float2*)ws.take(sizeof(float2) * NB * 60);
+  t.part0 = (double2*)ws.take(sizeof(double2) * (size_t)NB * 80 * g.tiles0);
+  t.part1 = (double2*)ws.take(sizeof(double2) * (size_t)NB * 60 * g.tiles1);
+  t.part2 = (double2*)ws.take(sizeof(double2) * (size_t)NB * 60 * g.tiles2);
+  t.P0 = (float*)ws.take(sizeof(float) * (size_t)NB * 80 * g.pool0);
+  t.P1 = (float*)ws.take(sizeof(float) * (size_t)NB * 60 * g.pool1);
+  t.P2 = (float*)ws.take(sizeof(float) * (size_t)NB * 60 * g.pool2);
   t.wav_part = nullptr;
   t.red0 = t.red1 = nullptr;
-  if (wav_slices(g) > 1) t.wav_part = (double2*)take(sizeof(double2) * (size_t)NB * wav_slices(g));
+  if (wav_slices(g) > 1) t.wav_part = (double2*)ws.take(sizeof(double2) * (size_t)NB * wav_slices(g));
   if (g.tiles0 > kFinGroup) {   // the largest stage's first reduction level; later levels are smaller
     const size_t n = (size_t)NB * 80 * ceil_div(g.tiles0, kFinGroup);
-    t.red0 = (double2*)take(sizeof(double2) * n);
-    t.red1 = (double2*)take(sizeof(double2) * n);
+    t.red0 = (double2*)ws.take(sizeof(double2) * n);
+    t.red1 = (double2*)ws.take(sizeof(double2) * n);
   }
   if (w) *w = t;
-  return align_up(off, 256);
+  return ws.bytes();
 }
 
 size_t sincnet_workspace_bytes(const SegGeom& g, int NB) { return carve(g, NB, nullptr, nullptr); }
@@ -403,16 +397,9 @@ int sincnet_forward(const SincNetWeights& W, const SegGeom& g, const float* wav,
                     const int* chunk_valid, int NB, void* ws, float* x0, int conv_impl, cudaStream_t stream) {
   SincWs w;
   carve(g, NB, ws, &w);
-  static bool attr = false;
   const size_t smem_sinc = (2176 + 126 * 80) * sizeof(float);
   const size_t smem_c80 = (80 * 196 + 20 * 300) * sizeof(float);
   const size_t smem_c60 = (60 * 196 + 20 * 300) * sizeof(float);
-  if (!attr) {
-    B200_CUDA_OK(cudaFuncSetAttribute(sinc_pool_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem_sinc));
-    B200_CUDA_OK(cudaFuncSetAttribute(conv5_pool_kernel<80>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem_c80));
-    B200_CUDA_OK(cudaFuncSetAttribute(conv5_pool_kernel<60>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem_c60));
-    attr = true;
-  }
   const int nslices = wav_slices(g);
   wav_stats_kernel<<<dim3(nslices, NB), 512, 0, stream>>>(wav, chunk_off, chunk_valid, g.W, W.wav_w, W.wav_b,
                                                           w.af_wav, w.wav_part);
@@ -426,6 +413,7 @@ int sincnet_forward(const SincNetWeights& W, const SegGeom& g, const float* wav,
                               stream)))
       return rc;
   } else {
+    B200_CUDA_OK(cudaFuncSetAttribute(sinc_pool_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem_sinc));
     sinc_pool_kernel<<<dim3(g.tiles0, NB), 128, smem_sinc, stream>>>(wav, chunk_off, chunk_valid, w.af_wav, W.sinc_f,
                                                                     g.W, w.P0, g.pool0, g.tiles0, w.part0);
   }
@@ -435,6 +423,7 @@ int sincnet_forward(const SincNetWeights& W, const SegGeom& g, const float* wav,
                                stream)))
       return rc;
   } else {
+    B200_CUDA_OK(cudaFuncSetAttribute(conv5_pool_kernel<80>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem_c80));
     conv5_pool_kernel<80><<<dim3(g.tiles1, NB), 192, smem_c80, stream>>>(w.P0, g.pool0, w.af0, W.conv_w[0],
                                                                          W.conv_b[0], w.P1, g.pool1, g.tiles1, w.part1);
   }
@@ -444,6 +433,7 @@ int sincnet_forward(const SincNetWeights& W, const SegGeom& g, const float* wav,
                                stream)))
       return rc;
   } else {
+    B200_CUDA_OK(cudaFuncSetAttribute(conv5_pool_kernel<60>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem_c60));
     conv5_pool_kernel<60><<<dim3(g.tiles2, NB), 192, smem_c60, stream>>>(w.P1, g.pool1, w.af1, W.conv_w[1],
                                                                          W.conv_b[1], w.P2, g.pool2, g.tiles2, w.part2);
   }

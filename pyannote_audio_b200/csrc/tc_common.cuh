@@ -169,9 +169,10 @@ struct WgmmaRS<256> {
   }
 };
 
-typedef CUresult (*PFN_encodeTiled)(CUtensorMap*, CUtensorMapDataType, cuuint32_t, void*, const cuuint64_t*,
-                                    const cuuint64_t*, const cuuint32_t*, const cuuint32_t*, CUtensorMapInterleave,
-                                    CUtensorMapSwizzle, CUtensorMapL2promotion, CUtensorMapFloatOOBfill);
-PFN_encodeTiled get_encode();
+// Tiled TMA map of an fp16 tensor of `rank` dims (innermost first; `strides` holds the rank - 1 outer byte strides),
+// no interleave, 256-byte L2 promotion, zeros for out-of-bounds elements.  estr = nullptr means element strides of 1;
+// `what` names the map in the error message.
+int encode_f16_map(CUtensorMap* tm, int rank, const void* ptr, const cuuint64_t* dims, const cuuint64_t* strides,
+                   const cuuint32_t* box, const cuuint32_t* estr, CUtensorMapSwizzle swizzle, const char* what);
 
 }  // namespace b200

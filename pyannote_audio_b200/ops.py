@@ -113,6 +113,44 @@ def sinc_filter_bank(low_hz_: torch.Tensor, band_hz_: torch.Tensor, window_: Opt
     return bank.contiguous()
 
 
+def _state_dict_reader(sd: Mapping[str, torch.Tensor]):
+    """``f(name)`` -> float pointer to a contiguous float32 CPU copy of ``sd[name]``.  The copies (and whatever else
+    goes into ``f.keep``) stay alive as long as ``f``, i.e. until the loader that reads them has returned."""
+    keep = []
+
+    def f(name):
+        t = sd[name].detach().to(torch.float32).cpu().contiguous()
+        keep.append(t)
+        return _fp(t)
+
+    f.keep = keep
+    return f
+
+
+def _fill_sincnet(w, sd: Mapping[str, torch.Tensor], f):
+    """The ``sincnet.*`` fields that SegWeights (PyanNet) and XvecWeights (XVectorSincNet) share."""
+    w.wav_norm_weight = float(sd["sincnet.wav_norm1d.weight"].reshape(-1)[0])
+    w.wav_norm_bias = float(sd["sincnet.wav_norm1d.bias"].reshape(-1)[0])
+    p = "sincnet.conv1d.0.filterbank."
+    bank = sinc_filter_bank(sd[p + "low_hz_"], sd[p + "band_hz_"], sd.get(p + "window_"), sd.get(p + "n_"))
+    f.keep.append(bank)
+    w.sinc_filters = _fp(bank)
+    for i in range(3):
+        w.norm_weight[i] = f(f"sincnet.norm1d.{i}.weight")
+        w.norm_bias[i] = f(f"sincnet.norm1d.{i}.bias")
+    for i in range(2):
+        w.conv_weight[i] = f(f"sincnet.conv1d.{i + 1}.weight")
+        w.conv_bias[i] = f(f"sincnet.conv1d.{i + 1}.bias")
+
+
+def _norm_mode(normalize) -> int:
+    """False/0: rows as given; True/1: fp64 L2 normalisation; "float32"/2: numpy's float32 normalisation of rows that
+    hold float32 values (what the reference does to float32 embeddings before scipy's linkage)."""
+    if normalize in ("float32", 2):
+        return 2
+    return int(bool(normalize))
+
+
 class Context:
     """Owns a ``b200_ctx`` (weights + workspaces) on one CUDA device."""
 
@@ -169,6 +207,12 @@ class Context:
         _lib.check(self.lib.b200_ctx_timer(self._h, name.encode(), C.byref(ms), C.byref(units)))
         return float(ms.value), int(units.value)
 
+    def _call(self, name: str, *args):
+        """``b200_<name>(ctx, *args, stream)`` with this ctx's device selected and its current stream; a failure
+        raises (ValueError, MemoryError or B200Error)."""
+        with torch.cuda.device(self.device):
+            _lib.check(getattr(self.lib, name)(self._h, *args, _stream(self.device)))
+
     # ---- weights ---------------------------------------------------------------------------------
     def load_segmentation(self, sd: Mapping[str, torch.Tensor], specifications=None):
         """PyanNet weights.  The head has ``classifier.weight``'s K rows (1 .. 32); its activation comes from
@@ -176,26 +220,9 @@ class Context:
         num_classes = int(sd["classifier.weight"].shape[0])
         check_seg_classes(num_classes)
         activation = SEG_LOGSOFTMAX if specifications is None else seg_activation(specifications)
-        keep = []
-
-        def f(name):
-            t = sd[name].detach().to(torch.float32).cpu().contiguous()
-            keep.append(t)
-            return _fp(t)
-
+        f = _state_dict_reader(sd)
         w = _lib.SegWeights()
-        w.wav_norm_weight = float(sd["sincnet.wav_norm1d.weight"].reshape(-1)[0])
-        w.wav_norm_bias = float(sd["sincnet.wav_norm1d.bias"].reshape(-1)[0])
-        p = "sincnet.conv1d.0.filterbank."
-        bank = sinc_filter_bank(sd[p + "low_hz_"], sd[p + "band_hz_"], sd.get(p + "window_"), sd.get(p + "n_"))
-        keep.append(bank)
-        w.sinc_filters = _fp(bank)
-        for i in range(3):
-            w.norm_weight[i] = f(f"sincnet.norm1d.{i}.weight")
-            w.norm_bias[i] = f(f"sincnet.norm1d.{i}.bias")
-        for i in range(2):
-            w.conv_weight[i] = f(f"sincnet.conv1d.{i + 1}.weight")
-            w.conv_bias[i] = f(f"sincnet.conv1d.{i + 1}.bias")
+        _fill_sincnet(w, sd, f)
         layers = 0
         while f"lstm.weight_ih_l{layers}" in sd:
             layers += 1
@@ -217,12 +244,7 @@ class Context:
         self.seg_loaded, self.seg_classes, self.seg_activation = True, num_classes, activation
 
     def load_embedding(self, sd: Mapping[str, torch.Tensor]):
-        keep = []
-
-        def f(name):
-            t = sd[name].detach().to(torch.float32).cpu().contiguous()
-            keep.append(t)
-            return _fp(t)
+        f = _state_dict_reader(sd)
 
         def conv_bn(dst, conv, bn):
             dst.conv_weight = f(conv + ".weight")
@@ -253,26 +275,9 @@ class Context:
 
     def load_xvector(self, sd: Mapping[str, torch.Tensor]):
         """XVectorSincNet weights (models/embedding/xvector.py:205-252) into the ctx's own slot."""
-        keep = []
-
-        def f(name):
-            t = sd[name].detach().to(torch.float32).cpu().contiguous()
-            keep.append(t)
-            return _fp(t)
-
+        f = _state_dict_reader(sd)
         w = _lib.XvecWeights()
-        w.wav_norm_weight = float(sd["sincnet.wav_norm1d.weight"].reshape(-1)[0])
-        w.wav_norm_bias = float(sd["sincnet.wav_norm1d.bias"].reshape(-1)[0])
-        p = "sincnet.conv1d.0.filterbank."
-        bank = sinc_filter_bank(sd[p + "low_hz_"], sd[p + "band_hz_"], sd.get(p + "window_"), sd.get(p + "n_"))
-        keep.append(bank)
-        w.sinc_filters = _fp(bank)
-        for i in range(3):
-            w.norm_weight[i] = f(f"sincnet.norm1d.{i}.weight")
-            w.norm_bias[i] = f(f"sincnet.norm1d.{i}.bias")
-        for i in range(2):
-            w.conv_weight[i] = f(f"sincnet.conv1d.{i + 1}.weight")
-            w.conv_bias[i] = f(f"sincnet.conv1d.{i + 1}.bias")
+        _fill_sincnet(w, sd, f)
         for layer, (cin, cout, k, _) in enumerate(XVEC_TDNN):
             conv, bn = f"tdnns.{3 * layer}", f"tdnns.{3 * layer + 2}"
             if tuple(sd[conv + ".weight"].shape) != (cout, cin, k):
@@ -329,9 +334,12 @@ class Context:
         self.emb_loaded, self.emb_channels = True, 1024
 
     # ---- helpers ---------------------------------------------------------------------------------
-    def _chunks(self, wav: torch.Tensor, chunk_off, chunk_valid):
+    def _check_waveform(self, wav: torch.Tensor):
         if wav.device != self.device or wav.dtype != torch.float32 or not wav.is_contiguous():
             raise ValueError(f"waveform must be a contiguous float32 tensor on {self.device}")
+
+    def _chunks(self, wav: torch.Tensor, chunk_off, chunk_valid):
+        self._check_waveform(wav)
         off = np.ascontiguousarray(chunk_off, dtype=np.int64)
         valid = np.ascontiguousarray(chunk_valid, dtype=np.int32)
         if off.shape != valid.shape or off.ndim != 1:
@@ -339,6 +347,18 @@ class Context:
         if len(off) and int((off + valid).max()) > wav.numel():
             raise ValueError("a chunk reads past the end of the waveform buffer")
         return off, valid
+
+    def _utterances(self, wav: torch.Tensor, off, num_samples: int, min_samples: int, too_short: str):
+        """Utterance i = wav[off[i] : off[i] + num_samples] -> (host int64 offsets, n, num_samples); ``too_short`` is
+        the error message (formatted with num_samples) for utterances shorter than ``min_samples``."""
+        self._check_waveform(wav)
+        off = np.ascontiguousarray(off, dtype=np.int64).reshape(-1)
+        n, num_samples = len(off), int(num_samples)
+        if num_samples < min_samples:
+            raise ValueError(too_short.format(num_samples))
+        if n and (int(off.min()) < 0 or int(off.max()) + num_samples > wav.numel()):
+            raise ValueError("an utterance reads outside the waveform buffer")
+        return off, n, num_samples
 
     # ---- segmentation ----------------------------------------------------------------------------
     def _out(self, out: Optional[torch.Tensor], shape, dtype) -> torch.Tensor:
@@ -366,38 +386,32 @@ class Context:
             if return_logp:
                 raise ValueError("the loaded segmentation head is a sigmoid head: it has scores, not log-probabilities")
             scores = self._out(out, (n, F, 1 if reduce_max else K), torch.float32)
-            with torch.cuda.device(self.device):
-                _lib.check(self.lib.b200_seg_forward_scores(
-                    self._h, _ptr(wav), off.ctypes.data, valid.ctypes.data, n, window,
-                    None if reduce_max else _ptr(scores), _ptr(scores) if reduce_max else None, _stream(self.device)))
+            self._call("b200_seg_forward_scores", _ptr(wav), off.ctypes.data, valid.ctypes.data, n, window,
+                       None if reduce_max else _ptr(scores), _ptr(scores) if reduce_max else None)
             return scores
         if reduce_max:
             raise ValueError("reduce_max needs a sigmoid segmentation head (use powerset_speech for a powerset head)")
         cls = self._out(out, (n, F), torch.uint8)
         logp = torch.empty((n, F, K), dtype=torch.float32, device=self.device) if return_logp else None
-        with torch.cuda.device(self.device):
-            _lib.check(self.lib.b200_seg_forward_window(self._h, _ptr(wav), off.ctypes.data, valid.ctypes.data, n,
-                                                        window, _ptr(cls), _ptr(logp), _stream(self.device)))
+        self._call("b200_seg_forward_window", _ptr(wav), off.ctypes.data, valid.ctypes.data, n, window, _ptr(cls),
+                   _ptr(logp))
         return (cls, logp) if return_logp else cls
 
     def sincnet_forward(self, wav, chunk_off, chunk_valid):
         off, valid = self._chunks(wav, chunk_off, chunk_valid)
         n = len(off)
         out = torch.empty((n, FRAMES, 60), dtype=torch.float32, device=self.device)
-        with torch.cuda.device(self.device):
-            _lib.check(self.lib.b200_sincnet_forward(self._h, _ptr(wav), off.ctypes.data, valid.ctypes.data, n,
-                                                     _ptr(out), _stream(self.device)))
+        self._call("b200_sincnet_forward", _ptr(wav), off.ctypes.data, valid.ctypes.data, n, _ptr(out))
         return out
 
     def powerset_to_multilabel(self, cls: torch.Tensor, num_speakers: int = SPEAKERS, max_per_frame: int = 2):
         """(…) uint8 powerset classes of ``num_speakers`` speakers with at most ``max_per_frame`` per frame ->
         (…, num_speakers) uint8 multilabel (Powerset.to_multilabel, hard)."""
         k = len(powerset_mapping(num_speakers, max_per_frame))
+        cls = cls.contiguous()
         out = torch.empty(tuple(cls.shape) + (int(num_speakers),), dtype=torch.uint8, device=self.device)
-        with torch.cuda.device(self.device):
-            _lib.check(self.lib.b200_powerset_to_multilabel_generic(self._h, _ptr(cls.contiguous()), cls.numel(), k,
-                                                                    int(num_speakers), int(max_per_frame), _ptr(out),
-                                                                    _stream(self.device)))
+        self._call("b200_powerset_to_multilabel_generic", _ptr(cls), cls.numel(), k, int(num_speakers),
+                   int(max_per_frame), _ptr(out))
         return out
 
     # ---- embeddings ------------------------------------------------------------------------------
@@ -410,15 +424,12 @@ class Context:
         if tuple(masks.shape) != (n, SPEAKERS, FRAMES) or masks.dtype != torch.uint8 or not masks.is_contiguous():
             raise ValueError(f"masks must be a contiguous uint8 tensor of shape ({n}, 3, 589)")
         emb = self._out(out, (n, SPEAKERS, EMB_DIM), torch.float32)
-        with torch.cuda.device(self.device):
-            if peers:
-                arr = (C.c_void_p * len(peers))(*[C.c_void_p(int(a)) for a in peers])
-                _lib.check(self.lib.b200_emb_forward_push(self._h, _ptr(wav), off.ctypes.data, valid.ctypes.data, n,
-                                                          _ptr(masks), _ptr(emb), arr, len(peers),
-                                                          _stream(self.device)))
-            else:
-                _lib.check(self.lib.b200_emb_forward(self._h, _ptr(wav), off.ctypes.data, valid.ctypes.data, n,
-                                                     _ptr(masks), _ptr(emb), _stream(self.device)))
+        args = (_ptr(wav), off.ctypes.data, valid.ctypes.data, n, _ptr(masks), _ptr(emb))
+        if peers:
+            arr = (C.c_void_p * len(peers))(*[C.c_void_p(int(a)) for a in peers])
+            self._call("b200_emb_forward_push", *args, arr, len(peers))
+        else:
+            self._call("b200_emb_forward", *args)
         return emb
 
     def _pool_weights(self, weights: Optional[torch.Tensor], n: int):
@@ -438,19 +449,12 @@ class Context:
         """Embeddings of utterances of one length: utterance i = wav[off[i] : off[i] + num_samples] (any length >= 400
         samples).  ``weights``: None or (n, Tw) / (n, S, Tw) soft pooling weights (any Tw, interpolated onto the
         trunk frames) -> (n, max(S, 1), 256) float32."""
-        if wav.device != self.device or wav.dtype != torch.float32 or not wav.is_contiguous():
-            raise ValueError(f"waveform must be a contiguous float32 tensor on {self.device}")
-        off = np.ascontiguousarray(off, dtype=np.int64).reshape(-1)
-        n, num_samples = len(off), int(num_samples)
-        if num_samples < 400:
-            raise ValueError(f"utterances of {num_samples} samples are shorter than one 400-sample fbank frame")
-        if n and (int(off.min()) < 0 or int(off.max()) + num_samples > wav.numel()):
-            raise ValueError("an utterance reads outside the waveform buffer")
+        off, n, num_samples = self._utterances(wav, off, num_samples, 400,
+                                               "utterances of {} samples are shorter than one 400-sample fbank frame")
         w, S, Tw = self._pool_weights(weights, n)
         emb = self._out(out, (n, S, EMB_DIM), torch.float32)
-        with torch.cuda.device(self.device):
-            _lib.check(self.lib.b200_emb_forward_utt(self._h, _ptr(wav), off.ctypes.data, num_samples, n, _ptr(w),
-                                                     S if w is not None else 0, Tw, _ptr(emb), _stream(self.device)))
+        self._call("b200_emb_forward_utt", _ptr(wav), off.ctypes.data, num_samples, n, _ptr(w),
+                   S if w is not None else 0, Tw, _ptr(emb))
         return emb
 
     def xvec_forward(self, wav, off, num_samples: int, weights: Optional[torch.Tensor] = None,
@@ -458,19 +462,12 @@ class Context:
         """XVectorSincNet embeddings of utterances of one length: utterance i = wav[off[i] : off[i] + num_samples]
         (>= 4771 samples).  ``weights``: None or (n, Tw) / (n, S, Tw) pooling weights of any real values (any Tw,
         nearest-interpolated onto the TDNN frames) -> (n, max(S, 1), dimension) float32."""
-        if wav.device != self.device or wav.dtype != torch.float32 or not wav.is_contiguous():
-            raise ValueError(f"waveform must be a contiguous float32 tensor on {self.device}")
-        off = np.ascontiguousarray(off, dtype=np.int64).reshape(-1)
-        n, num_samples = len(off), int(num_samples)
-        if num_samples < XVEC_MIN_SAMPLES:
-            raise ValueError(f"XVectorSincNet needs at least {XVEC_MIN_SAMPLES} samples, got {num_samples}")
-        if n and (int(off.min()) < 0 or int(off.max()) + num_samples > wav.numel()):
-            raise ValueError("an utterance reads outside the waveform buffer")
+        off, n, num_samples = self._utterances(wav, off, num_samples, XVEC_MIN_SAMPLES,
+                                               f"XVectorSincNet needs at least {XVEC_MIN_SAMPLES} samples, got {{}}")
         w, S, Tw = self._pool_weights(weights, n)
         emb = self._out(out, (n, S, self.xvec_dimension), torch.float32)
-        with torch.cuda.device(self.device):
-            _lib.check(self.lib.b200_xvec_forward(self._h, _ptr(wav), off.ctypes.data, num_samples, n, _ptr(w),
-                                                  S if w is not None else 0, Tw, _ptr(emb), _stream(self.device)))
+        self._call("b200_xvec_forward", _ptr(wav), off.ctypes.data, num_samples, n, _ptr(w), S if w is not None else 0,
+                   Tw, _ptr(emb))
         return emb
 
     def emb_forward_embedding(self, frames: torch.Tensor, weights: Optional[torch.Tensor] = None):
@@ -483,10 +480,7 @@ class Context:
         B, T = int(frames.shape[0]), int(frames.shape[3])
         w, S, Tw = self._pool_weights(weights, B)
         emb = torch.empty((B, S, EMB_DIM), dtype=torch.float32, device=self.device)
-        with torch.cuda.device(self.device):
-            _lib.check(self.lib.b200_emb_forward_embedding(self._h, _ptr(frames), B, T, _ptr(w),
-                                                           S if w is not None else 0, Tw, _ptr(emb),
-                                                           _stream(self.device)))
+        self._call("b200_emb_forward_embedding", _ptr(frames), B, T, _ptr(w), S if w is not None else 0, Tw, _ptr(emb))
         return emb
 
     def push(self, src: torch.Tensor, peers: Sequence[int]):
@@ -494,25 +488,20 @@ class Context:
         if not peers or src.numel() == 0:
             return
         arr = (C.c_void_p * len(peers))(*[C.c_void_p(int(a)) for a in peers])
-        with torch.cuda.device(self.device):
-            _lib.check(self.lib.b200_push(self._h, _ptr(src), src.numel() * src.element_size(), arr, len(peers),
-                                          _stream(self.device)))
+        self._call("b200_push", _ptr(src), src.numel() * src.element_size(), arr, len(peers))
 
     def emb_fbank(self, wav, chunk_off, chunk_valid):
         off, valid = self._chunks(wav, chunk_off, chunk_valid)
         n = len(off)
         fb = torch.empty((n, 998, 80), dtype=torch.float32, device=self.device)
-        with torch.cuda.device(self.device):
-            _lib.check(self.lib.b200_emb_fbank(self._h, _ptr(wav), off.ctypes.data, valid.ctypes.data, n, _ptr(fb),
-                                               _stream(self.device)))
+        self._call("b200_emb_fbank", _ptr(wav), off.ctypes.data, valid.ctypes.data, n, _ptr(fb))
         return fb
 
     def emb_trunk(self, fbank: torch.Tensor):
         n = fbank.shape[0]
         fbank = fbank.contiguous()
         out = torch.empty((n, self.emb_channels, 10, 125), dtype=torch.float32, device=self.device)
-        with torch.cuda.device(self.device):
-            _lib.check(self.lib.b200_emb_trunk(self._h, _ptr(fbank), n, _ptr(out), _stream(self.device)))
+        self._call("b200_emb_trunk", _ptr(fbank), n, _ptr(out))
         return out
 
     def stats_pool(self, seq: torch.Tensor, weights: Optional[torch.Tensor] = None):
@@ -529,9 +518,7 @@ class Context:
             weights = weights.contiguous().float()
             S, Tw = weights.shape[1], weights.shape[2]
         out = torch.empty((B, S, 2 * F), dtype=torch.float32, device=self.device)
-        with torch.cuda.device(self.device):
-            _lib.check(self.lib.b200_stats_pool(self._h, _ptr(seq), _ptr(weights), _ptr(out), B, F, T, S, Tw,
-                                                _stream(self.device)))
+        self._call("b200_stats_pool", _ptr(seq), _ptr(weights), _ptr(out), B, F, T, S, Tw)
         return out.squeeze(1) if squeeze else out
 
     # ---- overlap-add / reconstruction ----------------------------------------------------------------
@@ -555,9 +542,7 @@ class Context:
     def speaker_count(self, seg: torch.Tensor, start_frame, num_frames: int):
         sf = self.start_frames(start_frame)
         count = torch.empty((num_frames,), dtype=torch.uint8, device=self.device)
-        with torch.cuda.device(self.device):
-            _lib.check(self.lib.b200_speaker_count(self._h, _ptr(seg), _ptr(sf), sf.numel(), num_frames, _ptr(count),
-                                                   _stream(self.device)))
+        self._call("b200_speaker_count", _ptr(seg), _ptr(sf), sf.numel(), num_frames, _ptr(count))
         return count
 
     def reconstruct(self, seg: torch.Tensor, hard_clusters, start_frame, num_frames: int, count: torch.Tensor,
@@ -567,9 +552,8 @@ class Context:
             hard_clusters = torch.from_numpy(np.ascontiguousarray(hard_clusters, dtype=np.int8)).to(self.device)
         hc = hard_clusters.to(torch.int8).contiguous()
         out = torch.empty((num_frames, num_clusters_out), dtype=torch.uint8, device=self.device)
-        with torch.cuda.device(self.device):
-            _lib.check(self.lib.b200_reconstruct(self._h, _ptr(seg), _ptr(hc), _ptr(sf), sf.numel(), num_frames,
-                                                 _ptr(count), num_clusters_out, _ptr(out), _stream(self.device)))
+        self._call("b200_reconstruct", _ptr(seg), _ptr(hc), _ptr(sf), sf.numel(), num_frames, _ptr(count),
+                   num_clusters_out, _ptr(out))
         return out
 
     def frame_transitions(self, discrete: torch.Tensor, cap: int = 4096):
@@ -587,10 +571,8 @@ class Context:
             return []
         mats = [d.contiguous() for d in matrices]
         buf = torch.empty((m, 2 + 2 * cap), dtype=torch.int32, device=self.device)
-        with torch.cuda.device(self.device):
-            for i, d in enumerate(mats):
-                _lib.check(self.lib.b200_frame_transitions(self._h, _ptr(d), int(d.shape[0]), int(d.shape[1]), cap,
-                                                           _ptr(buf[i]), _stream(self.device)))
+        for i, d in enumerate(mats):
+            self._call("b200_frame_transitions", _ptr(d), int(d.shape[0]), int(d.shape[1]), cap, _ptr(buf[i]))
         host = buf.cpu().numpy()
         self.last_transfer_bytes = host.nbytes
         out = []
@@ -600,9 +582,7 @@ class Context:
             while max(n_on, n_off) > c:                       # rare: more events than slots -> this matrix again
                 c = 1 << int(max(n_on, n_off) - 1).bit_length()
                 big = torch.empty((2 + 2 * c,), dtype=torch.int32, device=self.device)
-                with torch.cuda.device(self.device):
-                    _lib.check(self.lib.b200_frame_transitions(self._h, _ptr(d), int(d.shape[0]), int(d.shape[1]), c,
-                                                               _ptr(big), _stream(self.device)))
+                self._call("b200_frame_transitions", _ptr(d), int(d.shape[0]), int(d.shape[1]), c, _ptr(big))
                 row = big.cpu().numpy()
                 self.last_transfer_bytes += row.nbytes
                 n_on, n_off = int(row[0]), int(row[1])
@@ -635,10 +615,8 @@ class Context:
             out = torch.empty((n,), dtype=torch.float32, device=self.device)
         elif out.dtype != torch.float32 or out.device != self.device or not out.is_contiguous() or out.numel() < n:
             raise ValueError(f"`out` must be a contiguous float32 tensor with at least {n} elements on {self.device}")
-        with torch.cuda.device(self.device):
-            _lib.check(self.lib.b200_audio_ingest(self._h, _ptr(pcm), fmt, int(channels), int(frames),
-                                                  int(sample_rate), target_rate, -1 if channel is None else int(channel),
-                                                  _ptr(out), out.numel(), _stream(self.device)))
+        self._call("b200_audio_ingest", _ptr(pcm), fmt, int(channels), int(frames), int(sample_rate), target_rate,
+                   -1 if channel is None else int(channel), _ptr(out), out.numel())
         return out[:n]
 
     # ---- generic overlap-add (Inference.aggregate) ---------------------------------------------------
@@ -671,94 +649,117 @@ class Context:
                 return w
             warm = self._window(("warm", F, wl, wr, epsilon), build)
         out = torch.empty((num_frames, scores.shape[2]), dtype=torch.float32, device=self.device)
-        with torch.cuda.device(self.device):
-            _lib.check(self.lib.b200_aggregate_window(self._h, _ptr(scores), _ptr(sf), sf.numel(), int(num_frames), F,
-                                                      int(scores.shape[2]), _ptr(ham), _ptr(warm), int(skip_average),
-                                                      float(missing), float(np.float32(epsilon)), _ptr(out),
-                                                      _stream(self.device)))
+        self._call("b200_aggregate_window", _ptr(scores), _ptr(sf), sf.numel(), int(num_frames), F,
+                   int(scores.shape[2]), _ptr(ham), _ptr(warm), int(skip_average), float(missing),
+                   float(np.float32(epsilon)), _ptr(out))
         return out
 
     def powerset_speech(self, cls: torch.Tensor, num_speakers: int = SPEAKERS, max_per_frame: int = 2) -> torch.Tensor:
         """(…) uint8 powerset classes -> (…, 1) float32 speech indicator (max over the speakers of the multilabel)."""
         k = len(powerset_mapping(num_speakers, max_per_frame))
+        cls = cls.contiguous()
         out = torch.empty(tuple(cls.shape) + (1,), dtype=torch.float32, device=self.device)
-        with torch.cuda.device(self.device):
-            _lib.check(self.lib.b200_powerset_speech_generic(self._h, _ptr(cls.contiguous()), cls.numel(), k,
-                                                             int(num_speakers), int(max_per_frame), _ptr(out),
-                                                             _stream(self.device)))
+        self._call("b200_powerset_speech_generic", _ptr(cls), cls.numel(), k, int(num_speakers), int(max_per_frame),
+                   _ptr(out))
         return out
 
     def clean_frames(self, seg: torch.Tensor):
         n = seg.shape[0]
         clean = torch.empty((n, SPEAKERS), dtype=torch.int32, device=self.device)
         active = torch.empty((n, SPEAKERS), dtype=torch.uint8, device=self.device)
-        with torch.cuda.device(self.device):
-            _lib.check(self.lib.b200_clean_frames(self._h, _ptr(seg), n, _ptr(clean), _ptr(active),
-                                                  _stream(self.device)))
+        self._call("b200_clean_frames", _ptr(seg), n, _ptr(clean), _ptr(active))
         return clean, active
 
+    # ---- clustering (fp64) -------------------------------------------------------------------------------
+    def plda_transform(self, x: torch.Tensor, mean1, mean2, lda, mu, trT) -> torch.Tensor:
+        """PLDA.__call__ on the device: x (n, Din) float64 -> (n, L) float64 (core/plda.py:50-63)."""
+        x, lda, trT = x.contiguous(), lda.contiguous(), trT.contiguous()
+        n, din = x.shape
+        dout, L = trT.shape
+        fea = torch.empty((n, L), dtype=torch.float64, device=self.device)
+        self._call("b200_plda_transform", _ptr(x), n, din, dout, L, _ptr(mean1), _ptr(mean2), _ptr(lda), _ptr(mu),
+                   _ptr(trT), _ptr(fea))
+        return fea
 
-# ---- clustering (fp64) -------------------------------------------------------------------------------
-def _ctx_method(fn):
-    setattr(Context, fn.__name__, fn)
-    return fn
+    def weighted_centroids(self, q: torch.Tensor, kept: torch.Tensor, train: torch.Tensor) -> torch.Tensor:
+        """(W.T @ train) / W.sum(0).T with W = q[:, kept] (clustering.py:620-621): q (n,S), train (n,dim) float64."""
+        q, train = q.contiguous(), train.contiguous()
+        kept = kept.to(device=self.device, dtype=torch.int32).contiguous()
+        out = torch.empty((kept.numel(), train.shape[1]), dtype=torch.float64, device=self.device)
+        self._call("b200_weighted_centroids", _ptr(q), q.shape[0], q.shape[1], _ptr(kept), kept.numel(), _ptr(train),
+                   train.shape[1], _ptr(out))
+        return out
 
+    def _linkage_check(self, name: str, *args):
+        """``_call`` of a linkage entry point.  A file above 32 768 observations allocates its packed distances
+        outside torch's caching allocator, so memory torch holds cached (e.g. from the segmentation and embedding of
+        that same file) cannot serve it: on an allocation failure the cache is returned to the device and the call
+        made once more."""
+        try:
+            self._call(name, *args)
+        except MemoryError:
+            torch.cuda.empty_cache()
+            self._call(name, *args)
 
-def _norm_mode(normalize) -> int:
-    """False/0: rows as given; True/1: fp64 L2 normalisation; "float32"/2: numpy's float32 normalisation of rows that
-    hold float32 values (what the reference does to float32 embeddings before scipy's linkage)."""
-    if normalize in ("float32", 2):
-        return 2
-    return int(bool(normalize))
+    def linkage_centroid(self, x: torch.Tensor, normalize=True) -> torch.Tensor:
+        """x (n, dim) float64 on device -> Z (n-1, 4) float64 on device (scipy linkage format)."""
+        n, dim = x.shape
+        x = x.contiguous()
+        Z = torch.empty((n - 1, 4), dtype=torch.float64, device=self.device)
+        self._linkage_check("b200_linkage_centroid", _ptr(x), n, dim, _norm_mode(normalize), _ptr(Z))
+        return Z
 
+    def linkage_centroid_batched(self, x: torch.Tensor, row_offsets, normalize=True) -> torch.Tensor:
+        """x (sum n_f, dim) f64; row_offsets host int array (F+1,) -> concatenated Z ((sum max(n_f-1,0)), 4) f64."""
+        x = x.contiguous()
+        ro = np.ascontiguousarray(row_offsets, dtype=np.int32)
+        nz = int(np.maximum(np.diff(ro) - 1, 0).sum())
+        Z = torch.empty((nz, 4), dtype=torch.float64, device=self.device)
+        self._linkage_check("b200_linkage_centroid_batched", _ptr(x), ro.ctypes.data, len(ro) - 1, x.shape[1],
+                            _norm_mode(normalize), _ptr(Z))
+        return Z
 
-@_ctx_method
-def plda_transform(self, x: torch.Tensor, mean1, mean2, lda, mu, trT) -> torch.Tensor:
-    """PLDA.__call__ on the device: x (n, Din) float64 -> (n, L) float64 (core/plda.py:50-63)."""
-    x = x.contiguous()
-    n, din = x.shape
-    dout, L = trT.shape
-    fea = torch.empty((n, L), dtype=torch.float64, device=self.device)
-    with torch.cuda.device(self.device):
-        _lib.check(self.lib.b200_plda_transform(self._h, _ptr(x), n, din, dout, L, _ptr(mean1), _ptr(mean2),
-                                                _ptr(lda.contiguous()), _ptr(mu), _ptr(trT.contiguous()), _ptr(fea),
-                                                _stream(self.device)))
-    return fea
+    def cdist_cosine(self, a: torch.Tensor, b: torch.Tensor) -> torch.Tensor:
+        a, b = a.contiguous(), b.contiguous()
+        m, dim = a.shape
+        k = b.shape[0]
+        d = torch.empty((m, k), dtype=torch.float64, device=self.device)
+        self._call("b200_cdist_cosine", _ptr(a), m, _ptr(b), k, dim, _ptr(d))
+        return d
 
+    def vbx(self, fea: torch.Tensor, phi: torch.Tensor, gamma0: torch.Tensor, Fa: float, Fb: float,
+            max_iters: int = 20, epsilon: float = 1e-4):
+        fea, phi = fea.contiguous(), phi.contiguous()
+        gamma = gamma0.contiguous().clone()
+        n, D = fea.shape
+        S = gamma.shape[1]
+        pi = torch.empty((S,), dtype=torch.float64, device=self.device)
+        iters = C.c_int32(0)
+        self._call("b200_vbx", _ptr(fea), _ptr(phi), n, D, S, C.c_double(Fa), C.c_double(Fb), max_iters,
+                   C.c_double(epsilon), _ptr(gamma), _ptr(pi), C.byref(iters))
+        return gamma, pi, int(iters.value)
 
-@_ctx_method
-def weighted_centroids(self, q: torch.Tensor, kept: torch.Tensor, train: torch.Tensor) -> torch.Tensor:
-    """(W.T @ train) / W.sum(0).T with W = q[:, kept] (clustering.py:620-621): q (n,S), train (n,dim) float64."""
-    q, train = q.contiguous(), train.contiguous()
-    kept = kept.to(device=self.device, dtype=torch.int32).contiguous()
-    out = torch.empty((kept.numel(), train.shape[1]), dtype=torch.float64, device=self.device)
-    with torch.cuda.device(self.device):
-        _lib.check(self.lib.b200_weighted_centroids(self._h, _ptr(q), q.shape[0], q.shape[1], _ptr(kept), kept.numel(),
-                                                    _ptr(train), train.shape[1], _ptr(out), _stream(self.device)))
-    return out
+    def vbx_batched(self, fea: torch.Tensor, phi: torch.Tensor, gamma0: torch.Tensor, n, S, Fa: float, Fb: float,
+                    max_iters: int = 20, epsilon: float = 1e-4, want_iters: bool = False):
+        """fea (sum n_f, D); gamma0 flat concatenation of the per-problem (n_f, S_f) initial responsibilities."""
+        fea, phi = fea.contiguous(), phi.contiguous()
+        gamma = gamma0.contiguous().clone()
+        n = np.ascontiguousarray(n, dtype=np.int32)
+        S = np.ascontiguousarray(S, dtype=np.int32)
+        pi = torch.empty((int(S.sum()),), dtype=torch.float64, device=self.device)
+        iters = np.zeros(len(n), dtype=np.int32)
+        self._call("b200_vbx_batched", _ptr(fea), _ptr(phi), n.ctypes.data, S.ctypes.data, len(n), fea.shape[1],
+                   C.c_double(Fa), C.c_double(Fb), max_iters, C.c_double(epsilon), _ptr(gamma), _ptr(pi),
+                   iters.ctypes.data if want_iters else None)
+        return gamma, pi, iters
 
-
-def _linkage_check(call):
-    """Runs a linkage ABI call.  A file above 32 768 observations allocates its packed distances outside torch's
-    caching allocator, so memory torch holds cached (e.g. from the segmentation and embedding of that same file) cannot
-    serve it: on an allocation failure the cache is returned to the device and the call made once more."""
-    try:
-        _lib.check(call())
-    except MemoryError:
-        torch.cuda.empty_cache()
-        _lib.check(call())
-
-
-@_ctx_method
-def linkage_centroid(self, x: torch.Tensor, normalize=True) -> torch.Tensor:
-    """x (n, dim) float64 on device -> Z (n-1, 4) float64 on device (scipy linkage format)."""
-    n, dim = x.shape
-    x = x.contiguous()
-    Z = torch.empty((n - 1, 4), dtype=torch.float64, device=self.device)
-    with torch.cuda.device(self.device):
-        _linkage_check(lambda: self.lib.b200_linkage_centroid(self._h, _ptr(x), n, dim, _norm_mode(normalize),
-                                                              _ptr(Z), _stream(self.device)))
-    return Z
+    def assign(self, soft: torch.Tensor, constrained: bool = True) -> torch.Tensor:
+        soft = soft.contiguous()
+        c, s, k = soft.shape
+        assert s == SPEAKERS
+        hard = torch.empty((c, s), dtype=torch.int8, device=self.device)
+        self._call("b200_assign", _ptr(soft), c, k, int(constrained), _ptr(hard))
+        return hard
 
 
 def fcluster_distance(Z: np.ndarray, t: float) -> np.ndarray:
@@ -770,58 +771,6 @@ def fcluster_distance(Z: np.ndarray, t: float) -> np.ndarray:
     return T
 
 
-@_ctx_method
-def cdist_cosine(self, a: torch.Tensor, b: torch.Tensor) -> torch.Tensor:
-    a, b = a.contiguous(), b.contiguous()
-    m, dim = a.shape
-    k = b.shape[0]
-    d = torch.empty((m, k), dtype=torch.float64, device=self.device)
-    with torch.cuda.device(self.device):
-        _lib.check(self.lib.b200_cdist_cosine(self._h, _ptr(a), m, _ptr(b), k, dim, _ptr(d), _stream(self.device)))
-    return d
-
-
-@_ctx_method
-def vbx(self, fea: torch.Tensor, phi: torch.Tensor, gamma0: torch.Tensor, Fa: float, Fb: float, max_iters: int = 20,
-        epsilon: float = 1e-4):
-    fea, phi = fea.contiguous(), phi.contiguous()
-    gamma = gamma0.contiguous().clone()
-    n, D = fea.shape
-    S = gamma.shape[1]
-    pi = torch.empty((S,), dtype=torch.float64, device=self.device)
-    iters = C.c_int32(0)
-    with torch.cuda.device(self.device):
-        _lib.check(self.lib.b200_vbx(self._h, _ptr(fea), _ptr(phi), n, D, S, C.c_double(Fa), C.c_double(Fb), max_iters,
-                                     C.c_double(epsilon), _ptr(gamma), _ptr(pi), C.byref(iters),
-                                     _stream(self.device)))
-    return gamma, pi, int(iters.value)
-
-
-@_ctx_method
-def assign(self, soft: torch.Tensor, constrained: bool = True) -> torch.Tensor:
-    soft = soft.contiguous()
-    c, s, k = soft.shape
-    assert s == SPEAKERS
-    hard = torch.empty((c, s), dtype=torch.int8, device=self.device)
-    with torch.cuda.device(self.device):
-        _lib.check(self.lib.b200_assign(self._h, _ptr(soft), c, k, int(constrained), _ptr(hard), _stream(self.device)))
-    return hard
-
-
-@_ctx_method
-def linkage_centroid_batched(self, x: torch.Tensor, row_offsets, normalize=True) -> torch.Tensor:
-    """x (sum n_f, dim) f64; row_offsets host int array (F+1,) -> concatenated Z ((sum max(n_f-1,0)), 4) f64."""
-    x = x.contiguous()
-    ro = np.ascontiguousarray(row_offsets, dtype=np.int32)
-    nz = int(np.maximum(np.diff(ro) - 1, 0).sum())
-    Z = torch.empty((nz, 4), dtype=torch.float64, device=self.device)
-    with torch.cuda.device(self.device):
-        _linkage_check(lambda: self.lib.b200_linkage_centroid_batched(self._h, _ptr(x), ro.ctypes.data, len(ro) - 1,
-                                                                      x.shape[1], _norm_mode(normalize), _ptr(Z),
-                                                                      _stream(self.device)))
-    return Z
-
-
 def linkage_bytes(row_offsets, dim: int) -> int:
     """Device bytes ``linkage_centroid_batched`` needs for these problems (host only, no device): the workspace it grows
     to plus the per-call packed distances of its largest problem above 32 768 observations."""
@@ -830,21 +779,3 @@ def linkage_bytes(row_offsets, dim: int) -> int:
     if nbytes <= 0:
         _lib.check(nbytes)
     return nbytes
-
-
-@_ctx_method
-def vbx_batched(self, fea: torch.Tensor, phi: torch.Tensor, gamma0: torch.Tensor, n, S, Fa: float, Fb: float,
-                max_iters: int = 20, epsilon: float = 1e-4, want_iters: bool = False):
-    """fea (sum n_f, D); gamma0 flat concatenation of the per-problem (n_f, S_f) initial responsibilities."""
-    fea, phi = fea.contiguous(), phi.contiguous()
-    gamma = gamma0.contiguous().clone()
-    n = np.ascontiguousarray(n, dtype=np.int32)
-    S = np.ascontiguousarray(S, dtype=np.int32)
-    pi = torch.empty((int(S.sum()),), dtype=torch.float64, device=self.device)
-    iters = np.zeros(len(n), dtype=np.int32)
-    with torch.cuda.device(self.device):
-        _lib.check(self.lib.b200_vbx_batched(self._h, _ptr(fea), _ptr(phi), n.ctypes.data, S.ctypes.data, len(n),
-                                             fea.shape[1], C.c_double(Fa), C.c_double(Fb), max_iters,
-                                             C.c_double(epsilon), _ptr(gamma), _ptr(pi),
-                                             iters.ctypes.data if want_iters else None, _stream(self.device)))
-    return gamma, pi, iters
