@@ -25,8 +25,14 @@
 //   Ck = 32 (64-B rows: layer 1): those fragments are read with ldmatrix, the 64-B swizzle applied in software, and
 //   issued as register-A wgmma.
 //   Each output sums its products in the (tap, 16-channel step) order of conv_tc_kernel, and the epilogue is the same,
-//   so the two kernels give bit-identical results.  With several channel chunks (layers 3 and 4) staging a row once
-//   for three taps would change that order to (kh, chunk, kw) and with it the last bits.
+//   so the two kernels give bit-identical results.
+// conv_chunk_row_kernel: the stride-1 3x3 convs with C_in = C_out = 128 or 256 (layers 3 and 4, 16 of the 35, and the
+//   conv2 of the bottleneck trunks' layers 3 and 4).  Persistent CTAs walk the output tiles of conv_tc_kernel with the
+//   same wgmma shapes.  For each kh the producer stages input row h - 1 + kh once per 64-channel chunk as a 136-pixel
+//   box, and tap kw reads it from pixel row kw on, as in conv_row_kernel: a third of the activation fill.  The
+//   consumers still walk (kh, kw, chunk, 16-channel step), so every chunk box of a kernel row stays resident until
+//   its tap kw = 2, and the results are bit-identical to conv_tc_kernel's.  Weight tiles stream through a ring of
+//   their own, and the producer stages the next tile while the consumers run the epilogue.
 #include "common.cuh"
 #include "emb.cuh"
 #include "tc_common.cuh"
@@ -261,6 +267,117 @@ conv_row_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__
   }
 }
 
+// Plan of conv_chunk_row_kernel<N>: a ring of 136-pixel row boxes (one 64-channel chunk each) and a ring of (tap,
+// chunk) weight tiles.  N = 128: two CTAs per SM (113 KB each), so one CTA's epilogue runs while the other's MMAs
+// do; N = 256 (128 accumulator registers per thread): one (227 KB).  A kernel row keeps all N / 64 of its chunk boxes
+// resident until its last tap, so the box ring holds one more than that; the weight ring takes the rest.
+template <int N>
+struct ChunkRowPlan {
+  static constexpr int kChunks = N / 64;
+  static constexpr int kCtasPerSm = N == 256 ? 1 : 2;
+  static constexpr uint32_t kABytes = (kTileM + kRowHalo) * 128;   // 17 KB, 1024-B multiple
+  static constexpr uint32_t kBBytes = N * 128;
+  static constexpr uint32_t kASlots = N == 256 ? 5 : 3;
+  static constexpr uint32_t kBSlots = N == 256 ? 4 : 3;
+  static constexpr size_t kSmem = 2048 + kASlots * kABytes + kBSlots * kBBytes;   // 101 / 215 KB
+  static_assert(kASlots > kChunks && kASlots <= 8 && kBSlots <= 8, "chunk row ring plan");
+};
+
+template <int N>
+__global__ void __launch_bounds__(kWgThreads, ChunkRowPlan<N>::kCtasPerSm)
+conv_chunk_row_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB, ConvParams p) {
+  using P = ChunkRowPlan<N>;
+  constexpr int CH = P::kChunks, KSTEPS = 9 * CH;           // K steps of one output tile: (kh, kw, chunk)
+  extern __shared__ uint8_t smem_raw[];
+  const uint32_t base = (smem_u32(smem_raw) + 1023u) & ~1023u;
+  const uint32_t full_a = base, empty_a = base + 64, full_b = base + 128, empty_b = base + 192;   // 8 x 8 B each
+  const uint32_t ring_a = base + 1024, ring_b = ring_a + P::kASlots * P::kABytes;
+  const int warp = threadIdx.x >> 5;
+
+  if (threadIdx.x == 0) {
+    for (uint32_t s = 0; s < P::kASlots; ++s) { mbar_init(full_a + 8 * s, 1); mbar_init(empty_a + 8 * s, 2); }
+    for (uint32_t s = 0; s < P::kBSlots; ++s) { mbar_init(full_b + 8 * s, 1); mbar_init(empty_b + 8 * s, 2); }
+    asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
+  }
+  __syncthreads();
+
+  // unit u: column tile u % tiles_w (neighbouring CTAs share the halo pixels in L2), then output row, then segment
+  if (warp == 8) {
+    if ((threadIdx.x & 31) == 0) {
+      prefetch_tensormap(&tmA);
+      prefetch_tensormap(&tmB);
+      uint32_t qa = 0, qb = 0;                              // row boxes / weight tiles staged so far
+      for (int u = blockIdx.x; u < p.num_tiles; u += gridDim.x) {
+        const int wt = u % p.tiles_w, t = u / p.tiles_w;
+        const int h = t % p.H_out, b = t / p.H_out;
+        for (int s = 0; s < KSTEPS; ++s) {
+          const int cc = s % CH, kw = (s / CH) % 3, kh = s / (3 * CH);
+          if (kw == 0) {                                    // row h - 1 + kh, chunk cc: read by taps kw = 0, 1, 2
+            const uint32_t q = qa + kh * CH + cc, slot = q % P::kASlots;
+            mbar_wait(empty_a + 8 * slot, ((q / P::kASlots) & 1) ^ 1);
+            mbar_expect_tx(full_a + 8 * slot, P::kABytes);
+            tma_load_4d(&tmA, full_a + 8 * slot, ring_a + slot * P::kABytes, cc * 64, wt * kTileM - 1, h - 1 + kh, b);
+          }
+          const uint32_t q = qb + s, slot = q % P::kBSlots;
+          mbar_wait(empty_b + 8 * slot, ((q / P::kBSlots) & 1) ^ 1);
+          mbar_expect_tx(full_b + 8 * slot, P::kBBytes);
+          tma_load_3d(&tmB, full_b + 8 * slot, ring_b + slot * P::kBBytes, cc * 64, 0, 3 * kh + kw);
+        }
+        qa += 3 * CH;
+        qb += KSTEPS;
+      }
+    }
+    return;
+  }
+
+  const int wg = __shfl_sync(0xffffffffu, warp >> 2, 0);    // warp-uniform to the compiler: no wgmma serialisation
+  const bool leader = (threadIdx.x & 127) == 0;
+  uint32_t qa = 0, qb = 0;
+  for (int u = blockIdx.x; u < p.num_tiles; u += gridDim.x) {
+    const int wt = u % p.tiles_w, t = u / p.tiles_w;
+    const int h = t % p.H_out, b = t / p.H_out;
+    float acc[N / 2];
+#pragma unroll
+    for (int i = 0; i < N / 2; ++i) {
+      acc[i] = 0.f;
+      asm volatile("" : "+f"(acc[i]));                      // zeroed before the first wg_fence, not sunk past it
+    }
+    // the previous K step's slots, released once its wgmma have read them
+    uint32_t prev_b = 0, prev_a = 0;
+    bool prev_frees_a = false;
+    auto release = [&]() {
+      if (leader) {
+        mbar_arrive(empty_b + 8 * prev_b);
+        if (prev_frees_a) mbar_arrive(empty_a + 8 * prev_a);
+      }
+    };
+    // (kh, kw, chunk, k16): the order of conv_tc_kernel; tap kw reads the row box from pixel row kw on
+    for (int s = 0; s < KSTEPS; ++s) {
+      const int cc = s % CH, kw = (s / CH) % 3, kh = s / (3 * CH);
+      const uint32_t qA = qa + kh * CH + cc, sa = qA % P::kASlots;
+      const uint32_t qB = qb + s, sb = qB % P::kBSlots;
+      mbar_wait(full_a + 8 * sa, (qA / P::kASlots) & 1);
+      mbar_wait(full_b + 8 * sb, (qB / P::kBSlots) & 1);
+      wg_fence();
+      const uint64_t ad = wg_desc(ring_a + sa * P::kABytes + (uint32_t)(wg * 64 + kw) * 128u, 128);
+      const uint64_t bd = wg_desc(ring_b + sb * P::kBBytes, 128);
+#pragma unroll
+      for (int k = 0; k < 4; ++k) Wgmma<N>::mma(acc, ad + 2 * k, bd + 2 * k);
+      wg_commit();
+      wg_wait<1>();
+      if (s > 0) release();
+      prev_b = sb;
+      prev_a = sa;
+      prev_frees_a = kw == 2;                               // chunk box (kh, cc) is done after tap (kh, 2)
+    }
+    wg_wait<0>();
+    release();                                              // the producer stages the next unit during the epilogue
+    qa += 3 * CH;
+    qb += KSTEPS;
+    conv_epilogue<N>(acc, p, (size_t)b * p.H_out + h, wt * kTileM + wg * 64);
+  }
+}
+
 // ------------------------------------------------------------------------------------------------
 // SIMT reference conv (same math, CUDA cores) -- A/B check for the tensor-core path
 // ------------------------------------------------------------------------------------------------
@@ -465,7 +582,10 @@ int conv_forward(const ConvLayer& L, const __half* in, const __half* residual, _
   // conv_row_kernel for the stride-1 3x3 convs with one channel chunk and C_in = C_out; impl 2 keeps every conv on
   // conv_tc_kernel, the bit-exact reference of the row kernel
   const bool rows = impl == 1 && L.ksize == 3 && L.stride == 1 && L.C_in == p.Ck && L.C_out == L.C_in;
-  p.a_rows = rows ? kTileM + kRowHalo : kTileM;
+  // conv_chunk_row_kernel for those with C_in = C_out = 128 or 256 (layers 3 and 4)
+  const bool chunk_rows =
+      impl == 1 && L.ksize == 3 && L.stride == 1 && L.C_out == L.C_in && (L.C_out == 128 || L.C_out == 256);
+  p.a_rows = rows || chunk_rows ? kTileM + kRowHalo : kTileM;
   p.a_tx = p.a_rows * p.Ck * 2;
   p.a_bytes = (p.a_tx + 1023u) & ~1023u;
   size_t smem;
@@ -488,6 +608,10 @@ int conv_forward(const ConvLayer& L, const __half* in, const __half* residual, _
     p.band = ceil_div(p.H_out, nbands);
     p.bands = ceil_div(p.H_out, p.band);
     p.num_tiles = strips * p.bands;
+  } else if (chunk_rows) {
+    // persistent over the output tiles (num_tiles as for conv_tc_kernel)
+    smem = L.C_out == 256 ? ChunkRowPlan<256>::kSmem : ChunkRowPlan<128>::kSmem;
+    ctas = (L.C_out == 256 ? ChunkRowPlan<256>::kCtasPerSm : ChunkRowPlan<128>::kCtasPerSm) * num_sms;
   } else {
     p.b_bytes = (uint32_t)(n_tile * p.Ck * 2);
     // C_out = 256 needs 128 accumulator registers per thread: one CTA per SM with 4 deep stages; the narrower layers
@@ -517,12 +641,13 @@ int conv_forward(const ConvLayer& L, const __half* in, const __half* residual, _
   }
   auto launch = [&](auto kernel) -> int {
     B200_CUDA_OK(cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-    const dim3 grid((unsigned)(rows ? std::min(p.num_tiles, ctas) : p.num_tiles), (unsigned)(L.C_out / n_tile));
+    const dim3 grid((unsigned)(ctas ? std::min(p.num_tiles, ctas) : p.num_tiles), (unsigned)(L.C_out / n_tile));
     kernel<<<grid, kWgThreads, smem, stream>>>(tmA, tmB, p);
     B200_CUDA_OK(cudaGetLastError());
     return B200_OK;
   };
   if (rows) return p.Ck == 32 ? launch(conv_row_kernel<32, 32>) : launch(conv_row_kernel<64, 64>);
+  if (chunk_rows) return L.C_out == 256 ? launch(conv_chunk_row_kernel<256>) : launch(conv_chunk_row_kernel<128>);
   if (p.Ck == 32) {
     switch (L.C_out) {
       case 32: return launch(conv_tc_kernel<32, 32>);

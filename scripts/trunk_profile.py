@@ -2,7 +2,7 @@
 
     python scripts/trunk_profile.py                  # the library in this tree (needs a GPU), ResNet34
     python scripts/trunk_profile.py --model resnet293   # a bottleneck trunk (resnet152 | resnet221 | resnet293)
-    python scripts/trunk_profile.py --root OTHER --plan reuse     # another tree's build, with its launch plan
+    python scripts/trunk_profile.py --root OTHER --plan resident  # another tree's build, with its launch plan
     python scripts/trunk_profile.py --model-only     # the byte model alone (no GPU)
 
 `ctx.emb_trunk` runs on --batch segments (the library's embedding sub-batch) under torch.profiler with CUDA
@@ -18,6 +18,9 @@ Byte model, per segment (computed from the shapes, not measured):
           resident: the stride-1 3x3 convs with one channel chunk and C_in = C_out (layers 1 and 2) stage each input
                     row of a band of output rows once as a 136-pixel box (plus two halo rows per band) and their nine
                     weight taps once per CTA (--sms CTAs per SM count as in conv_forward); the other convs stay per-tap
+          rows    : resident for layers 1 and 2; the stride-1 3x3 convs with C_in = C_out = 128 / 256 (layers 3 and 4)
+                    stage each of the three input rows of an output tile once per channel chunk as a 136-pixel box,
+                    and every weight tile; the other convs stay per-tap
   HBM   = input + output (+ residual) activations once, and the weights once per launch shared by --batch segments
 """
 import argparse
@@ -80,8 +83,9 @@ def conv_model(c, plan, batch, sms=132):
     n_tile = min(cout, 256)
     tiles = Ho * -(-Wo // TILE_M) * (cout // n_tile)
     b_tile = n_tile * ck * 2
-    reuse = plan == "reuse" and k == 3 and s == 1 and cin == ck and cout <= 64
-    if plan == "resident" and k == 3 and s == 1 and cin == ck and cout == cin:
+    reuse = k == 3 and s == 1 and ((plan == "reuse" and cin == ck and cout <= 64) or
+                                   (plan == "rows" and cin == cout and cout in (128, 256)))
+    if plan in ("resident", "rows") and k == 3 and s == 1 and cin == ck and cout == cin:
         tiles_w = -(-Wo // TILE_M)
         ctas, _, bands = resident_plan(cout, Ho, tiles_w, batch, sms)
         fill = tiles_w * (Ho + 2 * bands) * (TILE_M + HALO) * ck * 2 + ctas * k * k * b_tile / batch
@@ -122,9 +126,10 @@ def main():
     ap = argparse.ArgumentParser(description=__doc__, formatter_class=argparse.RawDescriptionHelpFormatter)
     ap.add_argument("--root", default=os.path.dirname(os.path.dirname(os.path.abspath(__file__))),
                     help="tree whose built library is timed (default: this one)")
-    ap.add_argument("--plan", choices=["resident", "reuse", "per-tap"], default="resident",
-                    help="launch plan of the timed library for the byte model (reuse: a library whose layer 1 and 2 "
-                         "convs stage one box per kh; per-tap: one box per tap)")
+    ap.add_argument("--plan", choices=["rows", "resident", "reuse", "per-tap"], default="rows",
+                    help="launch plan of the timed library for the byte model (resident: a library whose layer 3 and "
+                         "4 convs stage one box per tap; reuse: one whose layer 1 and 2 convs stage one box per kh; "
+                         "per-tap: one box per tap everywhere)")
     ap.add_argument("--sms", type=int, default=132, help="SMs of the GPU for the resident plan (H100 SXM: 132)")
     ap.add_argument("--batch", type=int, default=264, help="segments per emb_trunk call (library sub-batch: 264)")
     ap.add_argument("--iters", type=int, default=5, help="profiled emb_trunk calls")
