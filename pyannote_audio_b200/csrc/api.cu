@@ -175,13 +175,14 @@ int push_meta(b200_ctx* ctx, const int64_t* off, const int32_t* valid, int n, cu
   return B200_OK;
 }
 
-// fbank plan of a list of chunks processed in sub-batches of nbmax (emb.cuh: FbankRun): per sub-batch the runs
-// [run_base[s], run_base[s + 1]) and the number of fbank rows; frame0 / runs go to the device with the chunk table.
-// share = 0 (and every short or unaligned chunk): one private run per chunk, row0 = b * 998.
+// fbank plan of a list of segments of `samples` samples (T0 fbank frames) processed in sub-batches of nbmax (emb.cuh:
+// FbankRun): per sub-batch the runs [run_base[s], run_base[s + 1]) and the number of fbank rows; frame0 / runs go to
+// the device with the segment table.  share = 0 (and every short or unaligned segment): one private run per segment,
+// row0 = b * T0, limit = valid.
 struct FbankPlan {
   std::vector<int> run_base, nrows;
 };
-void plan_fbank(const int64_t* off, const int32_t* valid, int n, int nbmax, bool share,
+void plan_fbank(const int64_t* off, const int32_t* valid, int n, int nbmax, bool share, int samples, int T0,
                 std::vector<b200::FbankRun>* runs_out, std::vector<int>* frame0_out, FbankPlan* plan) {
   constexpr int kHop = 160;
   std::vector<b200::FbankRun>& runs = *runs_out;
@@ -195,23 +196,23 @@ void plan_fbank(const int64_t* off, const int32_t* valid, int n, int nbmax, bool
     const int nb = (n - c0) < nbmax ? (n - c0) : nbmax;
     plan->run_base.push_back((int)runs.size());
     int rows = 0, run_rows = 0;
-    bool open = false;                                       // the last run is made of full chunks and may be extended
+    bool open = false;                                       // the last run is made of full segments and may be extended
     for (int b = 0; b < nb; ++b) {
       const long long o = off[c0 + b];
-      const bool full = share && valid[c0 + b] == kChunk;
+      const bool full = share && valid[c0 + b] == samples;
       if (full && open) {
         const long long d = o - runs.back().src;
         if (d >= 0 && d % kHop == 0 && d / kHop <= run_rows) {
           const int f0 = (int)(d / kHop);
           frame0[c0 + b] = runs.back().row0 + f0;
-          if (f0 + kFbankFrames > run_rows) { rows += f0 + kFbankFrames - run_rows; run_rows = f0 + kFbankFrames; }
+          if (f0 + T0 > run_rows) { rows += f0 + T0 - run_rows; run_rows = f0 + T0; }
           continue;
         }
       }
       runs.push_back(b200::FbankRun{o, rows, full ? INT_MAX : (int)valid[c0 + b]});
       frame0[c0 + b] = rows;
-      rows += kFbankFrames;
-      run_rows = kFbankFrames;
+      rows += T0;
+      run_rows = T0;
       open = full;
     }
     plan->nrows.push_back(rows);
@@ -219,11 +220,11 @@ void plan_fbank(const int64_t* off, const int32_t* valid, int n, int nbmax, bool
   plan->run_base.push_back((int)runs.size());
 }
 
-int push_fbank_plan(b200_ctx* ctx, const int64_t* off, const int32_t* valid, int n, int nbmax, bool share,
-                    FbankPlan* plan, cudaStream_t st) {
+int push_fbank_plan(b200_ctx* ctx, const int64_t* off, const int32_t* valid, int n, int nbmax, bool share, int samples,
+                    int T0, FbankPlan* plan, cudaStream_t st) {
   std::vector<b200::FbankRun> runs;
   std::vector<int> frame0;
-  plan_fbank(off, valid, n, nbmax, share, &runs, &frame0, plan);
+  plan_fbank(off, valid, n, nbmax, share, samples, T0, &runs, &frame0, plan);
   B200_CUDA_OK(cudaMemcpyAsync(ctx->d_frame0, frame0.data(), sizeof(int) * n, cudaMemcpyHostToDevice, st));
   B200_CUDA_OK(cudaMemcpyAsync(ctx->d_runs, runs.data(), sizeof(b200::FbankRun) * runs.size(), cudaMemcpyHostToDevice, st));
   return B200_OK;
@@ -804,27 +805,39 @@ int b200_powerset_to_multilabel(b200_ctx* ctx, const uint8_t* classes, int64_t n
 }
 
 // ------------------------------------------------------------------------------------------------------
+// fbank frames of `samples` samples (kaldi framing: 400-sample frames every 160, snip_edges)
+static int64_t fbank_frames(int64_t samples) { return 1 + (samples - 400) / 160; }
+
+// trunk output width of T0 fbank frames: T0 after layer 1, then (T + 2 - 3) / 2 + 1 after each of layers 2, 3 and 4
+// (125 for the 998 frames of 10 s)
+static int trunk_width(int T0) {
+  int T = T0;
+  for (int l = 0; l < 3; ++l) T = (T + 2 - 3) / 2 + 1;
+  return T;
+}
+
 struct EmbWs {
-  float *fbank, *fmean, *stats;
+  float *fbank, *fmean;
+  double* part;   // pooling scratch, none when the trunk output has at most kPoolSlice frames
   __half *A, *Bf, *Cf, *D;
-  size_t cf_bytes;
 };
-// ResNet34: A, Bf and Cf hold the largest activation, layer 1's 32 channels at 80 x 998 per chunk.  Bottleneck trunk
-// (every later layer is half the size of layer 1 at the same width): A and D the 4p = 128 channels of layer 1, Bf
-// layer 2 block 0's conv1 output (64 channels at layer 1's resolution), Cf layer 1's conv2 output (32 channels).
-static size_t carve_emb(const EmbWeights& E, int NB, void* base, EmbWs* w) {
+// Workspace of a sub-batch of NB segments of T0 fbank frames pooled for S speakers.  fbank holds T0 rows per segment,
+// the most a plan needs (shared frames need fewer).  ResNet34: A, Bf and Cf hold the largest activation, layer 1's 32
+// channels at 80 x T0 per segment.  Bottleneck trunk (every later layer is half the size of layer 1 at the same
+// width): A and D the 4p = 128 channels of layer 1, Bf layer 2 block 0's conv1 output (64 channels at layer 1's
+// resolution), Cf layer 1's conv2 output (32 channels).
+static size_t carve_emb(const EmbWeights& E, int NB, int T0, int S, void* base, EmbWs* w) {
   Workspace ws(base, 1024);
   EmbWs t;
-  const size_t act = (size_t)NB * kMel * kFbankFrames * 32 * sizeof(__half);   // largest activation (layer1)
-  t.fbank = (float*)ws.take((size_t)NB * kFbankFrames * kMel * sizeof(float));
+  const size_t act = (size_t)NB * kMel * T0 * 32 * sizeof(__half);   // largest activation (layer1)
+  t.fbank = (float*)ws.take((size_t)NB * T0 * kMel * sizeof(float));
   t.fmean = (float*)ws.take((size_t)NB * kMel * sizeof(float));
-  t.stats = (float*)ws.take((size_t)NB * kSpeakers * 2 * 10 * E.C * sizeof(float));
+  t.part = (double*)ws.take(pool_scratch_bytes(NB, S, trunk_width(T0), E.C));
   const bool bn = !E.bottlenecks.empty();
   t.A = (__half*)ws.take(bn ? 4 * act : act);
   t.Bf = (__half*)ws.take(bn ? 2 * act : act);
   t.Cf = (__half*)ws.take(act);
   t.D = bn ? (__half*)ws.take(4 * act) : nullptr;
-  t.cf_bytes = act;
   if (w) *w = t;
   return ws.bytes();
 }
@@ -869,8 +882,7 @@ static int bottleneck_run(b200_ctx* ctx, const BottleneckWeights& B, __half* A, 
 }
 
 // conv1 + the 16 BasicBlocks (or the Bottlenecks) on nb segments of T0 fbank frames; returns the buffer holding the
-// result (NHWC fp16 [nb][10][T][C]) and its width T: T0 after layer 1, then (T + 2 - 3) / 2 + 1 after each of layers
-// 2, 3 and 4 (125 for the 998 frames of 10 s)
+// result (NHWC fp16 [nb][10][T][C]) and its width T = trunk_width(T0)
 static int trunk_run(b200_ctx* ctx, const EmbWs& w, const int* frame0, int nb, int T0, cudaStream_t st,
                      const __half** result, int* T_out) {
   const EmbWeights& E = ctx->emb;
@@ -897,20 +909,82 @@ static int trunk_run(b200_ctx* ctx, const EmbWs& w, const int* frame0, int nb, i
   return B200_OK;
 }
 
-static int emb_forward_impl(b200_ctx* ctx, const float* wav, const int64_t* chunk_off, const int32_t* chunk_valid,
-                            int32_t num_chunks, const uint8_t* masks, float* emb, float* const* emb_peers,
-                            int32_t n_peers, void* stream);
+// the Linear 20 C -> 256 on `rows` pooled statistics rows; with peers its epilogue also pushes every tile to the other
+// GPUs (fused all-gather of the embeddings over NVLink)
+static int emb_linear(b200_ctx* ctx, const __half* st_hi, const __half* st_lo, int64_t rows, float* emb, cudaStream_t st,
+                      float* const* peers = nullptr, int n_peers = 0) {
+  const int K = 20 * ctx->emb.C;
+  const int rc = gemm_tc_split(st_hi, st_lo, K, ctx->emb.seg1_w_hi, ctx->emb.seg1_w_lo, K, emb, kEmbDim, nullptr,
+                               nullptr, 0, ctx->emb.seg1_b, (int)rows, kEmbDim, K, 0, ctx->num_sms, st, peers, n_peers);
+  ctx->launches += 1;
+  return rc;
+}
+
+// WeSpeaker embeddings of n segments of `samples` samples: segment i is wav[off[i]] onwards, of which valid[i] samples
+// are read (the rest as zero).  Sub-batches of max(1, emb_max_batch * 998 / T0) segments (the workspace of
+// emb_max_batch 10 s chunks) run fbank -> trunk -> pooling into the fp16 (hi, lo) statistics rows of every segment;
+// one GEMM then runs the Linear on all of them.  share: overlapping full segments read shared fbank frames (FbankRun).
+// Pooling weights [n][S][Tw]: u8 masks or fp32 weights (at most one of the two), or neither with S = 1.
+static int emb_run(b200_ctx* ctx, const float* wav, const int64_t* off, const int32_t* valid, int n, int samples,
+                   bool share, const uint8_t* masks, const float* weights, int S, int Tw, float* emb,
+                   float* const* peers, int n_peers, cudaStream_t st) {
+  DeviceGuard g(ctx->device);
+  const EmbWeights& E = ctx->emb;
+  const int T0 = (int)fbank_frames(samples), T = trunk_width(T0);
+  const int nbmax = (int)std::min<int64_t>(n, std::max<int64_t>(1, (int64_t)ctx->emb_max_batch * kFbankFrames / T0));
+  // pooled statistics of ALL segments as fp16 (hi, lo) pairs -> one tensor-core GEMM for the Linear 20 C -> 256
+  // (5120 -> 256 for ResNet34; 20480 -> 256 for a bottleneck trunk, 80 KB of pairs per row)
+  const size_t rows = (size_t)n * S;
+  const size_t split_bytes = align_up(rows * 2 * 10 * E.C * sizeof(__half), 1024);
+  const size_t sub_bytes = carve_emb(E, nbmax, T0, S, nullptr, nullptr);
+  int rc = ensure_ws(ctx, sub_bytes + 2 * split_bytes + 4096);
+  if (rc) return rc;
+  if ((rc = push_meta(ctx, off, valid, n, st, samples))) return rc;
+  FbankPlan plan;
+  if ((rc = push_fbank_plan(ctx, off, valid, n, nbmax, share, samples, T0, &plan, st))) return rc;
+  EmbWs w;
+  carve_emb(E, nbmax, T0, S, ctx->ws, &w);
+  __half* st_hi = reinterpret_cast<__half*>(reinterpret_cast<char*>(ctx->ws) + sub_bytes);
+  __half* st_lo = reinterpret_cast<__half*>(reinterpret_cast<char*>(ctx->ws) + sub_bytes + split_bytes);
+  for (int c0 = 0, sb = 0; c0 < n; c0 += nbmax, ++sb) {
+    const int nb = std::min(nbmax, n - c0);
+    const int* frame0 = ctx->d_frame0 + c0;
+    if ((rc = fbank_forward(E, wav, ctx->d_runs + plan.run_base[sb], plan.run_base[sb + 1] - plan.run_base[sb],
+                            plan.nrows[sb], frame0, nb, T0, w.fbank, w.fmean, st)))
+      return rc;
+    ctx->launches += 2;
+    const __half* feat = nullptr;
+    {
+      ScopedTimer timer(ctx, &ctx->trunk_events, st);
+      int Tt = 0;
+      if ((rc = trunk_run(ctx, w, frame0, nb, T0, st, &feat, &Tt))) return rc;
+      B200_CHECK(Tt == T, B200_ERR_STATE, "trunk output width %d, expected %d", Tt, T);
+    }
+    if (ctx->profile) ctx->trunk_segments += nb;
+    const size_t o = (size_t)c0 * S * 2 * 10 * E.C, wo = (size_t)c0 * S * Tw;
+    rc = masks ? weighted_pool_forward(feat, nullptr, masks + wo, nb, T, S, Tw, E.C, w.part, st_hi + o, st_lo + o, st)
+               : weighted_pool_forward(feat, nullptr, weights ? weights + wo : nullptr, nb, T, S, Tw, E.C, w.part,
+                                       st_hi + o, st_lo + o, st);
+    if (rc) return rc;
+    ctx->launches += T <= kPoolSlice ? 1 : 3;
+  }
+  return emb_linear(ctx, st_hi, st_lo, (int64_t)rows, emb, st, peers, n_peers);
+}
 
 int b200_emb_forward(b200_ctx* ctx, const float* wav, const int64_t* chunk_off, const int32_t* chunk_valid,
                      int32_t num_chunks, const uint8_t* masks, float* emb, void* stream) {
-  return emb_forward_impl(ctx, wav, chunk_off, chunk_valid, num_chunks, masks, emb, nullptr, 0, stream);
+  return b200_emb_forward_push(ctx, wav, chunk_off, chunk_valid, num_chunks, masks, emb, nullptr, 0, stream);
 }
 
 int b200_emb_forward_push(b200_ctx* ctx, const float* wav, const int64_t* chunk_off, const int32_t* chunk_valid,
                           int32_t num_chunks, const uint8_t* masks, float* emb, float* const* emb_peers,
                           int32_t n_peers, void* stream) {
   B200_CHECK(n_peers >= 0 && n_peers <= 7 && (n_peers == 0 || emb_peers), B200_ERR_INVALID, "bad peer list");
-  return emb_forward_impl(ctx, wav, chunk_off, chunk_valid, num_chunks, masks, emb, emb_peers, n_peers, stream);
+  B200_CHECK(ctx && ctx->emb.loaded, B200_ERR_STATE, "embedding weights not loaded");
+  B200_CHECK(wav && chunk_off && chunk_valid && masks && emb && num_chunks >= 0, B200_ERR_INVALID, "bad arguments");
+  if (num_chunks == 0) return B200_OK;
+  return emb_run(ctx, wav, chunk_off, chunk_valid, num_chunks, kChunk, ctx->fbank_share != 0, masks, nullptr,
+                 kSpeakers, kFrames, emb, emb_peers, n_peers, (cudaStream_t)stream);
 }
 
 int b200_push(b200_ctx* ctx, const void* src, int64_t bytes, void* const* dsts, int32_t n_dsts, void* stream) {
@@ -919,59 +993,6 @@ int b200_push(b200_ctx* ctx, const void* src, int64_t bytes, void* const* dsts, 
   DeviceGuard g(ctx->device);
   ctx->launches += 1;
   return push_bytes(src, bytes, dsts, n_dsts, (cudaStream_t)stream);
-}
-
-static int emb_forward_impl(b200_ctx* ctx, const float* wav, const int64_t* chunk_off, const int32_t* chunk_valid,
-                            int32_t num_chunks, const uint8_t* masks, float* emb, float* const* emb_peers,
-                            int32_t n_peers, void* stream) {
-  B200_CHECK(ctx && ctx->emb.loaded, B200_ERR_STATE, "embedding weights not loaded");
-  B200_CHECK(wav && chunk_off && chunk_valid && masks && emb && num_chunks >= 0, B200_ERR_INVALID, "bad arguments");
-  if (num_chunks == 0) return B200_OK;
-  DeviceGuard g(ctx->device);
-  cudaStream_t st = (cudaStream_t)stream;
-  const int nbmax = num_chunks < ctx->emb_max_batch ? num_chunks : ctx->emb_max_batch;
-  // pooled statistics of ALL chunks as fp16 (hi, lo) pairs -> one tensor-core GEMM for the Linear 20 C -> 256
-  // (5120 -> 256 for ResNet34; 20480 -> 256 for a bottleneck trunk, 80 KB of pairs per row)
-  const int C = ctx->emb.C;
-  const size_t rows = (size_t)num_chunks * kSpeakers;
-  const size_t split_bytes = align_up(rows * 2 * 10 * C * sizeof(__half), 1024);
-  const size_t sub_bytes = carve_emb(ctx->emb, nbmax, nullptr, nullptr);
-  int rc = ensure_ws(ctx, sub_bytes + 2 * split_bytes + 4096);
-  if (rc) return rc;
-  if ((rc = push_meta(ctx, chunk_off, chunk_valid, num_chunks, st))) return rc;
-  FbankPlan plan;
-  if ((rc = push_fbank_plan(ctx, chunk_off, chunk_valid, num_chunks, nbmax, ctx->fbank_share != 0, &plan, st))) return rc;
-  EmbWs w;
-  carve_emb(ctx->emb, nbmax, ctx->ws, &w);
-  __half* st_hi = reinterpret_cast<__half*>(reinterpret_cast<char*>(ctx->ws) + sub_bytes);
-  __half* st_lo = reinterpret_cast<__half*>(reinterpret_cast<char*>(ctx->ws) + sub_bytes + split_bytes);
-  const __half* feat = nullptr;
-  for (int c0 = 0; c0 < num_chunks; c0 += nbmax) {
-    const int nb = (num_chunks - c0) < nbmax ? (num_chunks - c0) : nbmax;
-    const int sb = c0 / nbmax;
-    if ((rc = fbank_forward(ctx->emb, wav, ctx->d_runs + plan.run_base[sb], plan.run_base[sb + 1] - plan.run_base[sb],
-                            plan.nrows[sb], ctx->d_frame0 + c0, nb, kFbankFrames, w.fbank, w.fmean, st)))
-      return rc;
-    ctx->launches += 2;
-    {
-      ScopedTimer timer(ctx, &ctx->trunk_events, st);
-      int T = 0;
-      if ((rc = trunk_run(ctx, w, ctx->d_frame0 + c0, nb, kFbankFrames, st, &feat, &T))) return rc;
-    }
-    if (ctx->profile) ctx->trunk_segments += nb;
-    const size_t o = (size_t)c0 * kSpeakers * 2 * 10 * C;
-    if ((rc = stats_pool_forward(feat, masks + (size_t)c0 * kSpeakers * kFrames, nullptr, st_hi + o, st_lo + o, nb, C,
-                                 st)))
-      return rc;
-    ctx->launches += 1;
-  }
-  // the Linear 20 C -> 256 of ALL chunks; with peers its epilogue also pushes every tile to the other GPUs (fused
-  // all-gather of the embeddings over NVLink)
-  rc = gemm_tc_split(st_hi, st_lo, 20 * C, ctx->emb.seg1_w_hi, ctx->emb.seg1_w_lo, 20 * C, emb, kEmbDim,
-                     nullptr, nullptr, 0, ctx->emb.seg1_b, (int)rows, kEmbDim, 20 * C, 0, ctx->num_sms, st,
-                     emb_peers, n_peers);
-  ctx->launches += 1;
-  return rc;
 }
 
 int b200_emb_fbank(b200_ctx* ctx, const float* wav, const int64_t* chunk_off, const int32_t* chunk_valid,
@@ -985,7 +1006,9 @@ int b200_emb_fbank(b200_ctx* ctx, const float* wav, const int64_t* chunk_off, co
   if (rc) return rc;
   if ((rc = push_meta(ctx, chunk_off, chunk_valid, num_chunks, st))) return rc;
   FbankPlan plan;                                            // output layout [B][998][80]: one private run per chunk
-  if ((rc = push_fbank_plan(ctx, chunk_off, chunk_valid, num_chunks, num_chunks, false, &plan, st))) return rc;
+  if ((rc = push_fbank_plan(ctx, chunk_off, chunk_valid, num_chunks, num_chunks, false, kChunk, kFbankFrames, &plan,
+                            st)))
+    return rc;
   float* fmean = reinterpret_cast<float*>(ctx->ws);
   if ((rc = fbank_forward(ctx->emb, wav, ctx->d_runs, num_chunks, plan.nrows[0], ctx->d_frame0, num_chunks, kFbankFrames,
                           fbank, fmean, st)))
@@ -1002,7 +1025,7 @@ int64_t b200_emb_fbank_plan(const int64_t* chunk_off, const int32_t* chunk_valid
   std::vector<b200::FbankRun> runs;
   std::vector<int> f0;
   FbankPlan plan;
-  plan_fbank(chunk_off, chunk_valid, num_chunks, sub_batch, share != 0, &runs, &f0, &plan);
+  plan_fbank(chunk_off, chunk_valid, num_chunks, sub_batch, share != 0, kChunk, kFbankFrames, &runs, &f0, &plan);
   if (frame0) std::copy(f0.begin(), f0.end(), frame0);
   if (rows_per_sub_batch) std::copy(plan.nrows.begin(), plan.nrows.end(), rows_per_sub_batch);
   return (int64_t)runs.size();
@@ -1015,10 +1038,10 @@ int b200_emb_trunk(b200_ctx* ctx, const float* fbank, int32_t num_chunks, float*
   DeviceGuard g(ctx->device);
   cudaStream_t st = (cudaStream_t)stream;
   const int nbmax = num_chunks < ctx->emb_max_batch ? num_chunks : ctx->emb_max_batch;
-  int rc = ensure_ws(ctx, carve_emb(ctx->emb, nbmax, nullptr, nullptr) + 4096);
+  int rc = ensure_ws(ctx, carve_emb(ctx->emb, nbmax, kFbankFrames, 1, nullptr, nullptr) + 4096);
   if (rc) return rc;
   EmbWs w;
-  carve_emb(ctx->emb, nbmax, ctx->ws, &w);
+  carve_emb(ctx->emb, nbmax, kFbankFrames, 1, ctx->ws, &w);
   const int C = ctx->emb.C;
   for (int c0 = 0; c0 < num_chunks; c0 += nbmax) {
     const int nb = (num_chunks - c0) < nbmax ? (num_chunks - c0) : nbmax;
@@ -1035,14 +1058,6 @@ int b200_emb_trunk(b200_ctx* ctx, const float* fbank, int32_t num_chunks, float*
 }
 
 // ---- embeddings of utterances of any length ------------------------------------------------------------
-static int emb_linear(b200_ctx* ctx, const __half* st_hi, const __half* st_lo, int64_t rows, float* emb, cudaStream_t st) {
-  const int K = 20 * ctx->emb.C;
-  const int rc = gemm_tc_split(st_hi, st_lo, K, ctx->emb.seg1_w_hi, ctx->emb.seg1_w_lo, K, emb, kEmbDim, nullptr,
-                               nullptr, 0, ctx->emb.seg1_b, (int)rows, kEmbDim, K, 0, ctx->num_sms, st);
-  ctx->launches += 1;
-  return rc;
-}
-
 int b200_emb_forward_utt(b200_ctx* ctx, const float* wav, const int64_t* off, int64_t num_samples, int32_t num_utts,
                          const float* weights, int32_t num_speakers, int32_t num_weights, float* emb, void* stream) {
   B200_CHECK(ctx && ctx->emb.loaded, B200_ERR_STATE, "embedding weights not loaded");
@@ -1055,58 +1070,16 @@ int b200_emb_forward_utt(b200_ctx* ctx, const float* wav, const int64_t* off, in
   for (int i = 0; i < num_utts; ++i)
     B200_CHECK(off[i] >= 0, B200_ERR_INVALID, "utterance %d: negative offset %lld", i, (long long)off[i]);
   // a sub-batch holds at most emb_max_batch x 998 fbank frames: the workspace of emb_max_batch 10 s chunks
-  const int64_t T0l = 1 + (num_samples - 400) / 160;
+  const int64_t T0 = fbank_frames(num_samples);
   const int64_t budget = (int64_t)ctx->emb_max_batch * kFbankFrames;
-  B200_CHECK(T0l <= budget, B200_ERR_INVALID,
+  B200_CHECK(T0 <= budget, B200_ERR_INVALID,
              "an utterance of %lld samples has %lld fbank frames, more than the %lld frames of one embedding sub-batch "
              "(emb_max_batch %d x 998): set the option emb_max_batch to at least %lld, or embed shorter excerpts",
-             (long long)num_samples, (long long)T0l, (long long)budget, ctx->emb_max_batch,
-             (long long)((T0l + kFbankFrames - 1) / kFbankFrames));
-  DeviceGuard g(ctx->device);
-  cudaStream_t st = (cudaStream_t)stream;
-  const int T0 = (int)T0l;
-  const int S = weights ? num_speakers : 1;
-  const int nbu = (int)std::min<int64_t>(num_utts, std::max<int64_t>(1, budget / T0));   // utterances per sub-batch
-  const int nbc = (int)(((int64_t)nbu * T0 + kFbankFrames - 1) / kFbankFrames);          // the same bytes in chunks
-  int T = T0;                                                                            // trunk output width
-  for (int l = 0; l < 3; ++l) T = (T + 2 - 3) / 2 + 1;
-  const int C = ctx->emb.C;
-  const size_t rows = (size_t)num_utts * S;
-  const size_t split_bytes = align_up(rows * 2 * 10 * C * sizeof(__half), 1024);
-  EmbWs w;
-  const size_t sub_bytes = carve_emb(ctx->emb, nbc, nullptr, &w);
-  // fmean ([nbu][80] fp32) lives in the Bf scratch until the first block, the pooling partials in Cf after the
-  // trunk: fmean fits since nbu * T0 <= nbc * 998 frames and Bf / Cf hold at least nbc * 998 * 80 * 32 fp16
-  const size_t part_bytes = pool_scratch_bytes(nbu, S, T, C);
-  B200_CHECK(part_bytes <= w.cf_bytes, B200_ERR_INVALID,
-             "%d speakers x %d frames: pooling scratch exceeds the sub-batch workspace", S, T);
-  int rc = ensure_ws(ctx, sub_bytes + 2 * split_bytes + 4096);
-  if (rc) return rc;
-  if ((rc = ensure_meta(ctx, num_utts))) return rc;
-  std::vector<b200::FbankRun> runs((size_t)num_utts);                                    // one private run each
-  for (int i = 0; i < num_utts; ++i) runs[i] = b200::FbankRun{(long long)off[i], (i % nbu) * T0, (int)num_samples};
-  B200_CUDA_OK(cudaMemcpyAsync(ctx->d_runs, runs.data(), sizeof(b200::FbankRun) * runs.size(), cudaMemcpyHostToDevice, st));
-  carve_emb(ctx->emb, nbc, ctx->ws, &w);
-  w.fmean = reinterpret_cast<float*>(w.Bf);
-  double* part = reinterpret_cast<double*>(w.Cf);
-  __half* st_hi = reinterpret_cast<__half*>(reinterpret_cast<char*>(ctx->ws) + sub_bytes);
-  __half* st_lo = reinterpret_cast<__half*>(reinterpret_cast<char*>(ctx->ws) + sub_bytes + split_bytes);
-  for (int u0 = 0; u0 < num_utts; u0 += nbu) {
-    const int nb = std::min(nbu, num_utts - u0);
-    if ((rc = fbank_forward(ctx->emb, wav, ctx->d_runs + u0, nb, nb * T0, nullptr, nb, T0, w.fbank, w.fmean, st)))
-      return rc;
-    ctx->launches += 2;
-    const __half* feat = nullptr;
-    int Tt = 0;
-    if ((rc = trunk_run(ctx, w, nullptr, nb, T0, st, &feat, &Tt))) return rc;
-    B200_CHECK(Tt == T, B200_ERR_STATE, "trunk output width %d, expected %d", Tt, T);
-    const size_t o = (size_t)u0 * S * 2 * 10 * C;
-    if ((rc = weighted_pool_forward(feat, nullptr, weights ? weights + (size_t)u0 * S * num_weights : nullptr, nb, T, S,
-                                    num_weights, C, part, st_hi + o, st_lo + o, st)))
-      return rc;
-    ctx->launches += T <= kPoolSlice ? 1 : 3;
-  }
-  return emb_linear(ctx, st_hi, st_lo, (int64_t)rows, emb, st);
+             (long long)num_samples, (long long)T0, (long long)budget, ctx->emb_max_batch,
+             (long long)((T0 + kFbankFrames - 1) / kFbankFrames));
+  const std::vector<int32_t> valid((size_t)num_utts, (int32_t)num_samples);
+  return emb_run(ctx, wav, off, valid.data(), num_utts, (int)num_samples, false, nullptr, weights,
+                 weights ? num_speakers : 1, num_weights, emb, nullptr, 0, (cudaStream_t)stream);
 }
 
 int b200_emb_forward_embedding(b200_ctx* ctx, const float* frames, int32_t B, int32_t T, const float* weights,

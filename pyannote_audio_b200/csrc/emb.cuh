@@ -69,35 +69,33 @@ int conv1_forward(const float* fbank, const float* fmean, const int* frame0, con
 // arithmetic.  The host groups a sub-batch's chunks into runs of hop-aligned, overlapping full chunks; a run's frames
 // are computed once into consecutive rows of `fbank` ([nrows][80] fp32) and segment b reads rows
 // frame0[b] .. frame0[b] + 997 (conv1_forward, the per-segment mean).  Chunks that are short (valid < 160000: samples
-// past `limit` read as zero) or not hop-aligned get a private run, which is also the layout of the public
-// b200_emb_fbank ([B][998][80]).  Bit-identical to one private run per chunk; 10x fewer frames on a pipeline batch.
+// past `limit` read as zero) or not hop-aligned get a private run, and so does every segment when sharing is off
+// (utterances of any length, the public b200_emb_fbank's [B][998][80]): rows b * T0 .. b * T0 + T0 - 1 of a
+// sub-batch.  Bit-identical to one private run per chunk; 10x fewer frames on a pipeline batch.
 struct FbankRun {
   long long src;   // sample offset of the run's first frame in `wav`
   int row0;        // first row of the run in `fbank`
   int limit;       // valid samples counted from src (INT_MAX for runs of full chunks)
 };
-// fmean[b] = mean of the T0 rows of segment b (frame0 as in conv1_forward)
+// fmean[b] = mean of the T0 rows of segment b (frame0 as in conv1_forward, not NULL)
 int fbank_forward(const EmbWeights& W, const float* wav, const FbankRun* runs, int nruns, int nrows,
                   const int* frame0, int B, int T0, float* fbank, float* fmean, cudaStream_t stream);
 int fbank_center(float* fbank, const float* fmean, int B, cudaStream_t stream);
 // NHWC fp16 [B][10][T][C] -> NCHW fp32 [B][C][10][T]
 int frames_to_nchw(const __half* feat, float* out, int B, int T, int C, cudaStream_t stream);
 
-// masked statistics pooling: feat [B][10][125][C] fp16 NHWC (C = 256 or 1024), masks [B][3][589] u8 -> stats
-// [B*3][20 C] fp32
-int stats_pool_forward(const __half* feat, const unsigned char* masks, float* stats, __half* stats_hi,
-                       __half* stats_lo, int B, int C, cudaStream_t stream);
 // weighted statistics pooling for any T, S and Tw (pooling.py:30-61, 76-130) -> the fp16 (hi, lo) rows of the Linear:
 // feat NHWC fp16 [B][10][T][C] (trunk output) or frames NCHW fp32 [B][C][10][T] (caller frames, exactly one of
-// the two), w fp32 [B][S][Tw] any real values or NULL (mean and std(correction=1) over the T frames, S = 1).  The
-// weights reach the T frames by torch's CUDA nearest index (upsample_nearest1d).  T is split into slices of
-// kPoolSlice frames; with one slice the sums are the stats_pool_forward ones in the same order, with several the
-// per-slice fp32 sums are combined in fp64 in slice order (deterministic, no atomics).  part: fp64 scratch of
-// pool_scratch_bytes(B, S, T, C) bytes (none with one slice).  Rows of stats_hi / stats_lo: (b * S + s) * 20 C.
-// C = 256 or 1024.
+// the two), w [B][S][Tw] or NULL (mean and std(correction=1) over the T frames, S = 1): u8 masks (trunk output only)
+// or fp32 of any real values.  The weights reach the T frames by torch's CUDA nearest index (upsample_nearest1d).
+// Up to kSpeakers speakers of a sequence share one read of its features.  T is split into slices of kPoolSlice
+// frames; with several the per-slice fp32 sums are combined in fp64 in slice order (deterministic, no atomics).
+// part: fp64 scratch of pool_scratch_bytes(B, S, T, C) bytes (none with one slice).  Rows of stats_hi / stats_lo:
+// (b * S + s) * 20 C.  C = 256 or 1024.
 constexpr int kPoolSlice = 512;
 size_t pool_scratch_bytes(int B, int S, int T, int C, int H = 10);
-int weighted_pool_forward(const __half* feat, const float* frames, const float* w, int B, int T, int S, int Tw, int C,
+template <typename W>   // uint8_t or float
+int weighted_pool_forward(const __half* feat, const float* frames, const W* w, int B, int T, int S, int Tw, int C,
                           double* part, __half* stats_hi, __half* stats_lo, cudaStream_t stream);
 // the same pooling on frame-major fp32 rows x [B][F][kPoolRowsLd] (XVectorSincNet's last TDNN layer): the first T
 // frames and the first C channels of every sequence -> stats rows of ld_out fp16 (hi, lo), mean at c and std at C + c

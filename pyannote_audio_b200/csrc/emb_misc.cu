@@ -8,7 +8,8 @@
 // conv subtracts on load.
 //
 // stats pooling follows models/blocks/pooling.py:30-61,76-130 via resnet.py:61-66 (TSTP): nearest
-// interpolation of the 589-frame mask onto the 125 trunk frames, weighted mean and weighted unbiased std.
+// interpolation of the weights (the 589-frame masks of a 10 s chunk) onto the trunk frames, weighted mean and weighted
+// unbiased std.
 #include "common.cuh"
 #include "emb.cuh"
 #include <type_traits>
@@ -185,7 +186,7 @@ __global__ void __launch_bounds__(640) fbank_mean_kernel(const float* __restrict
   // 8 groups of 80 threads each sum an eighth of the T0 frames in fp64, combined in group order
   __shared__ double part[8][kMel];
   const int b = blockIdx.x, m = threadIdx.x % kMel, g = threadIdx.x / kMel;
-  const size_t r0 = frame0 ? (size_t)frame0[b] : (size_t)b * T0;
+  const size_t r0 = (size_t)frame0[b];
   double s = 0.0;
 #pragma unroll 8
   for (int t = g; t < T0; t += 8) s += (double)fb[(r0 + t) * kMel + m];
@@ -244,87 +245,14 @@ int fbank_forward(const EmbWeights& W, const float* wav, const FbankRun* runs, i
 }
 
 // ------------------------------------------------------------------------------------------------
-// masked stats pooling on the trunk output, all 3 local speakers from one pass; C = trunk channels (256 or 1024)
-// ------------------------------------------------------------------------------------------------
-template <int C>
-__global__ void __launch_bounds__(256) stats_pool_kernel(const __half* __restrict__ feat,
-                                                         const unsigned char* __restrict__ masks,
-                                                         float* __restrict__ stats, __half* __restrict__ stats_hi,
-                                                         __half* __restrict__ stats_lo) {
-  // grid (10 freq rows, B, C / 256); thread = channel c; feat[b][h][t][c]
-  __shared__ float s_w[kSpeakers][kEmbT];
-  const int h = blockIdx.x, b = blockIdx.y, c = (C == 256 ? 0 : (int)blockIdx.z * 256) + threadIdx.x;
-  for (int i = threadIdx.x; i < kSpeakers * kEmbT; i += blockDim.x) {
-    const int s = i / kEmbT, t = i % kEmbT;
-    // F.interpolate(mode="nearest"): src = floor(dst * in / out)   (pooling.py:116-117)
-    const int src = (int)(((long long)t * kFrames) / kEmbT);
-    s_w[s][t] = (float)masks[((size_t)b * kSpeakers + s) * kFrames + src];
-  }
-  __syncthreads();
-  const __half* fp = feat + (((size_t)b * 10 + h) * kEmbT) * C + c;
-  float v1[kSpeakers], v2[kSpeakers], sx[kSpeakers];
-#pragma unroll
-  for (int s = 0; s < kSpeakers; ++s) { v1[s] = 0.f; v2[s] = 0.f; sx[s] = 0.f; }
-  for (int t = 0; t < kEmbT; ++t) {
-    const float x = __half2float(fp[(size_t)t * C]);
-#pragma unroll
-    for (int s = 0; s < kSpeakers; ++s) {
-      const float w = s_w[s][t];
-      v1[s] += w;
-      v2[s] += w * w;
-      sx[s] += x * w;
-    }
-  }
-  float mean[kSpeakers], sd[kSpeakers];
-#pragma unroll
-  for (int s = 0; s < kSpeakers; ++s) {
-    v1[s] += 1e-8f;
-    mean[s] = sx[s] / v1[s];
-    sd[s] = 0.f;
-  }
-  for (int t = 0; t < kEmbT; ++t) {
-    const float x = __half2float(fp[(size_t)t * C]);
-#pragma unroll
-    for (int s = 0; s < kSpeakers; ++s) {
-      const float d = x - mean[s];
-      sd[s] += d * d * s_w[s][t];
-    }
-  }
-#pragma unroll
-  for (int s = 0; s < kSpeakers; ++s) {
-    const float var = sd[s] / (v1[s] - v2[s] / v1[s] + 1e-8f);
-    const size_t row = ((size_t)b * kSpeakers + s) * (2 * 10 * C);
-    const float sdv = sqrtf(var);
-    if (stats) {
-      stats[row + c * 10 + h] = mean[s];
-      stats[row + 10 * C + c * 10 + h] = sdv;
-    }
-    if (stats_hi) {   // (hi, lo) fp16 split consumed by gemm_tc_split (Linear 20 C -> 256)
-      const __half mh = __float2half_rn(mean[s]), sh = __float2half_rn(sdv);
-      stats_hi[row + c * 10 + h] = mh;
-      stats_lo[row + c * 10 + h] = __float2half_rn(mean[s] - __half2float(mh));
-      stats_hi[row + 10 * C + c * 10 + h] = sh;
-      stats_lo[row + 10 * C + c * 10 + h] = __float2half_rn(sdv - __half2float(sh));
-    }
-  }
-}
-
-int stats_pool_forward(const __half* feat, const unsigned char* masks, float* stats, __half* stats_hi,
-                       __half* stats_lo, int B, int C, cudaStream_t stream) {
-  B200_CHECK(C == 256 || C == 1024, B200_ERR_STATE, "stats pooling: %d channels unsupported", C);
-  dim3 grid(10, B, C / 256);
-  if (C == 256) stats_pool_kernel<256><<<grid, 256, 0, stream>>>(feat, masks, stats, stats_hi, stats_lo);
-  else stats_pool_kernel<1024><<<grid, 256, 0, stream>>>(feat, masks, stats, stats_hi, stats_lo);
-  B200_CUDA_OK(cudaGetLastError());
-  return B200_OK;
-}
-
-// ------------------------------------------------------------------------------------------------
-// weighted statistics pooling for any T, S and Tw (utterances of any length, caller frames, soft weights)
+// weighted statistics pooling for any T, S and Tw (diarization masks, utterances of any length, caller frames, soft
+// weights)
 // ------------------------------------------------------------------------------------------------
 // torch's CUDA nearest index (upsample_nearest1d, the device F.interpolate(mode="nearest") runs on): scale is
-// (float)Tw / T, src = min(floor(dst * scale), Tw - 1), with the exact special cases T == Tw and T == 2 Tw.  Not the
-// integer t * Tw / T of stats_pool_kernel: the two differ on a few frames of long sequences.
+// (float)Tw / T, src = min(floor(dst * scale), Tw - 1), with the exact special cases T == Tw and T == 2 Tw.  It differs
+// from the integer t * Tw / T on a few frames of long sequences, but not for the 589-frame masks on the 125 trunk
+// frames of 10 s: t * 589 / 125 is an integer only at t = 0 and otherwise at least 1/125 away from one, far more than
+// the rounding error of t * (589.f / 125.f) for t < 125.
 __device__ __forceinline__ int nearest_src(int dst, int T, int Tw, float scale) {
   if (T == Tw) return dst;
   if (T == 2 * Tw) return dst >> 1;
@@ -352,7 +280,7 @@ __device__ __forceinline__ void store_split(__half* hi, __half* lo, size_t row, 
 
 struct PoolArgs {
   const void* x;          // NHWC fp16 feat, NCHW fp32 frames or fp32 rows
-  const float* w;         // [B][S][Tw] or NULL
+  const void* w;          // [B][S][Tw] u8 or fp32, or NULL
   int S, T, Tw, nslices;
   float scale;            // (float)Tw / T
   int Cv;                 // channels pooled (C, or fewer than the row width C of kPoolRows)
@@ -371,76 +299,129 @@ __device__ __forceinline__ const PoolX<L>* pool_row(const PoolArgs& a, int b, in
   else { *stride = C; return x + (size_t)b * a.F * C + c; }
 }
 
-// PHASE 0: the whole sequence in one slice, finished here (the stats_pool_kernel sums, in its order);
-// PHASE 1: per-slice fp32 sums; PHASE 2: per-slice sum of w (x - mean)^2 around the mean of all slices' sums.
-// grid (B * S * H, nslices, C / 256), thread = channel
-template <int PHASE, int L, int C>
+// A block pools a group of up to kSpeakers speakers of one sequence, so that it reads x once for all of them; each
+// speaker keeps its own sums, in the same order as a group of one.  Unweighted pooling has S = 1.
+// PHASE 0: the whole sequence in one slice, finished here; PHASE 1: per-slice fp32 sums; PHASE 2: per-slice sum of
+// w (x - mean)^2 around the mean of all slices' sums.  W: weight element type (u8 masks or fp32).
+// grid (B * ceil(S / kSpeakers) * H, nslices, C / 256), thread = channel
+template <int PHASE, int L, int C, typename W>
 __global__ void __launch_bounds__(256) wpool_kernel(PoolArgs a) {
   constexpr int H = pool_h<L>();
-  __shared__ float s_w[kPoolSlice];
-  const int row = blockIdx.x / H, h = blockIdx.x % H;                        // row = b * S + s
+  __shared__ float s_w[kSpeakers][kPoolSlice];
+  const int groups = (a.S + kSpeakers - 1) / kSpeakers;
+  const int grp = blockIdx.x / H, h = blockIdx.x % H;                        // grp = b * groups + g
+  const int b = grp / groups, s0 = (grp % groups) * kSpeakers, ns = min(kSpeakers, a.S - s0);
+  const int row0 = b * a.S + s0;                                             // row of speaker s0: b * S + s0
   const int c = (C == 256 ? 0 : (int)blockIdx.z * 256) + threadIdx.x;
-  const int b = row / a.S, sl = blockIdx.y;
-  const int t0 = sl * kPoolSlice, t1 = min(a.T, t0 + kPoolSlice);
+  const int sl = blockIdx.y;
+  const int t0 = sl * kPoolSlice, t1 = min(a.T, t0 + kPoolSlice), n = t1 - t0;
   size_t xs;
   const PoolX<L>* xp = pool_row<L, C>(a, b, h, c, &xs);
-  const bool weighted = a.w != nullptr;
+  // u8 weights are masks, always given: without the unweighted branch the mask kernel fits in 32 registers
+  const bool weighted = std::is_same<W, uint8_t>::value || a.w != nullptr;
   if (weighted) {
-    const float* wr = a.w + (size_t)row * a.Tw;
-    for (int i = threadIdx.x; i < t1 - t0; i += blockDim.x) s_w[i] = wr[nearest_src(t0 + i, a.T, a.Tw, a.scale)];
+    const W* w = static_cast<const W*>(a.w) + (size_t)row0 * a.Tw;
+    for (int i = threadIdx.x; i < ns * n; i += blockDim.x) {
+      const int s = i / n, t = i % n;
+      s_w[s][t] = (float)w[(size_t)s * a.Tw + nearest_src(t0 + t, a.T, a.Tw, a.scale)];
+    }
   }
   __syncthreads();
   if (L == kPoolRows && c >= a.Cv) return;                   // padding channels of the rows
-  double* part = a.part + (((size_t)row * H + h) * a.nslices) * 4 * C + c;      // slot k of slice j: [(j*4+k)*C]
+  // slot k of slice j of speaker s0 + s: part[s * pstride + (j * 4 + k) * C]
+  const size_t pstride = (size_t)H * a.nslices * 4 * C;
+  double* part = a.part + (((size_t)row0 * H + h) * a.nslices) * 4 * C + c;
   if (PHASE == 0 || PHASE == 1) {
-    float v1 = 0.f, v2 = 0.f, sx = 0.f;
+    float v1[kSpeakers], v2[kSpeakers], sx[kSpeakers];
+#pragma unroll
+    for (int s = 0; s < kSpeakers; ++s) { v1[s] = 0.f; v2[s] = 0.f; sx[s] = 0.f; }
     if (weighted) {
       for (int t = t0; t < t1; ++t) {
         const float x = to_f(xp[(size_t)t * xs]);
-        const float w = s_w[t - t0];
-        v1 += w;
-        v2 += w * w;
-        sx += x * w;
+#pragma unroll
+        for (int s = 0; s < kSpeakers; ++s) {
+          if (s < ns) {
+            const float w = s_w[s][t - t0];
+            v1[s] += w;
+            v2[s] += w * w;
+            sx[s] += x * w;
+          }
+        }
       }
     } else {
-      for (int t = t0; t < t1; ++t) sx += to_f(xp[(size_t)t * xs]);
+      for (int t = t0; t < t1; ++t) sx[0] += to_f(xp[(size_t)t * xs]);
     }
     if (PHASE == 1) {
-      part[(sl * 4 + 0) * C] = weighted ? (double)v1 : (double)sx;
-      part[(sl * 4 + 1) * C] = (double)v2;
-      part[(sl * 4 + 2) * C] = (double)sx;
+#pragma unroll
+      for (int s = 0; s < kSpeakers; ++s) {
+        if (s < ns) {
+          part[s * pstride + (sl * 4 + 0) * C] = weighted ? (double)v1[s] : (double)sx[s];
+          part[s * pstride + (sl * 4 + 1) * C] = (double)v2[s];
+          part[s * pstride + (sl * 4 + 2) * C] = (double)sx[s];
+        }
+      }
       return;
     }
-    const size_t orow = (size_t)row * a.ld_out;
     if (weighted) {
-      v1 += 1e-8f;
-      const float mean = sx / v1;
-      float sd = 0.f;
-      for (int t = t0; t < t1; ++t) {
-        const float d = to_f(xp[(size_t)t * xs]) - mean;
-        sd += d * d * s_w[t - t0];
+      float mean[kSpeakers], sd[kSpeakers];
+#pragma unroll
+      for (int s = 0; s < kSpeakers; ++s) {
+        v1[s] += 1e-8f;
+        mean[s] = sx[s] / v1[s];
+        sd[s] = 0.f;
       }
-      const float var = sd / (v1 - v2 / v1 + 1e-8f);
-      store_split(a.hi, a.lo, orow, c, h, H, a.Cv, mean, sqrtf(var));
+      for (int t = t0; t < t1; ++t) {
+        const float x = to_f(xp[(size_t)t * xs]);
+#pragma unroll
+        for (int s = 0; s < kSpeakers; ++s) {
+          if (s < ns) {
+            const float d = x - mean[s];
+            sd[s] += d * d * s_w[s][t - t0];
+          }
+        }
+      }
+#pragma unroll
+      for (int s = 0; s < kSpeakers; ++s) {
+        if (s < ns) {
+          const float var = sd[s] / (v1[s] - v2[s] / v1[s] + 1e-8f);
+          store_split(a.hi, a.lo, (size_t)(row0 + s) * a.ld_out, c, h, H, a.Cv, mean[s], sqrtf(var));
+        }
+      }
     } else {                                               // torch mean / std(correction=1): T = 1 gives NaN
-      const float mean = sx / a.T;
+      const float mean = sx[0] / a.T;
       float acc = 0.f;
       for (int t = t0; t < t1; ++t) {
         const float d = to_f(xp[(size_t)t * xs]) - mean;
         acc += d * d;
       }
-      store_split(a.hi, a.lo, orow, c, h, H, a.Cv, mean, sqrtf(acc / (a.T - 1)));
+      store_split(a.hi, a.lo, (size_t)row0 * a.ld_out, c, h, H, a.Cv, mean, sqrtf(acc / (a.T - 1)));
     }
   } else {
-    double s0 = 0.0, s2 = 0.0;                             // every slice's sums, in slice order
-    for (int j = 0; j < a.nslices; ++j) { s0 += part[(j * 4 + 0) * C]; s2 += part[(j * 4 + 2) * C]; }
-    const float mean = weighted ? (float)(s2 / (s0 + 1e-8)) : (float)(s0 / a.T);
-    float sd = 0.f;
-    for (int t = t0; t < t1; ++t) {
-      const float d = to_f(xp[(size_t)t * xs]) - mean;
-      sd += weighted ? d * d * s_w[t - t0] : d * d;
+    float mean[kSpeakers], sd[kSpeakers];
+#pragma unroll
+    for (int s = 0; s < kSpeakers; ++s) {
+      double m0 = 0.0, m2 = 0.0;                           // every slice's sums, in slice order
+      if (s < ns)
+        for (int j = 0; j < a.nslices; ++j) {
+          m0 += part[s * pstride + (j * 4 + 0) * C];
+          m2 += part[s * pstride + (j * 4 + 2) * C];
+        }
+      mean[s] = weighted ? (float)(m2 / (m0 + 1e-8)) : (float)(m0 / a.T);
+      sd[s] = 0.f;
     }
-    part[(sl * 4 + 3) * C] = (double)sd;
+    for (int t = t0; t < t1; ++t) {
+      const float x = to_f(xp[(size_t)t * xs]);
+#pragma unroll
+      for (int s = 0; s < kSpeakers; ++s) {
+        if (s < ns) {
+          const float d = x - mean[s];
+          sd[s] += weighted ? d * d * s_w[s][t - t0] : d * d;
+        }
+      }
+    }
+#pragma unroll
+    for (int s = 0; s < kSpeakers; ++s)
+      if (s < ns) part[s * pstride + (sl * 4 + 3) * C] = (double)sd[s];
   }
 }
 
@@ -474,19 +455,20 @@ size_t pool_scratch_bytes(int B, int S, int T, int C, int H) {
   return nslices > 1 ? (size_t)B * S * H * nslices * 4 * C * sizeof(double) : 0;
 }
 
-template <int L, int C>
-static void wpool_launch(const PoolArgs& a, size_t rows, cudaStream_t stream) {
-  const dim3 grid((unsigned)(rows * pool_h<L>()), (unsigned)a.nslices, C / 256);
+template <int L, int C, typename W>
+static void wpool_launch(const PoolArgs& a, int B, cudaStream_t stream) {
+  const unsigned H = pool_h<L>();
+  const dim3 grid((unsigned)B * ceil_div(a.S, kSpeakers) * H, (unsigned)a.nslices, C / 256);
   if (a.nslices == 1) {
-    wpool_kernel<0, L, C><<<grid, 256, 0, stream>>>(a);
+    wpool_kernel<0, L, C, W><<<grid, 256, 0, stream>>>(a);
   } else {
-    wpool_kernel<1, L, C><<<grid, 256, 0, stream>>>(a);
-    wpool_kernel<2, L, C><<<grid, 256, 0, stream>>>(a);
-    wpool_final_kernel<L, C><<<dim3(grid.x, 1, C / 256), 256, 0, stream>>>(a);
+    wpool_kernel<1, L, C, W><<<grid, 256, 0, stream>>>(a);
+    wpool_kernel<2, L, C, W><<<grid, 256, 0, stream>>>(a);
+    wpool_final_kernel<L, C><<<dim3((unsigned)B * a.S * H, 1, C / 256), 256, 0, stream>>>(a);
   }
 }
 
-static int pool_args(const void* x, const float* w, int B, int T, int S, int Tw, double* part, __half* stats_hi,
+static int pool_args(const void* x, const void* w, int B, int T, int S, int Tw, double* part, __half* stats_hi,
                      __half* stats_lo, PoolArgs* a) {
   B200_CHECK(x != nullptr && T >= 1 && S >= 1 && (w == nullptr ? S == 1 : Tw >= 1), B200_ERR_INVALID,
              "weighted pooling: bad arguments");
@@ -503,26 +485,32 @@ static int pool_args(const void* x, const float* w, int B, int T, int S, int Tw,
   return B200_OK;
 }
 
-int weighted_pool_forward(const __half* feat, const float* frames, const float* w, int B, int T, int S, int Tw, int C,
+template <typename W>
+int weighted_pool_forward(const __half* feat, const float* frames, const W* w, int B, int T, int S, int Tw, int C,
                           double* part, __half* stats_hi, __half* stats_lo, cudaStream_t stream) {
-  B200_CHECK((feat == nullptr) != (frames == nullptr), B200_ERR_INVALID, "weighted pooling: bad arguments");
+  constexpr bool fp32_w = std::is_same<W, float>::value;   // u8 masks: always given, on the trunk output only
+  B200_CHECK((feat == nullptr) != (frames == nullptr) && (fp32_w || (feat && w)), B200_ERR_INVALID,
+             "weighted pooling: bad arguments");
   PoolArgs a;
   int rc;
   if ((rc = pool_args(feat ? (const void*)feat : (const void*)frames, w, B, T, S, Tw, part, stats_hi, stats_lo, &a)))
     return rc;
   a.Cv = C; a.F = T; a.ld_out = 2 * 10 * C;
   B200_CHECK(C == 256 || C == 1024, B200_ERR_STATE, "weighted pooling: %d channels unsupported", C);
-  const size_t rows = (size_t)B * S;
-  if (C == 256) {
-    if (feat) wpool_launch<kPoolNHWC, 256>(a, rows, stream);
-    else wpool_launch<kPoolNCHW, 256>(a, rows, stream);
-  } else {
-    if (feat) wpool_launch<kPoolNHWC, 1024>(a, rows, stream);
-    else wpool_launch<kPoolNCHW, 1024>(a, rows, stream);
+  if (feat) {
+    if (C == 256) wpool_launch<kPoolNHWC, 256, W>(a, B, stream);
+    else wpool_launch<kPoolNHWC, 1024, W>(a, B, stream);
+  } else if constexpr (fp32_w) {
+    if (C == 256) wpool_launch<kPoolNCHW, 256, W>(a, B, stream);
+    else wpool_launch<kPoolNCHW, 1024, W>(a, B, stream);
   }
   B200_CUDA_OK(cudaGetLastError());
   return B200_OK;
 }
+template int weighted_pool_forward(const __half*, const float*, const uint8_t*, int, int, int, int, int, double*,
+                                   __half*, __half*, cudaStream_t);
+template int weighted_pool_forward(const __half*, const float*, const float*, int, int, int, int, int, double*,
+                                   __half*, __half*, cudaStream_t);
 
 int weighted_pool_rows(const float* x, int F, int T, int C, const float* w, int B, int S, int Tw, double* part,
                        __half* stats_hi, __half* stats_lo, int ld_out, cudaStream_t stream) {
@@ -532,7 +520,7 @@ int weighted_pool_rows(const float* x, int F, int T, int C, const float* w, int 
   B200_CHECK(C >= 1 && C <= kPoolRowsLd && T <= F && ld_out >= 2 * C, B200_ERR_INVALID,
              "weighted pooling: %d channels of %d-wide rows, %d of %d frames", C, kPoolRowsLd, T, F);
   a.Cv = C; a.F = F; a.ld_out = ld_out;
-  wpool_launch<kPoolRows, kPoolRowsLd>(a, (size_t)B * S, stream);
+  wpool_launch<kPoolRows, kPoolRowsLd, float>(a, B, stream);
   B200_CUDA_OK(cudaGetLastError());
   return B200_OK;
 }
