@@ -44,6 +44,7 @@ int b200_ctx_create(b200_ctx** ctx, int device);
 int b200_ctx_destroy(b200_ctx* ctx);
 /* Tuning / A-B options (no reference counterpart; results do not depend on the sub-batch sizes):
  *   "seg_max_batch" (2112) / "emb_max_batch" (264): chunks per sub-batch = workspace size (INTEGRATION.md section 4);
+ *   "ssl_max_batch" (32): 10 s windows per SSeRiouSS sub-batch, also the longest SSeRiouSS window (32 x 10 s);
  *   "conv_impl" 1 = wgmma tensor-core trunk convs (default), 0 = CUDA-core reference conv; "seg_gemm_impl" 1 = wgmma
  *   split-precision GEMMs, 0 = fp32 CUDA-core twins; "seg_conv_impl" 1 = SincNet sinc / Conv1d layers as split-precision
  *   wgmma implicit GEMMs, 0 = fp32 CUDA-core twins; "seg_rec_impl" 1 = LSTM recurrence as split-precision wgmma on
@@ -158,6 +159,74 @@ typedef struct b200_xvec_weights {
 /* Loads XVectorSincNet into the ctx's own slot: a PyanNet, a WeSpeaker ResNet and an XVectorSincNet stay resident
  * side by side.  fp16 (hi, lo) splits and the BatchNorm scale / shift are made here, once. */
 int b200_xvec_load(b200_ctx* ctx, const b200_xvec_weights* w);
+
+/* SSeRiouSS (models/segmentation/SSeRiouSS.py) on the WavLM Base front end (torchaudio WAVLM_BASE / WAVLM_BASE_PLUS:
+ * conv feature extractor without conv biases and GroupNorm on conv 0, 768-wide post-LN transformer of 12 layers with
+ * 12 heads and gated relative position bias), then the PyanNet head: 1-4 BiLSTM layers of 128 with 768 inputs, two
+ * Linear+LeakyReLU layers of 128 and the classifier (fields and layouts as in b200_seg_weights).  Keys below are those
+ * of the state dict without the "wav2vec." prefix. */
+#define B200_SSL_LAYERS 12
+#define B200_SSL_REL_SPAN 1023
+typedef struct b200_ssl_layer_weights {
+  const float* in_proj_weight;                /* attention.attention.in_proj_weight [2304][768] (q, k, v)  */
+  const float* in_proj_bias;                  /* [2304]                                                    */
+  const float* out_proj_weight;               /* attention.attention.out_proj.weight [768][768]            */
+  const float* out_proj_bias;
+  const float* gru_weight;                    /* attention.gru_rel_pos_linear.weight [8][64]               */
+  const float* gru_bias;                      /* [8]                                                       */
+  const float* gru_const;                     /* attention.gru_rel_pos_const [12]                          */
+  const float* layer_norm_weight;             /* layer_norm [768]                                          */
+  const float* layer_norm_bias;
+  const float* ff1_weight;                    /* feed_forward.intermediate_dense.weight [3072][768]        */
+  const float* ff1_bias;
+  const float* ff2_weight;                    /* feed_forward.output_dense.weight [768][3072]              */
+  const float* ff2_bias;
+  const float* final_layer_norm_weight;       /* final_layer_norm [768]                                    */
+  const float* final_layer_norm_bias;
+} b200_ssl_layer_weights;
+typedef struct b200_ssl_weights {
+  const float* conv0_weight;                  /* feature_extractor.conv_layers.0.conv.weight [512][1][10]  */
+  const float* conv0_norm_weight;             /* feature_extractor.conv_layers.0.layer_norm (GroupNorm) [512] */
+  const float* conv0_norm_bias;
+  const float* conv_weight[6];                /* conv_layers.{1..6}.conv.weight [512][512][3] x4, [512][512][2] x2 */
+  const float* proj_norm_weight;              /* encoder.feature_projection.layer_norm [512]               */
+  const float* proj_norm_bias;
+  const float* proj_weight;                   /* encoder.feature_projection.projection.weight [768][512]   */
+  const float* proj_bias;
+  const float* pos_conv_weight;               /* pos_conv_embed.conv weight with its weight norm folded [768][48][128] */
+  const float* pos_conv_bias;                 /* [768]                                                     */
+  const float* encoder_norm_weight;           /* encoder.transformer.layer_norm [768]: applied after the positional
+                                                 conv's residual, before layer 0                              */
+  const float* encoder_norm_bias;
+  const float* rel_attn_embed;                /* layers.0.attention.rel_attn_embed.weight [320][12]        */
+  const int32_t* rel_bucket;                  /* [2 * B200_SSL_REL_SPAN + 1]: bucket of the offset j - i = d at
+                                                 d + 1023 (offsets beyond +-1023 take the saturated end values) */
+  int32_t num_layers;                         /* transformer layers run: 12, or wav2vec_layer (1 .. 12)    */
+  b200_ssl_layer_weights layer[B200_SSL_LAYERS];
+  const float* layer_weights;                 /* [num_layers] softmax(wav2vec_weights); NULL: the output of layer
+                                                 num_layers alone (wav2vec_layer >= 1)                      */
+  int32_t lstm_layers;                        /* 1 .. 4                                                    */
+  const float* lstm_w_ih[8];                  /* lstm.weight_ih_l{k}[_reverse]: [512][768] for layer 0     */
+  const float* lstm_w_hh[8];
+  const float* lstm_b_ih[8];
+  const float* lstm_b_hh[8];
+  const float* linear_weight[2];              /* linear.{0,1}.weight [128][256], [128][128]                */
+  const float* linear_bias[2];
+  const float* classifier_weight;             /* [num_classes][128]                                        */
+  const float* classifier_bias;
+} b200_ssl_weights;
+/* Loads SSeRiouSS into the ctx's own slot: a PyanNet, a WeSpeaker ResNet, an XVectorSincNet and an SSeRiouSS stay
+ * resident side by side.  num_classes / activation as in b200_seg_load_head. */
+int b200_ssl_load(b200_ctx* ctx, const b200_ssl_weights* w, int32_t num_classes, int32_t activation);
+/* SSeRiouSS.forward on windows of any length window >= 400 samples (arguments as in b200_seg_forward_window):
+ * T = 1 + (window - 400) / 320 frames for window >= 400 (499 for 160000).  GroupNorm statistics are taken over the
+ * whole padded window.  Windows run in sub-batches of at most ssl_max_batch x 160000 samples (option ssl_max_batch,
+ * default 32: 320 s); one window longer than that returns B200_STATUS_INVALID naming the option. */
+int b200_ssl_forward_window(b200_ctx* ctx, const float* wav, const int64_t* chunk_off, const int32_t* chunk_valid,
+                            int32_t num_chunks, int32_t window, uint8_t* classes, float* logp, void* stream);
+/* The same for a sigmoid head, outputs as in b200_seg_forward_scores. */
+int b200_ssl_forward_scores(b200_ctx* ctx, const float* wav, const int64_t* chunk_off, const int32_t* chunk_valid,
+                            int32_t num_chunks, int32_t window, float* scores, float* max_scores, void* stream);
 
 /* ---- audio ingest: Audio.__call__ / Audio.downmix_and_resample (core/io.py:223-265, 306-351) -----------------
  * pcm is a DEVICE buffer holding the raw decoded audio: B200_PCM_S16_INTERLEAVED = int16 [frame][channel] (what a

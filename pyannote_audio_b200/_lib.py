@@ -55,6 +55,30 @@ class XvecWeights(C.Structure):
     ]
 
 
+class SslLayerWeights(C.Structure):
+    _fields_ = [(name, c_float_p) for name in (
+        "in_proj_weight", "in_proj_bias", "out_proj_weight", "out_proj_bias", "gru_weight", "gru_bias", "gru_const",
+        "layer_norm_weight", "layer_norm_bias", "ff1_weight", "ff1_bias", "ff2_weight", "ff2_bias",
+        "final_layer_norm_weight", "final_layer_norm_bias")]
+
+
+class SslWeights(C.Structure):
+    _fields_ = [
+        ("conv0_weight", c_float_p), ("conv0_norm_weight", c_float_p), ("conv0_norm_bias", c_float_p),
+        ("conv_weight", c_float_p * 6),
+        ("proj_norm_weight", c_float_p), ("proj_norm_bias", c_float_p), ("proj_weight", c_float_p),
+        ("proj_bias", c_float_p), ("pos_conv_weight", c_float_p), ("pos_conv_bias", c_float_p),
+        ("encoder_norm_weight", c_float_p), ("encoder_norm_bias", c_float_p),
+        ("rel_attn_embed", c_float_p), ("rel_bucket", C.POINTER(C.c_int32)),
+        ("num_layers", C.c_int32), ("layer", SslLayerWeights * 12), ("layer_weights", c_float_p),
+        ("lstm_layers", C.c_int32),
+        ("lstm_w_ih", c_float_p * 8), ("lstm_w_hh", c_float_p * 8),
+        ("lstm_b_ih", c_float_p * 8), ("lstm_b_hh", c_float_p * 8),
+        ("linear_weight", c_float_p * 2), ("linear_bias", c_float_p * 2),
+        ("classifier_weight", c_float_p), ("classifier_bias", c_float_p),
+    ]
+
+
 class B200Error(RuntimeError):
     pass
 
@@ -76,6 +100,11 @@ _PROTOS = {
     "b200_xvec_load": (C.c_int, [C.c_void_p, C.POINTER(XvecWeights)]),
     "b200_xvec_forward": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_int64, C.c_int32, C.c_void_p, C.c_int32,
                                     C.c_int32, C.c_void_p, C.c_void_p]),
+    "b200_ssl_load": (C.c_int, [C.c_void_p, C.POINTER(SslWeights), C.c_int32, C.c_int32]),
+    "b200_ssl_forward_window": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_int32, C.c_int32,
+                                          C.c_void_p, C.c_void_p, C.c_void_p]),
+    "b200_ssl_forward_scores": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_int32, C.c_int32,
+                                          C.c_void_p, C.c_void_p, C.c_void_p]),
     "b200_seg_forward": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_int32, C.c_void_p, C.c_void_p,
                                    C.c_void_p]),
     "b200_seg_forward_window": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_int32, C.c_int32,

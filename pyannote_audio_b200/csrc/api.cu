@@ -7,6 +7,7 @@
 #include "emb.cuh"
 #include "post.cuh"
 #include "seg.cuh"
+#include "ssl.cuh"
 #include <algorithm>
 #include <climits>
 #include <cmath>
@@ -49,6 +50,9 @@ struct b200_ctx {
   // chunks per embedding sub-batch: 264 = 2 x 132 SMs, so that the conv tiles of every layer (8 / 4 / 2 / 1 tiles
   // of 128 pixels per image row) split evenly over the machine
   int emb_max_batch = 264;
+  // windows of 10 s per SSeRiouSS sub-batch (any window length: at most ssl_max_batch x 160000 samples); ~140 MB of
+  // workspace per 10 s, most of it the conv feature extractor's channel-last activations
+  int ssl_max_batch = 32;
   int fbank_share = 1;          // 1 = overlapping hop-aligned chunks share their fbank frames (emb.cuh: FbankRun)
   // smallest linkage problem that runs on the whole GPU over packed distances (cluster.cuh); at most the default, so
   // that every problem the dense one-CTA kernel cannot hold goes there
@@ -57,7 +61,8 @@ struct b200_ctx {
   SegWeights seg;
   EmbWeights emb;
   XvecWeights xvec;
-  std::vector<void*> owned_seg, owned_emb, owned_xvec;   // device allocations holding the weights of each network
+  SslWeights ssl;
+  std::vector<void*> owned_seg, owned_emb, owned_xvec, owned_ssl;   // device allocations holding the weights of each network
   std::vector<void*>* owned = &owned_seg;    // where upload() records allocations (set by the load entry points)
   void* ws = nullptr;
   size_t ws_cap = 0;
@@ -374,6 +379,66 @@ int load_sincnet(b200_ctx* ctx, float wav_w, float wav_b, const float* sinc_filt
   return B200_OK;
 }
 
+// The BiLSTM stack (layer 0: in0 inputs padded to kpad0), linear layers and classifier that PyanNet and SSeRiouSS share
+// (b200_seg_weights / b200_ssl_weights fields of the same names)
+template <class Wt>
+int load_lstm_head(b200_ctx* ctx, const Wt* w, int in0, int kpad0, int num_classes, SegWeights& S) {
+  int rc;
+  for (int l = 0; l < S.lstm_layers; ++l) {
+    const int I = l == 0 ? in0 : 256, Kp = l == 0 ? kpad0 : 256;
+    S.k_in[l] = Kp;
+    std::vector<float> wih((size_t)1024 * Kp, 0.f), bg(1024), whh((size_t)2 * 2 * 128 * 256);
+    for (int d = 0; d < 2; ++d) {
+      const float *Wi = w->lstm_w_ih[l * 2 + d], *Wh = w->lstm_w_hh[l * 2 + d];
+      const float *bi = w->lstm_b_ih[l * 2 + d], *bh = w->lstm_b_hh[l * 2 + d];
+      B200_CHECK(Wi && Wh && bi && bh, B200_ERR_INVALID, "lstm layer %d dir %d missing", l, d);
+      for (int u = 0; u < 128; ++u)
+        for (int gt = 0; gt < 4; ++gt) {
+          const int n = d * 512 + u * 4 + gt, src = gt * 128 + u;
+          for (int k = 0; k < I; ++k) wih[(size_t)n * Kp + k] = Wi[(size_t)src * I + k];
+          bg[n] = bi[src] + bh[src];
+        }
+      for (int r = 0; r < 2; ++r)
+        for (int k = 0; k < 128; ++k)
+          for (int p = 0; p < 2; ++p)
+            for (int tx = 0; tx < 32; ++tx)
+              for (int gt = 0; gt < 4; ++gt) {
+                const int unit = 64 * r + 2 * tx + p;
+                whh[(((size_t)(d * 2 + r) * 128 + k) * 256) + p * 128 + tx * 4 + gt] = Wh[(size_t)(gt * 128 + unit) * 128 + k];
+              }
+    }
+    if ((rc = upload_split(ctx, wih, &S.w_ih_hi[l], &S.w_ih_lo[l]))) return rc;
+    if ((rc = upload(ctx, wih, &S.w_ih[l]))) return rc;
+    if ((rc = upload(ctx, bg, &S.b_g[l]))) return rc;
+    if ((rc = upload(ctx, whh, &S.w_hh[l]))) return rc;
+    // wgmma recurrence: [dir][rank][n = 32 jj + 8 gate + u][k = unit 0..127], local unit 8 jj + u
+    std::vector<float> whh_wg((size_t)4 * 256 * 128);
+    for (int d = 0; d < 2; ++d)
+      for (int r = 0; r < 2; ++r)
+        for (int n = 0; n < 256; ++n) {
+          const int unit = 64 * r + 8 * (n / 32) + n % 8, gt = (n / 8) % 4;
+          for (int k = 0; k < 128; ++k)
+            whh_wg[((size_t)(d * 2 + r) * 256 + n) * 128 + k] =
+                w->lstm_w_hh[l * 2 + d][(size_t)(gt * 128 + unit) * 128 + k];
+        }
+    if ((rc = upload_split(ctx, whh_wg, &S.w_hh_hi[l], &S.w_hh_lo[l]))) return rc;
+  }
+  const int lin_in[2] = {256, 128};
+  for (int i = 0; i < 2; ++i) {
+    B200_CHECK(w->linear_weight[i] && w->linear_bias[i], B200_ERR_INVALID, "linear.%d missing", i);
+    std::vector<float> lw(w->linear_weight[i], w->linear_weight[i] + 128 * lin_in[i]), lb(w->linear_bias[i], w->linear_bias[i] + 128);
+    if ((rc = upload_split(ctx, lw, &S.lin_w_hi[i], &S.lin_w_lo[i]))) return rc;
+    if ((rc = upload(ctx, lw, &S.lin_w[i]))) return rc;
+    if ((rc = upload(ctx, lb, &S.lin_b[i]))) return rc;
+  }
+  B200_CHECK(w->classifier_weight && w->classifier_bias, B200_ERR_INVALID, "classifier missing");
+  std::vector<float> cw(w->classifier_weight, w->classifier_weight + (size_t)num_classes * 128),
+      cb(w->classifier_bias, w->classifier_bias + num_classes);
+  if ((rc = upload(ctx, cw, &S.cls_w))) return rc;
+  if ((rc = upload(ctx, cb, &S.cls_b))) return rc;
+  return B200_OK;
+}
+
 }  // namespace
 
 extern "C" {
@@ -407,6 +472,7 @@ int b200_ctx_destroy(b200_ctx* ctx) {
   for (void* p : ctx->owned_seg) cudaFree(p);
   for (void* p : ctx->owned_emb) cudaFree(p);
   for (void* p : ctx->owned_xvec) cudaFree(p);
+  for (void* p : ctx->owned_ssl) cudaFree(p);
   for (auto& t : ctx->resample_tables) cudaFree(t.dev);
   if (ctx->ws) cudaFree(ctx->ws);
   if (ctx->d_off) cudaFree(ctx->d_off);
@@ -423,6 +489,7 @@ int b200_ctx_set_option(b200_ctx* ctx, const char* key, int64_t value) {
   if (k == "conv_impl") ctx->conv_impl = (int)value;
   else if (k == "seg_max_batch") ctx->seg_max_batch = (int)value;
   else if (k == "emb_max_batch") ctx->emb_max_batch = (int)value;
+  else if (k == "ssl_max_batch") ctx->ssl_max_batch = (int)value;
   else if (k == "profile") ctx->profile = (int)value;
   else if (k == "seg_gemm_impl") ctx->seg_gemm_impl = (int)value;
   else if (k == "seg_conv_impl") ctx->seg_conv_impl = (int)value;
@@ -434,7 +501,7 @@ int b200_ctx_set_option(b200_ctx* ctx, const char* key, int64_t value) {
     ctx->linkage_grid_min = (int)value;
   }
   else B200_CHECK(false, B200_ERR_INVALID, "unknown option '%s'", key);
-  B200_CHECK(ctx->seg_max_batch >= 1 && ctx->emb_max_batch >= 1 && ctx->conv_impl >= 0 && ctx->conv_impl <= 2 &&
+  B200_CHECK(ctx->seg_max_batch >= 1 && ctx->emb_max_batch >= 1 && ctx->ssl_max_batch >= 1 && ctx->conv_impl >= 0 && ctx->conv_impl <= 2 &&
                  ctx->seg_gemm_impl >= 0 && ctx->seg_gemm_impl <= 1 && ctx->seg_conv_impl >= 0 && ctx->seg_conv_impl <= 1 &&
                  ctx->seg_rec_impl >= 0 && ctx->seg_rec_impl <= 1,
              B200_ERR_INVALID, "option '%s' value %lld out of range", key, (long long)value);
@@ -530,58 +597,7 @@ int b200_seg_load_head(b200_ctx* ctx, const b200_seg_weights* w, int32_t num_cla
   if ((rc = load_sincnet(ctx, w->wav_norm_weight, w->wav_norm_bias, w->sinc_filters, w->norm_weight, w->norm_bias,
                          w->conv_weight, w->conv_bias, &S.sinc)))
     return rc;
-  for (int l = 0; l < S.lstm_layers; ++l) {
-    const int I = l == 0 ? 60 : 256, Kp = l == 0 ? 64 : 256;
-    S.k_in[l] = Kp;
-    std::vector<float> wih((size_t)1024 * Kp, 0.f), bg(1024), whh((size_t)2 * 2 * 128 * 256);
-    for (int d = 0; d < 2; ++d) {
-      const float *Wi = w->lstm_w_ih[l * 2 + d], *Wh = w->lstm_w_hh[l * 2 + d];
-      const float *bi = w->lstm_b_ih[l * 2 + d], *bh = w->lstm_b_hh[l * 2 + d];
-      B200_CHECK(Wi && Wh && bi && bh, B200_ERR_INVALID, "lstm layer %d dir %d missing", l, d);
-      for (int u = 0; u < 128; ++u)
-        for (int gt = 0; gt < 4; ++gt) {
-          const int n = d * 512 + u * 4 + gt, src = gt * 128 + u;
-          for (int k = 0; k < I; ++k) wih[(size_t)n * Kp + k] = Wi[(size_t)src * I + k];
-          bg[n] = bi[src] + bh[src];
-        }
-      for (int r = 0; r < 2; ++r)
-        for (int k = 0; k < 128; ++k)
-          for (int p = 0; p < 2; ++p)
-            for (int tx = 0; tx < 32; ++tx)
-              for (int gt = 0; gt < 4; ++gt) {
-                const int unit = 64 * r + 2 * tx + p;
-                whh[(((size_t)(d * 2 + r) * 128 + k) * 256) + p * 128 + tx * 4 + gt] = Wh[(size_t)(gt * 128 + unit) * 128 + k];
-              }
-    }
-    if ((rc = upload_split(ctx, wih, &S.w_ih_hi[l], &S.w_ih_lo[l]))) return rc;
-    if ((rc = upload(ctx, wih, &S.w_ih[l]))) return rc;
-    if ((rc = upload(ctx, bg, &S.b_g[l]))) return rc;
-    if ((rc = upload(ctx, whh, &S.w_hh[l]))) return rc;
-    // wgmma recurrence: [dir][rank][n = 32 jj + 8 gate + u][k = unit 0..127], local unit 8 jj + u
-    std::vector<float> whh_wg((size_t)4 * 256 * 128);
-    for (int d = 0; d < 2; ++d)
-      for (int r = 0; r < 2; ++r)
-        for (int n = 0; n < 256; ++n) {
-          const int unit = 64 * r + 8 * (n / 32) + n % 8, gt = (n / 8) % 4;
-          for (int k = 0; k < 128; ++k)
-            whh_wg[((size_t)(d * 2 + r) * 256 + n) * 128 + k] =
-                w->lstm_w_hh[l * 2 + d][(size_t)(gt * 128 + unit) * 128 + k];
-        }
-    if ((rc = upload_split(ctx, whh_wg, &S.w_hh_hi[l], &S.w_hh_lo[l]))) return rc;
-  }
-  const int lin_in[2] = {256, 128};
-  for (int i = 0; i < 2; ++i) {
-    B200_CHECK(w->linear_weight[i] && w->linear_bias[i], B200_ERR_INVALID, "linear.%d missing", i);
-    std::vector<float> lw(w->linear_weight[i], w->linear_weight[i] + 128 * lin_in[i]), lb(w->linear_bias[i], w->linear_bias[i] + 128);
-    if ((rc = upload_split(ctx, lw, &S.lin_w_hi[i], &S.lin_w_lo[i]))) return rc;
-    if ((rc = upload(ctx, lw, &S.lin_w[i]))) return rc;
-    if ((rc = upload(ctx, lb, &S.lin_b[i]))) return rc;
-  }
-  B200_CHECK(w->classifier_weight && w->classifier_bias, B200_ERR_INVALID, "classifier missing");
-  std::vector<float> cw(w->classifier_weight, w->classifier_weight + (size_t)num_classes * 128),
-      cb(w->classifier_bias, w->classifier_bias + num_classes);
-  if ((rc = upload(ctx, cw, &S.cls_w))) return rc;
-  if ((rc = upload(ctx, cb, &S.cls_b))) return rc;
+  if ((rc = load_lstm_head(ctx, w, 60, 64, num_classes, S))) return rc;
   S.loaded = true;
   return B200_OK;
 }
@@ -693,7 +709,7 @@ static int seg_run(b200_ctx* ctx, const float* wav, const int64_t* chunk_off, co
   const int T = geom.pool2;
   const int nbmax = (int)std::min<int64_t>(std::min<int64_t>(n, budget / window), 65535);
   const size_t x0_bytes = align_up((size_t)nbmax * T * 64 * sizeof(float), 1024);
-  const size_t sinc_b = sincnet_workspace_bytes(geom, nbmax), lstm_b = lstm_workspace_bytes(nbmax, T);
+  const size_t sinc_b = sincnet_workspace_bytes(geom, nbmax), lstm_b = lstm_workspace_bytes(nbmax, T, 64);
   const size_t big = sinc_b > lstm_b ? sinc_b : lstm_b;    // the two phases reuse the same region
   int rc = ensure_ws(ctx, x0_bytes + big + 4096);
   if (rc) return rc;
@@ -751,6 +767,185 @@ int b200_seg_forward_scores(b200_ctx* ctx, const float* wav, const int64_t* chun
 int b200_seg_forward(b200_ctx* ctx, const float* wav, const int64_t* chunk_off, const int32_t* chunk_valid,
                      int32_t num_chunks, uint8_t* classes, float* logp, void* stream) {
   return b200_seg_forward_window(ctx, wav, chunk_off, chunk_valid, num_chunks, kChunk, classes, logp, stream);
+}
+
+// ------------------------------------------------------------------------------------------------------
+int b200_ssl_load(b200_ctx* ctx, const b200_ssl_weights* w, int32_t num_classes, int32_t activation) {
+  B200_CHECK(ctx && w, B200_ERR_INVALID, "NULL ctx/weights");
+  B200_CHECK(num_classes >= 1 && num_classes <= kSegMaxClasses, B200_ERR_INVALID,
+             "a classifier of %d classes is unsupported (1 .. %d)", (int)num_classes, kSegMaxClasses);
+  B200_CHECK(activation == B200_SEG_LOGSOFTMAX || activation == B200_SEG_SIGMOID, B200_ERR_INVALID,
+             "unknown classifier activation %d (B200_SEG_LOGSOFTMAX = 0, B200_SEG_SIGMOID = 1)", (int)activation);
+  B200_CHECK(w->lstm_layers >= 1 && w->lstm_layers <= 4, B200_ERR_INVALID, "lstm_layers=%d unsupported",
+             (int)w->lstm_layers);
+  B200_CHECK(w->num_layers >= 1 && w->num_layers <= kSslLayers, B200_ERR_INVALID, "num_layers=%d unsupported (1 .. 12)",
+             (int)w->num_layers);
+  B200_CHECK(w->conv0_weight && w->conv0_norm_weight && w->conv0_norm_bias && w->proj_norm_weight &&
+                 w->proj_norm_bias && w->proj_weight && w->proj_bias && w->pos_conv_weight && w->pos_conv_bias &&
+                 w->encoder_norm_weight && w->encoder_norm_bias &&
+                 w->rel_attn_embed && w->rel_bucket,
+             B200_ERR_INVALID, "WavLM front-end weights missing");
+  for (int l = 0; l < 6; ++l) B200_CHECK(w->conv_weight[l], B200_ERR_INVALID, "conv_layers.%d missing", l + 1);
+  for (int l = 0; l < w->num_layers; ++l) {
+    const b200_ssl_layer_weights& L = w->layer[l];
+    B200_CHECK(L.in_proj_weight && L.in_proj_bias && L.out_proj_weight && L.out_proj_bias && L.gru_weight &&
+                   L.gru_bias && L.gru_const && L.layer_norm_weight && L.layer_norm_bias && L.ff1_weight &&
+                   L.ff1_bias && L.ff2_weight && L.ff2_bias && L.final_layer_norm_weight && L.final_layer_norm_bias,
+               B200_ERR_INVALID, "transformer layer %d missing", l);
+  }
+  for (int i = 0; i < 2 * kSslRelSpan + 1; ++i)
+    B200_CHECK(w->rel_bucket[i] >= 0 && w->rel_bucket[i] < 320, B200_ERR_INVALID, "relative bucket %d out of range",
+               (int)w->rel_bucket[i]);
+  DeviceGuard g(ctx->device);
+  SslWeights& X = ctx->ssl;
+  X.loaded = false;
+  release_weights(ctx, &ctx->owned_ssl);
+  X.head = SegWeights();
+  X.head.lstm_layers = w->lstm_layers;
+  X.head.num_classes = num_classes;
+  X.head.activation = activation == B200_SEG_SIGMOID ? kSegSigmoid : kSegLogSoftmax;
+  int rc;
+  auto up = [&](const float* src, size_t n, float** dst) {
+    return upload(ctx, std::vector<float>(src, src + n), dst);
+  };
+  auto up_split = [&](const float* src, size_t n, __half** hi, __half** lo) {
+    return upload_split(ctx, std::vector<float>(src, src + n), hi, lo);
+  };
+  const int C = kSslConvDim, D = kSslDim;
+  if ((rc = up(w->conv0_weight, (size_t)C * 10, &X.conv0_w))) return rc;
+  if ((rc = up(w->conv0_norm_weight, C, &X.gn_w))) return rc;
+  if ((rc = up(w->conv0_norm_bias, C, &X.gn_b))) return rc;
+  // convs 1-6 on pair rows: B[n][tap * 512 + c] = W[n][c][tap], taps padded to an even count with zeros
+  for (int l = 0; l < 6; ++l) {
+    const int k = l < 4 ? 3 : 2, K = l < 4 ? 2048 : 1024;
+    std::vector<float> b((size_t)C * K, 0.f);
+    for (int n = 0; n < C; ++n)
+      for (int c = 0; c < C; ++c)
+        for (int t = 0; t < k; ++t) b[(size_t)n * K + t * C + c] = w->conv_weight[l][((size_t)n * C + c) * k + t];
+    if ((rc = upload_split(ctx, b, &X.conv_hi[l], &X.conv_lo[l]))) return rc;
+  }
+  if ((rc = up(w->proj_norm_weight, C, &X.fp_ln_w))) return rc;
+  if ((rc = up(w->proj_norm_bias, C, &X.fp_ln_b))) return rc;
+  if ((rc = up_split(w->proj_weight, (size_t)D * C, &X.proj_hi, &X.proj_lo))) return rc;
+  if ((rc = up(w->proj_bias, D, &X.proj_b))) return rc;
+  {  // positional conv per group: B_g[n][tap * 64 + c] = W[48 g + n][c][tap] (n, c < 48), bias [16][128]
+    const int Kp = kSslPosK * 64;
+    std::vector<float> b((size_t)kSslPosGroups * 128 * Kp, 0.f), bias((size_t)kSslPosGroups * 128, 0.f);
+    for (int gi = 0; gi < kSslPosGroups; ++gi)
+      for (int n = 0; n < 48; ++n) {
+        bias[gi * 128 + n] = w->pos_conv_bias[gi * 48 + n];
+        for (int c = 0; c < 48; ++c)
+          for (int t = 0; t < kSslPosK; ++t)
+            b[((size_t)gi * 128 + n) * Kp + t * 64 + c] = w->pos_conv_weight[((size_t)(gi * 48 + n) * 48 + c) * kSslPosK + t];
+      }
+    if ((rc = upload_split(ctx, b, &X.pos_hi, &X.pos_lo))) return rc;
+    if ((rc = upload(ctx, bias, &X.pos_b))) return rc;
+  }
+  if ((rc = up(w->encoder_norm_weight, D, &X.enc_ln_w))) return rc;
+  if ((rc = up(w->encoder_norm_bias, D, &X.enc_ln_b))) return rc;
+  {
+    std::vector<float> tab((size_t)kSslHeads * (2 * kSslRelSpan + 1));
+    for (int h = 0; h < kSslHeads; ++h)
+      for (int i = 0; i < 2 * kSslRelSpan + 1; ++i)
+        tab[(size_t)h * (2 * kSslRelSpan + 1) + i] = w->rel_attn_embed[w->rel_bucket[i] * kSslHeads + h];
+    if ((rc = upload(ctx, tab, &X.rel_tab))) return rc;
+  }
+  X.num_layers = w->num_layers;
+  for (int l = 0; l < kSslLayers; ++l) X.layer_w[l] = 0.f;
+  for (int l = 0; l < w->num_layers; ++l) {
+    const b200_ssl_layer_weights& L = w->layer[l];
+    SslLayerWeights& Y = X.layer[l];
+    Y = SslLayerWeights();
+    X.layer_w[l] = w->layer_weights ? w->layer_weights[l] : (l == w->num_layers - 1 ? 1.f : 0.f);
+    if ((rc = up_split(L.in_proj_weight, (size_t)3 * D * D, &Y.qkv_hi, &Y.qkv_lo))) return rc;
+    if ((rc = up(L.in_proj_bias, 3 * D, &Y.qkv_b))) return rc;
+    if ((rc = up_split(L.out_proj_weight, (size_t)D * D, &Y.out_hi, &Y.out_lo))) return rc;
+    if ((rc = up(L.out_proj_bias, D, &Y.out_b))) return rc;
+    if ((rc = up(L.gru_weight, 8 * 64, &Y.gru_w))) return rc;
+    if ((rc = up(L.gru_bias, 8, &Y.gru_b))) return rc;
+    if ((rc = up(L.gru_const, kSslHeads, &Y.gru_const))) return rc;
+    if ((rc = up(L.layer_norm_weight, D, &Y.ln1_w))) return rc;
+    if ((rc = up(L.layer_norm_bias, D, &Y.ln1_b))) return rc;
+    if ((rc = up_split(L.ff1_weight, (size_t)kSslFfn * D, &Y.ff1_hi, &Y.ff1_lo))) return rc;
+    if ((rc = up(L.ff1_bias, kSslFfn, &Y.ff1_b))) return rc;
+    if ((rc = up_split(L.ff2_weight, (size_t)D * kSslFfn, &Y.ff2_hi, &Y.ff2_lo))) return rc;
+    if ((rc = up(L.ff2_bias, D, &Y.ff2_b))) return rc;
+    if ((rc = up(L.final_layer_norm_weight, D, &Y.ln2_w))) return rc;
+    if ((rc = up(L.final_layer_norm_bias, D, &Y.ln2_b))) return rc;
+  }
+  if ((rc = load_lstm_head(ctx, w, D, D, num_classes, X.head))) return rc;
+  X.loaded = true;
+  return B200_OK;
+}
+
+// SSeRiouSS on n windows of `window` samples, in sub-batches of at most ssl_max_batch x 160000 samples
+static int ssl_run(b200_ctx* ctx, const float* wav, const int64_t* chunk_off, const int32_t* chunk_valid, int n,
+                   int window, const SegHeadOut& out, cudaStream_t st) {
+  B200_CHECK(ctx && ctx->ssl.loaded, B200_ERR_STATE, "SSeRiouSS weights not loaded");
+  B200_CHECK(wav && chunk_off && chunk_valid && n >= 0, B200_ERR_INVALID, "bad arguments");
+  B200_CHECK(window >= kSslMinWindow, B200_ERR_INVALID,
+             "windows of %d samples are too short: SSeRiouSS needs at least %d samples (one WavLM frame)", window,
+             kSslMinWindow);
+  const int64_t budget = (int64_t)ctx->ssl_max_batch * kChunk;
+  B200_CHECK(window <= budget, B200_ERR_INVALID,
+             "a window of %d samples is longer than the %lld samples of one SSeRiouSS sub-batch (ssl_max_batch %d x "
+             "160000): set the option ssl_max_batch to at least %lld, or segment shorter excerpts",
+             window, (long long)budget, ctx->ssl_max_batch, (long long)((window + kChunk - 1) / kChunk));
+  if (n == 0) return B200_OK;
+  DeviceGuard g(ctx->device);
+  const SslGeom geom = ssl_geom(window);
+  const int T = geom.T;
+  const int nbmax = (int)std::min<int64_t>(std::min<int64_t>(n, budget / window), 65535);
+  const size_t x0_bytes = align_up((size_t)nbmax * T * kSslDim * sizeof(float), 1024);
+  const size_t fe_b = ssl_workspace_bytes(geom, nbmax), lstm_b = lstm_workspace_bytes(nbmax, T, kSslDim);
+  int rc = ensure_ws(ctx, x0_bytes + std::max(fe_b, lstm_b) + 4096);   // the LSTM reuses the front end's region
+  if (rc) return rc;
+  if ((rc = push_meta(ctx, chunk_off, chunk_valid, n, st, window))) return rc;
+  float* x0 = reinterpret_cast<float*>(ctx->ws);
+  void* region = reinterpret_cast<char*>(ctx->ws) + x0_bytes;
+  const SslWeights& X = ctx->ssl;
+  for (int c0 = 0; c0 < n; c0 += nbmax) {
+    const int nb = (n - c0) < nbmax ? (n - c0) : nbmax;
+    if ((rc = ssl_frontend_forward(X, geom, wav, ctx->d_off + c0, ctx->d_valid + c0, nb, region, x0, ctx->num_sms, st)))
+      return rc;
+    const size_t row0 = (size_t)c0 * T, K = X.head.num_classes;
+    SegHeadOut sub;
+    sub.cls = out.cls ? out.cls + row0 : nullptr;
+    sub.logp = out.logp ? out.logp + row0 * K : nullptr;
+    sub.scores = out.scores ? out.scores + row0 * K : nullptr;
+    sub.max_scores = out.max_scores ? out.max_scores + row0 : nullptr;
+    if ((rc = lstm_head_forward(X.head, x0, nb, T, region, sub, ctx->num_sms, ctx->seg_gemm_impl, ctx->seg_rec_impl,
+                                st)))
+      return rc;
+    // conv 0 + GroupNorm (3), convs 1-6, LayerNorm, projection, positional conv (pack, 16 GEMMs, add), LayerNorm,
+    // 7 per layer
+    ctx->launches += 30 + 7 * X.num_layers + 2 * X.head.lstm_layers + 3;
+  }
+  return B200_OK;
+}
+
+int b200_ssl_forward_window(b200_ctx* ctx, const float* wav, const int64_t* chunk_off, const int32_t* chunk_valid,
+                            int32_t num_chunks, int32_t window, uint8_t* classes, float* logp, void* stream) {
+  B200_CHECK(!(ctx && ctx->ssl.loaded && ctx->ssl.head.activation != kSegLogSoftmax), B200_ERR_INVALID,
+             "the loaded SSeRiouSS head is a sigmoid (multi-label / binary) head: call b200_ssl_forward_scores");
+  if (num_chunks == 0) return B200_OK;
+  B200_CHECK(classes != nullptr, B200_ERR_INVALID, "classes is NULL");
+  SegHeadOut out;
+  out.cls = classes;
+  out.logp = logp;
+  return ssl_run(ctx, wav, chunk_off, chunk_valid, num_chunks, window, out, (cudaStream_t)stream);
+}
+
+int b200_ssl_forward_scores(b200_ctx* ctx, const float* wav, const int64_t* chunk_off, const int32_t* chunk_valid,
+                            int32_t num_chunks, int32_t window, float* scores, float* max_scores, void* stream) {
+  B200_CHECK(!(ctx && ctx->ssl.loaded && ctx->ssl.head.activation != kSegSigmoid), B200_ERR_INVALID,
+             "the loaded SSeRiouSS head is a log-softmax (powerset / mono-label) head: call b200_ssl_forward_window");
+  if (num_chunks == 0) return B200_OK;
+  B200_CHECK(scores || max_scores, B200_ERR_INVALID, "scores and max_scores are both NULL");
+  SegHeadOut out;
+  out.scores = scores;
+  out.max_scores = max_scores;
+  return ssl_run(ctx, wav, chunk_off, chunk_valid, num_chunks, window, out, (cudaStream_t)stream);
 }
 
 __global__ void strip_pad_kernel(const float* __restrict__ x64, float* __restrict__ out, size_t rows) {

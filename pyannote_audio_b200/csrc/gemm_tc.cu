@@ -30,7 +30,7 @@ constexpr uint32_t kGemmStageBytes = 4 * kGemmTile;
 struct GemmTcParams {
   int M, N, K, kblocks, tiles_n, act;
   const float* bias;
-  float* C;            // fp32 output [M][ldc] or nullptr
+  float* C;            // fp32 output [M][ldc] or nullptr  (act: 0 none, 1 LeakyReLU(0.01), 2 GELU)
   __half* C_hi;        // optional split output [M][ldc_h]
   __half* C_lo;
   int ldc, ldc_h;
@@ -45,6 +45,8 @@ struct GemmTcParams {
   const float* shift;
 };
 
+// GELU: the exact-GELU epilogue (act 2) is a separate instantiation, so that the other epilogues compile as before
+template <bool GELU>
 __global__ void __launch_bounds__(kGemmThreads, 1)
 gemm_tc_split_kernel(const __grid_constant__ CUtensorMap tmAh, const __grid_constant__ CUtensorMap tmAl,
                      const __grid_constant__ CUtensorMap tmBh, const __grid_constant__ CUtensorMap tmBl,
@@ -120,6 +122,10 @@ gemm_tc_split_kernel(const __grid_constant__ CUtensorMap tmAh, const __grid_cons
       float a = acc[4 * j + 2 * i], c = acc[4 * j + 2 * i + 1];
       if (p.bias) { a += p.bias[col]; c += p.bias[col + 1]; }
       if (p.act == 1) { a = a > 0.f ? a : 0.01f * a; c = c > 0.f ? c : 0.01f * c; }
+      if (GELU) {                                           // exact (erf) GELU, torch.nn.functional.gelu's default
+        a = 0.5f * a * (1.f + erff(a * 0.70710678118654752f));
+        c = 0.5f * c * (1.f + erff(c * 0.70710678118654752f));
+      }
       if (p.scale) { a = a * p.scale[col] + p.shift[col]; c = c * p.scale[col + 1] + p.shift[col + 1]; }
       if (p.C) {
         const float2 v = make_float2(a, c);
@@ -192,9 +198,10 @@ int gemm_tc_split(const __half* A_hi, const __half* A_lo, int lda, const __half*
   if ((rc = encode_f16_map(&tmBh, 2, B_hi, b_dims, b_str, b_box, nullptr, swz, "gemm"))) return rc;
   if ((rc = encode_f16_map(&tmBl, 2, B_lo, b_dims, b_str, b_box, nullptr, swz, "gemm"))) return rc;
   const size_t smem = 1024 + 1024 + (size_t)kGemmStages * kGemmStageBytes;
-  B200_CUDA_OK(cudaFuncSetAttribute(gemm_tc_split_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+  const auto kernel = act == 2 ? gemm_tc_split_kernel<true> : gemm_tc_split_kernel<false>;
+  B200_CUDA_OK(cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
   const unsigned grid = (unsigned)(ceil_div(M, kGemmM) * p.tiles_n);
-  gemm_tc_split_kernel<<<grid, kGemmThreads, smem, stream>>>(tmAh, tmAl, tmBh, tmBl, p);
+  kernel<<<grid, kGemmThreads, smem, stream>>>(tmAh, tmAl, tmBh, tmBl, p);
   B200_CUDA_OK(cudaGetLastError());
   return B200_OK;
 }

@@ -114,8 +114,9 @@ struct SegHeadOut {
   float* scores = nullptr;
   float* max_scores = nullptr;
 };
-// BiLSTM stack + linear layers + classifier on sequences of T frames
-size_t lstm_workspace_bytes(int NB, int T);
+// BiLSTM stack + linear layers + classifier on sequences of T frames of k0 = W.k_in[0] features (64: PyanNet's 60
+// SincNet features and 4 zero columns; 768: SSeRiouSS)
+size_t lstm_workspace_bytes(int NB, int T, int k0);
 int lstm_head_forward(const SegWeights& W, const float* x0, int NB, int T, void* ws, const SegHeadOut& out,
                       int num_sms, int gemm_impl, int rec_impl, cudaStream_t stream);
 

@@ -213,7 +213,7 @@ struct LstmWs {
   float *Gx, *Ya, *Yb, *Z1, *Z2;
   __half *Xh, *Xl, *Yah, *Yal, *Ybh, *Ybl, *Z1h, *Z1l;
 };
-static size_t carve_lstm(int NB, int T, void* base, LstmWs* w) {
+static size_t carve_lstm(int NB, int T, int k0, void* base, LstmWs* w) {
   Workspace ws(base, 256);
   LstmWs t;
   const size_t M = (size_t)NB * T;
@@ -222,8 +222,8 @@ static size_t carve_lstm(int NB, int T, void* base, LstmWs* w) {
   t.Yb = (float*)ws.take(M * 256 * sizeof(float));
   t.Z1 = (float*)ws.take(M * 128 * sizeof(float));
   t.Z2 = (float*)ws.take(M * 128 * sizeof(float));
-  t.Xh = (__half*)ws.take(M * 64 * sizeof(__half));
-  t.Xl = (__half*)ws.take(M * 64 * sizeof(__half));
+  t.Xh = (__half*)ws.take(M * k0 * sizeof(__half));
+  t.Xl = (__half*)ws.take(M * k0 * sizeof(__half));
   t.Yah = (__half*)ws.take(M * 256 * sizeof(__half));
   t.Yal = (__half*)ws.take(M * 256 * sizeof(__half));
   t.Ybh = (__half*)ws.take(M * 256 * sizeof(__half));
@@ -233,7 +233,7 @@ static size_t carve_lstm(int NB, int T, void* base, LstmWs* w) {
   if (w) *w = t;
   return ws.bytes();
 }
-size_t lstm_workspace_bytes(int NB, int T) { return carve_lstm(NB, T, nullptr, nullptr); }
+size_t lstm_workspace_bytes(int NB, int T, int k0) { return carve_lstm(NB, T, k0, nullptr, nullptr); }
 
 template <int RB>
 static int launch_rec(const float* Gx, const float* Whh, float* Y, __half* Yh, __half* Yl, int NB, int T,
@@ -250,14 +250,14 @@ static int launch_rec(const float* Gx, const float* Whh, float* Y, __half* Yh, _
 int lstm_head_forward(const SegWeights& W, const float* x0, int NB, int T, void* ws, const SegHeadOut& out,
                       int num_sms, int gemm_impl, int rec_impl, cudaStream_t stream) {
   LstmWs w;
-  carve_lstm(NB, T, ws, &w);
+  carve_lstm(NB, T, W.k_in[0], ws, &w);
   const int M = NB * T;          // rows of every GEMM (< 2^31); element offsets M * 1024 are formed in size_t
   const int clusters = num_sms / 2;
   const bool tc = gemm_impl != 0;
   int rc;
   const float* in = x0;
   const __half *in_h = w.Xh, *in_l = w.Xl;
-  if (tc && (rc = split_f16(x0, w.Xh, w.Xl, (size_t)M * 64, stream))) return rc;
+  if (tc && (rc = split_f16(x0, w.Xh, w.Xl, (size_t)M * W.k_in[0], stream))) return rc;
   float* outs[2] = {w.Ya, w.Yb};
   __half* outs_h[2] = {w.Yah, w.Ybh};
   __half* outs_l[2] = {w.Yal, w.Ybl};

@@ -115,7 +115,7 @@ class Inference(BaseInference):
         ``reduce_max`` their per-frame maximum (C,F,1)."""
         window_size = self.model.audio.get_num_samples(self.duration)
         step_size = round(self.step * sample_rate)
-        ops.check_seg_window(window_size)
+        self.model.check_window(window_size)
         _, num_samples = waveform.shape
         off, valid, num_chunks, has_last = chunk_layout(num_samples, window_size, step_size)
         ctx = self.model._ctx()

@@ -7,6 +7,7 @@ Reference interfaces mirrored (paths relative to /root/reference/src/pyannote/au
   models/segmentation/PyanNet.py:92-240 (ctor hyper-parameters, num_frames, receptive field, forward)
   models/embedding/wespeaker/__init__.py:41-466 (forward / forward_frames / forward_embedding / dimension)
   models/embedding/xvector.py:205-349 (XVectorSincNet)
+  models/segmentation/SSeRiouSS.py (SSeRiouSS on WavLM Base; module tree of torchaudio's wavlm_model)
 """
 from __future__ import annotations
 
@@ -60,7 +61,7 @@ class Model(nn.Module):
         self._weights_version = 0
         self.register_load_state_dict_post_hook(lambda module, incompatible: module._bump_weights())
 
-    _SLOT = ""          # "seg" | "emb" | "xvec": the context slot this model family uploads into
+    _SLOT = ""          # "seg" | "emb" | "xvec" | "ssl": the context slot this model family uploads into
 
     def _bump_weights(self):
         self._weights_version += 1
@@ -120,10 +121,10 @@ class Model(nn.Module):
         class_name = meta["architecture"]["class"]
         klass = {"PyanNet": PyanNet, "WeSpeakerResNet34": WeSpeakerResNet34, "WeSpeakerResNet152": WeSpeakerResNet152,
                  "WeSpeakerResNet221": WeSpeakerResNet221, "WeSpeakerResNet293": WeSpeakerResNet293,
-                 "XVectorSincNet": XVectorSincNet}.get(class_name)
+                 "XVectorSincNet": XVectorSincNet, "SSeRiouSS": SSeRiouSS}.get(class_name)
         if klass is None:
             raise NotImplementedError(f"architecture {meta['architecture']['module']}.{class_name} has no CUDA "
-                                      f"implementation (PyanNet, WeSpeakerResNet34 / 152 / 221 / 293 and "
+                                      f"implementation (PyanNet, SSeRiouSS, WeSpeakerResNet34 / 152 / 221 / 293 and "
                                       f"XVectorSincNet have one)")
         if cls not in (Model, klass) and not issubclass(klass, cls):
             raise ValueError(f"checkpoint holds a {class_name}, not a {cls.__name__}")
@@ -279,7 +280,7 @@ class PyanNet(Model):
         PyanNet.py:152-161): the classifier becomes a fresh Linear(128, dimension).  Heads without a kernel (more than
         32 classes, or a problem that is not a classification) are refused here, before any device work."""
         if isinstance(specifications, (tuple, list)):
-            raise ValueError("PyanNet does not support multi-tasking.")
+            raise ValueError(f"{type(self).__name__} does not support multi-tasking.")
         if not isinstance(specifications, Specifications):
             raise ValueError("Only regular specifications or tuple of specifications are supported.")
         ops.seg_activation(specifications)
@@ -313,6 +314,10 @@ class PyanNet(Model):
         for k, s in reversed(list(zip(self.KERNEL, self.STRIDE))):
             c = c * s + (k - 1) // 2
         return c
+
+    def check_window(self, num_samples: int):
+        """Refuses windows too short for the kernels (Inference checks its window with this)."""
+        ops.check_seg_window(num_samples)
 
     def _upload(self, ctx):
         ctx.load_segmentation(self.state_dict(), self.specifications)
@@ -634,3 +639,199 @@ class XVectorSincNet(Model):
         flat = waveforms.to(device=ctx.device, dtype=torch.float32).reshape(-1).contiguous()
         emb = self.forward_utterances(flat, np.arange(b, dtype=np.int64) * s, s, weights=weights)
         return emb if weights is not None and weights.dim() == 3 else emb[:, 0]
+
+
+# ---- SSeRiouSS ----------------------------------------------------------------------------------------------------
+# torchaudio.pipelines.WAVLM_BASE._params (== WAVLM_BASE_PLUS._params): the only front-end configuration the kernels
+# implement.  The package does not import torchaudio; the table is written out here.
+WAVLM_BASE_PARAMS = {
+    "extractor_mode": "group_norm", "extractor_conv_bias": False,
+    "extractor_conv_layer_config": [(512, 10, 5)] + [(512, 3, 2)] * 4 + [(512, 2, 2)] * 2,
+    "encoder_embed_dim": 768, "encoder_pos_conv_kernel": 128, "encoder_pos_conv_groups": 16,
+    "encoder_num_layers": 12, "encoder_num_heads": 12, "encoder_max_distance": 800, "encoder_num_buckets": 320,
+    "encoder_ff_interm_features": 3072, "encoder_layer_norm_first": False,
+}
+SSL_BUNDLES = ("WAVLM_BASE", "WAVLM_BASE_PLUS")
+
+
+class _ConvLayerParams(nn.Module):
+    def __init__(self, cin, k, s, norm):
+        super().__init__()
+        self.conv = nn.Conv1d(cin, 512, k, stride=s, bias=False)
+        if norm:
+            self.layer_norm = nn.GroupNorm(512, 512)
+
+
+class _FeatureExtractorParams(nn.Module):
+    def __init__(self):
+        super().__init__()
+        self.conv_layers = nn.ModuleList(
+            [_ConvLayerParams(1 if i == 0 else 512, k, s, i == 0)
+             for i, (_, k, s) in enumerate(WAVLM_BASE_PARAMS["extractor_conv_layer_config"])])
+
+
+class _WeightNormParams(nn.Module):
+    """torch.nn.utils.parametrizations.weight_norm(dim=2) of the positional conv: original0 = g, original1 = v."""
+
+    def __init__(self):
+        super().__init__()
+        self.original0 = nn.Parameter(torch.ones(1, 1, 128))
+        self.original1 = nn.Parameter(torch.randn(768, 48, 128) * 0.02)
+
+
+class _PosConvParams(nn.Module):
+    """pos_conv_embed.conv with the parametrization's key names.  Checkpoints saved with the older
+    torch.nn.utils.weight_norm spell the pair ``weight_g`` / ``weight_v``; they are renamed on load."""
+
+    def __init__(self):
+        super().__init__()
+        self.bias = nn.Parameter(torch.zeros(768))
+        self.parametrizations = nn.Module()
+        self.parametrizations.weight = _WeightNormParams()
+        self._register_load_state_dict_pre_hook(self._rename_weight_norm)
+
+    @staticmethod
+    def _rename_weight_norm(state_dict, prefix, *args):
+        for old, new in (("weight_g", "parametrizations.weight.original0"),
+                         ("weight_v", "parametrizations.weight.original1")):
+            if prefix + old in state_dict:
+                state_dict[prefix + new] = state_dict.pop(prefix + old)
+
+
+class _WavLMAttentionParams(nn.Module):
+    def __init__(self, first):
+        super().__init__()
+        if first:
+            self.rel_attn_embed = nn.Embedding(320, 12)
+        self.attention = nn.MultiheadAttention(768, 12, batch_first=True)
+        self.gru_rel_pos_linear = nn.Linear(64, 8)
+        self.gru_rel_pos_const = nn.Parameter(torch.ones(1, 12, 1, 1))
+
+
+class _FeedForwardParams(nn.Module):
+    def __init__(self):
+        super().__init__()
+        self.intermediate_dense = nn.Linear(768, 3072)
+        self.output_dense = nn.Linear(3072, 768)
+
+
+class _EncoderLayerParams(nn.Module):
+    def __init__(self, first):
+        super().__init__()
+        self.attention = _WavLMAttentionParams(first)
+        self.layer_norm = nn.LayerNorm(768)
+        self.feed_forward = _FeedForwardParams()
+        self.final_layer_norm = nn.LayerNorm(768)
+
+
+class _WavLMParams(nn.Module):
+    """Parameter container with the key names of torchaudio's wavlm_model(**WAVLM_BASE._params)."""
+
+    def __init__(self):
+        super().__init__()
+        self.feature_extractor = _FeatureExtractorParams()
+        self.encoder = nn.Module()
+        self.encoder.feature_projection = nn.Module()
+        self.encoder.feature_projection.layer_norm = nn.LayerNorm(512)
+        self.encoder.feature_projection.projection = nn.Linear(512, 768)
+        self.encoder.transformer = nn.Module()
+        self.encoder.transformer.pos_conv_embed = nn.Module()
+        self.encoder.transformer.pos_conv_embed.conv = _PosConvParams()
+        self.encoder.transformer.layer_norm = nn.LayerNorm(768)
+        self.encoder.transformer.layers = nn.ModuleList([_EncoderLayerParams(i == 0) for i in range(12)])
+
+
+class SSeRiouSS(Model):
+    """WavLM Base > LSTM > Feed forward > Classifier (models/segmentation/SSeRiouSS.py) with ``wav2vec`` one of
+    "WAVLM_BASE" / "WAVLM_BASE_PLUS", the PyanNet LSTM / linear shape (1-4 BiLSTM layers of 128, 2 linear layers of
+    128) and any head PyanNet accepts.  ``wav2vec_layer`` < 0 averages the 12 layer outputs with
+    softmax(``wav2vec_weights``); 1 .. 12 takes that layer's output.  ``wav2vec_frozen`` and dropout only concern
+    training and change nothing here."""
+
+    _SLOT = "ssl"
+    _HPARAMS = ("wav2vec", "wav2vec_frozen", "wav2vec_layer", "lstm", "linear", "sample_rate", "num_channels")
+    KERNEL = [k for (_, k, _) in WAVLM_BASE_PARAMS["extractor_conv_layer_config"]]
+    STRIDE = [s for (_, _, s) in WAVLM_BASE_PARAMS["extractor_conv_layer_config"]]
+    min_num_samples = ops.SSL_MIN_SAMPLES
+
+    def __init__(self, wav2vec=None, wav2vec_frozen: bool = False, wav2vec_layer: int = -1,
+                 lstm: Optional[dict] = None, linear: Optional[dict] = None, sample_rate: int = 16000,
+                 num_channels: int = 1, duration: float = 10.0):
+        super().__init__(sample_rate=sample_rate, num_channels=num_channels)
+        wav2vec = "WAVLM_BASE" if wav2vec is None else wav2vec
+        if not isinstance(wav2vec, str) or wav2vec not in SSL_BUNDLES:
+            raise NotImplementedError(f"SSeRiouSS has CUDA kernels for the WavLM Base front end only "
+                                      f"(wav2vec = {' / '.join(SSL_BUNDLES)}), not for {wav2vec!r}")
+        if sample_rate != 16000:
+            raise ValueError(f"Expected 16000Hz, found {sample_rate}Hz.")
+        wav2vec_layer = int(wav2vec_layer)
+        if not (wav2vec_layer < 0 or 1 <= wav2vec_layer <= 12):
+            raise ValueError(f"`wav2vec_layer` must be negative or between 1 and 12, got {wav2vec_layer}")
+        lstm_hp = {"hidden_size": 128, "num_layers": 4, "bidirectional": True, "monolithic": True, "dropout": 0.0}
+        lstm_hp.update(lstm or {})
+        linear_hp = {"hidden_size": 128, "num_layers": 2}
+        linear_hp.update(linear or {})
+        if (lstm_hp["hidden_size"], lstm_hp["bidirectional"], lstm_hp["monolithic"]) != (128, True, True) or \
+                not (1 <= lstm_hp["num_layers"] <= 4) or (linear_hp["hidden_size"], linear_hp["num_layers"]) != (128, 2):
+            raise NotImplementedError("the CUDA kernels implement the PyanNet head shape only: 1-4 monolithic "
+                                      "bidirectional LSTM layers of 128, 2 linear layers of 128")
+        self.hparams.wav2vec, self.hparams.wav2vec_frozen = wav2vec, bool(wav2vec_frozen)
+        self.hparams.wav2vec_layer, self.hparams.lstm, self.hparams.linear = wav2vec_layer, lstm_hp, linear_hp
+        self.wav2vec = _WavLMParams()
+        if wav2vec_layer < 0:
+            self.wav2vec_weights = nn.Parameter(torch.ones(12))
+        self.lstm = nn.LSTM(768, hidden_size=128, num_layers=lstm_hp["num_layers"], bidirectional=True,
+                            batch_first=True)
+        self.linear = nn.ModuleList([nn.Linear(256, 128), nn.Linear(128, 128)])
+        self.specifications = Specifications(problem=Problem.MONO_LABEL_CLASSIFICATION, resolution=Resolution.FRAME,
+                                             duration=duration, warm_up=(0.0, 0.0),
+                                             classes=["speaker#1", "speaker#2", "speaker#3"], powerset_max_classes=2,
+                                             permutation_invariant=True)
+
+    specifications = PyanNet.specifications
+    dimension = PyanNet.dimension
+
+    def num_frames(self, num_samples: int) -> int:
+        return ops.ssl_num_frames(num_samples)
+
+    def receptive_field_size(self, num_frames: int = 1) -> int:
+        rf = num_frames
+        for k, s in reversed(list(zip(self.KERNEL, self.STRIDE))):
+            rf = 1 + (k - 1) + (rf - 1) * s
+        return rf
+
+    def receptive_field_center(self, frame: int = 0) -> int:
+        c = frame
+        for k, s in reversed(list(zip(self.KERNEL, self.STRIDE))):
+            c = c * s + (k - 1) // 2
+        return c
+
+    def check_window(self, num_samples: int):
+        """Refuses windows shorter than one WavLM frame (400 samples)."""
+        ops.check_ssl_window(num_samples)
+
+    def _upload(self, ctx):
+        ctx.load_sseriouss(self.state_dict(), self.specifications, self.hparams.wav2vec_layer)
+
+    def forward_chunks(self, wav: torch.Tensor, chunk_off, chunk_valid, return_logp: bool = False, out=None,
+                       window: int = ops.CHUNK, reduce_max: bool = False):
+        """As PyanNet.forward_chunks, with ops.ssl_num_frames(window) frames per window (ops.Context.ssl_forward)."""
+        ops.check_ssl_window(window)
+        return self._ctx().ssl_forward(wav, chunk_off, chunk_valid, return_logp=return_logp, out=out, window=window,
+                                       reduce_max=reduce_max)
+
+    def forward(self, waveforms: torch.Tensor) -> torch.Tensor:
+        """waveforms (batch, channel, samples), samples >= 400 -> (batch, num_frames(samples), dimension):
+        log-probabilities of a log-softmax head, sigmoid scores of a sigmoid head."""
+        b, c, s = waveforms.shape
+        if c != 1:
+            raise ValueError(f"SSeRiouSS kernels expect mono waveforms, got {c} channels")
+        ops.check_ssl_window(s)
+        ctx = self._ctx()
+        flat = waveforms.to(device=ctx.device, dtype=torch.float32).reshape(-1).contiguous()
+        off = np.arange(b, dtype=np.int64) * s
+        valid = np.full(b, s, dtype=np.int32)
+        if ops.seg_activation(self.specifications) == ops.SEG_SIGMOID:
+            return ctx.ssl_forward(flat, off, valid, window=s)
+        _, logp = ctx.ssl_forward(flat, off, valid, return_logp=True, window=s)
+        return logp

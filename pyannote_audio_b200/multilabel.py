@@ -10,7 +10,7 @@ import torch
 from .audio import AudioFile
 from .core import Annotation, SlidingWindowFeature
 from .inference import Inference
-from .models import PyanNet
+from .models import PyanNet, SSeRiouSS
 from .signal import Binarize
 
 
@@ -20,7 +20,7 @@ class MultiLabelSegmentation:
     the two durations are the pipeline's ``min_duration_on`` / ``min_duration_off`` instead.  Until instantiated,
     onset = offset = 0.5 and the durations are 0."""
 
-    def __init__(self, segmentation: Union[PyanNet, Mapping, str, None] = None, fscore: bool = False,
+    def __init__(self, segmentation: Union[PyanNet, SSeRiouSS, Mapping, str, None] = None, fscore: bool = False,
                  share_min_duration: bool = False, token=None, cache_dir=None, device: Optional[torch.device] = None,
                  **inference_kwargs):
         from .loading import get_model, is_checkpoint_spec
@@ -30,7 +30,7 @@ class MultiLabelSegmentation:
         self.segmentation, self.fscore, self.share_min_duration = segmentation, fscore, share_min_duration
         model = get_model(segmentation, token=token, cache_dir=cache_dir) if is_checkpoint_spec(segmentation) \
             else segmentation
-        if not isinstance(model, PyanNet):
+        if not isinstance(model, (PyanNet, SSeRiouSS)):
             raise ValueError("`segmentation` must be a PyanNet instance or a local checkpoint (no hub access here)")
         device = device or torch.device("cuda", torch.cuda.current_device() if torch.cuda.is_available() else 0)
         model.to(device)

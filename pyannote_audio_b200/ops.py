@@ -37,6 +37,44 @@ def check_seg_window(num_samples: int):
                          f"{int(num_samples)}")
 
 
+SSL_MIN_SAMPLES = 400      # shortest SSeRiouSS window: one WavLM frame (receptive field 400 samples, step 320)
+SSL_LAYERS = 12
+SSL_REL_SPAN = 1023        # relative offsets beyond +-1023 frames share the (saturated) bucket of +-1023
+
+
+def ssl_num_frames(num_samples: int) -> int:
+    """WavLM Base feature-extractor frames of a window: conv (10, 5), 4 x conv (3, 2), 2 x conv (2, 2).  499 for
+    160000 samples, 1 for 400."""
+    n = 1 + (int(num_samples) - 10) // 5
+    for k in (3, 3, 3, 3, 2, 2):
+        n = 1 + (n - k) // 2
+    return n
+
+
+def check_ssl_window(num_samples: int):
+    if int(num_samples) < SSL_MIN_SAMPLES:
+        raise ValueError(f"SSeRiouSS needs windows of at least {SSL_MIN_SAMPLES} samples (one WavLM frame), got "
+                         f"{int(num_samples)}")
+
+
+def wavlm_relative_buckets(num_buckets: int = 320, max_distance: int = 800) -> torch.Tensor:
+    """int32 bucket of every relative offset d = key - query in [-1023, 1023] (index d + 1023), with the torch ops
+    of WavLM's bidirectional bucketing (torchaudio wavlm_attention.py), so that the float ``log`` rounds alike."""
+    d = torch.arange(-SSL_REL_SPAN, SSL_REL_SPAN + 1, dtype=torch.long)
+    half = num_buckets // 2
+    buckets = (d > 0).to(torch.long) * half
+    a = torch.abs(d)
+    max_exact = half // 2
+    large = max_exact + (torch.log(a.float() / max_exact) / np.log(max_distance / max_exact)
+                         * (half - max_exact)).to(torch.long)
+    large = torch.min(large, torch.full_like(large, half - 1))
+    buckets = buckets + torch.where(a < max_exact, a, large)
+    # the kernels clamp longer offsets to +-1023: the buckets must already be saturated there
+    if int(buckets[0]) != half - 1 or int(buckets[-1]) != num_buckets - 1:
+        raise AssertionError("relative position buckets are not saturated at +-1023 frames")
+    return buckets.to(torch.int32).contiguous()
+
+
 def check_seg_classes(num_classes: int):
     if not 1 <= int(num_classes) <= SEG_MAX_CLASSES:
         raise NotImplementedError(f"a PyanNet classifier of {int(num_classes)} classes has no CUDA kernel: the "
@@ -143,6 +181,18 @@ def _fill_sincnet(w, sd: Mapping[str, torch.Tensor], f):
         w.conv_bias[i] = f(f"sincnet.conv1d.{i + 1}.bias")
 
 
+def fold_weight_norm(sd: Mapping[str, torch.Tensor], prefix: str) -> torch.Tensor:
+    """The plain fp32 weight of a conv under weight norm over dim 2 (torch.nn.utils.parametrizations.weight_norm, or
+    the older torch.nn.utils.weight_norm): ``prefix + parametrizations.weight.original0 / original1`` or
+    ``prefix + weight_g / weight_v``, folded with torch's own kernel."""
+    if prefix + "parametrizations.weight.original0" in sd:
+        g, v = sd[prefix + "parametrizations.weight.original0"], sd[prefix + "parametrizations.weight.original1"]
+    else:
+        g, v = sd[prefix + "weight_g"], sd[prefix + "weight_v"]
+    g, v = g.detach().float().cpu(), v.detach().float().cpu()
+    return torch._weight_norm(v, g, 2).contiguous()
+
+
 def _norm_mode(normalize) -> int:
     """False/0: rows as given; True/1: fp64 L2 normalisation; "float32"/2: numpy's float32 normalisation of rows that
     hold float32 values (what the reference does to float32 embeddings before scipy's linkage)."""
@@ -173,7 +223,10 @@ class Context:
         self.emb_channels = 256   # trunk output channels of the loaded embedding model: 256 (ResNet34) or 1024
         self.xvec_loaded = False
         self.xvec_dimension = 512
-        self.owners = {}          # slot ("seg" | "emb" | "xvec") -> stamp of the model whose weights are resident
+        self.ssl_loaded = False
+        self.ssl_classes = CLASSES           # classifier head of the loaded SSeRiouSS
+        self.ssl_activation = SEG_LOGSOFTMAX
+        self.owners = {}    # slot ("seg" | "emb" | "xvec" | "ssl") -> stamp of the model whose weights are resident
         # A/B knob for scripts (like B200_CONV_IMPL / B200_EMB_MAX_BATCH / B200_SEG_MAX_BATCH, which the library
         # reads itself): B200_OPTIONS="key=value,..."
         # is applied through b200_ctx_set_option, so unknown keys / bad values fail loudly
@@ -300,6 +353,82 @@ class Context:
         _lib.check(self.lib.b200_xvec_load(self._h, C.byref(w)))
         self.xvec_loaded, self.xvec_dimension = True, int(dim)
 
+    def load_sseriouss(self, sd: Mapping[str, torch.Tensor], specifications=None, wav2vec_layer: int = -1):
+        """SSeRiouSS weights (models/segmentation/SSeRiouSS.py on WavLM Base) into the ctx's own slot.  ``sd`` uses
+        the module's keys; the positional conv's weight norm is folded here (either spelling).  The LSTM reads the
+        softmax(wav2vec_weights)-weighted average of the 12 layer outputs for ``wav2vec_layer`` < 0, else the output
+        of layer ``wav2vec_layer`` (1 .. 12), and then only that many layers run."""
+        num_classes = int(sd["classifier.weight"].shape[0])
+        check_seg_classes(num_classes)
+        activation = SEG_LOGSOFTMAX if specifications is None else seg_activation(specifications)
+        f = _state_dict_reader(sd)
+        w = _lib.SslWeights()
+        fe, enc = "wav2vec.feature_extractor.conv_layers.", "wav2vec.encoder."
+        w.conv0_weight = f(fe + "0.conv.weight")
+        w.conv0_norm_weight = f(fe + "0.layer_norm.weight")
+        w.conv0_norm_bias = f(fe + "0.layer_norm.bias")
+        for i in range(6):
+            w.conv_weight[i] = f(f"{fe}{i + 1}.conv.weight")
+        w.proj_norm_weight = f(enc + "feature_projection.layer_norm.weight")
+        w.proj_norm_bias = f(enc + "feature_projection.layer_norm.bias")
+        w.proj_weight = f(enc + "feature_projection.projection.weight")
+        w.proj_bias = f(enc + "feature_projection.projection.bias")
+        tr = enc + "transformer."
+        pos = fold_weight_norm(sd, tr + "pos_conv_embed.conv.")
+        f.keep.append(pos)
+        w.pos_conv_weight = _fp(pos)
+        w.pos_conv_bias = f(tr + "pos_conv_embed.conv.bias")
+        w.encoder_norm_weight = f(tr + "layer_norm.weight")
+        w.encoder_norm_bias = f(tr + "layer_norm.bias")
+        w.rel_attn_embed = f(tr + "layers.0.attention.rel_attn_embed.weight")
+        buckets = wavlm_relative_buckets()
+        f.keep.append(buckets)
+        w.rel_bucket = C.cast(C.c_void_p(buckets.data_ptr()), C.POINTER(C.c_int32))
+        if wav2vec_layer < 0:
+            num_layers = SSL_LAYERS
+            lw = torch.softmax(sd["wav2vec_weights"].detach().float().cpu(), dim=0).contiguous()
+            f.keep.append(lw)
+            w.layer_weights = _fp(lw)
+        else:
+            num_layers = int(wav2vec_layer)
+            if not 1 <= num_layers <= SSL_LAYERS:
+                raise ValueError(f"wav2vec_layer must be negative or between 1 and {SSL_LAYERS}, got {num_layers}")
+        w.num_layers = num_layers
+        names = {"in_proj_weight": "attention.attention.in_proj_weight",
+                 "in_proj_bias": "attention.attention.in_proj_bias",
+                 "out_proj_weight": "attention.attention.out_proj.weight",
+                 "out_proj_bias": "attention.attention.out_proj.bias",
+                 "gru_weight": "attention.gru_rel_pos_linear.weight", "gru_bias": "attention.gru_rel_pos_linear.bias",
+                 "gru_const": "attention.gru_rel_pos_const",
+                 "layer_norm_weight": "layer_norm.weight", "layer_norm_bias": "layer_norm.bias",
+                 "ff1_weight": "feed_forward.intermediate_dense.weight",
+                 "ff1_bias": "feed_forward.intermediate_dense.bias",
+                 "ff2_weight": "feed_forward.output_dense.weight", "ff2_bias": "feed_forward.output_dense.bias",
+                 "final_layer_norm_weight": "final_layer_norm.weight",
+                 "final_layer_norm_bias": "final_layer_norm.bias"}
+        for layer in range(num_layers):
+            for field, key in names.items():
+                setattr(w.layer[layer], field, f(f"{tr}layers.{layer}.{key}"))
+        layers = 0
+        while f"lstm.weight_ih_l{layers}" in sd:
+            layers += 1
+        w.lstm_layers = layers
+        for layer in range(layers):
+            for d, suffix in enumerate(("", "_reverse")):
+                w.lstm_w_ih[layer * 2 + d] = f(f"lstm.weight_ih_l{layer}{suffix}")
+                w.lstm_w_hh[layer * 2 + d] = f(f"lstm.weight_hh_l{layer}{suffix}")
+                w.lstm_b_ih[layer * 2 + d] = f(f"lstm.bias_ih_l{layer}{suffix}")
+                w.lstm_b_hh[layer * 2 + d] = f(f"lstm.bias_hh_l{layer}{suffix}")
+        for i in range(2):
+            w.linear_weight[i] = f(f"linear.{i}.weight")
+            w.linear_bias[i] = f(f"linear.{i}.bias")
+        w.classifier_weight = f("classifier.weight")
+        w.classifier_bias = f("classifier.bias")
+        self.owners.pop("ssl", None)
+        self.ssl_loaded = False
+        _lib.check(self.lib.b200_ssl_load(self._h, C.byref(w), num_classes, activation))
+        self.ssl_loaded, self.ssl_classes, self.ssl_activation = True, num_classes, activation
+
     def _load_bottleneck(self, sd, f, conv_bn):
         """WeSpeakerResNet152 / 221 / 293 (Bottleneck blocks, resnet.py:148-212): the block counts come from the keys."""
         counts = []
@@ -394,6 +523,31 @@ class Context:
         cls = self._out(out, (n, F), torch.uint8)
         logp = torch.empty((n, F, K), dtype=torch.float32, device=self.device) if return_logp else None
         self._call("b200_seg_forward_window", _ptr(wav), off.ctypes.data, valid.ctypes.data, n, window, _ptr(cls),
+                   _ptr(logp))
+        return (cls, logp) if return_logp else cls
+
+    def ssl_forward(self, wav, chunk_off, chunk_valid, return_logp=False, out: Optional[torch.Tensor] = None,
+                    window: int = CHUNK, reduce_max: bool = False):
+        """SSeRiouSS on windows of ``window`` samples (>= 400), arguments and outputs as in seg_forward with
+        F = ssl_num_frames(window) frames per window."""
+        check_ssl_window(window)
+        window = int(window)
+        off, valid = self._chunks(wav, chunk_off, chunk_valid)
+        n = len(off)
+        F = ssl_num_frames(window)
+        K = self.ssl_classes
+        if self.ssl_activation == SEG_SIGMOID:
+            if return_logp:
+                raise ValueError("the loaded SSeRiouSS head is a sigmoid head: it has scores, not log-probabilities")
+            scores = self._out(out, (n, F, 1 if reduce_max else K), torch.float32)
+            self._call("b200_ssl_forward_scores", _ptr(wav), off.ctypes.data, valid.ctypes.data, n, window,
+                       None if reduce_max else _ptr(scores), _ptr(scores) if reduce_max else None)
+            return scores
+        if reduce_max:
+            raise ValueError("reduce_max needs a sigmoid segmentation head (use powerset_speech for a powerset head)")
+        cls = self._out(out, (n, F), torch.uint8)
+        logp = torch.empty((n, F, K), dtype=torch.float32, device=self.device) if return_logp else None
+        self._call("b200_ssl_forward_window", _ptr(wav), off.ctypes.data, valid.ctypes.data, n, window, _ptr(cls),
                    _ptr(logp))
         return (cls, logp) if return_logp else cls
 

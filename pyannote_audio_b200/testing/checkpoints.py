@@ -9,7 +9,7 @@ def reference_style_checkpoint(kind):
     """``kind``: "seg" (PyanNet, community-1 head), "seg_multilabel" (PyanNet with a 4-label sigmoid head,
     permutation_invariant=False), "seg_binary" (a 1-class sigmoid ["speech"] head), "seg_powerset42" (a powerset
     head of 4 speakers with at most 2 per frame, 11 classes), "emb" (WeSpeakerResNet34), "emb293"
-    (WeSpeakerResNet293) or "xvec" (XVectorSincNet).  A Lightning-format pytorch_model.bin as the reference writes it (model.py:244-256): state_dict +
+    (WeSpeakerResNet293), "xvec" (XVectorSincNet) or "sseriouss" (SSeRiouSS on WavLM Base, 4-label sigmoid head).  A Lightning-format pytorch_model.bin as the reference writes it (model.py:244-256): state_dict +
     hyper_parameters + checkpoint["pyannote.audio"] whose `specifications` is pickled under the REFERENCE's module
     path pyannote.audio.core.task (registered here only while pickling, then removed again)."""
     import dataclasses
@@ -78,6 +78,21 @@ def reference_style_checkpoint(kind):
                                      "architecture": {"module": "pyannote.audio.models.embedding.wespeaker",
                                                       "class": "WeSpeakerResNet293"},
                                      "specifications": Specifications(Problem.REPRESENTATION, Resolution.CHUNK, 10.0)}}
+        elif kind == "sseriouss":
+            # a WavLM Base SSeRiouSS with a 4-label sigmoid head, layer average, the pre-parametrization weight-norm
+            # spelling of the positional conv (weight_g / weight_v)
+            ck = {"state_dict": syn.make_sseriouss_state_dict(5, num_classes=4, pos_weight_norm="weight_g"),
+                  "hyper_parameters": {"wav2vec": "WAVLM_BASE", "wav2vec_frozen": False, "wav2vec_layer": -1,
+                                       "lstm": {"hidden_size": 128, "num_layers": 4, "bidirectional": True,
+                                                "monolithic": True, "dropout": 0.0, "batch_first": True},
+                                       "linear": {"hidden_size": 128, "num_layers": 2},
+                                       "sample_rate": 16000, "num_channels": 1},
+                  "pyannote.audio": {"versions": {"pyannote.audio": "4.0.0"},
+                                     "architecture": {"module": "pyannote.audio.models.segmentation.SSeRiouSS",
+                                                      "class": "SSeRiouSS"},
+                                     "specifications": Specifications(
+                                         Problem.MULTI_LABEL_CLASSIFICATION, Resolution.FRAME, 5.0,
+                                         classes=["speech", "music", "noise", "laughter"])}}
         elif kind == "xvec":
             ck = {"state_dict": syn.make_xvector_state_dict(3),
                   "hyper_parameters": {"sincnet": {"stride": 10, "sample_rate": 16000}, "dimension": 512,

@@ -200,6 +200,72 @@ def make_xvector_state_dict(seed: int = 3, dimension: int = 512) -> "OrderedDict
 # ----------------------------------------------------------------------------------------
 
 
+def make_sseriouss_state_dict(seed: int = 5, wav2vec_layer: int = -1, lstm_layers: int = 4, num_classes: int = 7,
+                              pos_weight_norm: str = "parametrizations",
+                              logit_scale: float = 4.0) -> "OrderedDict[str, torch.Tensor]":
+    """SSeRiouSS on WavLM Base (models/segmentation/SSeRiouSS.py, torchaudio wavlm_model(**WAVLM_BASE._params)):
+    seeded weights under the module's keys.  Gains keep every activation O(1) through the conv stack and the 12
+    post-LN layers (no fp16 under- or overflow), and the relative position bias and layer weights are far from uniform
+    so that each part of the network shows in the output.  ``wav2vec_layer`` >= 1 drops ``wav2vec_weights`` (the
+    reference builds it only for the layer average); ``pos_weight_norm`` = "parametrizations" (current torch) or
+    "weight_g" (torch.nn.utils.weight_norm spelling of older checkpoints)."""
+    g = torch.Generator().manual_seed(seed)
+
+    def normal(shape, std):
+        return torch.randn(shape, generator=g, dtype=torch.float32) * std
+
+    def affine(prefix, c):
+        sd[prefix + ".weight"] = 1.0 + 0.1 * torch.randn(c, generator=g)
+        sd[prefix + ".bias"] = 0.05 * torch.randn(c, generator=g)
+
+    def linear(prefix, cout, cin, gain=1.0):
+        sd[prefix + ".weight"] = normal((cout, cin), gain / math.sqrt(cin))
+        sd[prefix + ".bias"] = normal((cout,), 0.02)
+
+    sd = OrderedDict()
+    fe, tr = "wav2vec.feature_extractor.conv_layers.", "wav2vec.encoder.transformer."
+    sd[fe + "0.conv.weight"] = normal((512, 1, 10), 1.0 / math.sqrt(10))
+    affine(fe + "0.layer_norm", 512)
+    for i, k in enumerate((3, 3, 3, 3, 2, 2), start=1):
+        sd[f"{fe}{i}.conv.weight"] = normal((512, 512, k), 1.8 / math.sqrt(512 * k))
+    affine("wav2vec.encoder.feature_projection.layer_norm", 512)
+    linear("wav2vec.encoder.feature_projection.projection", 768, 512)
+    pc = tr + "pos_conv_embed.conv."
+    g_, v_ = 2.0 + 0.2 * torch.randn((1, 1, 128), generator=g), normal((768, 48, 128), 1.0)
+    if pos_weight_norm == "parametrizations":
+        sd[pc + "parametrizations.weight.original0"], sd[pc + "parametrizations.weight.original1"] = g_, v_
+    else:
+        sd[pc + "weight_g"], sd[pc + "weight_v"] = g_, v_
+    sd[pc + "bias"] = normal((768,), 0.05)
+    affine(tr + "layer_norm", 768)
+    for layer in range(12):
+        p = f"{tr}layers.{layer}."
+        if layer == 0:
+            sd[p + "attention.rel_attn_embed.weight"] = normal((320, 12), 1.5)
+        sd[p + "attention.attention.in_proj_weight"] = normal((2304, 768), 1.5 / math.sqrt(768))
+        sd[p + "attention.attention.in_proj_bias"] = normal((2304,), 0.02)
+        linear(p + "attention.attention.out_proj", 768, 768)
+        linear(p + "attention.gru_rel_pos_linear", 8, 64, gain=0.5)
+        sd[p + "attention.gru_rel_pos_const"] = 1.0 + 0.2 * torch.randn((1, 12, 1, 1), generator=g)
+        affine(p + "layer_norm", 768)
+        linear(p + "feed_forward.intermediate_dense", 3072, 768)
+        linear(p + "feed_forward.output_dense", 768, 3072)
+        affine(p + "final_layer_norm", 768)
+    if wav2vec_layer < 0:
+        sd["wav2vec_weights"] = normal((12,), 1.0)
+    for layer in range(lstm_layers):
+        cin = 768 if layer == 0 else 256
+        for suffix in ("", "_reverse"):
+            sd[f"lstm.weight_ih_l{layer}{suffix}"] = normal((512, cin), 2.0 / math.sqrt(cin))
+            sd[f"lstm.weight_hh_l{layer}{suffix}"] = normal((512, 128), 1.0 / math.sqrt(128))
+            sd[f"lstm.bias_ih_l{layer}{suffix}"] = normal((512,), 0.1)
+            sd[f"lstm.bias_hh_l{layer}{suffix}"] = normal((512,), 0.1)
+    linear("linear.0", 128, 256, gain=2.0)
+    linear("linear.1", 128, 128, gain=2.0)
+    linear("classifier", num_classes, 128, gain=logit_scale)
+    return sd
+
+
 def make_plda(seed: int = 2, dim: int = 256, lda_dim: int = 128):
     rng = np.random.default_rng(seed)
     q, _ = np.linalg.qr(rng.standard_normal((dim, dim)))

@@ -12,12 +12,12 @@ import torch
 from .audio import AudioFile
 from .core import Annotation, Segment, SlidingWindow, SlidingWindowFeature
 from .inference import Inference, chunk_layout
-from .models import PyanNet
+from .models import PyanNet, SSeRiouSS
 from .signal import Binarize
 
 
 class VoiceActivityDetection:
-    def __init__(self, segmentation: Union[PyanNet, Mapping, str, None] = None, fscore: bool = False, token=None,
+    def __init__(self, segmentation: Union[PyanNet, SSeRiouSS, Mapping, str, None] = None, fscore: bool = False, token=None,
                  cache_dir=None, device: Optional[torch.device] = None, **inference_kwargs):
         from .loading import get_model, is_checkpoint_spec
 
@@ -28,7 +28,7 @@ class VoiceActivityDetection:
             model = PyanNet()
             model.load_state_dict(segmentation)
             segmentation = model
-        if not isinstance(segmentation, PyanNet):
+        if not isinstance(segmentation, (PyanNet, SSeRiouSS)):
             raise ValueError("`segmentation` must be a PyanNet instance or its state dict (no hub access here)")
         self.segmentation, self.fscore = segmentation, fscore
         device = device or torch.device("cuda", torch.cuda.current_device() if torch.cuda.is_available() else 0)
