@@ -1037,12 +1037,19 @@ static size_t carve_emb(const EmbWeights& E, int NB, int T0, int S, void* base, 
   return ws.bytes();
 }
 
-// one BasicBlock on nb segments: A -> (Bf, Cf) -> A, in place on the residual
-static int block_run(b200_ctx* ctx, const BlockWeights& B, __half* A, __half* Bf, __half* Cf, int nb, int H, int Wd,
+// one BasicBlock on nb segments: A -> (Bf, Cf) -> A, in place on the residual; a block with a fused kernel runs as
+// one launch A -> Bf, and A and Bf swap
+static int block_run(b200_ctx* ctx, const BlockWeights& B, __half*& A, __half*& Bf, __half* Cf, int nb, int H, int Wd,
                      cudaStream_t st) {
   const int s = B.conv1.stride;
   const int Ho = (H + 2 - 3) / s + 1, Wo = (Wd + 2 - 3) / s + 1;
   int rc;
+  if (block_fused(B, ctx->conv_impl)) {
+    if ((rc = block_forward(B, A, Bf, nb, H, Wd, ctx->num_sms, st))) return rc;
+    std::swap(A, Bf);
+    ctx->launches += 1;
+    return B200_OK;
+  }
   if ((rc = conv_forward(B.conv1, A, nullptr, Bf, nb, H, Wd, 1, ctx->conv_impl, ctx->num_sms, st))) return rc;
   const __half* res = A;
   if (B.has_shortcut) {

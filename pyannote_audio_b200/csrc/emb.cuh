@@ -56,9 +56,16 @@ struct EmbWeights {
 };
 
 // impl: 0 = SIMT reference conv, 1 = wgmma tensor-core convs (conv_row_kernel where it applies), 2 = conv_tc_kernel for
-// every conv (the bit-exact reference of conv_row_kernel)
+// every conv (the bit-exact reference of conv_row_kernel and block_row_kernel)
 int conv_forward(const ConvLayer& L, const __half* in, const __half* residual, __half* out, int B, int H_in, int W_in,
                  int relu, int impl, int num_sms, cudaStream_t stream);
+// Whether a BasicBlock runs as one block_row_kernel under conv_impl `impl`: impl = 1, stride 1, no shortcut, 32
+// channels (ResNet34 layer 1).
+bool block_fused(const BlockWeights& B, int impl);
+// relu(conv2(relu(conv1(in))) + in) of such a block (BN folded as in ConvLayer), NHWC fp16 [B][H][W][32]; out must not
+// alias in.  Bit-identical to conv_forward(conv1) followed by conv_forward(conv2) with `in` as the residual.
+int block_forward(const BlockWeights& B, const __half* in, __half* out, int Bn, int H, int W, int num_sms,
+                  cudaStream_t stream);
 // T0 fbank frames per segment (998 for 10 s); frame0 (device, [B], may be NULL = b * T0): first fbank row of each
 // segment, see fbank_forward.  out: NHWC fp16 [B][80][T0][32]
 int conv1_forward(const float* fbank, const float* fmean, const int* frame0, const float* w, const float* bias,

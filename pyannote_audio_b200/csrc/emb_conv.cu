@@ -12,8 +12,9 @@
 //   A stage of the mbarrier ring, filled by a TMA producer warp (warp 8), holds one 128-pixel box and one weight tap.
 //   Warpgroups 0 / 1 = output pixels [0, 64) / [64, 128) of the tile, fp32 accumulators in registers, epilogue
 //   (+bias (+residual) -> ReLU -> fp16 NHWC store) straight from the accumulator fragments.
-// conv_row_kernel: the stride-1 3x3 convs with one channel chunk and C_in = C_out (32 or 64: layers 1 and 2, 13 of the
-//   35), which are bound by HBM rather than by the tensor cores.  Persistent: about num_sms CTAs (two per SM for
+// conv_row_kernel: the stride-1 3x3 convs with one channel chunk and C_in = C_out (32 or 64: ResNet34's 7 stride-1
+//   layer-2 convs and the conv2 of the bottleneck trunks' layers 1 and 2), which are bound by HBM rather than by the
+//   tensor cores.  Persistent: about num_sms CTAs (two per SM for
 //   C_out = 32) walk units of one segment x one 128-pixel column tile x a band of consecutive output rows.
 //   - The nine weight taps are loaded once per CTA and stay in shared memory.
 //   - Input rows h0 - 1 .. h1 of a band are staged once each, as one box of 128 + 8 pixels, in a ring of row slots;
@@ -33,6 +34,10 @@
 //   consumers still walk (kh, kw, chunk, 16-channel step), so every chunk box of a kernel row stays resident until
 //   its tap kw = 2, and the results are bit-identical to conv_tc_kernel's.  Weight tiles stream through a ring of
 //   their own, and the producer stages the next tile while the consumers run the epilogue.
+// block_row_kernel: a whole stride-1 BasicBlock with 32 channels (the three blocks of ResNet34 layer 1) in one launch,
+//   built on conv_row_kernel's row walk: conv1's output rows go to a ring of intermediate row slots in shared memory
+//   and conv2 reads them from there, so a block reads its input and writes its output once instead of making five
+//   passes over 80 x T0 x 32 activations.  Bit-identical to the two convs run apart.
 #include "common.cuh"
 #include "emb.cuh"
 #include "tc_common.cuh"
@@ -148,6 +153,36 @@ conv_tc_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ 
   conv_epilogue<N, WIDE>(acc, p, (size_t)bh, wt * kTileM + wg * 64);
 }
 
+// acc[m] (the 64-pixel halves of a 128-pixel row) += the three kw taps of one kernel row over 32 input channels: the
+// row slot at `sa` is read from pixel row kw on, the taps' [N][32] weights lie at wts, wts + N * 64 and wts + N * 128.
+// Pixel row r of this warp's 16 (lanes 0-15 / 16-31: K columns 0-7 / 8-15 of each step) at 64-B rows, 16-B chunk c
+// stored at chunk c ^ ((row >> 1) & 3) (64-B swizzle; slots are 1024-B aligned).
+template <int N>
+__device__ __forceinline__ void row_taps_c32(float (&acc)[2][N / 2], uint32_t sa, uint32_t wts) {
+  constexpr uint32_t row_bytes = 64;
+  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+#pragma unroll
+  for (int kw = 0; kw < 3; ++kw) {
+    uint32_t af[2][2][4];
+#pragma unroll
+    for (int m = 0; m < 2; ++m)
+#pragma unroll
+      for (int k = 0; k < 2; ++k) {
+        const uint32_t row = (uint32_t)(m * 64 + (warp & 3) * 16 + (lane & 15) + kw);
+        const uint32_t chunk = (uint32_t)(2 * k + (lane >> 4)) ^ ((row >> 1) & 3u);
+        ldsm_x4(af[m][k], sa + row * row_bytes + chunk * 16u);
+      }
+    wg_fence();
+    const uint64_t bd = wg_desc(wts + kw * N * row_bytes, row_bytes);
+#pragma unroll
+    for (int k = 0; k < 2; ++k)
+#pragma unroll
+      for (int m = 0; m < 2; ++m) WgmmaRS<N>::mma(acc[m], af[m][k], bd + 2 * k);
+    wg_commit();
+    wg_wait<0>();                                           // the fragments are rewritten by the next ldmatrix
+  }
+}
+
 template <int N, int CK>
 __global__ void __launch_bounds__(kWgThreads, N == 32 ? 2 : 1)
 conv_row_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB, ConvParams p) {
@@ -192,7 +227,6 @@ conv_row_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__
   }
 
   const int wg = __shfl_sync(0xffffffffu, warp >> 2, 0);  // warp-uniform to the compiler: no wgmma serialisation
-  const int lane = threadIdx.x & 31;
   mbar_wait(bar_w, 0);
   uint32_t s = 0;                                           // first input row of the current unit
   int item = 0;                                             // output rows walked so far; row `item` is warpgroup item & 1's
@@ -216,28 +250,7 @@ conv_row_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__
         mbar_wait(bar_full + 8 * slot, (q / nslots) & 1);
         const uint32_t sa = slot0 + slot * p.a_bytes;
         if constexpr (CK == 32) {
-          // pixel row r of this warp's 16 (lanes 0-15 / 16-31: K columns 0-7 / 8-15 of each step) at 64-B rows, 16-B
-          // chunk c stored at chunk c ^ ((row >> 1) & 3) (64-B swizzle; slots are 1024-B aligned)
-#pragma unroll
-          for (int kw = 0; kw < 3; ++kw) {
-            uint32_t af[2][CK / 16][4];
-#pragma unroll
-            for (int m = 0; m < 2; ++m)
-#pragma unroll
-              for (int k = 0; k < CK / 16; ++k) {
-                const uint32_t row = (uint32_t)(m * 64 + (warp & 3) * 16 + (lane & 15) + kw);
-                const uint32_t chunk = (uint32_t)(2 * k + (lane >> 4)) ^ ((row >> 1) & 3u);
-                ldsm_x4(af[m][k], sa + row * row_bytes + chunk * 16u);
-              }
-            wg_fence();
-            const uint64_t bd = wg_desc(wts + (3 * kh + kw) * b_tap_bytes, row_bytes);
-#pragma unroll
-            for (int k = 0; k < CK / 16; ++k)
-#pragma unroll
-              for (int m = 0; m < 2; ++m) WgmmaRS<N>::mma(acc[m], af[m][k], bd + 2 * k);
-            wg_commit();
-            wg_wait<0>();                                   // the fragments are rewritten by the next ldmatrix
-          }
+          row_taps_c32<N>(acc, sa, wts + 3 * kh * b_tap_bytes);
         } else {
           wg_fence();
 #pragma unroll
@@ -264,6 +277,201 @@ conv_row_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__
       for (int m = 0; m < 2; ++m) conv_epilogue<N>(acc[m], p, row, wt * kTileM + m * 64);
     }
     s += n + 2;
+  }
+}
+
+// Plan of block_row_kernel<32>: both convs' nine taps resident (2 x 18 KB), a ring of input row slots and a ring of
+// intermediate row slots (136 pixels of 64 B each, padded to 9 KB), two CTAs per SM (110 KB each).  Four of each:
+// conv2 row h holds intermediate rows h - 1 .. h + 1 and input row h (its residual) while conv1 writes intermediate
+// row h + 2 from input rows h + 1 .. h + 3, and the fourth input slot lets the producer stage row h + 4 meanwhile.
+struct BlockRowPlan {
+  static constexpr uint32_t kTapBytes = 32 * 64;
+  static constexpr uint32_t kSlotBytes = 9 * 1024;
+  static constexpr uint32_t kInTx = (kTileM + kRowHalo) * 64;
+  static constexpr uint32_t kInSlots = 4, kMidSlots = 4;
+  static constexpr size_t kSmem = 2048 + 2 * 9 * kTapBytes + (kInSlots + kMidSlots) * kSlotBytes;
+  static_assert(kInTx <= kSlotBytes && kSmem <= 113 * 1024, "block row plan");
+};
+constexpr int kStripW = kTileM - 2;                         // output columns per column strip of block_row_kernel
+
+struct BlockParams {
+  int H, W, tiles_w, band, bands, num_tiles;
+  const float* bias1;
+  const float* bias2;
+  __half* out;
+};
+
+__device__ __forceinline__ void st_shared_u32(uint32_t a, uint32_t v) {
+  asm volatile("st.shared.b32 [%0], %1;" ::"r"(a), "r"(v) : "memory");
+}
+__device__ __forceinline__ uint32_t ld_shared_u32(uint32_t a) {
+  uint32_t v;
+  asm volatile("ld.shared.b32 %0, [%1];" : "=r"(v) : "r"(a) : "memory");
+  return v;
+}
+__device__ __forceinline__ uint32_t h2_bits(__half2 h) { return *reinterpret_cast<uint32_t*>(&h); }
+
+// One stride-1 BasicBlock with 32 channels and an identity shortcut, out = relu(bn2(conv2(relu(bn1(conv1(x))))) + x),
+// without the intermediate activation leaving the SM.  Persistent CTAs walk units of one segment x one column strip of
+// kStripW output columns [w0, w0 + 126) x a band of output rows [h0, h0 + n), as conv_row_kernel does.
+//   - Warp 8 stages input rows h0 - 2 .. h0 + n + 1 once each, as 136-pixel boxes from column w0 - 2.
+//   - Warpgroup 0 runs conv1 on intermediate rows h0 - 1 .. h0 + n, 128 pixels each (columns [w0 - 1, w0 + 127)),
+//     and its epilogue writes relu(acc + bias) as fp16 into a ring of intermediate row slots, in the 64-B swizzled
+//     layout a staged input row has.  Positions outside the image are conv2's zero padding and are written as zero.
+//   - Warpgroup 1 runs conv2 on output row h from intermediate rows h - 1 .. h + 1, adds the residual from the staged
+//     input row h and stores the first 126 of its 128 pixels.
+// The two warpgroups do the same arithmetic per row, so each one's epilogue overlaps the other's MMAs.  Every output
+// sums its products in the (tap, 16-channel step) order of conv_tc_kernel, and the intermediate is rounded to fp16 as
+// the unfused path stores it, so the result is bit-identical to two conv_forward calls.
+// Barriers: input slot "full" (TMA bytes) and "empty" (three conv1 reads + one residual read; conv1 arrives for the
+// missing ones at the band's edges, so that no slot waits on a conv2 row that needs a later input row); intermediate slot "full" (128 writer threads) and "empty" (three conv2 reads).
+__global__ void __launch_bounds__(kWgThreads, 2)
+block_row_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmW1,
+                 const __grid_constant__ CUtensorMap tmW2, BlockParams p) {
+  using P = BlockRowPlan;
+  constexpr uint32_t NI = P::kInSlots, NM = P::kMidSlots;
+  extern __shared__ uint8_t smem_raw[];
+  const uint32_t base = (smem_u32(smem_raw) + 1023u) & ~1023u;
+  const uint32_t bar_w = base, in_full = base + 8, in_empty = in_full + 8 * NI;
+  const uint32_t mid_full = in_empty + 8 * NI, mid_empty = mid_full + 8 * NM;
+  const uint32_t w1 = base + 1024, w2 = w1 + 9 * P::kTapBytes;
+  const uint32_t in0 = w2 + 9 * P::kTapBytes, mid0 = in0 + NI * P::kSlotBytes;
+  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+
+  if (threadIdx.x == 0) {
+    mbar_init(bar_w, 1);
+    for (uint32_t s = 0; s < NI; ++s) { mbar_init(in_full + 8 * s, 1); mbar_init(in_empty + 8 * s, 4); }
+    for (uint32_t s = 0; s < NM; ++s) { mbar_init(mid_full + 8 * s, 128); mbar_init(mid_empty + 8 * s, 3); }
+    asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
+  }
+  __syncthreads();
+
+  if (warp == 8) {
+    if (lane == 0) {
+      prefetch_tensormap(&tmA);
+      prefetch_tensormap(&tmW1);
+      prefetch_tensormap(&tmW2);
+      mbar_expect_tx(bar_w, 18 * P::kTapBytes);
+      for (int kh = 0; kh < 3; ++kh) {
+        tma_load_3d(&tmW1, bar_w, w1 + 3 * kh * P::kTapBytes, 0, 0, 3 * kh);
+        tma_load_3d(&tmW2, bar_w, w2 + 3 * kh * P::kTapBytes, 0, 0, 3 * kh);
+      }
+      uint32_t s = 0;                                       // input rows staged so far
+      for (int u = blockIdx.x; u < p.num_tiles; u += gridDim.x) {
+        const int wt = u % p.tiles_w, t = u / p.tiles_w;
+        const int h0 = (t % p.bands) * p.band, b = t / p.bands;
+        const int n = min(p.band, p.H - h0);
+        for (int r = 0; r < n + 4; ++r, ++s) {
+          const uint32_t slot = s % NI;
+          mbar_wait(in_empty + 8 * slot, ((s / NI) & 1) ^ 1);
+          mbar_expect_tx(in_full + 8 * slot, P::kInTx);
+          tma_load_4d(&tmA, in_full + 8 * slot, in0 + slot * P::kSlotBytes, 0, wt * kStripW - 2, h0 - 2 + r, b);
+        }
+      }
+    }
+    return;
+  }
+
+  const int wg = __shfl_sync(0xffffffffu, warp >> 2, 0);  // warp-uniform to the compiler: no wgmma serialisation
+  const bool leader = (threadIdx.x & 127) == 0;
+  const int c0 = 2 * (lane & 3);
+  float2 bias[4];                                           // channels 8 j + c0, c0 + 1 of this thread's fragments
+#pragma unroll
+  for (int j = 0; j < 4; ++j) bias[j] = __ldg(reinterpret_cast<const float2*>((wg ? p.bias2 : p.bias1) + 8 * j + c0));
+  mbar_wait(bar_w, 0);
+  uint32_t s = 0, mq = 0;                                   // first input / intermediate row of the current unit
+  for (int u = blockIdx.x; u < p.num_tiles; u += gridDim.x) {
+    const int wt = u % p.tiles_w, t = u / p.tiles_w;
+    const int h0 = (t % p.bands) * p.band, b = t / p.bands;
+    const int n = min(p.band, p.H - h0);
+    const int w0 = wt * kStripW;
+    const int rows = wg == 0 ? n + 2 : n;
+    for (int j = 0; j < rows; ++j) {
+      float acc[2][16];
+#pragma unroll
+      for (int m = 0; m < 2; ++m)
+#pragma unroll
+        for (int i = 0; i < 16; ++i) {
+          acc[m][i] = 0.f;
+          asm volatile("" : "+f"(acc[m][i]));               // zeroed before the first wg_fence, not sunk past it
+        }
+      if (wg == 0) {
+        // conv1: intermediate row h0 - 1 + j from input rows j .. j + 2 of the unit
+#pragma unroll
+        for (int kh = 0; kh < 3; ++kh) {
+          const uint32_t q = s + j + kh, slot = q % NI;
+          mbar_wait(in_full + 8 * slot, (q / NI) & 1);
+          row_taps_c32<32>(acc, in0 + slot * P::kSlotBytes, w1 + 3 * kh * P::kTapBytes);
+        }
+        // input row k = j + kh: one arrival per conv1 row that reads it (the band's first / last row also for the
+        // missing ones), and rows 0, 1, n + 2 and n + 3, which no conv2 row takes as its residual, one more on their
+        // last read
+        if (leader)
+#pragma unroll
+          for (int kh = 0; kh < 3; ++kh) {
+            const int k = j + kh;
+            const bool no_res = (k < 2 || k >= n + 2) && j == min(k, n + 1);
+            mbar_arrive_n(in_empty + 8 * ((s + k) % NI),
+                          1 + (j == 0 ? 2 - kh : 0) + (j == n + 1 ? kh : 0) + (no_res ? 1 : 0));
+          }
+        const uint32_t q = mq + j, slot = q % NM, sm = mid0 + slot * P::kSlotBytes;
+        mbar_wait(mid_empty + 8 * slot, ((q / NM) & 1) ^ 1);
+        const int r = h0 - 1 + j;
+        const bool live = r >= 0 && r < p.H;
+#pragma unroll
+        for (int m = 0; m < 2; ++m)
+#pragma unroll
+          for (int i = 0; i < 2; ++i) {
+            const int px = m * 64 + (warp & 3) * 16 + (lane >> 2) + 8 * i, w = w0 - 1 + px;
+            const bool in = live && w >= 0 && w < p.W;
+#pragma unroll
+            for (int jj = 0; jj < 4; ++jj) {
+              const float a = fmaxf(acc[m][4 * jj + 2 * i] + bias[jj].x, 0.f);
+              const float d = fmaxf(acc[m][4 * jj + 2 * i + 1] + bias[jj].y, 0.f);
+              const uint32_t v = in ? h2_bits(__floats2half2_rn(a, d)) : 0u;
+              st_shared_u32(sm + px * 64u + ((jj ^ ((px >> 1) & 3)) << 4) + 2 * c0, v);
+            }
+          }
+        mbar_arrive(mid_full + 8 * slot);
+      } else {
+        // conv2: output row h0 + j from intermediate rows j .. j + 2 of the unit, residual = input row j + 2
+#pragma unroll
+        for (int kh = 0; kh < 3; ++kh) {
+          const uint32_t q = mq + j + kh, slot = q % NM;
+          mbar_wait(mid_full + 8 * slot, (q / NM) & 1);
+          row_taps_c32<32>(acc, mid0 + slot * P::kSlotBytes, w2 + 3 * kh * P::kTapBytes);
+        }
+        if (leader)
+#pragma unroll
+          for (int kh = 0; kh < 3; ++kh)
+            mbar_arrive_n(mid_empty + 8 * ((mq + j + kh) % NM), 1 + (j == 0 ? 2 - kh : 0) + (j == n - 1 ? kh : 0));
+        const uint32_t q = s + j + 2, slot = q % NI, sr = in0 + slot * P::kSlotBytes;
+        mbar_wait(in_full + 8 * slot, (q / NI) & 1);
+        const size_t row = (size_t)b * p.H + h0 + j;
+#pragma unroll
+        for (int m = 0; m < 2; ++m)
+#pragma unroll
+          for (int i = 0; i < 2; ++i) {
+            const int px = m * 64 + (warp & 3) * 16 + (lane >> 2) + 8 * i, w = w0 + px;
+            if (px >= kStripW || w >= p.W) continue;
+            const int rp = px + 2;                          // the slot's pixel row of input column w
+            __half2* o = reinterpret_cast<__half2*>(p.out + (row * p.W + w) * 32 + c0);
+#pragma unroll
+            for (int jj = 0; jj < 4; ++jj) {
+              const uint32_t rb = ld_shared_u32(sr + rp * 64u + ((jj ^ ((rp >> 1) & 3)) << 4) + 2 * c0);
+              const float2 rv = __half22float2(*reinterpret_cast<const __half2*>(&rb));
+              float a = acc[m][4 * jj + 2 * i] + bias[jj].x, d = acc[m][4 * jj + 2 * i + 1] + bias[jj].y;
+              a += rv.x;
+              d += rv.y;
+              o[4 * jj] = __floats2half2_rn(fmaxf(a, 0.f), fmaxf(d, 0.f));
+            }
+          }
+        asm volatile("bar.sync 1, 128;" ::: "memory");     // every warp has read its residual before the slot is freed
+        if (leader) mbar_arrive(in_empty + 8 * slot);
+      }
+    }
+    s += n + 4;
+    mq += n + 2;
   }
 }
 
@@ -662,6 +870,51 @@ int conv_forward(const ConvLayer& L, const __half* in, const __half* residual, _
     case 256: return launch(conv_tc_kernel<256, 64>);
     default: return launch(conv_tc_kernel<256, 64, true>);
   }
+}
+
+bool block_fused(const BlockWeights& Bw, int impl) {
+  return impl == 1 && !Bw.has_shortcut && Bw.conv1.stride == 1 && Bw.conv1.ksize == 3 && Bw.conv2.ksize == 3 &&
+         Bw.conv1.C_in == 32 && Bw.conv1.C_out == 32 && Bw.conv2.C_in == 32 && Bw.conv2.C_out == 32;
+}
+
+int block_forward(const BlockWeights& Bw, const __half* in, __half* out, int B, int H, int W, int num_sms,
+                  cudaStream_t stream) {
+  B200_CHECK(block_fused(Bw, 1), B200_ERR_STATE, "block %d -> %d (stride %d) has no fused kernel", Bw.conv1.C_in,
+             Bw.conv1.C_out, Bw.conv1.stride);
+  B200_CHECK(in != out, B200_ERR_INVALID, "fused block: output must not alias the input");
+  BlockParams p{};
+  p.H = H; p.W = W; p.bias1 = Bw.conv1.bias; p.bias2 = Bw.conv2.bias; p.out = out;
+  p.tiles_w = ceil_div(W, kStripW);
+  // bands as for conv_row_kernel: full height while the column strips fill every CTA, else shorter ones; each band
+  // re-stages four input rows and re-computes two intermediate rows
+  const int ctas = 2 * num_sms;
+  const int strips = B * p.tiles_w;
+  const int nbands = std::min(H, ceil_div(ctas, strips));
+  p.band = ceil_div(H, nbands);
+  p.bands = ceil_div(H, p.band);
+  p.num_tiles = strips * p.bands;
+  CUtensorMap tmA, tmW1, tmW2;
+  int rc;
+  {
+    const cuuint64_t dims[4] = {32, (cuuint64_t)W, (cuuint64_t)H, (cuuint64_t)B};
+    const cuuint64_t strides[3] = {64, (cuuint64_t)W * 64, (cuuint64_t)H * W * 64};
+    const cuuint32_t box[4] = {32, kTileM + kRowHalo, 1, 1};
+    if ((rc = encode_f16_map(&tmA, 4, in, dims, strides, box, nullptr, CU_TENSOR_MAP_SWIZZLE_64B, "block A"))) return rc;
+  }
+  {
+    const cuuint64_t dims[3] = {32, 32, 9};
+    const cuuint64_t strides[2] = {64, 32 * 64};
+    const cuuint32_t box[3] = {32, 32, 3};
+    if ((rc = encode_f16_map(&tmW1, 3, Bw.conv1.w, dims, strides, box, nullptr, CU_TENSOR_MAP_SWIZZLE_64B, "block W1")))
+      return rc;
+    if ((rc = encode_f16_map(&tmW2, 3, Bw.conv2.w, dims, strides, box, nullptr, CU_TENSOR_MAP_SWIZZLE_64B, "block W2")))
+      return rc;
+  }
+  const size_t smem = BlockRowPlan::kSmem;
+  B200_CUDA_OK(cudaFuncSetAttribute(block_row_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+  block_row_kernel<<<(unsigned)std::min(p.num_tiles, ctas), kWgThreads, smem, stream>>>(tmA, tmW1, tmW2, p);
+  B200_CUDA_OK(cudaGetLastError());
+  return B200_OK;
 }
 
 int conv1_forward(const float* fbank, const float* fmean, const int* frame0, const float* w, const float* bias,

@@ -21,7 +21,11 @@ Byte model, per segment (computed from the shapes, not measured):
           rows    : resident for layers 1 and 2; the stride-1 3x3 convs with C_in = C_out = 128 / 256 (layers 3 and 4)
                     stage each of the three input rows of an output tile once per channel chunk as a 136-pixel box,
                     and every weight tile; the other convs stay per-tap
-  HBM   = input + output (+ residual) activations once, and the weights once per launch shared by --batch segments
+          fused   : rows, except that each stride-1 BasicBlock of layer 1 is one launch (block_row_kernel): it stages
+                    each input row of a band once (plus four halo rows per band) as a 136-pixel box per 126-column
+                    strip, and both convs' weights once per CTA; the intermediate activation stays on chip
+  HBM   = input + output (+ residual) activations once, and the weights once per launch shared by --batch segments;
+          a fused block reads its input once and writes its output once
 """
 import argparse
 import os
@@ -30,6 +34,7 @@ import sys
 
 TILE_M = 128
 HALO = 8
+STRIP_W = TILE_M - 2         # output columns per strip of block_row_kernel
 
 
 BOTTLENECK_BLOCKS = {"resnet152": (3, 8, 36, 3), "resnet221": (6, 16, 48, 3), "resnet293": (10, 20, 64, 3)}
@@ -73,6 +78,40 @@ def resident_plan(cout, ho, tiles_w, batch, sms):
     return min(ctas, strips * -(-ho // band)), band, -(-ho // band)
 
 
+def launches(model, plan):
+    """The trunk's kernel launches in order: lists of the trunk_convs() entries each one computes (two for a fused
+    block, conv1 and conv2)."""
+    convs = trunk_convs(model)
+    out = []
+    for c in convs:
+        fuse = (plan == "fused" and model == "resnet34" and c[0] == 1 and c[1].endswith(".conv2") and out and
+                out[-1][0][1].endswith(".conv1") and out[-1][0][5] == 1)
+        if fuse:
+            out[-1].append(c)
+        else:
+            out.append([c])
+    return out
+
+
+def fused_model(c1, c2, batch, sms=132):
+    """(GFLOP, fill MB, unique HBM MB) per segment of a fused block (block_row_kernel: two CTAs per SM)."""
+    _, _, cin, cout, k, _, H, W, _ = c1
+    strips = -(-W // STRIP_W)
+    ctas = 2 * sms
+    band = -(-H // min(H, -(-ctas // (batch * strips))))
+    bands = -(-H // band)
+    ctas = min(ctas, batch * strips * bands)
+    fill = strips * (H + 4 * bands) * (TILE_M + HALO) * cin * 2 + ctas * 2 * k * k * cin * cout * 2 / batch
+    hbm = H * W * cin * 2 + H * W * cout * 2 + 2 * k * k * cin * cout * 2 / batch
+    return 2 * 2.0 * H * W * cout * cin * k * k / 1e9, fill / 1e6, hbm / 1e6
+
+
+def launch_model(convs, plan, batch, sms=132):
+    if len(convs) == 2:
+        return fused_model(*convs, batch, sms)
+    return conv_model(convs[0], plan, batch, sms)
+
+
 def conv_model(c, plan, batch, sms=132):
     """(GFLOP, fill MB, unique HBM MB) per segment of one conv."""
     _, _, cin, cout, k, s, H, W, res = c
@@ -84,8 +123,8 @@ def conv_model(c, plan, batch, sms=132):
     tiles = Ho * -(-Wo // TILE_M) * (cout // n_tile)
     b_tile = n_tile * ck * 2
     reuse = k == 3 and s == 1 and ((plan == "reuse" and cin == ck and cout <= 64) or
-                                   (plan == "rows" and cin == cout and cout in (128, 256)))
-    if plan in ("resident", "rows") and k == 3 and s == 1 and cin == ck and cout == cin:
+                                   (plan in ("rows", "fused") and cin == cout and cout in (128, 256)))
+    if plan in ("resident", "rows", "fused") and k == 3 and s == 1 and cin == ck and cout == cin:
         tiles_w = -(-Wo // TILE_M)
         ctas, _, bands = resident_plan(cout, Ho, tiles_w, batch, sms)
         fill = tiles_w * (Ho + 2 * bands) * (TILE_M + HALO) * ck * 2 + ctas * k * k * b_tile / batch
@@ -99,17 +138,19 @@ def conv_model(c, plan, batch, sms=132):
 
 
 def print_model(plan, batch, sms, model="resnet34"):
-    rows = [(c, *conv_model(c, plan, batch, sms)) for c in trunk_convs(model)]
+    rows = [(cs, *launch_model(cs, plan, batch, sms)) for cs in launches(model, plan)]
     print(f"byte model of {model} ({plan} plan), per segment:")
-    print(f"{'layer':>6} {'convs':>5} {'GFLOP':>7} {'fill MB':>8} {'HBM MB':>7} {'FLOP/fill B':>11} {'FLOP/HBM B':>10}")
-    tot = [0, 0.0, 0.0, 0.0]
+    print(f"{'layer':>6} {'convs':>5} {'launches':>8} {'GFLOP':>7} {'fill MB':>8} {'HBM MB':>7} {'FLOP/fill B':>11} "
+          f"{'FLOP/HBM B':>10}")
+    tot = [0, 0, 0.0, 0.0, 0.0]
     for li in (1, 2, 3, 4):
-        sel = [r for r in rows if r[0][0] == li]
+        sel = [r for r in rows if r[0][0][0] == li]
+        nc = sum(len(r[0]) for r in sel)
         g, f, h = (sum(r[i] for r in sel) for i in (1, 2, 3))
-        tot = [tot[0] + len(sel), tot[1] + g, tot[2] + f, tot[3] + h]
-        print(f"{li:>6} {len(sel):>5} {g:7.2f} {f:8.1f} {h:7.1f} {g * 1e3 / f:11.0f} {g * 1e3 / h:10.0f}")
-    print(f"{'total':>6} {tot[0]:>5} {tot[1]:7.2f} {tot[2]:8.1f} {tot[3]:7.1f} {tot[1] * 1e3 / tot[2]:11.0f} "
-          f"{tot[1] * 1e3 / tot[3]:10.0f}")
+        tot = [tot[0] + nc, tot[1] + len(sel), tot[2] + g, tot[3] + f, tot[4] + h]
+        print(f"{li:>6} {nc:>5} {len(sel):>8} {g:7.2f} {f:8.1f} {h:7.1f} {g * 1e3 / f:11.0f} {g * 1e3 / h:10.0f}")
+    print(f"{'total':>6} {tot[0]:>5} {tot[1]:>8} {tot[2]:7.2f} {tot[3]:8.1f} {tot[4]:7.1f} {tot[2] * 1e3 / tot[3]:11.0f} "
+          f"{tot[2] * 1e3 / tot[4]:10.0f}")
     return rows
 
 
@@ -126,8 +167,9 @@ def main():
     ap = argparse.ArgumentParser(description=__doc__, formatter_class=argparse.RawDescriptionHelpFormatter)
     ap.add_argument("--root", default=os.path.dirname(os.path.dirname(os.path.abspath(__file__))),
                     help="tree whose built library is timed (default: this one)")
-    ap.add_argument("--plan", choices=["rows", "resident", "reuse", "per-tap"], default="rows",
-                    help="launch plan of the timed library for the byte model (resident: a library whose layer 3 and "
+    ap.add_argument("--plan", choices=["fused", "rows", "resident", "reuse", "per-tap"], default="fused",
+                    help="launch plan of the timed library for the byte model (rows: a library whose layer 1 blocks "
+                         "run as two conv launches each; resident: one whose layer 3 and "
                          "4 convs stage one box per tap; reuse: one whose layer 1 and 2 convs stage one box per kh; "
                          "per-tap: one box per tap everywhere)")
     ap.add_argument("--sms", type=int, default=132, help="SMs of the GPU for the resident plan (H100 SXM: 132)")
@@ -175,12 +217,12 @@ def main():
             if cur is not None:
                 runs.append(cur)
             cur = None
-        elif cur is not None and "conv" in e.name:
+        elif cur is not None and ("conv" in e.name or "block_row_kernel" in e.name):
             cur.append(e.time_range.end - e.time_range.start)        # us
     n = len(rows)
     runs = [r for r in runs if len(r) == n]
     if not runs:
-        raise SystemExit(f"found no emb_trunk call with {n} conv launches between conv1_kernel and frames_to_nchw")
+        raise SystemExit(f"found no emb_trunk call with {n} trunk launches between conv1_kernel and frames_to_nchw")
     us = [sum(r[i] for r in runs) / len(runs) for i in range(n)]
 
     print(f"\nGPU: {info}   (name, power limit, SM clock now, max SM clock)")
@@ -188,8 +230,11 @@ def main():
     print(f"{'conv':<20} {'Cin>Cout':>9} {'k/s':>4} {'HxW in':>8} {'us':>8} {'TFLOP/s':>8} {'fill GB/s':>9} {'HBM GB/s':>9}")
     tot_us = 0.0
     per_layer = {}
-    for (c, gf, fmb, hmb), t in zip(rows, us):
+    for (cs, gf, fmb, hmb), t in zip(rows, us):
+        c = cs[0]
         _, name, cin, cout, k, s, H, W, _ = c
+        if len(cs) == 2:
+            name = name.rsplit(".", 1)[0] + " (fused)"
         sec = t * 1e-6
         tot_us += t
         L = per_layer.setdefault(c[0], [0.0, 0.0, 0.0, 0.0])
