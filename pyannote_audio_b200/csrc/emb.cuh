@@ -15,7 +15,8 @@ struct ConvParams {
   int H_out, W_out, C_out;
   int taps_h, taps_w, stride, pad;
   int Ck, tiles_w, num_tiles, relu;
-  int band, bands;         // conv_row_kernel: output rows per unit, units per column strip (num_tiles = units)
+  int band, bands;         // conv_row_kernel / conv_chunk_row_kernel: output rows per unit, units per column strip
+                           // (num_tiles = units)
   const float* bias;
   const __half* residual;
   __half* out;

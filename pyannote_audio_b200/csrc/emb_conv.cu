@@ -28,12 +28,14 @@
 //   Each output sums its products in the (tap, 16-channel step) order of conv_tc_kernel, and the epilogue is the same,
 //   so the two kernels give bit-identical results.
 // conv_chunk_row_kernel: the stride-1 3x3 convs with C_in = C_out = 128 or 256 (layers 3 and 4, 16 of the 35, and the
-//   conv2 of the bottleneck trunks' layers 3 and 4).  Persistent CTAs walk the output tiles of conv_tc_kernel with the
-//   same wgmma shapes.  For each kh the producer stages input row h - 1 + kh once per 64-channel chunk as a 136-pixel
-//   box, and tap kw reads it from pixel row kw on, as in conv_row_kernel: a third of the activation fill.  The
-//   consumers still walk (kh, kw, chunk, 16-channel step), so every chunk box of a kernel row stays resident until
-//   its tap kw = 2, and the results are bit-identical to conv_tc_kernel's.  Weight tiles stream through a ring of
-//   their own, and the producer stages the next tile while the consumers run the epilogue.
+//   conv2 of the bottleneck trunks' layers 3 and 4).  Persistent CTAs, one per SM, walk units of one 128-pixel column
+//   tile x two output rows (C_out = 128; warpgroup r computes row h + r) or one (256; warpgroup r computes half r),
+//   with conv_tc_kernel's wgmma shapes.  The producer stages each input row of a unit once per 64-channel chunk as a
+//   136-pixel box, and tap kw reads it from pixel row kw on, as in conv_row_kernel.  Each weight tile is staged once
+//   per unit, so with two rows it feeds four m64 groups instead of two: about half the operand fill from L2 of one
+//   row per unit.  The consumers still walk (kh, kw, chunk, 16-channel step), so every chunk box of a kernel row stays
+//   resident until its tap kw = 2, and the results are bit-identical to conv_tc_kernel's.  Weight tiles stream through
+//   a ring of their own, and the producer stages the next unit while the consumers run the epilogue.
 // block_row_kernel: a whole stride-1 BasicBlock with 32 channels (the three blocks of ResNet34 layer 1) in one launch,
 //   built on conv_row_kernel's row walk: conv1's output rows go to a ring of intermediate row slots in shared memory
 //   and conv2 reads them from there, so a block reads its input and writes its output once instead of making five
@@ -49,23 +51,26 @@ constexpr int kTileM = 128;
 constexpr int kRowHalo = 8;                                 // 128 + 2 pixels needed for three taps, 8 keeps 8-row groups
 constexpr int kMaxSlots = 16;                               // row slots of conv_row_kernel (barrier area: 1024 B)
 
-// +bias (+residual) -> ReLU -> fp16 of the 64 x N accumulator fragment of output pixels [w0, w0 + 64) of image row
-// `row` (= b * H_out + h).  A residual aliasing `out` is read before it is overwritten, by the same thread.
+// +bias (+residual) -> ReLU -> fp16 of MH = 1 or 2 64 x N accumulator fragments, consecutive at `acc`: fragment m
+// holds output pixels [w0 + 64 m, w0 + 64 m + 64) of image row `row` (= b * H_out + h).  A residual aliasing `out` is
+// read before it is overwritten, by the same thread.
 // WIDE: the fragment is output channels [n0, n0 + N) of C_out (n0 = blockIdx.y * N), pixels C_out channels apart.
-template <int N, bool WIDE = false>
+template <int N, bool WIDE = false, int MH = 1>
 __device__ __forceinline__ void conv_epilogue(const float* acc, const ConvParams& p, size_t row, int w0) {
   const int lane = threadIdx.x & 31;
   const int c0 = 2 * (lane & 3) + (WIDE ? (int)blockIdx.y * N : 0);
 #pragma unroll
+  for (int m = 0; m < MH; ++m)
+#pragma unroll
   for (int i = 0; i < 2; ++i) {
-    const int w = w0 + ((threadIdx.x >> 5) & 3) * 16 + (lane >> 2) + 8 * i;
+    const int w = w0 + 64 * m + ((threadIdx.x >> 5) & 3) * 16 + (lane >> 2) + 8 * i;
     if (w >= p.W_out) continue;
     const size_t pix = (row * p.W_out + w) * (size_t)(WIDE ? p.C_out : N);
-    // up to C_out = 64 all of the pixel's residual loads are issued before its first store: `out` may alias
-    // `residual`, so a load after a store cannot be hoisted and each would wait a full memory round trip (from 128 on
-    // the registers are not there: conv_tc_kernel<256> would spill)
+    // up to C_out = 128 all of the pixel's residual loads are issued before its first store: `out` may alias
+    // `residual`, so a load after a store cannot be hoisted and each would wait a full memory round trip (at 256 the
+    // registers are not there: conv_tc_kernel<256> would spill)
     __half2 res[N / 8];
-    if (N <= 64 && p.residual) {
+    if (N <= 128 && p.residual) {
 #pragma unroll
       for (int j = 0; j < N / 8; ++j) res[j] = *reinterpret_cast<const __half2*>(p.residual + pix + 8 * j + c0);
     }
@@ -73,9 +78,9 @@ __device__ __forceinline__ void conv_epilogue(const float* acc, const ConvParams
     for (int j = 0; j < N / 8; ++j) {
       const int c = 8 * j + c0;
       const float2 bb = __ldg(reinterpret_cast<const float2*>(p.bias + c));
-      float a = acc[4 * j + 2 * i] + bb.x, d = acc[4 * j + 2 * i + 1] + bb.y;
+      float a = acc[m * (N / 2) + 4 * j + 2 * i] + bb.x, d = acc[m * (N / 2) + 4 * j + 2 * i + 1] + bb.y;
       if (p.residual) {
-        const float2 r = __half22float2(N <= 64 ? res[j] : *reinterpret_cast<const __half2*>(p.residual + pix + c));
+        const float2 r = __half22float2(N <= 128 ? res[j] : *reinterpret_cast<const __half2*>(p.residual + pix + c));
         a += r.x;
         d += r.y;
       }
@@ -475,27 +480,41 @@ block_row_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant_
   }
 }
 
-// Plan of conv_chunk_row_kernel<N>: a ring of 136-pixel row boxes (one 64-channel chunk each) and a ring of (tap,
-// chunk) weight tiles.  N = 128: two CTAs per SM (113 KB each), so one CTA's epilogue runs while the other's MMAs
-// do; N = 256 (128 accumulator registers per thread): one (227 KB).  A kernel row keeps all N / 64 of its chunk boxes
-// resident until its last tap, so the box ring holds one more than that; the weight ring takes the rest.
+// Plan of conv_chunk_row_kernel<N>: one CTA per SM, a ring of 136-pixel row boxes (one 64-channel chunk each) and a
+// ring of (tap, chunk) weight tiles.  A unit is kRows output rows of one 128-pixel column tile.
+//   N = 128: two rows, warpgroup r owns row h + r as two m64 halves (128 accumulator registers per thread), so each
+//     weight tile feeds four m64n128k16 groups instead of two.  The unit stages four input rows h - 1 .. h + 2 of
+//     two chunks; while rows kh and kh + 1 of the unit are read the producer stages row kh + 2, and the next unit's
+//     first two rows while the last two are read: 8 box slots and 5 weight slots (218 KB).
+//   N = 256 (128 accumulator registers per thread for one m64 half): one row, warpgroup r owns half r; a kernel row
+//     keeps all four chunk boxes resident until its last tap, and the box ring holds one more: 5 box slots and 4
+//     weight slots (215 KB).
 template <int N>
 struct ChunkRowPlan {
   static constexpr int kChunks = N / 64;
-  static constexpr int kCtasPerSm = N == 256 ? 1 : 2;
+  static constexpr int kRows = N == 128 ? 2 : 1;
+  static constexpr int kHalves = N == 128 ? 2 : 1;         // m64 halves per warpgroup
   static constexpr uint32_t kABytes = (kTileM + kRowHalo) * 128;   // 17 KB, 1024-B multiple
   static constexpr uint32_t kBBytes = N * 128;
-  static constexpr uint32_t kASlots = N == 256 ? 5 : 3;
-  static constexpr uint32_t kBSlots = N == 256 ? 4 : 3;
-  static constexpr size_t kSmem = 2048 + kASlots * kABytes + kBSlots * kBBytes;   // 101 / 215 KB
-  static_assert(kASlots > kChunks && kASlots <= 8 && kBSlots <= 8, "chunk row ring plan");
+  static constexpr uint32_t kASlots = N == 256 ? 5 : 8;
+  static constexpr uint32_t kBSlots = N == 256 ? 4 : 5;
+  static constexpr size_t kSmem = 2048 + kASlots * kABytes + kBSlots * kBBytes;   // 218 / 215 KB
+  // the boxes read at one kh (kRows rows of kChunks) and one more, so that the next kh's first box can be staged
+  static_assert(kASlots >= kRows * kChunks + 1 && kASlots <= 8 && kBSlots <= 8, "chunk row ring plan");
+  static_assert(kSmem <= 227 * 1024, "chunk row shared memory");
+  // ring position of the box of input row r (0 .. kRows + 1 of the unit), chunk cc: the first kRows rows are needed
+  // together from kh = 0 on and are staged chunk by chunk, each later row at its kh = r - kRows + 1
+  __device__ __forceinline__ static uint32_t box(int r, int cc) {
+    return r < kRows ? cc * kRows + r : kRows * kChunks + (r - kRows) * kChunks + cc;
+  }
 };
 
 template <int N>
-__global__ void __launch_bounds__(kWgThreads, ChunkRowPlan<N>::kCtasPerSm)
+__global__ void __launch_bounds__(kWgThreads, 1)
 conv_chunk_row_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB, ConvParams p) {
   using P = ChunkRowPlan<N>;
-  constexpr int CH = P::kChunks, KSTEPS = 9 * CH;           // K steps of one output tile: (kh, kw, chunk)
+  constexpr int CH = P::kChunks, R = P::kRows, KSTEPS = 9 * CH;   // K steps of one unit: (kh, kw, chunk)
+  constexpr uint32_t BOXES = (R + 2) * CH;                 // boxes staged per unit
   extern __shared__ uint8_t smem_raw[];
   const uint32_t base = (smem_u32(smem_raw) + 1023u) & ~1023u;
   const uint32_t full_a = base, empty_a = base + 64, full_b = base + 128, empty_b = base + 192;   // 8 x 8 B each
@@ -509,7 +528,8 @@ conv_chunk_row_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_cons
   }
   __syncthreads();
 
-  // unit u: column tile u % tiles_w (neighbouring CTAs share the halo pixels in L2), then output row, then segment
+  // unit u: column tile u % tiles_w (neighbouring CTAs share the halo pixels in L2), then the unit's R output rows,
+  // then segment (p.bands units of R rows per column tile; the last one of an odd H_out has one row)
   if (warp == 8) {
     if ((threadIdx.x & 31) == 0) {
       prefetch_tensormap(&tmA);
@@ -517,21 +537,22 @@ conv_chunk_row_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_cons
       uint32_t qa = 0, qb = 0;                              // row boxes / weight tiles staged so far
       for (int u = blockIdx.x; u < p.num_tiles; u += gridDim.x) {
         const int wt = u % p.tiles_w, t = u / p.tiles_w;
-        const int h = t % p.H_out, b = t / p.H_out;
+        const int h = (t % p.bands) * R, b = t / p.bands;
         for (int s = 0; s < KSTEPS; ++s) {
           const int cc = s % CH, kw = (s / CH) % 3, kh = s / (3 * CH);
-          if (kw == 0) {                                    // row h - 1 + kh, chunk cc: read by taps kw = 0, 1, 2
-            const uint32_t q = qa + kh * CH + cc, slot = q % P::kASlots;
-            mbar_wait(empty_a + 8 * slot, ((q / P::kASlots) & 1) ^ 1);
-            mbar_expect_tx(full_a + 8 * slot, P::kABytes);
-            tma_load_4d(&tmA, full_a + 8 * slot, ring_a + slot * P::kABytes, cc * 64, wt * kTileM - 1, h - 1 + kh, b);
-          }
+          if (kw == 0)                                      // input rows first read at this kh, chunk cc
+            for (int r = kh == 0 ? 0 : kh + R - 1; r < kh + R; ++r) {
+              const uint32_t q = qa + P::box(r, cc), slot = q % P::kASlots;
+              mbar_wait(empty_a + 8 * slot, ((q / P::kASlots) & 1) ^ 1);
+              mbar_expect_tx(full_a + 8 * slot, P::kABytes);
+              tma_load_4d(&tmA, full_a + 8 * slot, ring_a + slot * P::kABytes, cc * 64, wt * kTileM - 1, h - 1 + r, b);
+            }
           const uint32_t q = qb + s, slot = q % P::kBSlots;
           mbar_wait(empty_b + 8 * slot, ((q / P::kBSlots) & 1) ^ 1);
           mbar_expect_tx(full_b + 8 * slot, P::kBBytes);
           tma_load_3d(&tmB, full_b + 8 * slot, ring_b + slot * P::kBBytes, cc * 64, 0, 3 * kh + kw);
         }
-        qa += 3 * CH;
+        qa += BOXES;
         qb += KSTEPS;
       }
     }
@@ -540,49 +561,69 @@ conv_chunk_row_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_cons
 
   const int wg = __shfl_sync(0xffffffffu, warp >> 2, 0);    // warp-uniform to the compiler: no wgmma serialisation
   const bool leader = (threadIdx.x & 127) == 0;
+  const int ro = R == 2 ? wg : 0;                           // this warpgroup's output row of the unit
+  // a box holds two arrivals: one per warpgroup for N = 256 (each reads its half), one per reading row for N = 128,
+  // whose first and last input rows have one reader, which arrives twice
   uint32_t qa = 0, qb = 0;
   for (int u = blockIdx.x; u < p.num_tiles; u += gridDim.x) {
     const int wt = u % p.tiles_w, t = u / p.tiles_w;
-    const int h = t % p.H_out, b = t / p.H_out;
-    float acc[N / 2];
+    const int h = (t % p.bands) * R + ro, b = t / p.bands;
+    const int w0 = wt * kTileM + (R == 2 ? 0 : wg * 64);    // first output pixel of this warpgroup
+    // the epilogue's residual pixels [w0, w0 + 64 kHalves) x N channels (256 lines of 128 B) go to L2 now, so that its
+    // loads, issued after the MMAs with no second CTA to hide them, do not wait on HBM
+    if (p.residual && h < p.H_out)
 #pragma unroll
-    for (int i = 0; i < N / 2; ++i) {
-      acc[i] = 0.f;
-      asm volatile("" : "+f"(acc[i]));                      // zeroed before the first wg_fence, not sunk past it
-    }
+      for (int l = (threadIdx.x & 127); l < 256; l += 128) {
+        const int w = w0 + l / (N / 64);
+        if (w < p.W_out)
+          asm volatile("prefetch.global.L2 [%0];" ::"l"(p.residual + ((size_t)(b * p.H_out + h) * p.W_out + w) * N +
+                                                         (l % (N / 64)) * 64));
+      }
+    float acc[P::kHalves][N / 2];
+#pragma unroll
+    for (int m = 0; m < P::kHalves; ++m)
+#pragma unroll
+      for (int i = 0; i < N / 2; ++i) {
+        acc[m][i] = 0.f;
+        asm volatile("" : "+f"(acc[m][i]));                 // zeroed before the first wg_fence, not sunk past it
+      }
     // the previous K step's slots, released once its wgmma have read them
-    uint32_t prev_b = 0, prev_a = 0;
-    bool prev_frees_a = false;
+    uint32_t prev_b = 0, prev_a = 0, prev_frees_a = 0;
     auto release = [&]() {
       if (leader) {
         mbar_arrive(empty_b + 8 * prev_b);
-        if (prev_frees_a) mbar_arrive(empty_a + 8 * prev_a);
+        if (prev_frees_a) mbar_arrive_n(empty_a + 8 * prev_a, prev_frees_a);
       }
     };
     // (kh, kw, chunk, k16): the order of conv_tc_kernel; tap kw reads the row box from pixel row kw on
     for (int s = 0; s < KSTEPS; ++s) {
       const int cc = s % CH, kw = (s / CH) % 3, kh = s / (3 * CH);
-      const uint32_t qA = qa + kh * CH + cc, sa = qA % P::kASlots;
+      const uint32_t qA = qa + P::box(kh + ro, cc), sa = qA % P::kASlots;
       const uint32_t qB = qb + s, sb = qB % P::kBSlots;
       mbar_wait(full_a + 8 * sa, (qA / P::kASlots) & 1);
       mbar_wait(full_b + 8 * sb, (qB / P::kBSlots) & 1);
       wg_fence();
-      const uint64_t ad = wg_desc(ring_a + sa * P::kABytes + (uint32_t)(wg * 64 + kw) * 128u, 128);
       const uint64_t bd = wg_desc(ring_b + sb * P::kBBytes, 128);
 #pragma unroll
-      for (int k = 0; k < 4; ++k) Wgmma<N>::mma(acc, ad + 2 * k, bd + 2 * k);
+      for (int m = 0; m < P::kHalves; ++m) {
+        const uint32_t half = R == 2 ? m : wg;
+        const uint64_t ad = wg_desc(ring_a + sa * P::kABytes + (half * 64 + kw) * 128u, 128);
+#pragma unroll
+        for (int k = 0; k < 4; ++k) Wgmma<N>::mma(acc[m], ad + 2 * k, bd + 2 * k);
+      }
       wg_commit();
       wg_wait<1>();
       if (s > 0) release();
       prev_b = sb;
       prev_a = sa;
-      prev_frees_a = kw == 2;                               // chunk box (kh, cc) is done after tap (kh, 2)
+      // box (kh + ro, cc) is done after tap (kh, 2)
+      prev_frees_a = kw == 2 ? (R == 2 && kh == 2 * ro ? 2 : 1) : 0;
     }
     wg_wait<0>();
     release();                                              // the producer stages the next unit during the epilogue
-    qa += 3 * CH;
+    qa += BOXES;
     qb += KSTEPS;
-    conv_epilogue<N>(acc, p, (size_t)b * p.H_out + h, wt * kTileM + wg * 64);
+    if (h < p.H_out) conv_epilogue<N, false, P::kHalves>(acc[0], p, (size_t)b * p.H_out + h, w0);
   }
 }
 
@@ -817,9 +858,12 @@ int conv_forward(const ConvLayer& L, const __half* in, const __half* residual, _
     p.bands = ceil_div(p.H_out, p.band);
     p.num_tiles = strips * p.bands;
   } else if (chunk_rows) {
-    // persistent over the output tiles (num_tiles as for conv_tc_kernel)
+    // one persistent CTA per SM over units of ChunkRowPlan::kRows output rows of a column tile
+    p.band = L.C_out == 256 ? ChunkRowPlan<256>::kRows : ChunkRowPlan<128>::kRows;
+    p.bands = ceil_div(p.H_out, p.band);
+    p.num_tiles = B * p.bands * p.tiles_w;
     smem = L.C_out == 256 ? ChunkRowPlan<256>::kSmem : ChunkRowPlan<128>::kSmem;
-    ctas = (L.C_out == 256 ? ChunkRowPlan<256>::kCtasPerSm : ChunkRowPlan<128>::kCtasPerSm) * num_sms;
+    ctas = num_sms;
   } else {
     p.b_bytes = (uint32_t)(n_tile * p.Ck * 2);
     // C_out = 256 needs 128 accumulator registers per thread: one CTA per SM with 4 deep stages; the narrower layers

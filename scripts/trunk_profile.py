@@ -2,7 +2,7 @@
 
     python scripts/trunk_profile.py                  # the library in this tree (needs a GPU), ResNet34
     python scripts/trunk_profile.py --model resnet293   # a bottleneck trunk (resnet152 | resnet221 | resnet293)
-    python scripts/trunk_profile.py --root OTHER --plan resident  # another tree's build, with its launch plan
+    python scripts/trunk_profile.py --root OTHER --plan fused  # another tree's build, with its launch plan
     python scripts/trunk_profile.py --model-only     # the byte model alone (no GPU)
 
 `ctx.emb_trunk` runs on --batch segments (the library's embedding sub-batch) under torch.profiler with CUDA
@@ -24,6 +24,9 @@ Byte model, per segment (computed from the shapes, not measured):
           fused   : rows, except that each stride-1 BasicBlock of layer 1 is one launch (block_row_kernel): it stages
                     each input row of a band once (plus four halo rows per band) as a 136-pixel box per 126-column
                     strip, and both convs' weights once per CTA; the intermediate activation stays on chip
+          pairs   : fused, except that the stride-1 3x3 convs with C_in = C_out = 128 (layer 3) compute two output rows
+                    per unit: four input rows per channel chunk as 136-pixel boxes, and every weight tile once for
+                    both rows
   HBM   = input + output (+ residual) activations once, and the weights once per launch shared by --batch segments;
           a fused block reads its input once and writes its output once
 """
@@ -84,7 +87,7 @@ def launches(model, plan):
     convs = trunk_convs(model)
     out = []
     for c in convs:
-        fuse = (plan == "fused" and model == "resnet34" and c[0] == 1 and c[1].endswith(".conv2") and out and
+        fuse = (plan in ("fused", "pairs") and model == "resnet34" and c[0] == 1 and c[1].endswith(".conv2") and out and
                 out[-1][0][1].endswith(".conv1") and out[-1][0][5] == 1)
         if fuse:
             out[-1].append(c)
@@ -123,13 +126,15 @@ def conv_model(c, plan, batch, sms=132):
     tiles = Ho * -(-Wo // TILE_M) * (cout // n_tile)
     b_tile = n_tile * ck * 2
     reuse = k == 3 and s == 1 and ((plan == "reuse" and cin == ck and cout <= 64) or
-                                   (plan in ("rows", "fused") and cin == cout and cout in (128, 256)))
-    if plan in ("resident", "rows", "fused") and k == 3 and s == 1 and cin == ck and cout == cin:
+                                   (plan in ("rows", "fused", "pairs") and cin == cout and cout in (128, 256)))
+    if plan in ("resident", "rows", "fused", "pairs") and k == 3 and s == 1 and cin == ck and cout == cin:
         tiles_w = -(-Wo // TILE_M)
         ctas, _, bands = resident_plan(cout, Ho, tiles_w, batch, sms)
         fill = tiles_w * (Ho + 2 * bands) * (TILE_M + HALO) * ck * 2 + ctas * k * k * b_tile / batch
     elif reuse:
-        fill = tiles * (k * chunks * (TILE_M + HALO) * ck * 2 + k * k * chunks * b_tile)
+        rows = 2 if plan == "pairs" and cout == 128 else 1              # output rows per unit
+        units = -(-Ho // rows) * -(-Wo // TILE_M)
+        fill = units * ((rows + k - 1) * chunks * (TILE_M + HALO) * ck * 2 + k * k * chunks * b_tile)
     else:
         fill = tiles * k * k * chunks * (TILE_M * ck * 2 + b_tile)
     act_out = Ho * Wo * cout * 2
@@ -167,8 +172,9 @@ def main():
     ap = argparse.ArgumentParser(description=__doc__, formatter_class=argparse.RawDescriptionHelpFormatter)
     ap.add_argument("--root", default=os.path.dirname(os.path.dirname(os.path.abspath(__file__))),
                     help="tree whose built library is timed (default: this one)")
-    ap.add_argument("--plan", choices=["fused", "rows", "resident", "reuse", "per-tap"], default="fused",
-                    help="launch plan of the timed library for the byte model (rows: a library whose layer 1 blocks "
+    ap.add_argument("--plan", choices=["pairs", "fused", "rows", "resident", "reuse", "per-tap"], default="pairs",
+                    help="launch plan of the timed library for the byte model (fused: a library whose layer 3 convs "
+                         "compute one output row per unit; rows: one whose layer 1 blocks "
                          "run as two conv launches each; resident: one whose layer 3 and "
                          "4 convs stage one box per tap; reuse: one whose layer 1 and 2 convs stage one box per kh; "
                          "per-tap: one box per tap everywhere)")
