@@ -21,7 +21,7 @@ struct ConvParams {
   const __half* residual;
   __half* out;
   // tensor-core plan: a box of a_rows pixels x Ck channels (a_tx bytes, padded to a_bytes); conv_tc_kernel: a stage =
-  // a box + the weights of one tap x C_out x Ck (b_bytes); conv_row_kernel: a stage = a row slot
+  // a box + the weights of one tap x C_out x Ck (b_bytes); conv_row_kernel takes its plan from RowPlan
   uint32_t a_rows, a_tx, a_bytes, b_bytes, nstages, swizzle;
 };
 

@@ -22,6 +22,9 @@
 //     after its three consumer rows are done (rows at the band edges arrive for the missing ones).
 //   - Warpgroups 0 / 1 take alternate output rows, each a whole 128-pixel row as two m64 wgmma per K step, so one
 //     warpgroup's epilogue runs while the other's MMAs do.
+//   - The epilogue goes through a shared-memory tile per warpgroup: the producer stages the row's residual there by
+//     TMA while the MMAs run, and the finished row leaves with one TMA store.  The epilogue makes no global loads, so
+//     it does not wait on a memory round trip per residual load (the output may alias the residual).
 //   The A operand comes straight from shared memory, the descriptor start moved by kw rows of 128 B, except for
 //   Ck = 32 (64-B rows: layer 1): those fragments are read with ldmatrix, the 64-B swizzle applied in software, and
 //   issued as register-A wgmma.
@@ -188,22 +191,71 @@ __device__ __forceinline__ void row_taps_c32(float (&acc)[2][N / 2], uint32_t sa
   }
 }
 
+__device__ __forceinline__ void st_shared_u32(uint32_t a, uint32_t v) {
+  asm volatile("st.shared.b32 [%0], %1;" ::"r"(a), "r"(v) : "memory");
+}
+__device__ __forceinline__ uint32_t ld_shared_u32(uint32_t a) {
+  uint32_t v;
+  asm volatile("ld.shared.b32 %0, [%1];" : "=r"(v) : "r"(a) : "memory");
+  return v;
+}
+__device__ __forceinline__ uint32_t h2_bits(__half2 h) { return *reinterpret_cast<uint32_t*>(&h); }
+// bar.sync over the 128 threads of one warpgroup (ids 1, 2; 0 is __syncthreads)
+__device__ __forceinline__ void named_bar_sync(int id) { asm volatile("bar.sync %0, 128;" ::"r"(id) : "memory"); }
+
+// Plan of conv_row_kernel<N> (C_in = C_out = N = the channel chunk): the nine weight taps resident, one epilogue tile
+// per warpgroup (its output row: 128 pixels x N channels, the residual's and the output's TMA box) and a ring of input
+// row slots (136-pixel boxes, padded to 1024 B).  Two warpgroups on consecutive rows hold four slots, so the rest is
+// how many rows the producer stages ahead.
+//   N = 64: one CTA per SM, 2 KB of barriers + 72 KB of weights + 2 x 16 KB tiles + 7 slots of 17 KB (225 KB).
+//   N = 32: two CTAs per SM at 113 KB, 2 KB + 18 KB + 2 x 8 KB + 8 slots of 9 KB (108 KB).
+template <int N>
+struct RowPlan {
+  static constexpr uint32_t kRowBytes = N * 2;             // one pixel = the swizzle width (64 or 128 B)
+  static constexpr uint32_t kTapBytes = N * kRowBytes;
+  static constexpr uint32_t kInTx = (kTileM + kRowHalo) * kRowBytes;
+  static constexpr uint32_t kSlotBytes = (kInTx + 1023u) & ~1023u;
+  static constexpr uint32_t kTileBytes = kTileM * kRowBytes;
+  static constexpr uint32_t kSlots = N == 64 ? 7 : 8;
+  // the producer stages output row j's residual after input row j + kResLag of the unit (staged rows 0 .. n + 1);
+  // the slot of that row is freed by output row j - 2, whose store also frees row j's tile
+  static constexpr int kResLag = (int)kSlots - 2;
+  static constexpr int kCtasPerSm = N == 32 ? 2 : 1;
+  static constexpr size_t kBudget = N == 32 ? 113u * 1024 : 227u * 1024;
+  static constexpr size_t kSmem = 2048 + 9 * kTapBytes + 2 * kTileBytes + kSlots * kSlotBytes;
+  static_assert(N == 32 || N == 64, "row kernel: 32 or 64 channels");
+  static_assert(kSlots >= 6 && kSlots <= kMaxSlots, "row ring: four slots in use and two ahead");
+  static_assert(kSmem <= kBudget && kSmem + kSlotBytes > kBudget, "row plan: every slot that fits");
+};
+
+// The output row goes through the warpgroup's epilogue tile: the producer stages the residual row there by TMA (zeros
+// beyond W_out), each thread replaces its residual values with its results in place, and one TMA store (clipped at
+// W_out) writes the row.  The tile is 128 pixels of kRowBytes, 16-B chunk c of pixel px stored at chunk
+// c ^ (px & 7) (128-B swizzle) or c ^ ((px >> 1) & 3) (64-B swizzle), as the input boxes.  Barriers: tile "full" (the
+// residual's TMA bytes) and "empty" (the warpgroup leader, once the previous store has read the tile).
 template <int N, int CK>
 __global__ void __launch_bounds__(kWgThreads, N == 32 ? 2 : 1)
-conv_row_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB, ConvParams p) {
-  constexpr uint32_t row_bytes = CK * 2;                   // = the swizzle width (64 or 128 B)
-  constexpr uint32_t b_tap_bytes = N * row_bytes;
+conv_row_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB,
+                const __grid_constant__ CUtensorMap tmR, const __grid_constant__ CUtensorMap tmO, ConvParams p) {
+  using P = RowPlan<N>;
+  static_assert(CK == N, "row kernel: one channel chunk");
+  constexpr uint32_t row_bytes = P::kRowBytes;
+  constexpr uint32_t b_tap_bytes = P::kTapBytes;
+  constexpr uint32_t nslots = P::kSlots;
   extern __shared__ uint8_t smem_raw[];
   const uint32_t base = (smem_u32(smem_raw) + 1023u) & ~1023u;
   const uint32_t bar_w = base, bar_full = base + 8, bar_empty = base + 8 + 8 * kMaxSlots;
+  const uint32_t tile_full = base + 512, tile_empty = base + 528;   // 2 x 8 B each
   const uint32_t wts = base + 1024;                         // 9 taps x [N][CK]
-  const uint32_t slot0 = wts + 9 * b_tap_bytes;             // 18 / 72 KB: slots stay 1024-B aligned
-  const uint32_t nslots = p.nstages;
+  const uint32_t tile0 = wts + 9 * b_tap_bytes;             // 18 / 72 KB: tiles and slots stay 1024-B aligned
+  const uint32_t slot0 = tile0 + 2 * P::kTileBytes;
+  const bool has_res = p.residual != nullptr;
   const int warp = threadIdx.x >> 5;
 
   if (threadIdx.x == 0) {
     mbar_init(bar_w, 1);
     for (uint32_t s = 0; s < nslots; ++s) { mbar_init(bar_full + 8 * s, 1); mbar_init(bar_empty + 8 * s, 3); }
+    for (uint32_t s = 0; s < 2; ++s) { mbar_init(tile_full + 8 * s, 1); mbar_init(tile_empty + 8 * s, 1); }
     asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
   }
   __syncthreads();
@@ -213,25 +265,45 @@ conv_row_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__
     if ((threadIdx.x & 31) == 0) {
       prefetch_tensormap(&tmA);
       prefetch_tensormap(&tmB);
+      if (has_res) prefetch_tensormap(&tmR);
       mbar_expect_tx(bar_w, 9 * b_tap_bytes);
       for (int kh = 0; kh < 3; ++kh) tma_load_3d(&tmB, bar_w, wts + 3 * kh * b_tap_bytes, 0, 0, 3 * kh);
       uint32_t s = 0;                                       // input rows staged so far
+      uint32_t k = 0;                                       // residual rows staged so far; row k goes to tile k & 1
       for (int u = blockIdx.x; u < p.num_tiles; u += gridDim.x) {
         const int wt = u % p.tiles_w, t = u / p.tiles_w;
         const int h0 = (t % p.bands) * p.band, b = t / p.bands;
         const int n = min(p.band, p.H_out - h0);
+        auto stage_residual = [&](int j) {
+          const uint32_t tile = k & 1, use = k >> 1;
+          mbar_wait(tile_empty + 8 * tile, (use & 1) ^ 1);
+          mbar_expect_tx(tile_full + 8 * tile, P::kTileBytes);
+          tma_load_4d(&tmR, tile_full + 8 * tile, tile0 + tile * P::kTileBytes, 0, wt * kTileM, h0 + j, b);
+          ++k;
+        };
         for (int r = 0; r < n + 2; ++r, ++s) {
           const uint32_t slot = s % nslots;
           mbar_wait(bar_empty + 8 * slot, ((s / nslots) & 1) ^ 1);
-          mbar_expect_tx(bar_full + 8 * slot, p.a_tx);
-          tma_load_4d(&tmA, bar_full + 8 * slot, slot0 + slot * p.a_bytes, 0, wt * kTileM - 1, h0 - 1 + r, b);
+          mbar_expect_tx(bar_full + 8 * slot, P::kInTx);
+          tma_load_4d(&tmA, bar_full + 8 * slot, slot0 + slot * P::kSlotBytes, 0, wt * kTileM - 1, h0 - 1 + r, b);
+          if (has_res && r >= P::kResLag) stage_residual(r - P::kResLag);
         }
+        if (has_res)
+          for (int j = max(0, n + 2 - P::kResLag); j < n; ++j) stage_residual(j);
       }
     }
     return;
   }
 
   const int wg = __shfl_sync(0xffffffffu, warp >> 2, 0);  // warp-uniform to the compiler: no wgmma serialisation
+  const int lane = threadIdx.x & 31;
+  const bool leader = (threadIdx.x & 127) == 0;
+  const uint32_t tile = tile0 + wg * P::kTileBytes;
+  const int c0 = 2 * (lane & 3);
+  float2 bias[N / 8];                                       // channels 8 j + c0, c0 + 1 of this thread's fragments
+#pragma unroll
+  for (int j = 0; j < N / 8; ++j) bias[j] = __ldg(reinterpret_cast<const float2*>(p.bias + 8 * j + c0));
+  if (leader) prefetch_tensormap(&tmO);
   mbar_wait(bar_w, 0);
   uint32_t s = 0;                                           // first input row of the current unit
   int item = 0;                                             // output rows walked so far; row `item` is warpgroup item & 1's
@@ -253,7 +325,7 @@ conv_row_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__
       for (int kh = 0; kh < 3; ++kh) {
         const uint32_t q = s + j + kh, slot = q % nslots;
         mbar_wait(bar_full + 8 * slot, (q / nslots) & 1);
-        const uint32_t sa = slot0 + slot * p.a_bytes;
+        const uint32_t sa = slot0 + slot * P::kSlotBytes;
         if constexpr (CK == 32) {
           row_taps_c32<N>(acc, sa, wts + 3 * kh * b_tap_bytes);
         } else {
@@ -273,16 +345,52 @@ conv_row_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__
       }
       wg_wait<0>();
       // slot of input row j + kh: one arrival per consumer row, the band's first / last row also for the missing ones
-      if ((threadIdx.x & 127) == 0)
+      if (leader)
 #pragma unroll
         for (int kh = 0; kh < 3; ++kh)
           mbar_arrive_n(bar_empty + 8 * ((s + j + kh) % nslots), 1 + (j == 0 ? 2 - kh : 0) + (j == n - 1 ? kh : 0));
-      const size_t row = (size_t)b * p.H_out + h0 + j;
+      // the tile holds this row's residual, or (without one) the previous store has read it
+      if (has_res) {
+        mbar_wait(tile_full + 8 * wg, (item >> 1) & 1);
+      } else {
+        if (leader) bulk_wait_read<0>();
+        named_bar_sync(1 + wg);
+      }
+      // conv_epilogue's arithmetic: +bias (+residual) -> ReLU -> fp16, written over the residual it read
 #pragma unroll
-      for (int m = 0; m < 2; ++m) conv_epilogue<N>(acc[m], p, row, wt * kTileM + m * 64);
+      for (int m = 0; m < 2; ++m)
+#pragma unroll
+        for (int i = 0; i < 2; ++i) {
+          const uint32_t px = m * 64 + (warp & 3) * 16 + (lane >> 2) + 8 * i;
+          const uint32_t swz = row_bytes == 128 ? px & 7u : (px >> 1) & 3u;
+#pragma unroll
+          for (int jj = 0; jj < N / 8; ++jj) {
+            const uint32_t ta = tile + px * row_bytes + ((jj ^ swz) << 4) + 2 * c0;
+            float a = acc[m][4 * jj + 2 * i] + bias[jj].x, d = acc[m][4 * jj + 2 * i + 1] + bias[jj].y;
+            if (has_res) {
+              const uint32_t rb = ld_shared_u32(ta);
+              const float2 r = __half22float2(*reinterpret_cast<const __half2*>(&rb));
+              a += r.x;
+              d += r.y;
+            }
+            if (p.relu) { a = fmaxf(a, 0.f); d = fmaxf(d, 0.f); }
+            st_shared_u32(ta, h2_bits(__floats2half2_rn(a, d)));
+          }
+        }
+      fence_proxy_async();                                  // the tile's writes, visible to the TMA store
+      named_bar_sync(1 + wg);
+      if (leader) {
+        tma_store_4d(&tmO, tile, 0, wt * kTileM, h0 + j, b);
+        bulk_commit();
+        if (has_res) {                                      // the producer stages the next residual once it is read
+          bulk_wait_read<0>();
+          mbar_arrive(tile_empty + 8 * wg);
+        }
+      }
     }
     s += n + 2;
   }
+  if (leader) bulk_wait<0>();                               // the last stores are done before the CTA exits
 }
 
 // Plan of block_row_kernel<32>: both convs' nine taps resident (2 x 18 KB), a ring of input row slots and a ring of
@@ -306,15 +414,6 @@ struct BlockParams {
   __half* out;
 };
 
-__device__ __forceinline__ void st_shared_u32(uint32_t a, uint32_t v) {
-  asm volatile("st.shared.b32 [%0], %1;" ::"r"(a), "r"(v) : "memory");
-}
-__device__ __forceinline__ uint32_t ld_shared_u32(uint32_t a) {
-  uint32_t v;
-  asm volatile("ld.shared.b32 %0, [%1];" : "=r"(v) : "r"(a) : "memory");
-  return v;
-}
-__device__ __forceinline__ uint32_t h2_bits(__half2 h) { return *reinterpret_cast<uint32_t*>(&h); }
 
 // One stride-1 BasicBlock with 32 channels and an identity shortcut, out = relu(bn2(conv2(relu(bn1(conv1(x))))) + x),
 // without the intermediate activation leaving the SM.  Persistent CTAs walk units of one segment x one column strip of
@@ -840,15 +939,9 @@ int conv_forward(const ConvLayer& L, const __half* in, const __half* residual, _
   size_t smem;
   int ctas = 0;
   if (rows) {
-    // resident weights + as many row slots as fit: two CTAs per SM for C_out = 32 (113 KB each), one for C_out = 64
-    // (227 KB: 72 KB weights + 9 slots of 17 KB)
-    const int per_sm = L.C_out == 32 ? 2 : 1;
-    const size_t budget = per_sm == 2 ? 113u * 1024 : 227u * 1024;
-    const size_t fixed = 2048 + (size_t)9 * L.C_out * p.Ck * 2;
-    p.nstages = (uint32_t)std::min<size_t>(kMaxSlots, (budget - fixed) / p.a_bytes);
-    // two warpgroups on consecutive rows hold four slots; the rest lets the producer run ahead
-    B200_CHECK(p.nstages >= 6, B200_ERR_STATE, "conv %d -> %d: row ring too shallow", L.C_in, L.C_out);
-    smem = fixed + (size_t)p.nstages * p.a_bytes;
+    // RowPlan: resident weights, two epilogue tiles and a ring of row slots; two CTAs per SM for C_out = 32, one for 64
+    const int per_sm = L.C_out == 32 ? RowPlan<32>::kCtasPerSm : RowPlan<64>::kCtasPerSm;
+    smem = L.C_out == 32 ? RowPlan<32>::kSmem : RowPlan<64>::kSmem;
     // full-height bands while the column strips fill every CTA (a 264-segment sub-batch: 2112 / 1056 strips for
     // layers 1 / 2), else shorter bands so that small batches still reach every SM; each band re-stages two halo rows
     ctas = per_sm * num_sms;
@@ -891,6 +984,21 @@ int conv_forward(const ConvLayer& L, const __half* in, const __half* residual, _
     const cuuint32_t box[3] = {(cuuint32_t)p.Ck, (cuuint32_t)n_tile, rows ? 3u : 1u};
     if ((rc = encode_f16_map(&tmB, 3, L.w, dims, strides, box, nullptr, swz, "B"))) return rc;
   }
+  if (rows) {
+    // the residual and the output, as 128-pixel boxes of the output's shape: the row kernel's epilogue tiles
+    CUtensorMap tmR{}, tmO;
+    const cuuint64_t dims[4] = {(cuuint64_t)L.C_out, (cuuint64_t)p.W_out, (cuuint64_t)p.H_out, (cuuint64_t)B};
+    const cuuint64_t strides[3] = {(cuuint64_t)L.C_out * 2, (cuuint64_t)p.W_out * L.C_out * 2,
+                                   (cuuint64_t)p.H_out * p.W_out * L.C_out * 2};
+    const cuuint32_t box[4] = {(cuuint32_t)L.C_out, (cuuint32_t)kTileM, 1, 1};
+    if (residual && (rc = encode_f16_map(&tmR, 4, residual, dims, strides, box, nullptr, swz, "residual"))) return rc;
+    if ((rc = encode_f16_map(&tmO, 4, out, dims, strides, box, nullptr, swz, "out"))) return rc;
+    auto kernel = p.Ck == 32 ? conv_row_kernel<32, 32> : conv_row_kernel<64, 64>;
+    B200_CUDA_OK(cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+    kernel<<<(unsigned)std::min(p.num_tiles, ctas), kWgThreads, smem, stream>>>(tmA, tmB, tmR, tmO, p);
+    B200_CUDA_OK(cudaGetLastError());
+    return B200_OK;
+  }
   auto launch = [&](auto kernel) -> int {
     B200_CUDA_OK(cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
     const dim3 grid((unsigned)(ctas ? std::min(p.num_tiles, ctas) : p.num_tiles), (unsigned)(L.C_out / n_tile));
@@ -898,7 +1006,6 @@ int conv_forward(const ConvLayer& L, const __half* in, const __half* residual, _
     B200_CUDA_OK(cudaGetLastError());
     return B200_OK;
   };
-  if (rows) return p.Ck == 32 ? launch(conv_row_kernel<32, 32>) : launch(conv_row_kernel<64, 64>);
   if (chunk_rows) return L.C_out == 256 ? launch(conv_chunk_row_kernel<256>) : launch(conv_chunk_row_kernel<128>);
   if (p.Ck == 32) {
     switch (L.C_out) {

@@ -1,5 +1,5 @@
-// PTX wrappers shared by the Hopper tensor-core kernels (conv trunk, split-precision GEMM): mbarrier, TMA, wgmma and
-// its shared-memory descriptors.  Descriptor bit layout: PTX ISA, "Matrix Descriptor Format" of wgmma (sm_90a).
+// PTX wrappers shared by the Hopper tensor-core kernels (conv trunk, split-precision GEMM): mbarrier, TMA loads and
+// stores, wgmma and its shared-memory descriptors.  Descriptor bit layout: PTX ISA, "Matrix Descriptor Format" of wgmma (sm_90a).
 #pragma once
 #include "common.cuh"
 #include <cuda.h>
@@ -55,6 +55,22 @@ __device__ __forceinline__ void tma_load_2d(const CUtensorMap* tm, uint32_t bar,
 __device__ __forceinline__ void prefetch_tensormap(const CUtensorMap* tm) {
   asm volatile("prefetch.tensormap [%0];" ::"l"(reinterpret_cast<uint64_t>(tm)) : "memory");
 }
+// TMA store of a shared-memory tile (written in the map's swizzled layout) into the box at (c0 .. c3), clipped at the
+// tensor's bounds; one bulk group per commit.  The generic-proxy writes of the tile must be made visible to the async
+// proxy first (fence_proxy_async by every writing thread, then a barrier among them).
+__device__ __forceinline__ void tma_store_4d(const CUtensorMap* tm, uint32_t src, int c0, int c1, int c2, int c3) {
+  asm volatile("cp.async.bulk.tensor.4d.global.shared::cta.bulk_group [%0, {%2, %3, %4, %5}], [%1];"
+               ::"l"(reinterpret_cast<uint64_t>(tm)), "r"(src), "r"(c0), "r"(c1), "r"(c2), "r"(c3)
+               : "memory");
+}
+__device__ __forceinline__ void fence_proxy_async() { asm volatile("fence.proxy.async.shared::cta;" ::: "memory"); }
+__device__ __forceinline__ void bulk_commit() { asm volatile("cp.async.bulk.commit_group;" ::: "memory"); }
+// all but the newest N bulk groups of this thread have read their shared-memory source (it may be overwritten) ...
+template <int N>
+__device__ __forceinline__ void bulk_wait_read() { asm volatile("cp.async.bulk.wait_group.read %0;" ::"n"(N) : "memory"); }
+// ... or have completed
+template <int N>
+__device__ __forceinline__ void bulk_wait() { asm volatile("cp.async.bulk.wait_group %0;" ::"n"(N) : "memory"); }
 
 // wgmma shared-memory descriptor of a K-major operand tile written by TMA with hardware swizzle (8-row core groups
 // `sbo_bytes` apart):  [0,14) start >> 4 | [16,30) LBO >> 4 (unused for swizzled K-major, 1) | [32,46) SBO >> 4 |

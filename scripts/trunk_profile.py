@@ -2,7 +2,7 @@
 
     python scripts/trunk_profile.py                  # the library in this tree (needs a GPU), ResNet34
     python scripts/trunk_profile.py --model resnet293   # a bottleneck trunk (resnet152 | resnet221 | resnet293)
-    python scripts/trunk_profile.py --root OTHER --plan fused  # another tree's build, with its launch plan
+    python scripts/trunk_profile.py --root OTHER --plan pairs  # another tree's build, with its launch plan
     python scripts/trunk_profile.py --model-only     # the byte model alone (no GPU)
 
 `ctx.emb_trunk` runs on --batch segments (the library's embedding sub-batch) under torch.profiler with CUDA
@@ -27,11 +27,14 @@ Byte model, per segment (computed from the shapes, not measured):
           pairs   : fused, except that the stride-1 3x3 convs with C_in = C_out = 128 (layer 3) compute two output rows
                     per unit: four input rows per channel chunk as 136-pixel boxes, and every weight tile once for
                     both rows
+          epilogue: pairs, except that the resident convs with a residual (conv_row_kernel: layer 2's conv2) also
+                    stage each output row's residual, 128 pixels, into shared memory for the epilogue
   HBM   = input + output (+ residual) activations once, and the weights once per launch shared by --batch segments;
           a fused block reads its input once and writes its output once
 """
 import argparse
 import os
+import statistics
 import subprocess
 import sys
 
@@ -87,7 +90,7 @@ def launches(model, plan):
     convs = trunk_convs(model)
     out = []
     for c in convs:
-        fuse = (plan in ("fused", "pairs") and model == "resnet34" and c[0] == 1 and c[1].endswith(".conv2") and out and
+        fuse = (plan in ("fused", "pairs", "epilogue") and model == "resnet34" and c[0] == 1 and c[1].endswith(".conv2") and out and
                 out[-1][0][1].endswith(".conv1") and out[-1][0][5] == 1)
         if fuse:
             out[-1].append(c)
@@ -126,13 +129,16 @@ def conv_model(c, plan, batch, sms=132):
     tiles = Ho * -(-Wo // TILE_M) * (cout // n_tile)
     b_tile = n_tile * ck * 2
     reuse = k == 3 and s == 1 and ((plan == "reuse" and cin == ck and cout <= 64) or
-                                   (plan in ("rows", "fused", "pairs") and cin == cout and cout in (128, 256)))
-    if plan in ("resident", "rows", "fused", "pairs") and k == 3 and s == 1 and cin == ck and cout == cin:
+                                   (plan in ("rows", "fused", "pairs", "epilogue") and cin == cout and
+                                    cout in (128, 256)))
+    if plan in ("resident", "rows", "fused", "pairs", "epilogue") and k == 3 and s == 1 and cin == ck and cout == cin:
         tiles_w = -(-Wo // TILE_M)
         ctas, _, bands = resident_plan(cout, Ho, tiles_w, batch, sms)
         fill = tiles_w * (Ho + 2 * bands) * (TILE_M + HALO) * ck * 2 + ctas * k * k * b_tile / batch
+        if plan == "epilogue" and res:
+            fill += tiles_w * Ho * TILE_M * cout * 2
     elif reuse:
-        rows = 2 if plan == "pairs" and cout == 128 else 1              # output rows per unit
+        rows = 2 if plan in ("pairs", "epilogue") and cout == 128 else 1   # output rows per unit
         units = -(-Ho // rows) * -(-Wo // TILE_M)
         fill = units * ((rows + k - 1) * chunks * (TILE_M + HALO) * ck * 2 + k * k * chunks * b_tile)
     else:
@@ -172,8 +178,10 @@ def main():
     ap = argparse.ArgumentParser(description=__doc__, formatter_class=argparse.RawDescriptionHelpFormatter)
     ap.add_argument("--root", default=os.path.dirname(os.path.dirname(os.path.abspath(__file__))),
                     help="tree whose built library is timed (default: this one)")
-    ap.add_argument("--plan", choices=["pairs", "fused", "rows", "resident", "reuse", "per-tap"], default="pairs",
-                    help="launch plan of the timed library for the byte model (fused: a library whose layer 3 convs "
+    ap.add_argument("--plan", choices=["epilogue", "pairs", "fused", "rows", "resident", "reuse", "per-tap"],
+                    default="epilogue",
+                    help="launch plan of the timed library for the byte model (pairs: a library whose layer 2 convs "
+                         "read the residual from global memory; fused: one whose layer 3 convs "
                          "compute one output row per unit; rows: one whose layer 1 blocks "
                          "run as two conv launches each; resident: one whose layer 3 and "
                          "4 convs stage one box per tap; reuse: one whose layer 1 and 2 convs stage one box per kh; "
@@ -254,6 +262,17 @@ def main():
               f"fill {fmb * args.batch / sec / 1e3:6.0f} GB/s  HBM {hmb * args.batch / sec / 1e3:6.0f} GB/s")
     print(f"trunk convs: {tot_us / 1e3:.3f} ms per call of {args.batch} segments "
           f"({tot_us / args.batch:.1f} us per segment)")
+    # what the residual costs: median time of the single-launch stride-1 3x3 convs with a residual (BasicBlock conv2)
+    # over the median of those without one (conv1), per layer
+    for li in sorted(per_layer):
+        t = {True: [], False: []}
+        for (cs, *_), t_us in zip(rows, us):
+            c = cs[0]
+            if len(cs) == 1 and c[0] == li and c[4] == 3 and c[5] == 1:
+                t[c[8]].append(t_us)
+        if t[True] and t[False]:
+            print(f"layer{li} conv2/conv1: {statistics.median(t[True]) / statistics.median(t[False]):.3f} "
+                  f"({statistics.median(t[True]):.1f} / {statistics.median(t[False]):.1f} us, medians)")
 
 
 if __name__ == "__main__":
