@@ -47,7 +47,7 @@ int b200_ctx_destroy(b200_ctx* ctx);
  *   "ssl_max_batch" (32): 10 s windows per SSeRiouSS sub-batch, also the longest SSeRiouSS window (32 x 10 s);
  *   "conv_impl" 1 = wgmma tensor-core trunk convs (default), 0 = CUDA-core reference conv; "seg_gemm_impl" 1 = wgmma
  *   split-precision GEMMs, 0 = fp32 CUDA-core twins; "seg_conv_impl" 1 = SincNet sinc / Conv1d layers as split-precision
- *   wgmma implicit GEMMs, 0 = fp32 CUDA-core twins; "seg_rec_impl" 1 = LSTM recurrence as split-precision wgmma on
+ *   wgmma implicit GEMMs in persistent kernels, 2 = the same with one CTA per tile (bit-identical), 0 = fp32 CUDA-core twins; "seg_rec_impl" 1 = LSTM recurrence as split-precision wgmma on
  *   2-CTA clusters (with "seg_gemm_impl" 1), 0 = fp32 CUDA-core twin; "fbank_share" 1 = overlapping chunks share their fbank frames;
  *   "profile" 1 = CUDA-event timers around the trunk / the segmentation (b200_ctx_timer); "linkage_grid_min" (32769,
  *   from 2 up to that default): the smallest linkage problem that runs on the whole-GPU path (b200_linkage_centroid).

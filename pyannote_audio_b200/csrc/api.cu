@@ -41,7 +41,8 @@ struct b200_ctx {
   int num_sms = 132;
   int seg_gemm_impl = 1;   // 1 = split-fp16 wgmma GEMMs for the LSTM input projections / linear layers, 0 = fp32 SIMT
   int seg_rec_impl = 1;    // 1 = LSTM recurrence as split-fp16 wgmma on 2-CTA clusters (needs seg_gemm_impl = 1), 0 = fp32 SIMT
-  int seg_conv_impl = 1;   // 1 = SincNet sinc / Conv1d layers as split-fp16 wgmma implicit GEMMs, 0 = fp32 CUDA-core twins
+  int seg_conv_impl = 1;   // 1 = SincNet sinc / Conv1d layers as persistent split-fp16 wgmma implicit GEMMs, 0 = fp32
+                           // CUDA-core twins, 2 = wgmma with one CTA per tile (bit-exact reference of 1)
   int conv_impl = 1;       // 1 = wgmma implicit-GEMM trunk convs, 0 = fp32 CUDA-core reference conv, 2 = wgmma with
                            // one weight tap per stage for every conv (bit-exact reference of 1)
   // chunks per segmentation sub-batch: 2112 = 33 recurrence tiles of 64 sequences x 2 directions x 2-CTA clusters
@@ -502,7 +503,7 @@ int b200_ctx_set_option(b200_ctx* ctx, const char* key, int64_t value) {
   }
   else B200_CHECK(false, B200_ERR_INVALID, "unknown option '%s'", key);
   B200_CHECK(ctx->seg_max_batch >= 1 && ctx->emb_max_batch >= 1 && ctx->ssl_max_batch >= 1 && ctx->conv_impl >= 0 && ctx->conv_impl <= 2 &&
-                 ctx->seg_gemm_impl >= 0 && ctx->seg_gemm_impl <= 1 && ctx->seg_conv_impl >= 0 && ctx->seg_conv_impl <= 1 &&
+                 ctx->seg_gemm_impl >= 0 && ctx->seg_gemm_impl <= 1 && ctx->seg_conv_impl >= 0 && ctx->seg_conv_impl <= 2 &&
                  ctx->seg_rec_impl >= 0 && ctx->seg_rec_impl <= 1,
              B200_ERR_INVALID, "option '%s' value %lld out of range", key, (long long)value);
   return B200_OK;
@@ -1442,7 +1443,9 @@ int b200_xvec_forward(b200_ctx* ctx, const float* wav, const int64_t* off, int64
   for (int u0 = 0; u0 < num_utts; u0 += nbmax) {
     const int nb = std::min(nbmax, num_utts - u0);
     const int M = nb * F;
-    if ((rc = sincnet_forward(X.sinc, geom, wav, ctx->d_off + u0, ctx->d_valid + u0, nb, w.sinc, w.x0, 1, st)))
+    // always on the tensor cores; seg_conv_impl = 2 selects the per-tile reference kernels here too
+    const int sinc_impl = ctx->seg_conv_impl == 2 ? 2 : 1;
+    if ((rc = sincnet_forward(X.sinc, geom, wav, ctx->d_off + u0, ctx->d_valid + u0, nb, w.sinc, w.x0, sinc_impl, st)))
       return rc;
     ctx->launches += sincnet_launches(geom);
     if ((rc = split_f16(w.x0, w.xh, w.xl, (size_t)M * 64, st))) return rc;

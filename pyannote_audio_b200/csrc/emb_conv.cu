@@ -200,8 +200,6 @@ __device__ __forceinline__ uint32_t ld_shared_u32(uint32_t a) {
   return v;
 }
 __device__ __forceinline__ uint32_t h2_bits(__half2 h) { return *reinterpret_cast<uint32_t*>(&h); }
-// bar.sync over the 128 threads of one warpgroup (ids 1, 2; 0 is __syncthreads)
-__device__ __forceinline__ void named_bar_sync(int id) { asm volatile("bar.sync %0, 128;" ::"r"(id) : "memory"); }
 
 // Plan of conv_row_kernel<N> (C_in = C_out = N = the channel chunk): the nine weight taps resident, one epilogue tile
 // per warpgroup (its output row: 128 pixels x N channels, the residual's and the output's TMA box) and a ring of input

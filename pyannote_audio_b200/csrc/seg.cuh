@@ -92,12 +92,14 @@ int split_f16(const float* x, __half* hi, __half* lo, size_t n, cudaStream_t st)
 int lstm_rec_wg(const float* Gx, const __half* Wh, const __half* Wl, __half* Yh, __half* Yl, int NB, int T,
                 cudaStream_t stream);
 
-// SincNet layers on the tensor cores (seg_conv_wg.cu); same outputs and partial sums as the fp32 twins
+// SincNet layers on the tensor cores (seg_conv_wg.cu); same outputs and partial sums as the fp32 twins.  impl 1:
+// persistent, weight-resident kernels; 2: one CTA per tile, bit-identical to 1
 int sinc_wg_forward(const SegGeom& g, const float* wav, const long long* chunk_off, const int* chunk_valid,
                     const float2* affine, const __half* Wh, const __half* Wl, int NB, float* P0, double2* part,
-                    cudaStream_t stream);
+                    int impl, cudaStream_t stream);
 int conv5_wg_forward(const SegGeom& g, int layer, const float* Pin, const float2* affine, const __half* Wh,
-                     const __half* Wl, const float* bias, int NB, float* Pout, double2* part, cudaStream_t stream);
+                     const __half* Wl, const float* bias, int NB, float* Pout, double2* part, int impl,
+                     cudaStream_t stream);
 
 // SincNet front-end on NB windows of g.W samples: wav + per-window (offset, valid) -> X0 [NB][g.pool2][64] fp32
 // (60 features + 4 zero pad)

@@ -406,11 +406,12 @@ int sincnet_forward(const SincNetWeights& W, const SegGeom& g, const float* wav,
   if (nslices > 1)
     wav_finalize_kernel<<<ceil_div(NB, 128), 128, 0, stream>>>(w.wav_part, nslices, g.W, W.wav_w, W.wav_b, w.af_wav,
                                                                NB);
-  // conv_impl: 1 = split-fp16 wgmma kernels (default), 0 = the fp32 CUDA-core twins
+  // conv_impl: 1 = persistent split-fp16 wgmma kernels (default), 2 = one wgmma CTA per tile, 0 = the fp32 CUDA-core
+  // twins
   int rc;
   if (conv_impl) {
     if ((rc = sinc_wg_forward(g, wav, chunk_off, chunk_valid, w.af_wav, W.sinc_wg_hi, W.sinc_wg_lo, NB, w.P0, w.part0,
-                              stream)))
+                              conv_impl, stream)))
       return rc;
   } else {
     B200_CUDA_OK(cudaFuncSetAttribute(sinc_pool_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem_sinc));
@@ -420,7 +421,7 @@ int sincnet_forward(const SincNetWeights& W, const SegGeom& g, const float* wav,
   in_stats(w.part0, g.tiles0, w.red0, w.red1, g.pool0, 80, W.in_gamma[0], W.in_beta[0], w.af0, NB * 80, stream);
   if (conv_impl) {
     if ((rc = conv5_wg_forward(g, 0, w.P0, w.af0, W.conv_wg_hi[0], W.conv_wg_lo[0], W.conv_b[0], NB, w.P1, w.part1,
-                               stream)))
+                               conv_impl, stream)))
       return rc;
   } else {
     B200_CUDA_OK(cudaFuncSetAttribute(conv5_pool_kernel<80>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem_c80));
@@ -430,7 +431,7 @@ int sincnet_forward(const SincNetWeights& W, const SegGeom& g, const float* wav,
   in_stats(w.part1, g.tiles1, w.red0, w.red1, g.pool1, 60, W.in_gamma[1], W.in_beta[1], w.af1, NB * 60, stream);
   if (conv_impl) {
     if ((rc = conv5_wg_forward(g, 1, w.P1, w.af1, W.conv_wg_hi[1], W.conv_wg_lo[1], W.conv_b[1], NB, w.P2, w.part2,
-                               stream)))
+                               conv_impl, stream)))
       return rc;
   } else {
     B200_CUDA_OK(cudaFuncSetAttribute(conv5_pool_kernel<60>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem_c60));

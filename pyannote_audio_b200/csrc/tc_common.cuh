@@ -89,6 +89,8 @@ __device__ __forceinline__ void ldsm_x4(uint32_t* r, uint32_t saddr) {
                : "r"(saddr)
                : "memory");
 }
+// bar.sync over the 128 threads of one warpgroup (ids 1, 2; 0 is __syncthreads)
+__device__ __forceinline__ void named_bar_sync(int id) { asm volatile("bar.sync %0, 128;" ::"r"(id) : "memory"); }
 __device__ __forceinline__ void wg_fence() { asm volatile("wgmma.fence.sync.aligned;" ::: "memory"); }
 __device__ __forceinline__ void wg_commit() { asm volatile("wgmma.commit_group.sync.aligned;" ::: "memory"); }
 template <int N>
