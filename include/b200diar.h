@@ -48,7 +48,8 @@ int b200_ctx_destroy(b200_ctx* ctx);
  *   "conv_impl" 1 = wgmma tensor-core trunk convs (default), 0 = CUDA-core reference conv; "seg_gemm_impl" 1 = wgmma
  *   split-precision GEMMs, 0 = fp32 CUDA-core twins; "seg_conv_impl" 1 = SincNet sinc / Conv1d layers as split-precision
  *   wgmma implicit GEMMs in persistent kernels, 2 = the same with one CTA per tile (bit-identical), 0 = fp32 CUDA-core twins; "seg_rec_impl" 1 = LSTM recurrence as split-precision wgmma on
- *   2-CTA clusters (with "seg_gemm_impl" 1), 0 = fp32 CUDA-core twin; "fbank_share" 1 = overlapping chunks share their fbank frames;
+ *   2-CTA clusters with two warpgroups per CTA (with "seg_gemm_impl" 1), 2 = the same with one warpgroup per CTA
+ *   (bit-identical), 0 = fp32 CUDA-core twin; "fbank_share" 1 = overlapping chunks share their fbank frames;
  *   "profile" 1 = CUDA-event timers around the trunk / the segmentation (b200_ctx_timer); "linkage_grid_min" (32769,
  *   from 2 up to that default): the smallest linkage problem that runs on the whole-GPU path (b200_linkage_centroid).
  *   Unknown keys and values out of range return B200_ERR_INVALID. */

@@ -40,7 +40,8 @@ struct b200_ctx {
   int device = 0;
   int num_sms = 132;
   int seg_gemm_impl = 1;   // 1 = split-fp16 wgmma GEMMs for the LSTM input projections / linear layers, 0 = fp32 SIMT
-  int seg_rec_impl = 1;    // 1 = LSTM recurrence as split-fp16 wgmma on 2-CTA clusters (needs seg_gemm_impl = 1), 0 = fp32 SIMT
+  int seg_rec_impl = 1;    // 1 = LSTM recurrence as split-fp16 wgmma on 2-CTA clusters, two warpgroups per CTA (needs
+                           // seg_gemm_impl = 1), 0 = fp32 SIMT, 2 = one warpgroup per CTA (bit-exact reference of 1)
   int seg_conv_impl = 1;   // 1 = SincNet sinc / Conv1d layers as persistent split-fp16 wgmma implicit GEMMs, 0 = fp32
                            // CUDA-core twins, 2 = wgmma with one CTA per tile (bit-exact reference of 1)
   int conv_impl = 1;       // 1 = wgmma implicit-GEMM trunk convs, 0 = fp32 CUDA-core reference conv, 2 = wgmma with
@@ -504,7 +505,7 @@ int b200_ctx_set_option(b200_ctx* ctx, const char* key, int64_t value) {
   else B200_CHECK(false, B200_ERR_INVALID, "unknown option '%s'", key);
   B200_CHECK(ctx->seg_max_batch >= 1 && ctx->emb_max_batch >= 1 && ctx->ssl_max_batch >= 1 && ctx->conv_impl >= 0 && ctx->conv_impl <= 2 &&
                  ctx->seg_gemm_impl >= 0 && ctx->seg_gemm_impl <= 1 && ctx->seg_conv_impl >= 0 && ctx->seg_conv_impl <= 2 &&
-                 ctx->seg_rec_impl >= 0 && ctx->seg_rec_impl <= 1,
+                 ctx->seg_rec_impl >= 0 && ctx->seg_rec_impl <= 2,
              B200_ERR_INVALID, "option '%s' value %lld out of range", key, (long long)value);
   return B200_OK;
 }

@@ -88,8 +88,9 @@ int gemm_tc_split(const __half* A_hi, const __half* A_lo, int lda, const __half*
                   int act, int num_sms, cudaStream_t stream, float* const* C_peers = nullptr, int n_peers = 0,
                   const GemmTaps& taps = GemmTaps());
 int split_f16(const float* x, __half* hi, __half* lo, size_t n, cudaStream_t st);
-// tensor-core recurrence (seg_lstm_wg.cu): Gx [NB][T][1024] -> layer output as fp16 (hi, lo) [NB][T][256]
-int lstm_rec_wg(const float* Gx, const __half* Wh, const __half* Wl, __half* Yh, __half* Yl, int NB, int T,
+// tensor-core recurrence (seg_lstm_wg.cu): Gx [NB][T][1024] -> layer output as fp16 (hi, lo) [NB][T][256].  impl 1:
+// two warpgroups per CTA with Gx software-pipelined into registers; 2: one warpgroup per CTA, bit-identical to 1
+int lstm_rec_wg(const float* Gx, const __half* Wh, const __half* Wl, __half* Yh, __half* Yl, int NB, int T, int impl,
                 cudaStream_t stream);
 
 // SincNet layers on the tensor cores (seg_conv_wg.cu); same outputs and partial sums as the fp32 twins.  impl 1:

@@ -268,8 +268,9 @@ int lstm_head_forward(const SegWeights& W, const float* x0, int NB, int T, void*
     else
       rc = sgemm_nt(in, W.k_in[l], W.w_ih[l], W.k_in[l], w.Gx, 1024, W.b_g[l], M, 1024, W.k_in[l], 0, stream);
     if (rc) return rc;
-    if (tc && rec_impl == 1) {   // tensor-core recurrence (seg_lstm_wg.cu)
-      if ((rc = lstm_rec_wg(w.Gx, W.w_hh_hi[l], W.w_hh_lo[l], outs_h[l & 1], outs_l[l & 1], NB, T, stream))) return rc;
+    if (tc && rec_impl != 0) {   // tensor-core recurrence (seg_lstm_wg.cu)
+      if ((rc = lstm_rec_wg(w.Gx, W.w_hh_hi[l], W.w_hh_lo[l], outs_h[l & 1], outs_l[l & 1], NB, T, rec_impl, stream)))
+        return rc;
       in_h = outs_h[l & 1]; in_l = outs_l[l & 1];
       continue;
     }
