@@ -54,7 +54,7 @@ int b200_ctx_destroy(b200_ctx* ctx);
  *   from 2 up to that default): the smallest linkage problem that runs on the whole-GPU path (b200_linkage_centroid).
  *   Unknown keys and values out of range return B200_ERR_INVALID. */
 int b200_ctx_set_option(b200_ctx* ctx, const char* key, int64_t value);
-/* number of kernels this ctx has launched so far (bench.py's gpu_launches claim) */
+/* number of kernels this ctx has launched so far; memcpy and memset operations are not counted */
 int64_t b200_ctx_launch_count(const b200_ctx* ctx);
 /* with option "profile" = 1 the library brackets the ResNet trunk ("trunk": conv kernels) and the segmentation
  * network ("seg") with CUDA events on the caller's stream; this returns and resets the accumulated device time

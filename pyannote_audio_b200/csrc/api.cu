@@ -85,10 +85,20 @@ struct b200_ctx {
 
 namespace {
 
-struct DeviceGuard {
-  int prev = 0;
-  explicit DeviceGuard(int dev) { cudaGetDevice(&prev); cudaSetDevice(dev); }
-  ~DeviceGuard() { cudaSetDevice(prev); }
+// Scope of an entry point: selects the ctx's device and binds its launch counter, which b200::launch increments, and
+// restores both on exit, so that one entry point may call another.
+struct CtxScope {
+  int prev_device = 0;
+  int64_t* prev_counter = g_launch_counter;
+  explicit CtxScope(b200_ctx* ctx) {
+    cudaGetDevice(&prev_device);
+    cudaSetDevice(ctx->device);
+    g_launch_counter = &ctx->launches;
+  }
+  ~CtxScope() {
+    cudaSetDevice(prev_device);
+    g_launch_counter = prev_counter;
+  }
 };
 
 template <typename T>
@@ -469,7 +479,7 @@ int b200_ctx_create(b200_ctx** out, int device) {
 
 int b200_ctx_destroy(b200_ctx* ctx) {
   if (!ctx) return B200_OK;
-  DeviceGuard g(ctx->device);
+  CtxScope scope(ctx);
   cudaDeviceSynchronize();
   for (void* p : ctx->owned_seg) cudaFree(p);
   for (void* p : ctx->owned_emb) cudaFree(p);
@@ -514,7 +524,7 @@ int64_t b200_ctx_launch_count(const b200_ctx* ctx) { return ctx ? ctx->launches 
 
 int b200_ctx_timer(b200_ctx* ctx, const char* name, double* total_ms, int64_t* units) {
   B200_CHECK(ctx && name && total_ms && units, B200_ERR_INVALID, "bad arguments");
-  DeviceGuard g(ctx->device);
+  CtxScope scope(ctx);
   std::string k(name);
   std::vector<std::pair<cudaEvent_t, cudaEvent_t>>* v = nullptr;
   int64_t* u = nullptr;
@@ -558,7 +568,7 @@ int b200_audio_ingest(b200_ctx* ctx, const void* pcm, int32_t format, int32_t ch
   B200_CHECK(frames_out <= out_capacity, B200_ERR_INVALID, "output holds %lld samples, %lld needed",
              (long long)out_capacity, (long long)frames_out);
   if (frames_out == 0) return B200_OK;
-  DeviceGuard g(ctx->device);
+  CtxScope scope(ctx);
   const int64_t gg = gcd64(sr_in, sr_out);
   const int orig = (int)(sr_in / gg), nw = (int)(sr_out / gg);
   const b200_ctx::ResampleTable* tab = nullptr;
@@ -574,7 +584,6 @@ int b200_audio_ingest(b200_ctx* ctx, const void* pcm, int32_t format, int32_t ch
     ctx->resample_tables.push_back(t);
     tab = &ctx->resample_tables.back();
   }
-  ctx->launches += 1;
   return audio_ingest(pcm, format, channels, frames_in, channel, tab->dev, tab->orig, tab->nw, tab->width, out,
                       frames_out, (cudaStream_t)stream);
 }
@@ -586,7 +595,7 @@ int b200_seg_load_head(b200_ctx* ctx, const b200_seg_weights* w, int32_t num_cla
              "a classifier of %d classes is unsupported (1 .. %d)", (int)num_classes, kSegMaxClasses);
   B200_CHECK(activation == B200_SEG_LOGSOFTMAX || activation == B200_SEG_SIGMOID, B200_ERR_INVALID,
              "unknown classifier activation %d (B200_SEG_LOGSOFTMAX = 0, B200_SEG_SIGMOID = 1)", (int)activation);
-  DeviceGuard g(ctx->device);
+  CtxScope scope(ctx);
   SegWeights& S = ctx->seg;
   B200_CHECK(w->lstm_layers >= 1 && w->lstm_layers <= 4, B200_ERR_INVALID, "lstm_layers=%d unsupported",
              (int)w->lstm_layers);
@@ -610,7 +619,7 @@ int b200_seg_load(b200_ctx* ctx, const b200_seg_weights* w) {
 
 int b200_emb_load(b200_ctx* ctx, const b200_emb_weights* w) {
   B200_CHECK(ctx && w, B200_ERR_INVALID, "NULL ctx/weights");
-  DeviceGuard g(ctx->device);
+  CtxScope scope(ctx);
   EmbWeights& E = ctx->emb;
   int rc;
   E.loaded = false;
@@ -661,7 +670,7 @@ int b200_emb_load_bottleneck(b200_ctx* ctx, const b200_emb_bottleneck_weights* w
       }
   }
   B200_CHECK(w->seg1_weight && w->seg1_bias, B200_ERR_INVALID, "seg_1 missing");
-  DeviceGuard g(ctx->device);
+  CtxScope scope(ctx);
   EmbWeights& E = ctx->emb;
   int rc;
   E.loaded = false;
@@ -706,7 +715,7 @@ static int seg_run(b200_ctx* ctx, const float* wav, const int64_t* chunk_off, co
              "160000): set the option seg_max_batch to at least %lld, or segment shorter excerpts",
              window, (long long)budget, ctx->seg_max_batch, (long long)((window + kChunk - 1) / kChunk));
   if (n == 0) return B200_OK;
-  DeviceGuard g(ctx->device);
+  CtxScope scope(ctx);
   const SegGeom geom = seg_geom(window);
   const int T = geom.pool2;
   const int nbmax = (int)std::min<int64_t>(std::min<int64_t>(n, budget / window), 65535);
@@ -726,7 +735,6 @@ static int seg_run(b200_ctx* ctx, const float* wav, const int64_t* chunk_off, co
     if ((rc = sincnet_forward(ctx->seg.sinc, geom, wav, ctx->d_off + c0, ctx->d_valid + c0, nb, region, x0_dst,
                               ctx->seg_conv_impl, st)))
       return rc;
-    ctx->launches += sincnet_launches(geom);
     if (sinc_out) continue;
     const size_t row0 = (size_t)c0 * T, K = ctx->seg.num_classes;
     SegHeadOut sub;
@@ -737,7 +745,6 @@ static int seg_run(b200_ctx* ctx, const float* wav, const int64_t* chunk_off, co
     if ((rc = lstm_head_forward(ctx->seg, x0, nb, T, region, sub, ctx->num_sms, ctx->seg_gemm_impl, ctx->seg_rec_impl,
                                 st)))
       return rc;
-    ctx->launches += 2 * ctx->seg.lstm_layers + 3;
   }
   return B200_OK;
 }
@@ -798,7 +805,7 @@ int b200_ssl_load(b200_ctx* ctx, const b200_ssl_weights* w, int32_t num_classes,
   for (int i = 0; i < 2 * kSslRelSpan + 1; ++i)
     B200_CHECK(w->rel_bucket[i] >= 0 && w->rel_bucket[i] < 320, B200_ERR_INVALID, "relative bucket %d out of range",
                (int)w->rel_bucket[i]);
-  DeviceGuard g(ctx->device);
+  CtxScope scope(ctx);
   SslWeights& X = ctx->ssl;
   X.loaded = false;
   release_weights(ctx, &ctx->owned_ssl);
@@ -894,7 +901,7 @@ static int ssl_run(b200_ctx* ctx, const float* wav, const int64_t* chunk_off, co
              "160000): set the option ssl_max_batch to at least %lld, or segment shorter excerpts",
              window, (long long)budget, ctx->ssl_max_batch, (long long)((window + kChunk - 1) / kChunk));
   if (n == 0) return B200_OK;
-  DeviceGuard g(ctx->device);
+  CtxScope scope(ctx);
   const SslGeom geom = ssl_geom(window);
   const int T = geom.T;
   const int nbmax = (int)std::min<int64_t>(std::min<int64_t>(n, budget / window), 65535);
@@ -919,9 +926,6 @@ static int ssl_run(b200_ctx* ctx, const float* wav, const int64_t* chunk_off, co
     if ((rc = lstm_head_forward(X.head, x0, nb, T, region, sub, ctx->num_sms, ctx->seg_gemm_impl, ctx->seg_rec_impl,
                                 st)))
       return rc;
-    // conv 0 + GroupNorm (3), convs 1-6, LayerNorm, projection, positional conv (pack, 16 GEMMs, add), LayerNorm,
-    // 7 per layer
-    ctx->launches += 30 + 7 * X.num_layers + 2 * X.head.lstm_layers + 3;
   }
   return B200_OK;
 }
@@ -960,15 +964,14 @@ int b200_sincnet_forward(b200_ctx* ctx, const float* wav, const int64_t* chunk_o
                          int32_t num_chunks, float* out, void* stream) {
   B200_CHECK(out != nullptr, B200_ERR_INVALID, "out is NULL");
   if (num_chunks == 0) return B200_OK;
-  DeviceGuard g(ctx->device);
+  CtxScope scope(ctx);
   cudaStream_t st = (cudaStream_t)stream;
   float* tmp = nullptr;
   const size_t rows = (size_t)num_chunks * kFrames;
   B200_CUDA_OK(cudaMalloc((void**)&tmp, rows * 64 * sizeof(float)));
   int rc = seg_run(ctx, wav, chunk_off, chunk_valid, num_chunks, kChunk, SegHeadOut(), tmp, st);
   if (rc == B200_OK) {
-    strip_pad_kernel<<<(unsigned)((rows * 60 + 255) / 256), 256, 0, st>>>(tmp, out, rows);
-    ctx->launches += 1;
+    rc = launch(strip_pad_kernel, (unsigned)((rows * 60 + 255) / 256), 256, 0, st, tmp, out, rows);
     cudaStreamSynchronize(st);
   }
   cudaFree(tmp);
@@ -992,8 +995,7 @@ int b200_powerset_to_multilabel_generic(b200_ctx* ctx, const uint8_t* classes, i
   int rc;
   if ((rc = powerset_map_for(num_classes, num_speakers, max_per_frame, &map))) return rc;
   if (n == 0) return B200_OK;
-  DeviceGuard g(ctx->device);
-  ctx->launches += 1;
+  CtxScope scope(ctx);
   return powerset_to_multilabel(classes, n, map, multilabel, (cudaStream_t)stream);
 }
 
@@ -1049,7 +1051,6 @@ static int block_run(b200_ctx* ctx, const BlockWeights& B, __half*& A, __half*& 
   if (block_fused(B, ctx->conv_impl)) {
     if ((rc = block_forward(B, A, Bf, nb, H, Wd, ctx->num_sms, st))) return rc;
     std::swap(A, Bf);
-    ctx->launches += 1;
     return B200_OK;
   }
   if ((rc = conv_forward(B.conv1, A, nullptr, Bf, nb, H, Wd, 1, ctx->conv_impl, ctx->num_sms, st))) return rc;
@@ -1057,10 +1058,8 @@ static int block_run(b200_ctx* ctx, const BlockWeights& B, __half*& A, __half*& 
   if (B.has_shortcut) {
     if ((rc = conv_forward(B.shortcut, A, nullptr, Cf, nb, H, Wd, 0, ctx->conv_impl, ctx->num_sms, st))) return rc;
     res = Cf;
-    ctx->launches += 1;
   }
   if ((rc = conv_forward(B.conv2, Bf, res, A, nb, Ho, Wo, 1, ctx->conv_impl, ctx->num_sms, st))) return rc;
-  ctx->launches += 2;
   return B200_OK;
 }
 
@@ -1078,10 +1077,8 @@ static int bottleneck_run(b200_ctx* ctx, const BottleneckWeights& B, __half* A, 
   if (B.has_shortcut) {
     if ((rc = conv_forward(B.shortcut, A, nullptr, D, nb, H, Wd, 0, impl, sms, st))) return rc;
     res = D;
-    ctx->launches += 1;
   }
   if ((rc = conv_forward(B.conv3, Cf, res, A, nb, Ho, Wo, 1, impl, sms, st))) return rc;
-  ctx->launches += 3;
   return B200_OK;
 }
 
@@ -1096,7 +1093,6 @@ static int trunk_run(b200_ctx* ctx, const EmbWs& w, const int* frame0, int nb, i
   __half* s1 = w.Bf;
   __half* s2 = w.Cf;
   if ((rc = conv1_forward(w.fbank, w.fmean, frame0, E.conv1_w, E.conv1_b, cur, nb, T0, st))) return rc;
-  ctx->launches += 1;
   for (const BlockWeights& B : E.blocks) {
     const int s = B.conv1.stride;
     if ((rc = block_run(ctx, B, cur, s1, s2, nb, H, Wd, st))) return rc;
@@ -1118,10 +1114,8 @@ static int trunk_run(b200_ctx* ctx, const EmbWs& w, const int* frame0, int nb, i
 static int emb_linear(b200_ctx* ctx, const __half* st_hi, const __half* st_lo, int64_t rows, float* emb, cudaStream_t st,
                       float* const* peers = nullptr, int n_peers = 0) {
   const int K = 20 * ctx->emb.C;
-  const int rc = gemm_tc_split(st_hi, st_lo, K, ctx->emb.seg1_w_hi, ctx->emb.seg1_w_lo, K, emb, kEmbDim, nullptr,
-                               nullptr, 0, ctx->emb.seg1_b, (int)rows, kEmbDim, K, 0, ctx->num_sms, st, peers, n_peers);
-  ctx->launches += 1;
-  return rc;
+  return gemm_tc_split(st_hi, st_lo, K, ctx->emb.seg1_w_hi, ctx->emb.seg1_w_lo, K, emb, kEmbDim, nullptr, nullptr, 0,
+                       ctx->emb.seg1_b, (int)rows, kEmbDim, K, 0, ctx->num_sms, st, peers, n_peers);
 }
 
 // WeSpeaker embeddings of n segments of `samples` samples: segment i is wav[off[i]] onwards, of which valid[i] samples
@@ -1132,7 +1126,7 @@ static int emb_linear(b200_ctx* ctx, const __half* st_hi, const __half* st_lo, i
 static int emb_run(b200_ctx* ctx, const float* wav, const int64_t* off, const int32_t* valid, int n, int samples,
                    bool share, const uint8_t* masks, const float* weights, int S, int Tw, float* emb,
                    float* const* peers, int n_peers, cudaStream_t st) {
-  DeviceGuard g(ctx->device);
+  CtxScope scope(ctx);
   const EmbWeights& E = ctx->emb;
   const int T0 = (int)fbank_frames(samples), T = trunk_width(T0);
   const int nbmax = (int)std::min<int64_t>(n, std::max<int64_t>(1, (int64_t)ctx->emb_max_batch * kFbankFrames / T0));
@@ -1156,7 +1150,6 @@ static int emb_run(b200_ctx* ctx, const float* wav, const int64_t* off, const in
     if ((rc = fbank_forward(E, wav, ctx->d_runs + plan.run_base[sb], plan.run_base[sb + 1] - plan.run_base[sb],
                             plan.nrows[sb], frame0, nb, T0, w.fbank, w.fmean, st)))
       return rc;
-    ctx->launches += 2;
     const __half* feat = nullptr;
     {
       ScopedTimer timer(ctx, &ctx->trunk_events, st);
@@ -1170,7 +1163,6 @@ static int emb_run(b200_ctx* ctx, const float* wav, const int64_t* off, const in
                : weighted_pool_forward(feat, nullptr, weights ? weights + wo : nullptr, nb, T, S, Tw, E.C, w.part,
                                        st_hi + o, st_lo + o, st);
     if (rc) return rc;
-    ctx->launches += T <= kPoolSlice ? 1 : 3;
   }
   return emb_linear(ctx, st_hi, st_lo, (int64_t)rows, emb, st, peers, n_peers);
 }
@@ -1194,8 +1186,7 @@ int b200_emb_forward_push(b200_ctx* ctx, const float* wav, const int64_t* chunk_
 int b200_push(b200_ctx* ctx, const void* src, int64_t bytes, void* const* dsts, int32_t n_dsts, void* stream) {
   B200_CHECK(ctx && src && (n_dsts == 0 || dsts) && bytes >= 0 && n_dsts >= 0, B200_ERR_INVALID, "bad arguments");
   if (bytes == 0 || n_dsts == 0) return B200_OK;
-  DeviceGuard g(ctx->device);
-  ctx->launches += 1;
+  CtxScope scope(ctx);
   return push_bytes(src, bytes, dsts, n_dsts, (cudaStream_t)stream);
 }
 
@@ -1204,7 +1195,7 @@ int b200_emb_fbank(b200_ctx* ctx, const float* wav, const int64_t* chunk_off, co
   B200_CHECK(ctx && ctx->emb.loaded, B200_ERR_STATE, "embedding weights not loaded");
   B200_CHECK(wav && chunk_off && chunk_valid && fbank && num_chunks >= 0, B200_ERR_INVALID, "bad arguments");
   if (num_chunks == 0) return B200_OK;
-  DeviceGuard g(ctx->device);
+  CtxScope scope(ctx);
   cudaStream_t st = (cudaStream_t)stream;
   int rc = ensure_ws(ctx, (size_t)num_chunks * kMel * sizeof(float) + 4096);
   if (rc) return rc;
@@ -1217,7 +1208,6 @@ int b200_emb_fbank(b200_ctx* ctx, const float* wav, const int64_t* chunk_off, co
   if ((rc = fbank_forward(ctx->emb, wav, ctx->d_runs, num_chunks, plan.nrows[0], ctx->d_frame0, num_chunks, kFbankFrames,
                           fbank, fmean, st)))
     return rc;
-  ctx->launches += 3;
   return fbank_center(fbank, fmean, num_chunks, st);
 }
 
@@ -1239,7 +1229,7 @@ int b200_emb_trunk(b200_ctx* ctx, const float* fbank, int32_t num_chunks, float*
   B200_CHECK(ctx && ctx->emb.loaded, B200_ERR_STATE, "embedding weights not loaded");
   B200_CHECK(fbank && frames && num_chunks >= 0, B200_ERR_INVALID, "bad arguments");
   if (num_chunks == 0) return B200_OK;
-  DeviceGuard g(ctx->device);
+  CtxScope scope(ctx);
   cudaStream_t st = (cudaStream_t)stream;
   const int nbmax = num_chunks < ctx->emb_max_batch ? num_chunks : ctx->emb_max_batch;
   int rc = ensure_ws(ctx, carve_emb(ctx->emb, nbmax, kFbankFrames, 1, nullptr, nullptr) + 4096);
@@ -1256,7 +1246,6 @@ int b200_emb_trunk(b200_ctx* ctx, const float* fbank, int32_t num_chunks, float*
     int T = 0;
     if ((rc = trunk_run(ctx, w, nullptr, nb, kFbankFrames, st, &feat, &T))) return rc;
     if ((rc = frames_to_nchw(feat, frames + (size_t)c0 * C * 10 * kEmbT, nb, T, C, st))) return rc;
-    ctx->launches += 1;
   }
   return B200_OK;
 }
@@ -1293,7 +1282,7 @@ int b200_emb_forward_embedding(b200_ctx* ctx, const float* frames, int32_t B, in
   B200_CHECK(!weights || (num_speakers >= 1 && num_weights >= 1), B200_ERR_INVALID,
              "weights need num_speakers >= 1 and num_weights >= 1 (got %d, %d)", (int)num_speakers, (int)num_weights);
   if (B == 0) return B200_OK;
-  DeviceGuard g(ctx->device);
+  CtxScope scope(ctx);
   cudaStream_t st = (cudaStream_t)stream;
   const int S = weights ? num_speakers : 1;
   const int C = ctx->emb.C;
@@ -1307,7 +1296,6 @@ int b200_emb_forward_embedding(b200_ctx* ctx, const float* frames, int32_t B, in
   __half* st_lo = reinterpret_cast<__half*>(base + split_bytes);
   double* part = part_bytes ? reinterpret_cast<double*>(base + 2 * split_bytes) : nullptr;
   if ((rc = weighted_pool_forward(nullptr, frames, weights, B, T, S, num_weights, C, part, st_hi, st_lo, st))) return rc;
-  ctx->launches += T <= kPoolSlice ? 1 : 3;
   return emb_linear(ctx, st_hi, st_lo, (int64_t)rows, emb, st);
 }
 
@@ -1315,8 +1303,7 @@ int b200_stats_pool(b200_ctx* ctx, const float* seq, const float* weights, float
                     int32_t S, int32_t Tw, void* stream) {
   B200_CHECK(ctx && seq && out && B >= 0 && F > 0 && T > 0 && S > 0, B200_ERR_INVALID, "bad arguments");
   if (B == 0) return B200_OK;
-  DeviceGuard g(ctx->device);
-  ctx->launches += 1;
+  CtxScope scope(ctx);
   return stats_pool_generic(seq, weights, out, B, F, T, S, weights ? Tw : T, (cudaStream_t)stream);
 }
 
@@ -1329,7 +1316,7 @@ int b200_xvec_load(b200_ctx* ctx, const b200_xvec_weights* w) {
     B200_CHECK(w->tdnn_weight[l] && w->tdnn_bias[l] && w->bn_weight[l] && w->bn_bias[l] && w->bn_mean[l] && w->bn_var[l],
                B200_ERR_INVALID, "tdnns.%d / tdnns.%d missing", 3 * l, 3 * l + 2);
   B200_CHECK(w->embedding_weight && w->embedding_bias, B200_ERR_INVALID, "embedding missing");
-  DeviceGuard g(ctx->device);
+  CtxScope scope(ctx);
   XvecWeights& X = ctx->xvec;
   X.loaded = false;
   release_weights(ctx, &ctx->owned_xvec);
@@ -1416,7 +1403,7 @@ int b200_xvec_forward(b200_ctx* ctx, const float* wav, const int64_t* off, int64
   if (num_utts == 0) return B200_OK;
   for (int i = 0; i < num_utts; ++i)
     B200_CHECK(off[i] >= 0, B200_ERR_INVALID, "utterance %d: negative offset %lld", i, (long long)off[i]);
-  DeviceGuard g(ctx->device);
+  CtxScope scope(ctx);
   cudaStream_t st = (cudaStream_t)stream;
   const XvecWeights& X = ctx->xvec;
   const SegGeom geom = seg_geom((int)num_samples);
@@ -1440,7 +1427,6 @@ int b200_xvec_forward(b200_ctx* ctx, const float* wav, const int64_t* off, int64
   __half* st_lo = reinterpret_cast<__half*>(tail + split_bytes);
   float* out = out_bytes ? reinterpret_cast<float*>(tail + 2 * split_bytes) : emb;
   B200_CUDA_OK(cudaMemsetAsync(st_hi, 0, 2 * split_bytes, st));   // the 8 padding columns of every statistics row
-  ctx->launches += 1;
   for (int u0 = 0; u0 < num_utts; u0 += nbmax) {
     const int nb = std::min(nbmax, num_utts - u0);
     const int M = nb * F;
@@ -1448,9 +1434,7 @@ int b200_xvec_forward(b200_ctx* ctx, const float* wav, const int64_t* off, int64
     const int sinc_impl = ctx->seg_conv_impl == 2 ? 2 : 1;
     if ((rc = sincnet_forward(X.sinc, geom, wav, ctx->d_off + u0, ctx->d_valid + u0, nb, w.sinc, w.x0, sinc_impl, st)))
       return rc;
-    ctx->launches += sincnet_launches(geom);
     if ((rc = split_f16(w.x0, w.xh, w.xl, (size_t)M * 64, st))) return rc;
-    ctx->launches += 1;
     // Every window keeps the row stride F through the stack: output row b * F + t of layer l reads input rows
     // b * F + t + j * dil.  Rows t >= F - 4, F - 8, F - 14 (layers 1, 2, 3-5) compute values nothing uses, since a
     // valid row of layer l + 1 reads only valid rows of layer l and the pooling reads the first T = F - 14 rows of
@@ -1471,17 +1455,14 @@ int b200_xvec_forward(b200_ctx* ctx, const float* wav, const int64_t* off, int64
                          last ? nullptr : out_h[l], last ? nullptr : out_l[l], N, X.bias[l], M, N, K, 1,
                          ctx->num_sms, st, nullptr, 0, tp);
       if (rc) return rc;
-      ctx->launches += 1;
     }
     const size_t o = (size_t)u0 * S * kXvecStatsLd;
     if ((rc = weighted_pool_rows(w.y, F, T, 1500, weights ? weights + (size_t)u0 * S * num_weights : nullptr, nb, S,
                                  num_weights, w.part, st_hi + o, st_lo + o, kXvecStatsLd, st)))
       return rc;
-    ctx->launches += T <= kPoolSlice ? 1 : 3;
   }
   rc = gemm_tc_split(st_hi, st_lo, kXvecStatsLd, X.emb_hi, X.emb_lo, kXvecStatsLd, out, X.dim_pad, nullptr, nullptr, 0,
                      X.emb_b, (int)rows, X.dim_pad, kXvecStatsLd, 0, ctx->num_sms, st);
-  ctx->launches += 1;
   if (rc) return rc;
   if (out != emb)
     B200_CUDA_OK(cudaMemcpy2DAsync(emb, (size_t)X.dim * sizeof(float), out, (size_t)X.dim_pad * sizeof(float),
@@ -1493,8 +1474,7 @@ int b200_xvec_forward(b200_ctx* ctx, const float* wav, const int64_t* off, int64
 int b200_speaker_count(b200_ctx* ctx, const uint8_t* seg, const int32_t* start_frame, int32_t num_chunks,
                        int32_t num_frames, uint8_t* count, void* stream) {
   B200_CHECK(ctx && seg && start_frame && count && num_chunks > 0 && num_frames > 0, B200_ERR_INVALID, "bad arguments");
-  DeviceGuard g(ctx->device);
-  ctx->launches += 1;
+  CtxScope scope(ctx);
   return speaker_count(seg, start_frame, num_chunks, num_frames, count, (cudaStream_t)stream);
 }
 
@@ -1503,8 +1483,7 @@ int b200_reconstruct(b200_ctx* ctx, const uint8_t* seg, const int8_t* hard_clust
                      uint8_t* discrete, void* stream) {
   B200_CHECK(ctx && seg && hard_clusters && start_frame && count && discrete && num_chunks > 0 && num_frames > 0,
              B200_ERR_INVALID, "bad arguments");
-  DeviceGuard g(ctx->device);
-  ctx->launches += 1;
+  CtxScope scope(ctx);
   return reconstruct(seg, (const signed char*)hard_clusters, start_frame, num_chunks, num_frames, num_clusters_out,
                      count, discrete, (cudaStream_t)stream);
 }
@@ -1516,8 +1495,7 @@ int b200_aggregate_window(b200_ctx* ctx, const float* scores, const int32_t* sta
   B200_CHECK(ctx && scores && start_frame && out && num_chunks > 0 && num_frames > 0 && frames_per_chunk > 0 &&
                  num_classes > 0,
              B200_ERR_INVALID, "bad arguments");
-  DeviceGuard g(ctx->device);
-  ctx->launches += 1;
+  CtxScope scope(ctx);
   return aggregate_scores(scores, start_frame, num_chunks, num_frames, frames_per_chunk, num_classes, hamming, warm_up,
                           skip_average, missing, epsilon, out, (cudaStream_t)stream);
 }
@@ -1536,8 +1514,7 @@ int b200_powerset_speech_generic(b200_ctx* ctx, const uint8_t* classes, int64_t 
   int rc;
   if ((rc = powerset_map_for(num_classes, num_speakers, max_per_frame, &map))) return rc;
   if (n == 0) return B200_OK;
-  DeviceGuard g(ctx->device);
-  ctx->launches += 1;
+  CtxScope scope(ctx);
   return powerset_speech(classes, n, map, speech, (cudaStream_t)stream);
 }
 
@@ -1549,8 +1526,7 @@ int b200_frame_transitions(b200_ctx* ctx, const uint8_t* discrete, int32_t num_f
                            int32_t cap, int32_t* buf, void* stream) {
   B200_CHECK(ctx && discrete && buf && num_frames > 0 && num_clusters > 0 && cap > 0, B200_ERR_INVALID,
              "bad arguments");
-  DeviceGuard g(ctx->device);
-  ctx->launches += 1;
+  CtxScope scope(ctx);
   return frame_transitions(discrete, num_frames, num_clusters, cap, buf, (cudaStream_t)stream);
 }
 
@@ -1558,8 +1534,7 @@ int b200_clean_frames(b200_ctx* ctx, const uint8_t* seg, int32_t num_chunks, int
                       void* stream) {
   B200_CHECK(ctx && seg && clean && active && num_chunks >= 0, B200_ERR_INVALID, "bad arguments");
   if (num_chunks == 0) return B200_OK;
-  DeviceGuard g(ctx->device);
-  ctx->launches += 1;
+  CtxScope scope(ctx);
   return clean_frames(seg, num_chunks, clean, active, (cudaStream_t)stream);
 }
 
@@ -1585,12 +1560,9 @@ int b200_linkage_centroid_batched(b200_ctx* ctx, const double* x, const int32_t*
   B200_CHECK(ctx && x && row_offsets && Z && num_problems >= 1 && dim >= 1, B200_ERR_INVALID, "bad arguments");
   int rc = check_linkage_offsets(row_offsets, num_problems);
   if (rc) return rc;
-  DeviceGuard g(ctx->device);
+  CtxScope scope(ctx);
   rc = ensure_ws(ctx, linkage_workspace_bytes_batched(row_offsets, num_problems, dim, ctx->linkage_grid_min));
   if (rc) return rc;
-  int big = 0;
-  for (int f = 0; f < num_problems; ++f) big += row_offsets[f + 1] - row_offsets[f] >= ctx->linkage_grid_min;
-  ctx->launches += 2 + num_problems + big;
   return linkage_centroid_batched(x, row_offsets, num_problems, dim, normalize, Z, ctx->ws, (cudaStream_t)stream,
                                   ctx->linkage_grid_min);
 }
@@ -1613,8 +1585,7 @@ int b200_plda_transform(b200_ctx* ctx, const double* x, int32_t n, int32_t Din, 
   B200_CHECK(ctx && x && mean1 && mean2 && lda && mu && trT && fea && n >= 0 && Din >= 1 && Dout >= 1 && L >= 1 &&
                  L <= Dout && Din + Dout <= 4096, B200_ERR_INVALID, "bad arguments");
   if (n == 0) return B200_OK;
-  DeviceGuard g(ctx->device);
-  ctx->launches += 1;
+  CtxScope scope(ctx);
   return plda_transform(x, n, Din, Dout, L, mean1, mean2, lda, mu, trT, fea, (cudaStream_t)stream);
 }
 
@@ -1623,8 +1594,7 @@ int b200_weighted_centroids(b200_ctx* ctx, const double* q, int32_t n, int32_t S
   B200_CHECK(ctx && q && train && n >= 1 && S >= 1 && K >= 0 && dim >= 1, B200_ERR_INVALID, "bad arguments");
   if (K == 0) return B200_OK;        // no speaker kept: empty `kept` and `centroids` (null data pointers)
   B200_CHECK(kept && centroids, B200_ERR_INVALID, "bad arguments");
-  DeviceGuard g(ctx->device);
-  ctx->launches += 1;
+  CtxScope scope(ctx);
   return weighted_centroids(q, n, S, kept, K, train, dim, centroids, (cudaStream_t)stream);
 }
 
@@ -1632,8 +1602,7 @@ int b200_cdist_cosine(b200_ctx* ctx, const double* a, int32_t m, const double* b
                       void* stream) {
   B200_CHECK(ctx && a && b && d && m >= 0 && k >= 1 && dim >= 1, B200_ERR_INVALID, "bad arguments");
   if (m == 0) return B200_OK;
-  DeviceGuard g(ctx->device);
-  ctx->launches += 1;
+  CtxScope scope(ctx);
   return cdist_cosine(a, m, b, k, dim, d, (cudaStream_t)stream);
 }
 
@@ -1643,10 +1612,9 @@ int b200_vbx_batched(b200_ctx* ctx, const double* fea, const double* phi, const 
   B200_CHECK(ctx && fea && phi && n && S && gamma && pi && num_problems >= 1 && D >= 1 && max_iters >= 1,
              B200_ERR_INVALID, "bad arguments");
   for (int f = 0; f < num_problems; ++f) B200_CHECK(n[f] >= 0 && S[f] >= 0, B200_ERR_INVALID, "negative problem size");
-  DeviceGuard g(ctx->device);
+  CtxScope scope(ctx);
   int rc = ensure_ws(ctx, vbx_workspace_bytes_batched(n, S, num_problems, D));
   if (rc) return rc;
-  ctx->launches += 1;
   return vbx_run_batched(fea, phi, n, S, num_problems, D, Fa, Fb, max_iters, epsilon, gamma, pi, iters, ctx->ws,
                          (cudaStream_t)stream);
 }
@@ -1663,8 +1631,7 @@ int b200_assign(b200_ctx* ctx, const double* soft, int32_t num_chunks, int32_t n
   B200_CHECK(num_clusters <= 127, B200_ERR_INVALID, "assign: %d clusters, at most 127 fit the int8 cluster ids",
              (int)num_clusters);
   if (num_chunks == 0) return B200_OK;
-  DeviceGuard g(ctx->device);
-  ctx->launches += 1;
+  CtxScope scope(ctx);
   return assign_clusters(soft, num_chunks, num_clusters, constrained, (signed char*)hard, (cudaStream_t)stream);
 }
 

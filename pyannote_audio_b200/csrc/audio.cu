@@ -105,14 +105,8 @@ int audio_ingest(const void* src, int format, int channels, long long frames_in,
   const long long grid = (total_periods + periods - 1) / periods;
   if (grid == 0) return B200_OK;
   B200_CHECK(grid < (1ll << 31), B200_ERR_INVALID, "audio too long for one launch");
-  if (format == 0)
-    ingest_kernel<0><<<(unsigned)grid, kIngestThreads, 0, stream>>>(src, channels, frames_in, channel, table, orig, nw,
-                                                                    width, klen, periods, out, frames_out);
-  else
-    ingest_kernel<1><<<(unsigned)grid, kIngestThreads, 0, stream>>>(src, channels, frames_in, channel, table, orig, nw,
-                                                                    width, klen, periods, out, frames_out);
-  B200_CUDA_OK(cudaGetLastError());
-  return B200_OK;
+  return launch(format == 0 ? ingest_kernel<0> : ingest_kernel<1>, (unsigned)grid, kIngestThreads, 0, stream, src,
+                channels, frames_in, channel, table, orig, nw, width, klen, periods, out, frames_out);
 }
 
 }  // namespace b200

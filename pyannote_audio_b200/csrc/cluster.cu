@@ -812,22 +812,25 @@ int linkage_centroid_batched(const double* x, const int* row_offsets, int nfiles
   LinkJob* djobs = (LinkJob*)p;
   B200_CUDA_OK(cudaMemcpyAsync(djobs, jobs.data(), sizeof(LinkJob) * nfiles, cudaMemcpyHostToDevice, st));
   const double* src = x;
+  int rc;
   if (normalize && ntot > 0) {
-    if (normalize == 2) normalize_rows_np_f32_kernel<<<ceil_div(ntot, 64), 64, 0, st>>>(x, xn, ntot, dim);
-    else normalize_rows_kernel<<<ntot, 128, 0, st>>>(x, xn, ntot, dim);
+    if ((rc = normalize == 2 ? launch(normalize_rows_np_f32_kernel, ceil_div(ntot, 64), 64, 0, st, x, xn, ntot, dim)
+                             : launch(normalize_rows_kernel, ntot, 128, 0, st, x, xn, ntot, dim)))
+      return rc;
     src = xn;
   }
   for (int f = 0; f < nfiles; ++f) {
     const int n = jobs[f].n;
     if (n < 2) continue;
     dim3 grid(ceil_div(n, 16), ceil_div(n, 16));
-    pdist_kernel<false><<<grid, dim3(16, 16), 0, st>>>(src + (size_t)jobs[f].row_off * dim, D + jobs[f].d_off, n, dim);
+    if ((rc = launch(pdist_kernel<false>, grid, dim3(16, 16), 0, st, src + (size_t)jobs[f].row_off * dim,
+                     D + jobs[f].d_off, n, dim)))
+      return rc;
   }
   const size_t link_smem_bytes = (size_t)kLinkSmemRows * 17;
-  B200_CUDA_OK(cudaFuncSetAttribute(linkage_centroid_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize,
-                                    (int)link_smem_bytes));
-  linkage_centroid_kernel<<<nfiles, 1024, link_smem_bytes, st>>>(djobs, D, Z, nn_d, nn_i, size, id, alive, todo);
-  B200_CUDA_OK(cudaGetLastError());
+  if ((rc = launch(linkage_centroid_kernel, nfiles, 1024, link_smem_bytes, st, djobs, D, Z, nn_d, nn_i, size, id, alive,
+                   todo)))
+    return rc;
   if (big.empty()) return B200_OK;
 
   // large problems, one after another: packed distances, then a cooperative grid of one CTA per SM
@@ -840,18 +843,13 @@ int linkage_centroid_batched(const double* x, const int* row_offsets, int nfiles
   B200_CHECK(per_sm >= 1, B200_ERR_CUDA, "linkage: the whole-GPU kernel does not fit on an SM");
   const int nb = std::min(sms, kLinkGridMaxCtas);
   for (int f : big) {
-    int n = row_offsets[f + 1] - row_offsets[f];
+    const int n = row_offsets[f + 1] - row_offsets[f], ro = row_offsets[f];
     dim3 grid(ceil_div(n, 16), ceil_div(n, 16));
-    pdist_kernel<true><<<grid, dim3(16, 16), 0, st>>>(src + (size_t)row_offsets[f] * dim, P, n, dim);
-    B200_CUDA_OK(cudaGetLastError());
-    double* Zf = Z + (size_t)jobs[f].z_off * 4;
-    const int ro = row_offsets[f];
-    double* nn_d_f = nn_d + ro;
-    int *nn_i_f = nn_i + ro, *size_f = size + ro, *id_f = id + ro, *todo_f = todo + ro + f;
-    unsigned char* alive_f = alive + ro;
-    void* args[] = {&P, &n, &Zf, &nn_d_f, &nn_i_f, &size_f, &id_f, &alive_f, &todo_f, &ntodo, &part};
-    B200_CUDA_OK(cudaLaunchCooperativeKernel((const void*)linkage_centroid_grid_kernel, dim3(nb),
-                                             dim3(kLinkGridThreads), args, 0, st));
+    if ((rc = launch(pdist_kernel<true>, grid, dim3(16, 16), 0, st, src + (size_t)ro * dim, P, n, dim))) return rc;
+    if ((rc = launch<true>(linkage_centroid_grid_kernel, nb, kLinkGridThreads, 0, st, P, n,
+                           Z + (size_t)jobs[f].z_off * 4, nn_d + ro, nn_i + ro, size + ro, id + ro, alive + ro,
+                           todo + ro + f, ntodo, part)))
+      return rc;
   }
   free_p.p = nullptr;
   B200_CUDA_OK(cudaFreeAsync(P, st));
@@ -916,10 +914,8 @@ __global__ void __launch_bounds__(256) plda_transform_kernel(const double* __res
 
 int plda_transform(const double* x, int n, int Din, int Dout, int L, const double* mean1, const double* mean2,
                    const double* lda, const double* mu, const double* trT, double* fea, cudaStream_t st) {
-  plda_transform_kernel<<<n, 256, (size_t)(Din + Dout) * sizeof(double), st>>>(x, Din, Dout, L, mean1, mean2, lda, mu,
-                                                                             trT, fea);
-  B200_CUDA_OK(cudaGetLastError());
-  return B200_OK;
+  return launch(plda_transform_kernel, n, 256, (size_t)(Din + Dout) * sizeof(double), st, x, Din, Dout, L, mean1, mean2,
+                lda, mu, trT, fea);
 }
 
 // ------------------------------------------------------------------------------------------------------
@@ -944,15 +940,11 @@ __global__ void __launch_bounds__(256) weighted_centroids_kernel(const double* _
 
 int weighted_centroids(const double* q, int n, int S, const int* kept, int K, const double* train, int dim,
                        double* centroids, cudaStream_t st) {
-  weighted_centroids_kernel<<<K, 256, 0, st>>>(q, n, S, kept, train, dim, centroids);
-  B200_CUDA_OK(cudaGetLastError());
-  return B200_OK;
+  return launch(weighted_centroids_kernel, K, 256, 0, st, q, n, S, kept, train, dim, centroids);
 }
 
 int cdist_cosine(const double* a, int m, const double* b, int k, int dim, double* d, cudaStream_t st) {
-  cdist_cosine_kernel<<<ceil_div(m * k, 128), 128, 0, st>>>(a, m, b, k, dim, d);
-  B200_CUDA_OK(cudaGetLastError());
-  return B200_OK;
+  return launch(cdist_cosine_kernel, ceil_div(m * k, 128), 128, 0, st, a, m, b, k, dim, d);
 }
 
 size_t vbx_workspace_bytes_batched(const int* n, const int* S, int nfiles, int D) {
@@ -985,9 +977,9 @@ int vbx_run_batched(const double* fea, const double* phi, const int* n, const in
   VbxJob* djobs = (VbxJob*)p;
   int* iters = (int*)(djobs + nfiles);
   B200_CUDA_OK(cudaMemcpyAsync(djobs, jobs.data(), sizeof(VbxJob) * nfiles, cudaMemcpyHostToDevice, st));
-  vbx_kernel<<<nfiles * kVbxCtas, 1024, 0, st>>>(djobs, fea, phi, D, Fa, Fb, max_iters, epsilon, gamma, pi, rho, G, lpx,
-                                                 alpha, invL, cst, praw, part, iters);
-  B200_CUDA_OK(cudaGetLastError());
+  const int rc = launch(vbx_kernel, nfiles * kVbxCtas, 1024, 0, st, djobs, fea, phi, D, Fa, Fb, max_iters, epsilon,
+                        gamma, pi, rho, G, lpx, alpha, invL, cst, praw, part, iters);
+  if (rc) return rc;
   if (iters_host) {
     B200_CUDA_OK(cudaMemcpyAsync(iters_host, iters, sizeof(int) * nfiles, cudaMemcpyDeviceToHost, st));
     B200_CUDA_OK(cudaStreamSynchronize(st));
@@ -996,9 +988,7 @@ int vbx_run_batched(const double* fea, const double* phi, const int* n, const in
 }
 
 int assign_clusters(const double* soft, int C, int K, int constrained, signed char* hard, cudaStream_t st) {
-  assign_kernel<<<ceil_div(C, 128), 128, 0, st>>>(soft, C, K, constrained, hard);
-  B200_CUDA_OK(cudaGetLastError());
-  return B200_OK;
+  return launch(assign_kernel, ceil_div(C, 128), 128, 0, st, soft, C, K, constrained, hard);
 }
 
 // fcluster(Z, t, criterion="distance") -- scipy/_hierarchy.pyx cluster_dist -> cluster_monocrit

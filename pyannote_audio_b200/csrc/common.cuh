@@ -7,6 +7,7 @@
 #include <cstdarg>
 #include <cstring>
 #include <string>
+#include <utility>
 #include <vector>
 
 namespace b200 {
@@ -79,6 +80,34 @@ __device__ __forceinline__ void ffma2(f32x2_t& d, f32x2_t a, f32x2_t b) {   // d
   unpack2(a, a0, a1);
   unpack2(b, b0, b1);
   d = pack2(__fmaf_rn(a0, b0, d0), __fmaf_rn(a1, b1, d1));
+}
+#endif
+
+// Launch counter of the ctx whose entry point is running on this thread (api.cu: CtxScope binds it), null outside one.
+extern thread_local int64_t* g_launch_counter;
+
+#ifdef __CUDACC__
+// Every kernel of the library is launched here.  A kernel that takes dynamic shared memory is first opted into that
+// much, also below 48 KB, where its static shared memory may still take it past the default.  The attribute belongs to
+// one device's context, so it is set at every launch.  Then the kernel is launched, the
+// launch is checked and counted on the bound counter (b200_ctx_launch_count).  Cooperative = true makes a cooperative
+// launch, for kernels that synchronise the whole grid.
+template <bool Cooperative = false, typename... P, typename... Args>
+int launch(void (*kernel)(P...), dim3 grid, dim3 block, size_t smem, cudaStream_t st, Args&&... args) {
+  B200_CHECK(g_launch_counter, B200_ERR_STATE, "kernel launched outside an entry point's ctx scope");
+  if (smem) B200_CUDA_OK(cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+  if constexpr (Cooperative) {
+    auto run = [&](P... a) {   // the arguments converted to the kernel's parameter types, passed by address
+      void* argv[] = {&a...};
+      return cudaLaunchCooperativeKernel((const void*)kernel, grid, block, argv, smem, st);
+    };
+    B200_CUDA_OK(run(std::forward<Args>(args)...));
+  } else {
+    kernel<<<grid, block, smem, st>>>(std::forward<Args>(args)...);
+    B200_CUDA_OK(cudaGetLastError());
+  }
+  ++*g_launch_counter;
+  return B200_OK;
 }
 #endif
 

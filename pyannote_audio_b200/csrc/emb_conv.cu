@@ -920,9 +920,7 @@ int conv_forward(const ConvLayer& L, const __half* in, const __half* residual, _
 
   if (impl == 0) {
     const size_t total = (size_t)B * p.H_out * p.W_out * (L.C_out / 8);
-    conv_simt_kernel<<<(unsigned)((total + 255) / 256), 256, 0, stream>>>(in, L.w, p);
-    B200_CUDA_OK(cudaGetLastError());
-    return B200_OK;
+    return launch(conv_simt_kernel, (unsigned)((total + 255) / 256), 256, 0, stream, in, L.w, p);
   }
 
   // conv_row_kernel for the stride-1 3x3 convs with one channel chunk and C_in = C_out; impl 2 keeps every conv on
@@ -992,32 +990,24 @@ int conv_forward(const ConvLayer& L, const __half* in, const __half* residual, _
     if (residual && (rc = encode_f16_map(&tmR, 4, residual, dims, strides, box, nullptr, swz, "residual"))) return rc;
     if ((rc = encode_f16_map(&tmO, 4, out, dims, strides, box, nullptr, swz, "out"))) return rc;
     auto kernel = p.Ck == 32 ? conv_row_kernel<32, 32> : conv_row_kernel<64, 64>;
-    B200_CUDA_OK(cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-    kernel<<<(unsigned)std::min(p.num_tiles, ctas), kWgThreads, smem, stream>>>(tmA, tmB, tmR, tmO, p);
-    B200_CUDA_OK(cudaGetLastError());
-    return B200_OK;
+    return launch(kernel, (unsigned)std::min(p.num_tiles, ctas), kWgThreads, smem, stream, tmA, tmB, tmR, tmO, p);
   }
-  auto launch = [&](auto kernel) -> int {
-    B200_CUDA_OK(cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-    const dim3 grid((unsigned)(ctas ? std::min(p.num_tiles, ctas) : p.num_tiles), (unsigned)(L.C_out / n_tile));
-    kernel<<<grid, kWgThreads, smem, stream>>>(tmA, tmB, p);
-    B200_CUDA_OK(cudaGetLastError());
-    return B200_OK;
-  };
-  if (chunk_rows) return L.C_out == 256 ? launch(conv_chunk_row_kernel<256>) : launch(conv_chunk_row_kernel<128>);
+  const dim3 grid((unsigned)(ctas ? std::min(p.num_tiles, ctas) : p.num_tiles), (unsigned)(L.C_out / n_tile));
+  auto run = [&](auto kernel) { return launch(kernel, grid, kWgThreads, smem, stream, tmA, tmB, p); };
+  if (chunk_rows) return L.C_out == 256 ? run(conv_chunk_row_kernel<256>) : run(conv_chunk_row_kernel<128>);
   if (p.Ck == 32) {
     switch (L.C_out) {
-      case 32: return launch(conv_tc_kernel<32, 32>);
-      case 64: return launch(conv_tc_kernel<64, 32>);
-      default: return launch(conv_tc_kernel<128, 32>);   // bottleneck layer 1: conv3 / shortcut 32 -> 128
+      case 32: return run(conv_tc_kernel<32, 32>);
+      case 64: return run(conv_tc_kernel<64, 32>);
+      default: return run(conv_tc_kernel<128, 32>);   // bottleneck layer 1: conv3 / shortcut 32 -> 128
     }
   }
   switch (L.C_out) {
-    case 32: return launch(conv_tc_kernel<32, 64>);       // bottleneck layer 1: conv1 128 -> 32
-    case 64: return launch(conv_tc_kernel<64, 64>);
-    case 128: return launch(conv_tc_kernel<128, 64>);
-    case 256: return launch(conv_tc_kernel<256, 64>);
-    default: return launch(conv_tc_kernel<256, 64, true>);
+    case 32: return run(conv_tc_kernel<32, 64>);       // bottleneck layer 1: conv1 128 -> 32
+    case 64: return run(conv_tc_kernel<64, 64>);
+    case 128: return run(conv_tc_kernel<128, 64>);
+    case 256: return run(conv_tc_kernel<256, 64>);
+    default: return run(conv_tc_kernel<256, 64, true>);
   }
 }
 
@@ -1060,18 +1050,13 @@ int block_forward(const BlockWeights& Bw, const __half* in, __half* out, int B, 
       return rc;
   }
   const size_t smem = BlockRowPlan::kSmem;
-  B200_CUDA_OK(cudaFuncSetAttribute(block_row_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-  block_row_kernel<<<(unsigned)std::min(p.num_tiles, ctas), kWgThreads, smem, stream>>>(tmA, tmW1, tmW2, p);
-  B200_CUDA_OK(cudaGetLastError());
-  return B200_OK;
+  return launch(block_row_kernel, (unsigned)std::min(p.num_tiles, ctas), kWgThreads, smem, stream, tmA, tmW1, tmW2, p);
 }
 
 int conv1_forward(const float* fbank, const float* fmean, const int* frame0, const float* w, const float* bias,
                   __half* out, int B, int T0, cudaStream_t stream) {
   dim3 grid(B, ceil_div(T0, kC1Tile));
-  conv1_kernel<<<grid, kC1Tile, 0, stream>>>(fbank, fmean, frame0, w, bias, out, T0);
-  B200_CUDA_OK(cudaGetLastError());
-  return B200_OK;
+  return launch(conv1_kernel, grid, kC1Tile, 0, stream, fbank, fmean, frame0, w, bias, out, T0);
 }
 
 }  // namespace b200

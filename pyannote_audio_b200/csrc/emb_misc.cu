@@ -210,9 +210,7 @@ __global__ void fbank_center_kernel(float* __restrict__ fb, const float* __restr
 
 int fbank_center(float* fbank, const float* fmean, int B, cudaStream_t stream) {
   const size_t total = (size_t)B * kFbankFrames * kMel;
-  fbank_center_kernel<<<(unsigned)((total + 255) / 256), 256, 0, stream>>>(fbank, fmean, total);
-  B200_CUDA_OK(cudaGetLastError());
-  return B200_OK;
+  return launch(fbank_center_kernel, (unsigned)((total + 255) / 256), 256, 0, stream, fbank, fmean, total);
 }
 
 __global__ void frames_to_nchw_kernel(const __half* __restrict__ feat, float* __restrict__ out, int T, int C,
@@ -228,20 +226,16 @@ __global__ void frames_to_nchw_kernel(const __half* __restrict__ feat, float* __
 
 int frames_to_nchw(const __half* feat, float* out, int B, int T, int C, cudaStream_t stream) {
   const size_t total = (size_t)B * C * 10 * T;
-  frames_to_nchw_kernel<<<(unsigned)((total + 255) / 256), 256, 0, stream>>>(feat, out, T, C, total);
-  B200_CUDA_OK(cudaGetLastError());
-  return B200_OK;
+  return launch(frames_to_nchw_kernel, (unsigned)((total + 255) / 256), 256, 0, stream, feat, out, T, C, total);
 }
 
 int fbank_forward(const EmbWeights& W, const float* wav, const FbankRun* runs, int nruns, int nrows,
                   const int* frame0, int B, int T0, float* fbank, float* fmean, cudaStream_t stream) {
   const unsigned grid = (unsigned)ceil_div(nrows, 16);      // 8 warps x 2 frame rows per block
-  fbank_kernel<<<grid, 256, 0, stream>>>(wav, runs, nruns, nrows, W.window, W.twiddle, W.mel_w, W.mel_start,
-                                         W.mel_len, W.mel_off, fbank);
-  B200_CUDA_OK(cudaGetLastError());
-  fbank_mean_kernel<<<B, 640, 0, stream>>>(fbank, frame0, T0, fmean);
-  B200_CUDA_OK(cudaGetLastError());
-  return B200_OK;
+  const int rc = launch(fbank_kernel, grid, 256, 0, stream, wav, runs, nruns, nrows, W.window, W.twiddle, W.mel_w,
+                        W.mel_start, W.mel_len, W.mel_off, fbank);
+  if (rc) return rc;
+  return launch(fbank_mean_kernel, B, 640, 0, stream, fbank, frame0, T0, fmean);
 }
 
 // ------------------------------------------------------------------------------------------------
@@ -456,16 +450,14 @@ size_t pool_scratch_bytes(int B, int S, int T, int C, int H) {
 }
 
 template <int L, int C, typename W>
-static void wpool_launch(const PoolArgs& a, int B, cudaStream_t stream) {
+static int wpool_launch(const PoolArgs& a, int B, cudaStream_t stream) {
   const unsigned H = pool_h<L>();
   const dim3 grid((unsigned)B * ceil_div(a.S, kSpeakers) * H, (unsigned)a.nslices, C / 256);
-  if (a.nslices == 1) {
-    wpool_kernel<0, L, C, W><<<grid, 256, 0, stream>>>(a);
-  } else {
-    wpool_kernel<1, L, C, W><<<grid, 256, 0, stream>>>(a);
-    wpool_kernel<2, L, C, W><<<grid, 256, 0, stream>>>(a);
-    wpool_final_kernel<L, C><<<dim3((unsigned)B * a.S * H, 1, C / 256), 256, 0, stream>>>(a);
-  }
+  if (a.nslices == 1) return launch(wpool_kernel<0, L, C, W>, grid, 256, 0, stream, a);
+  int rc;
+  if ((rc = launch(wpool_kernel<1, L, C, W>, grid, 256, 0, stream, a))) return rc;
+  if ((rc = launch(wpool_kernel<2, L, C, W>, grid, 256, 0, stream, a))) return rc;
+  return launch(wpool_final_kernel<L, C>, dim3((unsigned)B * a.S * H, 1, C / 256), 256, 0, stream, a);
 }
 
 static int pool_args(const void* x, const void* w, int B, int T, int S, int Tw, double* part, __half* stats_hi,
@@ -497,14 +489,10 @@ int weighted_pool_forward(const __half* feat, const float* frames, const W* w, i
     return rc;
   a.Cv = C; a.F = T; a.ld_out = 2 * 10 * C;
   B200_CHECK(C == 256 || C == 1024, B200_ERR_STATE, "weighted pooling: %d channels unsupported", C);
-  if (feat) {
-    if (C == 256) wpool_launch<kPoolNHWC, 256, W>(a, B, stream);
-    else wpool_launch<kPoolNHWC, 1024, W>(a, B, stream);
-  } else if constexpr (fp32_w) {
-    if (C == 256) wpool_launch<kPoolNCHW, 256, W>(a, B, stream);
-    else wpool_launch<kPoolNCHW, 1024, W>(a, B, stream);
-  }
-  B200_CUDA_OK(cudaGetLastError());
+  if (feat)
+    return C == 256 ? wpool_launch<kPoolNHWC, 256, W>(a, B, stream) : wpool_launch<kPoolNHWC, 1024, W>(a, B, stream);
+  if constexpr (fp32_w)
+    return C == 256 ? wpool_launch<kPoolNCHW, 256, W>(a, B, stream) : wpool_launch<kPoolNCHW, 1024, W>(a, B, stream);
   return B200_OK;
 }
 template int weighted_pool_forward(const __half*, const float*, const uint8_t*, int, int, int, int, int, double*,
@@ -520,9 +508,7 @@ int weighted_pool_rows(const float* x, int F, int T, int C, const float* w, int 
   B200_CHECK(C >= 1 && C <= kPoolRowsLd && T <= F && ld_out >= 2 * C, B200_ERR_INVALID,
              "weighted pooling: %d channels of %d-wide rows, %d of %d frames", C, kPoolRowsLd, T, F);
   a.Cv = C; a.F = F; a.ld_out = ld_out;
-  wpool_launch<kPoolRows, kPoolRowsLd, float>(a, B, stream);
-  B200_CUDA_OK(cudaGetLastError());
-  return B200_OK;
+  return wpool_launch<kPoolRows, kPoolRowsLd, float>(a, B, stream);
 }
 
 // generic fp32 version (any F, T, S, Tw) used by the known-answer tests of the reference.  It keeps the integer index
@@ -566,9 +552,7 @@ __global__ void stats_pool_generic_kernel(const float* __restrict__ seq, const f
 int stats_pool_generic(const float* seq, const float* w, float* out, int B, int F, int T, int S, int Tw,
                        cudaStream_t stream) {
   const int total = B * S * F;
-  stats_pool_generic_kernel<<<ceil_div(total, 128), 128, 0, stream>>>(seq, w, out, B, F, T, S, Tw);
-  B200_CUDA_OK(cudaGetLastError());
-  return B200_OK;
+  return launch(stats_pool_generic_kernel, ceil_div(total, 128), 128, 0, stream, seq, w, out, B, F, T, S, Tw);
 }
 
 }  // namespace b200

@@ -156,9 +156,7 @@ __global__ void split_f16_kernel(const float* __restrict__ x, __half* __restrict
 
 int split_f16(const float* x, __half* hi, __half* lo, size_t n, cudaStream_t st) {
   if (n == 0) return B200_OK;
-  split_f16_kernel<<<(unsigned)((n + 255) / 256), 256, 0, st>>>(x, hi, lo, n);
-  B200_CUDA_OK(cudaGetLastError());
-  return B200_OK;
+  return launch(split_f16_kernel, (unsigned)((n + 255) / 256), 256, 0, st, x, hi, lo, n);
 }
 
 int gemm_tc_split(const __half* A_hi, const __half* A_lo, int lda, const __half* B_hi, const __half* B_lo, int ldb,
@@ -199,11 +197,8 @@ int gemm_tc_split(const __half* A_hi, const __half* A_lo, int lda, const __half*
   if ((rc = encode_f16_map(&tmBl, 2, B_lo, b_dims, b_str, b_box, nullptr, swz, "gemm"))) return rc;
   const size_t smem = 1024 + 1024 + (size_t)kGemmStages * kGemmStageBytes;
   const auto kernel = act == 2 ? gemm_tc_split_kernel<true> : gemm_tc_split_kernel<false>;
-  B200_CUDA_OK(cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
   const unsigned grid = (unsigned)(ceil_div(M, kGemmM) * p.tiles_n);
-  kernel<<<grid, kGemmThreads, smem, stream>>>(tmAh, tmAl, tmBh, tmBl, p);
-  B200_CUDA_OK(cudaGetLastError());
-  return B200_OK;
+  return launch(kernel, grid, kGemmThreads, smem, stream, tmAh, tmAl, tmBh, tmBl, p);
 }
 
 }  // namespace b200

@@ -52,9 +52,7 @@ __global__ void powerset_kernel(const unsigned char* __restrict__ cls, long long
 
 int powerset_to_multilabel(const unsigned char* cls, long long n, const PowersetMap& map, unsigned char* ml,
                            cudaStream_t stream) {
-  powerset_kernel<<<(unsigned)((n + 255) / 256), 256, 0, stream>>>(cls, n, map, ml);
-  B200_CUDA_OK(cudaGetLastError());
-  return B200_OK;
+  return launch(powerset_kernel, (unsigned)((n + 255) / 256), 256, 0, stream, cls, n, map, ml);
 }
 
 // first chunk whose window [start, start+nf) may contain frame f  (start_frame is non-decreasing)
@@ -83,9 +81,7 @@ __global__ void speaker_count_kernel(const unsigned char* __restrict__ seg, cons
 }
 
 int speaker_count(const unsigned char* seg, const int* sf, int C, int F, unsigned char* count, cudaStream_t stream) {
-  speaker_count_kernel<<<ceil_div(F, 256), 256, 0, stream>>>(seg, sf, C, F, count);
-  B200_CUDA_OK(cudaGetLastError());
-  return B200_OK;
+  return launch(speaker_count_kernel, ceil_div(F, 256), 256, 0, stream, seg, sf, C, F, count);
 }
 
 // ---- generic float overlap-add: Inference.aggregate (core/inference.py:498-620) ------------------------------------
@@ -122,10 +118,8 @@ int aggregate_scores(const float* scores, const int* sf, int C, int F, int nf, i
                      const double* warm, int skip_average, float missing, float epsilon, float* out,
                      cudaStream_t stream) {
   const long long n = (long long)F * K;
-  aggregate_kernel<<<(unsigned)((n + 255) / 256), 256, 0, stream>>>(scores, sf, C, F, nf, K, hamming, warm,
-                                                                     skip_average, missing, epsilon, out);
-  B200_CUDA_OK(cudaGetLastError());
-  return B200_OK;
+  return launch(aggregate_kernel, (unsigned)((n + 255) / 256), 256, 0, stream, scores, sf, C, F, nf, K, hamming, warm,
+                skip_average, missing, epsilon, out);
 }
 
 // speech score of a powerset frame = max over the speakers of its multilabel row = (its speaker set is not empty);
@@ -138,9 +132,7 @@ __global__ void powerset_speech_kernel(const unsigned char* __restrict__ cls, lo
 }
 
 int powerset_speech(const unsigned char* cls, long long n, const PowersetMap& map, float* out, cudaStream_t stream) {
-  powerset_speech_kernel<<<(unsigned)((n + 255) / 256), 256, 0, stream>>>(cls, n, map, out);
-  B200_CUDA_OK(cudaGetLastError());
-  return B200_OK;
+  return launch(powerset_speech_kernel, (unsigned)((n + 255) / 256), 256, 0, stream, cls, n, map, out);
 }
 
 // push a byte range to the same offsets of up to 7 peer buffers (P2P stores over NVLink, 16 bytes per thread): the
@@ -168,11 +160,8 @@ int push_bytes(const void* src, long long bytes, void* const* dsts, int n, cudaS
     d.d[i] = reinterpret_cast<unsigned char*>(dsts[i]);
   }
   const long long n16 = bytes / 16, tail0 = n16 * 16, total = n16 + (bytes - tail0);
-  push_bytes_kernel<<<(unsigned)((total + 255) / 256), 256, 0, stream>>>(reinterpret_cast<const uint4*>(src), d, n, n16,
-                                                                          reinterpret_cast<const unsigned char*>(src),
-                                                                          tail0, bytes);
-  B200_CUDA_OK(cudaGetLastError());
-  return B200_OK;
+  return launch(push_bytes_kernel, (unsigned)((total + 255) / 256), 256, 0, stream, reinterpret_cast<const uint4*>(src),
+                d, n, n16, reinterpret_cast<const unsigned char*>(src), tail0, bytes);
 }
 
 constexpr int kMaxK = 32;
@@ -259,12 +248,11 @@ int reconstruct(const unsigned char* seg, const signed char* hard, const int* sf
              "reconstruct: %d clusters unsupported (1..%d: hard clusters are int8 as in the reference's "
              "constrained_argmax; cap the speaker count with max_speakers)", Kout, kMaxKGeneric);
   const int grid = ceil_div(F, 128);
-  if (Kout > kMaxK) reconstruct_generic_kernel<<<grid, 128, 0, stream>>>(seg, hard, sf, C, F, Kout, count, out);
-  else if (Kout <= 8) reconstruct_kernel<8><<<grid, 128, 0, stream>>>(seg, hard, sf, C, F, Kout, count, out);
-  else if (Kout <= 16) reconstruct_kernel<16><<<grid, 128, 0, stream>>>(seg, hard, sf, C, F, Kout, count, out);
-  else reconstruct_kernel<32><<<grid, 128, 0, stream>>>(seg, hard, sf, C, F, Kout, count, out);
-  B200_CUDA_OK(cudaGetLastError());
-  return B200_OK;
+  const auto kernel = Kout > kMaxK ? reconstruct_generic_kernel
+                      : Kout <= 8  ? reconstruct_kernel<8>
+                      : Kout <= 16 ? reconstruct_kernel<16>
+                                   : reconstruct_kernel<32>;
+  return launch(kernel, grid, 128, 0, stream, seg, hard, sf, C, F, Kout, count, out);
 }
 
 // ---- onsets / offsets of the discrete diarization (Binarize with onset = offset = 0.5, utils/signal.py:254-318) ----
@@ -287,9 +275,7 @@ __global__ void __launch_bounds__(256) frame_transitions_kernel(const unsigned c
 
 int frame_transitions(const unsigned char* discrete, int F, int K, int cap, int* buf, cudaStream_t stream) {
   B200_CUDA_OK(cudaMemsetAsync(buf, 0, 2 * sizeof(int), stream));
-  frame_transitions_kernel<<<ceil_div(F + 1, 256), 256, 0, stream>>>(discrete, F, K, cap, buf);
-  B200_CUDA_OK(cudaGetLastError());
-  return B200_OK;
+  return launch(frame_transitions_kernel, ceil_div(F + 1, 256), 256, 0, stream, discrete, F, K, cap, buf);
 }
 
 __global__ void clean_frames_kernel(const unsigned char* __restrict__ seg, int C, int* __restrict__ clean,
@@ -319,9 +305,7 @@ __global__ void clean_frames_kernel(const unsigned char* __restrict__ seg, int C
 }
 
 int clean_frames(const unsigned char* seg, int C, int* clean, unsigned char* active, cudaStream_t stream) {
-  clean_frames_kernel<<<ceil_div(C * 32, 256), 256, 0, stream>>>(seg, C, clean, active);
-  B200_CUDA_OK(cudaGetLastError());
-  return B200_OK;
+  return launch(clean_frames_kernel, ceil_div(C * 32, 256), 256, 0, stream, seg, C, clean, active);
 }
 
 }  // namespace b200

@@ -105,7 +105,6 @@ int conv5_wg_forward(const SegGeom& g, int layer, const float* Pin, const float2
 // SincNet front-end on NB windows of g.W samples: wav + per-window (offset, valid) -> X0 [NB][g.pool2][64] fp32
 // (60 features + 4 zero pad)
 size_t sincnet_workspace_bytes(const SegGeom& g, int NB);
-int sincnet_launches(const SegGeom& g);   // kernels sincnet_forward launches per sub-batch
 int sincnet_forward(const SincNetWeights& W, const SegGeom& g, const float* wav, const long long* chunk_off,
                     const int* chunk_valid, int NB, void* ws, float* x0, int conv_impl, cudaStream_t stream);
 

@@ -196,10 +196,7 @@ static int launch_sc(const __half* Wh, const __half* Wl, SincConvWgParams p, int
   if ((rc = encode_f16_map(&tl, 2, Wl, dims, strides, box, nullptr, CU_TENSOR_MAP_SWIZZLE_128B, "sinc/conv weights")))
     return rc;
   auto kernel = sinc_conv_wg_kernel<CIN, CPAD, NW, NREAL, KT>;
-  B200_CUDA_OK(cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-  kernel<<<dim3(p.ntiles, NB), kSCThreads, smem, stream>>>(th, tl, p);   // one tile per 64 pooled outputs
-  B200_CUDA_OK(cudaGetLastError());
-  return B200_OK;
+  return launch(kernel, dim3(p.ntiles, NB), kSCThreads, smem, stream, th, tl, p);   // one tile per 64 pooled outputs
 }
 
 // ---- persistent, weight-resident kernels (seg_conv_impl = 1) -----------------------------------------------------
@@ -421,10 +418,7 @@ static int launch_persist(const __half* Wh, const __half* Wl, SincConvWgParams p
   B200_CHECK(units < (1ll << 31), B200_ERR_INVALID, "sinc/conv: %lld tiles in one call", units);
   const int ctas = (int)std::min<long long>((units + P::kWG - 1) / P::kWG, sms);
   auto kernel = sinc_conv_persist_kernel<CIN, CPAD, NW, NREAL, KT>;
-  B200_CUDA_OK(cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)P::kSmem));
-  kernel<<<ctas, P::kWG * 128, P::kSmem, stream>>>(th, tl, p);
-  B200_CUDA_OK(cudaGetLastError());
-  return B200_OK;
+  return launch(kernel, ctas, P::kWG * 128, P::kSmem, stream, th, tl, p);
 }
 
 // impl 1: the persistent kernels; 2: one CTA per tile (sinc_conv_wg_kernel, the bit-exact reference)

@@ -241,10 +241,7 @@ static int launch_rec(const float* Gx, const float* Whh, float* Y, __half* Yh, _
   constexpr int NBT = 8 * RB;
   const int ntiles = ceil_div(NB, NBT);
   const size_t smem = (128 * 256 + 2 * 128 * NBT) * sizeof(float);
-  B200_CUDA_OK(cudaFuncSetAttribute(lstm_rec_kernel<RB>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-  lstm_rec_kernel<RB><<<2 * 2 * ntiles, 256, smem, stream>>>(Gx, Whh, Y, Yh, Yl, NB, T, ntiles);
-  B200_CUDA_OK(cudaGetLastError());
-  return B200_OK;
+  return launch(lstm_rec_kernel<RB>, 2 * 2 * ntiles, 256, smem, stream, Gx, Whh, Y, Yh, Yl, NB, T, ntiles);
 }
 
 int lstm_head_forward(const SegWeights& W, const float* x0, int NB, int T, void* ws, const SegHeadOut& out,
@@ -298,9 +295,8 @@ int lstm_head_forward(const SegWeights& W, const float* x0, int NB, int T, void*
     if (rc) return rc;
   }
   const ClassifierFn head = (W.activation == kSegSigmoid ? kSigmoidHeads : kLogSoftmaxHeads)[W.num_classes - 1];
-  head<<<ceil_div(M, 8), 256, 0, stream>>>(w.Z2, W.cls_w, W.cls_b, out.cls, out.logp, out.scores, out.max_scores, M);
-  B200_CUDA_OK(cudaGetLastError());
-  return B200_OK;
+  return launch(head, ceil_div(M, 8), 256, 0, stream, w.Z2, W.cls_w, W.cls_b, out.cls, out.logp, out.scores,
+                out.max_scores, M);
 }
 
 }  // namespace b200

@@ -349,18 +349,11 @@ int lstm_rec_wg(const float* Gx, const __half* Wh, const __half* Wl, __half* Yh,
                              "lstm W_hh")))
       return rc;
   const int ntiles = ceil_div(NB, kRecSeqs);
-  if (impl == 1) {
-    const size_t smem = RecPipePlan::kSmem;
-    B200_CUDA_OK(cudaFuncSetAttribute(lstm_rec_pipe_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-    lstm_rec_pipe_kernel<<<2 * 2 * ntiles, RecPipePlan::kThreads, smem, stream>>>(tm[0], tm[1], Gx, Yh, Yl, NB, T,
-                                                                                  ntiles);
-  } else {
-    const size_t smem = 1024 + kRecXOff + 4u * 32u * kRecThreads * 4u;
-    B200_CUDA_OK(cudaFuncSetAttribute(lstm_rec_wg_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-    lstm_rec_wg_kernel<<<2 * 2 * ntiles, kRecThreads, smem, stream>>>(tm[0], tm[1], Gx, Yh, Yl, NB, T, ntiles);
-  }
-  B200_CUDA_OK(cudaGetLastError());
-  return B200_OK;
+  if (impl == 1)
+    return launch(lstm_rec_pipe_kernel, 2 * 2 * ntiles, RecPipePlan::kThreads, RecPipePlan::kSmem, stream, tm[0], tm[1],
+                  Gx, Yh, Yl, NB, T, ntiles);
+  const size_t smem = 1024 + kRecXOff + 4u * 32u * kRecThreads * 4u;
+  return launch(lstm_rec_wg_kernel, 2 * 2 * ntiles, kRecThreads, smem, stream, tm[0], tm[1], Gx, Yh, Yl, NB, T, ntiles);
 }
 
 }  // namespace b200

@@ -229,19 +229,21 @@ __global__ void part_reduce_kernel(const double2* __restrict__ in, int n_in, dou
 
 // partial sums [rows][ntiles] -> affine [rows]; up to kFinGroup tiles (every stage of a 10 s window) take the single
 // in_finalize_kernel pass, more are first combined in groups into red0 / red1 (ping-pong)
-static void in_stats(const double2* part, int ntiles, double2* red0, double2* red1, int n, int C, const float* gamma,
-                     const float* beta, float2* affine, int rows, cudaStream_t stream) {
+static int in_stats(const double2* part, int ntiles, double2* red0, double2* red1, int n, int C, const float* gamma,
+                    const float* beta, float2* affine, int rows, cudaStream_t stream) {
   const double2* cur = part;
   double2* bufs[2] = {red0, red1};
-  int k = 0;
+  int k = 0, rc;
   while (ntiles > kFinGroup) {
     const int n_out = ceil_div(ntiles, kFinGroup);
-    part_reduce_kernel<<<ceil_div(rows * n_out, 256), 256, 0, stream>>>(cur, ntiles, bufs[k], n_out, rows);
+    if ((rc = launch(part_reduce_kernel, ceil_div(rows * n_out, 256), 256, 0, stream, cur, ntiles, bufs[k], n_out,
+                     rows)))
+      return rc;
     cur = bufs[k];
     ntiles = n_out;
     k ^= 1;
   }
-  in_finalize_kernel<<<ceil_div(rows, 128), 128, 0, stream>>>(cur, ntiles, n, C, gamma, beta, affine, rows);
+  return launch(in_finalize_kernel, ceil_div(rows, 128), 128, 0, stream, cur, ntiles, n, C, gamma, beta, affine, rows);
 }
 
 // ---- Conv1d(CIN,60,5) + maxpool3 on the normalised, leaky-relu'd input --------------------------------
@@ -386,13 +388,6 @@ static size_t carve(const SegGeom& g, int NB, void* base, SincWs* w) {
 
 size_t sincnet_workspace_bytes(const SegGeom& g, int NB) { return carve(g, NB, nullptr, nullptr); }
 
-int sincnet_launches(const SegGeom& g) {
-  int n = 8 + (wav_slices(g) > 1);
-  for (int t : {g.tiles0, g.tiles1, g.tiles2})
-    for (; t > kFinGroup; t = ceil_div(t, kFinGroup)) ++n;
-  return n;
-}
-
 int sincnet_forward(const SincNetWeights& W, const SegGeom& g, const float* wav, const long long* chunk_off,
                     const int* chunk_valid, int NB, void* ws, float* x0, int conv_impl, cudaStream_t stream) {
   SincWs w;
@@ -401,48 +396,54 @@ int sincnet_forward(const SincNetWeights& W, const SegGeom& g, const float* wav,
   const size_t smem_c80 = (80 * 196 + 20 * 300) * sizeof(float);
   const size_t smem_c60 = (60 * 196 + 20 * 300) * sizeof(float);
   const int nslices = wav_slices(g);
-  wav_stats_kernel<<<dim3(nslices, NB), 512, 0, stream>>>(wav, chunk_off, chunk_valid, g.W, W.wav_w, W.wav_b,
-                                                          w.af_wav, w.wav_part);
-  if (nslices > 1)
-    wav_finalize_kernel<<<ceil_div(NB, 128), 128, 0, stream>>>(w.wav_part, nslices, g.W, W.wav_w, W.wav_b, w.af_wav,
-                                                               NB);
+  int rc;
+  if ((rc = launch(wav_stats_kernel, dim3(nslices, NB), 512, 0, stream, wav, chunk_off, chunk_valid, g.W, W.wav_w,
+                   W.wav_b, w.af_wav, w.wav_part)))
+    return rc;
+  if (nslices > 1 && (rc = launch(wav_finalize_kernel, ceil_div(NB, 128), 128, 0, stream, w.wav_part, nslices, g.W,
+                                  W.wav_w, W.wav_b, w.af_wav, NB)))
+    return rc;
   // conv_impl: 1 = persistent split-fp16 wgmma kernels (default), 2 = one wgmma CTA per tile, 0 = the fp32 CUDA-core
   // twins
-  int rc;
   if (conv_impl) {
     if ((rc = sinc_wg_forward(g, wav, chunk_off, chunk_valid, w.af_wav, W.sinc_wg_hi, W.sinc_wg_lo, NB, w.P0, w.part0,
                               conv_impl, stream)))
       return rc;
   } else {
-    B200_CUDA_OK(cudaFuncSetAttribute(sinc_pool_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem_sinc));
-    sinc_pool_kernel<<<dim3(g.tiles0, NB), 128, smem_sinc, stream>>>(wav, chunk_off, chunk_valid, w.af_wav, W.sinc_f,
-                                                                    g.W, w.P0, g.pool0, g.tiles0, w.part0);
+    if ((rc = launch(sinc_pool_kernel, dim3(g.tiles0, NB), 128, smem_sinc, stream, wav, chunk_off, chunk_valid,
+                     w.af_wav, W.sinc_f, g.W, w.P0, g.pool0, g.tiles0, w.part0)))
+      return rc;
   }
-  in_stats(w.part0, g.tiles0, w.red0, w.red1, g.pool0, 80, W.in_gamma[0], W.in_beta[0], w.af0, NB * 80, stream);
+  if ((rc = in_stats(w.part0, g.tiles0, w.red0, w.red1, g.pool0, 80, W.in_gamma[0], W.in_beta[0], w.af0, NB * 80,
+                     stream)))
+    return rc;
   if (conv_impl) {
     if ((rc = conv5_wg_forward(g, 0, w.P0, w.af0, W.conv_wg_hi[0], W.conv_wg_lo[0], W.conv_b[0], NB, w.P1, w.part1,
                                conv_impl, stream)))
       return rc;
   } else {
-    B200_CUDA_OK(cudaFuncSetAttribute(conv5_pool_kernel<80>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem_c80));
-    conv5_pool_kernel<80><<<dim3(g.tiles1, NB), 192, smem_c80, stream>>>(w.P0, g.pool0, w.af0, W.conv_w[0],
-                                                                         W.conv_b[0], w.P1, g.pool1, g.tiles1, w.part1);
+    if ((rc = launch(conv5_pool_kernel<80>, dim3(g.tiles1, NB), 192, smem_c80, stream, w.P0, g.pool0, w.af0,
+                     W.conv_w[0], W.conv_b[0], w.P1, g.pool1, g.tiles1, w.part1)))
+      return rc;
   }
-  in_stats(w.part1, g.tiles1, w.red0, w.red1, g.pool1, 60, W.in_gamma[1], W.in_beta[1], w.af1, NB * 60, stream);
+  if ((rc = in_stats(w.part1, g.tiles1, w.red0, w.red1, g.pool1, 60, W.in_gamma[1], W.in_beta[1], w.af1, NB * 60,
+                     stream)))
+    return rc;
   if (conv_impl) {
     if ((rc = conv5_wg_forward(g, 1, w.P1, w.af1, W.conv_wg_hi[1], W.conv_wg_lo[1], W.conv_b[1], NB, w.P2, w.part2,
                                conv_impl, stream)))
       return rc;
   } else {
-    B200_CUDA_OK(cudaFuncSetAttribute(conv5_pool_kernel<60>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem_c60));
-    conv5_pool_kernel<60><<<dim3(g.tiles2, NB), 192, smem_c60, stream>>>(w.P1, g.pool1, w.af1, W.conv_w[1],
-                                                                         W.conv_b[1], w.P2, g.pool2, g.tiles2, w.part2);
+    if ((rc = launch(conv5_pool_kernel<60>, dim3(g.tiles2, NB), 192, smem_c60, stream, w.P1, g.pool1, w.af1,
+                     W.conv_w[1], W.conv_b[1], w.P2, g.pool2, g.tiles2, w.part2)))
+      return rc;
   }
-  in_stats(w.part2, g.tiles2, w.red0, w.red1, g.pool2, 60, W.in_gamma[2], W.in_beta[2], w.af2, NB * 60, stream);
+  if ((rc = in_stats(w.part2, g.tiles2, w.red0, w.red1, g.pool2, 60, W.in_gamma[2], W.in_beta[2], w.af2, NB * 60,
+                     stream)))
+    return rc;
   const size_t total = (size_t)NB * g.pool2 * 64;
-  in_apply_transpose_kernel<<<(unsigned)((total + 255) / 256), 256, 0, stream>>>(w.P2, w.af2, x0, NB, g.pool2);
-  B200_CUDA_OK(cudaGetLastError());
-  return B200_OK;
+  return launch(in_apply_transpose_kernel, (unsigned)((total + 255) / 256), 256, 0, stream, w.P2, w.af2, x0, NB,
+                g.pool2);
 }
 
 }  // namespace b200

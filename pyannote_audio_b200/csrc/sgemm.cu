@@ -101,12 +101,8 @@ int sgemm_nt(const float* A, int lda, const float* Bw, int ldb, float* C, int ld
   B200_CHECK(K % BK == 0 && N % 4 == 0 && lda % 4 == 0 && ldb % 4 == 0 && ldc % 4 == 0, B200_ERR_INVALID,
              "sgemm_nt: unsupported shape M=%d N=%d K=%d", M, N, K);
   dim3 grid(ceil_div(M, BM), ceil_div(N, BN));
-  if (act == 1)
-    sgemm_nt_kernel<1><<<grid, 256, 0, stream>>>(A, lda, Bw, ldb, C, ldc, bias, M, N, K);
-  else
-    sgemm_nt_kernel<0><<<grid, 256, 0, stream>>>(A, lda, Bw, ldb, C, ldc, bias, M, N, K);
-  B200_CUDA_OK(cudaGetLastError());
-  return B200_OK;
+  return launch(act == 1 ? sgemm_nt_kernel<1> : sgemm_nt_kernel<0>, grid, 256, 0, stream, A, lda, Bw, ldb, C, ldc, bias,
+                M, N, K);
 }
 
 }  // namespace b200

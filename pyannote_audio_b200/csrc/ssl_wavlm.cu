@@ -351,17 +351,17 @@ int ssl_frontend_forward(const SslWeights& W, const SslGeom& g, const float* wav
   carve_ssl(g, NB, ws, &w);
   int rc;
   // feature extractor
-  ssl_conv0_kernel<<<dim3(ceil_div(g.len[0], kConv0T), NB), kSslConvDim, 0, st>>>(wav, chunk_off, chunk_valid,
-                                                                                   W.conv0_w, w.raw, g.len[0],
-                                                                                   g.stride[0]);
-  B200_CUDA_OK(cudaGetLastError());
+  if ((rc = launch(ssl_conv0_kernel, dim3(ceil_div(g.len[0], kConv0T), NB), kSslConvDim, 0, st, wav, chunk_off,
+                   chunk_valid, W.conv0_w, w.raw, g.len[0], g.stride[0])))
+    return rc;
   float2* stats = reinterpret_cast<float2*>(w.P);          // [NB][512], P is free until the positional conv
-  ssl_gn_stats_kernel<<<dim3(kSslConvDim / 32, NB), dim3(32, 16), 0, st>>>(w.raw, stats, g.len[0], g.stride[0]);
-  B200_CUDA_OK(cudaGetLastError());
+  if ((rc = launch(ssl_gn_stats_kernel, dim3(kSslConvDim / 32, NB), dim3(32, 16), 0, st, w.raw, stats, g.len[0],
+                   g.stride[0])))
+    return rc;
   const size_t R = (size_t)NB * g.stride[0] * kSslConvDim;
-  ssl_gn_apply_kernel<<<blocks_for(R, 256), 256, 0, st>>>(w.raw, stats, W.gn_w, W.gn_b, w.ah, w.al, g.len[0],
-                                                          g.stride[0], R);
-  B200_CUDA_OK(cudaGetLastError());
+  if ((rc = launch(ssl_gn_apply_kernel, blocks_for(R, 256), 256, 0, st, w.raw, stats, W.gn_w, W.gn_b, w.ah, w.al,
+                   g.len[0], g.stride[0], R)))
+    return rc;
   float* feat = reinterpret_cast<float*>(w.ah);             // conv 6 output fp32 (written into the free even buffer)
   for (int l = 1; l <= 6; ++l) {
     const bool from_a = (l & 1) == 1;
@@ -383,16 +383,16 @@ int ssl_frontend_forward(const SslWeights& W, const SslGeom& g, const float* wav
   // feature projection: LayerNorm(512) of the valid frames (compacted to [NB][T]) -> Linear 512 -> 768
   const int T = g.T, M = NB * T;
   __half *fh = w.xh, *fl = w.x1h;                           // [M][512] pairs in buffers free until layer 0
-  ssl_ln_kernel<kSslConvDim><<<ceil_div(M, 8), 256, 0, st>>>(feat, nullptr, T, g.stride[6], W.fp_ln_w, W.fp_ln_b,
-                                                             nullptr, fh, fl, nullptr, 0.f, 0, M);
-  B200_CUDA_OK(cudaGetLastError());
+  if ((rc = launch(ssl_ln_kernel<kSslConvDim>, ceil_div(M, 8), 256, 0, st, feat, nullptr, T, g.stride[6], W.fp_ln_w,
+                   W.fp_ln_b, nullptr, fh, fl, nullptr, 0.f, 0, M)))
+    return rc;
   if ((rc = gemm_tc_split(fh, fl, kSslConvDim, W.proj_hi, W.proj_lo, kSslConvDim, w.x, kSslDim, nullptr, nullptr, 0,
                           W.proj_b, M, kSslDim, kSslConvDim, 0, num_sms, st)))
     return rc;
   // positional conv: 16 group GEMMs of 128 taps over the zero-padded, group-major copy of x
   const size_t Mp = (size_t)NB * (T + kSslPosK);
-  ssl_pos_pack_kernel<<<blocks_for(Mp * 1024, 256), 256, 0, st>>>(w.x, w.ph, w.pl, T, Mp * 1024);
-  B200_CUDA_OK(cudaGetLastError());
+  if ((rc = launch(ssl_pos_pack_kernel, blocks_for(Mp * 1024, 256), 256, 0, st, w.x, w.ph, w.pl, T, Mp * 1024)))
+    return rc;
   GemmTaps ptaps;
   ptaps.taps = kSslPosK;
   ptaps.dil = 1;
@@ -404,31 +404,30 @@ int ssl_frontend_forward(const SslWeights& W, const SslGeom& g, const float* wav
       return rc;
   }
   const size_t MD = (size_t)M * kSslDim;
-  ssl_pos_add_kernel<<<blocks_for(MD, 256), 256, 0, st>>>(w.x, w.P, w.x1, T, MD);
-  B200_CUDA_OK(cudaGetLastError());
+  if ((rc = launch(ssl_pos_add_kernel, blocks_for(MD, 256), 256, 0, st, w.x, w.P, w.x1, T, MD))) return rc;
   // encoder.transformer.layer_norm: the post-LN encoder's Transformer normalises before its first layer
-  ssl_ln_kernel<kSslDim><<<ceil_div(M, 8), 256, 0, st>>>(w.x1, nullptr, T, T, W.enc_ln_w, W.enc_ln_b, w.x, w.xh, w.xl,
-                                                         nullptr, 0.f, 0, M);
-  B200_CUDA_OK(cudaGetLastError());
+  if ((rc = launch(ssl_ln_kernel<kSslDim>, ceil_div(M, 8), 256, 0, st, w.x1, nullptr, T, T, W.enc_ln_w, W.enc_ln_b, w.x,
+                   w.xh, w.xl, nullptr, 0.f, 0, M)))
+    return rc;
   // transformer layers
-  B200_CUDA_OK(cudaFuncSetAttribute(ssl_attention_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kAttSmem));
   bool averaged = false;                                    // x0 holds a first weighted layer output
   for (int l = 0; l < W.num_layers; ++l) {
     const SslLayerWeights& L = W.layer[l];
-    ssl_gate_kernel<<<ceil_div(M * kSslHeads, 256), 256, 0, st>>>(w.x, L.gru_w, L.gru_b, L.gru_const, w.gate, M);
-    B200_CUDA_OK(cudaGetLastError());
+    if ((rc = launch(ssl_gate_kernel, ceil_div(M * kSslHeads, 256), 256, 0, st, w.x, L.gru_w, L.gru_b, L.gru_const,
+                     w.gate, M)))
+      return rc;
     if ((rc = gemm_tc_split(w.xh, w.xl, kSslDim, L.qkv_hi, L.qkv_lo, kSslDim, w.qkv, 3 * kSslDim, nullptr, nullptr, 0,
                             L.qkv_b, M, 3 * kSslDim, kSslDim, 0, num_sms, st)))
       return rc;
-    ssl_attention_kernel<<<dim3(ceil_div(T, kAttTile), kSslHeads, NB), 256, kAttSmem, st>>>(w.qkv, w.gate, W.rel_tab,
-                                                                                          w.atth, w.attl, T);
-    B200_CUDA_OK(cudaGetLastError());
+    if ((rc = launch(ssl_attention_kernel, dim3(ceil_div(T, kAttTile), kSslHeads, NB), 256, kAttSmem, st, w.qkv, w.gate,
+                     W.rel_tab, w.atth, w.attl, T)))
+      return rc;
     if ((rc = gemm_tc_split(w.atth, w.attl, kSslDim, L.out_hi, L.out_lo, kSslDim, w.o, kSslDim, nullptr, nullptr, 0,
                             L.out_b, M, kSslDim, kSslDim, 0, num_sms, st)))
       return rc;
-    ssl_ln_kernel<kSslDim><<<ceil_div(M, 8), 256, 0, st>>>(w.o, w.x, T, T, L.ln1_w, L.ln1_b, w.x1, w.x1h, w.x1l,
-                                                           nullptr, 0.f, 0, M);
-    B200_CUDA_OK(cudaGetLastError());
+    if ((rc = launch(ssl_ln_kernel<kSslDim>, ceil_div(M, 8), 256, 0, st, w.o, w.x, T, T, L.ln1_w, L.ln1_b, w.x1, w.x1h,
+                     w.x1l, nullptr, 0.f, 0, M)))
+      return rc;
     if ((rc = gemm_tc_split(w.x1h, w.x1l, kSslDim, L.ff1_hi, L.ff1_lo, kSslDim, nullptr, 0, w.hh, w.hl, kSslFfn, L.ff1_b,
                             M, kSslFfn, kSslDim, 2, num_sms, st)))
       return rc;
@@ -437,9 +436,9 @@ int ssl_frontend_forward(const SslWeights& W, const SslGeom& g, const float* wav
       return rc;
     // the layer's output is the next layer's input x; the weighted layer average accumulates into x0
     const float aw = W.layer_w[l];
-    ssl_ln_kernel<kSslDim><<<ceil_div(M, 8), 256, 0, st>>>(w.o, w.x1, T, T, L.ln2_w, L.ln2_b, w.x, w.xh, w.xl,
-                                                           aw != 0.f ? x0 : nullptr, aw, !averaged, M);
-    B200_CUDA_OK(cudaGetLastError());
+    if ((rc = launch(ssl_ln_kernel<kSslDim>, ceil_div(M, 8), 256, 0, st, w.o, w.x1, T, T, L.ln2_w, L.ln2_b, w.x, w.xh,
+                     w.xl, aw != 0.f ? x0 : nullptr, aw, !averaged, M)))
+      return rc;
     averaged = averaged || aw != 0.f;
   }
   return B200_OK;
