@@ -140,12 +140,13 @@ struct ScopedTimer {
   std::vector<std::pair<cudaEvent_t, cudaEvent_t>>* sink;
   cudaStream_t st;
   cudaEvent_t a = nullptr, b = nullptr;
+  // a null sink times nothing
   ScopedTimer(b200_ctx* c, std::vector<std::pair<cudaEvent_t, cudaEvent_t>>* s, cudaStream_t stream)
       : ctx(c), sink(s), st(stream) {
-    if (ctx->profile) { a = take_event(ctx); b = take_event(ctx); cudaEventRecord(a, st); }
+    if (ctx->profile && sink) { a = take_event(ctx); b = take_event(ctx); cudaEventRecord(a, st); }
   }
   ~ScopedTimer() {
-    if (ctx->profile) { cudaEventRecord(b, st); sink->push_back({a, b}); }
+    if (ctx->profile && sink) { cudaEventRecord(b, st); sink->push_back({a, b}); }
   }
 };
 
@@ -391,10 +392,24 @@ int load_sincnet(b200_ctx* ctx, float wav_w, float wav_b, const float* sinc_filt
   return B200_OK;
 }
 
+// The head shape of a PyanNet or SSeRiouSS load, checked before the loader releases the resident weights, so that a
+// refused head leaves the loaded model in place
+int check_head(int lstm_layers, int num_classes, int activation) {
+  B200_CHECK(num_classes >= 1 && num_classes <= kSegMaxClasses, B200_ERR_INVALID,
+             "a classifier of %d classes is unsupported (1 .. %d)", num_classes, kSegMaxClasses);
+  B200_CHECK(activation == B200_SEG_LOGSOFTMAX || activation == B200_SEG_SIGMOID, B200_ERR_INVALID,
+             "unknown classifier activation %d (B200_SEG_LOGSOFTMAX = 0, B200_SEG_SIGMOID = 1)", activation);
+  B200_CHECK(lstm_layers >= 1 && lstm_layers <= 4, B200_ERR_INVALID, "lstm_layers=%d unsupported", lstm_layers);
+  return B200_OK;
+}
+
 // The BiLSTM stack (layer 0: in0 inputs padded to kpad0), linear layers and classifier that PyanNet and SSeRiouSS share
-// (b200_seg_weights / b200_ssl_weights fields of the same names)
+// (b200_seg_weights / b200_ssl_weights fields of the same names), of a head that passed check_head
 template <class Wt>
-int load_lstm_head(b200_ctx* ctx, const Wt* w, int in0, int kpad0, int num_classes, SegWeights& S) {
+int load_lstm_head(b200_ctx* ctx, const Wt* w, int in0, int kpad0, int num_classes, int activation, SegWeights& S) {
+  S.lstm_layers = w->lstm_layers;
+  S.num_classes = num_classes;
+  S.activation = activation == B200_SEG_SIGMOID ? kSegSigmoid : kSegLogSoftmax;
   int rc;
   for (int l = 0; l < S.lstm_layers; ++l) {
     const int I = l == 0 ? in0 : 256, Kp = l == 0 ? kpad0 : 256;
@@ -591,24 +606,16 @@ int b200_audio_ingest(b200_ctx* ctx, const void* pcm, int32_t format, int32_t ch
 // ------------------------------------------------------------------------------------------------------
 int b200_seg_load_head(b200_ctx* ctx, const b200_seg_weights* w, int32_t num_classes, int32_t activation) {
   B200_CHECK(ctx && w, B200_ERR_INVALID, "NULL ctx/weights");
-  B200_CHECK(num_classes >= 1 && num_classes <= kSegMaxClasses, B200_ERR_INVALID,
-             "a classifier of %d classes is unsupported (1 .. %d)", (int)num_classes, kSegMaxClasses);
-  B200_CHECK(activation == B200_SEG_LOGSOFTMAX || activation == B200_SEG_SIGMOID, B200_ERR_INVALID,
-             "unknown classifier activation %d (B200_SEG_LOGSOFTMAX = 0, B200_SEG_SIGMOID = 1)", (int)activation);
+  int rc;
+  if ((rc = check_head(w->lstm_layers, num_classes, activation))) return rc;
   CtxScope scope(ctx);
   SegWeights& S = ctx->seg;
-  B200_CHECK(w->lstm_layers >= 1 && w->lstm_layers <= 4, B200_ERR_INVALID, "lstm_layers=%d unsupported",
-             (int)w->lstm_layers);
   S.loaded = false;
   release_weights(ctx, &ctx->owned_seg);
-  S.lstm_layers = w->lstm_layers;
-  S.num_classes = num_classes;
-  S.activation = activation == B200_SEG_SIGMOID ? kSegSigmoid : kSegLogSoftmax;
-  int rc;
   if ((rc = load_sincnet(ctx, w->wav_norm_weight, w->wav_norm_bias, w->sinc_filters, w->norm_weight, w->norm_bias,
                          w->conv_weight, w->conv_bias, &S.sinc)))
     return rc;
-  if ((rc = load_lstm_head(ctx, w, 60, 64, num_classes, S))) return rc;
+  if ((rc = load_lstm_head(ctx, w, 60, 64, num_classes, activation, S))) return rc;
   S.loaded = true;
   return B200_OK;
 }
@@ -700,77 +707,124 @@ int b200_emb_load_bottleneck(b200_ctx* ctx, const b200_emb_bottleneck_weights* w
 }
 
 // ------------------------------------------------------------------------------------------------------
-// PyanNet on n windows of `window` samples.  A sub-batch holds at most seg_max_batch x 160000 window samples (the
-// workspace of seg_max_batch 10 s chunks) and at most 65535 windows (the y extent of the SincNet grids).
-static int seg_run(b200_ctx* ctx, const float* wav, const int64_t* chunk_off, const int32_t* chunk_valid, int n,
-                   int window, const SegHeadOut& out, float* sinc_out, cudaStream_t st) {
-  B200_CHECK(ctx && ctx->seg.loaded, B200_ERR_STATE, "segmentation weights not loaded");
+// The two front ends of the segmentation head (load_lstm_head, lstm_head_forward): SincNet writes PyanNet's head input
+// (60 features and 4 zero columns per frame), WavLM Base that of SSeRiouSS (768 features per frame)
+enum class SegFront { kSincNet, kWavLM };
+
+// the head behind a front end, or null while its model is not loaded
+static const SegWeights* loaded_head(const b200_ctx* ctx, SegFront front) {
+  const bool sinc = front == SegFront::kSincNet;
+  if (!ctx || !(sinc ? ctx->seg.loaded : ctx->ssl.loaded)) return nullptr;
+  return sinc ? &ctx->seg : &ctx->ssl.head;
+}
+
+// A segmentation model on n windows of `window` samples: per sub-batch, the front end writes x0 [nb][T][F] and the
+// head classifies it, both phases in the same workspace region.  A sub-batch holds at most max_batch x 160000
+// window samples (the workspace of max_batch 10 s windows; option seg_max_batch or ssl_max_batch) and at most 65535
+// windows (the y extent of the SincNet grids).  The "seg" timer covers PyanNet's sub-batches.  With sinc_out (SincNet
+// only), the front end writes there and the head does not run.
+static int seg_run(b200_ctx* ctx, SegFront front, const float* wav, const int64_t* chunk_off,
+                   const int32_t* chunk_valid, int n, int window, const SegHeadOut& out, float* sinc_out,
+                   cudaStream_t st) {
+  const bool sinc = front == SegFront::kSincNet;
+  const char* model = sinc ? "segmentation" : "SSeRiouSS";
+  const SegWeights* head = loaded_head(ctx, front);
+  B200_CHECK(head, B200_ERR_STATE, "%s weights not loaded", model);
   B200_CHECK(wav && chunk_off && chunk_valid && n >= 0, B200_ERR_INVALID, "bad arguments");
-  B200_CHECK(window >= kSegMinWindow, B200_ERR_INVALID,
-             "windows of %d samples are too short: PyanNet needs at least %d samples (2 output frames)", window,
-             kSegMinWindow);
-  const int64_t budget = (int64_t)ctx->seg_max_batch * kChunk;
+  const int min_window = sinc ? kSegMinWindow : kSslMinWindow;
+  B200_CHECK(window >= min_window, B200_ERR_INVALID,
+             "windows of %d samples are too short: %s needs at least %d samples (%s)", window,
+             sinc ? "PyanNet" : "SSeRiouSS", min_window, sinc ? "2 output frames" : "one WavLM frame");
+  const char* option = sinc ? "seg_max_batch" : "ssl_max_batch";
+  const int max_batch = sinc ? ctx->seg_max_batch : ctx->ssl_max_batch;
+  const int64_t budget = (int64_t)max_batch * kChunk;
   B200_CHECK(window <= budget, B200_ERR_INVALID,
-             "a window of %d samples is longer than the %lld samples of one segmentation sub-batch (seg_max_batch %d x "
-             "160000): set the option seg_max_batch to at least %lld, or segment shorter excerpts",
-             window, (long long)budget, ctx->seg_max_batch, (long long)((window + kChunk - 1) / kChunk));
+             "a window of %d samples is longer than the %lld samples of one %s sub-batch (%s %d x 160000): set the "
+             "option %s to at least %lld, or segment shorter excerpts",
+             window, (long long)budget, model, option, max_batch, option, (long long)((window + kChunk - 1) / kChunk));
   if (n == 0) return B200_OK;
   CtxScope scope(ctx);
-  const SegGeom geom = seg_geom(window);
-  const int T = geom.pool2;
   const int nbmax = (int)std::min<int64_t>(std::min<int64_t>(n, budget / window), 65535);
-  const size_t x0_bytes = align_up((size_t)nbmax * T * 64 * sizeof(float), 1024);
-  const size_t sinc_b = sincnet_workspace_bytes(geom, nbmax), lstm_b = lstm_workspace_bytes(nbmax, T, 64);
-  const size_t big = sinc_b > lstm_b ? sinc_b : lstm_b;    // the two phases reuse the same region
-  int rc = ensure_ws(ctx, x0_bytes + big + 4096);
+  SegGeom seg_g{};
+  SslGeom ssl_g{};
+  int T = 0, F = 0;            // frames and features per window
+  size_t front_b = 0;
+  switch (front) {
+    case SegFront::kSincNet:
+      seg_g = seg_geom(window);
+      T = seg_g.pool2;
+      F = 64;
+      front_b = sincnet_workspace_bytes(seg_g, nbmax);
+      break;
+    case SegFront::kWavLM:
+      ssl_g = ssl_geom(window);
+      T = ssl_g.T;
+      F = kSslDim;
+      front_b = ssl_workspace_bytes(ssl_g, nbmax);
+      break;
+  }
+  const size_t x0_bytes = align_up((size_t)nbmax * T * F * sizeof(float), 1024);
+  int rc = ensure_ws(ctx, x0_bytes + std::max(front_b, lstm_workspace_bytes(nbmax, T, F)) + 4096);
   if (rc) return rc;
   if ((rc = push_meta(ctx, chunk_off, chunk_valid, n, st, window))) return rc;
   float* x0 = reinterpret_cast<float*>(ctx->ws);
   void* region = reinterpret_cast<char*>(ctx->ws) + x0_bytes;
   for (int c0 = 0; c0 < n; c0 += nbmax) {
     const int nb = (n - c0) < nbmax ? (n - c0) : nbmax;
-    ScopedTimer timer(ctx, &ctx->seg_events, st);
-    if (ctx->profile) ctx->seg_chunks += nb;
-    float* x0_dst = sinc_out ? sinc_out + (size_t)c0 * T * 64 : x0;
-    if ((rc = sincnet_forward(ctx->seg.sinc, geom, wav, ctx->d_off + c0, ctx->d_valid + c0, nb, region, x0_dst,
-                              ctx->seg_conv_impl, st)))
-      return rc;
+    ScopedTimer timer(ctx, sinc ? &ctx->seg_events : nullptr, st);
+    if (ctx->profile && sinc) ctx->seg_chunks += nb;
+    switch (front) {
+      case SegFront::kSincNet:
+        rc = sincnet_forward(ctx->seg.sinc, seg_g, wav, ctx->d_off + c0, ctx->d_valid + c0, nb, region,
+                             sinc_out ? sinc_out + (size_t)c0 * T * F : x0, ctx->seg_conv_impl, st);
+        break;
+      case SegFront::kWavLM:
+        rc = ssl_frontend_forward(ctx->ssl, ssl_g, wav, ctx->d_off + c0, ctx->d_valid + c0, nb, region, x0,
+                                  ctx->num_sms, st);
+        break;
+    }
+    if (rc) return rc;
     if (sinc_out) continue;
-    const size_t row0 = (size_t)c0 * T, K = ctx->seg.num_classes;
+    const size_t row0 = (size_t)c0 * T, K = head->num_classes;
     SegHeadOut sub;
     sub.cls = out.cls ? out.cls + row0 : nullptr;
     sub.logp = out.logp ? out.logp + row0 * K : nullptr;
     sub.scores = out.scores ? out.scores + row0 * K : nullptr;
     sub.max_scores = out.max_scores ? out.max_scores + row0 : nullptr;
-    if ((rc = lstm_head_forward(ctx->seg, x0, nb, T, region, sub, ctx->num_sms, ctx->seg_gemm_impl, ctx->seg_rec_impl,
+    if ((rc = lstm_head_forward(*head, x0, nb, T, region, sub, ctx->num_sms, ctx->seg_gemm_impl, ctx->seg_rec_impl,
                                 st)))
       return rc;
   }
   return B200_OK;
 }
 
+// The forward entry points of one activation: kSegLogSoftmax writes out.cls (+ out.logp), kSegSigmoid out.scores and /
+// or out.max_scores.  A loaded head of the other activation is refused, naming the entry point to call.
+static int seg_forward_head(b200_ctx* ctx, SegFront front, int activation, const float* wav, const int64_t* chunk_off,
+                            const int32_t* chunk_valid, int32_t num_chunks, int32_t window, const SegHeadOut& out,
+                            void* stream) {
+  const bool sinc = front == SegFront::kSincNet, sigmoid = activation == kSegSigmoid;
+  const SegWeights* head = loaded_head(ctx, front);
+  B200_CHECK(!(head && head->activation != activation), B200_ERR_INVALID,
+             "the loaded %s head is a %s head: call b200_%s_forward_%s", sinc ? "segmentation" : "SSeRiouSS",
+             sigmoid ? "log-softmax (powerset / mono-label)" : "sigmoid (multi-label / binary)", sinc ? "seg" : "ssl",
+             sigmoid ? "window" : "scores");
+  if (num_chunks == 0) return B200_OK;
+  if (sigmoid) B200_CHECK(out.scores || out.max_scores, B200_ERR_INVALID, "scores and max_scores are both NULL");
+  else B200_CHECK(out.cls != nullptr, B200_ERR_INVALID, "classes is NULL");
+  return seg_run(ctx, front, wav, chunk_off, chunk_valid, num_chunks, window, out, nullptr, (cudaStream_t)stream);
+}
+
 int b200_seg_forward_window(b200_ctx* ctx, const float* wav, const int64_t* chunk_off, const int32_t* chunk_valid,
                             int32_t num_chunks, int32_t window, uint8_t* classes, float* logp, void* stream) {
-  B200_CHECK(!(ctx && ctx->seg.loaded && ctx->seg.activation != kSegLogSoftmax), B200_ERR_INVALID,
-             "the loaded segmentation head is a sigmoid (multi-label / binary) head: call b200_seg_forward_scores");
-  if (num_chunks == 0) return B200_OK;
-  B200_CHECK(classes != nullptr, B200_ERR_INVALID, "classes is NULL");
-  SegHeadOut out;
-  out.cls = classes;
-  out.logp = logp;
-  return seg_run(ctx, wav, chunk_off, chunk_valid, num_chunks, window, out, nullptr, (cudaStream_t)stream);
+  return seg_forward_head(ctx, SegFront::kSincNet, kSegLogSoftmax, wav, chunk_off, chunk_valid, num_chunks, window,
+                          SegHeadOut{classes, logp}, stream);
 }
 
 int b200_seg_forward_scores(b200_ctx* ctx, const float* wav, const int64_t* chunk_off, const int32_t* chunk_valid,
                             int32_t num_chunks, int32_t window, float* scores, float* max_scores, void* stream) {
-  B200_CHECK(!(ctx && ctx->seg.loaded && ctx->seg.activation != kSegSigmoid), B200_ERR_INVALID,
-             "the loaded segmentation head is a log-softmax (powerset / mono-label) head: call b200_seg_forward_window");
-  if (num_chunks == 0) return B200_OK;
-  B200_CHECK(scores || max_scores, B200_ERR_INVALID, "scores and max_scores are both NULL");
-  SegHeadOut out;
-  out.scores = scores;
-  out.max_scores = max_scores;
-  return seg_run(ctx, wav, chunk_off, chunk_valid, num_chunks, window, out, nullptr, (cudaStream_t)stream);
+  return seg_forward_head(ctx, SegFront::kSincNet, kSegSigmoid, wav, chunk_off, chunk_valid, num_chunks, window,
+                          SegHeadOut{nullptr, nullptr, scores, max_scores}, stream);
 }
 
 int b200_seg_forward(b200_ctx* ctx, const float* wav, const int64_t* chunk_off, const int32_t* chunk_valid,
@@ -781,12 +835,8 @@ int b200_seg_forward(b200_ctx* ctx, const float* wav, const int64_t* chunk_off, 
 // ------------------------------------------------------------------------------------------------------
 int b200_ssl_load(b200_ctx* ctx, const b200_ssl_weights* w, int32_t num_classes, int32_t activation) {
   B200_CHECK(ctx && w, B200_ERR_INVALID, "NULL ctx/weights");
-  B200_CHECK(num_classes >= 1 && num_classes <= kSegMaxClasses, B200_ERR_INVALID,
-             "a classifier of %d classes is unsupported (1 .. %d)", (int)num_classes, kSegMaxClasses);
-  B200_CHECK(activation == B200_SEG_LOGSOFTMAX || activation == B200_SEG_SIGMOID, B200_ERR_INVALID,
-             "unknown classifier activation %d (B200_SEG_LOGSOFTMAX = 0, B200_SEG_SIGMOID = 1)", (int)activation);
-  B200_CHECK(w->lstm_layers >= 1 && w->lstm_layers <= 4, B200_ERR_INVALID, "lstm_layers=%d unsupported",
-             (int)w->lstm_layers);
+  int rc;
+  if ((rc = check_head(w->lstm_layers, num_classes, activation))) return rc;
   B200_CHECK(w->num_layers >= 1 && w->num_layers <= kSslLayers, B200_ERR_INVALID, "num_layers=%d unsupported (1 .. 12)",
              (int)w->num_layers);
   B200_CHECK(w->conv0_weight && w->conv0_norm_weight && w->conv0_norm_bias && w->proj_norm_weight &&
@@ -810,10 +860,6 @@ int b200_ssl_load(b200_ctx* ctx, const b200_ssl_weights* w, int32_t num_classes,
   X.loaded = false;
   release_weights(ctx, &ctx->owned_ssl);
   X.head = SegWeights();
-  X.head.lstm_layers = w->lstm_layers;
-  X.head.num_classes = num_classes;
-  X.head.activation = activation == B200_SEG_SIGMOID ? kSegSigmoid : kSegLogSoftmax;
-  int rc;
   auto up = [&](const float* src, size_t n, float** dst) {
     return upload(ctx, std::vector<float>(src, src + n), dst);
   };
@@ -882,76 +928,21 @@ int b200_ssl_load(b200_ctx* ctx, const b200_ssl_weights* w, int32_t num_classes,
     if ((rc = up(L.final_layer_norm_weight, D, &Y.ln2_w))) return rc;
     if ((rc = up(L.final_layer_norm_bias, D, &Y.ln2_b))) return rc;
   }
-  if ((rc = load_lstm_head(ctx, w, D, D, num_classes, X.head))) return rc;
+  if ((rc = load_lstm_head(ctx, w, D, D, num_classes, activation, X.head))) return rc;
   X.loaded = true;
-  return B200_OK;
-}
-
-// SSeRiouSS on n windows of `window` samples, in sub-batches of at most ssl_max_batch x 160000 samples
-static int ssl_run(b200_ctx* ctx, const float* wav, const int64_t* chunk_off, const int32_t* chunk_valid, int n,
-                   int window, const SegHeadOut& out, cudaStream_t st) {
-  B200_CHECK(ctx && ctx->ssl.loaded, B200_ERR_STATE, "SSeRiouSS weights not loaded");
-  B200_CHECK(wav && chunk_off && chunk_valid && n >= 0, B200_ERR_INVALID, "bad arguments");
-  B200_CHECK(window >= kSslMinWindow, B200_ERR_INVALID,
-             "windows of %d samples are too short: SSeRiouSS needs at least %d samples (one WavLM frame)", window,
-             kSslMinWindow);
-  const int64_t budget = (int64_t)ctx->ssl_max_batch * kChunk;
-  B200_CHECK(window <= budget, B200_ERR_INVALID,
-             "a window of %d samples is longer than the %lld samples of one SSeRiouSS sub-batch (ssl_max_batch %d x "
-             "160000): set the option ssl_max_batch to at least %lld, or segment shorter excerpts",
-             window, (long long)budget, ctx->ssl_max_batch, (long long)((window + kChunk - 1) / kChunk));
-  if (n == 0) return B200_OK;
-  CtxScope scope(ctx);
-  const SslGeom geom = ssl_geom(window);
-  const int T = geom.T;
-  const int nbmax = (int)std::min<int64_t>(std::min<int64_t>(n, budget / window), 65535);
-  const size_t x0_bytes = align_up((size_t)nbmax * T * kSslDim * sizeof(float), 1024);
-  const size_t fe_b = ssl_workspace_bytes(geom, nbmax), lstm_b = lstm_workspace_bytes(nbmax, T, kSslDim);
-  int rc = ensure_ws(ctx, x0_bytes + std::max(fe_b, lstm_b) + 4096);   // the LSTM reuses the front end's region
-  if (rc) return rc;
-  if ((rc = push_meta(ctx, chunk_off, chunk_valid, n, st, window))) return rc;
-  float* x0 = reinterpret_cast<float*>(ctx->ws);
-  void* region = reinterpret_cast<char*>(ctx->ws) + x0_bytes;
-  const SslWeights& X = ctx->ssl;
-  for (int c0 = 0; c0 < n; c0 += nbmax) {
-    const int nb = (n - c0) < nbmax ? (n - c0) : nbmax;
-    if ((rc = ssl_frontend_forward(X, geom, wav, ctx->d_off + c0, ctx->d_valid + c0, nb, region, x0, ctx->num_sms, st)))
-      return rc;
-    const size_t row0 = (size_t)c0 * T, K = X.head.num_classes;
-    SegHeadOut sub;
-    sub.cls = out.cls ? out.cls + row0 : nullptr;
-    sub.logp = out.logp ? out.logp + row0 * K : nullptr;
-    sub.scores = out.scores ? out.scores + row0 * K : nullptr;
-    sub.max_scores = out.max_scores ? out.max_scores + row0 : nullptr;
-    if ((rc = lstm_head_forward(X.head, x0, nb, T, region, sub, ctx->num_sms, ctx->seg_gemm_impl, ctx->seg_rec_impl,
-                                st)))
-      return rc;
-  }
   return B200_OK;
 }
 
 int b200_ssl_forward_window(b200_ctx* ctx, const float* wav, const int64_t* chunk_off, const int32_t* chunk_valid,
                             int32_t num_chunks, int32_t window, uint8_t* classes, float* logp, void* stream) {
-  B200_CHECK(!(ctx && ctx->ssl.loaded && ctx->ssl.head.activation != kSegLogSoftmax), B200_ERR_INVALID,
-             "the loaded SSeRiouSS head is a sigmoid (multi-label / binary) head: call b200_ssl_forward_scores");
-  if (num_chunks == 0) return B200_OK;
-  B200_CHECK(classes != nullptr, B200_ERR_INVALID, "classes is NULL");
-  SegHeadOut out;
-  out.cls = classes;
-  out.logp = logp;
-  return ssl_run(ctx, wav, chunk_off, chunk_valid, num_chunks, window, out, (cudaStream_t)stream);
+  return seg_forward_head(ctx, SegFront::kWavLM, kSegLogSoftmax, wav, chunk_off, chunk_valid, num_chunks, window,
+                          SegHeadOut{classes, logp}, stream);
 }
 
 int b200_ssl_forward_scores(b200_ctx* ctx, const float* wav, const int64_t* chunk_off, const int32_t* chunk_valid,
                             int32_t num_chunks, int32_t window, float* scores, float* max_scores, void* stream) {
-  B200_CHECK(!(ctx && ctx->ssl.loaded && ctx->ssl.head.activation != kSegSigmoid), B200_ERR_INVALID,
-             "the loaded SSeRiouSS head is a log-softmax (powerset / mono-label) head: call b200_ssl_forward_window");
-  if (num_chunks == 0) return B200_OK;
-  B200_CHECK(scores || max_scores, B200_ERR_INVALID, "scores and max_scores are both NULL");
-  SegHeadOut out;
-  out.scores = scores;
-  out.max_scores = max_scores;
-  return ssl_run(ctx, wav, chunk_off, chunk_valid, num_chunks, window, out, (cudaStream_t)stream);
+  return seg_forward_head(ctx, SegFront::kWavLM, kSegSigmoid, wav, chunk_off, chunk_valid, num_chunks, window,
+                          SegHeadOut{nullptr, nullptr, scores, max_scores}, stream);
 }
 
 __global__ void strip_pad_kernel(const float* __restrict__ x64, float* __restrict__ out, size_t rows) {
@@ -969,7 +960,7 @@ int b200_sincnet_forward(b200_ctx* ctx, const float* wav, const int64_t* chunk_o
   float* tmp = nullptr;
   const size_t rows = (size_t)num_chunks * kFrames;
   B200_CUDA_OK(cudaMalloc((void**)&tmp, rows * 64 * sizeof(float)));
-  int rc = seg_run(ctx, wav, chunk_off, chunk_valid, num_chunks, kChunk, SegHeadOut(), tmp, st);
+  int rc = seg_run(ctx, SegFront::kSincNet, wav, chunk_off, chunk_valid, num_chunks, kChunk, SegHeadOut(), tmp, st);
   if (rc == B200_OK) {
     rc = launch(strip_pad_kernel, (unsigned)((rows * 60 + 255) / 256), 256, 0, st, tmp, out, rows);
     cudaStreamSynchronize(st);

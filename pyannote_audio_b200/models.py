@@ -234,36 +234,30 @@ class _SincNetParams(nn.Module):
                                      nn.InstanceNorm1d(60, affine=True)])
 
 
-class PyanNet(Model):
-    """SincNet > LSTM > Feed forward > Classifier, community-1 trunk (1-4 BiLSTM layers of 128, 2x128 linear) with
-    any head of 1 to 32 classes: log-softmax for powerset / mono-label problems, sigmoid for binary and multi-label
-    problems (core/model.py:271-300)."""
+class _SegmentationModel(Model):
+    """A front end, then the head PyanNet and SSeRiouSS share: 1-4 BiLSTM layers of 128, 2 linear layers of 128 and a
+    classifier of 1 to 32 classes, log-softmax for powerset / mono-label problems, sigmoid for binary and multi-label
+    problems (core/model.py:271-300).  A subclass holds its front-end modules and defines KERNEL / STRIDE (the front
+    end's convolutions), num_frames and check_window; its _SLOT ("seg" | "ssl") names its ops.Context head."""
 
-    _SLOT = "seg"
-    _HPARAMS = ("sincnet", "lstm", "linear", "sample_rate", "num_channels")
-    KERNEL = [251, 3, 5, 3, 5, 3]
-    STRIDE = [10, 3, 1, 3, 1, 3]
-
-    def __init__(self, sincnet: Optional[dict] = None, lstm: Optional[dict] = None, linear: Optional[dict] = None,
-                 sample_rate: int = 16000, num_channels: int = 1, duration: float = 10.0):
-        super().__init__(sample_rate=sample_rate, num_channels=num_channels)
-        if sample_rate != 16000:
-            raise NotImplementedError("SincNet only supports 16kHz audio for now.")
+    def _head_hparams(self, lstm: Optional[dict], linear: Optional[dict]):
+        """(lstm, linear) hyper-parameters with the defaults filled in; a head shape without a kernel is refused."""
         lstm_hp = {"hidden_size": 128, "num_layers": 4, "bidirectional": True, "monolithic": True, "dropout": 0.0}
         lstm_hp.update(lstm or {})
         linear_hp = {"hidden_size": 128, "num_layers": 2}
         linear_hp.update(linear or {})
-        sinc_hp = {"stride": 10}
-        sinc_hp.update(sincnet or {})
         if (lstm_hp["hidden_size"], lstm_hp["bidirectional"], lstm_hp["monolithic"]) != (128, True, True) or \
-                not (1 <= lstm_hp["num_layers"] <= 4) or (linear_hp["hidden_size"], linear_hp["num_layers"]) != (128, 2) \
-                or sinc_hp["stride"] != 10:
-            raise NotImplementedError("the CUDA kernels implement the community-1 PyanNet shape only: "
-                                      "SincNet stride 10, 1-4 bidirectional LSTM layers of 128, 2 linear layers of 128")
-        self.hparams.sincnet, self.hparams.lstm, self.hparams.linear = sinc_hp, lstm_hp, linear_hp
-        self.sincnet = _SincNetParams()
-        self.lstm = nn.LSTM(60, hidden_size=128, num_layers=lstm_hp["num_layers"], bidirectional=True,
-                            batch_first=True)
+                not (1 <= lstm_hp["num_layers"] <= 4) or (linear_hp["hidden_size"], linear_hp["num_layers"]) != (128, 2):
+            raise NotImplementedError(f"the CUDA kernels implement {type(self).__name__} with the community-1 head "
+                                      f"shape only: 1-4 monolithic bidirectional LSTM layers of 128, 2 linear layers "
+                                      f"of 128")
+        return lstm_hp, linear_hp
+
+    def _build_head(self, in_features: int, duration: float):
+        """The head's modules after the front end's (the state-dict order): lstm on ``in_features`` inputs, linear,
+        and the classifier of community-1's powerset specifications."""
+        self.lstm = nn.LSTM(in_features, hidden_size=128, num_layers=self.hparams.lstm["num_layers"],
+                            bidirectional=True, batch_first=True)
         self.linear = nn.ModuleList([nn.Linear(256, 128), nn.Linear(128, 128)])
         self.specifications = Specifications(problem=Problem.MONO_LABEL_CLASSIFICATION, resolution=Resolution.FRAME,
                                              duration=duration, warm_up=(0.0, 0.0),
@@ -297,12 +291,6 @@ class PyanNet(Model):
         specs = self.specifications
         return specs.num_powerset_classes if specs.powerset else len(specs.classes)
 
-    def num_frames(self, num_samples: int) -> int:
-        n = num_samples
-        for k, s in zip(self.KERNEL, self.STRIDE):
-            n = _conv1d_num_frames(n, k, s)
-        return n
-
     def receptive_field_size(self, num_frames: int = 1) -> int:
         rf = num_frames
         for k, s in reversed(list(zip(self.KERNEL, self.STRIDE))):
@@ -315,38 +303,68 @@ class PyanNet(Model):
             c = c * s + (k - 1) // 2
         return c
 
+    def forward_chunks(self, wav: torch.Tensor, chunk_off, chunk_valid, return_logp: bool = False, out=None,
+                       window: int = ops.CHUNK, reduce_max: bool = False):
+        """Hot-path entry: windows of ``window`` samples addressed inside one resident device waveform (no unfold
+        copy) -> classes (chunks, num_frames(window)) uint8 for a log-softmax head, sigmoid scores
+        (chunks, num_frames(window), dimension) float32 (or their per-frame maximum with ``reduce_max``) for a
+        sigmoid head (ops.Context.seg_forward / ssl_forward)."""
+        self.check_window(window)
+        ctx_forward = getattr(self._ctx(), self._SLOT + "_forward")           # seg_forward | ssl_forward
+        return ctx_forward(wav, chunk_off, chunk_valid, return_logp=return_logp, out=out, window=window,
+                           reduce_max=reduce_max)
+
+    def forward(self, waveforms: torch.Tensor) -> torch.Tensor:
+        """waveforms (batch, channel, samples), samples at least check_window's minimum -> (batch,
+        num_frames(samples), dimension): log-probabilities of a log-softmax head, sigmoid scores of a sigmoid head."""
+        b, c, s = waveforms.shape
+        if c != 1:
+            raise ValueError(f"{type(self).__name__} kernels expect mono waveforms, got {c} channels")
+        flat = waveforms.to(device=self.device, dtype=torch.float32).reshape(-1).contiguous()
+        off = np.arange(b, dtype=np.int64) * s
+        valid = np.full(b, s, dtype=np.int32)
+        if ops.seg_activation(self.specifications) == ops.SEG_SIGMOID:
+            return self.forward_chunks(flat, off, valid, window=s)
+        _, logp = self.forward_chunks(flat, off, valid, return_logp=True, window=s)
+        return logp
+
+
+class PyanNet(_SegmentationModel):
+    """SincNet > LSTM > Feed forward > Classifier, community-1 trunk (1-4 BiLSTM layers of 128, 2x128 linear) with
+    any head of 1 to 32 classes: log-softmax for powerset / mono-label problems, sigmoid for binary and multi-label
+    problems (core/model.py:271-300)."""
+
+    _SLOT = "seg"
+    _HPARAMS = ("sincnet", "lstm", "linear", "sample_rate", "num_channels")
+    KERNEL = [251, 3, 5, 3, 5, 3]
+    STRIDE = [10, 3, 1, 3, 1, 3]
+
+    def __init__(self, sincnet: Optional[dict] = None, lstm: Optional[dict] = None, linear: Optional[dict] = None,
+                 sample_rate: int = 16000, num_channels: int = 1, duration: float = 10.0):
+        super().__init__(sample_rate=sample_rate, num_channels=num_channels)
+        if sample_rate != 16000:
+            raise NotImplementedError("SincNet only supports 16kHz audio for now.")
+        sinc_hp = {"stride": 10}
+        sinc_hp.update(sincnet or {})
+        if sinc_hp["stride"] != 10:
+            raise NotImplementedError("the CUDA kernels implement the community-1 PyanNet shape only: SincNet stride 10")
+        lstm_hp, linear_hp = self._head_hparams(lstm, linear)
+        self.hparams.sincnet, self.hparams.lstm, self.hparams.linear = sinc_hp, lstm_hp, linear_hp
+        self.sincnet = _SincNetParams()
+        self._build_head(60, duration)
+
+    def num_frames(self, num_samples: int) -> int:
+        n = num_samples
+        for k, s in zip(self.KERNEL, self.STRIDE):
+            n = _conv1d_num_frames(n, k, s)
+        return n
+
     def check_window(self, num_samples: int):
         """Refuses windows too short for the kernels (Inference checks its window with this)."""
         ops.check_seg_window(num_samples)
 
     def _upload(self, ctx):
         ctx.load_segmentation(self.state_dict(), self.specifications)
-
-    def forward_chunks(self, wav: torch.Tensor, chunk_off, chunk_valid, return_logp: bool = False, out=None,
-                       window: int = ops.CHUNK, reduce_max: bool = False):
-        """Hot-path entry: windows of ``window`` samples addressed inside one resident device waveform (no unfold
-        copy) -> classes (chunks, num_frames(window)) uint8 for a log-softmax head, sigmoid scores
-        (chunks, num_frames(window), dimension) float32 (or their per-frame maximum with ``reduce_max``) for a
-        sigmoid head (ops.Context.seg_forward)."""
-        ops.check_seg_window(window)
-        return self._ctx().seg_forward(wav, chunk_off, chunk_valid, return_logp=return_logp, out=out, window=window,
-                                       reduce_max=reduce_max)
-
-    def forward(self, waveforms: torch.Tensor) -> torch.Tensor:
-        """waveforms (batch, channel, samples), samples >= 1261 -> (batch, num_frames(samples), dimension):
-        log-probabilities of a log-softmax head, sigmoid scores of a sigmoid head."""
-        b, c, s = waveforms.shape
-        if c != 1:
-            raise ValueError(f"PyanNet kernels expect mono waveforms, got {c} channels")
-        ops.check_seg_window(s)
-        ctx = self._ctx()
-        flat = waveforms.to(device=ctx.device, dtype=torch.float32).reshape(-1).contiguous()
-        off = np.arange(b, dtype=np.int64) * s
-        valid = np.full(b, s, dtype=np.int32)
-        if ops.seg_activation(self.specifications) == ops.SEG_SIGMOID:
-            return ctx.seg_forward(flat, off, valid, window=s)
-        _, logp = ctx.seg_forward(flat, off, valid, return_logp=True, window=s)
-        return logp
 
 
 class _BasicBlockParams(nn.Module):
@@ -741,7 +759,7 @@ class _WavLMParams(nn.Module):
         self.encoder.transformer.layers = nn.ModuleList([_EncoderLayerParams(i == 0) for i in range(12)])
 
 
-class SSeRiouSS(Model):
+class SSeRiouSS(_SegmentationModel):
     """WavLM Base > LSTM > Feed forward > Classifier (models/segmentation/SSeRiouSS.py) with ``wav2vec`` one of
     "WAVLM_BASE" / "WAVLM_BASE_PLUS", the PyanNet LSTM / linear shape (1-4 BiLSTM layers of 128, 2 linear layers of
     128) and any head PyanNet accepts.  ``wav2vec_layer`` < 0 averages the 12 layer outputs with
@@ -767,44 +785,16 @@ class SSeRiouSS(Model):
         wav2vec_layer = int(wav2vec_layer)
         if not (wav2vec_layer < 0 or 1 <= wav2vec_layer <= 12):
             raise ValueError(f"`wav2vec_layer` must be negative or between 1 and 12, got {wav2vec_layer}")
-        lstm_hp = {"hidden_size": 128, "num_layers": 4, "bidirectional": True, "monolithic": True, "dropout": 0.0}
-        lstm_hp.update(lstm or {})
-        linear_hp = {"hidden_size": 128, "num_layers": 2}
-        linear_hp.update(linear or {})
-        if (lstm_hp["hidden_size"], lstm_hp["bidirectional"], lstm_hp["monolithic"]) != (128, True, True) or \
-                not (1 <= lstm_hp["num_layers"] <= 4) or (linear_hp["hidden_size"], linear_hp["num_layers"]) != (128, 2):
-            raise NotImplementedError("the CUDA kernels implement the PyanNet head shape only: 1-4 monolithic "
-                                      "bidirectional LSTM layers of 128, 2 linear layers of 128")
+        lstm_hp, linear_hp = self._head_hparams(lstm, linear)
         self.hparams.wav2vec, self.hparams.wav2vec_frozen = wav2vec, bool(wav2vec_frozen)
         self.hparams.wav2vec_layer, self.hparams.lstm, self.hparams.linear = wav2vec_layer, lstm_hp, linear_hp
         self.wav2vec = _WavLMParams()
         if wav2vec_layer < 0:
             self.wav2vec_weights = nn.Parameter(torch.ones(12))
-        self.lstm = nn.LSTM(768, hidden_size=128, num_layers=lstm_hp["num_layers"], bidirectional=True,
-                            batch_first=True)
-        self.linear = nn.ModuleList([nn.Linear(256, 128), nn.Linear(128, 128)])
-        self.specifications = Specifications(problem=Problem.MONO_LABEL_CLASSIFICATION, resolution=Resolution.FRAME,
-                                             duration=duration, warm_up=(0.0, 0.0),
-                                             classes=["speaker#1", "speaker#2", "speaker#3"], powerset_max_classes=2,
-                                             permutation_invariant=True)
-
-    specifications = PyanNet.specifications
-    dimension = PyanNet.dimension
+        self._build_head(768, duration)
 
     def num_frames(self, num_samples: int) -> int:
         return ops.ssl_num_frames(num_samples)
-
-    def receptive_field_size(self, num_frames: int = 1) -> int:
-        rf = num_frames
-        for k, s in reversed(list(zip(self.KERNEL, self.STRIDE))):
-            rf = 1 + (k - 1) + (rf - 1) * s
-        return rf
-
-    def receptive_field_center(self, frame: int = 0) -> int:
-        c = frame
-        for k, s in reversed(list(zip(self.KERNEL, self.STRIDE))):
-            c = c * s + (k - 1) // 2
-        return c
 
     def check_window(self, num_samples: int):
         """Refuses windows shorter than one WavLM frame (400 samples)."""
@@ -812,26 +802,3 @@ class SSeRiouSS(Model):
 
     def _upload(self, ctx):
         ctx.load_sseriouss(self.state_dict(), self.specifications, self.hparams.wav2vec_layer)
-
-    def forward_chunks(self, wav: torch.Tensor, chunk_off, chunk_valid, return_logp: bool = False, out=None,
-                       window: int = ops.CHUNK, reduce_max: bool = False):
-        """As PyanNet.forward_chunks, with ops.ssl_num_frames(window) frames per window (ops.Context.ssl_forward)."""
-        ops.check_ssl_window(window)
-        return self._ctx().ssl_forward(wav, chunk_off, chunk_valid, return_logp=return_logp, out=out, window=window,
-                                       reduce_max=reduce_max)
-
-    def forward(self, waveforms: torch.Tensor) -> torch.Tensor:
-        """waveforms (batch, channel, samples), samples >= 400 -> (batch, num_frames(samples), dimension):
-        log-probabilities of a log-softmax head, sigmoid scores of a sigmoid head."""
-        b, c, s = waveforms.shape
-        if c != 1:
-            raise ValueError(f"SSeRiouSS kernels expect mono waveforms, got {c} channels")
-        ops.check_ssl_window(s)
-        ctx = self._ctx()
-        flat = waveforms.to(device=ctx.device, dtype=torch.float32).reshape(-1).contiguous()
-        off = np.arange(b, dtype=np.int64) * s
-        valid = np.full(b, s, dtype=np.int32)
-        if ops.seg_activation(self.specifications) == ops.SEG_SIGMOID:
-            return ctx.ssl_forward(flat, off, valid, window=s)
-        _, logp = ctx.ssl_forward(flat, off, valid, return_logp=True, window=s)
-        return logp

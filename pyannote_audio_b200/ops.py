@@ -165,6 +165,34 @@ def _state_dict_reader(sd: Mapping[str, torch.Tensor]):
     return f
 
 
+def _head_of(sd: Mapping[str, torch.Tensor], specifications) -> tuple:
+    """(classes, activation) of a PyanNet or SSeRiouSS head: ``classifier.weight``'s K rows (1 .. 32), and the
+    activation of ``specifications`` (sigmoid for binary / multi-label problems), log-softmax without them."""
+    num_classes = int(sd["classifier.weight"].shape[0])
+    check_seg_classes(num_classes)
+    return num_classes, SEG_LOGSOFTMAX if specifications is None else seg_activation(specifications)
+
+
+def _fill_head(w, sd: Mapping[str, torch.Tensor], f):
+    """The ``lstm.*``, ``linear.*`` and ``classifier.*`` fields that SegWeights (PyanNet) and SslWeights (SSeRiouSS)
+    share; the LSTM depth comes from the keys."""
+    layers = 0
+    while f"lstm.weight_ih_l{layers}" in sd:
+        layers += 1
+    w.lstm_layers = layers
+    for layer in range(layers):
+        for d, suffix in enumerate(("", "_reverse")):
+            w.lstm_w_ih[layer * 2 + d] = f(f"lstm.weight_ih_l{layer}{suffix}")
+            w.lstm_w_hh[layer * 2 + d] = f(f"lstm.weight_hh_l{layer}{suffix}")
+            w.lstm_b_ih[layer * 2 + d] = f(f"lstm.bias_ih_l{layer}{suffix}")
+            w.lstm_b_hh[layer * 2 + d] = f(f"lstm.bias_hh_l{layer}{suffix}")
+    for i in range(2):
+        w.linear_weight[i] = f(f"linear.{i}.weight")
+        w.linear_bias[i] = f(f"linear.{i}.bias")
+    w.classifier_weight = f("classifier.weight")
+    w.classifier_bias = f("classifier.bias")
+
+
 def _fill_sincnet(w, sd: Mapping[str, torch.Tensor], f):
     """The ``sincnet.*`` fields that SegWeights (PyanNet) and XvecWeights (XVectorSincNet) share."""
     w.wav_norm_weight = float(sd["sincnet.wav_norm1d.weight"].reshape(-1)[0])
@@ -216,16 +244,15 @@ class Context:
         h = C.c_void_p()
         _lib.check(self.lib.b200_ctx_create(C.byref(h), self.device.index))
         self._h = h
-        self.seg_loaded = False
-        self.seg_classes = CLASSES           # classifier head of the loaded PyanNet: K classes, log-softmax or sigmoid
-        self.seg_activation = SEG_LOGSOFTMAX
+        # PyanNet ("seg") and SSeRiouSS ("ssl") slots: the slots whose last load succeeded, and per slot the
+        # (classes, activation) of the last head the library accepted.  A refused load keeps that entry: the library
+        # checks a head before it releases the resident one, so it may go on running the previous head.
+        self._loaded = set()
+        self._heads = {}
         self.emb_loaded = False
         self.emb_channels = 256   # trunk output channels of the loaded embedding model: 256 (ResNet34) or 1024
         self.xvec_loaded = False
         self.xvec_dimension = 512
-        self.ssl_loaded = False
-        self.ssl_classes = CLASSES           # classifier head of the loaded SSeRiouSS
-        self.ssl_activation = SEG_LOGSOFTMAX
         self.owners = {}    # slot ("seg" | "emb" | "xvec" | "ssl") -> stamp of the model whose weights are resident
         # A/B knob for scripts (like B200_CONV_IMPL / B200_EMB_MAX_BATCH / B200_SEG_MAX_BATCH, which the library
         # reads itself): B200_OPTIONS="key=value,..."
@@ -246,6 +273,14 @@ class Context:
             self.close()
         except Exception:
             pass
+
+    @property
+    def seg_loaded(self) -> bool:
+        return "seg" in self._loaded
+
+    @property
+    def ssl_loaded(self) -> bool:
+        return "ssl" in self._loaded
 
     def set_option(self, key: str, value: int):
         _lib.check(self.lib.b200_ctx_set_option(self._h, key.encode(), int(value)))
@@ -270,31 +305,12 @@ class Context:
     def load_segmentation(self, sd: Mapping[str, torch.Tensor], specifications=None):
         """PyanNet weights.  The head has ``classifier.weight``'s K rows (1 .. 32); its activation comes from
         ``specifications`` (sigmoid for binary / multi-label problems), log-softmax without them."""
-        num_classes = int(sd["classifier.weight"].shape[0])
-        check_seg_classes(num_classes)
-        activation = SEG_LOGSOFTMAX if specifications is None else seg_activation(specifications)
+        head = _head_of(sd, specifications)
         f = _state_dict_reader(sd)
         w = _lib.SegWeights()
         _fill_sincnet(w, sd, f)
-        layers = 0
-        while f"lstm.weight_ih_l{layers}" in sd:
-            layers += 1
-        w.lstm_layers = layers
-        for layer in range(layers):
-            for d, suffix in enumerate(("", "_reverse")):
-                w.lstm_w_ih[layer * 2 + d] = f(f"lstm.weight_ih_l{layer}{suffix}")
-                w.lstm_w_hh[layer * 2 + d] = f(f"lstm.weight_hh_l{layer}{suffix}")
-                w.lstm_b_ih[layer * 2 + d] = f(f"lstm.bias_ih_l{layer}{suffix}")
-                w.lstm_b_hh[layer * 2 + d] = f(f"lstm.bias_hh_l{layer}{suffix}")
-        for i in range(2):
-            w.linear_weight[i] = f(f"linear.{i}.weight")
-            w.linear_bias[i] = f(f"linear.{i}.bias")
-        w.classifier_weight = f("classifier.weight")
-        w.classifier_bias = f("classifier.bias")
-        self.owners.pop("seg", None)          # whoever uploaded before no longer owns the slot
-        self.seg_loaded = False
-        _lib.check(self.lib.b200_seg_load_head(self._h, C.byref(w), num_classes, activation))
-        self.seg_loaded, self.seg_classes, self.seg_activation = True, num_classes, activation
+        _fill_head(w, sd, f)
+        self._load_head("seg", "b200_seg_load_head", w, head)
 
     def load_embedding(self, sd: Mapping[str, torch.Tensor]):
         f = _state_dict_reader(sd)
@@ -358,9 +374,7 @@ class Context:
         the module's keys; the positional conv's weight norm is folded here (either spelling).  The LSTM reads the
         softmax(wav2vec_weights)-weighted average of the 12 layer outputs for ``wav2vec_layer`` < 0, else the output
         of layer ``wav2vec_layer`` (1 .. 12), and then only that many layers run."""
-        num_classes = int(sd["classifier.weight"].shape[0])
-        check_seg_classes(num_classes)
-        activation = SEG_LOGSOFTMAX if specifications is None else seg_activation(specifications)
+        head = _head_of(sd, specifications)
         f = _state_dict_reader(sd)
         w = _lib.SslWeights()
         fe, enc = "wav2vec.feature_extractor.conv_layers.", "wav2vec.encoder."
@@ -409,25 +423,16 @@ class Context:
         for layer in range(num_layers):
             for field, key in names.items():
                 setattr(w.layer[layer], field, f(f"{tr}layers.{layer}.{key}"))
-        layers = 0
-        while f"lstm.weight_ih_l{layers}" in sd:
-            layers += 1
-        w.lstm_layers = layers
-        for layer in range(layers):
-            for d, suffix in enumerate(("", "_reverse")):
-                w.lstm_w_ih[layer * 2 + d] = f(f"lstm.weight_ih_l{layer}{suffix}")
-                w.lstm_w_hh[layer * 2 + d] = f(f"lstm.weight_hh_l{layer}{suffix}")
-                w.lstm_b_ih[layer * 2 + d] = f(f"lstm.bias_ih_l{layer}{suffix}")
-                w.lstm_b_hh[layer * 2 + d] = f(f"lstm.bias_hh_l{layer}{suffix}")
-        for i in range(2):
-            w.linear_weight[i] = f(f"linear.{i}.weight")
-            w.linear_bias[i] = f(f"linear.{i}.bias")
-        w.classifier_weight = f("classifier.weight")
-        w.classifier_bias = f("classifier.bias")
-        self.owners.pop("ssl", None)
-        self.ssl_loaded = False
-        _lib.check(self.lib.b200_ssl_load(self._h, C.byref(w), num_classes, activation))
-        self.ssl_loaded, self.ssl_classes, self.ssl_activation = True, num_classes, activation
+        _fill_head(w, sd, f)
+        self._load_head("ssl", "b200_ssl_load", w, head)
+
+    def _load_head(self, slot: str, entry: str, w, head):
+        """``entry``(ctx, w, classes, activation) into ``slot`` ("seg" | "ssl"), ``head`` = (classes, activation)."""
+        self.owners.pop(slot, None)           # whoever uploaded before no longer owns the slot
+        self._loaded.discard(slot)
+        _lib.check(getattr(self.lib, entry)(self._h, C.byref(w), *head))
+        self._loaded.add(slot)
+        self._heads[slot] = head
 
     def _load_bottleneck(self, sd, f, conv_bn):
         """WeSpeakerResNet152 / 221 / 293 (Bottleneck blocks, resnet.py:148-212): the block counts come from the keys."""
@@ -505,49 +510,40 @@ class Context:
         first valid[i] samples are real (zeros after); F = seg_num_frames(window), K the loaded head's classes.
         Log-softmax head -> classes (n, F) uint8 (+ log-probabilities (n, F, K)).  Sigmoid head -> scores (n, F, K)
         float32, or with ``reduce_max`` their per-frame maximum (n, F, 1) computed in the same kernel."""
-        check_seg_window(window)
-        window = int(window)
-        off, valid = self._chunks(wav, chunk_off, chunk_valid)
-        n = len(off)
-        F = seg_num_frames(window)
-        K = self.seg_classes
-        if self.seg_activation == SEG_SIGMOID:
-            if return_logp:
-                raise ValueError("the loaded segmentation head is a sigmoid head: it has scores, not log-probabilities")
-            scores = self._out(out, (n, F, 1 if reduce_max else K), torch.float32)
-            self._call("b200_seg_forward_scores", _ptr(wav), off.ctypes.data, valid.ctypes.data, n, window,
-                       None if reduce_max else _ptr(scores), _ptr(scores) if reduce_max else None)
-            return scores
-        if reduce_max:
-            raise ValueError("reduce_max needs a sigmoid segmentation head (use powerset_speech for a powerset head)")
-        cls = self._out(out, (n, F), torch.uint8)
-        logp = torch.empty((n, F, K), dtype=torch.float32, device=self.device) if return_logp else None
-        self._call("b200_seg_forward_window", _ptr(wav), off.ctypes.data, valid.ctypes.data, n, window, _ptr(cls),
-                   _ptr(logp))
-        return (cls, logp) if return_logp else cls
+        return self._head_forward("seg", wav, chunk_off, chunk_valid, return_logp, out, window, reduce_max)
 
     def ssl_forward(self, wav, chunk_off, chunk_valid, return_logp=False, out: Optional[torch.Tensor] = None,
                     window: int = CHUNK, reduce_max: bool = False):
         """SSeRiouSS on windows of ``window`` samples (>= 400), arguments and outputs as in seg_forward with
         F = ssl_num_frames(window) frames per window."""
-        check_ssl_window(window)
+        return self._head_forward("ssl", wav, chunk_off, chunk_valid, return_logp, out, window, reduce_max)
+
+    # per slot: the window check, frames per window, the model's name in messages and its entry points' prefix
+    _HEAD_SLOTS = {"seg": (check_seg_window, seg_num_frames, "segmentation", "b200_seg"),
+                   "ssl": (check_ssl_window, ssl_num_frames, "SSeRiouSS", "b200_ssl")}
+
+    def _head_forward(self, slot, wav, chunk_off, chunk_valid, return_logp, out, window, reduce_max):
+        """seg_forward / ssl_forward on the head resident in ``slot``.  A slot the library never accepted a head for
+        takes the log-softmax path, where the library reports the missing weights."""
+        check_window, num_frames, name, prefix = self._HEAD_SLOTS[slot]
+        check_window(window)
         window = int(window)
         off, valid = self._chunks(wav, chunk_off, chunk_valid)
         n = len(off)
-        F = ssl_num_frames(window)
-        K = self.ssl_classes
-        if self.ssl_activation == SEG_SIGMOID:
+        F = num_frames(window)
+        K, activation = self._heads.get(slot, (CLASSES, SEG_LOGSOFTMAX))
+        if activation == SEG_SIGMOID:
             if return_logp:
-                raise ValueError("the loaded SSeRiouSS head is a sigmoid head: it has scores, not log-probabilities")
+                raise ValueError(f"the loaded {name} head is a sigmoid head: it has scores, not log-probabilities")
             scores = self._out(out, (n, F, 1 if reduce_max else K), torch.float32)
-            self._call("b200_ssl_forward_scores", _ptr(wav), off.ctypes.data, valid.ctypes.data, n, window,
+            self._call(prefix + "_forward_scores", _ptr(wav), off.ctypes.data, valid.ctypes.data, n, window,
                        None if reduce_max else _ptr(scores), _ptr(scores) if reduce_max else None)
             return scores
         if reduce_max:
             raise ValueError("reduce_max needs a sigmoid segmentation head (use powerset_speech for a powerset head)")
         cls = self._out(out, (n, F), torch.uint8)
         logp = torch.empty((n, F, K), dtype=torch.float32, device=self.device) if return_logp else None
-        self._call("b200_ssl_forward_window", _ptr(wav), off.ctypes.data, valid.ctypes.data, n, window, _ptr(cls),
+        self._call(prefix + "_forward_window", _ptr(wav), off.ctypes.data, valid.ctypes.data, n, window, _ptr(cls),
                    _ptr(logp))
         return (cls, logp) if return_logp else cls
 
