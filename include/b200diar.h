@@ -161,6 +161,28 @@ typedef struct b200_xvec_weights {
  * side by side.  fp16 (hi, lo) splits and the BatchNorm scale / shift are made here, once. */
 int b200_xvec_load(b200_ctx* ctx, const b200_xvec_weights* w);
 
+/* XVectorMFCC (models/embedding/xvector.py:42-202): torchaudio's MFCC with its defaults at 16 kHz (n_mfcc 40, DCT-II
+ * "ortho", log_mels False: centred reflect-padded STFT with n_fft 400 and hop 200, power spectrum, 128-filter mel bank,
+ * AmplitudeToDB("power", top_db 80) over each whole utterance, DCT) in front of the TDNN stack, pooling and Linear of
+ * XVectorSincNet (same fields and meaning as in b200_xvec_weights; tdnns.0 has 40 input channels).  The three MFCC
+ * buffers are used as loaded. */
+typedef struct b200_xvec_mfcc_weights {
+  const float* dct_mat;                       /* mfcc.dct_mat [128][40]                                 */
+  const float* window;                        /* mfcc.MelSpectrogram.spectrogram.window [400]           */
+  const float* mel_fb;                        /* mfcc.MelSpectrogram.mel_scale.fb [201][128]            */
+  const float* tdnn_weight[5];                /* tdnns.{0,3,6,9,12}.weight [C_out][C_in][kernel]        */
+  const float* tdnn_bias[5];                  /* tdnns.{0,3,6,9,12}.bias [C_out]                        */
+  const float* bn_weight[5];                  /* tdnns.{2,5,8,11,14}.weight [C_out]                     */
+  const float* bn_bias[5];
+  const float* bn_mean[5];                    /* tdnns.{2,5,8,11,14}.running_mean                       */
+  const float* bn_var[5];                     /* tdnns.{2,5,8,11,14}.running_var                        */
+  int32_t dimension;                          /* embedding size                                         */
+  const float* embedding_weight;              /* embedding.weight [dimension][3000]                     */
+  const float* embedding_bias;                /* [dimension]                                            */
+} b200_xvec_mfcc_weights;
+/* Loads XVectorMFCC into the ctx's own slot, next to the PyanNet, WeSpeaker, XVectorSincNet and SSeRiouSS slots. */
+int b200_xvec_mfcc_load(b200_ctx* ctx, const b200_xvec_mfcc_weights* w);
+
 /* SSeRiouSS (models/segmentation/SSeRiouSS.py) on the WavLM Base front end (torchaudio WAVLM_BASE / WAVLM_BASE_PLUS:
  * conv feature extractor without conv biases and GroupNorm on conv 0, 768-wide post-LN transformer of 12 layers with
  * 12 heads and gated relative position bias), then the PyanNet head: 1-4 BiLSTM layers of 128 with 768 inputs, two
@@ -335,6 +357,15 @@ int b200_emb_forward_embedding(b200_ctx* ctx, const float* frames, int32_t B, in
  * samples; one utterance longer than that (43.9 min with the default) returns B200_STATUS_INVALID. */
 int b200_xvec_forward(b200_ctx* ctx, const float* wav, const int64_t* off, int64_t num_samples, int32_t num_utts,
                       const float* weights, int32_t num_speakers, int32_t num_weights, float* emb, void* stream);
+/* XVectorMFCC.forward (models/embedding/xvector.py:185-202) on utterances of one length num_samples >= 2800,
+ * arguments, pooling and sub-batches as in b200_xvec_forward.  MFCC gives F = 1 + num_samples / 200 frames, the TDNN
+ * stack T = F - 14. */
+int b200_xvec_mfcc_forward(b200_ctx* ctx, const float* wav, const int64_t* off, int64_t num_samples, int32_t num_utts,
+                           const float* weights, int32_t num_speakers, int32_t num_weights, float* emb, void* stream);
+/* The MFCC front end of the loaded XVectorMFCC alone: utterances as in b200_xvec_mfcc_forward (num_samples > 200) ->
+ * out fp32 DEVICE [num_utts][1 + num_samples / 200][40] (frame-major, the transpose of torchaudio's layout). */
+int b200_xvec_mfcc_features(b200_ctx* ctx, const float* wav, const int64_t* off, int64_t num_samples, int32_t num_utts,
+                            float* out, void* stream);
 /* StatsPool.forward (models/blocks/pooling.py:76-130): seq[B][F][T], weights[B][S][Tw] or NULL -> out[B][S][2F]. */
 int b200_stats_pool(b200_ctx* ctx, const float* seq, const float* weights, float* out, int32_t B, int32_t F, int32_t T,
                     int32_t S, int32_t Tw, void* stream);

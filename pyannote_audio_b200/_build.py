@@ -13,7 +13,7 @@ LIBDIR = os.path.join(HERE, "lib")
 LIB = os.path.join(LIBDIR, "libb200diar.so")
 SOURCES = ["err.cu", "api.cu", "sgemm.cu", "seg_sincnet.cu", "seg_conv_wg.cu", "seg_lstm.cu", "seg_lstm_wg.cu", "emb_conv.cu",
            "emb_misc.cu", "post.cu", "audio.cu", "cluster.cu", "gemm_tc.cu",
-           "ssl_wavlm.cu"]
+           "ssl_wavlm.cu", "xvec_mfcc.cu"]
 NVCC_FLAGS = ["-gencode", "arch=compute_90a,code=sm_90a", "-lineinfo", "-O3", "-std=c++17",
               "-Xcompiler", "-fPIC", "-Xcompiler", "-O2"]
 

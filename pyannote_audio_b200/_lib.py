@@ -55,6 +55,15 @@ class XvecWeights(C.Structure):
     ]
 
 
+class XvecMfccWeights(C.Structure):
+    _fields_ = [
+        ("dct_mat", c_float_p), ("window", c_float_p), ("mel_fb", c_float_p),
+        ("tdnn_weight", c_float_p * 5), ("tdnn_bias", c_float_p * 5),
+        ("bn_weight", c_float_p * 5), ("bn_bias", c_float_p * 5), ("bn_mean", c_float_p * 5), ("bn_var", c_float_p * 5),
+        ("dimension", C.c_int32), ("embedding_weight", c_float_p), ("embedding_bias", c_float_p),
+    ]
+
+
 class SslLayerWeights(C.Structure):
     _fields_ = [(name, c_float_p) for name in (
         "in_proj_weight", "in_proj_bias", "out_proj_weight", "out_proj_bias", "gru_weight", "gru_bias", "gru_const",
@@ -100,6 +109,11 @@ _PROTOS = {
     "b200_xvec_load": (C.c_int, [C.c_void_p, C.POINTER(XvecWeights)]),
     "b200_xvec_forward": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_int64, C.c_int32, C.c_void_p, C.c_int32,
                                     C.c_int32, C.c_void_p, C.c_void_p]),
+    "b200_xvec_mfcc_load": (C.c_int, [C.c_void_p, C.POINTER(XvecMfccWeights)]),
+    "b200_xvec_mfcc_forward": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_int64, C.c_int32, C.c_void_p,
+                                         C.c_int32, C.c_int32, C.c_void_p, C.c_void_p]),
+    "b200_xvec_mfcc_features": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_int64, C.c_int32, C.c_void_p,
+                                          C.c_void_p]),
     "b200_ssl_load": (C.c_int, [C.c_void_p, C.POINTER(SslWeights), C.c_int32, C.c_int32]),
     "b200_ssl_forward_window": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_int32, C.c_int32,
                                           C.c_void_p, C.c_void_p, C.c_void_p]),

@@ -15,14 +15,17 @@
 
 using namespace b200;
 
-// XVectorSincNet (models/embedding/xvector.py:205-349): the SincNet front end, five TDNN layers (Conv1d -> LeakyReLU
-// -> eval BatchNorm1d) as implicit GEMMs on gemm_tc_split, statistics pooling and the embedding Linear
+// XVectorSincNet (models/embedding/xvector.py:205-349) and XVectorMFCC (xvector.py:42-202): a front end (SincNet or
+// MFCC), five TDNN layers (Conv1d -> LeakyReLU -> eval BatchNorm1d) as implicit GEMMs on gemm_tc_split, statistics
+// pooling and the embedding Linear
 constexpr int kXvecLayers = 5;
-constexpr int kXvecMinSamples = 4771;   // 15 SincNet frames: the TDNN stack (receptive field 15) gives one frame
-constexpr int kXvecStatsLd = 3008;      // 2 x 1500 statistics, padded to whole 64-wide k-blocks
+constexpr int kXvecMinSamples = 4771;       // 15 SincNet frames: the TDNN stack (receptive field 15) gives one frame
+constexpr int kXvecMfccMinSamples = 2800;   // 15 MFCC frames
+constexpr int kXvecStatsLd = 3008;          // 2 x 1500 statistics, padded to whole 64-wide k-blocks
 struct XvecWeights {
   bool loaded = false;
-  SincNetWeights sinc;
+  SincNetWeights sinc;              // front end of the XVectorSincNet slot
+  MfccWeights mfcc;                 // front end of the XVectorMFCC slot
   int taps[kXvecLayers] = {5, 3, 3, 1, 1}, dil[kXvecLayers] = {1, 2, 3, 1, 1};
   int cin_pad[kXvecLayers] = {64, 512, 512, 512, 512}, cout_pad[kXvecLayers] = {512, 512, 512, 512, 1536};
   __half* w_hi[kXvecLayers] = {};   // [cout_pad][taps x cin_pad] fp16 (hi, lo), k = tap * cin_pad + c_in, zero padded
@@ -62,9 +65,10 @@ struct b200_ctx {
   int64_t launches = 0;
   SegWeights seg;
   EmbWeights emb;
-  XvecWeights xvec;
+  XvecWeights xvec, xvec_mfcc;
   SslWeights ssl;
-  std::vector<void*> owned_seg, owned_emb, owned_xvec, owned_ssl;   // device allocations holding the weights of each network
+  // device allocations holding the weights of each network
+  std::vector<void*> owned_seg, owned_emb, owned_xvec, owned_xvec_mfcc, owned_ssl;
   std::vector<void*>* owned = &owned_seg;    // where upload() records allocations (set by the load entry points)
   void* ws = nullptr;
   size_t ws_cap = 0;
@@ -466,6 +470,88 @@ int load_lstm_head(b200_ctx* ctx, const Wt* w, int in0, int kpad0, int num_class
   return B200_OK;
 }
 
+// The TDNN stack and embedding Linear that both x-vector loaders share (b200_xvec_weights / b200_xvec_mfcc_weights
+// fields of the same names), checked before the loader releases the resident weights
+template <class Wt>
+int check_xvec_tdnn(const Wt* w) {
+  B200_CHECK(w->dimension >= 1 && w->dimension <= 65536, B200_ERR_INVALID, "embedding dimension %d unsupported",
+             (int)w->dimension);
+  for (int l = 0; l < kXvecLayers; ++l)
+    B200_CHECK(w->tdnn_weight[l] && w->tdnn_bias[l] && w->bn_weight[l] && w->bn_bias[l] && w->bn_mean[l] && w->bn_var[l],
+               B200_ERR_INVALID, "tdnns.%d / tdnns.%d missing", 3 * l, 3 * l + 2);
+  B200_CHECK(w->embedding_weight && w->embedding_bias, B200_ERR_INVALID, "embedding missing");
+  return B200_OK;
+}
+
+// cin0: the front end's features per frame (60 SincNet, 40 MFCC), zero padded to cin_pad[0] = 64
+template <class Wt>
+int load_xvec_tdnn(b200_ctx* ctx, const Wt* w, int cin0, XvecWeights& X) {
+  int rc;
+  const int cin[kXvecLayers] = {cin0, 512, 512, 512, 512}, cout[kXvecLayers] = {512, 512, 512, 512, 1500};
+  for (int l = 0; l < kXvecLayers; ++l) {
+    const int k = X.taps[l], cp = X.cin_pad[l], np = X.cout_pad[l], K = k * cp;
+    std::vector<float> wt((size_t)np * K, 0.f), bias(np, 0.f), scale(np, 0.f), shift(np, 0.f);
+    for (int co = 0; co < cout[l]; ++co) {
+      for (int ci = 0; ci < cin[l]; ++ci)
+        for (int j = 0; j < k; ++j)
+          wt[(size_t)co * K + j * cp + ci] = w->tdnn_weight[l][((size_t)co * cin[l] + ci) * k + j];
+      bias[co] = w->tdnn_bias[l][co];
+      scale[co] = w->bn_weight[l][co] / std::sqrt(w->bn_var[l][co] + 1e-5f);
+      shift[co] = w->bn_bias[l][co] - w->bn_mean[l][co] * scale[co];
+    }
+    if ((rc = upload_split(ctx, wt, &X.w_hi[l], &X.w_lo[l]))) return rc;
+    if ((rc = upload(ctx, bias, &X.bias[l]))) return rc;
+    if ((rc = upload(ctx, scale, &X.scale[l]))) return rc;
+    if ((rc = upload(ctx, shift, &X.shift[l]))) return rc;
+  }
+  X.dim = w->dimension;
+  X.dim_pad = (int)ceil_div(X.dim, 128) * 128;
+  std::vector<float> ew((size_t)X.dim_pad * kXvecStatsLd, 0.f), b(X.dim_pad, 0.f);
+  for (int n = 0; n < X.dim; ++n) {
+    for (int kk = 0; kk < 3000; ++kk) ew[(size_t)n * kXvecStatsLd + kk] = w->embedding_weight[(size_t)n * 3000 + kk];
+    b[n] = w->embedding_bias[n];
+  }
+  if ((rc = upload_split(ctx, ew, &X.emb_hi, &X.emb_lo))) return rc;
+  return upload(ctx, b, &X.emb_b);
+}
+
+// The MFCC buffers in the layouts of xvec_mfcc.cu: the DFT basis with the window folded in (basis values in fp64 from
+// the fp32 window, the angle reduced exactly mod 400), every mel filter as its band of bins from the first to the last
+// nonzero weight, and dct_mat as is
+int load_mfcc(b200_ctx* ctx, const float* window, const float* mel_fb, const float* dct_mat, MfccWeights* out) {
+  B200_CHECK(window && mel_fb && dct_mat, B200_ERR_INVALID, "mfcc window / mel_fb / dct_mat missing");
+  MfccWeights& M = *out;
+  int rc;
+  std::vector<float> basis((size_t)kMfccSpecLd * 2 * kMfccRowLd, 0.f);
+  for (int k = 0; k < kMfccBins; ++k)
+    for (int s = 0; s < kMfccFft; ++s) {
+      const int j = s / kMfccHop, col = j * kMfccRowLd + s - j * kMfccHop;
+      const double a = 2.0 * M_PI * (double)((k * s) % kMfccFft) / kMfccFft;
+      basis[(size_t)k * 2 * kMfccRowLd + col] = (float)((double)window[s] * std::cos(a));
+      basis[(size_t)(kMfccSpecLd / 2 + k) * 2 * kMfccRowLd + col] = (float)((double)window[s] * std::sin(a));
+    }
+  if ((rc = upload_split(ctx, basis, &M.dft_hi, &M.dft_lo))) return rc;
+  std::vector<int> start(kMfccMels, 0), len(kMfccMels, 0), off(kMfccMels, 0);
+  std::vector<float> band;
+  for (int m = 0; m < kMfccMels; ++m) {
+    int first = -1, last = -1;
+    for (int k = 0; k < kMfccBins; ++k)
+      if (mel_fb[(size_t)k * kMfccMels + m] != 0.f) { if (first < 0) first = k; last = k; }
+    off[m] = (int)band.size();
+    if (first < 0) continue;                               // an all-zero filter: 0 energy, -100 dB
+    start[m] = first;
+    len[m] = last - first + 1;
+    for (int k = first; k <= last; ++k) band.push_back(mel_fb[(size_t)k * kMfccMels + m]);
+  }
+  band.push_back(0.f);                                     // never empty
+  if ((rc = upload(ctx, start, &M.band_start))) return rc;
+  if ((rc = upload(ctx, len, &M.band_len))) return rc;
+  if ((rc = upload(ctx, off, &M.band_off))) return rc;
+  if ((rc = upload(ctx, band, &M.band_w))) return rc;
+  std::vector<float> dct(dct_mat, dct_mat + (size_t)kMfccMels * kMfccCoefs);
+  return upload(ctx, dct, &M.dct);
+}
+
 }  // namespace
 
 extern "C" {
@@ -499,6 +585,7 @@ int b200_ctx_destroy(b200_ctx* ctx) {
   for (void* p : ctx->owned_seg) cudaFree(p);
   for (void* p : ctx->owned_emb) cudaFree(p);
   for (void* p : ctx->owned_xvec) cudaFree(p);
+  for (void* p : ctx->owned_xvec_mfcc) cudaFree(p);
   for (void* p : ctx->owned_ssl) cudaFree(p);
   for (auto& t : ctx->resample_tables) cudaFree(t.dev);
   if (ctx->ws) cudaFree(ctx->ws);
@@ -1298,93 +1385,110 @@ int b200_stats_pool(b200_ctx* ctx, const float* seq, const float* weights, float
   return stats_pool_generic(seq, weights, out, B, F, T, S, weights ? Tw : T, (cudaStream_t)stream);
 }
 
-// ---- XVectorSincNet ----------------------------------------------------------------------------------------
+// ---- XVectorSincNet / XVectorMFCC ---------------------------------------------------------------------------
 int b200_xvec_load(b200_ctx* ctx, const b200_xvec_weights* w) {
   B200_CHECK(ctx && w, B200_ERR_INVALID, "NULL ctx/weights");
-  B200_CHECK(w->dimension >= 1 && w->dimension <= 65536, B200_ERR_INVALID, "embedding dimension %d unsupported",
-             (int)w->dimension);
-  for (int l = 0; l < kXvecLayers; ++l)
-    B200_CHECK(w->tdnn_weight[l] && w->tdnn_bias[l] && w->bn_weight[l] && w->bn_bias[l] && w->bn_mean[l] && w->bn_var[l],
-               B200_ERR_INVALID, "tdnns.%d / tdnns.%d missing", 3 * l, 3 * l + 2);
-  B200_CHECK(w->embedding_weight && w->embedding_bias, B200_ERR_INVALID, "embedding missing");
+  int rc;
+  if ((rc = check_xvec_tdnn(w))) return rc;
   CtxScope scope(ctx);
   XvecWeights& X = ctx->xvec;
   X.loaded = false;
   release_weights(ctx, &ctx->owned_xvec);
-  int rc;
   if ((rc = load_sincnet(ctx, w->wav_norm_weight, w->wav_norm_bias, w->sinc_filters, w->norm_weight, w->norm_bias,
                          w->conv_weight, w->conv_bias, &X.sinc)))
     return rc;
-  const int cin[kXvecLayers] = {60, 512, 512, 512, 512}, cout[kXvecLayers] = {512, 512, 512, 512, 1500};
-  for (int l = 0; l < kXvecLayers; ++l) {
-    const int k = X.taps[l], cp = X.cin_pad[l], np = X.cout_pad[l], K = k * cp;
-    std::vector<float> wt((size_t)np * K, 0.f), bias(np, 0.f), scale(np, 0.f), shift(np, 0.f);
-    for (int co = 0; co < cout[l]; ++co) {
-      for (int ci = 0; ci < cin[l]; ++ci)
-        for (int j = 0; j < k; ++j)
-          wt[(size_t)co * K + j * cp + ci] = w->tdnn_weight[l][((size_t)co * cin[l] + ci) * k + j];
-      bias[co] = w->tdnn_bias[l][co];
-      scale[co] = w->bn_weight[l][co] / std::sqrt(w->bn_var[l][co] + 1e-5f);
-      shift[co] = w->bn_bias[l][co] - w->bn_mean[l][co] * scale[co];
-    }
-    if ((rc = upload_split(ctx, wt, &X.w_hi[l], &X.w_lo[l]))) return rc;
-    if ((rc = upload(ctx, bias, &X.bias[l]))) return rc;
-    if ((rc = upload(ctx, scale, &X.scale[l]))) return rc;
-    if ((rc = upload(ctx, shift, &X.shift[l]))) return rc;
-  }
-  X.dim = w->dimension;
-  X.dim_pad = (int)ceil_div(X.dim, 128) * 128;
-  {
-    std::vector<float> ew((size_t)X.dim_pad * kXvecStatsLd, 0.f), b(X.dim_pad, 0.f);
-    for (int n = 0; n < X.dim; ++n) {
-      for (int kk = 0; kk < 3000; ++kk) ew[(size_t)n * kXvecStatsLd + kk] = w->embedding_weight[(size_t)n * 3000 + kk];
-      b[n] = w->embedding_bias[n];
-    }
-    if ((rc = upload_split(ctx, ew, &X.emb_hi, &X.emb_lo))) return rc;
-    if ((rc = upload(ctx, b, &X.emb_b))) return rc;
-  }
+  if ((rc = load_xvec_tdnn(ctx, w, 60, X))) return rc;
   X.loaded = true;
   return B200_OK;
 }
 
-// Workspace of an XVectorSincNet sub-batch of nb windows of g.W samples (M = nb x F rows, F = g.pool2 SincNet frames):
-// X0 fp32 [M][64] and its (hi, lo) split, two ping-pong activations P / Q [M][512] fp16 (hi, lo), the last layer's fp32
-// rows Y [M][1536] (sharing its region with the SincNet scratch, which is dead by then) and the pooling partials.
+int b200_xvec_mfcc_load(b200_ctx* ctx, const b200_xvec_mfcc_weights* w) {
+  B200_CHECK(ctx && w, B200_ERR_INVALID, "NULL ctx/weights");
+  int rc;
+  if ((rc = check_xvec_tdnn(w))) return rc;
+  B200_CHECK(w->window && w->mel_fb && w->dct_mat, B200_ERR_INVALID, "mfcc window / mel_fb / dct_mat missing");
+  CtxScope scope(ctx);
+  XvecWeights& X = ctx->xvec_mfcc;
+  X.loaded = false;
+  release_weights(ctx, &ctx->owned_xvec_mfcc);
+  if ((rc = load_mfcc(ctx, w->window, w->mel_fb, w->dct_mat, &X.mfcc))) return rc;
+  if ((rc = load_xvec_tdnn(ctx, w, kMfccCoefs, X))) return rc;
+  X.loaded = true;
+  return B200_OK;
+}
+
+// The two front ends of the x-vector TDNN stack (load_xvec_tdnn): SincNet writes XVectorSincNet's first-layer input
+// (60 features and 4 zero columns per frame, through an fp32 copy split afterwards), MFCC that of XVectorMFCC (40
+// coefficients and 24 zero columns, split in place)
+enum class XvecFront { kSincNet, kMfcc };
+
+// Geometry of one utterance length: F front-end frames, T = F - 14 TDNN frames
+struct XvecGeom {
+  SegGeom seg{};     // SincNet only
+  int F = 0;
+};
+static XvecGeom xvec_geom(XvecFront front, int num_samples) {
+  XvecGeom g;
+  switch (front) {
+    case XvecFront::kSincNet:
+      g.seg = seg_geom(num_samples);
+      g.F = g.seg.pool2;
+      break;
+    case XvecFront::kMfcc:
+      g.F = mfcc_num_frames(num_samples);
+      break;
+  }
+  return g;
+}
+
+// Workspace of an x-vector sub-batch of nb utterances of L samples (M = nb x F rows): the first layer's input (SincNet:
+// X0 fp32 [M][64], then its (hi, lo) split; MFCC: the split only), two ping-pong activations P / Q [M][512] fp16 (hi,
+// lo), the last layer's fp32 rows Y [M][1536] (sharing its region with the front end's scratch, which is dead by then)
+// and the pooling partials.
 struct XvecWs {
   float* x0;
   __half *xh, *xl, *ph, *pl, *qh, *ql;
   float* y;
-  void* sinc;
+  void* front;
   double* part;
 };
-static size_t carve_xvec(const SegGeom& g, int nb, int S, void* base, XvecWs* w) {
+static size_t carve_xvec(XvecFront front, const XvecGeom& g, int L, int nb, int S, void* base, XvecWs* w) {
   Workspace ws(base, 1024);
-  const size_t M = (size_t)nb * g.pool2;
+  const size_t M = (size_t)nb * g.F;
+  const bool sinc = front == XvecFront::kSincNet;
   XvecWs t;
-  t.x0 = (float*)ws.take(M * 64 * sizeof(float));
+  t.x0 = sinc ? (float*)ws.take(M * 64 * sizeof(float)) : nullptr;
   t.xh = (__half*)ws.take(M * 64 * sizeof(__half));
   t.xl = (__half*)ws.take(M * 64 * sizeof(__half));
   t.ph = (__half*)ws.take(M * 512 * sizeof(__half));
   t.pl = (__half*)ws.take(M * 512 * sizeof(__half));
   t.qh = (__half*)ws.take(M * 512 * sizeof(__half));
   t.ql = (__half*)ws.take(M * 512 * sizeof(__half));
-  t.y = (float*)ws.take(std::max(M * kPoolRowsLd * sizeof(float), sincnet_workspace_bytes(g, nb)));
-  t.sinc = t.y;
-  t.part = (double*)ws.take(pool_scratch_bytes(nb, S, g.pool2 - 14, kPoolRowsLd, 1));
+  const size_t front_b = sinc ? sincnet_workspace_bytes(g.seg, nb) : mfcc_workspace_bytes(L, nb);
+  t.y = (float*)ws.take(std::max(M * kPoolRowsLd * sizeof(float), front_b));
+  t.front = t.y;
+  t.part = (double*)ws.take(pool_scratch_bytes(nb, S, g.F - 14, kPoolRowsLd, 1));
   if (w) *w = t;
   return ws.bytes();
 }
 
-int b200_xvec_forward(b200_ctx* ctx, const float* wav, const int64_t* off, int64_t num_samples, int32_t num_utts,
-                      const float* weights, int32_t num_speakers, int32_t num_weights, float* emb, void* stream) {
-  B200_CHECK(ctx && ctx->xvec.loaded, B200_ERR_STATE, "XVectorSincNet weights not loaded");
+// An x-vector model on num_utts utterances of one length: per sub-batch the front end writes the first layer's input
+// rows, the five TDNN layers run on gemm_tc_split and the pooling writes the statistics rows; then one GEMM applies the
+// embedding Linear to every row.  A sub-batch holds at most emb_max_batch x 160000 samples (the same budget as the
+// WeSpeaker sub-batches).
+static int xvec_run(b200_ctx* ctx, XvecFront front, const float* wav, const int64_t* off, int64_t num_samples,
+                    int32_t num_utts, const float* weights, int32_t num_speakers, int32_t num_weights, float* emb,
+                    void* stream) {
+  const bool sinc = front == XvecFront::kSincNet;
+  const char* model = sinc ? "XVectorSincNet" : "XVectorMFCC";
+  B200_CHECK(ctx && (sinc ? ctx->xvec : ctx->xvec_mfcc).loaded, B200_ERR_STATE, "%s weights not loaded", model);
   B200_CHECK(wav && off && emb && num_utts >= 0, B200_ERR_INVALID, "bad arguments");
-  B200_CHECK(num_samples >= kXvecMinSamples, B200_ERR_INVALID,
-             "utterances of %lld samples are too short: XVectorSincNet needs at least %d samples (15 SincNet frames "
-             "for one TDNN output frame)", (long long)num_samples, kXvecMinSamples);
+  const int min_samples = sinc ? kXvecMinSamples : kXvecMfccMinSamples;
+  B200_CHECK(num_samples >= min_samples, B200_ERR_INVALID,
+             "utterances of %lld samples are too short: %s needs at least %d samples (15 %s frames for one TDNN output "
+             "frame)", (long long)num_samples, model, min_samples, sinc ? "SincNet" : "MFCC");
   B200_CHECK(!weights || (num_speakers >= 1 && num_weights >= 1), B200_ERR_INVALID,
              "weights need num_speakers >= 1 and num_weights >= 1 (got %d, %d)", (int)num_speakers, (int)num_weights);
-  // a sub-batch holds at most emb_max_batch x 160000 samples (the same budget as the WeSpeaker sub-batches)
   const int64_t budget = (int64_t)ctx->emb_max_batch * kChunk;
   B200_CHECK(num_samples <= budget, B200_ERR_INVALID,
              "an utterance of %lld samples is longer than the %lld samples of one embedding sub-batch (emb_max_batch %d "
@@ -1396,15 +1500,16 @@ int b200_xvec_forward(b200_ctx* ctx, const float* wav, const int64_t* off, int64
     B200_CHECK(off[i] >= 0, B200_ERR_INVALID, "utterance %d: negative offset %lld", i, (long long)off[i]);
   CtxScope scope(ctx);
   cudaStream_t st = (cudaStream_t)stream;
-  const XvecWeights& X = ctx->xvec;
-  const SegGeom geom = seg_geom((int)num_samples);
-  const int F = geom.pool2, T = F - 14;                     // TDNN output frames (xvector.py:255-275)
+  const XvecWeights& X = sinc ? ctx->xvec : ctx->xvec_mfcc;
+  const int L = (int)num_samples;
+  const XvecGeom geom = xvec_geom(front, L);
+  const int F = geom.F, T = F - 14;                         // TDNN output frames (xvector.py:255-275)
   const int S = weights ? num_speakers : 1;
   const int nbmax = (int)std::min<int64_t>(std::min<int64_t>(num_utts, budget / num_samples), 65535);
   const size_t rows = (size_t)num_utts * S;
   const size_t split_bytes = align_up(rows * kXvecStatsLd * sizeof(__half), 1024);
   const size_t out_bytes = X.dim_pad != X.dim ? align_up(rows * X.dim_pad * sizeof(float), 1024) : 0;
-  const size_t sub_bytes = carve_xvec(geom, nbmax, S, nullptr, nullptr);
+  const size_t sub_bytes = carve_xvec(front, geom, L, nbmax, S, nullptr, nullptr);
   int rc = ensure_ws(ctx, sub_bytes + 2 * split_bytes + out_bytes + 4096);
   if (rc) return rc;
   {
@@ -1412,7 +1517,7 @@ int b200_xvec_forward(b200_ctx* ctx, const float* wav, const int64_t* off, int64
     if ((rc = push_meta(ctx, off, valid.data(), num_utts, st, (int)num_samples))) return rc;
   }
   XvecWs w;
-  carve_xvec(geom, nbmax, S, ctx->ws, &w);
+  carve_xvec(front, geom, L, nbmax, S, ctx->ws, &w);
   char* tail = reinterpret_cast<char*>(ctx->ws) + sub_bytes;
   __half* st_hi = reinterpret_cast<__half*>(tail);
   __half* st_lo = reinterpret_cast<__half*>(tail + split_bytes);
@@ -1421,11 +1526,21 @@ int b200_xvec_forward(b200_ctx* ctx, const float* wav, const int64_t* off, int64
   for (int u0 = 0; u0 < num_utts; u0 += nbmax) {
     const int nb = std::min(nbmax, num_utts - u0);
     const int M = nb * F;
-    // always on the tensor cores; seg_conv_impl = 2 selects the per-tile reference kernels here too
-    const int sinc_impl = ctx->seg_conv_impl == 2 ? 2 : 1;
-    if ((rc = sincnet_forward(X.sinc, geom, wav, ctx->d_off + u0, ctx->d_valid + u0, nb, w.sinc, w.x0, sinc_impl, st)))
-      return rc;
-    if ((rc = split_f16(w.x0, w.xh, w.xl, (size_t)M * 64, st))) return rc;
+    switch (front) {
+      case XvecFront::kSincNet: {
+        // always on the tensor cores; seg_conv_impl = 2 selects the per-tile reference kernels here too
+        const int sinc_impl = ctx->seg_conv_impl == 2 ? 2 : 1;
+        if ((rc = sincnet_forward(X.sinc, geom.seg, wav, ctx->d_off + u0, ctx->d_valid + u0, nb, w.front, w.x0,
+                                  sinc_impl, st)))
+          return rc;
+        rc = split_f16(w.x0, w.xh, w.xl, (size_t)M * 64, st);
+        break;
+      }
+      case XvecFront::kMfcc:
+        rc = mfcc_forward(X.mfcc, wav, ctx->d_off + u0, L, nb, w.front, w.xh, w.xl, nullptr, ctx->num_sms, st);
+        break;
+    }
+    if (rc) return rc;
     // Every window keeps the row stride F through the stack: output row b * F + t of layer l reads input rows
     // b * F + t + j * dil.  Rows t >= F - 4, F - 8, F - 14 (layers 1, 2, 3-5) compute values nothing uses, since a
     // valid row of layer l + 1 reads only valid rows of layer l and the pooling reads the first T = F - 14 rows of
@@ -1459,6 +1574,41 @@ int b200_xvec_forward(b200_ctx* ctx, const float* wav, const int64_t* off, int64
     B200_CUDA_OK(cudaMemcpy2DAsync(emb, (size_t)X.dim * sizeof(float), out, (size_t)X.dim_pad * sizeof(float),
                                    (size_t)X.dim * sizeof(float), rows, cudaMemcpyDeviceToDevice, st));
   return B200_OK;
+}
+
+int b200_xvec_forward(b200_ctx* ctx, const float* wav, const int64_t* off, int64_t num_samples, int32_t num_utts,
+                      const float* weights, int32_t num_speakers, int32_t num_weights, float* emb, void* stream) {
+  return xvec_run(ctx, XvecFront::kSincNet, wav, off, num_samples, num_utts, weights, num_speakers, num_weights, emb,
+                  stream);
+}
+
+int b200_xvec_mfcc_forward(b200_ctx* ctx, const float* wav, const int64_t* off, int64_t num_samples, int32_t num_utts,
+                           const float* weights, int32_t num_speakers, int32_t num_weights, float* emb, void* stream) {
+  return xvec_run(ctx, XvecFront::kMfcc, wav, off, num_samples, num_utts, weights, num_speakers, num_weights, emb,
+                  stream);
+}
+
+int b200_xvec_mfcc_features(b200_ctx* ctx, const float* wav, const int64_t* off, int64_t num_samples, int32_t num_utts,
+                            float* out, void* stream) {
+  B200_CHECK(ctx && ctx->xvec_mfcc.loaded, B200_ERR_STATE, "XVectorMFCC weights not loaded");
+  B200_CHECK(wav && off && out && num_utts >= 0 && num_utts <= 65535, B200_ERR_INVALID, "bad arguments");
+  B200_CHECK(num_samples > kMfccFft / 2 && num_samples <= INT_MAX, B200_ERR_INVALID,
+             "utterances of %lld samples: the MFCC front end needs more than %d samples (its reflect padding)",
+             (long long)num_samples, kMfccFft / 2);
+  if (num_utts == 0) return B200_OK;
+  for (int i = 0; i < num_utts; ++i)
+    B200_CHECK(off[i] >= 0, B200_ERR_INVALID, "utterance %d: negative offset %lld", i, (long long)off[i]);
+  CtxScope scope(ctx);
+  cudaStream_t st = (cudaStream_t)stream;
+  const int L = (int)num_samples;
+  int rc = ensure_ws(ctx, mfcc_workspace_bytes(L, num_utts) + 4096);
+  if (rc) return rc;
+  {
+    std::vector<int32_t> valid((size_t)num_utts, 0);
+    if ((rc = push_meta(ctx, off, valid.data(), num_utts, st))) return rc;
+  }
+  return mfcc_forward(ctx->xvec_mfcc.mfcc, wav, ctx->d_off, L, num_utts, ctx->ws, nullptr, nullptr, out, ctx->num_sms,
+                      st);
 }
 
 // ------------------------------------------------------------------------------------------------------

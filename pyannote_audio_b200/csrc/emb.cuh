@@ -115,4 +115,26 @@ int weighted_pool_rows(const float* x, int F, int T, int C, const float* w, int 
 int stats_pool_generic(const float* seq, const float* w, float* out, int B, int F, int T, int S, int Tw,
                        cudaStream_t stream);
 
+// MFCC front end of XVectorMFCC (xvec_mfcc.cu): torchaudio MFCC with its defaults at 16 kHz
+constexpr int kMfccHop = 200, kMfccFft = 400, kMfccBins = 201, kMfccMels = 128, kMfccCoefs = 40;
+constexpr int kMfccRowLd = 256;     // one 200-sample row of the padded signal, zero padded to whole 64-wide k-blocks
+constexpr int kMfccSpecLd = 512;    // DFT output row: 201 cosine sums at k, 201 sine sums at 256 + k
+constexpr int kMfccRowsOut = 64;    // the first TDNN layer's input rows: 40 coefficients, zero padded
+inline int mfcc_num_frames(int L) { return 1 + L / kMfccHop; }
+struct MfccWeights {
+  __half* dft_hi = nullptr;         // [512][2 taps x 256] fp16 (hi, lo) windowed DFT basis (see xvec_mfcc.cu)
+  __half* dft_lo = nullptr;
+  int* band_start = nullptr;        // [128] first nonzero bin of every mel filter (0 and length 0 for an empty one)
+  int* band_len = nullptr;          // [128]
+  int* band_off = nullptr;          // [128] offset of the filter's band in band_w
+  float* band_w = nullptr;          // the filters' weights over their bands, back to back
+  float* dct = nullptr;             // [128][40] dct_mat
+};
+// workspace of mfcc_forward on nb utterances of L samples
+size_t mfcc_workspace_bytes(int L, int nb);
+// nb utterances wav[off[b] .. off[b] + L), L > 200 -> F = 1 + L / 200 frames of 40 coefficients per utterance: as
+// fp16 (hi, lo) rows [nb * F][64] (x_hi / x_lo, zero columns 40..63) or, with x_hi NULL, fp32 rows [nb * F][40]
+int mfcc_forward(const MfccWeights& W, const float* wav, const long long* off, int L, int nb, void* ws, __half* x_hi,
+                 __half* x_lo, float* out, int num_sms, cudaStream_t st);
+
 }  // namespace b200

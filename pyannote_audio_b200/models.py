@@ -1,17 +1,18 @@
 """Model-level seam: ``PyanNet``, the WeSpeaker ResNets (``WeSpeakerResNet34`` and the bottleneck
-``WeSpeakerResNet152`` / ``221`` / ``293``) and ``XVectorSincNet`` with the reference's state-dict keys and
+``WeSpeakerResNet152`` / ``221`` / ``293``), ``XVectorSincNet`` and ``XVectorMFCC`` with the reference's state-dict keys and
 ``forward`` contract, computing through libb200diar.so (no torch ops on the forward path, no CPU fallback).
 
 Reference interfaces mirrored (paths relative to /root/reference/src/pyannote/audio):
   core/model.py:69-183 (Model: specifications, audio, receptive_field, device)
   models/segmentation/PyanNet.py:92-240 (ctor hyper-parameters, num_frames, receptive field, forward)
   models/embedding/wespeaker/__init__.py:41-466 (forward / forward_frames / forward_embedding / dimension)
-  models/embedding/xvector.py:205-349 (XVectorSincNet)
+  models/embedding/xvector.py:42-349 (XVectorMFCC, XVectorSincNet)
   models/segmentation/SSeRiouSS.py (SSeRiouSS on WavLM Base; module tree of torchaudio's wavlm_model)
 """
 from __future__ import annotations
 
 import itertools
+import math
 from functools import cached_property
 from typing import Dict, Optional
 
@@ -61,7 +62,7 @@ class Model(nn.Module):
         self._weights_version = 0
         self.register_load_state_dict_post_hook(lambda module, incompatible: module._bump_weights())
 
-    _SLOT = ""          # "seg" | "emb" | "xvec" | "ssl": the context slot this model family uploads into
+    _SLOT = ""          # "seg" | "emb" | "xvec" | "xvec_mfcc" | "ssl": the context slot this model family uploads into
 
     def _bump_weights(self):
         self._weights_version += 1
@@ -121,11 +122,11 @@ class Model(nn.Module):
         class_name = meta["architecture"]["class"]
         klass = {"PyanNet": PyanNet, "WeSpeakerResNet34": WeSpeakerResNet34, "WeSpeakerResNet152": WeSpeakerResNet152,
                  "WeSpeakerResNet221": WeSpeakerResNet221, "WeSpeakerResNet293": WeSpeakerResNet293,
-                 "XVectorSincNet": XVectorSincNet, "SSeRiouSS": SSeRiouSS}.get(class_name)
+                 "XVectorSincNet": XVectorSincNet, "XVectorMFCC": XVectorMFCC, "SSeRiouSS": SSeRiouSS}.get(class_name)
         if klass is None:
             raise NotImplementedError(f"architecture {meta['architecture']['module']}.{class_name} has no CUDA "
-                                      f"implementation (PyanNet, SSeRiouSS, WeSpeakerResNet34 / 152 / 221 / 293 and "
-                                      f"XVectorSincNet have one)")
+                                      f"implementation (PyanNet, SSeRiouSS, WeSpeakerResNet34 / 152 / 221 / 293, "
+                                      f"XVectorSincNet and XVectorMFCC have one)")
         if cls not in (Model, klass) and not issubclass(klass, cls):
             raise ValueError(f"checkpoint holds a {class_name}, not a {cls.__name__}")
         hparams = dict(loaded.get("hyper_parameters", {}))
@@ -575,28 +576,17 @@ class WeSpeakerResNet293(_BottleneckWeSpeakerResNet):
     NUM_BLOCKS = (10, 20, 64, 3)
 
 
-class XVectorSincNet(Model):
-    """x-vector on the SincNet front end (xvector.py:205-349; the architecture of pyannote/embedding): SincNet, five
-    dilated TDNN layers (Conv1d -> LeakyReLU -> BatchNorm1d), StatsPool and a Linear to ``dimension``."""
+class BaseXVector(Model):
+    """What XVectorSincNet and XVectorMFCC share behind their front ends (xvector.py): five dilated TDNN layers (Conv1d
+    -> LeakyReLU -> BatchNorm1d), StatsPool and a Linear to ``dimension``.  A subclass adds its front end's modules,
+    ``_SLOT``, ``_HPARAMS``, ``min_num_samples``, the front end's frame arithmetic and ``forward_utterances``."""
 
-    _SLOT = "xvec"
-    _HPARAMS = ("sincnet", "dimension", "sample_rate", "num_channels")
     KERNEL = [5, 3, 3, 1, 1]
     DILATION = [1, 2, 3, 1, 1]
-    min_num_samples = ops.XVEC_MIN_SAMPLES
+    min_num_samples = 0
 
-    def __init__(self, sample_rate: int = 16000, num_channels: int = 1, sincnet: Optional[dict] = None,
-                 dimension: int = 512):
-        super().__init__(sample_rate=sample_rate, num_channels=num_channels)
-        sinc_hp = {"stride": 10}
-        sinc_hp.update(sincnet or {})
-        sinc_hp["sample_rate"] = sample_rate
-        if sample_rate != 16000 or sinc_hp["stride"] != 10 or num_channels != 1 or int(dimension) < 1:
-            raise NotImplementedError("the CUDA kernels implement XVectorSincNet on mono 16 kHz audio with SincNet "
-                                      "stride 10 and a positive embedding dimension only")
-        self.hparams.sincnet, self.hparams.dimension = sinc_hp, int(dimension)
-        self.sincnet = _SincNetParams()
-        layers, in_channel = [], 60
+    def _build_tdnn(self, in_channel: int, dimension: int):
+        layers = []
         for (_, out_channel, k, d) in ops.XVEC_TDNN:
             layers += [nn.Conv1d(in_channel, out_channel, k, dilation=d), nn.LeakyReLU(), nn.BatchNorm1d(out_channel)]
             in_channel = out_channel
@@ -611,26 +601,75 @@ class XVectorSincNet(Model):
     def dimension(self) -> int:
         return self.hparams.dimension
 
-    def num_frames(self, num_samples: int) -> int:
-        n = num_samples
-        for k, s in zip(PyanNet.KERNEL, PyanNet.STRIDE):
-            n = _conv1d_num_frames(n, k, s)
+    def _tdnn_num_frames(self, n: int) -> int:
         for k, d in zip(self.KERNEL, self.DILATION):
             n = _conv1d_num_frames(n, k, 1, d=d)
         return n
 
-    def receptive_field_size(self, num_frames: int = 1) -> int:
+    def _tdnn_receptive_field_size(self, num_frames: int) -> int:
         rf = num_frames
         for k, d in reversed(list(zip(self.KERNEL, self.DILATION))):
             rf = 1 + (k - 1) * d + (rf - 1)
+        return rf
+
+    def _tdnn_receptive_field_center(self, frame: int) -> int:
+        c = frame
+        for k, d in reversed(list(zip(self.KERNEL, self.DILATION))):
+            c = c + (1 + (k - 1) * d - 1) // 2
+        return c
+
+    def forward(self, waveforms: torch.Tensor, weights: Optional[torch.Tensor] = None) -> torch.Tensor:
+        """waveforms (batch, 1, samples) with samples >= min_num_samples, weights None, (batch, frames) or
+        (batch, speakers, frames) of any real values -> (batch, dimension) or (batch, speakers, dimension)."""
+        name = type(self).__name__
+        b, c, s = waveforms.shape
+        if c != 1:
+            raise ValueError(f"{name} kernels expect mono waveforms, got {c} channels")
+        if s < self.min_num_samples:
+            raise ValueError(f"{name} needs at least {self.min_num_samples} samples, got {s}")
+        if weights is not None and (weights.dim() not in (2, 3) or weights.shape[0] != b or weights.shape[-1] < 1):
+            raise ValueError("weights must be (batch, frames) or (batch, speakers, frames)")
+        ctx = self._ctx()
+        flat = waveforms.to(device=ctx.device, dtype=torch.float32).reshape(-1).contiguous()
+        emb = self.forward_utterances(flat, np.arange(b, dtype=np.int64) * s, s, weights=weights)
+        return emb if weights is not None and weights.dim() == 3 else emb[:, 0]
+
+
+class XVectorSincNet(BaseXVector):
+    """x-vector on the SincNet front end (xvector.py:205-349; the architecture of pyannote/embedding): SincNet, five
+    dilated TDNN layers (Conv1d -> LeakyReLU -> BatchNorm1d), StatsPool and a Linear to ``dimension``."""
+
+    _SLOT = "xvec"
+    _HPARAMS = ("sincnet", "dimension", "sample_rate", "num_channels")
+    min_num_samples = ops.XVEC_MIN_SAMPLES
+
+    def __init__(self, sample_rate: int = 16000, num_channels: int = 1, sincnet: Optional[dict] = None,
+                 dimension: int = 512):
+        super().__init__(sample_rate=sample_rate, num_channels=num_channels)
+        sinc_hp = {"stride": 10}
+        sinc_hp.update(sincnet or {})
+        sinc_hp["sample_rate"] = sample_rate
+        if sample_rate != 16000 or sinc_hp["stride"] != 10 or num_channels != 1 or int(dimension) < 1:
+            raise NotImplementedError("the CUDA kernels implement XVectorSincNet on mono 16 kHz audio with SincNet "
+                                      "stride 10 and a positive embedding dimension only")
+        self.hparams.sincnet, self.hparams.dimension = sinc_hp, int(dimension)
+        self.sincnet = _SincNetParams()
+        self._build_tdnn(60, dimension)
+
+    def num_frames(self, num_samples: int) -> int:
+        n = num_samples
+        for k, s in zip(PyanNet.KERNEL, PyanNet.STRIDE):
+            n = _conv1d_num_frames(n, k, s)
+        return self._tdnn_num_frames(n)
+
+    def receptive_field_size(self, num_frames: int = 1) -> int:
+        rf = self._tdnn_receptive_field_size(num_frames)
         for k, s in reversed(list(zip(PyanNet.KERNEL, PyanNet.STRIDE))):
             rf = 1 + (k - 1) + (rf - 1) * s
         return rf
 
     def receptive_field_center(self, frame: int = 0) -> int:
-        c = frame
-        for k, d in reversed(list(zip(self.KERNEL, self.DILATION))):
-            c = c + (1 + (k - 1) * d - 1) // 2
+        c = self._tdnn_receptive_field_center(frame)
         for k, s in reversed(list(zip(PyanNet.KERNEL, PyanNet.STRIDE))):
             c = c * s + (k - 1) // 2
         return c
@@ -643,20 +682,106 @@ class XVectorSincNet(Model):
         (n, Tw) / (n, S, Tw) weights or None -> (n, max(S, 1), dimension)."""
         return self._ctx().xvec_forward(wav, off, num_samples, weights=weights)
 
-    def forward(self, waveforms: torch.Tensor, weights: Optional[torch.Tensor] = None) -> torch.Tensor:
-        """waveforms (batch, 1, samples) with samples >= 4771, weights None, (batch, frames) or
-        (batch, speakers, frames) of any real values -> (batch, dimension) or (batch, speakers, dimension)."""
+
+# torchaudio.transforms.MFCC's defaults at 16 kHz: the only MFCC configuration the kernels implement
+MFCC_DEFAULTS = {"n_mfcc": 40, "dct_type": 2, "norm": "ortho", "log_mels": False}
+MFCC_N_FFT, MFCC_HOP, MFCC_N_MELS = 400, 200, 128
+
+
+def mfcc_buffers(sample_rate: int = 16000) -> "OrderedDict[str, torch.Tensor]":
+    """The three buffers of torchaudio's default MFCC under the reference's keys (without the ``mfcc.`` prefix),
+    restated without torchaudio: dct_mat = torchaudio.functional.create_dct(40, 128, "ortho"), the periodic Hann
+    window of 400 samples and fb = melscale_fbanks(201, 0, sample_rate / 2, 128, sample_rate, norm=None,
+    mel_scale="htk")."""
+    from collections import OrderedDict
+
+    n_mels, n_mfcc, n_freqs = MFCC_N_MELS, MFCC_DEFAULTS["n_mfcc"], MFCC_N_FFT // 2 + 1
+    n = torch.arange(float(n_mels))
+    k = torch.arange(float(n_mfcc)).unsqueeze(1)
+    dct = torch.cos(math.pi / float(n_mels) * (n + 0.5) * k)
+    dct[0] *= 1.0 / math.sqrt(2.0)
+    dct *= math.sqrt(2.0 / float(n_mels))
+    all_freqs = torch.linspace(0, sample_rate // 2, n_freqs)
+    m_max = 2595.0 * math.log10(1.0 + (sample_rate / 2) / 700.0)
+    m_pts = torch.linspace(0.0, m_max, n_mels + 2)
+    f_pts = 700.0 * (10.0 ** (m_pts / 2595.0) - 1.0)
+    f_diff = f_pts[1:] - f_pts[:-1]
+    slopes = f_pts.unsqueeze(0) - all_freqs.unsqueeze(1)
+    down = (-1.0 * slopes[:, :-2]) / f_diff[:-1]
+    up = slopes[:, 2:] / f_diff[1:]
+    fb = torch.max(torch.zeros(1), torch.min(down, up))
+    return OrderedDict([("dct_mat", dct.t().contiguous()),
+                        ("MelSpectrogram.spectrogram.window", torch.hann_window(MFCC_N_FFT)),
+                        ("MelSpectrogram.mel_scale.fb", fb)])
+
+
+class _MfccParams(nn.Module):
+    """Holds torchaudio MFCC's buffers under the reference's state-dict keys (``mfcc.dct_mat``,
+    ``mfcc.MelSpectrogram.spectrogram.window``, ``mfcc.MelSpectrogram.mel_scale.fb``); the kernels use the loaded
+    values."""
+
+    def __init__(self, sample_rate: int = 16000):
+        super().__init__()
+        buf = mfcc_buffers(sample_rate)
+        self.register_buffer("dct_mat", buf["dct_mat"])
+        self.MelSpectrogram = nn.Module()
+        self.MelSpectrogram.spectrogram = nn.Module()
+        self.MelSpectrogram.spectrogram.register_buffer("window", buf["MelSpectrogram.spectrogram.window"])
+        self.MelSpectrogram.mel_scale = nn.Module()
+        self.MelSpectrogram.mel_scale.register_buffer("fb", buf["MelSpectrogram.mel_scale.fb"])
+
+
+class XVectorMFCC(BaseXVector):
+    """x-vector on torchaudio's MFCC (xvector.py:42-202): 40 MFCC per 200-sample hop, five dilated TDNN layers
+    (Conv1d -> LeakyReLU -> BatchNorm1d), StatsPool and a Linear to ``dimension``."""
+
+    _SLOT = "xvec_mfcc"
+    _HPARAMS = ("mfcc", "dimension", "sample_rate", "num_channels")
+    min_num_samples = ops.XVEC_MFCC_MIN_SAMPLES
+
+    def __init__(self, sample_rate: int = 16000, num_channels: int = 1, mfcc: Optional[dict] = None,
+                 dimension: int = 512):
+        super().__init__(sample_rate=sample_rate, num_channels=num_channels)
+        mfcc_hp = dict(MFCC_DEFAULTS)
+        mfcc_hp.update(mfcc or {})
+        if not mfcc_hp.get("melkwargs", True):
+            del mfcc_hp["melkwargs"]                       # melkwargs None / {}: torchaudio's defaults
+        mfcc_hp["sample_rate"] = sample_rate
+        if sample_rate != 16000 or num_channels != 1 or int(dimension) < 1 or \
+                mfcc_hp != dict(MFCC_DEFAULTS, sample_rate=sample_rate):
+            raise NotImplementedError(f"the CUDA kernels implement XVectorMFCC on mono 16 kHz audio with torchaudio's "
+                                      f"default MFCC ({MFCC_DEFAULTS}, no melkwargs) and a positive embedding "
+                                      f"dimension only, got sample_rate={sample_rate}, num_channels={num_channels}, "
+                                      f"mfcc={mfcc}")
+        self.hparams.mfcc, self.hparams.dimension = mfcc_hp, int(dimension)
+        self.mfcc = _MfccParams(sample_rate)
+        self._build_tdnn(MFCC_DEFAULTS["n_mfcc"], dimension)
+
+    def num_frames(self, num_samples: int) -> int:
+        return self._tdnn_num_frames(1 + num_samples // MFCC_HOP)          # center=True
+
+    def receptive_field_size(self, num_frames: int = 1) -> int:
+        return MFCC_N_FFT + (self._tdnn_receptive_field_size(num_frames) - 1) * MFCC_HOP
+
+    def receptive_field_center(self, frame: int = 0) -> int:
+        return self._tdnn_receptive_field_center(frame) * MFCC_HOP
+
+    def _upload(self, ctx):
+        ctx.load_xvector_mfcc(self.state_dict())
+
+    def forward_utterances(self, wav: torch.Tensor, off, num_samples: int, weights: Optional[torch.Tensor] = None):
+        """Embeddings of utterances of one length inside one device waveform (ops.Context.xvec_mfcc_forward): soft
+        (n, Tw) / (n, S, Tw) weights or None -> (n, max(S, 1), dimension)."""
+        return self._ctx().xvec_mfcc_forward(wav, off, num_samples, weights=weights)
+
+    def mfcc_features(self, waveforms: torch.Tensor) -> torch.Tensor:
+        """The MFCC front end alone: (batch, 1, samples) -> (batch, 40, 1 + samples // 200), torchaudio's layout."""
         b, c, s = waveforms.shape
         if c != 1:
-            raise ValueError(f"XVectorSincNet kernels expect mono waveforms, got {c} channels")
-        if s < ops.XVEC_MIN_SAMPLES:
-            raise ValueError(f"XVectorSincNet needs at least {ops.XVEC_MIN_SAMPLES} samples, got {s}")
-        if weights is not None and (weights.dim() not in (2, 3) or weights.shape[0] != b or weights.shape[-1] < 1):
-            raise ValueError("weights must be (batch, frames) or (batch, speakers, frames)")
+            raise ValueError(f"XVectorMFCC kernels expect mono waveforms, got {c} channels")
         ctx = self._ctx()
         flat = waveforms.to(device=ctx.device, dtype=torch.float32).reshape(-1).contiguous()
-        emb = self.forward_utterances(flat, np.arange(b, dtype=np.int64) * s, s, weights=weights)
-        return emb if weights is not None and weights.dim() == 3 else emb[:, 0]
+        return ctx.mfcc_features(flat, np.arange(b, dtype=np.int64) * s, s).transpose(1, 2)
 
 
 # ---- SSeRiouSS ----------------------------------------------------------------------------------------------------

@@ -21,6 +21,7 @@ SEG_LOGSOFTMAX, SEG_SIGMOID = 0, 1
 EMB_DIM = 256
 SEG_MIN_SAMPLES = 1261     # shortest PyanNet window: 2 output frames (one frame cannot be instance-normalised)
 XVEC_MIN_SAMPLES = 4771    # shortest XVectorSincNet input: 15 SincNet frames, one frame after the TDNN layers
+XVEC_MFCC_MIN_SAMPLES = 2800   # shortest XVectorMFCC input: 15 MFCC frames
 XVEC_TDNN = ((60, 512, 5, 1), (512, 512, 3, 2), (512, 512, 3, 3), (512, 512, 1, 1), (512, 1500, 1, 1))
 
 
@@ -209,6 +210,30 @@ def _fill_sincnet(w, sd: Mapping[str, torch.Tensor], f):
         w.conv_bias[i] = f(f"sincnet.conv1d.{i + 1}.bias")
 
 
+def _fill_tdnn(w, sd: Mapping[str, torch.Tensor], f, cin0: int) -> int:
+    """The ``tdnns.*`` and ``embedding.*`` fields that XvecWeights and XvecMfccWeights share (tdnns.0 has ``cin0``
+    input channels); returns the embedding dimension."""
+    for layer, (cin, cout, k, _) in enumerate(XVEC_TDNN):
+        cin = cin0 if layer == 0 else cin
+        conv, bn = f"tdnns.{3 * layer}", f"tdnns.{3 * layer + 2}"
+        if tuple(sd[conv + ".weight"].shape) != (cout, cin, k):
+            raise ValueError(f"{conv}.weight has shape {tuple(sd[conv + '.weight'].shape)}, expected "
+                             f"{(cout, cin, k)}")
+        w.tdnn_weight[layer] = f(conv + ".weight")
+        w.tdnn_bias[layer] = f(conv + ".bias")
+        w.bn_weight[layer] = f(bn + ".weight")
+        w.bn_bias[layer] = f(bn + ".bias")
+        w.bn_mean[layer] = f(bn + ".running_mean")
+        w.bn_var[layer] = f(bn + ".running_var")
+    dim, k_in = sd["embedding.weight"].shape
+    if k_in != 3000:
+        raise ValueError(f"embedding.weight has {k_in} inputs, expected 3000")
+    w.dimension = int(dim)
+    w.embedding_weight = f("embedding.weight")
+    w.embedding_bias = f("embedding.bias")
+    return int(dim)
+
+
 def fold_weight_norm(sd: Mapping[str, torch.Tensor], prefix: str) -> torch.Tensor:
     """The plain fp32 weight of a conv under weight norm over dim 2 (torch.nn.utils.parametrizations.weight_norm, or
     the older torch.nn.utils.weight_norm): ``prefix + parametrizations.weight.original0 / original1`` or
@@ -253,7 +278,10 @@ class Context:
         self.emb_channels = 256   # trunk output channels of the loaded embedding model: 256 (ResNet34) or 1024
         self.xvec_loaded = False
         self.xvec_dimension = 512
-        self.owners = {}    # slot ("seg" | "emb" | "xvec" | "ssl") -> stamp of the model whose weights are resident
+        self.xvec_mfcc_loaded = False
+        self.xvec_mfcc_dimension = 512
+        # slot ("seg" | "emb" | "xvec" | "xvec_mfcc" | "ssl") -> stamp of the model whose weights are resident
+        self.owners = {}
         # A/B knob for scripts (like B200_CONV_IMPL / B200_EMB_MAX_BATCH / B200_SEG_MAX_BATCH, which the library
         # reads itself): B200_OPTIONS="key=value,..."
         # is applied through b200_ctx_set_option, so unknown keys / bad values fail loudly
@@ -347,27 +375,28 @@ class Context:
         f = _state_dict_reader(sd)
         w = _lib.XvecWeights()
         _fill_sincnet(w, sd, f)
-        for layer, (cin, cout, k, _) in enumerate(XVEC_TDNN):
-            conv, bn = f"tdnns.{3 * layer}", f"tdnns.{3 * layer + 2}"
-            if tuple(sd[conv + ".weight"].shape) != (cout, cin, k):
-                raise ValueError(f"{conv}.weight has shape {tuple(sd[conv + '.weight'].shape)}, expected "
-                                 f"{(cout, cin, k)}")
-            w.tdnn_weight[layer] = f(conv + ".weight")
-            w.tdnn_bias[layer] = f(conv + ".bias")
-            w.bn_weight[layer] = f(bn + ".weight")
-            w.bn_bias[layer] = f(bn + ".bias")
-            w.bn_mean[layer] = f(bn + ".running_mean")
-            w.bn_var[layer] = f(bn + ".running_var")
-        dim, k_in = sd["embedding.weight"].shape
-        if k_in != 3000:
-            raise ValueError(f"embedding.weight has {k_in} inputs, expected 3000")
-        w.dimension = int(dim)
-        w.embedding_weight = f("embedding.weight")
-        w.embedding_bias = f("embedding.bias")
+        dim = _fill_tdnn(w, sd, f, 60)
         self.owners.pop("xvec", None)
         self.xvec_loaded = False
         _lib.check(self.lib.b200_xvec_load(self._h, C.byref(w)))
-        self.xvec_loaded, self.xvec_dimension = True, int(dim)
+        self.xvec_loaded, self.xvec_dimension = True, dim
+
+    def load_xvector_mfcc(self, sd: Mapping[str, torch.Tensor]):
+        """XVectorMFCC weights (models/embedding/xvector.py:42-89) into the ctx's own slot: the TDNN stack and Linear,
+        and the MFCC buffers as loaded."""
+        f = _state_dict_reader(sd)
+        w = _lib.XvecMfccWeights()
+        for field, key, shape in (("dct_mat", "mfcc.dct_mat", (128, 40)),
+                                  ("window", "mfcc.MelSpectrogram.spectrogram.window", (400,)),
+                                  ("mel_fb", "mfcc.MelSpectrogram.mel_scale.fb", (201, 128))):
+            if tuple(sd[key].shape) != shape:
+                raise ValueError(f"{key} has shape {tuple(sd[key].shape)}, expected {shape}")
+            setattr(w, field, f(key))
+        dim = _fill_tdnn(w, sd, f, 40)
+        self.owners.pop("xvec_mfcc", None)
+        self.xvec_mfcc_loaded = False
+        _lib.check(self.lib.b200_xvec_mfcc_load(self._h, C.byref(w)))
+        self.xvec_mfcc_loaded, self.xvec_mfcc_dimension = True, dim
 
     def load_sseriouss(self, sd: Mapping[str, torch.Tensor], specifications=None, wav2vec_layer: int = -1):
         """SSeRiouSS weights (models/segmentation/SSeRiouSS.py on WavLM Base) into the ctx's own slot.  ``sd`` uses
@@ -612,13 +641,32 @@ class Context:
         """XVectorSincNet embeddings of utterances of one length: utterance i = wav[off[i] : off[i] + num_samples]
         (>= 4771 samples).  ``weights``: None or (n, Tw) / (n, S, Tw) pooling weights of any real values (any Tw,
         nearest-interpolated onto the TDNN frames) -> (n, max(S, 1), dimension) float32."""
-        off, n, num_samples = self._utterances(wav, off, num_samples, XVEC_MIN_SAMPLES,
-                                               f"XVectorSincNet needs at least {XVEC_MIN_SAMPLES} samples, got {{}}")
+        return self._xvec_run("b200_xvec_forward", "XVectorSincNet", XVEC_MIN_SAMPLES, self.xvec_dimension, wav, off,
+                              num_samples, weights, out)
+
+    def xvec_mfcc_forward(self, wav, off, num_samples: int, weights: Optional[torch.Tensor] = None,
+                          out: Optional[torch.Tensor] = None):
+        """XVectorMFCC embeddings, as xvec_forward (>= 2800 samples)."""
+        return self._xvec_run("b200_xvec_mfcc_forward", "XVectorMFCC", XVEC_MFCC_MIN_SAMPLES, self.xvec_mfcc_dimension,
+                              wav, off, num_samples, weights, out)
+
+    def _xvec_run(self, entry: str, name: str, min_samples: int, dim: int, wav, off, num_samples: int, weights, out):
+        off, n, num_samples = self._utterances(wav, off, num_samples, min_samples,
+                                               f"{name} needs at least {min_samples} samples, got {{}}")
         w, S, Tw = self._pool_weights(weights, n)
-        emb = self._out(out, (n, S, self.xvec_dimension), torch.float32)
-        self._call("b200_xvec_forward", _ptr(wav), off.ctypes.data, num_samples, n, _ptr(w), S if w is not None else 0,
-                   Tw, _ptr(emb))
+        emb = self._out(out, (n, S, dim), torch.float32)
+        self._call(entry, _ptr(wav), off.ctypes.data, num_samples, n, _ptr(w), S if w is not None else 0, Tw,
+                   _ptr(emb))
         return emb
+
+    def mfcc_features(self, wav, off, num_samples: int) -> torch.Tensor:
+        """The loaded XVectorMFCC's front end alone on utterances of one length (> 200 samples) -> (n, frames, 40)
+        float32 MFCC, frames = 1 + num_samples // 200."""
+        off, n, num_samples = self._utterances(wav, off, num_samples, 201,
+                                               "the MFCC front end needs more than 200 samples, got {}")
+        out = torch.empty((n, 1 + num_samples // 200, 40), dtype=torch.float32, device=self.device)
+        self._call("b200_xvec_mfcc_features", _ptr(wav), off.ctypes.data, num_samples, n, _ptr(out))
+        return out
 
     def emb_forward_embedding(self, frames: torch.Tensor, weights: Optional[torch.Tensor] = None):
         """ResNet.forward_embedding on frames (B, C, 10, T) -> (B, max(S, 1), 256) float32, C the trunk channels of

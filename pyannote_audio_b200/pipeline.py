@@ -30,7 +30,7 @@ from .audio import Audio, AudioFile
 from .clustering import PLDA, AgglomerativeClustering, VBxClustering
 from .core import Annotation, SlidingWindow, SlidingWindowFeature
 from .inference import Inference, chunk_layout
-from .models import BaseWeSpeakerResNet, PyanNet, WeSpeakerResNet34, XVectorSincNet, get_context
+from .models import BaseWeSpeakerResNet, BaseXVector, PyanNet, WeSpeakerResNet34, get_context
 
 
 def set_num_speakers(num_speakers=None, min_speakers=None, max_speakers=None):
@@ -63,7 +63,7 @@ class DiarizeOutput:
 class PretrainedSpeakerEmbedding:
     """pipelines/speaker_verification.py:622-716 (PyannoteAudioPretrainedSpeakerEmbedding) over the CUDA model."""
 
-    def __init__(self, embedding: Union[BaseWeSpeakerResNet, XVectorSincNet], device: Optional[torch.device] = None):
+    def __init__(self, embedding: Union[BaseWeSpeakerResNet, BaseXVector], device: Optional[torch.device] = None):
         self.embedding = embedding
         self.model_ = embedding
         self.model_.eval()
@@ -93,7 +93,7 @@ class PretrainedSpeakerEmbedding:
     @property
     def min_num_samples(self) -> int:
         # the shortest input the model accepts (speaker_verification.py:688-702 finds it by bisection on exceptions):
-        # 400 for the WeSpeaker ResNets, 4771 for XVectorSincNet
+        # 400 for the WeSpeaker ResNets, 4771 for XVectorSincNet, 2800 for XVectorMFCC
         return self.model_.min_num_samples
 
     def __call__(self, waveforms: torch.Tensor, masks: Optional[torch.Tensor] = None) -> np.ndarray:

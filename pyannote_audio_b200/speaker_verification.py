@@ -8,7 +8,7 @@ import numpy as np
 import torch
 
 from .audio import AudioFile
-from .models import BaseWeSpeakerResNet, PyanNet, WeSpeakerResNet34, XVectorSincNet
+from .models import BaseWeSpeakerResNet, BaseXVector, PyanNet, WeSpeakerResNet34
 
 
 class SpeakerEmbedding:
@@ -16,7 +16,7 @@ class SpeakerEmbedding:
     file; with it, frames are weighted by the cubed aggregated speech score of the voice activity detection
     (max over the speakers of the segmentation model), interpolated onto the model's frames."""
 
-    def __init__(self, embedding: Union[BaseWeSpeakerResNet, XVectorSincNet, Mapping, str, None] = None,
+    def __init__(self, embedding: Union[BaseWeSpeakerResNet, BaseXVector, Mapping, str, None] = None,
                  segmentation: Union[PyanNet, Mapping, str, None] = None, token=None, cache_dir=None,
                  device: Optional[torch.device] = None):
         from .loading import get_model, is_checkpoint_spec
@@ -27,9 +27,9 @@ class SpeakerEmbedding:
             model = WeSpeakerResNet34()
             model.load_state_dict(embedding)
             embedding = model
-        if not isinstance(embedding, (BaseWeSpeakerResNet, XVectorSincNet)):
-            raise ValueError("`embedding` must be a WeSpeaker ResNet or XVectorSincNet instance, a ResNet34 state dict "
-                             "or a local checkpoint (no hub access here)")
+        if not isinstance(embedding, (BaseWeSpeakerResNet, BaseXVector)):
+            raise ValueError("`embedding` must be a WeSpeaker ResNet, XVectorSincNet or XVectorMFCC instance, a ResNet34 "
+                             "state dict or a local checkpoint (no hub access here)")
         device = device or torch.device("cuda", torch.cuda.current_device() if torch.cuda.is_available() else 0)
         self.embedding = embedding
         self.segmentation = segmentation

@@ -9,7 +9,7 @@ def reference_style_checkpoint(kind):
     """``kind``: "seg" (PyanNet, community-1 head), "seg_multilabel" (PyanNet with a 4-label sigmoid head,
     permutation_invariant=False), "seg_binary" (a 1-class sigmoid ["speech"] head), "seg_powerset42" (a powerset
     head of 4 speakers with at most 2 per frame, 11 classes), "emb" (WeSpeakerResNet34), "emb293"
-    (WeSpeakerResNet293), "xvec" (XVectorSincNet) or "sseriouss" (SSeRiouSS on WavLM Base, 4-label sigmoid head).  A Lightning-format pytorch_model.bin as the reference writes it (model.py:244-256): state_dict +
+    (WeSpeakerResNet293), "xvec" (XVectorSincNet), "xvec_mfcc" (XVectorMFCC) or "sseriouss" (SSeRiouSS on WavLM Base, 4-label sigmoid head).  A Lightning-format pytorch_model.bin as the reference writes it (model.py:244-256): state_dict +
     hyper_parameters + checkpoint["pyannote.audio"] whose `specifications` is pickled under the REFERENCE's module
     path pyannote.audio.core.task (registered here only while pickling, then removed again)."""
     import dataclasses
@@ -100,6 +100,15 @@ def reference_style_checkpoint(kind):
                   "pyannote.audio": {"versions": {"pyannote.audio": "4.0.0"},
                                      "architecture": {"module": "pyannote.audio.models.embedding.xvector",
                                                       "class": "XVectorSincNet"},
+                                     "specifications": Specifications(Problem.REPRESENTATION, Resolution.CHUNK, 3.0)}}
+        elif kind == "xvec_mfcc":
+            ck = {"state_dict": syn.make_xvector_mfcc_state_dict(5),
+                  "hyper_parameters": {"mfcc": {"n_mfcc": 40, "dct_type": 2, "norm": "ortho", "log_mels": False,
+                                                "sample_rate": 16000},
+                                       "dimension": 512, "sample_rate": 16000, "num_channels": 1},
+                  "pyannote.audio": {"versions": {"pyannote.audio": "4.0.0"},
+                                     "architecture": {"module": "pyannote.audio.models.embedding.xvector",
+                                                      "class": "XVectorMFCC"},
                                      "specifications": Specifications(Problem.REPRESENTATION, Resolution.CHUNK, 3.0)}}
         else:
             ck = {"state_dict": syn.make_embedding_state_dict(1),

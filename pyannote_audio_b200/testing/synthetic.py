@@ -9,6 +9,7 @@ with the *reference's state-dict key names and shapes* (real checkpoints drop in
 * embedding: ``WeSpeakerResNet34``; keys as in models/embedding/wespeaker/resnet.py:233-252; the bottleneck
   ``WeSpeakerResNet152`` / ``221`` / ``293`` (resnet.py:148-212) with ``make_bottleneck_state_dict``
 * x-vector: ``XVectorSincNet`` with ``make_xvector_state_dict``; keys as in models/embedding/xvector.py:205-252
+* x-vector on MFCC: ``XVectorMFCC`` with ``make_xvector_mfcc_state_dict``; keys as in models/embedding/xvector.py:42-89
 * PLDA: ``xvec_transform.npz{mean1,mean2,lda}`` + ``plda.npz{mu,tr,psi}`` (utils/vbx.py:195-199)
 
 Audio: a synthetic multi-speaker "conversation" (harmonic sources, 3-6 Hz amplitude modulation,
@@ -181,9 +182,28 @@ def make_xvector_state_dict(seed: int = 3, dimension: int = 512) -> "OrderedDict
     g = torch.Generator().manual_seed(seed)
     sd = OrderedDict((k, v) for k, v in make_segmentation_state_dict(seed, fitted_classifier=False).items()
                      if k.startswith("sincnet."))
+    return _xvector_tdnn(sd, g, 60, 1.0, dimension)
+
+
+def make_xvector_mfcc_state_dict(seed: int = 5, dimension: int = 512) -> "OrderedDict[str, torch.Tensor]":
+    """XVectorMFCC weights with the reference's keys (xvector.py:42-89): torchaudio's default MFCC buffers
+    (models.mfcc_buffers) and the TDNN stack and Linear drawn as in make_xvector_state_dict, except that the first
+    Conv1d's gain is 1/30 of it: MFCC coefficients are tens of units (c0 around -130 and reaching the hundreds on
+    synthetic speech, RMS ~28 over all 40), where SincNet's features are O(1)."""
+    from ..models import mfcc_buffers
+
+    g = torch.Generator().manual_seed(seed)
+    sd = OrderedDict(("mfcc." + k, v) for k, v in mfcc_buffers().items())
+    return _xvector_tdnn(sd, g, 40, 1.0 / 30.0, dimension)
+
+
+def _xvector_tdnn(sd, g, cin0: int, gain0: float, dimension: int):
+    """The ``tdnns.*`` and ``embedding.*`` entries of make_xvector_state_dict / make_xvector_mfcc_state_dict: tdnns.0
+    has ``cin0`` inputs and ``gain0`` times the other layers' gain."""
     for layer, (cin, cout, k) in enumerate(XVECTOR_TDNN):
+        cin, gain = (cin0, gain0) if layer == 0 else (cin, 1.0)
         conv, bn = f"tdnns.{3 * layer}", f"tdnns.{3 * layer + 2}"
-        sd[conv + ".weight"] = torch.randn(cout, cin, k, generator=g) * (1.5 / math.sqrt(cin * k))
+        sd[conv + ".weight"] = torch.randn(cout, cin, k, generator=g) * (gain * 1.5 / math.sqrt(cin * k))
         sd[conv + ".bias"] = 0.05 * torch.randn(cout, generator=g)
         sd[bn + ".weight"] = 0.8 + 0.4 * torch.rand(cout, generator=g)
         sd[bn + ".bias"] = 0.1 * torch.randn(cout, generator=g)
