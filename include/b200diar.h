@@ -250,6 +250,11 @@ int b200_ssl_forward_window(b200_ctx* ctx, const float* wav, const int64_t* chun
 /* The same for a sigmoid head, outputs as in b200_seg_forward_scores. */
 int b200_ssl_forward_scores(b200_ctx* ctx, const float* wav, const int64_t* chunk_off, const int32_t* chunk_valid,
                             int32_t num_chunks, int32_t window, float* scores, float* max_scores, void* stream);
+/* The WavLM Base front end alone, arguments as in b200_ssl_forward_window: out[num_chunks][T][768] fp32, the LSTM
+ * input of the forward (the softmax-weighted layer average, or the output of layer wav2vec_layer).  The head does not
+ * run; sub-batches, ssl_max_batch and the window checks are those of the forward. */
+int b200_ssl_features(b200_ctx* ctx, const float* wav, const int64_t* chunk_off, const int32_t* chunk_valid,
+                      int32_t num_chunks, int32_t window, float* out, void* stream);
 
 /* ---- audio ingest: Audio.__call__ / Audio.downmix_and_resample (core/io.py:223-265, 306-351) -----------------
  * pcm is a DEVICE buffer holding the raw decoded audio: B200_PCM_S16_INTERLEAVED = int16 [frame][channel] (what a

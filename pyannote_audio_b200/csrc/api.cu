@@ -808,10 +808,10 @@ static const SegWeights* loaded_head(const b200_ctx* ctx, SegFront front) {
 // A segmentation model on n windows of `window` samples: per sub-batch, the front end writes x0 [nb][T][F] and the
 // head classifies it, both phases in the same workspace region.  A sub-batch holds at most max_batch x 160000
 // window samples (the workspace of max_batch 10 s windows; option seg_max_batch or ssl_max_batch) and at most 65535
-// windows (the y extent of the SincNet grids).  The "seg" timer covers PyanNet's sub-batches.  With sinc_out (SincNet
-// only), the front end writes there and the head does not run.
+// windows (the y extent of the SincNet grids).  The "seg" timer covers PyanNet's sub-batches.  With front_out, the
+// front end writes its head input [n][T][F] there instead of x0 and the head does not run.
 static int seg_run(b200_ctx* ctx, SegFront front, const float* wav, const int64_t* chunk_off,
-                   const int32_t* chunk_valid, int n, int window, const SegHeadOut& out, float* sinc_out,
+                   const int32_t* chunk_valid, int n, int window, const SegHeadOut& out, float* front_out,
                    cudaStream_t st) {
   const bool sinc = front == SegFront::kSincNet;
   const char* model = sinc ? "segmentation" : "SSeRiouSS";
@@ -860,18 +860,19 @@ static int seg_run(b200_ctx* ctx, SegFront front, const float* wav, const int64_
     const int nb = (n - c0) < nbmax ? (n - c0) : nbmax;
     ScopedTimer timer(ctx, sinc ? &ctx->seg_events : nullptr, st);
     if (ctx->profile && sinc) ctx->seg_chunks += nb;
+    float* feat = front_out ? front_out + (size_t)c0 * T * F : x0;
     switch (front) {
       case SegFront::kSincNet:
-        rc = sincnet_forward(ctx->seg.sinc, seg_g, wav, ctx->d_off + c0, ctx->d_valid + c0, nb, region,
-                             sinc_out ? sinc_out + (size_t)c0 * T * F : x0, ctx->seg_conv_impl, st);
+        rc = sincnet_forward(ctx->seg.sinc, seg_g, wav, ctx->d_off + c0, ctx->d_valid + c0, nb, region, feat,
+                             ctx->seg_conv_impl, st);
         break;
       case SegFront::kWavLM:
-        rc = ssl_frontend_forward(ctx->ssl, ssl_g, wav, ctx->d_off + c0, ctx->d_valid + c0, nb, region, x0,
+        rc = ssl_frontend_forward(ctx->ssl, ssl_g, wav, ctx->d_off + c0, ctx->d_valid + c0, nb, region, feat,
                                   ctx->num_sms, st);
         break;
     }
     if (rc) return rc;
-    if (sinc_out) continue;
+    if (front_out) continue;
     const size_t row0 = (size_t)c0 * T, K = head->num_classes;
     SegHeadOut sub;
     sub.cls = out.cls ? out.cls + row0 : nullptr;
@@ -1030,6 +1031,13 @@ int b200_ssl_forward_scores(b200_ctx* ctx, const float* wav, const int64_t* chun
                             int32_t num_chunks, int32_t window, float* scores, float* max_scores, void* stream) {
   return seg_forward_head(ctx, SegFront::kWavLM, kSegSigmoid, wav, chunk_off, chunk_valid, num_chunks, window,
                           SegHeadOut{nullptr, nullptr, scores, max_scores}, stream);
+}
+
+int b200_ssl_features(b200_ctx* ctx, const float* wav, const int64_t* chunk_off, const int32_t* chunk_valid,
+                      int32_t num_chunks, int32_t window, float* out, void* stream) {
+  B200_CHECK(out != nullptr, B200_ERR_INVALID, "out is NULL");
+  return seg_run(ctx, SegFront::kWavLM, wav, chunk_off, chunk_valid, num_chunks, window, SegHeadOut(), out,
+                 (cudaStream_t)stream);
 }
 
 __global__ void strip_pad_kernel(const float* __restrict__ x64, float* __restrict__ out, size_t rows) {

@@ -583,6 +583,17 @@ class Context:
         self._call("b200_sincnet_forward", _ptr(wav), off.ctypes.data, valid.ctypes.data, n, _ptr(out))
         return out
 
+    def ssl_features(self, wav, chunk_off, chunk_valid, window: int = CHUNK):
+        """The loaded SSeRiouSS's WavLM Base front end alone, windows as in ssl_forward -> (n, F, 768) float32, the
+        LSTM input of ssl_forward (the weighted layer average, or the output of layer wav2vec_layer)."""
+        check_ssl_window(window)
+        window = int(window)
+        off, valid = self._chunks(wav, chunk_off, chunk_valid)
+        n = len(off)
+        out = torch.empty((n, ssl_num_frames(window), 768), dtype=torch.float32, device=self.device)
+        self._call("b200_ssl_features", _ptr(wav), off.ctypes.data, valid.ctypes.data, n, window, _ptr(out))
+        return out
+
     def powerset_to_multilabel(self, cls: torch.Tensor, num_speakers: int = SPEAKERS, max_per_frame: int = 2):
         """(…) uint8 powerset classes of ``num_speakers`` speakers with at most ``max_per_frame`` per frame ->
         (…, num_speakers) uint8 multilabel (Powerset.to_multilabel, hard)."""

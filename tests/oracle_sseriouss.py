@@ -11,7 +11,11 @@ import torch.nn.functional as F
 def relative_buckets(T, num_buckets=320, max_distance=800):
     """(T, T) bucket of key j - query i, WavLM's bidirectional bucketing."""
     pos = torch.arange(T, dtype=torch.long)   # on the CPU: the float log rounds as in the reference
-    rel = pos[None, :] - pos[:, None]
+    return relative_bucket(pos[None, :] - pos[:, None], num_buckets, max_distance)
+
+
+def relative_bucket(rel, num_buckets=320, max_distance=800):
+    """Bucket of every offset key - query in the CPU long tensor ``rel``."""
     half = num_buckets // 2
     buckets = (rel > 0).to(torch.long) * half
     a = torch.abs(rel)
@@ -27,7 +31,7 @@ def pos_conv_weight(sd, prefix):
         g, v = sd[prefix + "parametrizations.weight.original0"], sd[prefix + "parametrizations.weight.original1"]
     else:
         g, v = sd[prefix + "weight_g"], sd[prefix + "weight_v"]
-    return torch._weight_norm(v.float(), g.float(), 2)
+    return torch._weight_norm(v, g, 2)        # in the state dict's dtype: the fp64 oracle runs the same code
 
 
 def wavlm_layers(sd, wav, num_layers=12):
@@ -84,7 +88,14 @@ def sseriouss(sd, wav, wav2vec_layer=-1, sigmoid=False, device="cpu"):
     """wav (B, S) fp32 -> (B, T, K) log-probabilities (or sigmoid scores) on the CPU, computed on ``device`` (fp32:
     callers on a GPU disable TF32)."""
     sd = {k: v.detach().float().to(device) for k, v in sd.items()}
-    x = features(sd, wav.float().to(device), wav2vec_layer)
+    return head(sd, features(sd, wav.float().to(device), wav2vec_layer), sigmoid)
+
+
+@torch.no_grad()
+def head(sd, x, sigmoid=False):
+    """The LSTM input x (B, T, 768) -> (B, T, K) log-probabilities (or sigmoid scores) on the CPU: the BiLSTM, the
+    two Linears and the classifier of SSeRiouSS.forward, on x's device with the fp32 state dict ``sd`` there."""
+    device = x.device
     layers = 0
     while f"lstm.weight_ih_l{layers}" in sd:
         layers += 1
