@@ -338,6 +338,13 @@ int64_t b200_emb_fbank_plan(const int64_t* chunk_off, const int32_t* chunk_valid
 /* ResNet.forward_frames on a given fbank (resnet.py:399-419): frames[num_chunks][C][10][125] fp32 (NCHW), C = 256 for
  * ResNet34 and 1024 for a bottleneck trunk. */
 int b200_emb_trunk(b200_ctx* ctx, const float* fbank, int32_t num_chunks, float* frames, void* stream);
+/* One stage of the trunk of b200_emb_trunk on B segments of width W, as the embedding paths run it (conv_impl
+ * included).  Stage 0 is the stem: in = fp32 fbank[B][W][80], fmean[B][80] subtracted from it, out = NHWC fp16
+ * [B][80][W][32].  Stage k >= 1 is block k - 1 (BasicBlock or Bottleneck; fmean unused): in = NHWC fp16
+ * [B][H][W][C_in], H = 80, 40, 20 or 10 by the block's layer, out = NHWC fp16 [B][H'][W'][C_out].  B may not exceed
+ * one embedding sub-batch, max(1, emb_max_batch * 998 / W) segments. */
+int b200_emb_trunk_stage(b200_ctx* ctx, int32_t stage, const void* in, const float* fmean, int32_t B, int32_t W,
+                         void* out, void* stream);
 /* WeSpeakerResNet34.forward (models/embedding/wespeaker/__init__.py:324-343) on utterances of one length
  * num_samples >= 400 (a (num_utts, 1, num_samples) tensor): utterance i = wav[off[i] .. off[i] + num_samples), off a
  * HOST array.  compute_fbank (:113-139) gives T0 = 1 + (num_samples - 400) / 160 frames, the trunk

@@ -1168,29 +1168,42 @@ static int bottleneck_run(b200_ctx* ctx, const BottleneckWeights& B, __half* A, 
   return B200_OK;
 }
 
+// stages of the loaded trunk: the stem, then its BasicBlocks or its Bottlenecks
+static int trunk_stages(const EmbWeights& E) { return 1 + (int)(E.blocks.size() + E.bottlenecks.size()); }
+
+// stride and output channels of trunk stage k (0: the stem)
+static void stage_shape(const EmbWeights& E, int k, int* stride, int* C_out) {
+  if (k == 0) { *stride = 1; *C_out = 32; return; }
+  if (!E.blocks.empty()) { *stride = E.blocks[k - 1].conv1.stride; *C_out = E.blocks[k - 1].conv2.C_out; return; }
+  *stride = E.bottlenecks[k - 1].conv2.stride;
+  *C_out = E.bottlenecks[k - 1].conv3.C_out;
+}
+
+// Stage k of the trunk on nb segments: k = 0 the stem from w.fbank - w.fmean (T0 = Wd frames) into w.A, k >= 1 block
+// k - 1 on w.A (H x Wd in, H x Wd updated to its output's).  The result is in w.A: a fused block swaps w.A and w.Bf.
+static int trunk_stage(b200_ctx* ctx, int k, EmbWs& w, const int* frame0, int nb, int& H, int& Wd, cudaStream_t st) {
+  const EmbWeights& E = ctx->emb;
+  if (k == 0) return conv1_forward(w.fbank, w.fmean, frame0, E.conv1_w, E.conv1_b, w.A, nb, Wd, st);
+  const int rc = E.blocks.empty() ? bottleneck_run(ctx, E.bottlenecks[k - 1], w.A, w.Bf, w.Cf, w.D, nb, H, Wd, st)
+                                  : block_run(ctx, E.blocks[k - 1], w.A, w.Bf, w.Cf, nb, H, Wd, st);
+  if (rc) return rc;
+  int s, C;
+  stage_shape(E, k, &s, &C);
+  H = (H + 2 - 3) / s + 1; Wd = (Wd + 2 - 3) / s + 1;
+  return B200_OK;
+}
+
 // conv1 + the 16 BasicBlocks (or the Bottlenecks) on nb segments of T0 fbank frames; returns the buffer holding the
 // result (NHWC fp16 [nb][10][T][C]) and its width T = trunk_width(T0)
 static int trunk_run(b200_ctx* ctx, const EmbWs& w, const int* frame0, int nb, int T0, cudaStream_t st,
                      const __half** result, int* T_out) {
-  const EmbWeights& E = ctx->emb;
+  EmbWs cur = w;                // cur.A is the current activation; Bf, Cf and D are scratch
   int rc;
   int H = kMel, Wd = T0;
-  __half* cur = w.A;            // current activation; the other two buffers are scratch
-  __half* s1 = w.Bf;
-  __half* s2 = w.Cf;
-  if ((rc = conv1_forward(w.fbank, w.fmean, frame0, E.conv1_w, E.conv1_b, cur, nb, T0, st))) return rc;
-  for (const BlockWeights& B : E.blocks) {
-    const int s = B.conv1.stride;
-    if ((rc = block_run(ctx, B, cur, s1, s2, nb, H, Wd, st))) return rc;
-    H = (H + 2 - 3) / s + 1; Wd = (Wd + 2 - 3) / s + 1;
-  }
-  for (const BottleneckWeights& B : E.bottlenecks) {
-    const int s = B.conv2.stride;
-    if ((rc = bottleneck_run(ctx, B, cur, s1, s2, w.D, nb, H, Wd, st))) return rc;
-    H = (H + 2 - 3) / s + 1; Wd = (Wd + 2 - 3) / s + 1;
-  }
+  for (int k = 0; k < trunk_stages(ctx->emb); ++k)
+    if ((rc = trunk_stage(ctx, k, cur, frame0, nb, H, Wd, st))) return rc;
   B200_CHECK(H == 10 && (T0 != kFbankFrames || Wd == kEmbT), B200_ERR_STATE, "unexpected trunk output %dx%d", H, Wd);
-  *result = cur;
+  *result = cur.A;
   *T_out = Wd;
   return B200_OK;
 }
@@ -1333,6 +1346,46 @@ int b200_emb_trunk(b200_ctx* ctx, const float* fbank, int32_t num_chunks, float*
     if ((rc = trunk_run(ctx, w, nullptr, nb, kFbankFrames, st, &feat, &T))) return rc;
     if ((rc = frames_to_nchw(feat, frames + (size_t)c0 * C * 10 * kEmbT, nb, T, C, st))) return rc;
   }
+  return B200_OK;
+}
+
+int b200_emb_trunk_stage(b200_ctx* ctx, int32_t stage, const void* in, const float* fmean, int32_t B, int32_t W,
+                         void* out, void* stream) {
+  B200_CHECK(ctx && ctx->emb.loaded, B200_ERR_STATE, "embedding weights not loaded");
+  const EmbWeights& E = ctx->emb;
+  B200_CHECK(in && out && (stage > 0 || fmean) && B >= 0 && W >= 1, B200_ERR_INVALID, "bad arguments");
+  B200_CHECK(stage >= 0 && stage < trunk_stages(E), B200_ERR_INVALID, "stage %d: the trunk has stages 0 .. %d",
+             (int)stage, trunk_stages(E) - 1);
+  // one sub-batch of the embedding paths: the workspace of emb_max_batch 10 s chunks holds every stage at width W
+  const int64_t nbmax = std::max<int64_t>(1, (int64_t)ctx->emb_max_batch * kFbankFrames / W);
+  B200_CHECK(B <= nbmax, B200_ERR_INVALID,
+             "%d segments of width %d are more than one embedding sub-batch (%lld: emb_max_batch %d x 998 / %d)",
+             (int)B, (int)W, (long long)nbmax, ctx->emb_max_batch, (int)W);
+  if (B == 0) return B200_OK;
+  CtxScope scope(ctx);
+  cudaStream_t st = (cudaStream_t)stream;
+  // the stage's input height and channels: the stem's output shape through the strides of the blocks before it
+  int H = kMel, C_in = 32;
+  for (int k = 1; k < stage; ++k) {
+    int s;
+    stage_shape(E, k, &s, &C_in);
+    H = (H + 2 - 3) / s + 1;
+  }
+  int rc = ensure_ws(ctx, carve_emb(E, B, W, 1, nullptr, nullptr) + 4096);
+  if (rc) return rc;
+  EmbWs w;
+  carve_emb(E, B, W, 1, ctx->ws, &w);
+  if (stage == 0) {
+    w.fbank = (float*)in;
+    w.fmean = const_cast<float*>(fmean);
+  } else {
+    B200_CUDA_OK(cudaMemcpyAsync(w.A, in, (size_t)B * H * W * C_in * sizeof(__half), cudaMemcpyDeviceToDevice, st));
+  }
+  int Wd = W;
+  if ((rc = trunk_stage(ctx, stage, w, nullptr, B, H, Wd, st))) return rc;
+  int s, C_out;
+  stage_shape(E, stage, &s, &C_out);
+  B200_CUDA_OK(cudaMemcpyAsync(out, w.A, (size_t)B * H * Wd * C_out * sizeof(__half), cudaMemcpyDeviceToDevice, st));
   return B200_OK;
 }
 

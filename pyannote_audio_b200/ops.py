@@ -276,6 +276,7 @@ class Context:
         self._heads = {}
         self.emb_loaded = False
         self.emb_channels = 256   # trunk output channels of the loaded embedding model: 256 (ResNet34) or 1024
+        self.emb_blocks = []      # (C_in, C_out, stride) of each block of the loaded trunk, in order
         self.xvec_loaded = False
         self.xvec_dimension = 512
         self.xvec_mfcc_loaded = False
@@ -354,10 +355,11 @@ class Context:
             return self._load_bottleneck(sd, f, conv_bn)
         w = _lib.EmbWeights()
         conv_bn(w.stem, "resnet.conv1", "resnet.bn1")
-        bi = 0
+        bi, blocks = 0, []
         for li, n in enumerate((3, 4, 6, 3), start=1):
             for i in range(n):
                 p = f"resnet.layer{li}.{i}"
+                blocks.append((blocks[-1][1] if blocks else 32, 32 << (li - 1), 2 if i == 0 and li > 1 else 1))
                 conv_bn(w.block_conv1[bi], p + ".conv1", p + ".bn1")
                 conv_bn(w.block_conv2[bi], p + ".conv2", p + ".bn2")
                 if p + ".shortcut.0.weight" in sd:
@@ -368,7 +370,7 @@ class Context:
         self.owners.pop("emb", None)
         self.emb_loaded = False
         _lib.check(self.lib.b200_emb_load(self._h, C.byref(w)))
-        self.emb_loaded, self.emb_channels = True, 256
+        self.emb_loaded, self.emb_channels, self.emb_blocks = True, 256, blocks
 
     def load_xvector(self, sd: Mapping[str, torch.Tensor]):
         """XVectorSincNet weights (models/embedding/xvector.py:205-252) into the ctx's own slot."""
@@ -474,10 +476,11 @@ class Context:
         total = sum(counts)
         arrays = [(_lib.ConvBN * total)() for _ in range(4)]
         conv1, conv2, conv3, shortcut = arrays
-        bi = 0
+        bi, blocks = 0, []
         for li, n in enumerate(counts, start=1):
             for i in range(n):
                 p = f"resnet.layer{li}.{i}"
+                blocks.append((blocks[-1][1] if blocks else 32, 128 << (li - 1), 2 if i == 0 and li > 1 else 1))
                 conv_bn(conv1[bi], p + ".conv1", p + ".bn1")
                 conv_bn(conv2[bi], p + ".conv2", p + ".bn2")
                 conv_bn(conv3[bi], p + ".conv3", p + ".bn3")
@@ -494,7 +497,7 @@ class Context:
         self.owners.pop("emb", None)
         self.emb_loaded = False
         _lib.check(self.lib.b200_emb_load_bottleneck(self._h, C.byref(w)))
-        self.emb_loaded, self.emb_channels = True, 1024
+        self.emb_loaded, self.emb_channels, self.emb_blocks = True, 1024, blocks
 
     # ---- helpers ---------------------------------------------------------------------------------
     def _check_waveform(self, wav: torch.Tensor):
@@ -711,6 +714,33 @@ class Context:
         fbank = fbank.contiguous()
         out = torch.empty((n, self.emb_channels, 10, 125), dtype=torch.float32, device=self.device)
         self._call("b200_emb_trunk", _ptr(fbank), n, _ptr(out))
+        return out
+
+    def emb_trunk_stage(self, stage: int, x: torch.Tensor, fmean: Optional[torch.Tensor] = None):
+        """One stage of the loaded trunk on B segments of width W, as emb_trunk runs it under the ctx's conv_impl.
+        Stage 0 is the stem: fp32 fbank (B, W, 80) minus ``fmean`` (B, 80; zeros when None) -> NHWC float16
+        (B, 80, W, 32).  Stage k >= 1 is block k - 1: NHWC float16 (B, H, W, C_in) -> (B, H', W', C_out)."""
+        if not 0 <= stage <= len(self.emb_blocks):
+            raise ValueError(f"stage {stage}: the trunk has stages 0 .. {len(self.emb_blocks)}")
+        if x.dim() != (3 if stage == 0 else 4):
+            raise ValueError(f"stage {stage} takes a {3 if stage == 0 else 4}-d tensor, got shape {tuple(x.shape)}")
+        B, W = x.shape[0], x.shape[-2 if stage else 1]
+        if stage == 0:
+            shape, dtype, (H, C_out, s) = (B, W, 80), torch.float32, (80, 32, 1)
+            fmean = torch.zeros((B, 80)) if fmean is None else fmean
+            if tuple(fmean.shape) != (B, 80):
+                raise ValueError(f"fmean has shape {tuple(fmean.shape)}, expected {(B, 80)}")
+            fmean = fmean.to(device=self.device, dtype=torch.float32).contiguous()
+        else:
+            C_in, C_out, s = self.emb_blocks[stage - 1]
+            H = 80 >> sum(b[2] == 2 for b in self.emb_blocks[:stage - 1])
+            shape, dtype = (B, H, W, C_in), torch.float16
+        if tuple(x.shape) != shape or x.dtype != dtype:
+            raise ValueError(f"stage {stage} takes {dtype} of shape {shape}, got {x.dtype} {tuple(x.shape)}")
+        x = x.to(device=self.device).contiguous()
+        Ho, Wo = (H - 1) // s + 1, (W - 1) // s + 1
+        out = torch.empty((B, Ho, Wo, C_out), dtype=torch.float16, device=self.device)
+        self._call("b200_emb_trunk_stage", int(stage), _ptr(x), _ptr(fmean if stage == 0 else None), B, W, _ptr(out))
         return out
 
     def stats_pool(self, seq: torch.Tensor, weights: Optional[torch.Tensor] = None):
