@@ -292,6 +292,46 @@ int b200_seg_forward_window(b200_ctx* ctx, const float* wav, const int64_t* chun
  * not both.  A loaded log-softmax head returns B200_STATUS_INVALID. */
 int b200_seg_forward_scores(b200_ctx* ctx, const float* wav, const int64_t* chunk_off, const int32_t* chunk_valid,
                             int32_t num_chunks, int32_t window, float* scores, float* max_scores, void* stream);
+/* Intermediates of the segmentation network, for testing it stage by stage (b200_seg_stages, b200_seg_head_stages).
+ * Every pointer is a DEVICE buffer or NULL; after each stage the library copies that stage's result into every
+ * non-NULL buffer, in the layout the next stage reads.  n windows, T frames, float2 = (scale, shift). */
+typedef struct b200_seg_capture {
+  void* af_wav;                 /* [n] float2: wav_norm1d as an affine of the raw samples                   */
+  float* P0;                    /* [n][80][pool0] sinc conv -> |.| -> MaxPool 3                             */
+  void* af0;                    /* [n][80] float2: norm1d.0 as an affine of P0                              */
+  float* P1;                    /* [n][60][pool1] Conv1d 1 -> MaxPool 3 -> + bias                           */
+  void* af1;                    /* [n][60] float2                                                           */
+  float* P2;                    /* [n][60][pool2] Conv1d 2 -> MaxPool 3 -> + bias (pool2 = T)               */
+  void* af2;                    /* [n][60] float2                                                           */
+  float* x0;                    /* [n][T][64] head input: leaky_relu(P2 * scale + shift), 4 zero columns     */
+  float* gx[4];                 /* per LSTM layer [n][T][1024]: input projection + b_ih + b_hh, column
+                                   dir * 512 + unit * 4 + gate (i, f, g, o)                                 */
+  float* y[4];                  /* per LSTM layer [n][T][256] fp32 (seg_gemm_impl 0): forward units 0..127,
+                                   reverse 128..255                                                         */
+  void* y_hi[4];                /* the same as fp16 (hi, lo) pairs, y = hi + lo (seg_gemm_impl 1)            */
+  void* y_lo[4];
+  float* z1;                    /* [n][T][128] leaky_relu(linear.0): fp32 (seg_gemm_impl 0) ...              */
+  void* z1_hi;                  /* ... or fp16 (hi, lo) (seg_gemm_impl 1)                                   */
+  void* z1_lo;
+  float* z2;                    /* [n][T][128] leaky_relu(linear.1), fp32                                   */
+  uint8_t* cls;                 /* log-softmax heads: classes [n][T] (required) and logp [n][T][K]           */
+  float* logp;
+  float* scores;                /* sigmoid heads: scores [n][T][K] and max_scores [n][T]                    */
+  float* max_scores;
+} b200_seg_capture;
+/* PyanNet on n windows as b200_seg_forward_window / b200_seg_forward_scores run it (same kernels and launches, under
+ * the ctx's seg_*_impl options), with its intermediates copied into cap; the classifier writes cap's outputs.  n may
+ * not exceed one sub-batch (min(seg_max_batch * 160000 / window, 65535) windows), else B200_STATUS_INVALID. */
+int b200_seg_stages(b200_ctx* ctx, const float* wav, const int64_t* chunk_off, const int32_t* chunk_valid,
+                    int32_t num_chunks, int32_t window, const b200_seg_capture* cap, void* stream);
+/* The segmentation head of a loaded model alone on a caller input x0[n][T][k0] (DEVICE fp32), T >= 1: the BiLSTM stack,
+ * linear layers and classifier as the forward runs them, capturing gx, y, z1, z2 and the outputs into cap.  model
+ * B200_SEG_HEAD_PYANNET (k0 = 64: 60 SincNet features and 4 columns the weights ignore) or B200_SEG_HEAD_SSERIOUSS
+ * (k0 = 768). */
+#define B200_SEG_HEAD_PYANNET 0
+#define B200_SEG_HEAD_SSERIOUSS 1
+int b200_seg_head_stages(b200_ctx* ctx, int32_t model, const float* x0, int32_t n, int32_t T,
+                         const b200_seg_capture* cap, void* stream);
 /* SincNet.forward alone (models/blocks/sincnet.py:163-184): out[num_chunks][589][60] fp32 (frame-major). */
 int b200_sincnet_forward(b200_ctx* ctx, const float* wav, const int64_t* chunk_off, const int32_t* chunk_valid,
                          int32_t num_chunks, float* out, void* stream);

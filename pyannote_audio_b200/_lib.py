@@ -27,6 +27,16 @@ class SegWeights(C.Structure):
     ]
 
 
+class SegCapture(C.Structure):
+    _fields_ = [
+        ("af_wav", C.c_void_p), ("P0", C.c_void_p), ("af0", C.c_void_p), ("P1", C.c_void_p), ("af1", C.c_void_p),
+        ("P2", C.c_void_p), ("af2", C.c_void_p), ("x0", C.c_void_p),
+        ("gx", C.c_void_p * 4), ("y", C.c_void_p * 4), ("y_hi", C.c_void_p * 4), ("y_lo", C.c_void_p * 4),
+        ("z1", C.c_void_p), ("z1_hi", C.c_void_p), ("z1_lo", C.c_void_p), ("z2", C.c_void_p),
+        ("cls", C.c_void_p), ("logp", C.c_void_p), ("scores", C.c_void_p), ("max_scores", C.c_void_p),
+    ]
+
+
 class ConvBN(C.Structure):
     _fields_ = [("conv_weight", c_float_p), ("bn_weight", c_float_p), ("bn_bias", c_float_p),
                 ("bn_mean", c_float_p), ("bn_var", c_float_p)]
@@ -127,6 +137,10 @@ _PROTOS = {
                                           C.c_void_p, C.c_void_p, C.c_void_p]),
     "b200_seg_forward_scores": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_int32, C.c_int32,
                                           C.c_void_p, C.c_void_p, C.c_void_p]),
+    "b200_seg_stages": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_int32, C.c_int32,
+                                  C.POINTER(SegCapture), C.c_void_p]),
+    "b200_seg_head_stages": (C.c_int, [C.c_void_p, C.c_int32, C.c_void_p, C.c_int32, C.c_int32, C.POINTER(SegCapture),
+                                       C.c_void_p]),
     "b200_sincnet_forward": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_int32, C.c_void_p,
                                        C.c_void_p]),
     "b200_powerset_to_multilabel": (C.c_int, [C.c_void_p, C.c_void_p, C.c_int64, C.c_void_p, C.c_void_p]),

@@ -809,10 +809,11 @@ static const SegWeights* loaded_head(const b200_ctx* ctx, SegFront front) {
 // head classifies it, both phases in the same workspace region.  A sub-batch holds at most max_batch x 160000
 // window samples (the workspace of max_batch 10 s windows; option seg_max_batch or ssl_max_batch) and at most 65535
 // windows (the y extent of the SincNet grids).  The "seg" timer covers PyanNet's sub-batches.  With front_out, the
-// front end writes its head input [n][T][F] there instead of x0 and the head does not run.
+// front end writes its head input [n][T][F] there instead of x0 and the head does not run.  With cap (SincNet only),
+// the n windows must fit one sub-batch and every stage's result is also copied into cap's buffers.
 static int seg_run(b200_ctx* ctx, SegFront front, const float* wav, const int64_t* chunk_off,
                    const int32_t* chunk_valid, int n, int window, const SegHeadOut& out, float* front_out,
-                   cudaStream_t st) {
+                   cudaStream_t st, const SegCapture* cap = nullptr) {
   const bool sinc = front == SegFront::kSincNet;
   const char* model = sinc ? "segmentation" : "SSeRiouSS";
   const SegWeights* head = loaded_head(ctx, front);
@@ -829,9 +830,13 @@ static int seg_run(b200_ctx* ctx, SegFront front, const float* wav, const int64_
              "a window of %d samples is longer than the %lld samples of one %s sub-batch (%s %d x 160000): set the "
              "option %s to at least %lld, or segment shorter excerpts",
              window, (long long)budget, model, option, max_batch, option, (long long)((window + kChunk - 1) / kChunk));
+  const int64_t sub_batch = std::min<int64_t>(budget / window, 65535);
+  B200_CHECK(!cap || n <= sub_batch, B200_ERR_INVALID,
+             "%d windows of %d samples are more than one %s sub-batch (%lld: %s %d x 160000 / %d, at most 65535)", n,
+             window, model, (long long)sub_batch, option, max_batch, window);
   if (n == 0) return B200_OK;
   CtxScope scope(ctx);
-  const int nbmax = (int)std::min<int64_t>(std::min<int64_t>(n, budget / window), 65535);
+  const int nbmax = (int)std::min<int64_t>(n, sub_batch);
   SegGeom seg_g{};
   SslGeom ssl_g{};
   int T = 0, F = 0;            // frames and features per window
@@ -864,7 +869,7 @@ static int seg_run(b200_ctx* ctx, SegFront front, const float* wav, const int64_
     switch (front) {
       case SegFront::kSincNet:
         rc = sincnet_forward(ctx->seg.sinc, seg_g, wav, ctx->d_off + c0, ctx->d_valid + c0, nb, region, feat,
-                             ctx->seg_conv_impl, st);
+                             ctx->seg_conv_impl, st, cap);
         break;
       case SegFront::kWavLM:
         rc = ssl_frontend_forward(ctx->ssl, ssl_g, wav, ctx->d_off + c0, ctx->d_valid + c0, nb, region, feat,
@@ -880,7 +885,7 @@ static int seg_run(b200_ctx* ctx, SegFront front, const float* wav, const int64_
     sub.scores = out.scores ? out.scores + row0 * K : nullptr;
     sub.max_scores = out.max_scores ? out.max_scores + row0 : nullptr;
     if ((rc = lstm_head_forward(*head, x0, nb, T, region, sub, ctx->num_sms, ctx->seg_gemm_impl, ctx->seg_rec_impl,
-                                st)))
+                                st, cap)))
       return rc;
   }
   return B200_OK;
@@ -918,6 +923,47 @@ int b200_seg_forward_scores(b200_ctx* ctx, const float* wav, const int64_t* chun
 int b200_seg_forward(b200_ctx* ctx, const float* wav, const int64_t* chunk_off, const int32_t* chunk_valid,
                      int32_t num_chunks, uint8_t* classes, float* logp, void* stream) {
   return b200_seg_forward_window(ctx, wav, chunk_off, chunk_valid, num_chunks, kChunk, classes, logp, stream);
+}
+
+// the classifier outputs of a capture; a log-softmax head writes its classes unconditionally
+static int capture_outputs(const SegWeights& head, const SegCapture* cap, SegHeadOut* out) {
+  B200_CHECK(head.activation != kSegLogSoftmax || cap->cls, B200_ERR_INVALID,
+             "the loaded head is a log-softmax head: cap->cls is required");
+  *out = SegHeadOut{cap->cls, cap->logp, cap->scores, cap->max_scores};
+  return B200_OK;
+}
+
+int b200_seg_stages(b200_ctx* ctx, const float* wav, const int64_t* chunk_off, const int32_t* chunk_valid,
+                    int32_t num_chunks, int32_t window, const b200_seg_capture* cap, void* stream) {
+  B200_CHECK(cap, B200_ERR_INVALID, "cap is NULL");
+  const SegWeights* head = loaded_head(ctx, SegFront::kSincNet);
+  B200_CHECK(head, B200_ERR_STATE, "segmentation weights not loaded");
+  SegHeadOut out;
+  int rc;
+  if ((rc = capture_outputs(*head, cap, &out))) return rc;
+  return seg_run(ctx, SegFront::kSincNet, wav, chunk_off, chunk_valid, num_chunks, window, out, nullptr,
+                 (cudaStream_t)stream, cap);
+}
+
+int b200_seg_head_stages(b200_ctx* ctx, int32_t model, const float* x0, int32_t n, int32_t T,
+                         const b200_seg_capture* cap, void* stream) {
+  B200_CHECK(model == B200_SEG_HEAD_PYANNET || model == B200_SEG_HEAD_SSERIOUSS, B200_ERR_INVALID,
+             "unknown model %d (B200_SEG_HEAD_PYANNET = 0, B200_SEG_HEAD_SSERIOUSS = 1)", (int)model);
+  const bool sinc = model == B200_SEG_HEAD_PYANNET;
+  const SegWeights* head = loaded_head(ctx, sinc ? SegFront::kSincNet : SegFront::kWavLM);
+  B200_CHECK(head, B200_ERR_STATE, "%s weights not loaded", sinc ? "segmentation" : "SSeRiouSS");
+  B200_CHECK(x0 && cap && n >= 0 && T >= 1, B200_ERR_INVALID, "bad arguments");
+  // as in the forward's largest sub-batch, the n * T * 1024 elements of the input projection fit an int
+  B200_CHECK((int64_t)n * T * 1024 < INT_MAX, B200_ERR_INVALID, "%d sequences of %d frames are too many", (int)n,
+             (int)T);
+  SegHeadOut out;
+  int rc;
+  if ((rc = capture_outputs(*head, cap, &out))) return rc;
+  if (n == 0) return B200_OK;
+  CtxScope scope(ctx);
+  if ((rc = ensure_ws(ctx, lstm_workspace_bytes(n, T, head->k_in[0]) + 4096))) return rc;
+  return lstm_head_forward(*head, x0, n, T, ctx->ws, out, ctx->num_sms, ctx->seg_gemm_impl, ctx->seg_rec_impl,
+                           (cudaStream_t)stream, cap);
 }
 
 // ------------------------------------------------------------------------------------------------------

@@ -1,8 +1,14 @@
 // Segmentation path (PyanNet: SincNet front-end -> 4x BiLSTM -> Linear x2 -> classifier -> powerset argmax or sigmoid).
 #pragma once
+#include "../../include/b200diar.h"
 #include "common.cuh"
 
 namespace b200 {
+
+// Intermediates copied out after each stage (b200_seg_stages / b200_seg_head_stages); the forward passes null
+using SegCapture = b200_seg_capture;
+// D2D copy of `bytes` from src into dst when dst is not null
+int capture(void* dst, const void* src, size_t bytes, cudaStream_t stream);
 
 // Per-stage lengths of PyanNet on a window of W samples (models/blocks/sincnet.py:163-184): sinc conv (K 251,
 // stride 10), MaxPool 3, Conv1d 5, MaxPool 3, Conv1d 5, MaxPool 3.  W = 160000 gives the kSincLen .. kPool2 constants.
@@ -106,7 +112,8 @@ int conv5_wg_forward(const SegGeom& g, int layer, const float* Pin, const float2
 // (60 features + 4 zero pad)
 size_t sincnet_workspace_bytes(const SegGeom& g, int NB);
 int sincnet_forward(const SincNetWeights& W, const SegGeom& g, const float* wav, const long long* chunk_off,
-                    const int* chunk_valid, int NB, void* ws, float* x0, int conv_impl, cudaStream_t stream);
+                    const int* chunk_valid, int NB, void* ws, float* x0, int conv_impl, cudaStream_t stream,
+                    const SegCapture* cap = nullptr);
 
 // Outputs of the classifier, written straight to the caller's buffers.  Log-softmax heads: cls [NB][T] u8 (+ optional
 // logp [NB][T][K]); sigmoid heads: scores [NB][T][K] and / or max_scores [NB][T] (either may be null).
@@ -120,6 +127,6 @@ struct SegHeadOut {
 // SincNet features and 4 zero columns; 768: SSeRiouSS)
 size_t lstm_workspace_bytes(int NB, int T, int k0);
 int lstm_head_forward(const SegWeights& W, const float* x0, int NB, int T, void* ws, const SegHeadOut& out,
-                      int num_sms, int gemm_impl, int rec_impl, cudaStream_t stream);
+                      int num_sms, int gemm_impl, int rec_impl, cudaStream_t stream, const SegCapture* cap = nullptr);
 
 }  // namespace b200

@@ -245,10 +245,13 @@ static int launch_rec(const float* Gx, const float* Whh, float* Y, __half* Yh, _
 }
 
 int lstm_head_forward(const SegWeights& W, const float* x0, int NB, int T, void* ws, const SegHeadOut& out,
-                      int num_sms, int gemm_impl, int rec_impl, cudaStream_t stream) {
+                      int num_sms, int gemm_impl, int rec_impl, cudaStream_t stream, const SegCapture* cap) {
   LstmWs w;
   carve_lstm(NB, T, W.k_in[0], ws, &w);
   const int M = NB * T;          // rows of every GEMM (< 2^31); element offsets M * 1024 are formed in size_t
+  const SegCapture none{};
+  const SegCapture& c = cap ? *cap : none;
+  const size_t f32 = sizeof(float) * M, f16 = sizeof(__half) * M;
   const int clusters = num_sms / 2;
   const bool tc = gemm_impl != 0;
   int rc;
@@ -265,10 +268,13 @@ int lstm_head_forward(const SegWeights& W, const float* x0, int NB, int T, void*
     else
       rc = sgemm_nt(in, W.k_in[l], W.w_ih[l], W.k_in[l], w.Gx, 1024, W.b_g[l], M, 1024, W.k_in[l], 0, stream);
     if (rc) return rc;
+    if ((rc = capture(c.gx[l], w.Gx, f32 * 1024, stream))) return rc;
     if (tc && rec_impl != 0) {   // tensor-core recurrence (seg_lstm_wg.cu)
       if ((rc = lstm_rec_wg(w.Gx, W.w_hh_hi[l], W.w_hh_lo[l], outs_h[l & 1], outs_l[l & 1], NB, T, rec_impl, stream)))
         return rc;
       in_h = outs_h[l & 1]; in_l = outs_l[l & 1];
+      if ((rc = capture(c.y_hi[l], in_h, f16 * 256, stream)) || (rc = capture(c.y_lo[l], in_l, f16 * 256, stream)))
+        return rc;
       continue;
     }
     float* y = tc ? nullptr : outs[l & 1];
@@ -280,20 +286,27 @@ int lstm_head_forward(const SegWeights& W, const float* x0, int NB, int T, void*
     else rc = launch_rec<2>(w.Gx, W.w_hh[l], y, yh, yl, NB, T, stream);
     if (rc) return rc;
     in = y; in_h = yh; in_l = yl;
+    if (tc && ((rc = capture(c.y_hi[l], yh, f16 * 256, stream)) || (rc = capture(c.y_lo[l], yl, f16 * 256, stream))))
+      return rc;
+    if (!tc && (rc = capture(c.y[l], y, f32 * 256, stream))) return rc;
   }
   if (tc) {
     rc = gemm_tc_split(in_h, in_l, 256, W.lin_w_hi[0], W.lin_w_lo[0], 256, nullptr, 0, w.Z1h, w.Z1l, 128, W.lin_b[0], M,
                        128, 256, 1, num_sms, stream);
     if (rc) return rc;
+    if ((rc = capture(c.z1_hi, w.Z1h, f16 * 128, stream)) || (rc = capture(c.z1_lo, w.Z1l, f16 * 128, stream)))
+      return rc;
     rc = gemm_tc_split(w.Z1h, w.Z1l, 128, W.lin_w_hi[1], W.lin_w_lo[1], 128, w.Z2, 128, nullptr, nullptr, 0,
                        W.lin_b[1], M, 128, 128, 1, num_sms, stream);
     if (rc) return rc;
   } else {
     rc = sgemm_nt(in, 256, W.lin_w[0], 256, w.Z1, 128, W.lin_b[0], M, 128, 256, 1, stream);
     if (rc) return rc;
+    if ((rc = capture(c.z1, w.Z1, f32 * 128, stream))) return rc;
     rc = sgemm_nt(w.Z1, 128, W.lin_w[1], 128, w.Z2, 128, W.lin_b[1], M, 128, 128, 1, stream);
     if (rc) return rc;
   }
+  if ((rc = capture(c.z2, w.Z2, f32 * 128, stream))) return rc;
   const ClassifierFn head = (W.activation == kSegSigmoid ? kSigmoidHeads : kLogSoftmaxHeads)[W.num_classes - 1];
   return launch(head, ceil_div(M, 8), 256, 0, stream, w.Z2, W.cls_w, W.cls_b, out.cls, out.logp, out.scores,
                 out.max_scores, M);

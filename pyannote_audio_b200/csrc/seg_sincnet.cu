@@ -388,10 +388,19 @@ static size_t carve(const SegGeom& g, int NB, void* base, SincWs* w) {
 
 size_t sincnet_workspace_bytes(const SegGeom& g, int NB) { return carve(g, NB, nullptr, nullptr); }
 
+int capture(void* dst, const void* src, size_t bytes, cudaStream_t stream) {
+  if (dst && bytes) B200_CUDA_OK(cudaMemcpyAsync(dst, src, bytes, cudaMemcpyDeviceToDevice, stream));
+  return B200_OK;
+}
+
 int sincnet_forward(const SincNetWeights& W, const SegGeom& g, const float* wav, const long long* chunk_off,
-                    const int* chunk_valid, int NB, void* ws, float* x0, int conv_impl, cudaStream_t stream) {
+                    const int* chunk_valid, int NB, void* ws, float* x0, int conv_impl, cudaStream_t stream,
+                    const SegCapture* cap) {
   SincWs w;
   carve(g, NB, ws, &w);
+  const SegCapture none{};
+  const SegCapture& c = cap ? *cap : none;
+  const size_t f2 = sizeof(float2) * NB;
   const size_t smem_sinc = (2176 + 126 * 80) * sizeof(float);
   const size_t smem_c80 = (80 * 196 + 20 * 300) * sizeof(float);
   const size_t smem_c60 = (60 * 196 + 20 * 300) * sizeof(float);
@@ -403,6 +412,7 @@ int sincnet_forward(const SincNetWeights& W, const SegGeom& g, const float* wav,
   if (nslices > 1 && (rc = launch(wav_finalize_kernel, ceil_div(NB, 128), 128, 0, stream, w.wav_part, nslices, g.W,
                                   W.wav_w, W.wav_b, w.af_wav, NB)))
     return rc;
+  if ((rc = capture(c.af_wav, w.af_wav, f2, stream))) return rc;
   // conv_impl: 1 = persistent split-fp16 wgmma kernels (default), 2 = one wgmma CTA per tile, 0 = the fp32 CUDA-core
   // twins
   if (conv_impl) {
@@ -417,6 +427,8 @@ int sincnet_forward(const SincNetWeights& W, const SegGeom& g, const float* wav,
   if ((rc = in_stats(w.part0, g.tiles0, w.red0, w.red1, g.pool0, 80, W.in_gamma[0], W.in_beta[0], w.af0, NB * 80,
                      stream)))
     return rc;
+  if ((rc = capture(c.P0, w.P0, sizeof(float) * NB * 80 * g.pool0, stream))) return rc;
+  if ((rc = capture(c.af0, w.af0, f2 * 80, stream))) return rc;
   if (conv_impl) {
     if ((rc = conv5_wg_forward(g, 0, w.P0, w.af0, W.conv_wg_hi[0], W.conv_wg_lo[0], W.conv_b[0], NB, w.P1, w.part1,
                                conv_impl, stream)))
@@ -429,6 +441,8 @@ int sincnet_forward(const SincNetWeights& W, const SegGeom& g, const float* wav,
   if ((rc = in_stats(w.part1, g.tiles1, w.red0, w.red1, g.pool1, 60, W.in_gamma[1], W.in_beta[1], w.af1, NB * 60,
                      stream)))
     return rc;
+  if ((rc = capture(c.P1, w.P1, sizeof(float) * NB * 60 * g.pool1, stream))) return rc;
+  if ((rc = capture(c.af1, w.af1, f2 * 60, stream))) return rc;
   if (conv_impl) {
     if ((rc = conv5_wg_forward(g, 1, w.P1, w.af1, W.conv_wg_hi[1], W.conv_wg_lo[1], W.conv_b[1], NB, w.P2, w.part2,
                                conv_impl, stream)))
@@ -441,9 +455,13 @@ int sincnet_forward(const SincNetWeights& W, const SegGeom& g, const float* wav,
   if ((rc = in_stats(w.part2, g.tiles2, w.red0, w.red1, g.pool2, 60, W.in_gamma[2], W.in_beta[2], w.af2, NB * 60,
                      stream)))
     return rc;
+  if ((rc = capture(c.P2, w.P2, sizeof(float) * NB * 60 * g.pool2, stream))) return rc;
+  if ((rc = capture(c.af2, w.af2, f2 * 60, stream))) return rc;
   const size_t total = (size_t)NB * g.pool2 * 64;
-  return launch(in_apply_transpose_kernel, (unsigned)((total + 255) / 256), 256, 0, stream, w.P2, w.af2, x0, NB,
-                g.pool2);
+  if ((rc = launch(in_apply_transpose_kernel, (unsigned)((total + 255) / 256), 256, 0, stream, w.P2, w.af2, x0, NB,
+                   g.pool2)))
+    return rc;
+  return capture(c.x0, x0, sizeof(float) * total, stream);
 }
 
 }  // namespace b200

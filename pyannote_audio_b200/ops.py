@@ -274,6 +274,8 @@ class Context:
         # checks a head before it releases the resident one, so it may go on running the previous head.
         self._loaded = set()
         self._heads = {}
+        self._lstm_layers = {}    # slot -> BiLSTM layers of the head the library accepted last
+        self._options = {}        # options set through set_option, by key
         self.emb_loaded = False
         self.emb_channels = 256   # trunk output channels of the loaded embedding model: 256 (ResNet34) or 1024
         self.emb_blocks = []      # (C_in, C_out, stride) of each block of the loaded trunk, in order
@@ -313,6 +315,7 @@ class Context:
 
     def set_option(self, key: str, value: int):
         _lib.check(self.lib.b200_ctx_set_option(self._h, key.encode(), int(value)))
+        self._options[key] = int(value)
 
     @property
     def launch_count(self) -> int:
@@ -464,6 +467,7 @@ class Context:
         _lib.check(getattr(self.lib, entry)(self._h, C.byref(w), *head))
         self._loaded.add(slot)
         self._heads[slot] = head
+        self._lstm_layers[slot] = int(w.lstm_layers)
 
     def _load_bottleneck(self, sd, f, conv_bn):
         """WeSpeakerResNet152 / 221 / 293 (Bottleneck blocks, resnet.py:148-212): the block counts come from the keys."""
@@ -596,6 +600,85 @@ class Context:
         out = torch.empty((n, ssl_num_frames(window), 768), dtype=torch.float32, device=self.device)
         self._call("b200_ssl_features", _ptr(wav), off.ctypes.data, valid.ctypes.data, n, window, _ptr(out))
         return out
+
+    def seg_stages(self, wav, chunk_off, chunk_valid, window: int = CHUNK) -> dict:
+        """The loaded PyanNet on windows as seg_forward runs them (same kernels, under the ctx's seg_*_impl options),
+        returning every intermediate: "af_wav" (n, 2), "P0" (n, 80, pool0), "af0" (n, 80, 2), "P1" (n, 60, pool1),
+        "af1", "P2" (n, 60, F), "af2", "x0" (n, F, 64), and the head's tensors as seg_head_stages returns them.  The
+        affines are (scale, shift) pairs.  The windows must fit one sub-batch (ValueError otherwise)."""
+        check_seg_window(window)
+        window = int(window)
+        off, valid = self._chunks(wav, chunk_off, chunk_valid)
+        n = len(off)
+        sinc_len = 1 + (window - 251) // 10
+        pool0 = sinc_len // 3
+        pool1 = (pool0 - 4) // 3
+        pool2 = (pool1 - 4) // 3
+        f32 = dict(dtype=torch.float32, device=self.device)
+        out = {"af_wav": torch.empty((n, 2), **f32), "P0": torch.empty((n, 80, pool0), **f32),
+               "af0": torch.empty((n, 80, 2), **f32), "P1": torch.empty((n, 60, pool1), **f32),
+               "af1": torch.empty((n, 60, 2), **f32), "P2": torch.empty((n, 60, pool2), **f32),
+               "af2": torch.empty((n, 60, 2), **f32), "x0": torch.empty((n, pool2, 64), **f32)}
+        cap = self._head_capture("seg", n, pool2, out)
+        for name in ("af_wav", "P0", "af0", "P1", "af1", "P2", "af2", "x0"):
+            setattr(cap, name, out[name].data_ptr())
+        self._call("b200_seg_stages", _ptr(wav), off.ctypes.data, valid.ctypes.data, n, window, C.byref(cap))
+        return out
+
+    def seg_head_stages(self, model: str, x0: torch.Tensor) -> dict:
+        """The segmentation head of the loaded ``model`` ("seg": PyanNet, x0 (n, T, 64); "ssl": SSeRiouSS, x0
+        (n, T, 768)) on any input, T >= 1, as the forward runs it, returning "gx" (per LSTM layer (n, T, 1024): input
+        projection plus both biases, column dir * 512 + unit * 4 + gate), "y" (per layer (n, T, 256) float32 under
+        seg_gemm_impl 0, else a (hi, lo) pair of float16 tensors), "z1" (n, T, 128) likewise, "z2" (n, T, 128) and the
+        classifier's outputs: "cls" (n, T) uint8 and "logp" (n, T, K), or "scores" (n, T, K) and "max_scores" (n, T)."""
+        k0 = {"seg": 64, "ssl": 768}.get(model)
+        if k0 is None:
+            raise ValueError(f"model must be 'seg' (PyanNet) or 'ssl' (SSeRiouSS), got {model!r}")
+        if x0.dim() != 3 or x0.shape[2] != k0 or x0.shape[1] < 1:
+            raise ValueError(f"x0 must have shape (n, T >= 1, {k0}), got {tuple(x0.shape)}")
+        x0 = x0.to(device=self.device, dtype=torch.float32).contiguous()
+        n, T = int(x0.shape[0]), int(x0.shape[1])
+        out = {}
+        cap = self._head_capture(model, n, T, out)
+        self._call("b200_seg_head_stages", 0 if model == "seg" else 1, _ptr(x0), n, T, C.byref(cap))
+        return out
+
+    def _head_capture(self, slot: str, n: int, T: int, out: dict) -> "_lib.SegCapture":
+        """A capture of every head tensor of ``slot``'s loaded head for n sequences of T frames, allocated into
+        ``out``."""
+        K, activation = self._heads.get(slot, (CLASSES, SEG_LOGSOFTMAX))
+        layers = self._lstm_layers.get(slot, 4)
+        split = self._options.get("seg_gemm_impl", 1) != 0
+        f32 = dict(dtype=torch.float32, device=self.device)
+        f16 = dict(dtype=torch.float16, device=self.device)
+        cap = _lib.SegCapture()
+        out["gx"], out["y"] = [], []
+        for layer in range(layers):
+            out["gx"].append(torch.empty((n, T, 1024), **f32))
+            cap.gx[layer] = out["gx"][-1].data_ptr()
+            if split:
+                hi, lo = torch.empty((n, T, 256), **f16), torch.empty((n, T, 256), **f16)
+                cap.y_hi[layer], cap.y_lo[layer] = hi.data_ptr(), lo.data_ptr()
+                out["y"].append((hi, lo))
+            else:
+                out["y"].append(torch.empty((n, T, 256), **f32))
+                cap.y[layer] = out["y"][-1].data_ptr()
+        if split:
+            out["z1"] = (torch.empty((n, T, 128), **f16), torch.empty((n, T, 128), **f16))
+            cap.z1_hi, cap.z1_lo = out["z1"][0].data_ptr(), out["z1"][1].data_ptr()
+        else:
+            out["z1"] = torch.empty((n, T, 128), **f32)
+            cap.z1 = out["z1"].data_ptr()
+        out["z2"] = torch.empty((n, T, 128), **f32)
+        cap.z2 = out["z2"].data_ptr()
+        if activation == SEG_SIGMOID:
+            out["scores"], out["max_scores"] = torch.empty((n, T, K), **f32), torch.empty((n, T), **f32)
+            cap.scores, cap.max_scores = out["scores"].data_ptr(), out["max_scores"].data_ptr()
+        else:
+            out["cls"], out["logp"] = torch.empty((n, T), dtype=torch.uint8, device=self.device), \
+                torch.empty((n, T, K), **f32)
+            cap.cls, cap.logp = out["cls"].data_ptr(), out["logp"].data_ptr()
+        return cap
 
     def powerset_to_multilabel(self, cls: torch.Tensor, num_speakers: int = SPEAKERS, max_per_frame: int = 2):
         """(…) uint8 powerset classes of ``num_speakers`` speakers with at most ``max_per_frame`` per frame ->
